@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py - Groth16 proofs/sec (BN254, 2^20-constraint-domain circom squaring chain) on B200, next to the CPU path.
+"""bench.py - Groth16 proofs/sec (BN254, 2^20-constraint-domain circom squaring chain) on H100, next to the CPU path.
 
 One "step" = one call of Groth16::<Bn254, CircomReduction>::create_proof_with_reduction_and_matrices
 (/root/reference/benches/groth16.rs:69-84 times exactly this): proving key + matrices resident, witness given, fixed r, s.
@@ -11,6 +11,8 @@ Output: ONE JSON line (rank 0).  `value` = device-resident throughput (witness a
 Groth16.create_proof_with_reduction_and_matrices with a pinned HOST witness (H2D 32 B x n_vars and D2H 256 B inside the
 timed region), `roofline` = the dominant kernel (MSM bucket accumulation, G1) against measured HBM bandwidth,
 `cpu_baseline` = oracle/cref.c on the host cores, same key / witness / (r, s), proof bytes asserted identical.
+--dump-outputs DIR: after the timed steps, the proof of the last timed step (what the caller receives) is written as
+DIR/proof_{a,b,c}.npy, float64 arrays of the canonical coordinates in 16-bit little-endian limbs (exact in float64).
 N > 1: the headline is N replicas (whole provers, weak scaling); `other_mode` is the same 2^20 proof base-sharded over the
 N GPUs (strong scaling: latency), and `config4` is BASELINE.json config 4: a 2^22 chain, MSM bases sharded over the N GPUs.
 """
@@ -41,7 +43,7 @@ def measured_peaks():
             return float(json.load(open(p))['hbm_gbs']), 'measured (MEASURED_PEAKS.json)'
         except Exception:
             pass
-    return 6650.0, 'fallback (B200_PROFILING.md)'
+    return 3350.0, 'fallback (H100 SXM data sheet HBM3 bandwidth, not measured)'
 
 
 class ClockSampler:
@@ -160,7 +162,7 @@ def workload_config(args, circ):
     return {"workload": f"circom squaring chain (reference bench family, test-vectors/complex-circuit), domain 2^{args.log_n}, "
                         f"n_vars={circ.n_vars}, constraints={circ.num_constraints}, BN254, synthetic trapdoor zkey seed 0xB200, fixed r,s",
             "witness": args.workload, "log_n": args.log_n,
-            "l2": "inputs larger than L2 (proving-key tables ~6 GB per proof pass vs 126 MB L2)"}
+            "l2": "inputs larger than L2 (proving-key tables ~6 GB per proof pass vs 50 MB L2)"}
 
 
 def run_reference(args):
@@ -181,13 +183,15 @@ def run_reference(args):
     za, wm = oracle_key(pk, cm), fr_to_mont(w)
     for _ in range(args.warmup):
         cref.prove(za, R_FIX, S_FIX, wm, nthreads=cores)
-    steps = []
+    steps, proof = [], None
     t0 = time.perf_counter()
     for _ in range(args.steps):
         t1 = time.perf_counter()
-        cref.prove(za, R_FIX, S_FIX, wm, nthreads=cores)
+        proof = cref.prove(za, R_FIX, S_FIX, wm, nthreads=cores)
         steps.append(time.perf_counter() - t1)
     dt = time.perf_counter() - t0
+    if args.dump_outputs:
+        dump_proof(args.dump_outputs, proof)
     val = args.steps / dt
     sample = f"{args.steps} full proofs of the {args.workload} 2^{args.log_n} workload, oracle/cref.c (C + OpenMP restatement of ark-groth16 0.5), {cores} threads pinned one per core"
     out = {"impl": "reference", "metric": METRIC, "value": val, "unit": "proofs/s", "n_gpus": args.gpus, "steps": args.steps, "warmup": args.warmup,
@@ -200,14 +204,15 @@ def run_reference(args):
     emit(out)
 
 
-def static_kernel_profile():
-    """per-launch DRAM traffic and IMAD.WIDE count of the dominant kernel come from an ncu capture, not from this run: the
-    committed summary profiles/kernel_profile.json (written by tools/ncu_summary.py from the capture named inside it)."""
-    p = os.path.join(ROOT, 'profiles', 'kernel_profile.json')
-    try:
-        return json.load(open(p))
-    except Exception:
-        return None
+def dump_proof(out_dir, proof_bytes):
+    """proof bytes (A.x, A.y, B.x.c0, B.x.c1, B.y.c0, B.y.c1, C.x, C.y; 32-byte canonical LE each) -> DIR/proof_{a,b,c}.npy,
+    every coordinate as 16 little-endian 16-bit limbs in float64 (exact)"""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    limbs = np.frombuffer(bytes(proof_bytes), dtype='<u2').astype(np.float64).reshape(8, 16)
+    for name, part in (('proof_a', limbs[0:2]), ('proof_b', limbs[2:6].reshape(2, 2, 16)), ('proof_c', limbs[6:8])):
+        np.save(os.path.join(out_dir, name + '.npy'), part)
+    log(f"[bench] wrote the last timed proof to {out_dir}/proof_{{a,b,c}}.npy")
 
 
 def run_ours(args):
@@ -412,6 +417,8 @@ def run_ours(args):
     proof = main["proof"]
     ctx = main["ctxs"][0]
 
+    if rank == 0 and args.dump_outputs:
+        dump_proof(args.dump_outputs, proof.data)
     if rank == 0 and not args.skip_check:
         wl.check_closed_form(proof)
         log("[bench] proof matches the trapdoor closed form (h-independent) and the witness map matches the trapdoor")
@@ -424,19 +431,11 @@ def run_ours(args):
         # dominant kernel group: the bucket accumulation of one G1 MSM (H query: n = domain bases / scalars), run alone
         msm_ms, acc_ms = ctx.bench_msm(pk, cm, 0, 5)
         alg = pk.domain_size // shard_div * 96.0
-        prof = static_kernel_profile() or {}
-        roof = {"bound": "hbm", "kernel": "G1 bucket accumulation (H query): " + prof.get("g1_kernels", "msm_accumulate_kernel<G1>"),
+        roof = {"bound": "hbm", "kernel": "G1 bucket accumulation (H query): msm_accumulate_kernel<G1>",
                 "achieved": alg / (acc_ms * 1e-3) / 1e9, "peak": peak, "unit": "GB/s",
-                "frac": alg / (acc_ms * 1e-3) / 1e9 / peak, "traffic": (prof.get("g1_dram_bytes_per_launch") or 0) / shard_div or None, "peak_source": how,
+                "frac": alg / (acc_ms * 1e-3) / 1e9 / peak, "peak_source": how,
                 "algorithmic_bytes": alg, "kernel_ms": acc_ms, "whole_msm_ms": msm_ms,
-                "traffic_source": "static: " + prof.get("source", "no committed ncu summary (profiles/kernel_profile.json missing)"),
                 "note": "254-bit Pippenger is bound by the IMAD.WIDE (fmaheavy) pipe, not by HBM (DESIGN.md section 5)"}
-        if prof.get("g1_fmaheavy_pct") and args.log_n == prof.get("log_n") and shard_div == 1:
-            # the binding roofline: the integer multiply-add ("fmaheavy") pipe.  Utilisation is a static ncu fact of the kernel
-            # (sm__pipe_fmaheavy_cycles_active), rescaled by ncu-time / live CUDA-event time of this run
-            frac = prof["g1_fmaheavy_pct"] / 100.0 * (prof["g1_time_us_ncu"] * 1e-3) / acc_ms
-            roof["int_pipe"] = {"bound": "IMAD.WIDE issue (fmaheavy pipe)", "frac": frac, "static_pct_ncu": prof["g1_fmaheavy_pct"],
-                                "static_kernel_us_ncu": prof["g1_time_us_ncu"], "source": "static: " + prof.get("source", "")}
         g2_ms, g2_acc = ctx.bench_msm(pk, cm, 4, 3)
         extra["msm_g2"] = {"whole_msm_ms": g2_ms, "kernel_ms": g2_acc, "algorithmic_gbs": (pk.n_vars - 1) / shard_div * 160.0 / (g2_acc * 1e-3) / 1e9}
         extra["single_proof_latency_ms"] = main["latency_ms"]
@@ -555,6 +554,7 @@ def main():
     ap.add_argument('--host-driver', default='async', choices=['async', 'threads'], help="e2e loop: one host thread with b2g_prove_submit/wait (async) or one thread per in-flight proof")
     ap.add_argument('--no-cpu', action='store_true', help='skip the cpu_baseline leg')
     ap.add_argument('--skip-check', action='store_true')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None, help='write the proof of the last timed step to DIR/proof_{a,b,c}.npy')
     args = ap.parse_args()
     if args.steps is None:
         args.steps = 3 if args.impl == 'reference' else 20

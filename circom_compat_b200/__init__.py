@@ -1,8 +1,8 @@
-"""circom_compat_b200 - B200-native Groth16 (BN254) prover hot path behind the ark-circom API surface.
+"""circom_compat_b200 - H100-native Groth16 (BN254) prover hot path behind the ark-circom API surface.
 
 Host-side mirror of the reference's public interface (/root/reference/src/lib.rs:4-14) for the proving path:
 read_zkey, ProvingKey, ConstraintMatrices, CircomReduction, Groth16.  All arithmetic runs in libb2groth.so
-(hand-written sm_100a CUDA behind include/b2groth.h); there is no CPU fallback.
+(hand-written sm_90a CUDA behind include/b2groth.h); there is no CPU fallback.
 """
 from .zkey import read_zkey, ProvingKey, ConstraintMatrices, fr_to_mont, fr_from_mont  # noqa: F401
 from .groth16 import Groth16, CircomReduction, LibsnarkReduction, Proof, Context, release, release_all  # noqa: F401

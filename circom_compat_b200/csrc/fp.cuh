@@ -1,4 +1,4 @@
-// fp.cuh - 254-bit prime-field arithmetic for BN254 (Fq base field, Fr scalar field) on sm_100a.
+// fp.cuh - 254-bit prime-field arithmetic for BN254 (Fq base field, Fr scalar field) on sm_90a.
 //
 // Replaces, on the device, what ark-ff 0.5.0's Fp256<MontBackend> (+asm, /root/reference/Cargo.toml:25) does on the
 // CPU for the prover hot path.  Representation: 8 x 32-bit limbs, little-endian, Montgomery form with R = 2^256 -
@@ -61,8 +61,7 @@ __device__ __forceinline__ fe fe_load(const void* p) {
     fe r; r.l[0] = a.x; r.l[1] = a.y; r.l[2] = a.z; r.l[3] = a.w; r.l[4] = b.x; r.l[5] = b.y; r.l[6] = b.z; r.l[7] = b.w;
     return r;
 }
-// read-only (non-coherent) load of one element: two 128-bit LDG.CONSTANT.  (One 256-bit ld.global.nc.v8.u32 =
-// LDG.E.ENL2.256.CONSTANT was measured in round 2: no difference on these pipe-bound kernels, profiles/r2_load_width.md.)
+// read-only (non-coherent) load of one element: two 128-bit LDG.CONSTANT (sm_90 has no 256-bit global load).
 __device__ __forceinline__ fe fe_load_nc(const void* p) {
     const uint4* q = reinterpret_cast<const uint4*>(p);
     uint4 a = __ldg(q), b = __ldg(q + 1);
@@ -464,7 +463,8 @@ struct Fp {
 
     // Column form of the same product: sixteen independent 8-limb chains on zero-initialised even/odd accumulators.  More
     // ALU instructions than mul_wide() but no row-to-row dependency; the Fq2 routines, which run at 3 warps per scheduler
-    // inside the G2 accumulation kernel and live off instruction-level parallelism, are 4 % faster with it (measured).
+    // inside the G2 accumulation kernel and live off instruction-level parallelism, use it (a choice carried over from the
+    // previous target GPU, not re-measured on H100).
     static __device__ __forceinline__ void mul_wide_cols(uint32_t* t, const fe& a, const fe& b) {
         uint32_t ev[17], od[16];
         #pragma unroll
@@ -538,7 +538,8 @@ using Fr = Fp<FrParams>;
 // ---------------------------------------------------------------------------------------------- Fq2 = Fq[u]/(u^2+1)
 struct fe2 { fe c0, c1; };
 
-// Fq2 mul / sqr are real calls: inlining them makes the G2 accumulation kernel 13 k instructions (210 KB) and 1.6x slower
+// Fq2 mul / sqr are real calls: inlined, the G2 accumulation kernel grows to ~13 k instructions (a choice carried over from the
+// previous target GPU, where the inlined kernel was slower; not re-measured on H100)
 #define B2G_FQ2_CALL __noinline__
 struct Fq2 {
     using elem = fe2;
@@ -580,9 +581,8 @@ struct Fq2 {
               "r"(b.l[0]), "r"(b.l[1]), "r"(b.l[2]), "r"(b.l[3]), "r"(b.l[4]), "r"(b.l[5]), "r"(b.l[6]), "r"(b.l[7]));
         return s;
     }
-    // (a fused a*b - c*d with six wide products and two reductions was measured 3 - 8 % SLOWER inside the G2 kernel:
-    // fewer IMAD.WIDE but one long dependent chain; the kernel is latency-, not issue-bound at 3 warps per scheduler)
-    // a real call like mul/sqr (that is the build that was measured)
+    // two calls rather than a fused a*b - c*d with six wide products and two reductions: the fused form has fewer IMAD.WIDE but
+    // one long dependent chain, and was slower on the previous target GPU (not re-measured on H100)
     static __device__ B2G_FQ2_CALL fe2 mul_sub(const fe2& a, const fe2& b, const fe2& c, const fe2& d) { return sub(mul(a, b), mul(c, d)); }
     static __device__ B2G_FQ2_CALL fe2 sqr(const fe2& a) {
         fe s = Fq::add(a.c0, a.c1), d = Fq::sub(a.c0, a.c1), m = Fq::mul(a.c0, a.c1);

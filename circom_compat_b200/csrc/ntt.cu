@@ -130,8 +130,7 @@ __device__ __forceinline__ void sm_put(uint32_t* sm, uint32_t tile, uint32_t i, 
     for (int l = 0; l < 8; l++) sm[l * tile + i] = v.l[l];
 }
 
-// 2 CTAs/SM (<= 64 registers): with one 512-thread CTA per SM every stage barrier idled the whole SM (ncu: register-limited
-// to 1 block, fmaheavy 45-52 %).  POINTWISE is a template parameter so that the plain passes do not carry the a*b accumulators.
+// 2 CTAs/SM (<= 64 registers): with one 512-thread CTA per SM every stage barrier would idle the whole SM.  POINTWISE is a template parameter so that the plain passes do not carry the a*b accumulators.
 template <bool POINTWISE>
 __global__ void __launch_bounds__(512, 2) ntt_pass_kernel(NttPassArgs A) {
     extern __shared__ __align__(16) uint32_t sm[];
@@ -397,11 +396,11 @@ void ntt_domain_create(NttDomain& d, int logn, cudaStream_t st, bool libsnark) {
     d.pass_sb[d.npass] = 0; d.pass_k[d.npass] = d.tl; d.pass_tl[d.npass] = d.tl; d.npass++;
     int rem = logn - d.tl;
     if (rem > 0) {
-        // index bits per strided pass.  Up to 2^20 the three vectors (96 MB) live in the 126 MB L2, 32-byte strided accesses cost
-        // nothing extra and the fewest passes win (1024 x 1 tiles; B2G_NTT_MAXK=5 / 6 = 2-D tiles measured equal, DESIGN.md section 8).
-        // From 2^21 on the passes stream from DRAM, where single 32-byte sectors at a 64 KB stride run at a fraction of the
-        // bandwidth: strided tiles become 2-D with rows of >= 8 consecutive elements (256 B), i.e. <= 7 index bits per pass
-        // (measured at 2^22: witness map 12.2 ms with 11 + 11 bits on 2048 x 1 tiles vs 6.8 ms with 10 + 6 + 6).
+        // index bits per strided pass.  At 2^20 the three vectors (96 MB) already exceed the H100's 50 MB L2, but 2-D tiles
+        // (B2G_NTT_MAXK=7) measured the same inside a whole 2^20 proof on an H100 (31.75 vs 31.84 proofs/s device-resident), so
+        // the fewest passes (1024 x 1 tiles) stay up to 2^20.  From 2^21 on, strided tiles become 2-D with rows of >= 8
+        // consecutive elements (256 B), i.e. <= 7 index bits per pass, so that no pass reads single 32-byte sectors at a
+        // stride of 64 KB or more from DRAM.
         int maxk = logn > 20 && d.tl > 7 ? 7 : d.tl;
         if (const char* e = getenv("B2G_NTT_MAXK")) { int v = atoi(e); if (v >= 1 && v <= d.tl) maxk = v; }
         int np = (rem + maxk - 1) / maxk, sb = d.tl;

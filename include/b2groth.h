@@ -1,4 +1,4 @@
-/* b2groth.h - C ABI of libb2groth.so, the B200-native (sm_100a CUDA) Groth16/BN254 prover hot path that stands in
+/* b2groth.h - C ABI of libb2groth.so, the H100-native (sm_90a CUDA) Groth16/BN254 prover hot path that stands in
  * for what ark-circom 0.5 obtains from ark-groth16 / ark-ec / ark-poly on the CPU.
  *
  * The reference (arkworks-rs/circom-compat) has no FFI; its extension points are Rust traits and generic functions.

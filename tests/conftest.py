@@ -11,17 +11,15 @@ GOLDEN = os.path.join(ROOT, 'tests', 'golden')
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with `-m gpu`)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; select with `-m gpu`)")
 
 
 def pytest_sessionstart(session):
-    """Build artefacts are git-ignored: compile them once if this checkout has none (nvcc cross-compiles without a GPU)."""
+    """Build artefacts are git-ignored: bring them up to date (nvcc cross-compiles without a GPU).  make rebuilds what is
+    missing or stale (e.g. objects from an older Makefile's architecture flags) and does nothing otherwise."""
     import subprocess
-    need = [os.path.join(ROOT, 'circom_compat_b200', 'libb2groth.so'), os.path.join(ROOT, 'circom_compat_b200', 'host', 'groth16_bench')]
-    if not all(os.path.exists(p) for p in need):
-        subprocess.check_call(['make', '-C', os.path.join(ROOT, 'circom_compat_b200', 'csrc'), '-j4'], stdout=subprocess.DEVNULL)
-    if not os.path.exists(os.path.join(ROOT, 'oracle', 'libcref.so')):
-        subprocess.check_call(['make', '-C', os.path.join(ROOT, 'oracle')], stdout=subprocess.DEVNULL)
+    subprocess.check_call(['make', '-C', os.path.join(ROOT, 'circom_compat_b200', 'csrc'), '-j4'], stdout=subprocess.DEVNULL)
+    subprocess.check_call(['make', '-C', os.path.join(ROOT, 'oracle')], stdout=subprocess.DEVNULL)
 
 
 @pytest.fixture(scope='session')

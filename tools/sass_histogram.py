@@ -2,7 +2,7 @@
 """Per-kernel SASS instruction histogram of libb2groth.so (cuobjdump -sass), the static evidence behind the pipe-bound
 claims in DESIGN.md: how many IMAD.WIDE (the 32x32->64 multiply-add the fmaheavy pipe issues once per 4 cycles per SM
 sub-partition), other IMAD-class instructions (same pipe, half cost), integer adds, global loads by width, and
-local-memory (stack) loads / stores each kernel contains.  Usage: python tools/sass_histogram.py [lib.so] > profiles/rN_sass_histogram.txt"""
+local-memory (stack) loads / stores each kernel contains.  Usage: python tools/sass_histogram.py [lib.so]"""
 import collections
 import os
 import re
@@ -38,7 +38,7 @@ for line in sass.splitlines():
 
 names = demangle(list(kernels))
 cols = ['total', 'IMAD.WIDE', 'IMAD other', 'IADD3/IADD', 'LOP3/SHF/SEL', 'LDG.128', 'LDG.256', 'LDG other', 'LDS/STS', 'LDL', 'STL', 'SHFL', 'BAR', 'CALL']
-print('# cuobjdump -sass', os.path.relpath(lib, ROOT), '(sm_100a).  Static instruction counts per kernel / device function.')
+print('# cuobjdump -sass', os.path.relpath(lib, ROOT), '(sm_90a).  Static instruction counts per kernel / device function.')
 print('# IMAD.WIDE = IMAD.WIDE(.U32)(.X); "IMAD other" = IMAD / IMAD.X / IMAD.MOV / IMAD.SHL / IMAD.IADD / IMAD.HI (same pipe); LDL/STL = local (stack) traffic')
 print('%-74s' % 'function' + ''.join('%13s' % c for c in cols))
 for k, cnt in kernels.items():
