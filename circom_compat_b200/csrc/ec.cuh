@@ -139,6 +139,59 @@ struct Curve {
 using G1 = Curve<Fq>;
 using G2 = Curve<Fq2>;
 
+// ---------------------------------------------------------------------------------------------- G2 on a lane pair
+// Two adjacent lanes (2k = A, 2k+1 = B) hold one XYZZ accumulator between them and split the ten Fq2 products of the mixed
+// addition 5 / 5 by role, running the same instruction sequence on lane-selected operands:
+//   lane A holds (X, ZZ) and the table point's x:   U2 = x2 ZZ1,   PP = P^2,  Q = X1 PP,    ZZ3 = ZZ1 PP,    R (Q - X3)
+//   lane B holds (Y, ZZZ) and the table point's y:  S2 = y2 ZZZ1,  RR = R^2,  PPP = P PP,   ZZZ3 = ZZZ1 PPP, Y1 PPP
+// Intermediates cross by __shfl_xor_sync(pair, ., 1); every branch is taken on values both lanes hold, so a pair never
+// diverges.  `s0` / `s1` are the lane's two coordinates (A: X, ZZ; B: Y, ZZZ) - the halves of the 256 B XYZZ record each
+// lane loads and stores - and `empty` (identical on both lanes) marks the accumulator at infinity (s0 = s1 = 0).
+struct G2Pair {
+    // acc = 2 q for the affine point q (mdbl-2008-s-1); `qc` is the lane's coordinate of q (A: x, B: y)
+    static __device__ __forceinline__ void dbl_affine(fe2& s0, fe2& s1, const fe2& qc, bool A, unsigned mask) {
+        const fe2 o1 = Fq2::sel(A, qc, Fq2::dbl(qc));                     // A: x,  B: U = 2y
+        const fe2 sq = Fq2::sqr_inline(o1), sq_o = Fq2::shfl_pair(mask, sq); // A: XX, B: V = U^2
+        const fe2 v = Fq2::sel(A, sq_o, sq), xx = Fq2::sel(A, sq, sq_o);
+        const fe2 m2 = Fq2::mul_inline(o1, v), m2_o = Fq2::shfl_pair(mask, m2);    // A: S = x V, B: W = U V
+        const fe2 s = Fq2::sel(A, m2, m2_o), w = Fq2::sel(A, m2_o, m2);
+        const fe2 m = Fq2::add(Fq2::dbl(xx), xx);
+        const fe2 x3 = Fq2::sub(Fq2::sqr_inline(m), Fq2::dbl(s));
+        const fe2 m4 = Fq2::mul_inline(Fq2::sel(A, m, w), Fq2::sel(A, Fq2::sub(s, x3), qc));   // A: M (S - X3), B: W y
+        const fe2 m4_o = Fq2::shfl_pair(mask, m4);
+        s0 = Fq2::sel(A, x3, Fq2::sub(m4_o, m4));
+        s1 = Fq2::sel(A, v, w);
+    }
+
+    // acc += q (madd-2008-s), every exceptional case handled; `qc` is the lane's coordinate of q (A: x, B: y)
+    static __device__ __forceinline__ void madd(fe2& s0, fe2& s1, bool& empty, const fe2& qc, bool A, unsigned mask) {
+        const bool qz = Fq2::is_zero(qc);
+        const bool qz_o = __shfl_xor_sync(mask, (int)qz, 1) != 0;
+        if (qz && qz_o) return;                                               // q at infinity
+        if (empty) { s0 = qc; s1 = Fq2::one(); empty = false; return; }
+        const fe2 d = Fq2::sub(Fq2::mul_inline(qc, s1), s0);                  // A: P = U2 - X1, B: R = S2 - Y1
+        const fe2 d_o = Fq2::shfl_pair(mask, d);
+        const bool z = Fq2::is_zero(d), z_o = Fq2::is_zero(d_o);
+        if (A ? z : z_o) {                                                    // P == 0: q == acc (R == 0) or q == -acc
+            if (A ? z_o : z) dbl_affine(s0, s1, qc, A, mask);
+            else { s0 = Fq2::zero(); s1 = Fq2::zero(); empty = true; }
+            return;
+        }
+        const fe2 u = Fq2::sel(A, s0, d_o);                                   // A: X1, B: P
+        const fe2 v = Fq2::sel(A, d_o, s0);                                   // A: R,  B: Y1
+        const fe2 sq = Fq2::sqr_inline(d);                                    // A: PP, B: RR
+        const fe2 pp = Fq2::sel(A, sq, Fq2::shfl_pair(mask, sq));
+        const fe2 m3 = Fq2::mul_inline(u, pp);                                // A: Q,  B: PPP
+        const fe2 rp = Fq2::shfl_pair(mask, Fq2::sub(sq, m3));                // A receives RR - PPP
+        const fe2 x3 = Fq2::sub(rp, Fq2::dbl(m3));                            // A: X3 = RR - PPP - 2Q
+        const fe2 b5 = Fq2::sel(A, Fq2::sub(m3, x3), m3);                     // A: Q - X3, B: PPP
+        s1 = Fq2::mul_inline(s1, Fq2::sel(A, pp, m3));                        // A: ZZ3 = ZZ1 PP, B: ZZZ3 = ZZZ1 PPP
+        const fe2 m5 = Fq2::mul_inline(v, b5);                                // A: R (Q - X3), B: Y1 PPP
+        const fe2 m5_o = Fq2::shfl_pair(mask, m5);
+        s0 = Fq2::sel(A, x3, Fq2::sub(m5_o, m5));                             // B: Y3 = R (Q - X3) - Y1 PPP
+    }
+};
+
 // curve constants b (y^2 = x^3 + b): G1 b = 3, G2 b = 3 / (9 + u)   (SURVEY.md App. A)
 __device__ __forceinline__ fe curve_b(const Fq*) { fe t = fe_zero(); t.l[0] = 3; return Fq::from_canonical(t); }
 __device__ __forceinline__ fe2 curve_b(const Fq2*) {

@@ -462,9 +462,8 @@ struct Fp {
     }
 
     // Column form of the same product: sixteen independent 8-limb chains on zero-initialised even/odd accumulators.  More
-    // ALU instructions than mul_wide() but no row-to-row dependency; the Fq2 routines, which run at 3 warps per scheduler
-    // inside the G2 accumulation kernel and live off instruction-level parallelism, use it (a choice carried over from the
-    // previous target GPU, not re-measured on H100).
+    // ALU instructions and live registers than mul_wide() but no row-to-row dependency; the called Fq2::mul uses it for the
+    // latency-bound single-thread chains (fold, reduce, glue).
     static __device__ __forceinline__ void mul_wide_cols(uint32_t* t, const fe& a, const fe& b) {
         uint32_t ev[17], od[16];
         #pragma unroll
@@ -538,8 +537,9 @@ using Fr = Fp<FrParams>;
 // ---------------------------------------------------------------------------------------------- Fq2 = Fq[u]/(u^2+1)
 struct fe2 { fe c0, c1; };
 
-// Fq2 mul / sqr are real calls: inlined, the G2 accumulation kernel grows to ~13 k instructions (a choice carried over from the
-// previous target GPU, where the inlined kernel was slower; not re-measured on H100)
+// Fq2 mul / sqr / mul_sub are real calls for the kernels that use the generic Curve<Fq2> formulas (key-load tables, fold,
+// reduce, glue): those are latency chains on few threads, and inlining every call multiplies their code size.  The G2
+// accumulation kernel does not use them: it runs the lane-pair addition of ec.cuh on mul_inline / sqr_inline.
 #define B2G_FQ2_CALL __noinline__
 struct Fq2 {
     using elem = fe2;
@@ -553,12 +553,20 @@ struct Fq2 {
     static __device__ __forceinline__ fe2 neg(const fe2& a) { fe2 r; r.c0 = Fq::neg(a.c0); r.c1 = Fq::neg(a.c1); return r; }
     // Karatsuba over Fq2 with lazy reduction: three 512-bit products, two Montgomery reductions
     //   c0 = a0 b0 - a1 b1,  c1 = (a0 + a1)(b0 + b1) - a0 b0 - a1 b1
-    static __device__ B2G_FQ2_CALL fe2 mul(const fe2& a, const fe2& b) {
+    // COLS picks the column form of the 512-bit products (Fq::mul_wide_cols) over the row form (Fq::mul_wide).
+    template <bool COLS>
+    static __device__ __forceinline__ fe2 karatsuba(const fe2& a, const fe2& b) {
         uint32_t v0[16], v1[16], v2[16];
         fe sa = add_noreduce(a.c0, a.c1), sb = add_noreduce(b.c0, b.c1);      // < 2p < 2^255
-        Fq::mul_wide_cols(v0, a.c0, b.c0);
-        Fq::mul_wide_cols(v1, a.c1, b.c1);
-        Fq::mul_wide_cols(v2, sa, sb);
+        if (COLS) {
+            Fq::mul_wide_cols(v0, a.c0, b.c0);
+            Fq::mul_wide_cols(v1, a.c1, b.c1);
+            Fq::mul_wide_cols(v2, sa, sb);
+        } else {
+            Fq::mul_wide(v0, a.c0, b.c0);
+            Fq::mul_wide(v1, a.c1, b.c1);
+            Fq::mul_wide(v2, sa, sb);
+        }
         Fq::sub_wide(v2, v0);
         Fq::sub_wide(v2, v1);                                                 // a0 b1 + a1 b0 in [0, 2 p^2)
         const uint32_t br = Fq::sub_wide(v0, v1);                             // a0 b0 - a1 b1 (mod 2^512)
@@ -566,6 +574,11 @@ struct Fq2 {
         fe2 r; r.c0 = Fq::redc(v0); r.c1 = Fq::redc(v2);
         return r;
     }
+    // the called form keeps the column products: no row-to-row dependency for the single-thread chains that call it
+    static __device__ B2G_FQ2_CALL fe2 mul(const fe2& a, const fe2& b) { return karatsuba<true>(a, b); }
+    // the inlined form uses the row products: 16 fewer live accumulator registers per product, which the lane-pair
+    // accumulation needs to stay inside 128 registers (and it has four independent warps per scheduler to hide latency)
+    static __device__ __forceinline__ fe2 mul_inline(const fe2& a, const fe2& b) { return karatsuba<false>(a, b); }
     static __device__ __forceinline__ fe add_noreduce(const fe& a, const fe& b) {
         fe s;
         asm("add.cc.u32 %0, %8, %16;\n\t"
@@ -581,12 +594,28 @@ struct Fq2 {
               "r"(b.l[0]), "r"(b.l[1]), "r"(b.l[2]), "r"(b.l[3]), "r"(b.l[4]), "r"(b.l[5]), "r"(b.l[6]), "r"(b.l[7]));
         return s;
     }
-    // two calls rather than a fused a*b - c*d with six wide products and two reductions: the fused form has fewer IMAD.WIDE but
-    // one long dependent chain, and was slower on the previous target GPU (not re-measured on H100)
+    // two calls rather than a fused a*b - c*d: only the glue kernels' handful of mixed additions use it (the G2 accumulation
+    // computes the two products on the two lanes of a pair)
     static __device__ B2G_FQ2_CALL fe2 mul_sub(const fe2& a, const fe2& b, const fe2& c, const fe2& d) { return sub(mul(a, b), mul(c, d)); }
-    static __device__ B2G_FQ2_CALL fe2 sqr(const fe2& a) {
+    // (a0 + a1 u)^2 = (a0 + a1)(a0 - a1) + 2 a0 a1 u: two Montgomery products
+    static __device__ __forceinline__ fe2 sqr_inline(const fe2& a) {
         fe s = Fq::add(a.c0, a.c1), d = Fq::sub(a.c0, a.c1), m = Fq::mul(a.c0, a.c1);
         fe2 r; r.c0 = Fq::mul(s, d); r.c1 = Fq::dbl(m);
+        return r;
+    }
+    static __device__ B2G_FQ2_CALL fe2 sqr(const fe2& a) { return sqr_inline(a); }
+    // c ? a : b without a branch (SEL per limb)
+    static __device__ __forceinline__ fe2 sel(bool c, const fe2& a, const fe2& b) {
+        fe2 r;
+        #pragma unroll
+        for (int i = 0; i < 8; i++) { r.c0.l[i] = c ? a.c0.l[i] : b.c0.l[i]; r.c1.l[i] = c ? a.c1.l[i] : b.c1.l[i]; }
+        return r;
+    }
+    // the value held by the other lane of an aligned lane pair (lanes 2k, 2k+1; `mask` names the pair)
+    static __device__ __forceinline__ fe2 shfl_pair(unsigned mask, const fe2& a) {
+        fe2 r;
+        #pragma unroll
+        for (int i = 0; i < 8; i++) { r.c0.l[i] = __shfl_xor_sync(mask, a.c0.l[i], 1); r.c1.l[i] = __shfl_xor_sync(mask, a.c1.l[i], 1); }
         return r;
     }
     static __device__ __noinline__ fe2 inv(const fe2& a) {

@@ -1,5 +1,6 @@
 // msm.cu - kernels and launchers of the fixed-base-table Pippenger MSM described in msm.cuh.
 #include <algorithm>
+#include <type_traits>
 #include <vector>
 #include "msm.cuh"
 #include "util.cuh"
@@ -370,21 +371,50 @@ __global__ void __launch_bounds__(128) msm_aff_apply_kernel(const void* __restri
 }
 
 // ------------------------------------------------------------------------------------------------ (4) accumulate
-// Thread t owns sorted positions [t*chunk, (t+1)*chunk).  Buckets that lie entirely inside the run are written to
-// buckets[]; a run's first / last segment that belongs to a bucket crossing the run boundary goes to frag_first[t] /
-// frag_last[t].
-// occupancy targets: G1 runs 4 CTAs/SM at 128 registers; G2 would sit just over the 3-CTA limit (170 registers), so it is capped
-// there (2 CTAs/SM leave the IMAD pipe waiting on dependent-issue latency with 2 warps per scheduler).  The register file is the
-// same 64 K x 32 bit per SM on H100 as on the parts these targets were first chosen for.
+// Run t = sorted positions [t*chunk, (t+1)*chunk), owned by one thread (G1) or one lane pair (G2).  Buckets that lie entirely
+// inside the run are written to buckets[]; a run's first / last segment that belongs to a bucket crossing the run boundary
+// goes to frag_first[t] / frag_last[t].
+// occupancy target: G1 runs 4 CTAs/SM at 128 registers.
 template <class F> struct AccOcc;
 #ifndef B2G_G1_CTAS
 #define B2G_G1_CTAS 4
 #endif
 template <> struct AccOcc<Fq> { static constexpr int MIN_CTAS = B2G_G1_CTAS; };
-#ifndef B2G_G2_CTAS
-#define B2G_G2_CTAS 3
-#endif
-template <> struct AccOcc<Fq2> { static constexpr int MIN_CTAS = B2G_G2_CTAS; };
+
+// slab_words != 0: the CTA's contiguous slab of the sorted entry list (G1: 128 runs = 32 KB at the default run length) is
+// brought into shared memory by ONE bulk asynchronous copy (cp.async.bulk -> UBLKCP, completion on an mbarrier) instead of
+// 64 strided 4-byte loads per run.  Every thread of the CTA calls this.
+__device__ __forceinline__ void acc_stage_slab(uint32_t* slab, unsigned long long* slab_bar, const uint32_t* __restrict__ entries,
+                                               uint64_t cta_first, uint32_t total, uint32_t slab_words) {
+    const uint32_t bar = (uint32_t)__cvta_generic_to_shared(slab_bar);
+    if (threadIdx.x == 0) {
+        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(bar));
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    if (threadIdx.x == 0 && cta_first < total) {
+        const uint64_t left = total - cta_first;
+        const uint32_t bytes = (uint32_t)(((left < slab_words ? left : (uint64_t)slab_words) * 4 + 15) & ~15ull);    // the list is padded by 16 B
+        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(bar), "r"(bytes) : "memory");
+        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                     :: "r"((uint32_t)__cvta_generic_to_shared(slab)), "l"(entries + cta_first), "r"(bytes), "r"(bar) : "memory");
+    }
+    if (cta_first < total) {
+        uint32_t done = 0;
+        while (!done)
+            asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(done) : "r"(bar) : "memory");
+    }
+}
+
+// first bucket of the run starting at `start`: largest b with offsets[b] <= start, skipping empty buckets that share the offset
+__device__ __forceinline__ uint32_t acc_first_bucket(const uint32_t* __restrict__ offsets, uint32_t nb, uint32_t start, uint32_t& bucket_end) {
+    uint32_t lo = 0, hi = nb;                       // invariant: offsets[lo] <= start < offsets[hi]
+    while (hi - lo > 1) { uint32_t mid = (lo + hi) >> 1; if (offsets[mid] <= start) lo = mid; else hi = mid; }
+    uint32_t b = lo;
+    bucket_end = offsets[b + 1];
+    while (bucket_end <= start) { b++; bucket_end = offsets[b + 1]; }
+    return b;
+}
 
 template <class C, class F>
 __global__ void __launch_bounds__(128, AccOcc<F>::MIN_CTAS) msm_accumulate_kernel(const void* __restrict__ table, const uint32_t* __restrict__ entries,
@@ -394,41 +424,15 @@ __global__ void __launch_bounds__(128, AccOcc<F>::MIN_CTAS) msm_accumulate_kerne
     const uint32_t total = offsets[nb];
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     const uint64_t start64 = (uint64_t)t * chunk;
-    // slab_words != 0 (default for G1): the CTA's contiguous slab of the sorted entry list (128 runs = 32 KB at the default run
-    // length) is brought into shared memory by ONE bulk asynchronous copy (cp.async.bulk -> UBLKCP, completion on an mbarrier)
-    // instead of 64 strided 4-byte loads per thread
     extern __shared__ __align__(128) uint32_t slab[];
     __shared__ __align__(8) unsigned long long slab_bar;
     const uint64_t cta_first = (uint64_t)blockIdx.x * blockDim.x * chunk;
-    if (slab_words) {
-        const uint32_t bar = (uint32_t)__cvta_generic_to_shared(&slab_bar);
-        if (threadIdx.x == 0) {
-            asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(bar));
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        }
-        __syncthreads();
-        if (threadIdx.x == 0 && cta_first < total) {
-            const uint64_t left = total - cta_first;
-            const uint32_t bytes = (uint32_t)(((left < slab_words ? left : (uint64_t)slab_words) * 4 + 15) & ~15ull);    // the list is padded by 16 B
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(bar), "r"(bytes) : "memory");
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                         :: "r"((uint32_t)__cvta_generic_to_shared(slab)), "l"(entries + cta_first), "r"(bytes), "r"(bar) : "memory");
-        }
-        if (cta_first < total) {
-            uint32_t done = 0;
-            while (!done)
-                asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(done) : "r"(bar) : "memory");
-        }
-    }
+    if (slab_words) acc_stage_slab(slab, &slab_bar, entries, cta_first, total, slab_words);
     if (start64 >= total) return;
     const uint32_t start = (uint32_t)start64;
     const uint32_t end = (uint32_t)min((uint64_t)total, start64 + chunk);
-    // bucket containing `start`: largest b with offsets[b] <= start (and non-empty by construction of the search)
-    uint32_t lo = 0, hi = nb;                       // invariant: offsets[lo] <= start < offsets[hi]
-    while (hi - lo > 1) { uint32_t mid = (lo + hi) >> 1; if (offsets[mid] <= start) lo = mid; else hi = mid; }
-    uint32_t b = lo;
-    uint32_t bucket_end = offsets[b + 1];
-    while (bucket_end <= start) { b++; bucket_end = offsets[b + 1]; }    // skip empty buckets sharing the offset
+    uint32_t bucket_end;
+    uint32_t b = acc_first_bucket(offsets, nb, start, bucket_end);
     Pt acc = C::infinity();
     uint32_t seg_start = start;
     for (uint32_t pos = start; pos < end;) {
@@ -443,6 +447,56 @@ __global__ void __launch_bounds__(128, AccOcc<F>::MIN_CTAS) msm_accumulate_kerne
             else if (seg_start == start) pt_store<F>(frag_first, t, acc);
             else pt_store<F>(frag_last, t, acc);
             acc = C::infinity();
+            seg_start = pos;
+            if (pos == bucket_end && pos < end) {
+                do { b++; bucket_end = offsets[b + 1]; } while (bucket_end <= pos);
+            }
+        }
+    }
+}
+
+// G2: lane pair t (threads 2t, 2t+1 of the grid) owns run t and runs the lane-pair mixed addition of ec.cuh (G2Pair).  Both
+// lanes walk the same entries; each loads its 64 B half of the 128 B table row (A: x, B: y - so the sign of an entry
+// negates on lane B) and stores its two coordinates of the 256 B XYZZ record (A: X, ZZ at bytes 0 / 128; B: Y, ZZZ at 64 / 192).
+// 3 CTAs x 128 threads per SM (166 registers, no stack): 192 chains per SM.  Capped at 128 registers for 4 CTAs/SM the kernel
+// spills ~150 B per thread and measured slower (H100 80GB HBM3, 400 W: 9.04-9.08 ms vs 8.49-8.52 ms per 2^20 accumulation).
+__global__ void __launch_bounds__(128, 3) msm_accumulate_g2_kernel(const void* __restrict__ table, const uint32_t* __restrict__ entries,
+                                      const uint32_t* __restrict__ offsets, uint32_t nb, uint32_t chunk,
+                                      void* __restrict__ buckets, void* __restrict__ frag_first, void* __restrict__ frag_last, uint32_t slab_words) {
+    const uint32_t total = offsets[nb];
+    const uint32_t t = (blockIdx.x * blockDim.x + threadIdx.x) >> 1;
+    const uint32_t half = threadIdx.x & 1u;
+    const bool A = half == 0;
+    const unsigned mask = 3u << (threadIdx.x & 30u);
+    const uint64_t start64 = (uint64_t)t * chunk;
+    extern __shared__ __align__(128) uint32_t slab[];
+    __shared__ __align__(8) unsigned long long slab_bar;
+    const uint64_t cta_first = (uint64_t)blockIdx.x * (blockDim.x / 2) * chunk;
+    if (slab_words) acc_stage_slab(slab, &slab_bar, entries, cta_first, total, slab_words);
+    if (start64 >= total) return;
+    const uint32_t start = (uint32_t)start64;
+    const uint32_t end = (uint32_t)min((uint64_t)total, start64 + chunk);
+    uint32_t bucket_end;
+    uint32_t b = acc_first_bucket(offsets, nb, start, bucket_end);
+    fe2 s0 = Fq2::zero(), s1 = Fq2::zero();
+    bool empty = true;
+    uint32_t seg_start = start;
+    for (uint32_t pos = start; pos < end;) {
+        const uint32_t e = slab_words ? slab[pos - (uint32_t)cta_first] : (entries ? entries[pos] : pos);   // entries == nullptr: `table` is a pre-reduced point list (4a)
+        fe2 qc;
+        elem_load_nc(qc, (const char*)table + (size_t)(e & 0x7fffffffu) * 128 + half * 64);
+        qc = Fq2::sel((e >> 31) && !A, Fq2::neg(qc), qc);
+        G2Pair::madd(s0, s1, empty, qc, A, mask);
+        pos++;
+        if (pos == bucket_end || pos == end) {
+            const uint32_t bucket_start = offsets[b];
+            char* rec;
+            if (bucket_start >= start && bucket_end <= end) rec = (char*)buckets + (size_t)b * 256;
+            else if (seg_start == start) rec = (char*)frag_first + (size_t)t * 256;
+            else rec = (char*)frag_last + (size_t)t * 256;
+            elem_store(rec + half * 64, s0);
+            elem_store(rec + 128 + half * 64, s1);
+            s0 = Fq2::zero(); s1 = Fq2::zero(); empty = true;
             seg_start = pos;
             if (pos == bucket_end && pos < end) {
                 do { b++; bucket_end = offsets[b + 1]; } while (bucket_end <= pos);
@@ -730,6 +784,20 @@ void msm_sort(const MsmPlan& plan, MsmScratch& s, const fe* scalars_dev, uint32_
     CUDA_CHECK(cudaGetLastError());
 }
 
+// one accumulation launch over `nruns` runs: one thread per run for G1, one lane pair per run for G2 (64 runs per CTA)
+template <class C, class F>
+static void launch_accumulate(const void* table, const uint32_t* entries, const uint32_t* offsets, uint32_t nb, uint32_t chunk, uint32_t nruns,
+                              const MsmScratch& s, bool bulk, cudaStream_t st) {
+    constexpr bool g2 = std::is_same<F, Fq2>::value;
+    constexpr uint32_t runs_per_cta = g2 ? 64u : 128u;
+    const uint32_t slab_words = bulk && (size_t)chunk * runs_per_cta * 4 <= 48 * 1024 ? chunk * runs_per_cta : 0u;
+    const unsigned blocks = (unsigned)(((uint64_t)nruns + runs_per_cta - 1) / runs_per_cta);
+    if constexpr (g2)
+        msm_accumulate_g2_kernel<<<blocks, 128, (size_t)slab_words * 4, st>>>(table, entries, offsets, nb, chunk, s.buckets, s.frag_first, s.frag_last, slab_words);
+    else
+        msm_accumulate_kernel<C, F><<<blocks, 128, (size_t)slab_words * 4, st>>>(table, entries, offsets, nb, chunk, s.buckets, s.frag_first, s.frag_last, slab_words);
+}
+
 template <class C, class F>
 static void msm_accumulate_t(const MsmPlan& plan, const MsmScratch& sorted, MsmScratch& s, cudaStream_t st) {
     using Pt = typename C::Pt;
@@ -767,17 +835,15 @@ static void msm_accumulate_t(const MsmPlan& plan, const MsmScratch& sorted, MsmS
         g_launch_count += 3 * rounds;
         offsets = sorted.aff_off[rounds];
         const uint32_t nthreads_r = (uint32_t)(((uint64_t)sorted.aff_nmax[rounds] + chunk - 1) / chunk);
-        msm_accumulate_kernel<C, F><<<(nthreads_r + 127) / 128, 128, 0, st>>>(prev, nullptr, offsets, nb, chunk, s.buckets, s.frag_first, s.frag_last, 0u);
+        launch_accumulate<C, F>(prev, nullptr, offsets, nb, chunk, nthreads_r, s, false, st);
     } else
     {
-        // the bulk-staged slab is on for G1, off for G2 (the split chosen on the previous target GPU).  On an H100 (700 W, 2^20
-        // chain) neither switch is measurable: G1 accumulation 2.66-2.68 ms on vs 2.69 ms off, G2 8.46-8.52 ms off vs 8.45 ms
-        // on, whole proof within the run-to-run spread.  B2G_ACC_BULK=0 / 1 forces it off / on for both
+        // the bulk-staged slab is on for G1, off for G2.  On an H100 (2^20 chain) neither switch is measurable: G1 accumulation
+        // 2.66-2.68 ms on vs 2.69 ms off (700 W); lane-pair G2 at 4 CTAs/SM 9.04-9.08 ms off vs 9.12 ms on (400 W).
+        // B2G_ACC_BULK=0 / 1 forces it off / on for both
         static const char* bulk_env = getenv("B2G_ACC_BULK");
         const bool bulk = bulk_env && *bulk_env ? *bulk_env == '1' : !plan.g2;
-        const uint32_t slab_words = bulk && (size_t)chunk * 128 * 4 <= 48 * 1024 ? chunk * 128u : 0u;
-        msm_accumulate_kernel<C, F><<<(nthreads + 127) / 128, 128, (size_t)slab_words * 4, st>>>(plan.table, sorted.entries, sorted.offsets, nb, chunk, s.buckets, s.frag_first,
-                                                                                                  s.frag_last, slab_words);
+        launch_accumulate<C, F>(plan.table, sorted.entries, sorted.offsets, nb, chunk, nthreads, s, bulk, st);
     }
     if (s.prof1) CUDA_CHECK(cudaEventRecord(s.prof1, st));
     cudaStream_t main_st = st;
