@@ -406,6 +406,8 @@ __device__ __forceinline__ void acc_stage_slab(uint32_t* slab, unsigned long lon
     }
 }
 
+constexpr int MSM_SLAB_MAX_BYTES = 48 * 1024;   // larger slabs are not staged: the runs read the entry list directly
+
 // first bucket of the run starting at `start`: largest b with offsets[b] <= start, skipping empty buckets that share the offset
 __device__ __forceinline__ uint32_t acc_first_bucket(const uint32_t* __restrict__ offsets, uint32_t nb, uint32_t start, uint32_t& bucket_end) {
     uint32_t lo = 0, hi = nb;                       // invariant: offsets[lo] <= start < offsets[hi]
@@ -688,6 +690,13 @@ void msm_scratch_alloc(MsmScratch& s, uint32_t n, int nwin, uint32_t nbuckets, b
     const size_t nent = (size_t)n * nwin;
     const size_t nchunks = (nent + s.chunk - 1) / s.chunk + 1;
     s.reduce_chunk = env_u32("B2G_MSM_REDUCE_CHUNK", MSM_REDUCE_CHUNK_DEFAULT);
+    // the bulk-staged slab of the accumulation is on for G1, off for G2.  On an H100 (2^20 chain) neither switch is
+    // measurable: G1 accumulation 2.66-2.68 ms on vs 2.69 ms off (700 W); lane-pair G2 at 4 CTAs/SM 9.04-9.08 ms off vs
+    // 9.12 ms on (400 W).  B2G_ACC_BULK=0 / 1 forces it off / on for both; read here, like the chunk, for every scratch
+    {
+        const char* bulk_env = getenv("B2G_ACC_BULK");
+        s.bulk = bulk_env && *bulk_env ? *bulk_env == '1' : !g2;
+    }
     const size_t npart = (size_t)nbuckets / (s.reduce_chunk * 32) + 64;
     if (with_sort) {
         CUDA_CHECK(cudaMalloc(&s.counts, (size_t)nbuckets * 4));
@@ -790,7 +799,7 @@ static void launch_accumulate(const void* table, const uint32_t* entries, const 
                               const MsmScratch& s, bool bulk, cudaStream_t st) {
     constexpr bool g2 = std::is_same<F, Fq2>::value;
     constexpr uint32_t runs_per_cta = g2 ? 64u : 128u;
-    const uint32_t slab_words = bulk && (size_t)chunk * runs_per_cta * 4 <= 48 * 1024 ? chunk * runs_per_cta : 0u;
+    const uint32_t slab_words = bulk && (size_t)chunk * runs_per_cta * 4 <= MSM_SLAB_MAX_BYTES ? chunk * runs_per_cta : 0u;
     const unsigned blocks = (unsigned)(((uint64_t)nruns + runs_per_cta - 1) / runs_per_cta);
     if constexpr (g2)
         msm_accumulate_g2_kernel<<<blocks, 128, (size_t)slab_words * 4, st>>>(table, entries, offsets, nb, chunk, s.buckets, s.frag_first, s.frag_last, slab_words);
@@ -836,14 +845,8 @@ static void msm_accumulate_t(const MsmPlan& plan, const MsmScratch& sorted, MsmS
         offsets = sorted.aff_off[rounds];
         const uint32_t nthreads_r = (uint32_t)(((uint64_t)sorted.aff_nmax[rounds] + chunk - 1) / chunk);
         launch_accumulate<C, F>(prev, nullptr, offsets, nb, chunk, nthreads_r, s, false, st);
-    } else
-    {
-        // the bulk-staged slab is on for G1, off for G2.  On an H100 (2^20 chain) neither switch is measurable: G1 accumulation
-        // 2.66-2.68 ms on vs 2.69 ms off (700 W); lane-pair G2 at 4 CTAs/SM 9.04-9.08 ms off vs 9.12 ms on (400 W).
-        // B2G_ACC_BULK=0 / 1 forces it off / on for both
-        static const char* bulk_env = getenv("B2G_ACC_BULK");
-        const bool bulk = bulk_env && *bulk_env ? *bulk_env == '1' : !plan.g2;
-        launch_accumulate<C, F>(plan.table, sorted.entries, sorted.offsets, nb, chunk, nthreads, s, bulk, st);
+    } else {
+        launch_accumulate<C, F>(plan.table, sorted.entries, sorted.offsets, nb, chunk, nthreads, s, s.bulk, st);
     }
     if (s.prof1) CUDA_CHECK(cudaEventRecord(s.prof1, st));
     cudaStream_t main_st = st;
@@ -874,6 +877,12 @@ void msm_run(const MsmPlan& plan, MsmScratch& s, const fe* scalars_dev, uint32_t
     msm_accumulate(plan, s, s, st);
 }
 
-void msm_init_kernels() {}   // all tail kernels use < 48 KiB of dynamic shared memory
+// A full entry slab is 48 KiB (G1 128 runs x 96 entries, G2 64 runs x 192) on top of the accumulation kernels' static mbarrier
+// word, which is more than the default dynamic limit (48 KiB minus the static size): without the opt-in such launches fail
+// with "invalid argument".  The tail kernels use < 48 KiB of dynamic shared memory.
+void msm_init_kernels() {
+    CUDA_CHECK(cudaFuncSetAttribute(msm_accumulate_kernel<G1, Fq>, cudaFuncAttributeMaxDynamicSharedMemorySize, MSM_SLAB_MAX_BYTES));
+    CUDA_CHECK(cudaFuncSetAttribute(msm_accumulate_g2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, MSM_SLAB_MAX_BYTES));
+}
 
 }  // namespace b2g

@@ -49,6 +49,7 @@ struct MsmScratch {                      // one per in-flight MSM
     void *frag_first = nullptr, *frag_last = nullptr, *buckets = nullptr, *partials = nullptr, *result = nullptr;
     fe* scalars_canon = nullptr;         // n canonical scalars (filled by the digit pass)
     bool g2 = false, result_owned = false;
+    bool bulk = false;                   // stage each CTA's slab of the entry list by one bulk copy (B2G_ACC_BULK)
     cudaEvent_t prof0 = nullptr, prof1 = nullptr;   // optional: bracket the accumulate kernel (b2g_bench_msm)
     cudaStream_t tail = nullptr;                     // high-priority stream for the low-parallelism fold / weighted-sum kernels
     cudaEvent_t ev_acc = nullptr, ev_tail = nullptr;

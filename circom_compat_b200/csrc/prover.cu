@@ -418,7 +418,68 @@ __global__ void __launch_bounds__(128) fixed_base_kernel(const void* __restrict_
     aff_store<F>(out, i, C::to_affine(acc));
 }
 
+// Bytes per row of each test op's operands and result (0: operand not read).  XYZZ records are 4 coordinates (G1 128 B,
+// G2 256 B); a G2Pair entry is a 128 B affine point followed by a 32 B word whose bit 0 is the entry's sign.
+struct TestOpShape { uint32_t a, b, out, threads; };
+constexpr int TEST_PAIR_RUN = 16;                          // entries one lane pair folds in op 27
+constexpr uint32_t TEST_PAIR_ENTRY = 160;
+static bool test_op_shape(int op, TestOpShape& s) {
+    if (op < 0 || op > 29) return false;
+    if (op <= 7 || (op >= 14 && op <= 16)) s = {32, (op == 6 || op == 7) ? 0u : 32u, 32, 1};
+    else if (op == 8 || op == 12) s = {64, 64, 64, 1};
+    else if (op == 10) s = {64, 0, 64, 1};
+    else if (op == 9 || op == 13) s = {128, 128, 128, 1};
+    else if (op == 11) s = {128, 0, 128, 1};
+    else if (op <= 19 || op == 28) s = {64, 64, 64, 1};
+    else if (op == 20) s = {128, 128, 128, 1};
+    else if (op == 21) s = {128, 64, 128, 1};
+    else if (op == 22) s = {128, 0, 128, 1};
+    else if (op == 23) s = {256, 256, 256, 1};
+    else if (op == 24) s = {256, 128, 256, 1};
+    else if (op == 25) s = {256, 0, 256, 1};
+    else if (op == 26) s = {256, TEST_PAIR_ENTRY, 256, 2};
+    else if (op == 27) s = {TEST_PAIR_RUN * TEST_PAIR_ENTRY, 0, 256, 2};
+    else s = {32, 32, 64, 1};                              // 29
+    return true;
+}
+
+// the lane's coordinate of a signed G2Pair entry, negated on lane B only (as msm_accumulate_g2_kernel applies an entry's sign)
+__device__ __forceinline__ fe2 test_pair_entry(const uint8_t* e, bool A) {
+    fe2 qc;
+    elem_load(qc, e + (A ? 0 : 64));
+    const bool neg = (*reinterpret_cast<const uint32_t*>(e + 128) & 1u) != 0;
+    return Fq2::sel(neg && !A, Fq2::neg(qc), qc);
+}
+
+// ops 26 / 27: lane pair `row` (threads 2 row, 2 row + 1) runs G2Pair::madd and stores the raw record as the accumulation
+// kernel does (A: X, ZZ; B: Y, ZZZ)
+__device__ __forceinline__ void test_op_pair(int op, const uint8_t* __restrict__ a, const uint8_t* __restrict__ b, uint32_t n,
+                                             uint8_t* __restrict__ out) {
+    const uint32_t row = (blockIdx.x * blockDim.x + threadIdx.x) >> 1;
+    if (row >= n) return;                                  // both lanes of a pair leave together
+    const uint32_t half = threadIdx.x & 1u;
+    const bool A = half == 0;
+    const unsigned mask = 3u << (threadIdx.x & 30u);
+    fe2 s0 = Fq2::zero(), s1 = Fq2::zero();
+    bool empty = true;
+    if (op == 26) {                                        // one addition onto a given record (empty iff ZZ == 0)
+        const uint8_t* rec = a + (size_t)row * 256;
+        fe2 zz; elem_load(zz, rec + 128);
+        empty = Fq2::is_zero(zz);
+        if (!empty) { elem_load(s0, rec + half * 64); elem_load(s1, rec + 128 + half * 64); }
+        G2Pair::madd(s0, s1, empty, test_pair_entry(b + (size_t)row * TEST_PAIR_ENTRY, A), A, mask);
+    } else {                                               // one run of TEST_PAIR_RUN entries from empty
+        const uint8_t* run = a + (size_t)row * (TEST_PAIR_RUN * TEST_PAIR_ENTRY);
+        #pragma unroll 1
+        for (int k = 0; k < TEST_PAIR_RUN; k++) G2Pair::madd(s0, s1, empty, test_pair_entry(run + k * TEST_PAIR_ENTRY, A), A, mask);
+    }
+    uint8_t* rec = out + (size_t)row * 256;
+    elem_store(rec + half * 64, s0);
+    elem_store(rec + 128 + half * 64, s1);
+}
+
 __global__ void test_op_kernel(int op, const uint8_t* __restrict__ a, const uint8_t* __restrict__ b, uint32_t n, uint8_t* __restrict__ out) {
+    if (op == 26 || op == 27) { test_op_pair(op, a, b, n, out); return; }
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     if (op <= 7) {
@@ -460,14 +521,34 @@ __global__ void test_op_kernel(int op, const uint8_t* __restrict__ a, const uint
         else if (op == 15) r = Fq::mul_sub(x, y, y, y);
         else { uint32_t t[16]; Fq::mul_wide(t, x, y); r = Fq::redc(t); }
         fe_store(out + 32 * (size_t)i, r);
-    } else {                    // 17 fq2_mul, 18 fq2_sqr, 19 fq2_mul_sub(a, b, b, swap(a))
+    } else if (op <= 19 || op == 28) {   // 17 fq2_mul, 18 fq2_sqr, 19 fq2_mul_sub(a, b, b, swap(a)), 28 fq2_mul_inline
         fe2 x, y, r;
         x.c0 = fe_load(a + 64 * (size_t)i); x.c1 = fe_load(a + 64 * (size_t)i + 32);
         y.c0 = fe_load(b + 64 * (size_t)i); y.c1 = fe_load(b + 64 * (size_t)i + 32);
         if (op == 17) r = Fq2::mul(x, y);
         else if (op == 18) r = Fq2::sqr(x);
+        else if (op == 28) r = Fq2::mul_inline(x, y);
         else { fe2 z; z.c0 = x.c1; z.c1 = x.c0; r = Fq2::mul_sub(x, y, y, z); }
         fe_store(out + 64 * (size_t)i, r.c0); fe_store(out + 64 * (size_t)i + 32, r.c1);
+    } else if (op <= 22) {      // G1 on raw XYZZ records, result not normalised: 20 add(a, b), 21 madd(a, affine b), 22 dbl(a)
+        G1::Pt acc = pt_load<Fq>(a, i);
+        if (op == 20) { G1::Pt q = pt_load<Fq>(b, i); G1::add(acc, q); }
+        else if (op == 21) G1::madd(acc, aff_load<Fq>(b, i));
+        else acc = G1::dbl(acc);
+        pt_store<Fq>(out, i, acc);
+    } else if (op <= 25) {      // the same for G2: 23 add, 24 madd, 25 dbl
+        G2::Pt acc = pt_load<Fq2>(a, i);
+        if (op == 23) { G2::Pt q = pt_load<Fq2>(b, i); G2::add(acc, q); }
+        else if (op == 24) G2::madd(acc, aff_load<Fq2>(b, i));
+        else acc = G2::dbl(acc);
+        pt_store<Fq2>(out, i, acc);
+    } else {                    // 29: the plain 512-bit product a * b (a < 2^255)
+        uint32_t t[16];
+        Fq::mul_wide(t, fe_load(a + 32 * (size_t)i), fe_load(b + 32 * (size_t)i));
+        fe lo, hi;
+        #pragma unroll
+        for (int k = 0; k < 8; k++) { lo.l[k] = t[k]; hi.l[k] = t[8 + k]; }
+        fe_store(out + 64 * (size_t)i, lo); fe_store(out + 64 * (size_t)i + 32, hi);
     }
 }
 
@@ -1403,19 +1484,21 @@ int b2g_fixed_base_g2(b2g_ctx* ctx, const void* scalars_canon, size_t n, void* o
 
 int b2g_test_op(b2g_ctx* ctx, int op, const void* a, const void* b, size_t n, void* out) {
     return guarded([&] {
-        if (!ctx || !a || !out || op < 0 || op > 19) throw_error(B2G_E_SHAPE, "bad arguments");
+        TestOpShape s;
+        if (!ctx || !a || !out || !test_op_shape(op, s)) throw_error(B2G_E_SHAPE, "bad arguments");
+        if (!b && s.b && s.b != s.a) throw_error(B2G_E_SHAPE, "this op needs operand b");
         if (n == 0) return;
         DevGuard g(ctx->device);
         cudaStream_t st = ctx->st[0];
-        const size_t esz = (op <= 7 || (op >= 14 && op <= 16)) ? 32 : ((op == 9 || op == 11 || op == 13) ? 128 : 64);
-        uint8_t* da = dev_upload<uint8_t>(a, n * esz, st);
-        uint8_t* db = dev_upload<uint8_t>(b ? b : a, n * esz, st);
-        uint8_t* dout = nullptr; CUDA_CHECK(cudaMalloc(&dout, n * esz));
-        test_op_kernel<<<(unsigned)((n + 63) / 64), 64, 0, st>>>(op, da, db, (uint32_t)n, dout);
+        uint8_t* da = dev_upload<uint8_t>(a, n * s.a, st);
+        uint8_t* db = s.b ? dev_upload<uint8_t>(b ? b : a, n * s.b, st) : nullptr;
+        uint8_t* dout = nullptr; CUDA_CHECK(cudaMalloc(&dout, n * s.out));
+        const size_t threads = n * s.threads;
+        test_op_kernel<<<(unsigned)((threads + 63) / 64), 64, 0, st>>>(op, da, db, (uint32_t)n, dout);
         g_launch_count += 1;
-        CUDA_CHECK(cudaMemcpyAsync(out, dout, n * esz, cudaMemcpyDeviceToHost, st));
+        CUDA_CHECK(cudaMemcpyAsync(out, dout, n * s.out, cudaMemcpyDeviceToHost, st));
         cudaError_t e = cudaStreamSynchronize(st);
-        cudaFree(da); cudaFree(db); cudaFree(dout);
+        cudaFree(da); if (db) cudaFree(db); cudaFree(dout);
         CUDA_CHECK(e);
     });
 }

@@ -28,6 +28,15 @@ def _c(a, dtype=np.uint64):
     return np.ascontiguousarray(a, dtype=dtype)
 
 
+# b2g_test_op (include/b2groth.h): 64-bit words per row of operand a, operand b (0: not read) and the result
+_TEST_OP_WORDS = {**{op: (4, 4, 4) for op in (0, 1, 2, 3, 4, 5, 14, 15, 16)}, 6: (4, 0, 4), 7: (4, 0, 4),
+                  8: (8, 8, 8), 10: (8, 0, 8), 12: (8, 8, 8), 9: (16, 16, 16), 11: (16, 0, 16), 13: (16, 16, 16),
+                  17: (8, 8, 8), 18: (8, 8, 8), 19: (8, 8, 8), 28: (8, 8, 8),
+                  20: (16, 16, 16), 21: (16, 8, 16), 22: (16, 0, 16), 23: (32, 32, 32), 24: (32, 16, 32), 25: (32, 0, 32),
+                  26: (32, 20, 32), 27: (16 * 20, 0, 32), 29: (4, 4, 8)}
+TEST_PAIR_RUN = 16            # entries per row of op 27; an entry is 16 words of affine point + 4 words whose bit 0 is the sign
+
+
 # Device-resident keys / matrices are cached per (host object, device, shard): every Context of that device and shard
 # can use them, so several proofs can be in flight on one GPU (one Context per in-flight proof) without duplicating
 # the 6 GiB of tables.  release(obj) / release_all() free them.
@@ -171,10 +180,13 @@ class Context:
         return out
 
     def test_op(self, op: int, a, b=None) -> np.ndarray:
+        """b2g_test_op: n rows of operand a (and b), returns (n, result words) uint64.  Sizes per op: _TEST_OP_WORDS."""
         a = _c(a); b = _c(b) if b is not None else None
-        words = 4 if (op <= 7 or 14 <= op <= 16) else (16 if op in (9, 11, 13) else 8)
-        n = a.size // words
-        out = np.zeros_like(a)
+        a_words, b_words, out_words = _TEST_OP_WORDS.get(op, (4, 4, 4))    # an unknown op is refused by the library
+        n = a.size // a_words
+        if b is not None and b_words and b.size < n * b_words:
+            raise ValueError(f"test op {op}: operand b holds fewer than {n} rows of {b_words} words")
+        out = np.zeros((n, out_words), dtype=np.uint64)
         N.check(N.lib().b2g_test_op(self._h, op, _ptr(a), _ptr(b) if b is not None else None, n, _ptr(out)))
         return out
 

@@ -178,7 +178,16 @@ B2G_API int b2g_fixed_base_g2(b2g_ctx* ctx, const void* scalars_canon, size_t n,
  * op: 0 fq_mul, 1 fq_add, 2 fq_sub, 3 fr_mul, 4 fr_add, 5 fr_sub, 6 fq_inv, 7 fr_inv (b ignored),
  *     8 g1_add (a, b, out = n x 64 B affine), 9 g2_add (n x 128 B), 10 g1_dbl, 11 g2_dbl (b ignored),
  *     12 g1 mixed add, 13 g2 mixed add, 14 fq_sqr, 15 fq a*b - b*b, 16 fq mul through the lazy-reduction blocks (32 B),
- *     17 fq2_mul, 18 fq2_sqr, 19 fq2 a*b - b*swap(a) (n x 64 B: c0 || c1). */
+ *     17 fq2_mul, 18 fq2_sqr, 19 fq2 a*b - b*swap(a) (n x 64 B: c0 || c1).
+ * Ops 20 and up take and return raw XYZZ records (X || Y || ZZ || ZZZ, Montgomery, infinity iff ZZ == 0; G1 128 B, G2 256 B)
+ * and do not normalise the result:
+ *     20 g1 add(a, b), 21 g1 madd(a, b = 64 B affine), 22 g1 dbl(a); 23 g2 add, 24 g2 madd (b = 128 B affine), 25 g2 dbl,
+ *     26 one G2 lane-pair mixed addition (the G2 accumulation kernel's) onto record a of entry b,
+ *     27 one lane pair folds a run of 16 entries (a = 16 x 160 B) from empty, out = the record as the two lanes store it;
+ *        an entry is a 128 B affine point and a 32 B word whose bit 0 negates it,
+ *     28 fq2 product as the G2 accumulation kernel inlines it (n x 64 B),
+ *     29 fq plain 512-bit product a * b for a < 2^255 (a, b: 32 B; out: 64 B little-endian).
+ * Operand and result sizes per row therefore differ by op; b may be NULL where the op does not read it. */
 B2G_API int b2g_test_op(b2g_ctx* ctx, int op, const void* a, const void* b, size_t n, void* out);
 
 /* Timing of the last b2g_prove / b2g_prove_partial on this ctx, CUDA-event milliseconds:

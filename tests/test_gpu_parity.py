@@ -8,7 +8,9 @@ import numpy as np
 import pytest
 
 from oracle import cref as c
+from oracle import msm_digits as md
 from oracle import pyref as o
+from oracle import xyzz as X
 
 pytestmark = pytest.mark.gpu
 
@@ -79,6 +81,19 @@ def test_lazy_reduction_blocks(ctx):
         p1, p2 = mul2(a, b), mul2(b, (a[1], a[0]))
         exp.append(((p1[0] - p2[0]) % q, (p1[1] - p2[1]) % q))
     assert c.limbs_to_ints(ctx.test_op(19, xl, yl)) == flat(exp)
+    # the inlined Karatsuba the G2 accumulation runs (row products); pairs such as (q-1, q-2) make a0 + a1 close to 2q
+    assert c.limbs_to_ints(ctx.test_op(28, xl, yl)) == flat([mul2(a, b) for a, b in zip(x2, y2)])
+    # Fq::mul_wide over its whole input range: a < 2^255 (Karatsuba passes a0 + a1 < 2q), b any 256-bit value
+    m = 0xffffffff
+    wa = [0, 1, q - 1, q, 2 * q - 2, 2 * q - 1, (1 << 255) - 1, 1 << 254, (1 << 255) - (1 << 224), (m >> 1) << 224]
+    wb = [(1 << 256) - 1, 0, 1, (1 << 256) - 1, (1 << 256) - 1, q - 1, (1 << 256) - 1, (1 << 256) - 1, m, 1 << 255]
+    while len(wa) < 3000:
+        wa.append(sum(rng.choice([0, 1, m, m - 1, 0x80000000, 0x7fffffff, rng.getrandbits(32)]) << (32 * i) for i in range(8)) % (1 << 255)
+                  if rng.random() < 0.5 else rng.randrange(1 << 255))
+        wb.append(sum(rng.choice([0, 1, m, m - 1, 0x80000000, rng.getrandbits(32)]) << (32 * i) for i in range(8))
+                  if rng.random() < 0.5 else rng.getrandbits(256))
+    got = c.limbs_to_ints(ctx.test_op(29, c.ints_to_limbs(wa), c.ints_to_limbs(wb)))
+    assert [lo | (hi << 256) for lo, hi in zip(got[0::2], got[1::2])] == [a * b for a, b in zip(wa, wb)]
 
 
 def test_group_ops(ctx):
@@ -100,6 +115,23 @@ def test_group_ops(ctx):
     assert np.array_equal(ctx.test_op(9, qa, qb), exp2)
     assert np.array_equal(ctx.test_op(13, qa, qb), exp2)
     assert np.array_equal(ctx.test_op(11, qa), np.stack([c.add_g2(x, x) for x in qa]))
+    # Curve::add / madd / dbl on raw XYZZ records (ops 20-25): projective operands on every exceptional branch, the result
+    # checked as a record (ZZ^3 = ZZZ^2, X = x ZZ, Y = y ZZZ), not through an affine conversion
+    for g2, rows in ((False, pa[5:12]), (True, qa[5:12])):
+        pts = [X.aff(r, g2) for r in rows]
+        curve = o.G2 if g2 else o.G1
+        cases = X.addition_cases(rng, g2, pts)
+        zs = X.z_values(rng, g2)
+        acc = np.stack([X.record(P, z, g2) for _, P, z, _ in cases])
+        q_rec = np.stack([X.record(Q, zs[(i + 3) % len(zs)], g2) for i, (_, _, _, Q) in enumerate(cases)])   # projective q too
+        q_aff = np.stack([X.aff_row(Q, g2) for _, _, _, Q in cases])
+        base = 23 if g2 else 20
+        for op, b, exp in ((base, q_rec, [curve.add(P, Q) for _, P, _, Q in cases]),
+                           (base + 1, q_aff, [curve.add(P, Q) for _, P, _, Q in cases]),
+                           (base + 2, None, [curve.add(P, P) for _, P, _, _ in cases])):
+            out = ctx.test_op(op, acc, b)
+            bad = [(i, cases[i][0], err) for i in range(len(cases)) if (err := X.check_record(out[i], exp[i], g2))]
+            assert not bad, (op, len(bad), bad[:6])
 
 
 def test_fixed_base(ctx):
@@ -205,7 +237,7 @@ def test_msm_g1(ctx, n, dist):
     assert np.array_equal(ctx.msm_g1(bases, c.fr_to_mont(scl), scalars_mont=True), exp)
 
 
-@pytest.mark.parametrize('n,dist', [(1, 'uniform'), (3, 'ones'), (300, 'circomlike'), (5000, 'uniform'), (40000, 'circomlike')])
+@pytest.mark.parametrize('n,dist', [(1, 'uniform'), (3, 'ones'), (300, 'circomlike'), (5000, 'uniform'), (5000, 'same'), (40000, 'circomlike')])
 def test_msm_g2(ctx, n, dist):
     rng = random.Random(n * 13 + len(dist))
     ks, sc = _msm_case(rng, n, dist)
@@ -226,6 +258,37 @@ def test_msm_small_chunks_exercise_fragments(ctx, monkeypatch):
     for chunk in ('1', '2', '3', '7'):
         monkeypatch.setenv('B2G_MSM_CHUNK', chunk)
         assert np.array_equal(ctx.msm_g1(bases, scl), exp), chunk
+    # the bulk-copied entry slab (B2G_ACC_BULK) on and off around its size limit (128 runs x 96 entries = 48 KB per CTA); the
+    # entry count is not a multiple of 4, so the last CTA's slab is partial and its copy is rounded up
+    monkeypatch.setenv('B2G_MSM_C', '11')
+    m = md.partial_slab_prefix(sc, 11)
+    exp_m = c.msm_g1(bases[:m], scl[:m])
+    for chunk in ('1', '64', '96', '97'):
+        monkeypatch.setenv('B2G_MSM_CHUNK', chunk)
+        for bulk in ('0', '1'):
+            monkeypatch.setenv('B2G_ACC_BULK', bulk)
+            assert np.array_equal(ctx.msm_g1(bases[:m], scl[:m]), exp_m), (chunk, bulk)
+    monkeypatch.delenv('B2G_ACC_BULK')
+    # the weighted bucket sum with every per-thread bucket count, at two window sizes
+    monkeypatch.delenv('B2G_MSM_CHUNK')
+    for cw in ('8', '13'):
+        monkeypatch.setenv('B2G_MSM_C', cw)
+        for rchunk in ('1', '3', '7', '1000'):
+            monkeypatch.setenv('B2G_MSM_REDUCE_CHUNK', rchunk)
+            assert np.array_equal(ctx.msm_g1(bases, scl), exp), (cw, rchunk)
+    monkeypatch.delenv('B2G_MSM_REDUCE_CHUNK')
+    # buckets spanning exactly MSM_BIG_FRAGS runs (msm_fold_kernel) and one more (msm_fold_big_kernel), starting on and off
+    # a run boundary; then four equal points in runs of two: each fragment is 2P in projective form, the fold doubles it
+    monkeypatch.setenv('B2G_MSM_C', '8')
+    sc2, ch = md.fold_boundary_scalars(rng)
+    monkeypatch.setenv('B2G_MSM_CHUNK', str(ch))
+    bases2 = c.fixed_base_g1(c.ints_to_limbs([rng.randrange(1, o.R_MOD) for _ in range(len(sc2))]))
+    scl2 = c.ints_to_limbs(sc2)
+    assert np.array_equal(ctx.msm_g1(bases2, scl2), c.msm_g1(bases2, scl2))
+    monkeypatch.setenv('B2G_MSM_CHUNK', '2')
+    for v in (3, rng.randrange(o.R_MOD)):
+        b4, s4 = np.stack([bases2[0]] * 4), c.ints_to_limbs([v] * 4)
+        assert np.array_equal(ctx.msm_g1(b4, s4), c.msm_g1(b4, s4)), v
 
 
 @pytest.mark.parametrize('rounds', ['1', '2', '3', '6'])
