@@ -53,10 +53,13 @@ __global__ void __launch_bounds__(256) msm_validate_kernel(const void* __restric
 }
 
 // ------------------------------------------------------------------------------------------------ (1) digits + histogram
-// (1a) scalars -> canonical integers (one Montgomery reduction each)
-__global__ void __launch_bounds__(256) msm_canon_kernel(const fe* __restrict__ scalars, uint32_t n, int scalars_mont, fe* __restrict__ canon_out) {
+// (1a) scalars -> canonical integers (one Montgomery reduction each).  (1a)-(1c) take proof j = blockIdx.y of a batch: its
+// scalars start at j * scalar_stride, its canonical copy at j * n and its counters at j * nb.
+__global__ void __launch_bounds__(256) msm_canon_kernel(const fe* __restrict__ scalars, uint32_t n, uint32_t scalar_stride, int scalars_mont, fe* __restrict__ canon_out) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    scalars += (size_t)blockIdx.y * scalar_stride;
+    canon_out += (size_t)blockIdx.y * n;
     fe k = fe_load_nc(&scalars[i]);
     if (scalars_mont) k = Fr::to_canonical(k);
     fe_store(&canon_out[i], k);
@@ -94,7 +97,9 @@ __device__ __forceinline__ int32_t msm_digit_at(const uint32_t* __restrict__ k, 
 // leader's with high probability, and on uniform data the rounds cost four ballots.  Lanes still pending add individually.
 constexpr int MSM_LEADER_ROUNDS = 2;
 
-__global__ void __launch_bounds__(256) msm_count_kernel(const fe* __restrict__ canon, uint32_t n, int c, int nwin, uint32_t* __restrict__ counts) {
+__global__ void __launch_bounds__(256) msm_count_kernel(const fe* __restrict__ canon, uint32_t n, int c, int nwin, uint32_t nb, uint32_t* __restrict__ counts) {
+    canon += (size_t)blockIdx.y * n;
+    counts += (size_t)blockIdx.y * nb;
     const uint64_t tid = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const uint32_t w = (uint32_t)(tid / n), i = (uint32_t)(tid % n);
     int32_t d = 0;
@@ -158,8 +163,11 @@ __global__ void __launch_bounds__(1024) msm_scan_kernel(const uint32_t* __restri
 }
 
 // ------------------------------------------------------------------------------------------------ (3) scatter
-__global__ void __launch_bounds__(256) msm_scatter_kernel(const fe* __restrict__ canon, uint32_t n, uint32_t row_stride, int c, int nwin,
+__global__ void __launch_bounds__(256) msm_scatter_kernel(const fe* __restrict__ canon, uint32_t n, uint32_t row_stride, int c, int nwin, uint32_t nb,
                                    const uint32_t* __restrict__ offsets, uint32_t* __restrict__ cursor, uint32_t* __restrict__ entries) {
+    canon += (size_t)blockIdx.y * n;
+    offsets += (size_t)blockIdx.y * nb;                    // global positions in the batch's one sorted list
+    cursor += (size_t)blockIdx.y * nb;
     const uint64_t tid = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const uint32_t w = (uint32_t)(tid / n), i = (uint32_t)(tid % n);
     int32_t d = 0;
@@ -596,11 +604,14 @@ __global__ void __launch_bounds__(TailThreads<F>::N) msm_fold_big_kernel(const u
 // ------------------------------------------------------------------------------------------------ (6) weighted bucket sum
 // sum_b (b+1) * B_b.  Thread t takes buckets [t*S, (t+1)*S): running sums give A_t = sum_j (j+1) B_{tS+j} and
 // S_t = sum_j B_{tS+j}; its contribution is A_t + (t*S) * S_t (small double-and-add); a CTA tree adds them up.
+// blockIdx.y = proof of a batch: its nb buckets start at y * nb and its partials at y * gridDim.x, so the weights restart at 1.
 template <class C, class F>
 __global__ void __launch_bounds__(TailThreads<F>::N) msm_reduce_kernel(const void* __restrict__ buckets, uint32_t nb, uint32_t rchunk, void* __restrict__ partials) {
     using Pt = typename C::Pt;
     extern __shared__ __align__(32) unsigned char smem_raw[];
     Pt* sh = reinterpret_cast<Pt*>(smem_raw);
+    buckets = (const char*)buckets + (size_t)blockIdx.y * nb * sizeof(Pt);
+    partials = (char*)partials + (size_t)blockIdx.y * gridDim.x * sizeof(Pt);
     const uint32_t t = blockIdx.x * TailThreads<F>::N + threadIdx.x;
     const uint32_t base = t * rchunk;
     Pt run = C::infinity(), acc = C::infinity();
@@ -623,12 +634,14 @@ __global__ void __launch_bounds__(TailThreads<F>::N) msm_reduce_kernel(const voi
     if (threadIdx.x == 0) pt_store<F>(partials, blockIdx.x, r);
 }
 
-// sum of `count` points (count <= a few hundred) by one CTA
+// sum of `count` points (count <= a few hundred) by one CTA; CTA j sums points [j * count, (j + 1) * count) into out + j * out_stride
 template <class C, class F>
-__global__ void __launch_bounds__(TailThreads<F>::N) msm_sum_kernel(const void* __restrict__ pts, uint32_t count, void* __restrict__ out) {
+__global__ void __launch_bounds__(TailThreads<F>::N) msm_sum_kernel(const void* __restrict__ pts, uint32_t count, void* __restrict__ out, size_t out_stride) {
     using Pt = typename C::Pt;
     extern __shared__ __align__(32) unsigned char smem_raw[];
     Pt* sh = reinterpret_cast<Pt*>(smem_raw);
+    pts = (const char*)pts + (size_t)blockIdx.x * count * sizeof(Pt);
+    out = (char*)out + (size_t)blockIdx.x * out_stride;
     Pt acc = C::infinity();
     for (uint32_t i = threadIdx.x; i < count; i += TailThreads<F>::N) { Pt q = pt_load<F>(pts, i); C::add(acc, q); }
     Pt r = block_sum_points<C, F, TailThreads<F>::N>(acc, sh);
@@ -683,11 +696,13 @@ void msm_build_table(MsmPlan& plan, const void* bases_dev, uint32_t n, bool g2, 
 
 void msm_free_table(MsmPlan& plan) { if (plan.table) cudaFree(plan.table); plan.table = nullptr; }
 
-void msm_scratch_alloc(MsmScratch& s, uint32_t n, int nwin, uint32_t nbuckets, bool g2, bool with_sort) {
-    s.g2 = g2; s.cap_n = n; s.cap_nwin = nwin; s.cap_buckets = nbuckets;
+// count: proofs of a batch the buffers hold (sorted entries, buckets, fragments and partials scale with it)
+void msm_scratch_alloc(MsmScratch& s, uint32_t n, int nwin, uint32_t nbuckets_one, bool g2, bool with_sort, uint32_t count) {
+    s.g2 = g2; s.cap_n = n; s.cap_nwin = nwin; s.cap_buckets = nbuckets_one; s.cap_count = count;
     s.chunk = env_u32(g2 ? "B2G_MSM_CHUNK_G2" : "B2G_MSM_CHUNK", env_u32("B2G_MSM_CHUNK", 64));
     const size_t pt = (g2 ? 4 * 64 : 4 * 32);
-    const size_t nent = (size_t)n * nwin;
+    const size_t nent = (size_t)n * nwin * count;
+    const size_t nbuckets = (size_t)nbuckets_one * count;
     const size_t nchunks = (nent + s.chunk - 1) / s.chunk + 1;
     s.reduce_chunk = env_u32("B2G_MSM_REDUCE_CHUNK", MSM_REDUCE_CHUNK_DEFAULT);
     // the bulk-staged slab of the accumulation is on for G1, off for G2.  On an H100 (2^20 chain) neither switch is
@@ -697,13 +712,13 @@ void msm_scratch_alloc(MsmScratch& s, uint32_t n, int nwin, uint32_t nbuckets, b
         const char* bulk_env = getenv("B2G_ACC_BULK");
         s.bulk = bulk_env && *bulk_env ? *bulk_env == '1' : !g2;
     }
-    const size_t npart = (size_t)nbuckets / (s.reduce_chunk * 32) + 64;
+    const size_t npart = ((size_t)nbuckets_one / (s.reduce_chunk * 32) + 64) * count;
     if (with_sort) {
         CUDA_CHECK(cudaMalloc(&s.counts, (size_t)nbuckets * 4));
         CUDA_CHECK(cudaMalloc(&s.offsets, ((size_t)nbuckets + 1) * 4));
         CUDA_CHECK(cudaMalloc(&s.cursor, (size_t)nbuckets * 4));
         CUDA_CHECK(cudaMalloc(&s.entries, (nent + 8) * 4));          // + 16 B: the bulk copy of the last slab is rounded up
-        CUDA_CHECK(cudaMalloc(&s.scalars_canon, ((size_t)n + 1) * sizeof(fe)));
+        CUDA_CHECK(cudaMalloc(&s.scalars_canon, ((size_t)n * count + 1) * sizeof(fe)));
     }
     CUDA_CHECK(cudaMalloc(&s.big_list, (size_t)nbuckets * 4));
     CUDA_CHECK(cudaMalloc(&s.big_count, 4));
@@ -721,7 +736,7 @@ void msm_scratch_alloc(MsmScratch& s, uint32_t n, int nwin, uint32_t nbuckets, b
         if (ov && *ov) { long x = strtol(ov, nullptr, 10); rounds = x < 0 ? 0 : (x > MSM_AFF_MAX_ROUNDS ? MSM_AFF_MAX_ROUNDS : (int)x); }
         s.aff_cap_rounds = rounds;
         s.aff_nmax[0] = (uint32_t)nent;
-        for (int k = 1; k <= rounds; k++) s.aff_nmax[k] = s.aff_nmax[k - 1] / 2 + nbuckets / 2 + 1;
+        for (int k = 1; k <= rounds; k++) s.aff_nmax[k] = s.aff_nmax[k - 1] / 2 + (uint32_t)(nbuckets / 2) + 1;
         if (rounds) {
             const size_t elem = g2 ? 64 : 32, aff = 2 * elem;
             if (with_sort) {
@@ -765,20 +780,22 @@ void msm_scratch_free(MsmScratch& s) {
     s = MsmScratch();
 }
 
-void msm_sort(const MsmPlan& plan, MsmScratch& s, const fe* scalars_dev, uint32_t n, bool scalars_mont, cudaStream_t st) {
+// count scalar vectors of n, the j-th at scalars_dev + j * scalar_stride, into one list of count * nbuckets buckets
+void msm_sort(const MsmPlan& plan, MsmScratch& s, const fe* scalars_dev, uint32_t n, bool scalars_mont, cudaStream_t st, uint32_t count,
+              uint32_t scalar_stride) {
     if (n > plan.n) n = plan.n;                                  // msm_bigint truncates to the shorter side
-    s.sorted_n = n;
+    s.sorted_n = n; s.sorted_count = count;
     if (n == 0 || plan.table == nullptr) return;
-    if (n > s.cap_n || plan.nwin > s.cap_nwin || plan.nbuckets > s.cap_buckets || !s.entries) throw_error(B2G_E_SHAPE, "msm: sort scratch too small");
-    const uint32_t nb = plan.nbuckets;
+    if (n > s.cap_n || plan.nwin > s.cap_nwin || plan.nbuckets > s.cap_buckets || count > s.cap_count || !s.entries) throw_error(B2G_E_SHAPE, "msm: sort scratch too small");
+    const uint32_t nb = plan.nbuckets * count;
     constexpr unsigned SORT_CTA = 256;
     CUDA_CHECK(cudaMemsetAsync(s.counts, 0, (size_t)nb * 4, st));
-    const unsigned pair_blocks = (unsigned)(((uint64_t)n * plan.nwin + SORT_CTA - 1) / SORT_CTA);
-    msm_canon_kernel<<<(n + SORT_CTA - 1) / SORT_CTA, SORT_CTA, 0, st>>>(scalars_dev, n, scalars_mont ? 1 : 0, s.scalars_canon);
-    msm_count_kernel<<<pair_blocks, SORT_CTA, 0, st>>>(s.scalars_canon, n, plan.c, plan.nwin, s.counts);
+    const dim3 pair_grid((unsigned)(((uint64_t)n * plan.nwin + SORT_CTA - 1) / SORT_CTA), count);
+    msm_canon_kernel<<<dim3((n + SORT_CTA - 1) / SORT_CTA, count), SORT_CTA, 0, st>>>(scalars_dev, n, scalar_stride ? scalar_stride : n, scalars_mont ? 1 : 0, s.scalars_canon);
+    msm_count_kernel<<<pair_grid, SORT_CTA, 0, st>>>(s.scalars_canon, n, plan.c, plan.nwin, plan.nbuckets, s.counts);
     msm_scan_kernel<<<1, 1024, 0, st>>>(s.counts, nb, s.offsets, s.cursor);
     // table rows are indexed w * plan.n + i (the table was built over plan.n bases, n may be shorter)
-    msm_scatter_kernel<<<pair_blocks, SORT_CTA, 0, st>>>(s.scalars_canon, n, plan.n, plan.c, plan.nwin, s.offsets, s.cursor, s.entries);
+    msm_scatter_kernel<<<pair_grid, SORT_CTA, 0, st>>>(s.scalars_canon, n, plan.n, plan.c, plan.nwin, plan.nbuckets, s.offsets, s.cursor, s.entries);
     g_launch_count += 4;
     // level structure of the batched-affine pre-reduction (shared by every query accumulated against this sort)
     s.aff_rounds = s.aff_off_dev ? s.aff_cap_rounds : 0;
@@ -811,12 +828,13 @@ template <class C, class F>
 static void msm_accumulate_t(const MsmPlan& plan, const MsmScratch& sorted, MsmScratch& s, cudaStream_t st) {
     using Pt = typename C::Pt;
     const size_t ptb = sizeof(Pt);
-    const uint32_t n = sorted.sorted_n;
-    if (n == 0 || plan.table == nullptr) { CUDA_CHECK(cudaMemsetAsync(s.result, 0, ptb, st)); return; }
-    if (plan.nbuckets > s.cap_buckets || n > s.cap_n || plan.nwin > s.cap_nwin) throw_error(B2G_E_SHAPE, "msm: accumulate scratch too small");
-    const uint32_t nb = plan.nbuckets, chunk = s.chunk;
+    const uint32_t n = sorted.sorted_n, count = sorted.sorted_count;
+    const size_t rstride = s.result_stride ? s.result_stride : ptb;
+    if (n == 0 || plan.table == nullptr) { CUDA_CHECK(cudaMemset2DAsync(s.result, rstride, 0, ptb, count, st)); return; }
+    if (plan.nbuckets > s.cap_buckets || n > s.cap_n || plan.nwin > s.cap_nwin || count > s.cap_count) throw_error(B2G_E_SHAPE, "msm: accumulate scratch too small");
+    const uint32_t nb = plan.nbuckets * count, chunk = s.chunk;   // every proof's buckets in one range: runs cross proofs freely
     CUDA_CHECK(cudaMemsetAsync(s.big_count, 0, 4, st));
-    const uint64_t nent = (uint64_t)n * plan.nwin;
+    const uint64_t nent = (uint64_t)n * plan.nwin * count;
     const uint32_t nthreads = (uint32_t)((nent + chunk - 1) / chunk);
     if (s.prof0) CUDA_CHECK(cudaEventRecord(s.prof0, st));
     int rounds = sorted.aff_rounds < s.aff_cap_rounds ? sorted.aff_rounds : s.aff_cap_rounds;
@@ -855,11 +873,11 @@ static void msm_accumulate_t(const MsmPlan& plan, const MsmScratch& sorted, MsmS
     constexpr int NT = TailThreads<F>::N;
     const size_t sh = (size_t)NT * ptb;
     msm_fold_big_kernel<C, F><<<128, NT, sh, st>>>(offsets, chunk, s.buckets, s.frag_first, s.frag_last, s.big_list, s.big_count);
-    const uint32_t rchunk = s.reduce_chunk;
-    const uint32_t nred = (nb + rchunk - 1) / rchunk;
-    const uint32_t npart = (nred + NT - 1) / NT;
-    msm_reduce_kernel<C, F><<<npart, NT, sh, st>>>(s.buckets, nb, rchunk, s.partials);
-    msm_sum_kernel<C, F><<<1, NT, sh, st>>>(s.partials, npart, s.result);
+    const uint32_t rchunk = s.reduce_chunk, nb1 = plan.nbuckets;
+    const uint32_t nred = (nb1 + rchunk - 1) / rchunk;
+    const uint32_t npart = (nred + NT - 1) / NT;                 // per proof
+    msm_reduce_kernel<C, F><<<dim3(npart, count), NT, sh, st>>>(s.buckets, nb1, rchunk, s.partials);
+    msm_sum_kernel<C, F><<<count, NT, sh, st>>>(s.partials, npart, s.result, rstride);
     if (s.tail) { CUDA_CHECK(cudaEventRecord(s.ev_tail, s.tail)); CUDA_CHECK(cudaStreamWaitEvent(main_st, s.ev_tail, 0)); }
     g_launch_count += 5;
     CUDA_CHECK(cudaGetLastError());
@@ -872,8 +890,9 @@ void msm_accumulate(const MsmPlan& plan, const MsmScratch& sorted, MsmScratch& a
     else msm_accumulate_t<G1, Fq>(plan, sorted, acc, st);
 }
 
-void msm_run(const MsmPlan& plan, MsmScratch& s, const fe* scalars_dev, uint32_t n, bool scalars_mont, cudaStream_t st) {
-    msm_sort(plan, s, scalars_dev, n, scalars_mont, st);
+void msm_run(const MsmPlan& plan, MsmScratch& s, const fe* scalars_dev, uint32_t n, bool scalars_mont, cudaStream_t st, uint32_t count,
+             uint32_t scalar_stride) {
+    msm_sort(plan, s, scalars_dev, n, scalars_mont, st, count, scalar_stride);
     msm_accumulate(plan, s, s, st);
 }
 

@@ -42,8 +42,14 @@ constexpr int MSM_AFF_MAX_ROUNDS = 6;
 constexpr int MSM_AFF_M = 16;            // additions per thread and level (interleaved: thread t owns slots t + i * stride)
 constexpr int MSM_AFF_S = 64;            // thread totals per inversion thread
 
+// Batched MSMs (b2g_prove_many): `count` scalar vectors against the same table are sorted into ONE list whose bucket key is
+// j * nbuckets + b for proof j, so accumulation and fold run unchanged over count * nbuckets buckets.  Table rows, and so the
+// entry word, do not depend on j.  The weighted reduction restarts its bucket weights per proof (grid.y = proof) and proof
+// j's result is written at result + j * result_stride.
 struct MsmScratch {                      // one per in-flight MSM
     uint32_t cap_n = 0; int cap_nwin = 0; uint32_t cap_buckets = 0; uint32_t chunk = 64; uint32_t sorted_n = 0; uint32_t reduce_chunk = 8;
+    uint32_t cap_count = 1, sorted_count = 1;   // proofs the buffers hold / proofs in the last sort
+    size_t result_stride = 0;                   // bytes between the results of consecutive proofs (0: one point)
     uint32_t *counts = nullptr, *offsets = nullptr, *cursor = nullptr, *entries = nullptr;
     uint32_t *big_list = nullptr, *big_count = nullptr;
     void *frag_first = nullptr, *frag_last = nullptr, *buckets = nullptr, *partials = nullptr, *result = nullptr;

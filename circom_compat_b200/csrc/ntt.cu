@@ -67,14 +67,17 @@ __global__ void __launch_bounds__(256) ntt_tables_kernel(int logn, const fe* __r
 
 // ------------------------------------------------------------------------------------------------ sparse mat-vec
 // a_i = <A_i, w>, b_i = <B_i, w> (evaluate_constraint, ark-groth16 0.5.0, called at qap.rs:42-43), c_i = a_i*b_i,
-// a[m + j] = w[j] for j < num_inputs (qap.rs:46-50), everything else zero.
-__global__ void __launch_bounds__(256) spmv_kernel(uint32_t n, uint32_t m, uint32_t num_inputs,
+// a[m + j] = w[j] for j < num_inputs (qap.rs:46-50), everything else zero.  blockIdx.y = proof of a batch: its assignment
+// starts at w + y * w_stride, its a, b, c at y * n.
+__global__ void __launch_bounds__(256) spmv_kernel(uint32_t n, uint32_t m, uint32_t num_inputs, uint32_t w_stride,
                             const uint32_t* __restrict__ a_rowptr, const uint32_t* __restrict__ a_col, const fe* __restrict__ a_val,
                             const uint32_t* __restrict__ b_rowptr, const uint32_t* __restrict__ b_col, const fe* __restrict__ b_val,
                             const fe* __restrict__ w, fe* __restrict__ a, fe* __restrict__ b, fe* __restrict__ c,
                             const uint32_t* __restrict__ c_rowptr, const uint32_t* __restrict__ c_col, const fe* __restrict__ c_val) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    w += (size_t)blockIdx.y * w_stride;
+    a += (size_t)blockIdx.y * n; b += (size_t)blockIdx.y * n; c += (size_t)blockIdx.y * n;
     fe ra = fe_zero(), rb = fe_zero(), rc = fe_zero();
     if (i < m) {
         const fe one = Fr::one();
@@ -110,6 +113,7 @@ struct NttPassArgs {
     int logn, tl;         // tl = log2(tile)
     int sb, k;            // transform bits [sb, sb + k) of the element index
     int do_dif, do_scale, do_dit, pointwise;
+    size_t bstride;       // elements between the vectors of consecutive proofs of a batch (blockIdx.z = proof)
 };
 
 __device__ __forceinline__ uint32_t tile_global_index(uint32_t loc, uint32_t tile_id, int cols_log, int sb, int k) {
@@ -141,8 +145,10 @@ __global__ void __launch_bounds__(512, 2) ntt_pass_kernel(NttPassArgs A) {
     const uint32_t g1 = tile_global_index(tid + half, blockIdx.x, cols_log, A.sb, A.k);
     const int nv = POINTWISE ? 3 : 1;
     fe acc0 = fe_zero(), acc1 = fe_zero();
+    const size_t zoff = (size_t)blockIdx.z * A.bstride;
+    fe* const out = POINTWISE ? A.out + zoff : nullptr;
     for (int vi = 0; vi < nv; vi++) {
-        fe* vec = POINTWISE ? A.vec[vi] : A.vec[blockIdx.y];
+        fe* vec = (POINTWISE ? A.vec[vi] : A.vec[blockIdx.y]) + zoff;
         if (tid < half || half == 0) {
             sm_put(sm, tile, tid, fe_load(&vec[g0]));
             if (half) sm_put(sm, tile, tid + half, fe_load(&vec[g1]));
@@ -204,8 +210,8 @@ __global__ void __launch_bounds__(512, 2) ntt_pass_kernel(NttPassArgs A) {
             else {
                 fe r0 = Fr::sub(acc0, x0), r1 = Fr::sub(acc1, x1);        // h = a*b - c   (qap.rs:75-85)
                 if (A.pw_scale) { const fe z = *A.pw_scale; r0 = Fr::mul(r0, z); r1 = Fr::mul(r1, z); }
-                fe_store(&A.out[g0], r0);
-                if (half) fe_store(&A.out[g1], r1);
+                fe_store(&out[g0], r0);
+                if (half) fe_store(&out[g1], r1);
             }
         }
         __syncthreads();
@@ -260,8 +266,10 @@ __global__ void __launch_bounds__(256, 2) ntt_pass8_kernel(NttPassArgs A) {
     const int cols_log = A.tl - A.k, ftop = A.tl - 3;
     const uint32_t n = 1u << A.logn;
     const int nv = POINTWISE ? 3 : 1;
+    const size_t zoff = (size_t)blockIdx.z * A.bstride;
+    fe* const out = POINTWISE ? A.out + zoff : nullptr;
     for (int vi = 0; vi < nv; vi++) {
-        fe* vec = POINTWISE ? A.vec[vi] : A.vec[blockIdx.y];
+        fe* vec = (POINTWISE ? A.vec[vi] : A.vec[blockIdx.y]) + zoff;
         fe x[8];
         int f = A.do_dif ? ftop : (cols_log < ftop ? cols_log : ftop), k = 0;
         #pragma unroll
@@ -334,12 +342,12 @@ __global__ void __launch_bounds__(256, 2) ntt_pass8_kernel(NttPassArgs A) {
             for (int p = 0; p < 4; p++) {
                 const uint32_t g = tile_global_index(ntt8_loc(tid, p + 4 * h, f), blockIdx.x, cols_log, A.sb, A.k);
                 if (!POINTWISE) fe_store(&vec[g], x[p]);
-                else if (vi == 0) fe_store(&A.out[g], x[p]);
-                else if (vi == 1) fe_store(&A.out[g], Fr::mul(fe_load(&A.out[g]), x[p]));
+                else if (vi == 0) fe_store(&out[g], x[p]);
+                else if (vi == 1) fe_store(&out[g], Fr::mul(fe_load(&out[g]), x[p]));
                 else {
-                    fe r = Fr::sub(fe_load(&A.out[g]), x[p]);
+                    fe r = Fr::sub(fe_load(&out[g]), x[p]);
                     if (A.pw_scale) r = Fr::mul(r, *A.pw_scale);
-                    fe_store(&A.out[g], r);
+                    fe_store(&out[g], r);
                 }
             }
             #pragma unroll
@@ -348,11 +356,12 @@ __global__ void __launch_bounds__(256, 2) ntt_pass8_kernel(NttPassArgs A) {
     }
 }
 
-// out[bitrev(i)] = in[i] * (scale ? *scale : 1)
+// out[bitrev(i)] = in[i] * (scale ? *scale : 1); blockIdx.y = proof of a batch (vectors 2^logn apart)
 __global__ void __launch_bounds__(256) bitrev_copy_kernel(const fe* __restrict__ in, fe* __restrict__ out, int logn, const fe* __restrict__ scale,
                                                           const fe* __restrict__ table) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (1u << logn)) return;
+    in += (size_t)blockIdx.y << logn; out += (size_t)blockIdx.y << logn;
     uint32_t j = logn ? (__brev(i) >> (32 - logn)) : 0u;
     fe v = fe_load(&in[i]);
     if (scale) v = Fr::mul(v, *scale);
@@ -426,14 +435,14 @@ void ntt_domain_destroy(NttDomain& d) {
 }
 
 static void launch_pass(const NttDomain& d, fe* v0, fe* v1, fe* v2, int nvec, fe* out, int pass, int dif, int scale, int dit, int pointwise,
-                        cudaStream_t st, const fe* coset_table = nullptr, const fe* pw_scale = nullptr) {
+                        cudaStream_t st, const fe* coset_table = nullptr, const fe* pw_scale = nullptr, uint32_t count = 1) {
     NttPassArgs A;
     A.vec[0] = v0; A.vec[1] = v1; A.vec[2] = v2; A.out = out; A.tw = d.tw; A.ct = coset_table ? coset_table : d.ct; A.pw_scale = pw_scale;
     A.logn = d.logn; A.tl = d.pass_tl[pass]; A.sb = d.pass_sb[pass]; A.k = d.pass_k[pass];
-    A.do_dif = dif; A.do_scale = scale; A.do_dit = dit; A.pointwise = pointwise;
+    A.do_dif = dif; A.do_scale = scale; A.do_dit = dit; A.pointwise = pointwise; A.bstride = (size_t)1 << d.logn;
     const uint32_t tile = 1u << A.tl;
     const uint32_t ntiles = (uint32_t)(((size_t)1 << d.logn) >> A.tl);
-    dim3 grid(ntiles, pointwise ? 1 : nvec);
+    dim3 grid(ntiles, pointwise ? 1 : nvec, count);
     if (d.radix8) {
         if (pointwise) ntt_pass8_kernel<true><<<grid, tile / 8, tile * 32, st>>>(A);
         else ntt_pass8_kernel<false><<<grid, tile / 8, tile * 32, st>>>(A);
@@ -445,12 +454,12 @@ static void launch_pass(const NttDomain& d, fe* v0, fe* v1, fe* v2, int nvec, fe
     g_launch_count += 1;
 }
 
-// the three vectors a, b, c (natural order, in place) -> h (natural order) in `out`
-void ntt_witness_transform(const NttDomain& d, fe* a, fe* b, fe* c, fe* out, cudaStream_t st) {
-    for (int p = d.npass - 1; p >= 1; p--) launch_pass(d, a, b, c, 3, nullptr, p, 1, 0, 0, 0, st);
+// the three vectors a, b, c (natural order, in place) -> h (natural order) in `out`; `count` proofs whose vectors are n apart
+void ntt_witness_transform(const NttDomain& d, fe* a, fe* b, fe* c, fe* out, cudaStream_t st, uint32_t count) {
+    for (int p = d.npass - 1; p >= 1; p--) launch_pass(d, a, b, c, 3, nullptr, p, 1, 0, 0, 0, st, nullptr, nullptr, count);
     const bool single = d.npass == 1;
-    launch_pass(d, a, b, c, 3, out, 0, 1, 1, 1, single ? 1 : 0, st);
-    for (int p = 1; p < d.npass; p++) launch_pass(d, a, b, c, 3, out, p, 0, 0, 1, p == d.npass - 1 ? 1 : 0, st);
+    launch_pass(d, a, b, c, 3, out, 0, 1, 1, 1, single ? 1 : 0, st, nullptr, nullptr, count);
+    for (int p = 1; p < d.npass; p++) launch_pass(d, a, b, c, 3, out, p, 0, 0, 1, p == d.npass - 1 ? 1 : 0, st, nullptr, nullptr, count);
     CUDA_CHECK(cudaGetLastError());
 }
 
@@ -469,15 +478,15 @@ void ntt_transform_single(const NttDomain& d, fe* v, cudaStream_t st) {
 // g*H (g = 5) -> (a*b - c) / Z(g) -> coset iFFT -> the n coefficients of h, natural order, in `out`.
 // Same kernels as the Circom map; the coset tables are cg / cginv, and the last inverse transform is a DIF pass set
 // followed by one bit-reversing copy that applies n^-1 g^-i.
-void ntt_witness_transform_libsnark(const NttDomain& d, fe* a, fe* b, fe* c, fe* scratch, fe* out, cudaStream_t st) {
+void ntt_witness_transform_libsnark(const NttDomain& d, fe* a, fe* b, fe* c, fe* scratch, fe* out, cudaStream_t st, uint32_t count) {
     if (!d.cg) throw_error(B2G_E_SHAPE, "matrices were not loaded for LibsnarkReduction");
-    for (int p = d.npass - 1; p >= 1; p--) launch_pass(d, a, b, c, 3, nullptr, p, 1, 0, 0, 0, st);
+    for (int p = d.npass - 1; p >= 1; p--) launch_pass(d, a, b, c, 3, nullptr, p, 1, 0, 0, 0, st, nullptr, nullptr, count);
     const bool single = d.npass == 1;
-    launch_pass(d, a, b, c, 3, scratch, 0, 1, 1, 1, single ? 1 : 0, st, d.cg, d.zinv);
-    for (int p = 1; p < d.npass; p++) launch_pass(d, a, b, c, 3, scratch, p, 0, 0, 1, p == d.npass - 1 ? 1 : 0, st, d.cg, d.zinv);
-    for (int p = d.npass - 1; p >= 0; p--) launch_pass(d, scratch, nullptr, nullptr, 1, nullptr, p, 1, 0, 0, 0, st);
+    launch_pass(d, a, b, c, 3, scratch, 0, 1, 1, 1, single ? 1 : 0, st, d.cg, d.zinv, count);
+    for (int p = 1; p < d.npass; p++) launch_pass(d, a, b, c, 3, scratch, p, 0, 0, 1, p == d.npass - 1 ? 1 : 0, st, d.cg, d.zinv, count);
+    for (int p = d.npass - 1; p >= 0; p--) launch_pass(d, scratch, nullptr, nullptr, 1, nullptr, p, 1, 0, 0, 0, st, nullptr, nullptr, count);
     const size_t n = (size_t)1 << d.logn;
-    bitrev_copy_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(scratch, out, d.logn, nullptr, d.cginv);
+    bitrev_copy_kernel<<<dim3((unsigned)((n + 255) / 256), count), 256, 0, st>>>(scratch, out, d.logn, nullptr, d.cginv);
     g_launch_count += 1;
     CUDA_CHECK(cudaGetLastError());
 }
@@ -500,8 +509,8 @@ void ntt_plain(const NttDomain& d, fe* data, fe* tmp, bool inverse, cudaStream_t
 
 void spmv_launch(uint32_t n, uint32_t m, uint32_t num_inputs, const uint32_t* a_rowptr, const uint32_t* a_col, const fe* a_val,
                  const uint32_t* b_rowptr, const uint32_t* b_col, const fe* b_val, const fe* w, fe* a, fe* b, fe* c, cudaStream_t st,
-                 const uint32_t* c_rowptr, const uint32_t* c_col, const fe* c_val) {
-    spmv_kernel<<<(n + 255) / 256, 256, 0, st>>>(n, m, num_inputs, a_rowptr, a_col, a_val, b_rowptr, b_col, b_val, w, a, b, c, c_rowptr, c_col, c_val);
+                 const uint32_t* c_rowptr, const uint32_t* c_col, const fe* c_val, uint32_t count, uint32_t w_stride) {
+    spmv_kernel<<<dim3((n + 255) / 256, count), 256, 0, st>>>(n, m, num_inputs, w_stride, a_rowptr, a_col, a_val, b_rowptr, b_col, b_val, w, a, b, c, c_rowptr, c_col, c_val);
     g_launch_count += 1;
     CUDA_CHECK(cudaGetLastError());
 }

@@ -17,12 +17,14 @@ struct NttDomain {
 
 void ntt_domain_create(NttDomain& d, int logn, cudaStream_t st, bool libsnark = false);
 void ntt_domain_destroy(NttDomain& d);
-void ntt_witness_transform(const NttDomain& d, fe* a, fe* b, fe* c, fe* out, cudaStream_t st);
+// count > 1: a batch of proofs whose vectors lie 2^logn elements apart (b2g_prove_many)
+void ntt_witness_transform(const NttDomain& d, fe* a, fe* b, fe* c, fe* out, cudaStream_t st, uint32_t count = 1);
 void ntt_transform_single(const NttDomain& d, fe* v, cudaStream_t st);
-void ntt_witness_transform_libsnark(const NttDomain& d, fe* a, fe* b, fe* c, fe* scratch, fe* out, cudaStream_t st);
+void ntt_witness_transform_libsnark(const NttDomain& d, fe* a, fe* b, fe* c, fe* scratch, fe* out, cudaStream_t st, uint32_t count = 1);
 void ntt_plain(const NttDomain& d, fe* data, fe* tmp, bool inverse, cudaStream_t st);
 void spmv_launch(uint32_t n, uint32_t m, uint32_t num_inputs, const uint32_t* a_rowptr, const uint32_t* a_col, const fe* a_val,
                  const uint32_t* b_rowptr, const uint32_t* b_col, const fe* b_val, const fe* w, fe* a, fe* b, fe* c, cudaStream_t st,
-                 const uint32_t* c_rowptr = nullptr, const uint32_t* c_col = nullptr, const fe* c_val = nullptr);
+                 const uint32_t* c_rowptr = nullptr, const uint32_t* c_col = nullptr, const fe* c_val = nullptr,
+                 uint32_t count = 1, uint32_t w_stride = 0);       // count assignments w_stride apart -> a, b, c of count x n
 
 }  // namespace b2g

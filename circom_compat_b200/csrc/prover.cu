@@ -20,16 +20,20 @@ namespace b2g {
 // from msm.cu
 void msm_build_table(MsmPlan& plan, const void* bases_dev, uint32_t n, bool g2, cudaStream_t st);
 void msm_free_table(MsmPlan& plan);
-void msm_scratch_alloc(MsmScratch& s, uint32_t n, int nwin, uint32_t nbuckets, bool g2, bool with_sort);
-void msm_sort(const MsmPlan& plan, MsmScratch& s, const fe* scalars_dev, uint32_t n, bool scalars_mont, cudaStream_t st);
+void msm_scratch_alloc(MsmScratch& s, uint32_t n, int nwin, uint32_t nbuckets, bool g2, bool with_sort, uint32_t count = 1);
+void msm_sort(const MsmPlan& plan, MsmScratch& s, const fe* scalars_dev, uint32_t n, bool scalars_mont, cudaStream_t st, uint32_t count = 1,
+              uint32_t scalar_stride = 0);
 void msm_accumulate(const MsmPlan& plan, const MsmScratch& sorted, MsmScratch& acc, cudaStream_t st);
 void msm_scratch_free(MsmScratch& s);
-void msm_run(const MsmPlan& plan, MsmScratch& s, const fe* scalars_dev, uint32_t n, bool scalars_mont, cudaStream_t st);
+void msm_run(const MsmPlan& plan, MsmScratch& s, const fe* scalars_dev, uint32_t n, bool scalars_mont, cudaStream_t st, uint32_t count = 1,
+             uint32_t scalar_stride = 0);
 void msm_init_kernels();
 void msm_validate_points(const void* pts_dev, uint32_t n, bool g2, cudaStream_t st, const char* what);
 
 enum { Q_H = 0, Q_L = 1, Q_A = 2, Q_B1 = 3, Q_B2 = 4, NQ = 5 };
 static const size_t PARTIAL_OFF[NQ] = {0, 128, 256, 384, 512};
+constexpr size_t REC_BYTES = B2G_PARTIAL_BYTES + 256;  // device-side record of one proof (or rank): the public 768-byte partial + [s*A_k, r*B1_k]
+constexpr uint32_t MAX_BATCH = 65535;                 // proofs per b2g_prove_many call: the batch is a grid dimension of the sort kernels
 
 }  // namespace b2g
 
@@ -41,14 +45,16 @@ struct b2g_ctx {
     cudaEvent_t ev_w = nullptr, ev_sort = nullptr, ev_pre = nullptr, ev_fork = nullptr, ev_done[NQ] = {}, ev_t[20] = {};
     MsmScratch scratch[NQ];
     bool scratch_ok = false;
+    // Per-proof buffers hold cap_batch proofs (b2g_prove_many; 1 until a batch needs more), proof j at j x its size
+    uint32_t cap_batch = 1;
     uint8_t* d_partial = nullptr;        // REC_BYTES: the public partial [H, L, A, B1] G1 XYZZ + B2 G2 XYZZ (768 B), then [s*A, r*B1]
     uint8_t* d_partials_all = nullptr;   // up to 64 ranks x REC_BYTES
     uint8_t* d_proof = nullptr;          // 256 B
     uint8_t* d_pre = nullptr;            // glue precomputation: r*d1, s*d1, rs*d1, K_C (G1 XYZZ) + s*d2 (G2 XYZZ)
-    fe *d_w = nullptr, *d_a = nullptr, *d_b = nullptr, *d_c = nullptr, *d_h = nullptr;
-    fe* d_wb = nullptr; size_t cap_wb = 0;     // gathered scalars of a sparse B query (b2g_pk::d_bidx)
+    fe *d_w = nullptr, *d_a = nullptr, *d_b = nullptr, *d_c = nullptr, *d_h = nullptr;   // batch: assignments n_vars apart, vectors n apart
+    fe* d_wb = nullptr; size_t cap_wb = 0;     // gathered scalars of a sparse B query (b2g_pk::d_bidx), b_compact apart
     cudaEvent_t ev_sortb = nullptr; bool scratch_bsort = false;
-    size_t cap_w = 0, cap_n = 0;
+    size_t cap_w = 0, cap_n = 0;               // elements d_w / d_a.. hold
     float last_ms[16] = {};
     bool pre_valid = false; uint32_t pre_r[8] = {}, pre_s[8] = {};   // (r, s) whose glue_pre result sits in d_pre
     uint8_t *d_rs = nullptr, *h_rs = nullptr;  // r | s (canonical, 2 x 32 B): device copy read by the glue kernels, pinned staging
@@ -56,8 +62,8 @@ struct b2g_ctx {
     // One proof's whole device pipeline (all streams, ~100 launches) captured once per (key, matrices) as a CUDA graph and
     // replayed with a single launch: the host cost of a proof drops from ~130 driver calls to a handful (B2G_GRAPH=0 disables)
     bool use_graph = true;
-    cudaGraphExec_t gexec[2] = {nullptr, nullptr};             // [0] whole proof, [1] sharded proof with the peer-memory exchange
-    uint64_t g_key[2][3] = {};                                  // (key uid, matrices uid, buffer generation) each graph was captured for
+    cudaGraphExec_t gexec[2] = {nullptr, nullptr};             // [0] whole proof (or batch), [1] sharded proof with the peer-memory exchange
+    uint64_t g_key[2][4] = {};                                  // (key uid, matrices uid, buffer generation, batch count) each graph was captured for
     uint64_t alloc_gen = 1;                                    // bumped whenever a buffer the graphs point into is (re)allocated
     uint64_t g_launches[2] = {0, 0};
     unsigned long long* d_epoch = nullptr;                     // exchange epoch (device-resident so that it survives graph replay)
@@ -134,12 +140,15 @@ __device__ __forceinline__ typename C::Pt warp_fixed_mul(const void* __restrict_
 // table is built at b2g_pk_load, so each product is 32 table look-ups and a 5-level tree inside one warp instead of a
 // 254-step double-and-add on one thread.  K_C is what is left of C = s*A + r*B1 - rs*delta1 + L + H once the MSM results
 // are taken out:  C = K_C + s*msm_A + r*msm_B1 + msm_L + msm_H  (A = alpha + a0 + msm_A + r*delta1, B1 likewise).
+// One CTA per proof of a batch: CTA j reads (r, s) at rs[2j], rs[2j + 1] and writes pre + j * PRE_BYTES.
 constexpr size_t PRE_BYTES = 4 * 128 + 256;
 __global__ void __launch_bounds__(192) glue_pre_kernel(const void* __restrict__ tab_d1, const void* __restrict__ tab_d2, const void* __restrict__ tab_aa,
                                                        const void* __restrict__ tab_bb, const Scalar256* __restrict__ rs, uint8_t* __restrict__ pre) {
     __shared__ G1::Pt sh1[5][32];
     __shared__ G2::Pt sh2[32];
     __shared__ G1::Pt res[5];
+    rs += 2 * blockIdx.x;
+    pre += (size_t)blockIdx.x * PRE_BYTES;
     const Scalar256 r = rs[0], s = rs[1];
     const int warp = threadIdx.x >> 5;
     const bool lead = (threadIdx.x & 31) == 0;
@@ -172,9 +181,11 @@ __global__ void __launch_bounds__(192) glue_pre_kernel(const void* __restrict__ 
 }
 
 // out = k * p for one XYZZ point (the partial A / B1 MSM result of this rank) - issued on that MSM's own stream as soon as
-// it finishes, so the two variable-base scalar multiplications of the proof overlap the longest MSM instead of following it
+// it finishes, so the two variable-base scalar multiplications of the proof overlap the longest MSM instead of following it.
+// CTA j of a batch: pt and out in record j (REC_BYTES apart), k = the scalar of proof j (r, s pairs: 2 apart).
 __global__ void scale_partial_kernel(const uint8_t* __restrict__ pt, const Scalar256* __restrict__ k, uint8_t* __restrict__ out) {
     if (threadIdx.x != 0) return;
+    pt += blockIdx.x * REC_BYTES; out += blockIdx.x * REC_BYTES; k += 2 * blockIdx.x;
     const Scalar256 kk = *k;
     G1::Pt p = pt_load<Fq>(pt, 0);
     pt_store<Fq>(out, 0, G1::mul_scalar(p, kk.l));       // k == 0 -> infinity (r == 0: B1 drops out, prover.rs)
@@ -186,9 +197,14 @@ __device__ __forceinline__ void store_canon(uint8_t* out, int slot, const fe& v)
 // scaled_off >= 0, [s*A_k, r*B1_k] (G1 XYZZ) at that offset.  Folds them in rank order and assembles the proof
 // (ark-groth16 0.5.0 create_proof_with_assignment).  With the scaled points present no scalar multiplication is left here:
 // A, B2 and C are three independent sums, converted to affine by three warps side by side.
+// CTA j of a batch assembles proof j from its own `count` records, (r, s), precomputation and 256-byte proof slot.
 __global__ void glue_post_kernel(const uint8_t* __restrict__ partials, int count, int stride, int scaled_off, const uint8_t* __restrict__ consts,
                                  const uint8_t* __restrict__ pre, const Scalar256* __restrict__ rs, uint8_t* __restrict__ proof) {
     __shared__ G1::Pt shA, shB1, shsA, shrB1;
+    partials += (size_t)blockIdx.x * count * stride;
+    pre += (size_t)blockIdx.x * PRE_BYTES;
+    rs += 2 * blockIdx.x;
+    proof += (size_t)blockIdx.x * 256;
     const Scalar256 r = rs[0], s = rs[1];
     const int warp = threadIdx.x >> 5;
     const bool lead = (threadIdx.x & 31) == 0;
@@ -253,7 +269,6 @@ __global__ void glue_post_kernel(const uint8_t* __restrict__ partials, int count
 }
 
 // ------------------------------------------------------------------------------------------------ peer-memory exchange
-constexpr size_t REC_BYTES = B2G_PARTIAL_BYTES + 256;  // device-side record of one rank: the public 768-byte partial + [s*A_k, r*B1_k]
 constexpr size_t XCHG_SLOT = 256 + REC_BYTES;         // epoch word at +0, record at +256
 constexpr size_t XCHG_BYTES = 2 * XCHG_SLOT;
 // The exchange arena of a rank (one cudaMalloc, mapped by its peers through CUDA IPC):
@@ -354,8 +369,10 @@ __global__ void __launch_bounds__(256) h_slice_kernel(uint8_t* const* __restrict
     fe_store(&h[lo + i], Fr::sub(Fr::mul(a, b), c));
 }
 
-__global__ void __launch_bounds__(256) gather_scalars_kernel(const fe* __restrict__ w, const uint32_t* __restrict__ idx, uint32_t n, fe* __restrict__ out) {
+// blockIdx.y = proof of a batch: its assignment at w + y * w_stride, its compacted scalars at out + y * n
+__global__ void __launch_bounds__(256) gather_scalars_kernel(const fe* __restrict__ w, uint32_t w_stride, const uint32_t* __restrict__ idx, uint32_t n, fe* __restrict__ out) {
     const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+    w += (size_t)blockIdx.y * w_stride; out += (size_t)blockIdx.y * n;
     if (j < n) fe_store(&out[j], fe_load_nc(&w[idx[j]]));
 }
 
@@ -567,54 +584,86 @@ static T* dev_upload(const void* host, size_t bytes, cudaStream_t st) {
     return d;
 }
 
-static void ensure_witness_buffers(b2g_ctx* ctx, size_t n_vars, size_t n) {
+// witness and witness-map vectors of `count` proofs (assignments n_vars apart, a / b / c / h n apart)
+static void ensure_witness_buffers(b2g_ctx* ctx, size_t n_vars, size_t n, uint32_t count = 1) {
+    n_vars *= count; n *= count;
     if (n_vars > ctx->cap_w) {
         if (ctx->d_w) cudaFree(ctx->d_w);
+        ctx->d_w = nullptr; ctx->cap_w = 0;
         CUDA_CHECK(cudaMalloc(&ctx->d_w, (n_vars + 1) * sizeof(fe)));
         ctx->cap_w = n_vars; ctx->alloc_gen++;
     }
     if (n > ctx->cap_n) {
-        for (fe** p : {&ctx->d_a, &ctx->d_b, &ctx->d_c, &ctx->d_h}) { if (*p) cudaFree(*p); CUDA_CHECK(cudaMalloc(p, n * sizeof(fe))); }
+        ctx->cap_n = 0;
+        for (fe** p : {&ctx->d_a, &ctx->d_b, &ctx->d_c, &ctx->d_h}) if (*p) { cudaFree(*p); *p = nullptr; }
+        for (fe** p : {&ctx->d_a, &ctx->d_b, &ctx->d_c, &ctx->d_h}) CUDA_CHECK(cudaMalloc(p, n * sizeof(fe)));
         ctx->cap_n = n; ctx->alloc_gen++;
     }
 }
 
-// per-stream MSM scratch of this context, sized for `pk` (re-created if a later key is larger)
-static void ensure_scratch(b2g_ctx* ctx, const b2g_pk* pk) {
-    bool ok = ctx->scratch_ok && (!pk->d_bidx || (ctx->scratch_bsort && pk->b_compact <= ctx->cap_wb));
+// the per-proof records, proof slots, (r, s) and glue precomputation of `count` proofs; grown on demand, never shrunk
+static void ensure_batch_buffers(b2g_ctx* ctx, uint32_t count) {
+    if (count <= ctx->cap_batch) return;
+    CUDA_CHECK(cudaDeviceSynchronize());
+    for (uint8_t** p : {&ctx->d_partial, &ctx->d_proof, &ctx->d_pre, &ctx->d_rs}) { cudaFree(*p); *p = nullptr; }
+    for (uint8_t** p : {&ctx->h_rs, &ctx->h_proof}) { cudaFreeHost(*p); *p = nullptr; }
+    ctx->cap_batch = 0; ctx->alloc_gen++;
+    if (ctx->scratch_ok) for (int q = 0; q < NQ; q++) ctx->scratch[q].result = nullptr;
+    CUDA_CHECK(cudaMalloc(&ctx->d_partial, count * REC_BYTES));
+    CUDA_CHECK(cudaMemset(ctx->d_partial, 0, count * REC_BYTES));
+    CUDA_CHECK(cudaMalloc(&ctx->d_proof, count * 256));
+    CUDA_CHECK(cudaMalloc(&ctx->d_pre, count * PRE_BYTES));
+    CUDA_CHECK(cudaMalloc(&ctx->d_rs, count * 64));
+    CUDA_CHECK(cudaMallocHost(&ctx->h_rs, count * 64));
+    CUDA_CHECK(cudaMallocHost(&ctx->h_proof, count * 256));
+    ctx->cap_batch = count;
+    if (ctx->scratch_ok) for (int q = 0; q < NQ; q++) ctx->scratch[q].result = ctx->d_partial + PARTIAL_OFF[q];
+}
+
+// per-stream MSM scratch of this context, sized for `pk` and `count` proofs.  Kept while later calls fit (a smaller batch
+// reuses it); re-created for exactly (pk, count) when they do not, so a larger key after a large batch does not inherit
+// that batch's size.
+static void ensure_scratch(b2g_ctx* ctx, const b2g_pk* pk, uint32_t count = 1) {
+    const size_t nwb = (size_t)pk->b_compact * count;
+    bool ok = ctx->scratch_ok && (!pk->d_bidx || (ctx->scratch_bsort && nwb <= ctx->cap_wb));
     for (int q = 0; q < NQ && ok; q++) {
         const MsmPlan& p = pk->plan[q]; const MsmScratch& sc = ctx->scratch[q];
-        if ((p.n ? p.n : 1) > sc.cap_n || p.nwin > sc.cap_nwin || p.nbuckets > sc.cap_buckets) ok = false;
+        if ((p.n ? p.n : 1) > sc.cap_n || p.nwin > sc.cap_nwin || p.nbuckets > sc.cap_buckets || count > sc.cap_count) ok = false;
     }
     if (ok) return;
     CUDA_CHECK(cudaDeviceSynchronize());
-    if (ctx->scratch_ok) { for (int q = 0; q < NQ; q++) msm_scratch_free(ctx->scratch[q]); ctx->scratch_ok = false; }
+    for (int q = 0; q < NQ; q++) msm_scratch_free(ctx->scratch[q]);     // also the remains of an allocation that failed
+    ctx->scratch_ok = false; ctx->alloc_gen++;
     for (int q = 0; q < NQ; q++) {
         const MsmPlan& p = pk->plan[q];
-        msm_scratch_alloc(ctx->scratch[q], p.n ? p.n : 1, p.nwin, p.nbuckets, q == Q_B2, q == Q_H || q == Q_L || (q == Q_B1 && pk->d_bidx));
+        msm_scratch_alloc(ctx->scratch[q], p.n ? p.n : 1, p.nwin, p.nbuckets, q == Q_B2, q == Q_H || q == Q_L || (q == Q_B1 && pk->d_bidx), count);
         cudaFree(ctx->scratch[q].result);
         ctx->scratch[q].result = ctx->d_partial + PARTIAL_OFF[q];
         ctx->scratch[q].result_owned = false;
+        ctx->scratch[q].result_stride = REC_BYTES;
     }
     ctx->scratch_bsort = pk->d_bidx != nullptr;
-    if (pk->b_compact > ctx->cap_wb) {
+    const size_t nwb_cap = (size_t)pk->b_compact * count;
+    if (nwb_cap > ctx->cap_wb) {
         if (ctx->d_wb) cudaFree(ctx->d_wb);
-        CUDA_CHECK(cudaMalloc(&ctx->d_wb, ((size_t)pk->b_compact + 1) * sizeof(fe)));
-        ctx->cap_wb = pk->b_compact;
+        ctx->d_wb = nullptr; ctx->cap_wb = 0;
+        CUDA_CHECK(cudaMalloc(&ctx->d_wb, (nwb_cap + 1) * sizeof(fe)));
+        ctx->cap_wb = nwb_cap;
     }
-    ctx->scratch_ok = true; ctx->alloc_gen++;
+    ctx->scratch_ok = true;
 }
 
-static void run_witness_map(b2g_ctx* ctx, b2g_mat* mat, cudaStream_t st) {
+// the witness map of `count` proofs side by side: one launch per kernel of the chain, the batch on a grid dimension
+static void run_witness_map(b2g_ctx* ctx, b2g_mat* mat, cudaStream_t st, uint32_t count = 1) {
     if (mat->reduction == B2G_REDUCTION_LIBSNARK) {
         spmv_launch(mat->n, mat->m, mat->num_inputs, mat->a_rowptr, mat->a_col, mat->a_val, mat->b_rowptr, mat->b_col, mat->b_val,
-                    ctx->d_w, ctx->d_a, ctx->d_b, ctx->d_c, st, mat->c_rowptr, mat->c_col, mat->c_val);
-        ntt_witness_transform_libsnark(mat->dom, ctx->d_a, ctx->d_b, ctx->d_c, ctx->d_a, ctx->d_h, st);   // d_a doubles as scratch
+                    ctx->d_w, ctx->d_a, ctx->d_b, ctx->d_c, st, mat->c_rowptr, mat->c_col, mat->c_val, count, mat->n_vars);
+        ntt_witness_transform_libsnark(mat->dom, ctx->d_a, ctx->d_b, ctx->d_c, ctx->d_a, ctx->d_h, st, count);   // d_a doubles as scratch
         return;
     }
     spmv_launch(mat->n, mat->m, mat->num_inputs, mat->a_rowptr, mat->a_col, mat->a_val, mat->b_rowptr, mat->b_col, mat->b_val,
-                ctx->d_w, ctx->d_a, ctx->d_b, ctx->d_c, st);
-    ntt_witness_transform(mat->dom, ctx->d_a, ctx->d_b, ctx->d_c, ctx->d_h, st);
+                ctx->d_w, ctx->d_a, ctx->d_b, ctx->d_c, st, nullptr, nullptr, nullptr, count, mat->n_vars);
+    ntt_witness_transform(mat->dom, ctx->d_a, ctx->d_b, ctx->d_c, ctx->d_h, st, count);
 }
 
 // a key's tables live on one device and describe one shard: checked before the first kernel that dereferences them
@@ -681,20 +730,21 @@ static void run_witness_map_split(b2g_ctx* ctx, b2g_mat* mat, uint32_t lo, uint3
     CUDA_CHECK(cudaGetLastError());
 }
 
-static void launch_msms(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, bool timed, bool scale, bool split_map = false) {
+// count > 1: a batch of proofs (witnesses pk->n_vars apart in d_w); every MSM sorts and accumulates the whole batch at once
+static void launch_msms(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, bool timed, bool scale, bool split_map = false, uint32_t count = 1) {
     cudaStream_t s0 = ctx->st[0], ssort = ctx->st[Q_L];
     CUDA_CHECK(cudaEventRecord(ctx->ev_w, s0));
     CUDA_CHECK(cudaStreamWaitEvent(ssort, ctx->ev_w, 0));
-    msm_sort(pk->plan[Q_A], ctx->scratch[Q_L], ctx->d_w + pk->scalar_off[Q_A] + pk->lo[Q_A], pk->cnt[Q_A], true, ssort);
+    msm_sort(pk->plan[Q_A], ctx->scratch[Q_L], ctx->d_w + pk->scalar_off[Q_A] + pk->lo[Q_A], pk->cnt[Q_A], true, ssort, count, pk->n_vars);
     CUDA_CHECK(cudaEventRecord(ctx->ev_sort, ssort));
     const bool bsparse = pk->d_bidx != nullptr;
     if (bsparse) {
         // B1 and B2 over the compacted base set: gather their scalars and sort them separately (on the B1 stream)
         cudaStream_t sb = ctx->st[Q_B1];
         CUDA_CHECK(cudaStreamWaitEvent(sb, ctx->ev_w, 0));
-        if (pk->b_compact) gather_scalars_kernel<<<(pk->b_compact + 255) / 256, 256, 0, sb>>>(ctx->d_w + pk->scalar_off[Q_B1] + pk->lo[Q_B1], pk->d_bidx, pk->b_compact, ctx->d_wb);
+        if (pk->b_compact) gather_scalars_kernel<<<dim3((pk->b_compact + 255) / 256, count), 256, 0, sb>>>(ctx->d_w + pk->scalar_off[Q_B1] + pk->lo[Q_B1], pk->n_vars, pk->d_bidx, pk->b_compact, ctx->d_wb);
         g_launch_count += 1;
-        msm_sort(pk->plan[Q_B1], ctx->scratch[Q_B1], ctx->d_wb, pk->b_compact, true, sb);
+        msm_sort(pk->plan[Q_B1], ctx->scratch[Q_B1], ctx->d_wb, pk->b_compact, true, sb, count, pk->b_compact);
         CUDA_CHECK(cudaEventRecord(ctx->ev_sortb, sb));
     }
     const int* order = witness_order();
@@ -707,7 +757,7 @@ static void launch_msms(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, bool timed, bool
         msm_accumulate(pk->plan[q], on_b ? ctx->scratch[Q_B1] : ctx->scratch[Q_L], ctx->scratch[q], ctx->st[q]);
         if (scale && (q == Q_A || q == Q_B1)) {
             const Scalar256* rs = reinterpret_cast<const Scalar256*>(ctx->d_rs);
-            scale_partial_kernel<<<1, 32, 0, ctx->st[q]>>>(ctx->d_partial + PARTIAL_OFF[q], q == Q_A ? rs + 1 : rs, ctx->d_partial + B2G_PARTIAL_BYTES + (q == Q_A ? 0 : 128));
+            scale_partial_kernel<<<count, 32, 0, ctx->st[q]>>>(ctx->d_partial + PARTIAL_OFF[q], q == Q_A ? rs + 1 : rs, ctx->d_partial + B2G_PARTIAL_BYTES + (q == Q_A ? 0 : 128));
             g_launch_count += 1;
         }
         if (timed) CUDA_CHECK(cudaEventRecord(ctx->ev_t[2 * q + 1], ctx->st[q]));
@@ -715,10 +765,10 @@ static void launch_msms(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, bool timed, bool
     }
     if (timed) CUDA_CHECK(cudaEventRecord(ctx->ev_t[10], s0));
     if (split_map) run_witness_map_split(ctx, mat, pk->lo[Q_H], pk->cnt[Q_H], s0);
-    else run_witness_map(ctx, mat, s0);
+    else run_witness_map(ctx, mat, s0, count);
     if (timed) CUDA_CHECK(cudaEventRecord(ctx->ev_t[11], s0));
     if (timed) CUDA_CHECK(cudaEventRecord(ctx->ev_t[0], s0));
-    msm_run(pk->plan[Q_H], ctx->scratch[Q_H], ctx->d_h + pk->lo[Q_H], pk->cnt[Q_H], true, s0);   // pairs min(#bases, #h) terms
+    msm_run(pk->plan[Q_H], ctx->scratch[Q_H], ctx->d_h + pk->lo[Q_H], pk->cnt[Q_H], true, s0, count, mat->n);   // pairs min(#bases, #h) terms
     if (timed) CUDA_CHECK(cudaEventRecord(ctx->ev_t[1], s0));
     for (int q = 1; q < NQ; q++) CUDA_CHECK(cudaStreamWaitEvent(s0, ctx->ev_done[q], 0));
 }
@@ -737,28 +787,33 @@ static void pk_release(b2g_pk* pk) {
 
 
 // (r, s) -> ctx->d_rs on stream 0.  Every entry point synchronises stream 0 before it returns (b2g_bench_device stages once),
-// so the pinned staging slot is free again by the time the next call overwrites it.
-static void stage_rs(b2g_ctx* ctx, const void* r, const void* s) {
-    memcpy(ctx->h_rs, r, 32); memcpy(ctx->h_rs + 32, s, 32);
-    CUDA_CHECK(cudaMemcpyAsync(ctx->d_rs, ctx->h_rs, 64, cudaMemcpyHostToDevice, ctx->st[0]));
+// so the pinned staging slot is free again by the time the next call overwrites it.  count proofs: r, s = count x 32 B each,
+// staged as r_j | s_j pairs.
+static void stage_rs(b2g_ctx* ctx, const void* r, const void* s, uint32_t count = 1) {
+    for (uint32_t j = 0; j < count; j++) {
+        memcpy(ctx->h_rs + 64 * j, (const uint8_t*)r + 32 * j, 32);
+        memcpy(ctx->h_rs + 64 * j + 32, (const uint8_t*)s + 32 * j, 32);
+    }
+    CUDA_CHECK(cudaMemcpyAsync(ctx->d_rs, ctx->h_rs, 64 * (size_t)count, cudaMemcpyHostToDevice, ctx->st[0]));
     memcpy(ctx->pre_r, r, 32); memcpy(ctx->pre_s, s, 32);
 }
 
 // r*delta1, s*delta1, rs*delta1, s*delta2 depend only on (r, s): forked from stream 0 (after d_rs is written and after the
 // previous proof's assembly has read d_pre) onto a side stream, so they overlap the MSMs
-static void launch_glue_pre(b2g_ctx* ctx, b2g_pk* pk) {
+static void launch_glue_pre(b2g_ctx* ctx, b2g_pk* pk, uint32_t count = 1) {
     CUDA_CHECK(cudaEventRecord(ctx->ev_fork, ctx->st[0]));
     CUDA_CHECK(cudaStreamWaitEvent(ctx->st_glue, ctx->ev_fork, 0));
-    glue_pre_kernel<<<1, 192, 0, ctx->st_glue>>>(pk->d_tab_delta1, pk->d_tab_delta2, pk->d_tab_aa, pk->d_tab_bb, reinterpret_cast<const Scalar256*>(ctx->d_rs), ctx->d_pre);
+    glue_pre_kernel<<<count, 192, 0, ctx->st_glue>>>(pk->d_tab_delta1, pk->d_tab_delta2, pk->d_tab_aa, pk->d_tab_bb, reinterpret_cast<const Scalar256*>(ctx->d_rs), ctx->d_pre);
     CUDA_CHECK(cudaEventRecord(ctx->ev_pre, ctx->st_glue));
     ctx->pre_valid = true;
     g_launch_count += 1;
 }
 
-// scaled = true: records of REC_BYTES with [s*A_k, r*B1_k] behind the partial; false: bare 768-byte partials (host-mediated exchange)
-static void launch_glue_post(b2g_ctx* ctx, b2g_pk* pk, const uint8_t* partials_dev, int count, bool scaled, cudaStream_t st) {
+// scaled = true: records of REC_BYTES with [s*A_k, r*B1_k] behind the partial; false: bare 768-byte partials (host-mediated exchange).
+// nproofs > 1: proofs of a batch, each assembled from its own `count` records
+static void launch_glue_post(b2g_ctx* ctx, b2g_pk* pk, const uint8_t* partials_dev, int count, bool scaled, cudaStream_t st, uint32_t nproofs = 1) {
     CUDA_CHECK(cudaStreamWaitEvent(st, ctx->ev_pre, 0));
-    glue_post_kernel<<<1, 128, 0, st>>>(partials_dev, count, scaled ? (int)REC_BYTES : B2G_PARTIAL_BYTES, scaled ? B2G_PARTIAL_BYTES : -1, pk->d_consts, ctx->d_pre,
+    glue_post_kernel<<<nproofs, 128, 0, st>>>(partials_dev, count, scaled ? (int)REC_BYTES : B2G_PARTIAL_BYTES, scaled ? B2G_PARTIAL_BYTES : -1, pk->d_consts, ctx->d_pre,
                                         reinterpret_cast<const Scalar256*>(ctx->d_rs), ctx->d_proof);
     g_launch_count += 1;
     CUDA_CHECK(cudaGetLastError());
@@ -766,13 +821,14 @@ static void launch_glue_post(b2g_ctx* ctx, b2g_pk* pk, const uint8_t* partials_d
 
 
 // Everything one proof does on the device between "witness and (r, s) are in HBM" and "proof bytes are in d_proof".
-// kind 0: whole proof; kind 1: base-sharded proof whose partials are exchanged through NVLink peer memory.
-static void enqueue_proof(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, int kind, bool timed) {
+// kind 0: whole proof, or `count` whole proofs of a batch; kind 1: base-sharded proof whose partials are exchanged through
+// NVLink peer memory.
+static void enqueue_proof(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, int kind, bool timed, uint32_t count = 1) {
     cudaStream_t s0 = ctx->st[0];
     unsigned int* d_flag = kind == 1 ? reinterpret_cast<unsigned int*>(ctx->d_xchg + XCHG_BYTES) : nullptr;   // local word after the two slots
     if (kind == 1) CUDA_CHECK(cudaMemsetAsync(d_flag, 0, 4, s0));
-    launch_glue_pre(ctx, pk);
-    launch_msms(ctx, pk, mat, timed, true, kind == 1 && map_is_split(ctx, mat));
+    launch_glue_pre(ctx, pk, count);
+    launch_msms(ctx, pk, mat, timed, true, kind == 1 && map_is_split(ctx, mat), count);
     if (timed) CUDA_CHECK(cudaEventRecord(ctx->ev_t[14], s0));
     if (kind == 1) {
         xchg_publish_kernel<<<1, 64, 0, s0>>>(ctx->d_partial, ctx->d_xchg, ctx->d_epoch);
@@ -780,22 +836,22 @@ static void enqueue_proof(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, int kind, bool
         g_launch_count += 2;
         launch_glue_post(ctx, pk, ctx->d_partials_all, ctx->shard_count, true, s0);
     } else {
-        launch_glue_post(ctx, pk, ctx->d_partial, 1, true, s0);
+        launch_glue_post(ctx, pk, ctx->d_partial, 1, true, s0, count);
     }
 }
 
 // Replays the captured pipeline (capturing it first if this context has none for (pk, mat)); falls back to direct launches
 // when graphs are disabled or the capture fails.
-static void run_proof(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, int kind) {
+static void run_proof(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, int kind, uint32_t count = 1) {
     cudaStream_t s0 = ctx->st[0];
-    if (!ctx->use_graph) { enqueue_proof(ctx, pk, mat, kind, true); return; }
-    const uint64_t key[3] = {pk->uid, mat->uid, ctx->alloc_gen};
+    if (!ctx->use_graph) { enqueue_proof(ctx, pk, mat, kind, true, count); return; }
+    const uint64_t key[4] = {pk->uid, mat->uid, ctx->alloc_gen, count};
     if (ctx->gexec[kind] && memcmp(ctx->g_key[kind], key, sizeof key)) { cudaGraphExecDestroy(ctx->gexec[kind]); ctx->gexec[kind] = nullptr; }
     if (!ctx->gexec[kind]) {
         const uint64_t before = g_launch_count.load();
         cudaGraph_t graph = nullptr;
         CUDA_CHECK(cudaStreamBeginCapture(s0, cudaStreamCaptureModeThreadLocal));
-        try { enqueue_proof(ctx, pk, mat, kind, false); }
+        try { enqueue_proof(ctx, pk, mat, kind, false, count); }
         catch (...) { cudaStreamEndCapture(s0, &graph); if (graph) cudaGraphDestroy(graph); cudaGetLastError(); g_launch_count = before; throw; }
         cudaError_t e = cudaStreamEndCapture(s0, &graph);
         if (e == cudaSuccess) e = cudaGraphInstantiate(&ctx->gexec[kind], graph, 0);
@@ -805,7 +861,7 @@ static void run_proof(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, int kind) {
         if (e != cudaSuccess) {                       // not fatal: run this context without graphs from now on
             cudaGetLastError();
             ctx->gexec[kind] = nullptr; ctx->use_graph = false;
-            enqueue_proof(ctx, pk, mat, kind, true);
+            enqueue_proof(ctx, pk, mat, kind, true, count);
             return;
         }
         memcpy(ctx->g_key[kind], key, sizeof key);
@@ -1102,6 +1158,7 @@ static void prove_common(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, const void* w_m
     check_shapes(ctx, pk, mat);
     if (!w_mont) throw_error(B2G_E_SHAPE, "null witness");
     ensure_witness_buffers(ctx, mat->n_vars, mat->n);
+    ensure_batch_buffers(ctx, 1);
     ensure_scratch(ctx, pk);
     cudaStream_t s0 = ctx->st[0];
     CUDA_CHECK(cudaEventRecord(ctx->ev_t[12], s0));
@@ -1165,6 +1222,49 @@ int b2g_prove_submit(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, const void* r_canon
     });
 }
 
+int b2g_prove_many(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, uint32_t count, const void* r_canon, const void* s_canon, const void* const* w_mont,
+                   uint8_t* proofs_out) {
+    return guarded([&] {
+        if (!ctx || !r_canon || !s_canon || !w_mont || !proofs_out) throw_error(B2G_E_SHAPE, "null pointer");
+        if (ctx->shard_count != 1) throw_error(B2G_E_SHAPE, "b2g_prove_many needs an unsharded context");
+        if (ctx->pending_out) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
+        if (count == 0 || count > MAX_BATCH) throw_error(B2G_E_SHAPE, "b2g_prove_many: count must be in [1, " + std::to_string(MAX_BATCH) + "]");
+        for (uint32_t j = 0; j < count; j++) if (!w_mont[j]) throw_error(B2G_E_SHAPE, "null witness " + std::to_string(j));
+        check_shapes(ctx, pk, mat);
+        // the sorted entries and bucket keys of a whole batch are u32 positions into one list
+        for (int q = 0; q < NQ; q++) {
+            const MsmPlan& p = pk->plan[q];
+            if (!p.table) continue;
+            if ((uint64_t)count * p.n * p.nwin >= (1ull << 32) || (uint64_t)count * p.nbuckets >= (1ull << 32))
+                throw_error(B2G_E_SHAPE, "b2g_prove_many: count x bases x windows of a query reaches 2^32 sorted entries; prove fewer per call");
+        }
+        DevGuard g(ctx->device);
+        try {
+            ensure_witness_buffers(ctx, mat->n_vars, mat->n, count);
+            ensure_batch_buffers(ctx, count);
+            ensure_scratch(ctx, pk, count);
+        } catch (const B2gError& e) {
+            if (e.code != B2G_E_DEVICE) throw;
+            cudaGetLastError();
+            throw_error(B2G_E_DEVICE, "b2g_prove_many: the device buffers of " + std::to_string(count) +
+                                      " proofs do not fit in device memory; prove fewer per call (" + e.what() + ")");
+        }
+        cudaStream_t s0 = ctx->st[0];
+        CUDA_CHECK(cudaEventRecord(ctx->ev_t[12], s0));
+        for (uint32_t j = 0; j < count; j++)
+            CUDA_CHECK(cudaMemcpyAsync(ctx->d_w + (size_t)j * mat->n_vars, w_mont[j], (size_t)mat->n_vars * 32, cudaMemcpyHostToDevice, s0));
+        CUDA_CHECK(cudaEventRecord(ctx->ev_t[13], s0));
+        stage_rs(ctx, r_canon, s_canon, count);
+        run_proof(ctx, pk, mat, 0, count);
+        ctx->pre_valid = false;
+        CUDA_CHECK(cudaMemcpyAsync(ctx->h_proof, ctx->d_proof, (size_t)count * 256, cudaMemcpyDeviceToHost, s0));
+        CUDA_CHECK(cudaEventRecord(ctx->ev_t[15], s0));
+        CUDA_CHECK(cudaStreamSynchronize(s0));
+        memcpy(proofs_out, ctx->h_proof, (size_t)count * 256);
+        collect_timings(ctx);
+    });
+}
+
 int b2g_host_register(const void* ptr, size_t bytes) {
     return guarded([&] {
         if (!ptr || !bytes) throw_error(B2G_E_SHAPE, "null pointer");
@@ -1215,6 +1315,7 @@ int b2g_prove_finish(b2g_ctx* ctx, b2g_pk* pk, const void* partials_all, int cou
         if (count < 1 || count > 64) throw_error(B2G_E_SHAPE, "partial count out of range");
         check_pk_ctx(ctx, pk);
         DevGuard g(ctx->device);
+        ensure_batch_buffers(ctx, 1);
         cudaStream_t s0 = ctx->st[0];
         if (!(ctx->pre_valid && !memcmp(ctx->pre_r, r_canon, 32) && !memcmp(ctx->pre_s, s_canon, 32))) { stage_rs(ctx, r_canon, s_canon); launch_glue_pre(ctx, pk); }
         ctx->pre_valid = false;

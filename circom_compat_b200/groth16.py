@@ -7,6 +7,8 @@
         <- /root/reference/src/circom/qap.rs:23-88
     Groth16.prove(pk, matrices, full_assignment, rng)
         <- Groth16::<Bn254, CircomReduction>::prove (src/zkey.rs:866): draws r then s, then the call above.
+    Groth16.create_proofs(pk, rs, matrices, assignments)
+        <- the first call above for many witnesses of one circuit, proved together in one device pass (b2g_prove_many).
 Arguments keep the reference's meaning; field elements are (n, 4) uint64 Montgomery limb arrays (fr_to_mont).
 """
 from __future__ import annotations
@@ -306,6 +308,30 @@ class Groth16:
         out = np.zeros(256, dtype=np.uint8)
         N.check(N.lib().b2g_prove(ctx._h, ph, mh, _ptr(rr), _ptr(ss), _ptr(w), _ptr(out)))
         return Proof(out.tobytes())
+
+    @staticmethod
+    def create_proofs(pk: ProvingKey, rs, matrices: ConstraintMatrices, assignments, ctx: Context = None, reduction=CircomReduction) -> list:
+        """create_proof_with_reduction_and_matrices for many witnesses of one circuit in ONE device pass (b2g_prove_many):
+        rs = sequence of (r, s), assignments = sequence of Montgomery full assignments; returns [Proof], proof i byte-identical
+        to the single call with (r_i, s_i, assignments[i]).  Unlike K contexts with submit / wait, every kernel of the
+        pipeline runs once for the whole batch; the context keeps device buffers for the largest batch it has proved."""
+        ctx = ctx or default_context()
+        rs, assignments = list(rs), list(assignments)
+        if len(rs) != len(assignments):
+            raise ValueError("create_proofs: one (r, s) per assignment")
+        if not assignments:
+            return []
+        ws = [_c(w) for w in assignments]
+        for w in ws:
+            if w.size // 4 != pk.n_vars:
+                raise ValueError("full_assignment length != n_vars")
+        ph, mh = ctx.pk_handle(pk), ctx.mat_handle(matrices, pk.n_vars, reduction.ID)
+        rr = np.concatenate([_scalar_bytes(r) for r, _ in rs])
+        ss = np.concatenate([_scalar_bytes(s) for _, s in rs])
+        ptrs = (C.c_void_p * len(ws))(*[w.ctypes.data for w in ws])
+        out = np.zeros((len(ws), 256), dtype=np.uint8)
+        N.check(N.lib().b2g_prove_many(ctx._h, ph, mh, len(ws), _ptr(rr), _ptr(ss), ptrs, _ptr(out)))
+        return [Proof(row.tobytes()) for row in out]
 
     @staticmethod
     def submit(pk: ProvingKey, r, s, matrices: ConstraintMatrices, full_assignment, ctx: Context, reduction=CircomReduction) -> 'PendingProof':

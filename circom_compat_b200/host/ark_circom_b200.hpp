@@ -418,6 +418,30 @@ struct Groth16T {                                       // Groth16::<Bn254, QAP>
         return out;
     }
 
+    // Many proofs for one key in ONE device pass (b2g_prove_many): every kernel of the pipeline runs once for the whole batch.
+    // Unlike prove_batch, which queues K independent proofs on K contexts, this is K proofs on one context, sorted and reduced
+    // together; proofs[i] is byte-identical to create_proof_with_reduction_and_matrices(rs[i], assignments[i]).  README.md
+    // gives the measured rates: it is the faster route up to 2^16 domains, prove_batch from 2^18 up.  The batch's device
+    // buffers stay with `gpu`.
+    static std::vector<Proof> create_proofs(const ProvingKey& pk, const ConstraintMatrices& matrices, const std::vector<std::pair<Fr, Fr>>& rs,
+                                            const std::vector<const std::vector<Fr>*>& assignments, Gpu& gpu = Gpu::instance()) {
+        if (rs.size() != assignments.size()) throw SynthesisError("create_proofs: one (r, s) per assignment");
+        const size_t n = rs.size();
+        if (n == 0) return {};
+        std::vector<BigInt256> rb(n), sb(n);
+        std::vector<const void*> ws(n);
+        for (size_t i = 0; i < n; i++) {
+            if (assignments[i]->size() != pk.a_query.size()) throw SynthesisError("AssignmentMissing: full_assignment length != n_vars");
+            rb[i] = rs[i].first.into_bigint(); sb[i] = rs[i].second.into_bigint();
+            ws[i] = assignments[i]->data();
+        }
+        std::vector<Proof> out(n);
+        std::vector<uint8_t> bytes(n * 256);
+        check(b2g_prove_many(gpu.ctx(), gpu.pk(pk), gpu.mat(matrices, pk.a_query.size(), QAP::ID), (uint32_t)n, rb.data(), sb.data(), ws.data(), bytes.data()));
+        for (size_t i = 0; i < n; i++) memcpy(out[i].bytes, bytes.data() + 256 * i, 256);
+        return out;
+    }
+
     template <class Rng>
     static Proof prove(const ProvingKey& pk, const ConstraintMatrices& matrices, const std::vector<Fr>& full_assignment, Rng& rng,
                        Gpu& gpu = Gpu::instance()) {

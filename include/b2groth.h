@@ -12,6 +12,7 @@
  *                             0.5.0 create_proof_with_assignment, restated in SURVEY.md 3.4)
  *   b2g_msm_g1 / b2g_msm_g2<- VariableBaseMSM::msm_bigint (ark-ec 0.5.0) as used by that function
  *   b2g_ntt                <- Radix2EvaluationDomain::{fft,ifft}_in_place (ark-poly 0.5.0) as used at qap.rs:60-81
+ *   b2g_prove_many         <- the same function called for many witnesses of one circuit, in one device pass
  *   b2g_prove_partial / b2g_prove_finish : the same proof split for base-range sharding over several GPUs
  *   b2g_fixed_base_g1/g2   <- the batch fixed-base multiplications of generate_random_parameters_with_reduction
  *                             (tests/groth16.rs:25); used to manufacture synthetic proving keys
@@ -129,6 +130,21 @@ B2G_API int b2g_prove(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, const void* r_cano
 B2G_API int b2g_prove_submit(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, const void* r_canon, const void* s_canon, const void* w_mont,
                              uint8_t proof_out[256]);
 B2G_API int b2g_prove_wait(b2g_ctx* ctx);
+
+/* b2g_prove_many <- the same Groth16::<Bn254, CircomReduction>::create_proof_with_reduction_and_matrices as b2g_prove, called
+ * for many witnesses of one circuit (a caller's loop over that function).
+ * count proofs for one (pk, mat) in one device pass: r_canon / s_canon = count x 32 B, w_mont = count pointers to n_vars x
+ * 32 B full assignments, proofs_out = count x 256 B.  proofs_out[i] is byte-identical to b2g_prove with (r_i, s_i, w_i).
+ * Synchronous.  Requires shard_count == 1 and 1 <= count <= 65535.  Every MSM sorts the whole batch into one list whose
+ * bucket key is (proof, bucket), so each kernel of the pipeline runs once per batch with count times the parallelism, and
+ * the latency-bound tails (fold, weighted bucket sum, glue) are paid once per batch.  The context's buffers grow to the
+ * largest batch seen and are kept; DESIGN.md lists the device memory per batched proof and the largest count per size.
+ * Errors: B2G_E_SHAPE for count == 0, null pointers, a sharded context, a shape mismatch, or count x bases x windows of a
+ * query >= 2^32 (checked before anything is allocated); B2G_E_DEVICE when the batch's buffers do not fit in device memory.
+ * It is the faster route up to 2^16 domains (H100 at 400 W: 2.3x three contexts in flight on the 2^14 bench key at count
+ * 64, 1.1x at 2^16); from 2^18 up, where one proof fills the GPU, several contexts in flight are faster (README.md). */
+B2G_API int b2g_prove_many(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, uint32_t count, const void* r_canon, const void* s_canon,
+                           const void* const* w_mont, uint8_t* proofs_out);
 /* Page-lock / release a host buffer (cudaHostRegister): a witness vector owned by the caller (a Rust Vec<Fr>, a std::vector)
  * uploads asynchronously and at full PCIe speed once registered.  Registering twice / unregistering an unknown pointer is not
  * an error. */
