@@ -12,8 +12,10 @@
 #include "../../include/b2groth.h"
 #include "ec.cuh"
 #include "msm.cuh"
+#include "fixed.cuh"
 #include "ntt.cuh"
 #include "util.cuh"
+#include "verify.cuh"
 
 namespace b2g {
 
@@ -73,6 +75,7 @@ struct b2g_ctx {
     uint8_t** d_peer_ptrs = nullptr;           // device array [shard_count]
     void* peer_mapped[64] = {};                // cudaIpcOpenMemHandle results (to close)
     int peers_imported = 0;
+    VerifyBufs* vbufs = nullptr;               // b2g_verify_many scratch (verify.cu), grown on demand
 };
 
 static std::atomic<uint64_t> g_next_uid{1};            // handles are told apart by uid, not by address (addresses get reused)
@@ -106,35 +109,13 @@ struct b2g_mat {
 
 namespace b2g {
 
-static thread_local std::string g_last_error;
-
-template <class Fn>
-static int guarded(Fn&& fn) {
-    try { fn(); return B2G_OK; }
-    catch (const B2gError& e) { g_last_error = e.what(); return e.code; }
-    catch (const std::exception& e) { g_last_error = e.what(); return B2G_E_DEVICE; }
-    catch (...) { g_last_error = "unknown error"; return B2G_E_DEVICE; }
-}
+thread_local std::string g_last_error;
 
 struct Scalar256 { uint32_t l[8]; };
 
+CtxView ctx_view(b2g_ctx* ctx) { return {ctx->device, ctx->st[0], ctx->pending_out != nullptr, &ctx->vbufs}; }
+
 // ------------------------------------------------------------------------------------------------ glue kernels
-// k * P from the 8-bit window table of P: lane w looks up digit w, a shared-memory tree adds the 32 partial points
-template <class C, class F>
-__device__ __forceinline__ typename C::Pt warp_fixed_mul(const void* __restrict__ table, const uint32_t* k, typename C::Pt* sh) {
-    const uint32_t lane = threadIdx.x & 31;
-    const uint32_t byte = (k[lane >> 2] >> (8 * (lane & 3))) & 255u;
-    typename C::Pt v = C::infinity();
-    if (byte) v = C::from_affine(aff_load<F>(table, (size_t)lane * 255u + byte - 1u));
-    sh[lane] = v;
-    __syncwarp();
-    #pragma unroll 1
-    for (int d = 16; d > 0; d >>= 1) {
-        if ((int)lane < d) { typename C::Pt a = sh[lane]; typename C::Pt q = sh[lane + d]; C::add(a, q); sh[lane] = a; }
-        __syncwarp();
-    }
-    return sh[0];
-}
 // pre[0] = r*delta1, pre[1] = s*delta1, pre[2] = (r*s)*delta1, pre[3] = K_C = s*(alpha1 + a_query[0]) + r*(beta1 + b_g1_query[0])
 // + (r*s)*delta1 (G1 XYZZ, 128 B each); then s*delta2 (G2 XYZZ, 256 B).  Every base here is fixed per key: its 8-bit window
 // table is built at b2g_pk_load, so each product is 32 table look-ups and a 5-level tree inside one warp instead of a
@@ -384,42 +365,11 @@ __global__ void xyzz_to_affine_kernel(const void* __restrict__ pts, uint32_t n, 
     aff_store<F>(out, i, C::to_affine(pt_load<F>(pts, i)));
 }
 
-__device__ __forceinline__ fe fe_from_words(uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t a4, uint32_t a5, uint32_t a6, uint32_t a7) {
-    fe r; r.l[0] = a0; r.l[1] = a1; r.l[2] = a2; r.l[3] = a3; r.l[4] = a4; r.l[5] = a5; r.l[6] = a6; r.l[7] = a7; return r;
-}
-// standard generators: G1 = (1, 2); G2 = /root/reference/src/zkey.rs:443-463
-__device__ __forceinline__ G1::Aff g1_generator() { G1::Aff g; g.x = Fq::one(); g.y = Fq::add(g.x, g.x); return g; }
-__device__ __forceinline__ G2::Aff g2_generator() {
-    G2::Aff g;
-    g.x.c0 = Fq::from_canonical(fe_from_words(0xd992f6edu, 0x46debd5cu, 0xf75edaddu, 0x674322d4u, 0x5e5c4479u, 0x426a0066u, 0x121f1e76u, 0x1800deefu));
-    g.x.c1 = Fq::from_canonical(fe_from_words(0xaef312c2u, 0x97e485b7u, 0x35a9e712u, 0xf1aa4933u, 0x31fb5d25u, 0x7260bfb7u, 0x920d483au, 0x198e9393u));
-    g.y.c0 = Fq::from_canonical(fe_from_words(0x66fa7daau, 0x4ce6cc01u, 0x0c43d37bu, 0xe3d1e769u, 0x8dcb408fu, 0x4aab7180u, 0xdb8c6debu, 0x12c85ea5u));
-    g.y.c1 = Fq::from_canonical(fe_from_words(0xd122975bu, 0x55acdadcu, 0x70b38ef3u, 0xbc4b3133u, 0x690c3395u, 0xec9e99adu, 0x585ff075u, 0x090689d0u));
-    return g;
-}
-template <class C> struct Gen;
-template <> struct Gen<G1> { static __device__ __forceinline__ G1::Aff get() { return g1_generator(); } };
-template <> struct Gen<G2> { static __device__ __forceinline__ G2::Aff get() { return g2_generator(); } };
-
 // out = pts[i] + pts[j] (G1 affine, 64-byte records), affine
 __global__ void affine_sum_kernel(const uint8_t* __restrict__ pts, int i, int j, uint8_t* __restrict__ out) {
     G1::Pt acc = G1::from_affine(aff_load<Fq>(pts, (size_t)i));
     G1::madd(acc, aff_load<Fq>(pts, (size_t)j));
     aff_store<Fq>(out, 0, G1::to_affine(acc));
-}
-
-// table[w][d-1] = d * 256^w * G (affine), w < 32, d = 1..255
-// base = nullptr: the group generator; else the affine point at `base` (e.g. delta of a proving key)
-template <class C, class F>
-__global__ void fixed_table_kernel(void* __restrict__ table, const void* __restrict__ base) {
-    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= 32u * 255u) return;
-    uint32_t w = i / 255u, d = i % 255u + 1u;
-    uint32_t k[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    k[w >> 2] = d << (8 * (w & 3));
-    typename C::Aff g = base ? aff_load<F>(base, 0) : Gen<C>::get();
-    typename C::Pt p = C::mul_scalar(C::from_affine(g), k);
-    aff_store<F>(table, i, C::to_affine(p));
 }
 
 template <class C, class F>
@@ -570,20 +520,6 @@ __global__ void test_op_kernel(int op, const uint8_t* __restrict__ a, const uint
 }
 
 // ------------------------------------------------------------------------------------------------ host helpers
-struct DevGuard {
-    int prev = 0;
-    explicit DevGuard(int dev) { cudaGetDevice(&prev); CUDA_CHECK(cudaSetDevice(dev)); }
-    ~DevGuard() { cudaSetDevice(prev); }
-};
-
-template <class T>
-static T* dev_upload(const void* host, size_t bytes, cudaStream_t st) {
-    T* d = nullptr;
-    CUDA_CHECK(cudaMalloc(&d, bytes ? bytes : 1));
-    if (bytes) CUDA_CHECK(cudaMemcpyAsync(d, host, bytes, cudaMemcpyHostToDevice, st));
-    return d;
-}
-
 // witness and witness-map vectors of `count` proofs (assignments n_vars apart, a / b / c / h n apart)
 static void ensure_witness_buffers(b2g_ctx* ctx, size_t n_vars, size_t n, uint32_t count = 1) {
     n_vars *= count; n *= count;
@@ -964,6 +900,7 @@ int b2g_ctx_destroy(b2g_ctx* ctx) {
         if (ctx->d_epoch) cudaFree(ctx->d_epoch);
         for (auto& e : ctx->ev_t) cudaEventDestroy(e);
         for (int k = 0; k < 64; k++) if (ctx->peer_mapped[k]) cudaIpcCloseMemHandle(ctx->peer_mapped[k]);
+        verify_bufs_free(ctx->vbufs);
         for (void* p : {(void*)ctx->d_xchg, (void*)ctx->d_peer_ptrs, (void*)ctx->d_partial, (void*)ctx->d_partials_all, (void*)ctx->d_proof, (void*)ctx->d_pre, (void*)ctx->d_w,
                         (void*)ctx->d_a, (void*)ctx->d_b, (void*)ctx->d_c, (void*)ctx->d_h}) if (p) cudaFree(p);
         delete ctx;
@@ -1585,6 +1522,7 @@ int b2g_fixed_base_g2(b2g_ctx* ctx, const void* scalars_canon, size_t n, void* o
 
 int b2g_test_op(b2g_ctx* ctx, int op, const void* a, const void* b, size_t n, void* out) {
     return guarded([&] {
+        if (ctx && op >= PAIRING_TEST_OP0) { DevGuard g(ctx->device); pairing_test_op(ctx->st[0], op, a, b, n, out); return; }
         TestOpShape s;
         if (!ctx || !a || !out || !test_op_shape(op, s)) throw_error(B2G_E_SHAPE, "bad arguments");
         if (!b && s.b && s.b != s.a) throw_error(B2G_E_SHAPE, "this op needs operand b");

@@ -24,6 +24,8 @@ struct B2gError : public std::runtime_error {
 
 extern std::atomic<uint64_t> g_launch_count;   // kernels launched by this library (defined in msm.cu)
 
+extern thread_local std::string g_last_error;   // b2g_last_error() (defined in prover.cu)
+
 [[noreturn]] inline void throw_error(int code, const std::string& msg) { throw B2gError(code, msg); }
 
 #define CUDA_CHECK(expr)                                                                                   \
@@ -33,5 +35,29 @@ extern std::atomic<uint64_t> g_launch_count;   // kernels launched by this libra
             ::b2g::throw_error(B2G_E_DEVICE, std::string("CUDA error ") + cudaGetErrorString(_e) + " at " + \
                                                  __FILE__ + ":" + std::to_string(__LINE__) + " (" #expr ")"); \
     } while (0)
+
+// runs the body of a C entry point: returns B2G_OK, or the error code with its message left for b2g_last_error()
+template <class Fn>
+inline int guarded(Fn&& fn) {
+    try { fn(); return B2G_OK; }
+    catch (const B2gError& e) { g_last_error = e.what(); return e.code; }
+    catch (const std::exception& e) { g_last_error = e.what(); return B2G_E_DEVICE; }
+    catch (...) { g_last_error = "unknown error"; return B2G_E_DEVICE; }
+}
+
+// ------------------------------------------------------------------------------------------------ host helpers
+struct DevGuard {
+    int prev = 0;
+    explicit DevGuard(int dev) { cudaGetDevice(&prev); CUDA_CHECK(cudaSetDevice(dev)); }
+    ~DevGuard() { cudaSetDevice(prev); }
+};
+
+template <class T>
+inline T* dev_upload(const void* host, size_t bytes, cudaStream_t st) {
+    T* d = nullptr;
+    CUDA_CHECK(cudaMalloc(&d, bytes ? bytes : 1));
+    if (bytes) CUDA_CHECK(cudaMemcpyAsync(d, host, bytes, cudaMemcpyHostToDevice, st));
+    return d;
+}
 
 }  // namespace b2g

@@ -1,0 +1,21 @@
+// verify.cuh - what the context code (prover.cu) and the batched verifier (verify.cu) share.
+#pragma once
+#include <cstddef>
+#include <cuda_runtime.h>
+
+struct b2g_ctx;
+
+namespace b2g {
+
+struct VerifyBufs;                          // a context's b2g_verify_many buffers (verify.cu)
+void verify_bufs_free(VerifyBufs* v);
+
+// the parts of a context verify.cu uses (b2g_ctx is private to prover.cu)
+struct CtxView { int device; cudaStream_t st; bool proof_pending; VerifyBufs** vbufs; };
+CtxView ctx_view(b2g_ctx* ctx);
+
+// b2g_test_op ops PAIRING_TEST_OP0 and up: the Fq12 tower and the pairing (verify.cu)
+constexpr int PAIRING_TEST_OP0 = 30;
+void pairing_test_op(cudaStream_t st, int op, const void* a, const void* b, size_t n, void* out);
+
+}  // namespace b2g

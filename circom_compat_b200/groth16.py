@@ -9,6 +9,9 @@
         <- Groth16::<Bn254, CircomReduction>::prove (src/zkey.rs:866): draws r then s, then the call above.
     Groth16.create_proofs(pk, rs, matrices, assignments)
         <- the first call above for many witnesses of one circuit, proved together in one device pass (b2g_prove_many).
+    Groth16.verify_many(vk, public_inputs, proofs)
+        <- Groth16::verify_with_processed_vk (src/zkey.rs:869-870, 914-916) for many proofs of one key in one device pass
+           (b2g_verify_many, with the key prepared on the device by b2g_vk_load <- process_vk).
 Arguments keep the reference's meaning; field elements are (n, 4) uint64 Montgomery limb arrays (fr_to_mont).
 """
 from __future__ import annotations
@@ -35,24 +38,29 @@ _TEST_OP_WORDS = {**{op: (4, 4, 4) for op in (0, 1, 2, 3, 4, 5, 14, 15, 16)}, 6:
                   8: (8, 8, 8), 10: (8, 0, 8), 12: (8, 8, 8), 9: (16, 16, 16), 11: (16, 0, 16), 13: (16, 16, 16),
                   17: (8, 8, 8), 18: (8, 8, 8), 19: (8, 8, 8), 28: (8, 8, 8),
                   20: (16, 16, 16), 21: (16, 8, 16), 22: (16, 0, 16), 23: (32, 32, 32), 24: (32, 16, 32), 25: (32, 0, 32),
-                  26: (32, 20, 32), 27: (16 * 20, 0, 32), 29: (4, 4, 8)}
+                  26: (32, 20, 32), 27: (16 * 20, 0, 32), 29: (4, 4, 8),
+                  # the pairing tower (csrc/pairing.cuh): Fq12 = 48 words, G1 / G2 affine = 8 / 16, a line (3 Fq2) = 24
+                  30: (48, 48, 48), **{op: (48, 0, 48) for op in (31, 32, 33, 34, 35, 36, 38)}, 37: (8, 16, 48), 39: (48, 24, 48),
+                  40: (8, 16, 48), 41: (24, 0, 48), 42: (24, 16, 48)}
 TEST_PAIR_RUN = 16            # entries per row of op 27; an entry is 16 words of affine point + 4 words whose bit 0 is the sign
 
 
 # Device-resident keys / matrices are cached per (host object, device, shard): every Context of that device and shard
 # can use them, so several proofs can be in flight on one GPU (one Context per in-flight proof) without duplicating
-# the 6 GiB of tables.  release(obj) / release_all() free them.
-_PK_HANDLES, _MAT_HANDLES = {}, {}
+# the 6 GiB of tables.  Device verifying keys (b2g_vk_load) are cached the same way per (host key object, device).
+# release(obj) / release_all() free them.
+_PK_HANDLES, _MAT_HANDLES, _VK_HANDLES = {}, {}, {}
+_CACHES = ((_PK_HANDLES, 'b2g_pk_free'), (_MAT_HANDLES, 'b2g_matrices_free'), (_VK_HANDLES, 'b2g_vk_free'))
 
 
 def release(obj):
-    for cache, free in ((_PK_HANDLES, 'b2g_pk_free'), (_MAT_HANDLES, 'b2g_matrices_free')):
+    for cache, free in _CACHES:
         for key in [k for k in cache if k[0] == id(obj)]:
             getattr(N.lib(), free)(cache.pop(key)[0])
 
 
 def release_all():
-    for cache, free in ((_PK_HANDLES, 'b2g_pk_free'), (_MAT_HANDLES, 'b2g_matrices_free')):
+    for cache, free in _CACHES:
         for key in list(cache):
             getattr(N.lib(), free)(cache.pop(key)[0])
 
@@ -108,6 +116,26 @@ class Context:
             N.check(N.lib().b2g_matrices_load(self._h, C.byref(d), C.byref(h)))
             _MAT_HANDLES[key] = (h, m)
         return _MAT_HANDLES[key][0]
+
+    def vk_handle(self, key):
+        """device verifying key for a verifier.VerifyingKey, PreparedVerifyingKey or ProvingKey (cached per host object)"""
+        from . import verifier
+        cache_key = (id(key), self.device)
+        if cache_key not in _VK_HANDLES:
+            vk = key.vk if isinstance(key, verifier.PreparedVerifyingKey) else key
+            if not isinstance(vk, verifier.VerifyingKey):
+                vk = verifier.VerifyingKey.from_proving_key(vk)
+            keep = {'alpha_g1': _mont_points([vk.alpha_g1], False), 'beta_g2': _mont_points([vk.beta_g2], True),
+                    'gamma_g2': _mont_points([vk.gamma_g2], True), 'delta_g2': _mont_points([vk.delta_g2], True),
+                    'gamma_abc_g1': _mont_points(vk.gamma_abc_g1, False)}
+            d = N.VkDesc()
+            d.n_public = len(vk.gamma_abc_g1) - 1
+            for name, arr in keep.items():
+                setattr(d, name, arr.ctypes.data)
+            h = C.c_void_p()
+            N.check(N.lib().b2g_vk_load(self._h, C.byref(d), C.byref(h)))
+            _VK_HANDLES[cache_key] = (h, key)
+        return _VK_HANDLES[cache_key][0]
 
     def prepare(self, pk: ProvingKey, matrices: ConstraintMatrices, reduction_id: int = N.REDUCTION_CIRCOM) -> None:
         """load (pk, matrices) and allocate this context's scratch now instead of inside the first proof"""
@@ -263,6 +291,17 @@ def fr_rand(rng) -> int:
 _R_INV_R = pow(1 << 256, -1, R_MOD)
 
 
+def _mont_points(points, g2: bool) -> np.ndarray:
+    """canonical affine points (None = infinity) -> rows of Montgomery words, all-zero = infinity"""
+    from .zkey import Q_MOD
+    vals = []
+    for pt in points:
+        coords = ([0] * (4 if g2 else 2) if pt is None else
+                  [pt[0][0], pt[0][1], pt[1][0], pt[1][1]] if g2 else [pt[0], pt[1]])
+        vals += [0 if pt is None else (int(v) << 256) % Q_MOD for v in coords]
+    return np.frombuffer(b''.join(v.to_bytes(32, 'little') for v in vals), dtype='<u8').copy()
+
+
 class CircomReduction:
     """R1CSToQAP implementation selected by Groth16<Bn254, CircomReduction> (src/circom/qap.rs:12-14)."""
     ID = N.REDUCTION_CIRCOM
@@ -380,6 +419,36 @@ class Groth16:
     def verify(vk, public_inputs, proof) -> bool:
         from . import verifier
         return verifier.verify(vk, public_inputs, proof)
+
+    @staticmethod
+    def verify_many(vk, public_inputs, proofs, ctx: Context = None) -> list:
+        """verify_with_processed_vk for many proofs of one key in ONE device pass (b2g_verify_many): `vk` is a VerifyingKey,
+        PreparedVerifyingKey or ProvingKey (prepared on the device once and cached per object), public_inputs = one
+        sequence of ints per proof, proofs = [Proof].  Returns [bool].  Verdicts equal the host call's, except that a proof
+        coordinate >= p is invalid here (arkworks cannot deserialise it) where the host verifier reduces it.  A public input
+        outside [0, r) raises B2gError (B2G_E_INPUT); an input count that does not match the key raises MalformedVerifyingKey."""
+        from . import verifier
+        public_inputs, proofs = [list(x) for x in public_inputs], list(proofs)
+        if len(public_inputs) != len(proofs):
+            raise ValueError("verify_many: one public-input list per proof")
+        if not proofs:
+            return []
+        base = vk.vk if isinstance(vk, verifier.PreparedVerifyingKey) else vk
+        n_public = len(base.gamma_abc_g1) - 1
+        for xs in public_inputs:
+            if len(xs) != n_public:
+                raise verifier.MalformedVerifyingKey(f"{len(xs)} public inputs for a key with {n_public}")
+            for x in xs:
+                if not 0 <= int(x) < R_MOD:        # the library refuses >= r too; this also covers values no 32 B word holds
+                    raise N.B2gError(N.B2G_E_INPUT, f"public input {int(x)} is not in [0, r)")
+        ctx = ctx or default_context()
+        vh = ctx.vk_handle(vk)
+        pub = b''.join(int(x).to_bytes(32, 'little') for xs in public_inputs for x in xs)
+        pub_arr = np.frombuffer(pub, dtype=np.uint8).copy() if pub else None
+        data = np.frombuffer(b''.join(p.data for p in proofs), dtype=np.uint8).copy()
+        out = np.zeros(len(proofs), dtype=np.uint8)
+        N.check(N.lib().b2g_verify_many(ctx._h, vh, len(proofs), _ptr(pub_arr) if pub_arr is not None else None, _ptr(data), _ptr(out)))
+        return [bool(v) for v in out]
 
     # base-range sharded variant: every rank calls prove_partial, the 768-byte partials are all-gathered by the caller
     # (torch.distributed / NCCL), then every rank calls prove_finish and obtains the same proof.

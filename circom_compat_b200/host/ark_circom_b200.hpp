@@ -9,6 +9,7 @@
 //   ark_circom::Groth16::create_proof_with_reduction_and_matrices <- call sites src/zkey.rs:903-912, benches/groth16.rs:52-61
 //   ark_circom::Groth16::prove                         <- src/zkey.rs:866 (draws r then s, SURVEY.md App. C.5)
 //   ark_circom::Groth16::process_vk / verify_with_processed_vk / verify <- src/zkey.rs:868-870, tests/groth16.rs:33-35
+//   ark_circom::Groth16::verify_many          <- verify_with_processed_vk for many proofs of one key, in one device pass
 //                                                         (host pairing, ark_circom_verifier.hpp; no GPU involved)
 //   ark_circom::read_wtns                              <- snarkjs .wtns (test-vectors/circuit2_js/witness.wtns; the reference
 //                                                         computes witnesses with WASM instead, out of scope here)
@@ -293,6 +294,13 @@ public:
     ~Gpu() { if (ctx_) b2g_ctx_destroy(ctx_); }
     Gpu(const Gpu&) = delete; Gpu& operator=(const Gpu&) = delete;
     static Gpu& instance() { static Gpu g(0); return g; }
+    static Gpu& on(int device) {                                       // one shared context per device (device 0: instance())
+        if (device == 0) return instance();
+        static std::map<int, std::unique_ptr<Gpu>> gpus;
+        auto& g = gpus[device];
+        if (!g) g.reset(new Gpu(device));
+        return *g;
+    }
     b2g_ctx* ctx() { return ctx_; }
 
     b2g_pk* pk(const ProvingKey& k) {
@@ -368,6 +376,32 @@ struct Groth16T {                                       // Groth16::<Bn254, QAP>
     }
     static bool verify(const VerifyingKey& vk, const std::vector<Fr>& public_inputs, const Proof& proof) {
         return ark_circom::verify_with_processed_vk(prepare_verifying_key(vk), public_inputs, proof);
+    }
+    // verify_with_processed_vk for many proofs of one key in ONE device pass (b2g_verify_many).  The key is prepared on the
+    // device at first use (b2g_vk_load) and kept in pvk.device.  Verdicts equal the host call's, except for a proof
+    // coordinate >= p: the host call throws SerializationError there, the batch reports the proof invalid.
+    static std::vector<bool> verify_many(const PreparedVerifyingKey& pvk, const std::vector<std::vector<Fr>>& public_inputs,
+                                         const std::vector<Proof>& proofs, int device = 0) {
+        if (public_inputs.size() != proofs.size()) throw SynthesisError("verify_many: one public-input list per proof");
+        const size_t n = proofs.size(), n_public = pvk.vk.gamma_abc_g1.size() - 1;
+        if (n == 0) return {};
+        for (const auto& xs : public_inputs) if (xs.size() != n_public) throw MalformedVerifyingKey();
+        Gpu& gpu = Gpu::on(device);
+        b2g_vk* vk = (b2g_vk*)pvk.device.find(gpu.ctx(), 0);
+        if (!vk) {
+            b2g_vk_desc d; memset(&d, 0, sizeof d);
+            d.n_public = (uint32_t)n_public;
+            d.alpha_g1 = &pvk.vk.alpha_g1; d.beta_g2 = &pvk.vk.beta_g2; d.gamma_g2 = &pvk.vk.gamma_g2; d.delta_g2 = &pvk.vk.delta_g2;
+            d.gamma_abc_g1 = pvk.vk.gamma_abc_g1.data();
+            check(b2g_vk_load(gpu.ctx(), &d, &vk));
+            pvk.device.put(gpu.ctx(), 0, vk, [](void* p) { b2g_vk_free((b2g_vk*)p); });
+        }
+        std::vector<BigInt256> pub(n * n_public);
+        for (size_t i = 0; i < n; i++) for (size_t k = 0; k < n_public; k++) pub[i * n_public + k] = public_inputs[i][k].into_bigint();
+        std::vector<uint8_t> bytes(n * 256), verdicts(n);
+        for (size_t i = 0; i < n; i++) memcpy(&bytes[i * 256], proofs[i].bytes, 256);
+        check(b2g_verify_many(gpu.ctx(), vk, (uint32_t)n, pub.empty() ? nullptr : pub.data(), bytes.data(), verdicts.data()));
+        return std::vector<bool>(verdicts.begin(), verdicts.end());
     }
     static Proof create_proof_with_reduction_and_matrices(const ProvingKey& pk, const Fr& r, const Fr& s, const ConstraintMatrices& matrices,
                                                           size_t num_inputs, size_t num_constraints, const std::vector<Fr>& full_assignment,

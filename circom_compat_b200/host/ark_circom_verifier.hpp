@@ -235,6 +235,8 @@ struct PreparedVerifyingKey {
     VerifyingKey vk;
     pairing::Fq12 alpha_g1_beta_g2;
     pairing::P2 gamma_g2_neg, delta_g2_neg;
+    DeviceSlot device;                                  // the key prepared on a device (b2g_vk_load) by Groth16::verify_many
+    void release_device() const { device.release(); }
 };
 
 inline PreparedVerifyingKey prepare_verifying_key(const VerifyingKey& vk) {

@@ -5,6 +5,9 @@
 //   groth16_bench --verify <circuit.zkey> <proof_hex> [inputs...]  host-only: process_vk + verify_with_processed_vk
 //   groth16_bench --ethereum <circuit.zkey> <proof_hex> [inputs...] host-only: src/ethereum.rs views of vk / proof / inputs, both directions
 //   groth16_bench <circuit.zkey> chain:<a>|<witness.wtns> [iters] [r_hex s_hex]
+//       B2G_MANY=K: also K proofs in one device pass (Groth16::create_proofs)
+//       B2G_VERIFY_MANY=K: also prove K proofs, negate A in every other one, and compare Groth16::verify_many's verdicts with
+//       verify_with_processed_vk called per proof (timing both)
 //       chain:<a> = the witness of the reference's squaring-chain bench family for input a
 //       (test-vectors/complex-circuit/input.json has a = 3), computed on the host instead of by WASM.
 #include <chrono>
@@ -189,6 +192,42 @@ int main(int argc, char** argv) {
             for (int i = 0; i < k; i++) std::printf("many[%d]=%s\n", i, proofs[(size_t)i].hex().c_str());
             std::printf("batched (%d proofs in one device pass, one context): %.3f ms/proof over %d calls, first_identical=%d\n", k, pms, reps,
                         !memcmp(proofs[0].bytes, proof.bytes, 256) ? 1 : 0);
+        }
+        if (const char* vm = std::getenv("B2G_VERIFY_MANY")) {           // batched verification against the host verifier
+            const int k = std::atoi(vm);
+            if (k < 1) throw SynthesisError("B2G_VERIFY_MANY must be >= 1");
+            std::vector<std::vector<Fr>> wv((size_t)k, full_assignment);
+            if (wsrc.rfind("chain:", 0) == 0)
+                for (int i = 1; i < k; i++) wv[(size_t)i] = chain_witness(params.a_query.size(), std::stoull(wsrc.substr(6)) + (unsigned long long)i);
+            std::vector<const std::vector<Fr>*> ws;
+            for (const auto& w : wv) ws.push_back(&w);
+            std::mt19937_64 rng(0xC0DE);
+            std::vector<std::pair<Fr, Fr>> rs;
+            for (int i = 0; i < k; i++) rs.push_back({Fr::rand(rng), Fr::rand(rng)});
+            std::vector<Proof> proofs = Groth16::create_proofs(params, matrices, rs, ws);
+            std::vector<std::vector<Fr>> inputs;
+            for (const auto& w : wv) inputs.emplace_back(w.begin() + 1, w.begin() + num_inputs);
+            for (int i = 1; i < k; i += 2) {                              // A -> -A: y -> p - y (y != 0 on the curve)
+                uint64_t y[4], d[4]; memcpy(y, proofs[(size_t)i].bytes + 32, 32);
+                unsigned __int128 borrow = 0;
+                for (int j = 0; j < 4; j++) { unsigned __int128 t = (unsigned __int128)detail::FQ_P[j] - y[j] - borrow; d[j] = (uint64_t)t; borrow = (t >> 64) & 1; }
+                memcpy(proofs[(size_t)i].bytes + 32, d, 32);
+            }
+            auto pvk = Groth16::process_vk(params.vk);
+            std::vector<bool> got = Groth16::verify_many(pvk, inputs, proofs);    // also loads the key on the device
+            auto t1 = std::chrono::steady_clock::now();
+            got = Groth16::verify_many(pvk, inputs, proofs);
+            const double dev_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t1).count();
+            int agree = 1, valid = 0;
+            auto t2 = std::chrono::steady_clock::now();
+            for (int i = 0; i < k; i++) {
+                const bool host = Groth16::verify_with_processed_vk(pvk, inputs[(size_t)i], proofs[(size_t)i]);
+                agree &= host == got[(size_t)i];
+                valid += host;
+            }
+            const double host_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t2).count();
+            std::printf("verify_many %d proofs (%d valid): agree=%d, device %.3f ms/batch (%.1f proofs/s), host verify_with_processed_vk "
+                        "%.3f ms/proof on one core (%.1f proofs/s)\n", k, valid, agree, dev_ms, k / (dev_ms / 1e3), host_ms / k, k / (host_ms / 1e3));
         }
         return 0;
     } catch (const std::exception& e) {

@@ -14,6 +14,9 @@
  *   b2g_ntt                <- Radix2EvaluationDomain::{fft,ifft}_in_place (ark-poly 0.5.0) as used at qap.rs:60-81
  *   b2g_prove_many         <- the same function called for many witnesses of one circuit, in one device pass
  *   b2g_prove_partial / b2g_prove_finish : the same proof split for base-range sharding over several GPUs
+ *   b2g_vk_load            <- GrothBn::process_vk(&params.vk) (src/zkey.rs:868, 914): the prepared verifying key, on the device
+ *   b2g_verify_many        <- GrothBn::verify_with_processed_vk(&pvk, &inputs, &proof) (src/zkey.rs:869-870, 915-916), called
+ *                             for many proofs of one key in one device pass
  *   b2g_fixed_base_g1/g2   <- the batch fixed-base multiplications of generate_random_parameters_with_reduction
  *                             (tests/groth16.rs:25); used to manufacture synthetic proving keys
  *
@@ -53,6 +56,7 @@ extern "C" {
 typedef struct b2g_ctx b2g_ctx;
 typedef struct b2g_pk b2g_pk;
 typedef struct b2g_mat b2g_mat;
+typedef struct b2g_vk b2g_vk;
 
 /* Proving key as read_zkey() produces it (src/zkey.rs:121-130); every pointer is a HOST pointer. */
 typedef struct {
@@ -183,6 +187,41 @@ B2G_API int b2g_p2p_connect_local(b2g_ctx** ctxs, int count);
 B2G_API int b2g_prove_sharded_p2p(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, const void* r_canon, const void* s_canon,
                                   const void* w_mont, uint8_t proof_out[256]);
 
+/* Verifying key as ark-groth16's VerifyingKey<Bn254> holds it (params.vk, src/zkey.rs:103-119); every pointer is a HOST
+ * pointer, points are affine Montgomery with the conventions of b2g_pk_desc (all-zero = infinity). */
+typedef struct {
+    uint32_t n_public;        /* public inputs per proof */
+    uint32_t reserved;
+    const void* alpha_g1;     /* 64 B  */
+    const void* beta_g2;      /* 128 B */
+    const void* gamma_g2;     /* 128 B */
+    const void* delta_g2;     /* 128 B */
+    const void* gamma_abc_g1; /* (n_public + 1) G1 */
+} b2g_vk_desc;
+
+/* b2g_vk_load <- GrothBn::process_vk (src/zkey.rs:868, 914; ark-groth16 0.5.0 prepare_verifying_key).  Checks that every point
+ * is on its curve (B2G_E_INPUT otherwise), computes e(alpha, beta) with the device pairing, the line coefficients of -gamma and
+ * -delta for every Miller-loop step, and an 8-bit window table per gamma_abc_g1[i + 1] (510 KiB each).  Like b2g_pk, the key is
+ * a device object any context of the same device can use. */
+B2G_API int b2g_vk_load(b2g_ctx* ctx, const b2g_vk_desc* desc, b2g_vk** out);
+B2G_API int b2g_vk_free(b2g_vk* vk);
+/* e(alpha, beta) as the loaded key holds it (PreparedVerifyingKey::alpha_g1_beta_g2): 384 B, twelve Montgomery Fq in the
+ * order c0.c0.c0, c0.c0.c1, c0.c1.c0, ..., c1.c2.c1 (host pointer) */
+B2G_API int b2g_vk_alpha_beta(b2g_vk* vk, void* out);
+
+/* b2g_verify_many <- GrothBn::verify_with_processed_vk (src/zkey.rs:869-870, 915-916), for count proofs of one key in one device
+ * pass.  public_inputs = count x n_public canonical 32 B scalars (may be NULL when n_public == 0); proofs = count x 256 B in the
+ * layout b2g_prove writes (canonical, all-zero point = infinity); verdicts_out = count bytes, 1 = valid, 0 = invalid.
+ * A proof is valid iff e(A, B) e(IC[0] + sum x_i IC[i + 1], -gamma) e(C, -delta) == e(alpha, beta), with the host verifier's
+ * semantics: a point at infinity contributes 1 to the product, a point not on its curve makes the proof invalid, and so does a
+ * coordinate >= p (arkworks cannot deserialise such a proof; the C++ mirror's single call throws there instead).  No G2
+ * subgroup check beyond the host verifier's.  Synchronous.
+ * Errors: B2G_E_SHAPE for count == 0, null pointers, a key of another device or a proof pending on the context; B2G_E_INPUT for
+ * a public input >= r (checked before anything runs); B2G_E_DEVICE when the batch's buffers do not fit in device memory (the
+ * context stays usable).  The context's buffers grow to the largest batch seen and are kept. */
+B2G_API int b2g_verify_many(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs,
+                            uint8_t* verdicts_out);
+
 /* Kernel-level entry points (parity tests, benchmarks). All pointers host. */
 B2G_API int b2g_msm_g1(b2g_ctx* ctx, const void* bases, const void* scalars, size_t n, int scalars_mont, void* out_xy_mont);
 B2G_API int b2g_msm_g2(b2g_ctx* ctx, const void* bases, const void* scalars, size_t n, int scalars_mont, void* out_xy_mont);
@@ -203,6 +242,14 @@ B2G_API int b2g_fixed_base_g2(b2g_ctx* ctx, const void* scalars_canon, size_t n,
  *        an entry is a 128 B affine point and a 32 B word whose bit 0 negates it,
  *     28 fq2 product as the G2 accumulation kernel inlines it (n x 64 B),
  *     29 fq plain 512-bit product a * b for a < 2^255 (a, b: 32 B; out: 64 B little-endian).
+ * Ops 30 and up are the pairing tower (csrc/pairing.cuh) on Fq12 values of 12 x 32 B Montgomery, in the order
+ * c0.c0.c0, c0.c0.c1, c0.c1.c0, ..., c1.c2.c1 (out always 384 B):
+ *     30 fq12 mul(a, b), 31 fq12 sqr, 32 cyclotomic sqr, 33 / 34 / 35 Frobenius a^p / a^(p^2) / a^(p^3),
+ *     36 final exponentiation a^((p^12 - 1) / r), 37 pairing e(a, b) (a: 64 B G1 affine, b: 128 B G2 affine), 38 fq12 inverse,
+ *     39 sparse line product a * (c0 + c3 w + c4 w^3) (b: c0 || c3 || c4, 3 x 64 B Fq2),
+ *     40 Miller loop of the pair (a, b) without the final exponentiation (a: G1, b: G2 affine),
+ *     41 / 42 one projective doubling / addition of b (G2 affine) step on the twist point a = X || Y || Z (3 x 64 B):
+ *        out = the new X || Y || Z followed by the line's c0 || c1 || c2.
  * Operand and result sizes per row therefore differ by op; b may be NULL where the op does not read it. */
 B2G_API int b2g_test_op(b2g_ctx* ctx, int op, const void* a, const void* b, size_t n, void* out);
 
