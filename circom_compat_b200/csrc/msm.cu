@@ -1,7 +1,5 @@
 // msm.cu - kernels and launchers of the fixed-base-table Pippenger MSM described in msm.cuh.
-#include <algorithm>
 #include <type_traits>
-#include <vector>
 #include "msm.cuh"
 #include "util.cuh"
 
@@ -208,188 +206,12 @@ __global__ void __launch_bounds__(256) msm_scatter_kernel(const fe* __restrict__
     if (pending) entries[offsets[b] + atomicAdd(&cursor[b], 1u)] = entry;
 }
 
-// ------------------------------------------------------------------------------------------------ (4a) batched-affine pre-reduction
-// Level structure (depends only on the sorted scalars).  cnt_k[b] = ceil(cnt_{k-1}[b] / 2); off_k = exclusive scan.
-// One CTA; levels are processed one after the other (each needs the previous one's offsets).
-__global__ void __launch_bounds__(1024) msm_aff_levels_kernel(uint32_t nb, int rounds, uint32_t* const* __restrict__ off) {
-    __shared__ uint32_t warp_sums[32];
-    __shared__ uint32_t carry_s;
-    const uint32_t tid = threadIdx.x, per = (nb + 1023u) / 1024u;
-    const uint32_t lo = min(tid * per, nb), hi = min(lo + per, nb);
-    for (int k = 1; k <= rounds; k++) {
-        const uint32_t* prev = off[k - 1];
-        uint32_t* cur = off[k];
-        uint32_t s = 0;
-        for (uint32_t j = lo; j < hi; j++) s += (prev[j + 1] - prev[j] + 1u) >> 1;
-        uint32_t v = s;
-        #pragma unroll
-        for (int d = 1; d < 32; d <<= 1) { uint32_t t = __shfl_up_sync(0xffffffffu, v, d); if ((tid & 31) >= (uint32_t)d) v += t; }
-        if ((tid & 31) == 31) warp_sums[tid >> 5] = v;
-        __syncthreads();
-        if (tid < 32) {
-            uint32_t w = warp_sums[tid], x = w;
-            #pragma unroll
-            for (int d = 1; d < 32; d <<= 1) { uint32_t t = __shfl_up_sync(0xffffffffu, x, d); if (tid >= (uint32_t)d) x += t; }
-            warp_sums[tid] = x - w;
-            if (tid == 31) carry_s = x;
-        }
-        __syncthreads();
-        uint32_t run = warp_sums[tid >> 5] + v - s;
-        for (uint32_t j = lo; j < hi; j++) { cur[j] = run; run += (prev[j + 1] - prev[j] + 1u) >> 1; }
-        if (tid == 0) cur[nb] = carry_s;
-        __syncthreads();                                   // cur is complete (and visible to the block) before it becomes prev
-    }
-}
-
-// src[q] for every slot q of level k: first input slot in level k-1, bit 31 set when the slot is the sum of a pair
-// (clear: the odd element of its bucket, copied through).
-__global__ void __launch_bounds__(256) msm_aff_src_kernel(const uint32_t* __restrict__ off_prev, const uint32_t* __restrict__ off_cur, uint32_t nb,
-                                                          uint32_t* __restrict__ src) {
-    const uint32_t total = off_cur[nb];
-    for (uint32_t q = blockIdx.x * blockDim.x + threadIdx.x; q < total; q += gridDim.x * blockDim.x) {
-        uint32_t lo = 0, hi = nb;                          // invariant: off_cur[lo] <= q < off_cur[hi]
-        while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (off_cur[mid] <= q) lo = mid; else hi = mid; }
-        const uint32_t j = q - off_cur[lo];
-        const uint32_t p0 = off_prev[lo], cnt = off_prev[lo + 1] - p0;
-        src[q] = (p0 + 2u * j) | ((2u * j + 1u < cnt) ? 0x80000000u : 0u);
-    }
-}
-
-// what one slot of a level is made of, and the denominator its affine addition needs
-enum : int { AFF_COPY_P = 0, AFF_COPY_Q = 1, AFF_INF = 2, AFF_ADD = 3, AFF_DBL = 4 };
-
-template <class C, class F, bool LEVEL0>
-__device__ __forceinline__ int aff_fetch(const void* __restrict__ table, const uint32_t* __restrict__ entries, const void* __restrict__ prev,
-                                         uint32_t s, typename C::Aff& P, typename C::Aff& Q, typename F::elem& d) {
-    const uint32_t i0 = s & 0x7fffffffu;
-    const bool pair = (s >> 31) != 0;
-    if (LEVEL0) {
-        const uint32_t e0 = entries[i0];
-        P = aff_load<F>(table, (size_t)(e0 & 0x7fffffffu));
-        if (e0 >> 31) P.y = F::neg(P.y);
-        if (pair) {
-            const uint32_t e1 = entries[i0 + 1];
-            Q = aff_load<F>(table, (size_t)(e1 & 0x7fffffffu));
-            if (e1 >> 31) Q.y = F::neg(Q.y);
-        }
-    } else {
-        P = aff_load<F>(prev, (size_t)i0);
-        if (pair) Q = aff_load<F>(prev, (size_t)i0 + 1);
-    }
-    if (!pair) return AFF_COPY_P;
-    if (C::aff_is_inf(P)) return AFF_COPY_Q;
-    if (C::aff_is_inf(Q)) return AFF_COPY_P;
-    if (F::eq(P.x, Q.x)) {
-        if (F::eq(P.y, Q.y) && !F::is_zero(P.y)) { d = F::dbl(P.y); return AFF_DBL; }
-        return AFF_INF;                                    // P + (-P)
-    }
-    d = F::sub(Q.x, P.x);
-    return AFF_ADD;
-}
-
-// pass 1: exclusive prefix products of the denominators along each thread's slots, thread total -> totals[t]
-template <class C, class F, bool LEVEL0>
-__global__ void __launch_bounds__(128) msm_aff_prod_kernel(const void* __restrict__ table, const uint32_t* __restrict__ entries, const void* __restrict__ prev,
-                                                           const uint32_t* __restrict__ src, const uint32_t* __restrict__ off_cur, uint32_t nb,
-                                                           void* __restrict__ pref, void* __restrict__ totals) {
-    using E = typename F::elem; using Aff = typename C::Aff;
-    const uint32_t total = off_cur[nb];
-    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x, stride = gridDim.x * blockDim.x;
-    E run = F::one();
-    #pragma unroll 1
-    for (int i = 0; i < MSM_AFF_M; i++) {
-        const uint64_t q64 = (uint64_t)t + (uint64_t)i * stride;
-        if (q64 >= total) break;
-        const uint32_t q = (uint32_t)q64;
-        Aff P, Q; E d;
-        const int kind = aff_fetch<C, F, LEVEL0>(table, entries, prev, src[q], P, Q, d);
-        if (kind >= AFF_ADD) {
-            elem_store((char*)pref + (size_t)q * Bytes<F>::ELEM, run);
-            run = F::mul(run, d);
-        }
-    }
-    elem_store((char*)totals + (size_t)t * Bytes<F>::ELEM, run);
-}
-
-// pass 2: totals[i] <- 1 / totals[i] for i < count (all non-zero by construction).  Thread u owns the strided set
-// u, u + U, u + 2U, ... (coalesced across the warp), forms their product with the prefixes parked in `scratch`, inverts
-// once, and unwinds.
-template <class F>
-__global__ void __launch_bounds__(64) msm_aff_invert_kernel(void* __restrict__ totals, void* __restrict__ scratch, uint32_t count, uint32_t U) {
-    using E = typename F::elem;
-    const uint32_t u = blockIdx.x * blockDim.x + threadIdx.x;
-    if (u >= U) return;
-    constexpr size_t B = Bytes<F>::ELEM;
-    E run = F::one();
-    int last = -1;
-    #pragma unroll 1
-    for (int v = 0; v < MSM_AFF_S; v++) {
-        const uint64_t idx = (uint64_t)u + (uint64_t)v * U;
-        if (idx >= count) break;
-        E x; elem_load(x, (const char*)totals + idx * B);
-        elem_store((char*)scratch + idx * B, run);
-        run = F::mul(run, x);
-        last = v;
-    }
-    if (last < 0) return;
-    E inv = F::inv(run);
-    #pragma unroll 1
-    for (int v = last; v >= 0; v--) {
-        const uint64_t idx = (uint64_t)u + (uint64_t)v * U;
-        E x, pre; elem_load(x, (const char*)totals + idx * B); elem_load(pre, (const char*)scratch + idx * B);
-        elem_store((char*)totals + idx * B, F::mul(inv, pre));
-        inv = F::mul(inv, x);
-    }
-}
-
-// pass 3: back-substitution.  1/d_i = inv * pref_i, inv *= d_i; lambda = (yQ - yP) / d (or 3 xP^2 / (2 yP));
-// x3 = lambda^2 - xP - xQ, y3 = lambda (xP - x3) - yP.
-template <class C, class F, bool LEVEL0>
-__global__ void __launch_bounds__(128) msm_aff_apply_kernel(const void* __restrict__ table, const uint32_t* __restrict__ entries, const void* __restrict__ prev,
-                                                            const uint32_t* __restrict__ src, const uint32_t* __restrict__ off_cur, uint32_t nb,
-                                                            const void* __restrict__ pref, const void* __restrict__ totals_inv, void* __restrict__ out) {
-    using E = typename F::elem; using Aff = typename C::Aff;
-    const uint32_t total = off_cur[nb];
-    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x, stride = gridDim.x * blockDim.x;
-    if (t >= total) return;
-    E inv; elem_load(inv, (const char*)totals_inv + (size_t)t * Bytes<F>::ELEM);
-    int i = MSM_AFF_M - 1;
-    while ((uint64_t)t + (uint64_t)i * stride >= total) i--;
-    #pragma unroll 1
-    for (; i >= 0; i--) {
-        const uint32_t q = t + (uint32_t)i * stride;
-        Aff P, Q; E d;
-        const int kind = aff_fetch<C, F, LEVEL0>(table, entries, prev, src[q], P, Q, d);
-        Aff r;
-        if (kind >= AFF_ADD) {
-            E pre; elem_load(pre, (const char*)pref + (size_t)q * Bytes<F>::ELEM);
-            const E inv_d = F::mul(inv, pre);
-            inv = F::mul(inv, d);
-            E num;
-            if (kind == AFF_ADD) num = F::sub(Q.y, P.y);
-            else { const E xx = F::sqr(P.x); num = F::add(F::dbl(xx), xx); Q.x = P.x; }
-            const E lam = F::mul(num, inv_d);
-            r.x = F::sub(F::sub(F::sqr(lam), P.x), Q.x);
-            r.y = F::sub(F::mul(lam, F::sub(P.x, r.x)), P.y);
-        } else if (kind == AFF_COPY_P) r = P;
-        else if (kind == AFF_COPY_Q) r = Q;
-        else { r.x = F::zero(); r.y = F::zero(); }
-        aff_store<F>(out, (size_t)q, r);
-    }
-}
-
 // ------------------------------------------------------------------------------------------------ (4) accumulate
 // Run t = sorted positions [t*chunk, (t+1)*chunk), owned by one thread (G1) or one lane pair (G2).  Buckets that lie entirely
 // inside the run are written to buckets[]; a run's first / last segment that belongs to a bucket crossing the run boundary
 // goes to frag_first[t] / frag_last[t].
-// occupancy target: G1 runs 4 CTAs/SM at 128 registers.
-template <class F> struct AccOcc;
-#ifndef B2G_G1_CTAS
-#define B2G_G1_CTAS 4
-#endif
-template <> struct AccOcc<Fq> { static constexpr int MIN_CTAS = B2G_G1_CTAS; };
 
-// slab_words != 0: the CTA's contiguous slab of the sorted entry list (G1: 128 runs = 32 KB at the default run length) is
+// slab_words != 0: the CTA's contiguous slab of the sorted entry list (128 runs = 32 KB at the default run length) is
 // brought into shared memory by ONE bulk asynchronous copy (cp.async.bulk -> UBLKCP, completion on an mbarrier) instead of
 // 64 strided 4-byte loads per run.  Every thread of the CTA calls this.
 __device__ __forceinline__ void acc_stage_slab(uint32_t* slab, unsigned long long* slab_bar, const uint32_t* __restrict__ entries,
@@ -414,7 +236,7 @@ __device__ __forceinline__ void acc_stage_slab(uint32_t* slab, unsigned long lon
     }
 }
 
-constexpr int MSM_SLAB_MAX_BYTES = 48 * 1024;   // larger slabs are not staged: the runs read the entry list directly
+constexpr int MSM_SLAB_MAX_BYTES = 48 * 1024;   // larger G1 slabs are not staged: the runs read the entry list directly
 
 // first bucket of the run starting at `start`: largest b with offsets[b] <= start, skipping empty buckets that share the offset
 __device__ __forceinline__ uint32_t acc_first_bucket(const uint32_t* __restrict__ offsets, uint32_t nb, uint32_t start, uint32_t& bucket_end) {
@@ -426,8 +248,9 @@ __device__ __forceinline__ uint32_t acc_first_bucket(const uint32_t* __restrict_
     return b;
 }
 
+// occupancy target: 4 CTAs/SM at 128 registers
 template <class C, class F>
-__global__ void __launch_bounds__(128, AccOcc<F>::MIN_CTAS) msm_accumulate_kernel(const void* __restrict__ table, const uint32_t* __restrict__ entries,
+__global__ void __launch_bounds__(128, 4) msm_accumulate_kernel(const void* __restrict__ table, const uint32_t* __restrict__ entries,
                                       const uint32_t* __restrict__ offsets, uint32_t nb, uint32_t chunk,
                                       void* __restrict__ buckets, void* __restrict__ frag_first, void* __restrict__ frag_last, uint32_t slab_words) {
     using Pt = typename C::Pt; using Aff = typename C::Aff;
@@ -446,7 +269,8 @@ __global__ void __launch_bounds__(128, AccOcc<F>::MIN_CTAS) msm_accumulate_kerne
     Pt acc = C::infinity();
     uint32_t seg_start = start;
     for (uint32_t pos = start; pos < end;) {
-        const uint32_t e = slab_words ? slab[pos - (uint32_t)cta_first] : (entries ? entries[pos] : pos);   // entries == nullptr: `table` is a pre-reduced point list (4a)
+        // slab index pos - cta_first, formed in 32 bits: with the 64-bit cta_first live across the loop, CUDA 12.9 spills 8 B
+        const uint32_t e = slab_words ? slab[pos - start + threadIdx.x * chunk] : entries[pos];
         Aff p = aff_load<F>(table, (size_t)(e & 0x7fffffffu));
         if (e >> 31) p.y = F::neg(p.y);
         C::madd(acc, p);
@@ -472,17 +296,13 @@ __global__ void __launch_bounds__(128, AccOcc<F>::MIN_CTAS) msm_accumulate_kerne
 // spills ~150 B per thread and measured slower (H100 80GB HBM3, 400 W: 9.04-9.08 ms vs 8.49-8.52 ms per 2^20 accumulation).
 __global__ void __launch_bounds__(128, 3) msm_accumulate_g2_kernel(const void* __restrict__ table, const uint32_t* __restrict__ entries,
                                       const uint32_t* __restrict__ offsets, uint32_t nb, uint32_t chunk,
-                                      void* __restrict__ buckets, void* __restrict__ frag_first, void* __restrict__ frag_last, uint32_t slab_words) {
+                                      void* __restrict__ buckets, void* __restrict__ frag_first, void* __restrict__ frag_last) {
     const uint32_t total = offsets[nb];
     const uint32_t t = (blockIdx.x * blockDim.x + threadIdx.x) >> 1;
     const uint32_t half = threadIdx.x & 1u;
     const bool A = half == 0;
     const unsigned mask = 3u << (threadIdx.x & 30u);
     const uint64_t start64 = (uint64_t)t * chunk;
-    extern __shared__ __align__(128) uint32_t slab[];
-    __shared__ __align__(8) unsigned long long slab_bar;
-    const uint64_t cta_first = (uint64_t)blockIdx.x * (blockDim.x / 2) * chunk;
-    if (slab_words) acc_stage_slab(slab, &slab_bar, entries, cta_first, total, slab_words);
     if (start64 >= total) return;
     const uint32_t start = (uint32_t)start64;
     const uint32_t end = (uint32_t)min((uint64_t)total, start64 + chunk);
@@ -492,7 +312,7 @@ __global__ void __launch_bounds__(128, 3) msm_accumulate_g2_kernel(const void* _
     bool empty = true;
     uint32_t seg_start = start;
     for (uint32_t pos = start; pos < end;) {
-        const uint32_t e = slab_words ? slab[pos - (uint32_t)cta_first] : (entries ? entries[pos] : pos);   // entries == nullptr: `table` is a pre-reduced point list (4a)
+        const uint32_t e = entries[pos];
         fe2 qc;
         elem_load_nc(qc, (const char*)table + (size_t)(e & 0x7fffffffu) * 128 + half * 64);
         qc = Fq2::sel((e >> 31) && !A, Fq2::neg(qc), qc);
@@ -705,13 +525,6 @@ void msm_scratch_alloc(MsmScratch& s, uint32_t n, int nwin, uint32_t nbuckets_on
     const size_t nbuckets = (size_t)nbuckets_one * count;
     const size_t nchunks = (nent + s.chunk - 1) / s.chunk + 1;
     s.reduce_chunk = env_u32("B2G_MSM_REDUCE_CHUNK", MSM_REDUCE_CHUNK_DEFAULT);
-    // the bulk-staged slab of the accumulation is on for G1, off for G2.  On an H100 (2^20 chain) neither switch is
-    // measurable: G1 accumulation 2.66-2.68 ms on vs 2.69 ms off (700 W); lane-pair G2 at 4 CTAs/SM 9.04-9.08 ms off vs
-    // 9.12 ms on (400 W).  B2G_ACC_BULK=0 / 1 forces it off / on for both; read here, like the chunk, for every scratch
-    {
-        const char* bulk_env = getenv("B2G_ACC_BULK");
-        s.bulk = bulk_env && *bulk_env ? *bulk_env == '1' : !g2;
-    }
     const size_t npart = ((size_t)nbuckets_one / (s.reduce_chunk * 32) + 64) * count;
     if (with_sort) {
         CUDA_CHECK(cudaMalloc(&s.counts, (size_t)nbuckets * 4));
@@ -727,55 +540,20 @@ void msm_scratch_alloc(MsmScratch& s, uint32_t n, int nwin, uint32_t nbuckets_on
     CUDA_CHECK(cudaMalloc(&s.buckets, (size_t)nbuckets * pt));
     CUDA_CHECK(cudaMalloc(&s.partials, (npart + 1) * pt));
     CUDA_CHECK(cudaMalloc(&s.result, pt)); s.result_owned = true;
-    // batched-affine pre-reduction (4a): OFF by default.  The 36 % multiply saving is paid for with the DRAM traffic of the
-    // three-pass structure (every point gathered twice per level, plus the intermediate lists) and the latency of the shared
-    // inversion.  B2G_MSM_AFFINE_ROUNDS=R opts in.
-    {
-        int rounds = 0;
-        const char* ov = getenv("B2G_MSM_AFFINE_ROUNDS");
-        if (ov && *ov) { long x = strtol(ov, nullptr, 10); rounds = x < 0 ? 0 : (x > MSM_AFF_MAX_ROUNDS ? MSM_AFF_MAX_ROUNDS : (int)x); }
-        s.aff_cap_rounds = rounds;
-        s.aff_nmax[0] = (uint32_t)nent;
-        for (int k = 1; k <= rounds; k++) s.aff_nmax[k] = s.aff_nmax[k - 1] / 2 + (uint32_t)(nbuckets / 2) + 1;
-        if (rounds) {
-            const size_t elem = g2 ? 64 : 32, aff = 2 * elem;
-            if (with_sort) {
-                std::vector<uint32_t*> offs(MSM_AFF_MAX_ROUNDS + 1, nullptr);
-                offs[0] = s.offsets;
-                for (int k = 1; k <= rounds; k++) {
-                    CUDA_CHECK(cudaMalloc(&s.aff_off[k], ((size_t)nbuckets + 1) * 4));
-                    CUDA_CHECK(cudaMalloc(&s.aff_src[k], ((size_t)s.aff_nmax[k] + 1) * 4));
-                    offs[k] = s.aff_off[k];
-                }
-                s.aff_off[0] = s.offsets;
-                CUDA_CHECK(cudaMalloc(&s.aff_off_dev, (MSM_AFF_MAX_ROUNDS + 1) * sizeof(uint32_t*)));
-                CUDA_CHECK(cudaMemcpy(s.aff_off_dev, offs.data(), (MSM_AFF_MAX_ROUNDS + 1) * sizeof(uint32_t*), cudaMemcpyHostToDevice));
-            }
-            CUDA_CHECK(cudaMalloc(&s.aff_list[0], ((size_t)s.aff_nmax[1] + 1) * aff));
-            if (rounds > 1) CUDA_CHECK(cudaMalloc(&s.aff_list[1], ((size_t)s.aff_nmax[2] + 1) * aff));
-            const size_t threads1 = ((size_t)s.aff_nmax[1] + MSM_AFF_M - 1) / MSM_AFF_M + 128;
-            CUDA_CHECK(cudaMalloc(&s.aff_pref, ((size_t)s.aff_nmax[1] + 1) * elem));
-            CUDA_CHECK(cudaMalloc(&s.aff_totals, threads1 * elem));
-            CUDA_CHECK(cudaMalloc(&s.aff_tscratch, threads1 * elem));
-        }
-    }
-    if (env_u32("B2G_MSM_TAIL_PRIORITY", 1) == 1) {
-        // the tail kernels occupy a handful of CTAs for a long dependent chain: let them be dispatched ahead of the
-        // thousands of pending accumulation CTAs of the other queries
-        int least = 0, greatest = 0;
-        CUDA_CHECK(cudaDeviceGetStreamPriorityRange(&least, &greatest));
-        CUDA_CHECK(cudaStreamCreateWithPriority(&s.tail, cudaStreamNonBlocking, greatest));
-        CUDA_CHECK(cudaEventCreateWithFlags(&s.ev_acc, cudaEventDisableTiming));
-        CUDA_CHECK(cudaEventCreateWithFlags(&s.ev_tail, cudaEventDisableTiming));
-    }
+    // the tail kernels occupy a handful of CTAs for a long dependent chain: let them be dispatched ahead of the
+    // thousands of pending accumulation CTAs of the other queries
+    int least = 0, greatest = 0;
+    CUDA_CHECK(cudaDeviceGetStreamPriorityRange(&least, &greatest));
+    CUDA_CHECK(cudaStreamCreateWithPriority(&s.tail, cudaStreamNonBlocking, greatest));
+    CUDA_CHECK(cudaEventCreateWithFlags(&s.ev_acc, cudaEventDisableTiming));
+    CUDA_CHECK(cudaEventCreateWithFlags(&s.ev_tail, cudaEventDisableTiming));
 }
 
 void msm_scratch_free(MsmScratch& s) {
     void* ptrs[] = {s.counts, s.offsets, s.cursor, s.entries, s.big_list, s.big_count, s.frag_first, s.frag_last,
-                    s.buckets, s.partials, s.result_owned ? s.result : nullptr, s.scalars_canon,
-                    s.aff_list[0], s.aff_list[1], s.aff_pref, s.aff_totals, s.aff_tscratch, s.aff_off_dev};
+                    s.buckets, s.partials, s.result_owned ? s.result : nullptr, s.scalars_canon};
     for (void* p : ptrs) if (p) cudaFree(p);
-    for (int k = 1; k <= MSM_AFF_MAX_ROUNDS; k++) { if (s.aff_off[k]) cudaFree(s.aff_off[k]); if (s.aff_src[k]) cudaFree(s.aff_src[k]); }
+    // a scratch that was never allocated, or whose allocation failed before the stream was made, has no tail stream
     if (s.tail) { cudaStreamDestroy(s.tail); cudaEventDestroy(s.ev_acc); cudaEventDestroy(s.ev_tail); }
     s = MsmScratch();
 }
@@ -797,31 +575,22 @@ void msm_sort(const MsmPlan& plan, MsmScratch& s, const fe* scalars_dev, uint32_
     // table rows are indexed w * plan.n + i (the table was built over plan.n bases, n may be shorter)
     msm_scatter_kernel<<<pair_grid, SORT_CTA, 0, st>>>(s.scalars_canon, n, plan.n, plan.c, plan.nwin, plan.nbuckets, s.offsets, s.cursor, s.entries);
     g_launch_count += 4;
-    // level structure of the batched-affine pre-reduction (shared by every query accumulated against this sort)
-    s.aff_rounds = s.aff_off_dev ? s.aff_cap_rounds : 0;
-    if (s.aff_rounds) {
-        msm_aff_levels_kernel<<<1, 1024, 0, st>>>(nb, s.aff_rounds, s.aff_off_dev);
-        for (int k = 1; k <= s.aff_rounds; k++) {
-            const unsigned blocks = (unsigned)std::min<uint64_t>(((uint64_t)s.aff_nmax[k] + 255) / 256, 1u << 20);
-            msm_aff_src_kernel<<<blocks, 256, 0, st>>>(s.aff_off[k - 1], s.aff_off[k], nb, s.aff_src[k]);
-        }
-        g_launch_count += 1 + s.aff_rounds;
-    }
     CUDA_CHECK(cudaGetLastError());
 }
 
 // one accumulation launch over `nruns` runs: one thread per run for G1, one lane pair per run for G2 (64 runs per CTA)
 template <class C, class F>
 static void launch_accumulate(const void* table, const uint32_t* entries, const uint32_t* offsets, uint32_t nb, uint32_t chunk, uint32_t nruns,
-                              const MsmScratch& s, bool bulk, cudaStream_t st) {
+                              const MsmScratch& s, cudaStream_t st) {
     constexpr bool g2 = std::is_same<F, Fq2>::value;
     constexpr uint32_t runs_per_cta = g2 ? 64u : 128u;
-    const uint32_t slab_words = bulk && (size_t)chunk * runs_per_cta * 4 <= MSM_SLAB_MAX_BYTES ? chunk * runs_per_cta : 0u;
     const unsigned blocks = (unsigned)(((uint64_t)nruns + runs_per_cta - 1) / runs_per_cta);
-    if constexpr (g2)
-        msm_accumulate_g2_kernel<<<blocks, 128, (size_t)slab_words * 4, st>>>(table, entries, offsets, nb, chunk, s.buckets, s.frag_first, s.frag_last, slab_words);
-    else
+    if constexpr (g2) {
+        msm_accumulate_g2_kernel<<<blocks, 128, 0, st>>>(table, entries, offsets, nb, chunk, s.buckets, s.frag_first, s.frag_last);
+    } else {
+        const uint32_t slab_words = (size_t)chunk * runs_per_cta * 4 <= MSM_SLAB_MAX_BYTES ? chunk * runs_per_cta : 0u;
         msm_accumulate_kernel<C, F><<<blocks, 128, (size_t)slab_words * 4, st>>>(table, entries, offsets, nb, chunk, s.buckets, s.frag_first, s.frag_last, slab_words);
+    }
 }
 
 template <class C, class F>
@@ -833,42 +602,15 @@ static void msm_accumulate_t(const MsmPlan& plan, const MsmScratch& sorted, MsmS
     if (n == 0 || plan.table == nullptr) { CUDA_CHECK(cudaMemset2DAsync(s.result, rstride, 0, ptb, count, st)); return; }
     if (plan.nbuckets > s.cap_buckets || n > s.cap_n || plan.nwin > s.cap_nwin || count > s.cap_count) throw_error(B2G_E_SHAPE, "msm: accumulate scratch too small");
     const uint32_t nb = plan.nbuckets * count, chunk = s.chunk;   // every proof's buckets in one range: runs cross proofs freely
+    const uint32_t* offsets = sorted.offsets;
     CUDA_CHECK(cudaMemsetAsync(s.big_count, 0, 4, st));
     const uint64_t nent = (uint64_t)n * plan.nwin * count;
     const uint32_t nthreads = (uint32_t)((nent + chunk - 1) / chunk);
     if (s.prof0) CUDA_CHECK(cudaEventRecord(s.prof0, st));
-    int rounds = sorted.aff_rounds < s.aff_cap_rounds ? sorted.aff_rounds : s.aff_cap_rounds;
-    if (rounds && (sorted.aff_nmax[1] > s.aff_nmax[1] || !s.aff_list[0])) rounds = 0;
-    const uint32_t* offsets = sorted.offsets;
-    if (rounds) {
-        // (4a) R levels of pairwise affine additions inside the buckets; three kernels per level
-        const void* prev = nullptr;
-        for (int k = 1; k <= rounds; k++) {
-            const uint32_t nk = sorted.aff_nmax[k];
-            const unsigned blocks = (unsigned)(((uint64_t)nk + (uint64_t)MSM_AFF_M * 128 - 1) / ((uint64_t)MSM_AFF_M * 128));
-            const uint32_t stride = blocks * 128u, U = (stride + MSM_AFF_S - 1) / MSM_AFF_S;
-            void* out = s.aff_list[(k - 1) & 1];
-            if (k == 1) {
-                msm_aff_prod_kernel<C, F, true><<<blocks, 128, 0, st>>>(plan.table, sorted.entries, nullptr, sorted.aff_src[k], sorted.aff_off[k], nb, s.aff_pref, s.aff_totals);
-                msm_aff_invert_kernel<F><<<(U + 63) / 64, 64, 0, st>>>(s.aff_totals, s.aff_tscratch, stride, U);
-                msm_aff_apply_kernel<C, F, true><<<blocks, 128, 0, st>>>(plan.table, sorted.entries, nullptr, sorted.aff_src[k], sorted.aff_off[k], nb, s.aff_pref, s.aff_totals, out);
-            } else {
-                msm_aff_prod_kernel<C, F, false><<<blocks, 128, 0, st>>>(nullptr, nullptr, prev, sorted.aff_src[k], sorted.aff_off[k], nb, s.aff_pref, s.aff_totals);
-                msm_aff_invert_kernel<F><<<(U + 63) / 64, 64, 0, st>>>(s.aff_totals, s.aff_tscratch, stride, U);
-                msm_aff_apply_kernel<C, F, false><<<blocks, 128, 0, st>>>(nullptr, nullptr, prev, sorted.aff_src[k], sorted.aff_off[k], nb, s.aff_pref, s.aff_totals, out);
-            }
-            prev = out;
-        }
-        g_launch_count += 3 * rounds;
-        offsets = sorted.aff_off[rounds];
-        const uint32_t nthreads_r = (uint32_t)(((uint64_t)sorted.aff_nmax[rounds] + chunk - 1) / chunk);
-        launch_accumulate<C, F>(prev, nullptr, offsets, nb, chunk, nthreads_r, s, false, st);
-    } else {
-        launch_accumulate<C, F>(plan.table, sorted.entries, sorted.offsets, nb, chunk, nthreads, s, s.bulk, st);
-    }
+    launch_accumulate<C, F>(plan.table, sorted.entries, offsets, nb, chunk, nthreads, s, st);
     if (s.prof1) CUDA_CHECK(cudaEventRecord(s.prof1, st));
     cudaStream_t main_st = st;
-    if (s.tail) { CUDA_CHECK(cudaEventRecord(s.ev_acc, st)); CUDA_CHECK(cudaStreamWaitEvent(s.tail, s.ev_acc, 0)); st = s.tail; }
+    CUDA_CHECK(cudaEventRecord(s.ev_acc, st)); CUDA_CHECK(cudaStreamWaitEvent(s.tail, s.ev_acc, 0)); st = s.tail;
     msm_fold_kernel<C, F><<<(nb + 127) / 128, 128, 0, st>>>(offsets, nb, chunk, s.buckets, s.frag_first, s.frag_last, s.big_list, s.big_count);
     constexpr int NT = TailThreads<F>::N;
     const size_t sh = (size_t)NT * ptb;
@@ -878,7 +620,7 @@ static void msm_accumulate_t(const MsmPlan& plan, const MsmScratch& sorted, MsmS
     const uint32_t npart = (nred + NT - 1) / NT;                 // per proof
     msm_reduce_kernel<C, F><<<dim3(npart, count), NT, sh, st>>>(s.buckets, nb1, rchunk, s.partials);
     msm_sum_kernel<C, F><<<count, NT, sh, st>>>(s.partials, npart, s.result, rstride);
-    if (s.tail) { CUDA_CHECK(cudaEventRecord(s.ev_tail, s.tail)); CUDA_CHECK(cudaStreamWaitEvent(main_st, s.ev_tail, 0)); }
+    CUDA_CHECK(cudaEventRecord(s.ev_tail, s.tail)); CUDA_CHECK(cudaStreamWaitEvent(main_st, s.ev_tail, 0));
     g_launch_count += 5;
     CUDA_CHECK(cudaGetLastError());
 }
@@ -896,12 +638,11 @@ void msm_run(const MsmPlan& plan, MsmScratch& s, const fe* scalars_dev, uint32_t
     msm_accumulate(plan, s, s, st);
 }
 
-// A full entry slab is 48 KiB (G1 128 runs x 96 entries, G2 64 runs x 192) on top of the accumulation kernels' static mbarrier
-// word, which is more than the default dynamic limit (48 KiB minus the static size): without the opt-in such launches fail
-// with "invalid argument".  The tail kernels use < 48 KiB of dynamic shared memory.
+// A full entry slab is 48 KiB (128 runs x 96 entries) on top of the G1 accumulation kernel's static mbarrier word, which is
+// more than the default dynamic limit (48 KiB minus the static size): without the opt-in such launches fail with "invalid
+// argument".  The tail kernels use < 48 KiB of dynamic shared memory.
 void msm_init_kernels() {
     CUDA_CHECK(cudaFuncSetAttribute(msm_accumulate_kernel<G1, Fq>, cudaFuncAttributeMaxDynamicSharedMemorySize, MSM_SLAB_MAX_BYTES));
-    CUDA_CHECK(cudaFuncSetAttribute(msm_accumulate_g2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, MSM_SLAB_MAX_BYTES));
 }
 
 }  // namespace b2g

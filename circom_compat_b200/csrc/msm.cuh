@@ -31,17 +31,6 @@ struct MsmPlan {                         // static per query
     bool g2 = false;
 };
 
-// ---- batched-affine pre-reduction (msm.cu section 4a) --------------------------------------------------------------
-// Before the XYZZ accumulation, the bucket-sorted list is halved R times by pairwise AFFINE additions inside each bucket
-// (level k list: bucket b holds ceil(cnt_{k-1}[b] / 2) points).  An affine addition costs 1 inversion + 2M + 1S; the
-// inversions of a whole level are shared by Montgomery's trick across the grid (three kernels per level: prefix products,
-// batch inversion of the per-thread totals, back-substitution), i.e. 5M + 1S per addition instead of the 8M + 2S of an XYZZ
-// mixed addition.  The level structure depends only on the sorted scalars, so it lives in the sorting scratch and is shared
-// by every query that pairs the same scalars (L, A, B1, B2).
-constexpr int MSM_AFF_MAX_ROUNDS = 6;
-constexpr int MSM_AFF_M = 16;            // additions per thread and level (interleaved: thread t owns slots t + i * stride)
-constexpr int MSM_AFF_S = 64;            // thread totals per inversion thread
-
 // Batched MSMs (b2g_prove_many): `count` scalar vectors against the same table are sorted into ONE list whose bucket key is
 // j * nbuckets + b for proof j, so accumulation and fold run unchanged over count * nbuckets buckets.  Table rows, and so the
 // entry word, do not depend on j.  The weighted reduction restarts its bucket weights per proof (grid.y = proof) and proof
@@ -55,19 +44,9 @@ struct MsmScratch {                      // one per in-flight MSM
     void *frag_first = nullptr, *frag_last = nullptr, *buckets = nullptr, *partials = nullptr, *result = nullptr;
     fe* scalars_canon = nullptr;         // n canonical scalars (filled by the digit pass)
     bool g2 = false, result_owned = false;
-    bool bulk = false;                   // stage each CTA's slab of the entry list by one bulk copy (B2G_ACC_BULK)
     cudaEvent_t prof0 = nullptr, prof1 = nullptr;   // optional: bracket the accumulate kernel (b2g_bench_msm)
     cudaStream_t tail = nullptr;                     // high-priority stream for the low-parallelism fold / weighted-sum kernels
     cudaEvent_t ev_acc = nullptr, ev_tail = nullptr;
-    // batched-affine pre-reduction.  Sorting scratch: level offsets / source maps; accumulating scratch: point lists.
-    int aff_rounds = 0;                              // levels planned by the last msm_sort (0 = straight to XYZZ)
-    int aff_cap_rounds = 0;                          // levels the buffers were sized for
-    uint32_t aff_nmax[MSM_AFF_MAX_ROUNDS + 1] = {};  // host-side upper bounds of the level list lengths
-    uint32_t* aff_off[MSM_AFF_MAX_ROUNDS + 1] = {};  // [k] = offsets of level k (nb + 1); [0] aliases `offsets`
-    uint32_t** aff_off_dev = nullptr;                // device copy of aff_off[] for the level-planning kernel
-    uint32_t* aff_src[MSM_AFF_MAX_ROUNDS + 1] = {};  // [k][q] = first input slot in level k-1 | (pair << 31)
-    void* aff_list[2] = {nullptr, nullptr};          // ping-pong affine point lists (levels 1, 3, 5 / 2, 4, 6)
-    void *aff_pref = nullptr, *aff_totals = nullptr, *aff_tscratch = nullptr;
 };
 
 // Window size by base count.  Larger windows than the textbook log2(n) - 3 pay off for small keys because the table removes

@@ -42,7 +42,7 @@ constexpr uint32_t MAX_BATCH = 65535;                 // proofs per b2g_prove_ma
 using namespace b2g;
 
 struct b2g_ctx {
-    int device = 0, shard_rank = 0, shard_count = 1, stream_priority = 0;
+    int device = 0, shard_rank = 0, shard_count = 1;
     cudaStream_t st[NQ] = {}, st_glue = nullptr;
     cudaEvent_t ev_w = nullptr, ev_sort = nullptr, ev_pre = nullptr, ev_fork = nullptr, ev_done[NQ] = {}, ev_t[20] = {};
     MsmScratch scratch[NQ];
@@ -627,13 +627,8 @@ static void check_shapes(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat) {
 // bucket reduction, and for A / B1 the scalar multiplication by s / r; B2's tail is shorter, L's the shortest).  The chains with
 // the longest tails go first so that their tails run under the accumulations that follow: A, B1, B2, L.  On one GPU at 2^20 the
 // accumulations are long enough to hide every tail; in one shard of a many-way sharded proof they are short and the order
-// decides which tail sticks out.  B2G_MSM_ORDER=b2 restores B2-first.
-static const int WITNESS_ORDER_TAILS[4] = {Q_A, Q_B1, Q_B2, Q_L};
-static const int WITNESS_ORDER_B2[4] = {Q_B2, Q_A, Q_B1, Q_L};
-static const int* witness_order() {
-    const char* e = getenv("B2G_MSM_ORDER");
-    return (e && e[0] == 'b' && e[1] == '2') ? WITNESS_ORDER_B2 : WITNESS_ORDER_TAILS;
-}
+// decides which tail sticks out.
+static const int WITNESS_ORDER[4] = {Q_A, Q_B1, Q_B2, Q_L};
 
 // scale: also compute s*msm_A and r*msm_B1 (d_rs must hold r, s) on those MSMs' own streams, right behind them
 static unsigned long long p2p_timeout_ns() {
@@ -644,7 +639,7 @@ static unsigned long long p2p_timeout_ns() {
 
 static bool map_is_split(const b2g_ctx* ctx, const b2g_mat* mat) {
     return ctx->shard_count >= MAP_RANKS && ctx->peers_imported == ctx->shard_count && mat->reduction == B2G_REDUCTION_CIRCOM &&
-           ctx->eval_common >= mat->n && getenv("B2G_NO_SPLIT_MAP") == nullptr;
+           ctx->eval_common >= mat->n;
 }
 
 // witness map of a sharded proof with the three transforms on ranks 0, 1, 2 (kernels above); fills d_h[lo, lo + cnt) only
@@ -683,9 +678,7 @@ static void launch_msms(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, bool timed, bool
         msm_sort(pk->plan[Q_B1], ctx->scratch[Q_B1], ctx->d_wb, pk->b_compact, true, sb, count, pk->b_compact);
         CUDA_CHECK(cudaEventRecord(ctx->ev_sortb, sb));
     }
-    const int* order = witness_order();
-    for (int oi = 0; oi < 4; oi++) {
-        const int q = order[oi];
+    for (int q : WITNESS_ORDER) {
         const bool on_b = bsparse && (q == Q_B1 || q == Q_B2);
         if (on_b) { if (q != Q_B1) CUDA_CHECK(cudaStreamWaitEvent(ctx->st[q], ctx->ev_sortb, 0)); }
         else if (q != Q_L) CUDA_CHECK(cudaStreamWaitEvent(ctx->st[q], ctx->ev_sort, 0));
@@ -841,26 +834,16 @@ int b2g_ctx_create(int device, int shard_rank, int shard_count, b2g_ctx** out) {
         DevGuard g(device);
         b2g_ctx* ctx = new b2g_ctx();
         ctx->device = device; ctx->shard_rank = shard_rank; ctx->shard_count = shard_count;
-        // Stream priority of this context's proof streams (the MSM tail kernels always run at the highest).  Spreading
-        // successive contexts over different priorities to pipeline concurrent proofs is opt-in: B2G_CTX_PRIORITY_SPREAD=1.
-        int prio = 0;
-        {
-            static std::atomic<unsigned> ctx_seq[64];
-            int least = 0, greatest = 0;
-            CUDA_CHECK(cudaDeviceGetStreamPriorityRange(&least, &greatest));
-            const char* sp = getenv("B2G_CTX_PRIORITY_SPREAD");
-            const int levels = least - greatest - 1;                        // levels below the tail kernels' priority
-            if (sp && *sp == '1' && levels >= 2 && shard_count == 1) prio = greatest + 1 + (int)(ctx_seq[device & 63]++ % (unsigned)(levels < 3 ? levels : 3));
-            else prio = least;
-        }
-        ctx->stream_priority = prio;
-        for (int i = 0; i < NQ; i++) { CUDA_CHECK(cudaStreamCreateWithPriority(&ctx->st[i], cudaStreamNonBlocking, prio)); CUDA_CHECK(cudaEventCreateWithFlags(&ctx->ev_done[i], cudaEventDisableTiming)); }
+        // the proof streams run at the least priority, below the MSM tail kernels' streams (msm_scratch_alloc)
+        int least = 0, greatest = 0;
+        CUDA_CHECK(cudaDeviceGetStreamPriorityRange(&least, &greatest));
+        for (int i = 0; i < NQ; i++) { CUDA_CHECK(cudaStreamCreateWithPriority(&ctx->st[i], cudaStreamNonBlocking, least)); CUDA_CHECK(cudaEventCreateWithFlags(&ctx->ev_done[i], cudaEventDisableTiming)); }
         CUDA_CHECK(cudaEventCreateWithFlags(&ctx->ev_w, cudaEventDisableTiming));
         CUDA_CHECK(cudaEventCreateWithFlags(&ctx->ev_sort, cudaEventDisableTiming));
         CUDA_CHECK(cudaEventCreateWithFlags(&ctx->ev_pre, cudaEventDisableTiming));
         CUDA_CHECK(cudaEventCreateWithFlags(&ctx->ev_fork, cudaEventDisableTiming));
         CUDA_CHECK(cudaEventCreateWithFlags(&ctx->ev_sortb, cudaEventDisableTiming));
-        CUDA_CHECK(cudaStreamCreateWithPriority(&ctx->st_glue, cudaStreamNonBlocking, prio));
+        CUDA_CHECK(cudaStreamCreateWithPriority(&ctx->st_glue, cudaStreamNonBlocking, least));
         for (auto& e : ctx->ev_t) CUDA_CHECK(cudaEventCreate(&e));
         CUDA_CHECK(cudaMalloc(&ctx->d_partial, REC_BYTES));
         CUDA_CHECK(cudaMemset(ctx->d_partial, 0, REC_BYTES));
@@ -876,9 +859,8 @@ int b2g_ctx_create(int device, int shard_rank, int shard_count, b2g_ctx** out) {
         // L2 -> DRAM fetch granularity: a 64-byte gather from the fixed-base tables needs only 64 B, so the hint asks for 64 B
         // instead of the device default (128 B); it cut the G1 accumulation's DRAM traffic on the previous target GPU.  On an
         // H100 (700 W, 2^20 chain) it is neutral: 42.2 / 41.8 proofs/s with 64 B vs 41.8 with 128 B, G1 accumulation 2.66-2.68 vs
-        // 2.68 ms (DRAM traffic not measured).  Device-wide hint; B2G_L2_FETCH=128 restores the default, 32 / 64 / 128 accepted.
-        { const char* g = getenv("B2G_L2_FETCH"); const size_t gran = g && *g ? (size_t)strtol(g, nullptr, 10) : 64;
-          if (gran == 32 || gran == 64 || gran == 128) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, gran); cudaGetLastError(); }
+        // 2.68 ms (DRAM traffic not measured).  Device-wide hint: a failure to set it is ignored.
+        cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, 64); cudaGetLastError();
         CUDA_CHECK(cudaMalloc(&ctx->d_peer_ptrs, 64 * sizeof(uint8_t*)));
         msm_init_kernels();
         *out = ctx;

@@ -126,9 +126,9 @@ def entry_count(k: int, c: int) -> int:
 
 
 def partial_slab_prefix(sc, c: int) -> int:
-    """Length of the longest prefix of the scalars whose entry count is not a multiple of 4.  A CTA's slab of the entry
-    list is 128 (G1) or 64 (G2) runs of `chunk` entries, a multiple of 4, so the last CTA's slab is then partial and not a
-    whole number of 16-byte units."""
+    """Length of the longest prefix of the scalars whose entry count is not a multiple of 4.  A G1 CTA's slab of the
+    entry list is 128 runs of `chunk` entries, a multiple of 4, so the last CTA's slab is then partial and not a whole
+    number of 16-byte units."""
     total = sum(entry_count(k, c) for k in sc)
     for m in range(len(sc), 0, -1):
         if total % 4:

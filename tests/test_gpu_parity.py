@@ -258,17 +258,15 @@ def test_msm_small_chunks_exercise_fragments(ctx, monkeypatch):
     for chunk in ('1', '2', '3', '7'):
         monkeypatch.setenv('B2G_MSM_CHUNK', chunk)
         assert np.array_equal(ctx.msm_g1(bases, scl), exp), chunk
-    # the bulk-copied entry slab (B2G_ACC_BULK) on and off around its size limit (128 runs x 96 entries = 48 KB per CTA); the
-    # entry count is not a multiple of 4, so the last CTA's slab is partial and its copy is rounded up
+    # the bulk-copied entry slab around its size limit (128 runs x 96 entries = 48 KB per CTA): up to 96 entries per run it
+    # is staged, from 97 the runs read the entry list directly; the entry count is not a multiple of 4, so the last CTA's
+    # slab is partial and its copy is rounded up
     monkeypatch.setenv('B2G_MSM_C', '11')
     m = md.partial_slab_prefix(sc, 11)
     exp_m = c.msm_g1(bases[:m], scl[:m])
     for chunk in ('1', '64', '96', '97'):
         monkeypatch.setenv('B2G_MSM_CHUNK', chunk)
-        for bulk in ('0', '1'):
-            monkeypatch.setenv('B2G_ACC_BULK', bulk)
-            assert np.array_equal(ctx.msm_g1(bases[:m], scl[:m]), exp_m), (chunk, bulk)
-    monkeypatch.delenv('B2G_ACC_BULK')
+        assert np.array_equal(ctx.msm_g1(bases[:m], scl[:m]), exp_m), chunk
     # the weighted bucket sum with every per-thread bucket count, at two window sizes
     monkeypatch.delenv('B2G_MSM_CHUNK')
     for cw in ('8', '13'):
@@ -291,38 +289,9 @@ def test_msm_small_chunks_exercise_fragments(ctx, monkeypatch):
         assert np.array_equal(ctx.msm_g1(b4, s4), c.msm_g1(b4, s4)), v
 
 
-@pytest.mark.parametrize('rounds', ['1', '2', '3', '6'])
-def test_msm_batched_affine_levels(ctx, monkeypatch, rounds):
-    """The batched-affine pre-reduction (msm.cu 4a: R levels of pairwise affine additions inside the buckets, inversions shared
-    by Montgomery's trick) forced on at small sizes, G1 and G2, against oracle/cref.c: uniform and circom-like scalars (one
-    300-entry bucket next to near-empty ones), more levels than the largest bucket can be halved, points at infinity in the
-    table, and tiny chunks of the final XYZZ stage."""
-    monkeypatch.setenv('B2G_MSM_AFFINE_ROUNDS', rounds)
-    rng = random.Random(1000 + int(rounds))
-    for n, dist in ((1, 'uniform'), (2, 'ones'), (37, 'uniform'), (3000, 'circomlike'), (20000, 'uniform'), (20000, 'same')):
-        ks, sc = _msm_case(rng, n, dist)
-        bases = c.fixed_base_g1(c.ints_to_limbs(ks))
-        if n > 40:
-            bases[5] = 0; bases[9] = bases[8]; sc[8] = 5; sc[9] = o.R_MOD - 5; sc[0] = 0; sc[1] = 1; sc[2] = o.R_MOD - 1
-        scl = c.ints_to_limbs(sc)
-        assert np.array_equal(ctx.msm_g1(bases, scl), c.msm_g1(bases, scl)), (n, dist)
-    for n, dist in ((3, 'ones'), (700, 'circomlike'), (6000, 'uniform')):
-        ks, sc = _msm_case(rng, n, dist)
-        bases = c.fixed_base_g2(c.ints_to_limbs(ks))
-        if n > 40:
-            bases[5] = 0; bases[9] = bases[8]; sc[8] = 5; sc[9] = o.R_MOD - 5
-        scl = c.ints_to_limbs(sc)
-        assert np.array_equal(ctx.msm_g2(bases, scl), c.msm_g2(bases, scl)), (n, dist)
-    monkeypatch.setenv('B2G_MSM_CHUNK', '3')
-    ks, sc = _msm_case(rng, 5000, 'circomlike')
-    bases = c.fixed_base_g1(c.ints_to_limbs(ks)); scl = c.ints_to_limbs(sc)
-    assert np.array_equal(ctx.msm_g1(bases, scl), c.msm_g1(bases, scl))
-
-
-def test_msm_batched_affine_exceptional_pairs(ctx, monkeypatch):
-    """Buckets that hold exactly two points make the pairing deterministic: P + P (the doubling branch of the affine
-    addition), P + (-P) (sum at infinity, denominator replaced by one) and P + infinity."""
-    monkeypatch.setenv('B2G_MSM_AFFINE_ROUNDS', '2')
+def test_msm_g1_two_entry_buckets(ctx):
+    """Buckets that hold exactly two points make the XYZZ mixed addition's exceptional cases deterministic: P + P (the
+    doubling branch), P + (-P) (sum at infinity), P + infinity and infinity + infinity; then four equal points."""
     rng = random.Random(4242)
     k = rng.randrange(1, o.R_MOD)
     P = c.fixed_base_g1(c.ints_to_limbs([k]))[0]
@@ -333,13 +302,6 @@ def test_msm_batched_affine_exceptional_pairs(ctx, monkeypatch):
         for pair in ((P, P), (P, Pn), (P, inf), (inf, P), (inf, inf)):
             bases = np.stack(pair)
             assert np.array_equal(ctx.msm_g1(bases, scl), c.msm_g1(bases, scl)), sv
-    Q = c.fixed_base_g2(c.ints_to_limbs([k]))[0]
-    Qn = c.fixed_base_g2(c.ints_to_limbs([o.R_MOD - k]))[0]
-    scl = c.ints_to_limbs([7, 7])
-    for pair in ((Q, Q), (Q, Qn), (Q, np.zeros_like(Q))):
-        bases = np.stack(pair)
-        assert np.array_equal(ctx.msm_g2(bases, scl), c.msm_g2(bases, scl))
-    # four equal points: level 1 doubles twice, level 2 doubles the doubles
     bases = np.stack((P, P, P, P)); scl = c.ints_to_limbs([3, 3, 3, 3])
     assert np.array_equal(ctx.msm_g1(bases, scl), c.msm_g1(bases, scl))
 

@@ -103,17 +103,14 @@ def test_msm_g2_small_chunks_exercise_fragments(ctx, monkeypatch):
     b_f = c.fixed_base_g2(c.ints_to_limbs([rng.randrange(1, o.R_MOD) for _ in range(len(sc_f))]))
     s_f = c.ints_to_limbs(sc_f)
     assert np.array_equal(ctx.msm_g2(b_f, s_f), c.msm_g2(b_f, s_f))
-    # the bulk-copied slab in the lane-pair kernel (64 runs per CTA, at most 192 entries per run) on and off around that
-    # limit; the entry count is not a multiple of 4, so the last CTA's slab is partial
+    # run lengths from one entry to 193 on a prefix whose entry count is not a multiple of 4: at 64 and 192 the last run is
+    # cut short
     monkeypatch.setenv('B2G_MSM_C', '11')
     m = md.partial_slab_prefix(sc, 11)
     exp_m = c.msm_g2(bases[:m], scl[:m])
     for chunk in ('1', '3', '64', '192', '193'):
         monkeypatch.setenv('B2G_MSM_CHUNK_G2', chunk)
-        for bulk in ('0', '1'):
-            monkeypatch.setenv('B2G_ACC_BULK', bulk)
-            assert np.array_equal(ctx.msm_g2(bases[:m], scl[:m]), exp_m), (chunk, bulk)
-    monkeypatch.delenv('B2G_ACC_BULK')
+        assert np.array_equal(ctx.msm_g2(bases[:m], scl[:m]), exp_m), chunk
     monkeypatch.delenv('B2G_MSM_CHUNK_G2')
     # the weighted bucket sum with one and with all buckets per thread
     for cw in ('8', '13'):

@@ -152,11 +152,10 @@ def chain12(ctx):
     {'B2G_MSM_C': '13', 'B2G_MSM_REDUCE_CHUNK': '1000'},
     {'B2G_MSM_CHUNK': '1'},
     {'B2G_MSM_CHUNK': '97', 'B2G_MSM_CHUNK_G2': '193'},
-    {'B2G_MSM_AFFINE_ROUNDS': '2'},
 ], ids=lambda e: ','.join(f'{k[8:]}={v}' for k, v in e.items()))
 def test_bucket_layout_variants(monkeypatch, chain12, env):
-    """window sizes, reduce chunks, run lengths whose runs straddle proof boundaries and the batched-affine levels over
-    count * nb buckets: a fresh context (and key tables) built under each setting"""
+    """window sizes, reduce chunks and run lengths whose runs straddle proof boundaries over count * nb buckets: a fresh
+    context (and key tables) built under each setting"""
     from circom_compat_b200 import Context, release
     pk, cm, ws, rs, expect = chain12
     for k, v in env.items():
