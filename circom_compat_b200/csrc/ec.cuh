@@ -124,6 +124,24 @@ struct Curve {
         return acc;
     }
 
+    // k * p for an affine p and a short scalar of `words` x u32 (little-endian): double-and-add over every bit with mixed
+    // additions (the batch verifier's 128-bit weights, the G2 subgroup check's 63-bit x)
+    static __device__ __noinline__ Pt mul_affine(const Aff& p, const uint32_t* k, int words) {
+        Pt acc = infinity();
+        #pragma unroll 1
+        for (int i = 32 * words - 1; i >= 0; i--) {
+            acc = dbl(acc);
+            if ((k[i >> 5] >> (i & 31)) & 1u) madd(acc, p);
+        }
+        return acc;
+    }
+
+    // the same point: X1 ZZ2 == X2 ZZ1 and Y1 ZZZ2 == Y2 ZZZ1, or both at infinity
+    static __device__ __forceinline__ bool pt_eq(const Pt& a, const Pt& b) {
+        if (is_inf(a) || is_inf(b)) return is_inf(a) && is_inf(b);
+        return F::eq(F::mul(a.x, b.zz), F::mul(b.x, a.zz)) && F::eq(F::mul(a.y, b.zzz), F::mul(b.y, a.zzz));
+    }
+
     // XYZZ -> affine (Montgomery); infinity -> zeros.  One inversion: iz = 1/ZZZ, 1/ZZ = ZZ^2 * iz^2.
     static __device__ __noinline__ Aff to_affine(const Pt& p) {
         Aff r;

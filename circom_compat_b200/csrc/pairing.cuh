@@ -201,6 +201,19 @@ struct Fq12 {
         }
         r = acc;
     }
+    // f^k for a cyclotomic f and a canonical 256-bit k (8 x u32): square-and-multiply from the top set bit
+    static __device__ __noinline__ void cyclotomic_exp(fe12& r, const fe12& f, const uint32_t* k) {
+        int top = 255;
+        while (top >= 0 && !((k[top >> 5] >> (top & 31)) & 1u)) top--;
+        if (top < 0) { r = one(); return; }
+        fe12 acc = f;
+        #pragma unroll 1
+        for (int i = top - 1; i >= 0; i--) {
+            cyclotomic_sqr(acc, acc);
+            if ((k[i >> 5] >> (i & 31)) & 1u) mul(acc, acc, f);
+        }
+        r = acc;
+    }
 
     // f^((p^12 - 1) / r).  Hard part: with g cyclotomic and y0 = g^(p + p^2 + p^3), y1 = conj(g), y2 = (g^(x^2))^(p^2),
     // y3 = conj((g^x)^p), y4 = conj(g^x (g^(x^2))^p), y5 = conj(g^(x^2)), y6 = conj(g^(x^3) (g^(x^3))^p), the result is
@@ -285,6 +298,32 @@ __device__ __forceinline__ void twist_frobenius(fe2& x1, fe2& y1, fe2& x2, fe2& 
     y1 = Fq2::mul(fq2_conj(qy), frob_coeff(1, 3));
     x2 = Fq2::mul(qx, frob_coeff(2, 2));
     y2 = Fq2::neg(Fq2::mul(qy, frob_coeff(2, 3)));
+}
+
+// psi, the first map of twist_frobenius, on an XYZZ point: x = X / ZZ gives conj(x) FROB = conj(X) FROB / conj(ZZ)
+__device__ __forceinline__ G2::Pt g2_psi(const G2::Pt& q) {
+    G2::Pt r;
+    r.x = Fq2::mul(fq2_conj(q.x), frob_coeff(1, 2));
+    r.y = Fq2::mul(fq2_conj(q.y), frob_coeff(1, 3));
+    r.zz = fq2_conj(q.zz);
+    r.zzz = fq2_conj(q.zzz);
+    return r;
+}
+
+// Q in G2, the order-r subgroup of the twist, for Q on the twist (infinity included):
+//     [x + 1] Q + psi([x] Q) + psi^2([x] Q) == psi^3([2x] Q)
+// (El Housni, Guillevic, Piellard, "Co-factor clearing and subgroup membership testing on pairing-friendly curves"), one
+// 63-bit product instead of the 254-bit [r] Q
+__device__ __noinline__ bool g2_in_subgroup(const G2::Aff& q) {
+    if (G2::aff_is_inf(q)) return true;
+    const uint32_t x[2] = {(uint32_t)PAIRING_X, (uint32_t)(PAIRING_X >> 32)};
+    const G2::Pt xq = G2::mul_affine(q, x, 2);
+    const G2::Pt p1 = g2_psi(xq);
+    G2::Pt lhs = xq;
+    G2::madd(lhs, q);
+    G2::add(lhs, p1);
+    G2::add(lhs, g2_psi(p1));
+    return G2::pt_eq(lhs, g2_psi(g2_psi(g2_psi(G2::dbl(xq)))));
 }
 
 // The line sequence of a G2 argument Q (affine, not infinity), in loop order.  `emit(c)` receives each line; the prepared

@@ -11,6 +11,20 @@
 //   prepare  parse the proof (canonical coordinates; >= p or off the curve -> invalid), sum the prepared inputs, affine
 //   miller   one multi-Miller loop over (A, B), (prepared, -gamma), (C, -delta) sharing one f; only B is stepped here
 //   final    the final exponentiation, compared with e(alpha, beta) -> one verdict byte
+// b2g_verify_batch checks the whole batch with one random linear combination instead (weights r_i from the caller):
+//     prod e(r_i A_i, B_i) * e(sum r_i C_i, -delta) * e(s_0 IC[0] + sum_j s_j IC[j], -gamma) == e(alpha, beta)^s_0,
+//     s_0 = sum r_i, s_j = sum r_i x_ij (mod r), x_ij the j-th public input of proof i (j = 1..n_public)
+//   prepare  one proof per thread: the parse and on-curve checks above, r_i A_i (affine) and r_i C_i (XYZZ)
+//   g2       one proof per thread: B in G2
+//   scalars  one CTA per (j, chunk of proofs): partial sums of r_i x_ij (x_i0 = 1)
+//   inputs   one warp per j: s_j from the partial sums, then s_j IC[j] from the window table (IC[0]: a variable-base product)
+//   miller   one proof per thread: the one-pair Miller loop of (r_i A_i, B_i)
+//   reduce   tree products of the Miller values, tree sums of the r_i C_i and of the s_j IC[j], one CTA level per launch
+//   pairs    one thread: the Miller loop of the two prepared pairs
+//   rhs      one thread: e(alpha, beta)^s_0
+//   final    one thread: one final exponentiation, compared with rhs -> one verdict byte
+// Only prepare -> miller -> product -> final run on the context's stream; the rest runs next to them on two side streams.
+#include <algorithm>
 #include <cstring>
 #include <string>
 #include <vector>
@@ -46,14 +60,20 @@ namespace b2g {
 constexpr size_t REC_BYTES_V = 384, REC_OK = 320;
 
 struct VerifyBufs {
-    size_t cap_count = 0, cap_inputs = 0;
+    size_t cap_count = 0, cap_pub = 0, cap_part = 0, cap_batch = 0;
     uint8_t *d_proofs = nullptr, *d_rec = nullptr, *d_f = nullptr, *d_verdict = nullptr;   // per proof
     uint8_t *d_pub = nullptr, *d_part = nullptr;                                            // per (proof, input)
+    uint8_t* d_batch = nullptr;                   // b2g_verify_batch: weights, reduction levels, scalar sums, tail values
+    cudaStream_t side[2] = {nullptr, nullptr};    // b2g_verify_batch's tail pieces, next to the per-proof kernels
+    cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
 };
 
 void verify_bufs_free(VerifyBufs* v) {
     if (!v) return;
-    for (void* p : {(void*)v->d_proofs, (void*)v->d_rec, (void*)v->d_f, (void*)v->d_verdict, (void*)v->d_pub, (void*)v->d_part}) if (p) cudaFree(p);
+    for (cudaStream_t s : v->side) if (s) cudaStreamDestroy(s);
+    for (cudaEvent_t e : v->ev) if (e) cudaEventDestroy(e);
+    for (void* p : {(void*)v->d_proofs, (void*)v->d_rec, (void*)v->d_f, (void*)v->d_verdict, (void*)v->d_pub, (void*)v->d_part,
+                    (void*)v->d_batch}) if (p) cudaFree(p);
     delete v;
 }
 
@@ -76,18 +96,22 @@ __device__ __forceinline__ bool fe_below_p(const fe& a) {
     return false;
 }
 
+// a 256-byte proof as affine Montgomery points; true when every coordinate is below p and every point on its curve
+__device__ __forceinline__ bool proof_parse(const uint8_t* pr, G1::Aff& a, G2::Aff& b, G1::Aff& cc) {
+    fe c[8];
+    bool ok = true;
+    for (int k = 0; k < 8; k++) { const fe v = fe_load(pr + 32 * k); ok &= fe_below_p(v); c[k] = Fq::from_canonical(v); }
+    a.x = c[0]; a.y = c[1]; b.x.c0 = c[2]; b.x.c1 = c[3]; b.y.c0 = c[4]; b.y.c1 = c[5]; cc.x = c[6]; cc.y = c[7];
+    return ok && aff_on_curve<G1, Fq>(a) && aff_on_curve<G1, Fq>(cc) && aff_on_curve<G2, Fq2>(b);
+}
+
 __global__ void __launch_bounds__(128) verify_prepare_kernel(const uint8_t* __restrict__ proofs, const uint8_t* __restrict__ g1,
                                                              const uint8_t* __restrict__ part, uint32_t n_public, uint32_t count,
                                                              uint8_t* __restrict__ rec) {
     const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= count) return;
-    const uint8_t* pr = proofs + (size_t)j * 256;
-    fe c[8];
-    bool ok = true;
-    for (int k = 0; k < 8; k++) { const fe v = fe_load(pr + 32 * k); ok &= fe_below_p(v); c[k] = Fq::from_canonical(v); }
     G1::Aff a, cc; G2::Aff b;
-    a.x = c[0]; a.y = c[1]; b.x.c0 = c[2]; b.x.c1 = c[3]; b.y.c0 = c[4]; b.y.c1 = c[5]; cc.x = c[6]; cc.y = c[7];
-    ok = ok && aff_on_curve<G1, Fq>(a) && aff_on_curve<G1, Fq>(cc) && aff_on_curve<G2, Fq2>(b);
+    const bool ok = proof_parse(proofs + (size_t)j * 256, a, b, cc);
     G1::Pt acc = G1::from_affine(aff_load<Fq>(g1, 1));   // IC[0]
     for (uint32_t i = 0; i < n_public; i++) G1::add(acc, pt_load<Fq>(part, (size_t)j * n_public + i));
     uint8_t* r = rec + (size_t)j * REC_BYTES_V;
@@ -124,6 +148,178 @@ __global__ void __launch_bounds__(64) verify_final_kernel(const uint8_t* __restr
     fe12 e;
     Fq12::final_exponentiation(e, Fq12::load(fin + (size_t)j * F12_BYTES));
     verdict[j] = Fq12::eq(e, Fq12::load(eab));
+}
+
+// ---------------------------------------------------------------------------------------------- b2g_verify_batch kernels
+// Per-proof record of the batch check, REC_BYTES_V apart: r A (affine, 64 B), B (affine, 128 B), r C (XYZZ, 128 B).  The
+// batch's ok word starts all ones and any failed parse, on-curve or G2 check clears it.
+constexpr size_t BREC_B = 64, BREC_RC = 192;
+constexpr uint32_t SCALAR_CHUNK = 2048;            // proofs per CTA of batch_scalars_kernel
+// tail values (Fq12 384 B, G1 XYZZ 128 B): the product of the per-proof Miller values, the Miller value of the prepared
+// pairs, e(alpha, beta)^s_0, sum r C, the prepared inputs, s_0
+constexpr size_t TAIL_F = 0, TAIL_G = 384, TAIL_RHS = 768, TAIL_RC = 1152, TAIL_PREP = 1280, TAIL_S0 = 1408, TAIL_BYTES = 1536;
+
+__device__ __forceinline__ void weight_load(uint32_t* k, const uint32_t* w, size_t i) {
+    for (int t = 0; t < 4; t++) k[t] = w[4 * i + t];
+}
+
+__global__ void __launch_bounds__(128) batch_prepare_kernel(const uint8_t* __restrict__ proofs, const uint32_t* __restrict__ w,
+                                                            uint32_t count, uint8_t* __restrict__ rec, uint32_t* __restrict__ ok_all) {
+    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= count) return;
+    G1::Aff a, cc; G2::Aff b;
+    // a failed proof's record is not written: the Miller kernel skips every proof once the ok word is cleared, the r C sum
+    // still reads the stale record, and batch_final_kernel discards what was computed from it
+    if (!proof_parse(proofs + (size_t)j * 256, a, b, cc)) { atomicAnd(ok_all, 0u); return; }
+    uint32_t k[4];
+    weight_load(k, w, j);
+    uint8_t* r = rec + (size_t)j * REC_BYTES_V;
+    aff_store<Fq>(r, 0, G1::to_affine(G1::mul_affine(a, k, 4)));
+    aff_store<Fq2>(r + BREC_B, 0, b);
+    pt_store<Fq>(r + BREC_RC, 0, G1::mul_affine(cc, k, 4));
+}
+
+// G2 membership of every B, one proof per thread, on a side stream next to the Miller kernel (only the ok word needs it)
+__global__ void __launch_bounds__(128) batch_g2_kernel(const uint8_t* __restrict__ proofs, uint32_t count, uint32_t* __restrict__ ok_all) {
+    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= count) return;
+    G1::Aff a, cc; G2::Aff b;
+    if (proof_parse(proofs + (size_t)j * 256, a, b, cc) && !g2_in_subgroup(b)) atomicAnd(ok_all, 0u);
+}
+
+// CTA (j, chunk): part[j * gridDim.y + chunk] = the sum over the chunk's proofs i of r_i (j = 0) or of
+// Fr::mul(r_i, x_ij) = r_i x_ij / R (j >= 1)
+__global__ void __launch_bounds__(128) batch_scalars_kernel(const uint32_t* __restrict__ w, const uint32_t* __restrict__ pub,
+                                                            uint32_t n_public, uint32_t count, uint8_t* __restrict__ part) {
+    __shared__ fe sh[128];
+    const uint32_t j = blockIdx.x, end = min(count, (blockIdx.y + 1) * SCALAR_CHUNK);
+    fe acc = Fr::zero();
+    for (uint32_t i = blockIdx.y * SCALAR_CHUNK + threadIdx.x; i < end; i += 128) {
+        fe wi = fe_zero();
+        weight_load(wi.l, w, i);
+        acc = Fr::add(acc, j ? Fr::mul(wi, fe_load(pub + 8 * ((size_t)i * n_public + j - 1))) : wi);
+    }
+    sh[threadIdx.x] = acc;
+    __syncthreads();
+    for (int d = 64; d > 0; d >>= 1) {
+        if ((int)threadIdx.x < d) sh[threadIdx.x] = Fr::add(sh[threadIdx.x], sh[threadIdx.x + d]);
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) fe_store(part + ((size_t)j * gridDim.y + blockIdx.y) * 32, sh[0]);
+}
+
+// one warp per j = 0..n_public: s_j from the chunk sums, pts[j] = s_j IC[j]; also s_0 to the tail
+__global__ void __launch_bounds__(128) batch_inputs_kernel(const uint8_t* __restrict__ tabs, const uint8_t* __restrict__ g1,
+                                                           const uint8_t* __restrict__ part, uint32_t chunks, uint32_t n_public,
+                                                           uint8_t* __restrict__ pts, uint8_t* __restrict__ tail) {
+    __shared__ G1::Pt sh[4][32];
+    __shared__ fe s[4];
+    const uint32_t wid = threadIdx.x >> 5, lane = threadIdx.x & 31, j = blockIdx.x * 4 + wid;
+    if (j > n_public) return;                              // whole warps leave together
+    if (lane == 0) {
+        fe acc = Fr::zero();
+        for (uint32_t c = 0; c < chunks; c++) acc = Fr::add(acc, fe_load(part + ((size_t)j * chunks + c) * 32));
+        s[wid] = j ? Fr::from_canonical(acc) : acc;       // from_canonical multiplies by R, cancelling the products' 1 / R
+    }
+    __syncwarp();
+    if (j) {
+        const G1::Pt p = warp_fixed_mul<G1, Fq>(tabs + (size_t)(j - 1) * TABLE_BYTES, s[wid].l, sh[wid]);
+        if (lane == 0) pt_store<Fq>(pts, j, p);
+    } else if (lane == 0) {
+        pt_store<Fq>(pts, 0, G1::mul_scalar(G1::from_affine(aff_load<Fq>(g1, 1)), s[wid].l));
+        fe_store(tail + TAIL_S0, s[wid]);
+    }
+}
+
+__global__ void __launch_bounds__(64) batch_miller_kernel(const uint8_t* __restrict__ rec, const uint32_t* __restrict__ ok_all,
+                                                          uint32_t count, uint8_t* __restrict__ fout) {
+    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= count) return;
+    fe12 f = Fq12::one();
+    if (*ok_all) {
+        const uint8_t* r = rec + (size_t)j * REC_BYTES_V;
+        const G1::Aff a = aff_load<Fq>(r, 0);
+        const G2::Aff b = aff_load<Fq2>(r + BREC_B, 0);
+        if (!G1::aff_is_inf(a) && !G2::aff_is_inf(b)) miller_loop_t<true, 0>(f, a, b, nullptr, nullptr);
+    }
+    Fq12::store(fout + (size_t)j * F12_BYTES, f);
+}
+
+// one level of a tree product: dst[b] = the product of src[64 b .. 64 b + 63] (Fq12, `stride` bytes apart)
+__global__ void __launch_bounds__(64) f12_product_kernel(const uint8_t* __restrict__ src, size_t stride, uint32_t n, uint8_t* __restrict__ dst) {
+    __shared__ fe12 sh[64];
+    const uint32_t t = threadIdx.x, i = blockIdx.x * 64 + t;
+    sh[t] = i < n ? Fq12::load(src + (size_t)i * stride) : Fq12::one();
+    __syncthreads();
+    for (uint32_t d = 32; d > 0; d >>= 1) {
+        if (t < d) { fe12 x = sh[t]; Fq12::mul(x, x, sh[t + d]); sh[t] = x; }
+        __syncthreads();
+    }
+    if (t == 0) Fq12::store(dst + (size_t)blockIdx.x * F12_BYTES, sh[0]);
+}
+
+// one level of a tree sum: dst[b] = the sum of src[128 b .. 128 b + 127] (G1 XYZZ, `stride` bytes apart)
+__global__ void __launch_bounds__(128) g1_sum_kernel(const uint8_t* __restrict__ src, size_t stride, uint32_t n, uint8_t* __restrict__ dst) {
+    __shared__ G1::Pt sh[128];
+    const uint32_t t = threadIdx.x, i = blockIdx.x * 128 + t;
+    sh[t] = i < n ? pt_load<Fq>(src + (size_t)i * stride, 0) : G1::infinity();
+    __syncthreads();
+    for (uint32_t d = 64; d > 0; d >>= 1) {
+        if (t < d) { G1::Pt x = sh[t]; G1::add(x, sh[t + d]); sh[t] = x; }
+        __syncthreads();
+    }
+    if (t == 0) pt_store<Fq>(dst, blockIdx.x, sh[0]);
+}
+
+// the Miller value of the prepared pairs (prepared inputs, -gamma) and (sum r C, -delta); 1 when both drop out
+__global__ void batch_pairs_kernel(uint8_t* __restrict__ tail, const uint8_t* __restrict__ lines, bool gamma_on, bool delta_on) {
+    const G1::Aff prep = G1::to_affine(pt_load<Fq>(tail + TAIL_PREP, 0)), c = G1::to_affine(pt_load<Fq>(tail + TAIL_RC, 0));
+    G1::Aff fp[2];
+    const uint8_t* fl[2];
+    int nfix = 0;
+    if (gamma_on && !G1::aff_is_inf(prep)) { fp[nfix] = prep; fl[nfix++] = lines; }
+    if (delta_on && !G1::aff_is_inf(c)) { fp[nfix] = c; fl[nfix++] = lines + ATE_LINES * LINE_BYTES; }
+    G2::Aff none; none.x = Fq2::zero(); none.y = Fq2::zero();
+    fe12 g;
+    miller_loop(g, false, fp[0], none, nfix, fp, fl);
+    Fq12::store(tail + TAIL_G, g);
+}
+
+// e(alpha, beta)^s_0
+__global__ void batch_rhs_kernel(uint8_t* __restrict__ tail, const uint8_t* __restrict__ eab) {
+    fe12 rhs;
+    const fe s0 = fe_load(tail + TAIL_S0);
+    Fq12::cyclotomic_exp(rhs, Fq12::load(eab), s0.l);
+    Fq12::store(tail + TAIL_RHS, rhs);
+}
+
+// the verdict: ok, and the final exponentiation of (per-proof product) x (prepared pairs) equals e(alpha, beta)^s_0
+__global__ void batch_final_kernel(const uint8_t* __restrict__ tail, const uint32_t* __restrict__ ok_all, uint8_t* __restrict__ verdict) {
+    if (!*ok_all) { *verdict = 0; return; }
+    fe12 f = Fq12::load(tail + TAIL_F), e;
+    Fq12::mul(f, f, Fq12::load(tail + TAIL_G));
+    Fq12::final_exponentiation(e, f);
+    *verdict = Fq12::eq(e, Fq12::load(tail + TAIL_RHS));
+}
+
+// b2g_test_op ops 43-45: G2 membership of a G2 affine point (out: 8 B, 1 or 0), r * P for a G1 affine P and a 128-bit r
+// (b: 16 B; out: 64 B affine), f^k for a cyclotomic Fq12 f and a canonical 256-bit k (b: 32 B; out: 384 B)
+__global__ void batch_test_kernel(int op, const uint8_t* __restrict__ a, const uint8_t* __restrict__ b, uint32_t n, uint8_t* __restrict__ out) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    if (op == 43) {
+        const uint64_t v = g2_in_subgroup(aff_load<Fq2>(a, i));
+        reinterpret_cast<uint64_t*>(out)[i] = v;
+    } else if (op == 44) {
+        uint32_t k[4];
+        weight_load(k, reinterpret_cast<const uint32_t*>(b), i);
+        aff_store<Fq>(out, i, G1::to_affine(G1::mul_affine(aff_load<Fq>(a, i), k, 4)));
+    } else {
+        fe12 r;
+        const fe k = fe_load(b + (size_t)i * 32);
+        Fq12::cyclotomic_exp(r, Fq12::load(a + (size_t)i * F12_BYTES), k.l);
+        Fq12::store(out + (size_t)i * F12_BYTES, r);
+    }
 }
 
 // lines of -gamma (thread 0) and -delta (thread 1) for every loop step, in the order miller_loop reads them
@@ -189,19 +385,25 @@ __global__ void pairing_test_kernel(int op, const uint8_t* __restrict__ a, const
 }
 
 void pairing_test_op(cudaStream_t st, int op, const void* a, const void* b, size_t n, void* out) {
-    if (op > 42 || !a || !out) throw_error(B2G_E_SHAPE, "bad arguments");
-    const size_t sa = (op == 37 || op == 40) ? 64 : ((op == 41 || op == 42) ? LINE_BYTES : F12_BYTES);
-    const size_t sb = op == 30 ? F12_BYTES : ((op == 37 || op == 40 || op == 42) ? 128 : (op == 39 ? LINE_BYTES : 0));
+    if (op > 45 || !a || !out) throw_error(B2G_E_SHAPE, "bad arguments");
+    const bool batch_op = op >= 43;
+    size_t sa = (op == 37 || op == 40) ? 64 : ((op == 41 || op == 42) ? LINE_BYTES : F12_BYTES);
+    size_t sb = op == 30 ? F12_BYTES : ((op == 37 || op == 40 || op == 42) ? 128 : (op == 39 ? LINE_BYTES : 0));
+    size_t so = F12_BYTES;
+    if (op == 43) { sa = 128; sb = 0; so = 8; }
+    if (op == 44) { sa = 64; sb = 16; so = 64; }
+    if (op == 45) { sa = F12_BYTES; sb = 32; so = F12_BYTES; }
     if (sb && !b) throw_error(B2G_E_SHAPE, "this op needs operand b");
     if (n == 0) return;
     struct Bufs { uint8_t *a = nullptr, *b = nullptr, *o = nullptr; ~Bufs() { for (void* p : {(void*)a, (void*)b, (void*)o}) if (p) cudaFree(p); } } d;
     d.a = dev_upload<uint8_t>(a, n * sa, st);
     if (sb) d.b = dev_upload<uint8_t>(b, n * sb, st);
-    CUDA_CHECK(cudaMalloc(&d.o, n * F12_BYTES));
-    pairing_test_kernel<<<(unsigned)((n + 63) / 64), 64, 0, st>>>(op, d.a, d.b, (uint32_t)n, d.o);
+    CUDA_CHECK(cudaMalloc(&d.o, n * so));
+    if (batch_op) batch_test_kernel<<<(unsigned)((n + 63) / 64), 64, 0, st>>>(op, d.a, d.b, (uint32_t)n, d.o);
+    else pairing_test_kernel<<<(unsigned)((n + 63) / 64), 64, 0, st>>>(op, d.a, d.b, (uint32_t)n, d.o);
     g_launch_count += 1;
     CUDA_CHECK(cudaGetLastError());
-    CUDA_CHECK(cudaMemcpyAsync(out, d.o, n * F12_BYTES, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaMemcpyAsync(out, d.o, n * so, cudaMemcpyDeviceToHost, st));
     CUDA_CHECK(cudaStreamSynchronize(st));
 }
 
@@ -224,9 +426,19 @@ static bool below_r(const uint32_t* k) {
     return false;
 }
 
-// grows the context's verification buffers to `count` proofs and `inputs` (proof, input) pairs; never shrinks them.  A
-// buffer set is marked empty before it is reallocated, so a failed allocation leaves the context consistent.
-static void vbufs_ensure(VerifyBufs*& v, size_t count, size_t inputs) {
+// grows one of the context's verification buffers to `bytes`; never shrinks it.  The buffer is marked empty before it is
+// reallocated, so a failed allocation leaves the context consistent.
+static void vbuf_grow(uint8_t*& p, size_t& cap, size_t bytes) {
+    if (bytes <= cap) return;
+    if (p) cudaFree(p);
+    p = nullptr; cap = 0;
+    CUDA_CHECK(cudaMalloc(&p, bytes));
+    cap = bytes;
+}
+
+// grows the context's verification buffers to `count` proofs, `inputs` public-input scalars, `parts` (proof, input) G1
+// records and `batch` bytes of b2g_verify_batch scratch; never shrinks them, and a failed allocation leaves them consistent
+static void vbufs_ensure(VerifyBufs*& v, size_t count, size_t inputs, size_t parts, size_t batch = 0) {
     if (!v) v = new VerifyBufs();
     if (count > v->cap_count) {
         for (uint8_t** p : {&v->d_proofs, &v->d_rec, &v->d_f, &v->d_verdict}) { if (*p) cudaFree(*p); *p = nullptr; }
@@ -237,12 +449,34 @@ static void vbufs_ensure(VerifyBufs*& v, size_t count, size_t inputs) {
         CUDA_CHECK(cudaMalloc(&v->d_verdict, count));
         v->cap_count = count;
     }
-    if (inputs > v->cap_inputs) {
-        for (uint8_t** p : {&v->d_pub, &v->d_part}) { if (*p) cudaFree(*p); *p = nullptr; }
-        v->cap_inputs = 0;
-        CUDA_CHECK(cudaMalloc(&v->d_pub, inputs * 32));
-        CUDA_CHECK(cudaMalloc(&v->d_part, inputs * 128));
-        v->cap_inputs = inputs;
+    vbuf_grow(v->d_pub, v->cap_pub, inputs * 32);
+    vbuf_grow(v->d_part, v->cap_part, parts * 128);
+    vbuf_grow(v->d_batch, v->cap_batch, batch);
+}
+
+// the two side streams and five events of b2g_verify_batch, created at its first call on the context.  The side streams have
+// the greatest priority, so that their one-thread tail kernels are scheduled ahead of queued per-proof CTAs.
+static void batch_streams(VerifyBufs& v) {
+    if (v.ev[4]) return;
+    int least = 0, greatest = 0;
+    CUDA_CHECK(cudaDeviceGetStreamPriorityRange(&least, &greatest));
+    for (cudaStream_t& s : v.side) if (!s) CUDA_CHECK(cudaStreamCreateWithPriority(&s, cudaStreamNonBlocking, greatest));
+    for (cudaEvent_t& e : v.ev) if (!e) CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+}
+
+// one tree reduction of n records of `src` (`stride` bytes apart) into `dst`: a launch per level of `per` records per CTA,
+// the levels alternating between the scratch areas x and y
+template <class Level>
+static void tree_reduce(const uint8_t* src, size_t stride, size_t rec_bytes, uint32_t n, uint32_t per, uint8_t* x, uint8_t* y,
+                        uint8_t* dst, Level&& level) {
+    for (;;) {
+        const uint32_t blocks = (n + per - 1) / per;
+        uint8_t* out = blocks == 1 ? dst : x;
+        level(blocks, src, stride, n, out);
+        g_launch_count += 1;
+        if (blocks == 1) return;
+        src = out; stride = rec_bytes; n = blocks;
+        std::swap(x, y);
     }
 }
 
@@ -304,28 +538,41 @@ int b2g_vk_alpha_beta(b2g_vk* vk, void* out) {
     });
 }
 
+// the argument checks b2g_verify_many and b2g_verify_batch share; returns the context
+static CtxView verify_args(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs,
+                           const void* out) {
+    if (!ctx || !vk || !proofs || !out || (vk->n_public && !public_inputs)) throw_error(B2G_E_SHAPE, "null pointer");
+    if (count == 0) throw_error(B2G_E_SHAPE, std::string(fn) + ": count must be at least 1");
+    const CtxView cv = ctx_view(ctx);
+    if (vk->device != cv.device) throw_error(B2G_E_SHAPE, "the verifying key belongs to another device");
+    if (cv.proof_pending) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
+    const size_t inputs = (size_t)count * vk->n_public;
+    const uint32_t* pub = (const uint32_t*)public_inputs;
+    for (size_t k = 0; k < inputs; k++)
+        if (!below_r(pub + 8 * k)) throw_error(B2G_E_INPUT, "public input " + std::to_string(k % vk->n_public) + " of proof " +
+                                                             std::to_string(k / vk->n_public) + " is not below the scalar field modulus r");
+    return cv;
+}
+
+// vbufs_ensure, reporting a batch that does not fit as B2G_E_DEVICE with advice
+static void verify_bufs_ensure(const char* fn, VerifyBufs*& v, uint32_t count, size_t inputs, size_t parts, size_t batch = 0) {
+    try {
+        vbufs_ensure(v, count, inputs, parts, batch);
+    } catch (const B2gError& e) {
+        if (e.code != B2G_E_DEVICE) throw;
+        cudaGetLastError();
+        throw_error(B2G_E_DEVICE, std::string(fn) + ": the device buffers of " + std::to_string(count) +
+                                  " proofs do not fit in device memory; verify fewer per call (" + e.what() + ")");
+    }
+}
+
 int b2g_verify_many(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs, uint8_t* verdicts_out) {
     return guarded([&] {
-        if (!ctx || !vk || !proofs || !verdicts_out || (vk->n_public && !public_inputs)) throw_error(B2G_E_SHAPE, "null pointer");
-        if (count == 0) throw_error(B2G_E_SHAPE, "b2g_verify_many: count must be at least 1");
-        const CtxView cv = ctx_view(ctx);
-        if (vk->device != cv.device) throw_error(B2G_E_SHAPE, "the verifying key belongs to another device");
-        if (cv.proof_pending) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
+        const CtxView cv = verify_args("b2g_verify_many", ctx, vk, count, public_inputs, proofs, verdicts_out);
         const size_t inputs = (size_t)count * vk->n_public;
-        const uint32_t* pub = (const uint32_t*)public_inputs;
-        for (size_t k = 0; k < inputs; k++)
-            if (!below_r(pub + 8 * k)) throw_error(B2G_E_INPUT, "public input " + std::to_string(k % vk->n_public) + " of proof " +
-                                                                 std::to_string(k / vk->n_public) + " is not below the scalar field modulus r");
         DevGuard g(cv.device);
         cudaStream_t st = cv.st;
-        try {
-            vbufs_ensure(*cv.vbufs, count, inputs);
-        } catch (const B2gError& e) {
-            if (e.code != B2G_E_DEVICE) throw;
-            cudaGetLastError();
-            throw_error(B2G_E_DEVICE, "b2g_verify_many: the device buffers of " + std::to_string(count) +
-                                      " proofs do not fit in device memory; verify fewer per call (" + e.what() + ")");
-        }
+        verify_bufs_ensure("b2g_verify_many", *cv.vbufs, count, inputs, inputs);
         VerifyBufs& v = **cv.vbufs;
         CUDA_CHECK(cudaMemcpyAsync(v.d_proofs, proofs, (size_t)count * 256, cudaMemcpyHostToDevice, st));
         if (inputs) {
@@ -338,6 +585,75 @@ int b2g_verify_many(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public
         g_launch_count += 3 + (inputs ? 1 : 0);
         CUDA_CHECK(cudaGetLastError());
         CUDA_CHECK(cudaMemcpyAsync(verdicts_out, v.d_verdict, count, cudaMemcpyDeviceToHost, st));
+        CUDA_CHECK(cudaStreamSynchronize(st));
+    });
+}
+
+int b2g_verify_batch(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs, const void* weights,
+                     uint8_t* verdict_out) {
+    return guarded([&] {
+        if (!weights) throw_error(B2G_E_SHAPE, "null pointer");
+        const CtxView cv = verify_args("b2g_verify_batch", ctx, vk, count, public_inputs, proofs, verdict_out);
+        for (uint32_t i = 0; i < count; i++)
+            if (all_zero((const uint8_t*)weights + 16 * (size_t)i, 16)) throw_error(B2G_E_INPUT, "weight " + std::to_string(i) + " is zero");
+        const uint32_t n_pts = vk->n_public + 1, chunks = (count + SCALAR_CHUNK - 1) / SCALAR_CHUNK;
+        const size_t inputs = (size_t)count * vk->n_public;
+        // scratch: weights, four reduction levels (x, y on the main stream, x2, y2 on the side streams), chunk sums of the
+        // scalars, s_j IC[j], tail values and the ok word
+        auto up = [](size_t b) { return (b + 255) & ~(size_t)255; };
+        const size_t level = up(std::max({(size_t)((count + 63) / 64) * F12_BYTES, (size_t)((count + 127) / 128) * 128,
+                                          (size_t)((n_pts + 127) / 128) * 128}));
+        const size_t o_w = 0, o_x = up((size_t)count * 16), o_y = o_x + level, o_x2 = o_y + level, o_y2 = o_x2 + level;
+        const size_t o_part = o_y2 + level, o_pts = o_part + up((size_t)n_pts * chunks * 32), o_tail = o_pts + up((size_t)n_pts * 128);
+        const size_t o_ok = o_tail + TAIL_BYTES, bytes = o_ok + 256;
+        DevGuard g(cv.device);
+        cudaStream_t st = cv.st;
+        verify_bufs_ensure("b2g_verify_batch", *cv.vbufs, count, inputs, 0, bytes);
+        VerifyBufs& v = **cv.vbufs;
+        batch_streams(v);
+        cudaStream_t s2 = v.side[0], s3 = v.side[1];
+        cudaEvent_t ev_up = v.ev[0], ev_prep = v.ev[1], ev_pts = v.ev[2], ev_s2 = v.ev[3], ev_s3 = v.ev[4];
+        uint8_t* B = v.d_batch;
+        uint8_t* tail = B + o_tail;
+        const uint32_t* w = (const uint32_t*)(B + o_w);
+        uint32_t* ok = (uint32_t*)(B + o_ok);
+        auto prod = [](cudaStream_t s) {
+            return [s](uint32_t blocks, const uint8_t* src, size_t stride, uint32_t n, uint8_t* o) { f12_product_kernel<<<blocks, 64, 0, s>>>(src, stride, n, o); };
+        };
+        auto sum = [](cudaStream_t s) {
+            return [s](uint32_t blocks, const uint8_t* src, size_t stride, uint32_t n, uint8_t* o) { g1_sum_kernel<<<blocks, 128, 0, s>>>(src, stride, n, o); };
+        };
+        CUDA_CHECK(cudaMemcpyAsync(v.d_proofs, proofs, (size_t)count * 256, cudaMemcpyHostToDevice, st));
+        CUDA_CHECK(cudaMemcpyAsync(B + o_w, weights, (size_t)count * 16, cudaMemcpyHostToDevice, st));
+        if (inputs) CUDA_CHECK(cudaMemcpyAsync(v.d_pub, public_inputs, inputs * 32, cudaMemcpyHostToDevice, st));
+        CUDA_CHECK(cudaMemsetAsync(ok, 0xff, 4, st));
+        CUDA_CHECK(cudaEventRecord(ev_up, st));
+        // main stream: per-proof parse and scaling, Miller loops, their product, then the verdict
+        batch_prepare_kernel<<<(count + 127) / 128, 128, 0, st>>>(v.d_proofs, w, count, v.d_rec, ok);
+        CUDA_CHECK(cudaEventRecord(ev_prep, st));
+        batch_miller_kernel<<<(count + 63) / 64, 64, 0, st>>>(v.d_rec, ok, count, v.d_f);
+        tree_reduce(v.d_f, F12_BYTES, F12_BYTES, count, 64, B + o_x, B + o_y, tail + TAIL_F, prod(st));
+        // side stream 2: the input scalars, the prepared inputs, e(alpha, beta)^s_0, the G2 membership of every B
+        CUDA_CHECK(cudaStreamWaitEvent(s2, ev_up, 0));
+        batch_scalars_kernel<<<dim3(n_pts, chunks), 128, 0, s2>>>(w, (const uint32_t*)v.d_pub, vk->n_public, count, B + o_part);
+        batch_inputs_kernel<<<(n_pts + 3) / 4, 128, 0, s2>>>(vk->d_tabs, vk->d_g1, B + o_part, chunks, vk->n_public, B + o_pts, tail);
+        tree_reduce(B + o_pts, 128, 128, n_pts, 128, B + o_x2, B + o_y2, tail + TAIL_PREP, sum(s2));
+        CUDA_CHECK(cudaEventRecord(ev_pts, s2));
+        batch_rhs_kernel<<<1, 1, 0, s2>>>(tail, vk->d_eab);
+        batch_g2_kernel<<<(count + 127) / 128, 128, 0, s2>>>(v.d_proofs, count, ok);
+        CUDA_CHECK(cudaEventRecord(ev_s2, s2));
+        // side stream 3, once the r C and the prepared inputs exist: sum r C, then the Miller loop of the prepared pairs
+        CUDA_CHECK(cudaStreamWaitEvent(s3, ev_prep, 0));
+        CUDA_CHECK(cudaStreamWaitEvent(s3, ev_pts, 0));
+        tree_reduce(v.d_rec + BREC_RC, REC_BYTES_V, 128, count, 128, B + o_x2, B + o_y2, tail + TAIL_RC, sum(s3));
+        batch_pairs_kernel<<<1, 1, 0, s3>>>(tail, vk->d_lines, !vk->gamma_inf, !vk->delta_inf);
+        CUDA_CHECK(cudaEventRecord(ev_s3, s3));
+        CUDA_CHECK(cudaStreamWaitEvent(st, ev_s2, 0));
+        CUDA_CHECK(cudaStreamWaitEvent(st, ev_s3, 0));
+        batch_final_kernel<<<1, 1, 0, st>>>(tail, ok, v.d_verdict);
+        g_launch_count += 8;
+        CUDA_CHECK(cudaGetLastError());
+        CUDA_CHECK(cudaMemcpyAsync(verdict_out, v.d_verdict, 1, cudaMemcpyDeviceToHost, st));
         CUDA_CHECK(cudaStreamSynchronize(st));
     });
 }

@@ -12,6 +12,8 @@
     Groth16.verify_many(vk, public_inputs, proofs)
         <- Groth16::verify_with_processed_vk (src/zkey.rs:869-870, 914-916) for many proofs of one key in one device pass
            (b2g_verify_many, with the key prepared on the device by b2g_vk_load <- process_vk).
+    Groth16.verify_batch(vk, public_inputs, proofs)
+        <- the same check for a whole batch at once: one random-linear-combination pairing check (b2g_verify_batch).
 Arguments keep the reference's meaning; field elements are (n, 4) uint64 Montgomery limb arrays (fr_to_mont).
 """
 from __future__ import annotations
@@ -41,7 +43,9 @@ _TEST_OP_WORDS = {**{op: (4, 4, 4) for op in (0, 1, 2, 3, 4, 5, 14, 15, 16)}, 6:
                   26: (32, 20, 32), 27: (16 * 20, 0, 32), 29: (4, 4, 8),
                   # the pairing tower (csrc/pairing.cuh): Fq12 = 48 words, G1 / G2 affine = 8 / 16, a line (3 Fq2) = 24
                   30: (48, 48, 48), **{op: (48, 0, 48) for op in (31, 32, 33, 34, 35, 36, 38)}, 37: (8, 16, 48), 39: (48, 24, 48),
-                  40: (8, 16, 48), 41: (24, 0, 48), 42: (24, 16, 48)}
+                  40: (8, 16, 48), 41: (24, 0, 48), 42: (24, 16, 48),
+                  # the batch check's pieces: G2 membership, 128-bit G1 product, cyclotomic exponentiation
+                  43: (16, 0, 1), 44: (8, 2, 8), 45: (48, 4, 48)}
 TEST_PAIR_RUN = 16            # entries per row of op 27; an entry is 16 words of affine point + 4 words whose bit 0 is the sign
 
 
@@ -264,6 +268,31 @@ class PendingProof:
         return Proof(self._out.tobytes())
 
 
+def _verify_args(fn, vk, public_inputs, proofs, ctx):
+    """the argument checks and encoding verify_many and verify_batch share: None for an empty batch, else (ctx, device key,
+    count, public inputs as 32 B words or None, proofs as 256 B rows)"""
+    from . import verifier
+    public_inputs, proofs = [list(x) for x in public_inputs], list(proofs)
+    if len(public_inputs) != len(proofs):
+        raise ValueError(f"{fn}: one public-input list per proof")
+    if not proofs:
+        return None
+    base = vk.vk if isinstance(vk, verifier.PreparedVerifyingKey) else vk
+    n_public = len(base.gamma_abc_g1) - 1
+    for xs in public_inputs:
+        if len(xs) != n_public:
+            raise verifier.MalformedVerifyingKey(f"{len(xs)} public inputs for a key with {n_public}")
+        for x in xs:
+            if not 0 <= int(x) < R_MOD:        # the library refuses >= r too; this also covers values no 32 B word holds
+                raise N.B2gError(N.B2G_E_INPUT, f"public input {int(x)} is not in [0, r)")
+    ctx = ctx or default_context()
+    vh = ctx.vk_handle(vk)
+    pub = b''.join(int(x).to_bytes(32, 'little') for xs in public_inputs for x in xs)
+    pub_arr = np.frombuffer(pub, dtype=np.uint8).copy() if pub else None
+    data = np.frombuffer(b''.join(p.data for p in proofs), dtype=np.uint8).copy()
+    return ctx, vh, len(proofs), pub_arr, data
+
+
 def _scalar_bytes(v) -> np.ndarray:
     if isinstance(v, (int, np.integer)):
         return np.frombuffer((int(v) % R_MOD).to_bytes(32, 'little'), dtype='<u8').copy()
@@ -427,28 +456,46 @@ class Groth16:
         sequence of ints per proof, proofs = [Proof].  Returns [bool].  Verdicts equal the host call's, except that a proof
         coordinate >= p is invalid here (arkworks cannot deserialise it) where the host verifier reduces it.  A public input
         outside [0, r) raises B2gError (B2G_E_INPUT); an input count that does not match the key raises MalformedVerifyingKey."""
-        from . import verifier
-        public_inputs, proofs = [list(x) for x in public_inputs], list(proofs)
-        if len(public_inputs) != len(proofs):
-            raise ValueError("verify_many: one public-input list per proof")
-        if not proofs:
+        args = _verify_args('verify_many', vk, public_inputs, proofs, ctx)
+        if args is None:
             return []
-        base = vk.vk if isinstance(vk, verifier.PreparedVerifyingKey) else vk
-        n_public = len(base.gamma_abc_g1) - 1
-        for xs in public_inputs:
-            if len(xs) != n_public:
-                raise verifier.MalformedVerifyingKey(f"{len(xs)} public inputs for a key with {n_public}")
-            for x in xs:
-                if not 0 <= int(x) < R_MOD:        # the library refuses >= r too; this also covers values no 32 B word holds
-                    raise N.B2gError(N.B2G_E_INPUT, f"public input {int(x)} is not in [0, r)")
-        ctx = ctx or default_context()
-        vh = ctx.vk_handle(vk)
-        pub = b''.join(int(x).to_bytes(32, 'little') for xs in public_inputs for x in xs)
-        pub_arr = np.frombuffer(pub, dtype=np.uint8).copy() if pub else None
-        data = np.frombuffer(b''.join(p.data for p in proofs), dtype=np.uint8).copy()
-        out = np.zeros(len(proofs), dtype=np.uint8)
-        N.check(N.lib().b2g_verify_many(ctx._h, vh, len(proofs), _ptr(pub_arr) if pub_arr is not None else None, _ptr(data), _ptr(out)))
+        ctx, vh, count, pub_arr, data = args
+        out = np.zeros(count, dtype=np.uint8)
+        N.check(N.lib().b2g_verify_many(ctx._h, vh, count, _ptr(pub_arr) if pub_arr is not None else None, _ptr(data), _ptr(out)))
         return [bool(v) for v in out]
+
+    @staticmethod
+    def verify_batch(vk, public_inputs, proofs, ctx: Context = None, weights=None) -> bool:
+        """Whether ALL proofs are valid, from one random-linear-combination pairing check on the device (b2g_verify_batch):
+        cheaper per proof than verify_many, but one verdict for the batch.  On False, call verify_many to find the invalid
+        proofs.  True iff every proof would pass verify_many, every B lies in G2 (verify_many does not check that), except
+        with probability at most 1 / (2^128 - 1) when the weights are uniform.  Arguments and errors as verify_many; an empty
+        batch is True.  `weights` (one int in [1, 2^128) per proof) are drawn with secrets.randbits(128) when not given;
+        weights a prover could know or choose before fixing its proofs make the check unsound.  A zero or too large weight
+        raises B2gError (B2G_E_INPUT)."""
+        import secrets
+        proofs = list(proofs)
+        if weights is not None:                    # checked before the key is loaded on the device
+            weights = [int(w) for w in weights]
+            if len(weights) != len(proofs):
+                raise ValueError("verify_batch: one weight per proof")
+            for w in weights:
+                if not 0 < w < 1 << 128:
+                    raise N.B2gError(N.B2G_E_INPUT, f"weight {w} is not in [1, 2^128)")
+        args = _verify_args('verify_batch', vk, public_inputs, proofs, ctx)
+        if args is None:
+            return True
+        ctx, vh, count, pub_arr, data = args
+        if weights is None:
+            weights = []
+            while len(weights) < count:
+                w = secrets.randbits(128)
+                if w:
+                    weights.append(w)
+        wb = np.frombuffer(b''.join(w.to_bytes(16, 'little') for w in weights), dtype=np.uint8).copy()
+        out = np.zeros(1, dtype=np.uint8)
+        N.check(N.lib().b2g_verify_batch(ctx._h, vh, count, _ptr(pub_arr) if pub_arr is not None else None, _ptr(data), _ptr(wb), _ptr(out)))
+        return bool(out[0])
 
     # base-range sharded variant: every rank calls prove_partial, the 768-byte partials are all-gathered by the caller
     # (torch.distributed / NCCL), then every rank calls prove_finish and obtains the same proof.

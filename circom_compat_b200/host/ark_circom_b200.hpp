@@ -11,6 +11,7 @@
 //   ark_circom::Groth16::process_vk / verify_with_processed_vk / verify <- src/zkey.rs:868-870, tests/groth16.rs:33-35
 //   ark_circom::Groth16::verify_many          <- verify_with_processed_vk for many proofs of one key, in one device pass
 //                                                         (host pairing, ark_circom_verifier.hpp; no GPU involved)
+//   ark_circom::Groth16::verify_batch         <- the same for a whole batch at once: one random-linear-combination check
 //   ark_circom::read_wtns                              <- snarkjs .wtns (test-vectors/circuit2_js/witness.wtns; the reference
 //                                                         computes witnesses with WASM instead, out of scope here)
 // Parsing and key handling stay on the host; every field/curve operation of the proof runs in libb2groth.so.
@@ -367,6 +368,38 @@ typedef Reduction<B2G_REDUCTION_LIBSNARK> LibsnarkReduction;   // ark-groth16's 
 #include "ark_circom_ethereum.hpp"
 namespace ark_circom {
 
+// what Groth16::verify_many and verify_batch share: the argument checks, the key prepared on the device at first use
+// (b2g_vk_load, kept in pvk.device) and the encoded public inputs and proofs
+struct VerifyCall {
+    size_t n = 0;
+    Gpu* gpu = nullptr;
+    b2g_vk* vk = nullptr;
+    std::vector<BigInt256> pub;
+    std::vector<uint8_t> bytes;
+    VerifyCall(const char* fn, const PreparedVerifyingKey& pvk, const std::vector<std::vector<Fr>>& public_inputs,
+               const std::vector<Proof>& proofs, int device) {
+        if (public_inputs.size() != proofs.size()) throw SynthesisError(std::string(fn) + ": one public-input list per proof");
+        const size_t n_public = pvk.vk.gamma_abc_g1.size() - 1;
+        if (proofs.empty()) return;
+        for (const auto& xs : public_inputs) if (xs.size() != n_public) throw MalformedVerifyingKey();
+        n = proofs.size();
+        gpu = &Gpu::on(device);
+        vk = (b2g_vk*)pvk.device.find(gpu->ctx(), 0);
+        if (!vk) {
+            b2g_vk_desc d; memset(&d, 0, sizeof d);
+            d.n_public = (uint32_t)n_public;
+            d.alpha_g1 = &pvk.vk.alpha_g1; d.beta_g2 = &pvk.vk.beta_g2; d.gamma_g2 = &pvk.vk.gamma_g2; d.delta_g2 = &pvk.vk.delta_g2;
+            d.gamma_abc_g1 = pvk.vk.gamma_abc_g1.data();
+            check(b2g_vk_load(gpu->ctx(), &d, &vk));
+            pvk.device.put(gpu->ctx(), 0, vk, [](void* p) { b2g_vk_free((b2g_vk*)p); });
+        }
+        pub.resize(n * n_public);
+        for (size_t i = 0; i < n; i++) for (size_t k = 0; k < n_public; k++) pub[i * n_public + k] = public_inputs[i][k].into_bigint();
+        bytes.resize(n * 256);
+        for (size_t i = 0; i < n; i++) memcpy(&bytes[i * 256], proofs[i].bytes, 256);
+    }
+};
+
 template <class QAP = CircomReduction>
 struct Groth16T {                                       // Groth16::<Bn254, QAP>
     // verification (host pairing, ark_circom_verifier.hpp): src/zkey.rs:868-870, 914-916; tests/groth16.rs:33-35
@@ -382,26 +415,28 @@ struct Groth16T {                                       // Groth16::<Bn254, QAP>
     // coordinate >= p: the host call throws SerializationError there, the batch reports the proof invalid.
     static std::vector<bool> verify_many(const PreparedVerifyingKey& pvk, const std::vector<std::vector<Fr>>& public_inputs,
                                          const std::vector<Proof>& proofs, int device = 0) {
-        if (public_inputs.size() != proofs.size()) throw SynthesisError("verify_many: one public-input list per proof");
-        const size_t n = proofs.size(), n_public = pvk.vk.gamma_abc_g1.size() - 1;
-        if (n == 0) return {};
-        for (const auto& xs : public_inputs) if (xs.size() != n_public) throw MalformedVerifyingKey();
-        Gpu& gpu = Gpu::on(device);
-        b2g_vk* vk = (b2g_vk*)pvk.device.find(gpu.ctx(), 0);
-        if (!vk) {
-            b2g_vk_desc d; memset(&d, 0, sizeof d);
-            d.n_public = (uint32_t)n_public;
-            d.alpha_g1 = &pvk.vk.alpha_g1; d.beta_g2 = &pvk.vk.beta_g2; d.gamma_g2 = &pvk.vk.gamma_g2; d.delta_g2 = &pvk.vk.delta_g2;
-            d.gamma_abc_g1 = pvk.vk.gamma_abc_g1.data();
-            check(b2g_vk_load(gpu.ctx(), &d, &vk));
-            pvk.device.put(gpu.ctx(), 0, vk, [](void* p) { b2g_vk_free((b2g_vk*)p); });
-        }
-        std::vector<BigInt256> pub(n * n_public);
-        for (size_t i = 0; i < n; i++) for (size_t k = 0; k < n_public; k++) pub[i * n_public + k] = public_inputs[i][k].into_bigint();
-        std::vector<uint8_t> bytes(n * 256), verdicts(n);
-        for (size_t i = 0; i < n; i++) memcpy(&bytes[i * 256], proofs[i].bytes, 256);
-        check(b2g_verify_many(gpu.ctx(), vk, (uint32_t)n, pub.empty() ? nullptr : pub.data(), bytes.data(), verdicts.data()));
+        VerifyCall c("verify_many", pvk, public_inputs, proofs, device);
+        if (c.n == 0) return {};
+        std::vector<uint8_t> verdicts(c.n);
+        check(b2g_verify_many(c.gpu->ctx(), c.vk, (uint32_t)c.n, c.pub.empty() ? nullptr : c.pub.data(), c.bytes.data(), verdicts.data()));
         return std::vector<bool>(verdicts.begin(), verdicts.end());
+    }
+    // whether ALL proofs are valid, from one random-linear-combination pairing check (b2g_verify_batch): true iff every
+    // proof passes verify_many and every B lies in G2, except with probability <= 1 / (2^128 - 1).  The 128-bit weights
+    // come from std::random_device, drawn after the proofs are fixed.  On false, call verify_many to find the invalid
+    // proofs.  An empty batch is true.
+    static bool verify_batch(const PreparedVerifyingKey& pvk, const std::vector<std::vector<Fr>>& public_inputs,
+                             const std::vector<Proof>& proofs, int device = 0) {
+        VerifyCall c("verify_batch", pvk, public_inputs, proofs, device);
+        if (c.n == 0) return true;
+        std::random_device rd;
+        std::vector<uint32_t> w(4 * c.n);
+        for (size_t i = 0; i < c.n; i++) {
+            do { for (int t = 0; t < 4; t++) w[4 * i + t] = (uint32_t)rd(); } while (!(w[4 * i] | w[4 * i + 1] | w[4 * i + 2] | w[4 * i + 3]));
+        }
+        uint8_t verdict = 0;
+        check(b2g_verify_batch(c.gpu->ctx(), c.vk, (uint32_t)c.n, c.pub.empty() ? nullptr : c.pub.data(), c.bytes.data(), w.data(), &verdict));
+        return verdict != 0;
     }
     static Proof create_proof_with_reduction_and_matrices(const ProvingKey& pk, const Fr& r, const Fr& s, const ConstraintMatrices& matrices,
                                                           size_t num_inputs, size_t num_constraints, const std::vector<Fr>& full_assignment,

@@ -8,6 +8,8 @@
 //       B2G_MANY=K: also K proofs in one device pass (Groth16::create_proofs)
 //       B2G_VERIFY_MANY=K: also prove K proofs, negate A in every other one, and compare Groth16::verify_many's verdicts with
 //       verify_with_processed_vk called per proof (timing both)
+//       B2G_VERIFY_BATCH=K: also prove K proofs and compare Groth16::verify_batch's verdict, on them and with the last
+//       proof's A negated, with verify_with_processed_vk over every proof (timing the batch call)
 //       chain:<a> = the witness of the reference's squaring-chain bench family for input a
 //       (test-vectors/complex-circuit/input.json has a = 3), computed on the host instead of by WASM.
 #include <chrono>
@@ -228,6 +230,39 @@ int main(int argc, char** argv) {
             const double host_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t2).count();
             std::printf("verify_many %d proofs (%d valid): agree=%d, device %.3f ms/batch (%.1f proofs/s), host verify_with_processed_vk "
                         "%.3f ms/proof on one core (%.1f proofs/s)\n", k, valid, agree, dev_ms, k / (dev_ms / 1e3), host_ms / k, k / (host_ms / 1e3));
+        }
+        if (const char* vb = std::getenv("B2G_VERIFY_BATCH")) {          // one batch verdict against the host verifier
+            const int k = std::atoi(vb);
+            if (k < 1) throw SynthesisError("B2G_VERIFY_BATCH must be >= 1");
+            std::vector<std::vector<Fr>> wv((size_t)k, full_assignment);
+            if (wsrc.rfind("chain:", 0) == 0)
+                for (int i = 1; i < k; i++) wv[(size_t)i] = chain_witness(params.a_query.size(), std::stoull(wsrc.substr(6)) + (unsigned long long)i);
+            std::vector<const std::vector<Fr>*> ws;
+            for (const auto& w : wv) ws.push_back(&w);
+            std::mt19937_64 rng(0xBA7C);
+            std::vector<std::pair<Fr, Fr>> rs;
+            for (int i = 0; i < k; i++) rs.push_back({Fr::rand(rng), Fr::rand(rng)});
+            std::vector<Proof> proofs = Groth16::create_proofs(params, matrices, rs, ws);
+            std::vector<std::vector<Fr>> inputs;
+            for (const auto& w : wv) inputs.emplace_back(w.begin() + 1, w.begin() + num_inputs);
+            auto pvk = Groth16::process_vk(params.vk);
+            const bool valid = Groth16::verify_batch(pvk, inputs, proofs);      // also loads the key on the device
+            auto t1 = std::chrono::steady_clock::now();
+            const bool again = Groth16::verify_batch(pvk, inputs, proofs);
+            const double dev_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t1).count();
+            std::vector<Proof> bad = proofs;                                 // the last proof's A -> -A: y -> p - y
+            uint64_t y[4], d[4]; memcpy(y, bad.back().bytes + 32, 32);
+            unsigned __int128 borrow = 0;
+            for (int j = 0; j < 4; j++) { unsigned __int128 t = (unsigned __int128)detail::FQ_P[j] - y[j] - borrow; d[j] = (uint64_t)t; borrow = (t >> 64) & 1; }
+            memcpy(bad.back().bytes + 32, d, 32);
+            const bool tampered = Groth16::verify_batch(pvk, inputs, bad);
+            bool host = true, host_bad = true;
+            for (int i = 0; i < k; i++) {
+                host = host && Groth16::verify_with_processed_vk(pvk, inputs[(size_t)i], proofs[(size_t)i]);
+                host_bad = host_bad && Groth16::verify_with_processed_vk(pvk, inputs[(size_t)i], bad[(size_t)i]);
+            }
+            std::printf("verify_batch %d proofs: valid=%d tampered=%d host=%d/%d agree=%d, device %.3f ms/batch (%.1f proofs/s)\n", k,
+                        valid && again, tampered, host, host_bad, (valid && again) == host && tampered == host_bad, dev_ms, k / (dev_ms / 1e3));
         }
         return 0;
     } catch (const std::exception& e) {

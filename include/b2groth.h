@@ -17,6 +17,7 @@
  *   b2g_vk_load            <- GrothBn::process_vk(&params.vk) (src/zkey.rs:868, 914): the prepared verifying key, on the device
  *   b2g_verify_many        <- GrothBn::verify_with_processed_vk(&pvk, &inputs, &proof) (src/zkey.rs:869-870, 915-916), called
  *                             for many proofs of one key in one device pass
+ *   b2g_verify_batch       <- the same check for a whole batch at once, as one random linear combination of the proofs
  *   b2g_fixed_base_g1/g2   <- the batch fixed-base multiplications of generate_random_parameters_with_reduction
  *                             (tests/groth16.rs:25); used to manufacture synthetic proving keys
  *
@@ -222,6 +223,26 @@ B2G_API int b2g_vk_alpha_beta(b2g_vk* vk, void* out);
 B2G_API int b2g_verify_many(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs,
                             uint8_t* verdicts_out);
 
+/* b2g_verify_batch: whether ALL count proofs are valid, from one random-linear-combination pairing check, for callers that
+ * only need the batch's verdict (an aggregator, a rollup node, a bridge) and fall back to b2g_verify_many when it is 0.
+ * public_inputs and proofs are laid out as for b2g_verify_many; weights = count x 16 B little-endian 128-bit weights r_i;
+ * *verdict_out = 1 or 0.  The verdict is 1 iff every coordinate is below p, every point is on its curve, every B_i not at
+ * infinity lies in G2 (the order-r subgroup of the twist; a proof whose B is outside G2 makes the batch invalid), and
+ *     prod_i e(r_i A_i, B_i) * e(sum_i r_i C_i, -delta) * e(s_0 IC[0] + sum_j s_j IC[j + 1], -gamma) == e(alpha, beta)^s_0
+ * with s_0 = sum_i r_i and s_j = sum_i r_i x_ij (mod r).  A point at infinity contributes 1 to the product, or nothing to a
+ * sum, as in b2g_verify_many.
+ * Soundness: for given weights the verdict is deterministic.  If every proof is valid under b2g_verify_many and every B is in
+ * G2, the verdict is always 1; otherwise it is 0 except with probability at most 1 / (2^128 - 1) over uniformly drawn nonzero
+ * weights.  This holds only if the weights are drawn AFTER the proofs are fixed, from a source the prover cannot predict or
+ * influence (a CSPRNG); with weights the prover knows, invalid proofs can be made to cancel.
+ * Cost: per proof a one-pair Miller loop, two 128-bit G1 products and a G2 membership test; the prepared pairs, the final
+ * exponentiation and the public-input products are paid once per batch.  No per-(proof, input) G1 records are allocated.
+ * Synchronous.  Errors as b2g_verify_many (B2G_E_SHAPE for count == 0, null pointers, a key of another device or a pending
+ * proof; B2G_E_INPUT for a public input >= r; B2G_E_DEVICE when the buffers do not fit), plus B2G_E_INPUT for a zero weight;
+ * every error leaves the context usable. */
+B2G_API int b2g_verify_batch(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs,
+                             const void* weights, uint8_t* verdict_out);
+
 /* Kernel-level entry points (parity tests, benchmarks). All pointers host. */
 B2G_API int b2g_msm_g1(b2g_ctx* ctx, const void* bases, const void* scalars, size_t n, int scalars_mont, void* out_xy_mont);
 B2G_API int b2g_msm_g2(b2g_ctx* ctx, const void* bases, const void* scalars, size_t n, int scalars_mont, void* out_xy_mont);
@@ -250,6 +271,10 @@ B2G_API int b2g_fixed_base_g2(b2g_ctx* ctx, const void* scalars_canon, size_t n,
  *     40 Miller loop of the pair (a, b) without the final exponentiation (a: G1, b: G2 affine),
  *     41 / 42 one projective doubling / addition of b (G2 affine) step on the twist point a = X || Y || Z (3 x 64 B):
  *        out = the new X || Y || Z followed by the line's c0 || c1 || c2.
+ * Ops 43-45 are the batch check's pieces:
+ *     43 G2 membership of a (128 B G2 affine, on the twist): out = 8 B, 1 if a is in G2 (or infinity), else 0,
+ *     44 r * a for a G1 affine a (64 B) and a 128-bit r (b: 16 B little-endian): out = 64 B affine,
+ *     45 a^k for a cyclotomic Fq12 a and a canonical 256-bit k (b: 32 B): out = 384 B.
  * Operand and result sizes per row therefore differ by op; b may be NULL where the op does not read it. */
 B2G_API int b2g_test_op(b2g_ctx* ctx, int op, const void* a, const void* b, size_t n, void* out);
 
