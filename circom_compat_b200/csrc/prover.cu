@@ -4,7 +4,8 @@
 // benches/groth16.rs:52-61; body restated in SURVEY.md 3.3/3.4):
 //     stream 0: H2D witness -> sparse mat-vec -> iNTT/coset/NTT -> h (stays in HBM) -> MSM over h_query
 //     streams 1..4: MSMs over l_query / a_query[1..] / b_g1_query[1..] / b_g2_query[1..] against the witness
-//     stream 0: glue (r*delta, s*delta, vk terms, s*A + r*B1 - rs*delta + L + H, three affine conversions) -> D2H 256 B
+//     streams 2, 3: s*msm_A, r*msm_B1 right behind those MSMs; side stream: r*delta1, s*delta2, K_C (the (r, s)-only terms)
+//     stream 0: glue (A, B2 and C = K_C + s*msm_A + r*msm_B1 + msm_L + msm_H, three affine conversions) -> D2H 256 B
 #include <atomic>
 #include <chrono>
 #include <cstring>
@@ -52,7 +53,7 @@ struct b2g_ctx {
     uint8_t* d_partial = nullptr;        // REC_BYTES: the public partial [H, L, A, B1] G1 XYZZ + B2 G2 XYZZ (768 B), then [s*A, r*B1]
     uint8_t* d_partials_all = nullptr;   // up to 64 ranks x REC_BYTES
     uint8_t* d_proof = nullptr;          // 256 B
-    uint8_t* d_pre = nullptr;            // glue precomputation: r*d1, s*d1, rs*d1, K_C (G1 XYZZ) + s*d2 (G2 XYZZ)
+    uint8_t* d_pre = nullptr;            // glue precomputation: r*d1, K_C (G1 XYZZ) + s*d2 (G2 XYZZ)
     fe *d_w = nullptr, *d_a = nullptr, *d_b = nullptr, *d_c = nullptr, *d_h = nullptr;   // batch: assignments n_vars apart, vectors n apart
     fe* d_wb = nullptr; size_t cap_wb = 0;     // gathered scalars of a sparse B query (b2g_pk::d_bidx), b_compact apart
     cudaEvent_t ev_sortb = nullptr; bool scratch_bsort = false;
@@ -60,7 +61,8 @@ struct b2g_ctx {
     float last_ms[16] = {};
     bool pre_valid = false; uint32_t pre_r[8] = {}, pre_s[8] = {};   // (r, s) whose glue_pre result sits in d_pre
     uint8_t *d_rs = nullptr, *h_rs = nullptr;  // r | s (canonical, 2 x 32 B): device copy read by the glue kernels, pinned staging
-    uint8_t *h_proof = nullptr, *pending_out = nullptr;   // pinned landing slot of the proof bytes; caller's buffer of a submitted proof
+    uint8_t *h_proof = nullptr, *pending_out = nullptr;   // pinned landing slot of the proof bytes; caller's buffer of submitted proofs
+    uint32_t pending_count = 0;                           // proofs pending_out receives
     // One proof's whole device pipeline (all streams, ~100 launches) captured once per (key, matrices) as a CUDA graph and
     // replayed with a single launch: the host cost of a proof drops from ~130 driver calls to a handful (B2G_GRAPH=0 disables)
     bool use_graph = true;
@@ -116,27 +118,27 @@ struct Scalar256 { uint32_t l[8]; };
 CtxView ctx_view(b2g_ctx* ctx) { return {ctx->device, ctx->st[0], ctx->pending_out != nullptr, &ctx->vbufs}; }
 
 // ------------------------------------------------------------------------------------------------ glue kernels
-// pre[0] = r*delta1, pre[1] = s*delta1, pre[2] = (r*s)*delta1, pre[3] = K_C = s*(alpha1 + a_query[0]) + r*(beta1 + b_g1_query[0])
-// + (r*s)*delta1 (G1 XYZZ, 128 B each); then s*delta2 (G2 XYZZ, 256 B).  Every base here is fixed per key: its 8-bit window
-// table is built at b2g_pk_load, so each product is 32 table look-ups and a 5-level tree inside one warp instead of a
-// 254-step double-and-add on one thread.  K_C is what is left of C = s*A + r*B1 - rs*delta1 + L + H once the MSM results
-// are taken out:  C = K_C + s*msm_A + r*msm_B1 + msm_L + msm_H  (A = alpha + a0 + msm_A + r*delta1, B1 likewise).
+// pre[0] = r*delta1, pre[1] = K_C = (r*s)*delta1 + s*(alpha1 + a_query[0]) + r*(beta1 + b_g1_query[0]) (G1 XYZZ, 128 B
+// each); then s*delta2 (G2 XYZZ, 256 B).  Every base here is fixed per key: its 8-bit window table is built at b2g_pk_load,
+// so each product is 32 table look-ups and a 5-level tree inside one warp instead of a 254-step double-and-add on one
+// thread.  K_C is what is left of C = s*A + r*B1 - rs*delta1 + L + H once the MSM results are taken out:
+// C = K_C + s*msm_A + r*msm_B1 + msm_L + msm_H  (A = alpha + a0 + msm_A + r*delta1, B1 likewise).
 // One CTA per proof of a batch: CTA j reads (r, s) at rs[2j], rs[2j + 1] and writes pre + j * PRE_BYTES.
-constexpr size_t PRE_BYTES = 4 * 128 + 256;
-__global__ void __launch_bounds__(192) glue_pre_kernel(const void* __restrict__ tab_d1, const void* __restrict__ tab_d2, const void* __restrict__ tab_aa,
+constexpr size_t PRE_BYTES = 2 * 128 + 256;
+__global__ void __launch_bounds__(160) glue_pre_kernel(const void* __restrict__ tab_d1, const void* __restrict__ tab_d2, const void* __restrict__ tab_aa,
                                                        const void* __restrict__ tab_bb, const Scalar256* __restrict__ rs, uint8_t* __restrict__ pre) {
-    __shared__ G1::Pt sh1[5][32];
+    __shared__ G1::Pt sh1[4][32];
     __shared__ G2::Pt sh2[32];
-    __shared__ G1::Pt res[5];
+    __shared__ G1::Pt res[4];
     rs += 2 * blockIdx.x;
     pre += (size_t)blockIdx.x * PRE_BYTES;
     const Scalar256 r = rs[0], s = rs[1];
     const int warp = threadIdx.x >> 5;
     const bool lead = (threadIdx.x & 31) == 0;
-    if (warp < 5) {
-        // warp 0: r*d1   1: s*d1   2: rs*d1   3: s*(alpha + a0)   4: r*(beta1 + b0)
-        Scalar256 k = (warp == 0 || warp == 4) ? r : s;
-        if (warp == 2) {
+    if (warp < 4) {
+        // warp 0: r*d1   1: rs*d1   2: s*(alpha + a0)   3: r*(beta1 + b0)
+        Scalar256 k = (warp == 0 || warp == 3) ? r : s;
+        if (warp == 1) {
             fe rc, sc;                                   // Scalar256 is only 4-byte aligned: copy limb by limb
             #pragma unroll
             for (int i = 0; i < 8; i++) { rc.l[i] = r.l[i]; sc.l[i] = s.l[i]; }
@@ -145,28 +147,29 @@ __global__ void __launch_bounds__(192) glue_pre_kernel(const void* __restrict__ 
             #pragma unroll
             for (int i = 0; i < 8; i++) k.l[i] = rs_.l[i];
         }
-        const void* tab = warp < 3 ? tab_d1 : (warp == 3 ? tab_aa : tab_bb);
+        const void* tab = warp < 2 ? tab_d1 : (warp == 2 ? tab_aa : tab_bb);
         G1::Pt p = warp_fixed_mul<G1, Fq>(tab, k.l, sh1[warp]);
-        if (lead) { res[warp] = p; if (warp < 3) pt_store<Fq>(pre, warp, p); }
+        if (lead) { res[warp] = p; if (warp == 0) pt_store<Fq>(pre, 0, p); }
     } else {
         G2::Pt p = warp_fixed_mul<G2, Fq2>(tab_d2, s.l, sh2);
-        if (lead) pt_store<Fq2>(pre + 4 * 128, 0, p);
+        if (lead) pt_store<Fq2>(pre + 2 * 128, 0, p);
     }
     __syncthreads();
     if (threadIdx.x == 0) {
-        G1::Pt kc = res[2];
+        G1::Pt kc = res[1];
+        G1::add(kc, res[2]);
         G1::add(kc, res[3]);
-        G1::add(kc, res[4]);
-        pt_store<Fq>(pre, 3, kc);
+        pt_store<Fq>(pre, 1, kc);
     }
 }
 
-// out = k * p for one XYZZ point (the partial A / B1 MSM result of this rank) - issued on that MSM's own stream as soon as
-// it finishes, so the two variable-base scalar multiplications of the proof overlap the longest MSM instead of following it.
-// CTA j of a batch: pt and out in record j (REC_BYTES apart), k = the scalar of proof j (r, s pairs: 2 apart).
-__global__ void scale_partial_kernel(const uint8_t* __restrict__ pt, const Scalar256* __restrict__ k, uint8_t* __restrict__ out) {
+// out = k * p for one XYZZ point (the partial A / B1 MSM result of a rank) - in a whole proof issued on that MSM's own stream
+// as soon as it finishes, so the two variable-base scalar multiplications of the proof overlap the longest MSM instead of
+// following it.  CTA j: pt and out in record j (REC_BYTES apart), k at k + j * kstep (2 for the proofs of a batch, whose
+// (r, s) pairs are 2 apart; 0 for the rank records of one proof, which share one (r, s)).
+__global__ void scale_partial_kernel(const uint8_t* __restrict__ pt, const Scalar256* __restrict__ k, uint8_t* __restrict__ out, int kstep) {
     if (threadIdx.x != 0) return;
-    pt += blockIdx.x * REC_BYTES; out += blockIdx.x * REC_BYTES; k += 2 * blockIdx.x;
+    pt += blockIdx.x * REC_BYTES; out += blockIdx.x * REC_BYTES; k += kstep * blockIdx.x;
     const Scalar256 kk = *k;
     G1::Pt p = pt_load<Fq>(pt, 0);
     pt_store<Fq>(out, 0, G1::mul_scalar(p, kk.l));       // k == 0 -> infinity (r == 0: B1 drops out, prover.rs)
@@ -174,78 +177,46 @@ __global__ void scale_partial_kernel(const uint8_t* __restrict__ pt, const Scala
 
 __device__ __forceinline__ void store_canon(uint8_t* out, int slot, const fe& v) { fe_store(out + 32 * slot, Fq::to_canonical(v)); }
 
-// partials = count records of `stride` bytes: the 768-byte partial [H, L, A, B1 (G1 XYZZ), B2 (G2 XYZZ)] and, when
-// scaled_off >= 0, [s*A_k, r*B1_k] (G1 XYZZ) at that offset.  Folds them in rank order and assembles the proof
-// (ark-groth16 0.5.0 create_proof_with_assignment).  With the scaled points present no scalar multiplication is left here:
-// A, B2 and C are three independent sums, converted to affine by three warps side by side.
-// CTA j of a batch assembles proof j from its own `count` records, (r, s), precomputation and 256-byte proof slot.
-__global__ void glue_post_kernel(const uint8_t* __restrict__ partials, int count, int stride, int scaled_off, const uint8_t* __restrict__ consts,
-                                 const uint8_t* __restrict__ pre, const Scalar256* __restrict__ rs, uint8_t* __restrict__ proof) {
-    __shared__ G1::Pt shA, shB1, shsA, shrB1;
-    partials += (size_t)blockIdx.x * count * stride;
+// partials = count records of REC_BYTES: the 768-byte partial [H, L, A, B1 (G1 XYZZ), B2 (G2 XYZZ)], then [s*A_k, r*B1_k]
+// (G1 XYZZ, scale_partial_kernel).  Folds them in rank order and assembles the proof (ark-groth16 0.5.0
+// create_proof_with_assignment).  No scalar multiplication is left here: A, B2 and C are three independent sums, converted
+// to affine by three warps side by side.
+// CTA j of a batch assembles proof j from its own `count` records, precomputation and 256-byte proof slot.
+__global__ void glue_post_kernel(const uint8_t* __restrict__ partials, int count, const uint8_t* __restrict__ consts, const uint8_t* __restrict__ pre,
+                                 uint8_t* __restrict__ proof) {
+    partials += (size_t)blockIdx.x * count * REC_BYTES;
     pre += (size_t)blockIdx.x * PRE_BYTES;
-    rs += 2 * blockIdx.x;
     proof += (size_t)blockIdx.x * 256;
-    const Scalar256 r = rs[0], s = rs[1];
     const int warp = threadIdx.x >> 5;
-    const bool lead = (threadIdx.x & 31) == 0;
-    const bool legacy = scaled_off < 0;
-    if (lead && (warp == 0 || (warp == 1 && legacy))) {
-        // A = r*delta1 + a_query[0] + msm_A + alpha1 ;  B1 = s*delta1 + b_g1_query[0] + msm_B1 + beta1
-        G1::Pt acc = pt_load<Fq>(pre, warp);
-        G1::madd(acc, aff_load<Fq>(consts, warp == 0 ? 3 : 4));
-        for (int k = 0; k < count; k++) { G1::Pt q = pt_load<Fq>(partials + (size_t)k * stride + (warp == 0 ? 256 : 384), 0); G1::add(acc, q); }
-        G1::madd(acc, aff_load<Fq>(consts, warp == 0 ? 0 : 1));
-        if (warp == 0) shA = acc; else shB1 = acc;
-        if (warp == 0 && !legacy) {
-            G1::Aff a = G1::to_affine(acc);
-            store_canon(proof, 0, a.x); store_canon(proof, 1, a.y);
-        }
-    }
-    if (lead && warp == 1 && !legacy) {
+    if ((threadIdx.x & 31) != 0) return;
+    if (warp == 0) {
+        // A = r*delta1 + a_query[0] + msm_A + alpha1
+        G1::Pt acc = pt_load<Fq>(pre, 0);
+        G1::madd(acc, aff_load<Fq>(consts, 3));
+        for (int k = 0; k < count; k++) { G1::Pt q = pt_load<Fq>(partials + (size_t)k * REC_BYTES + 256, 0); G1::add(acc, q); }
+        G1::madd(acc, aff_load<Fq>(consts, 0));
+        G1::Aff a = G1::to_affine(acc);
+        store_canon(proof, 0, a.x); store_canon(proof, 1, a.y);
+    } else if (warp == 1) {
         // C = K_C + sum_k (s*A_k + r*B1_k + L_k + H_k)
-        G1::Pt acc = pt_load<Fq>(pre, 3);
+        G1::Pt acc = pt_load<Fq>(pre, 1);
         for (int k = 0; k < count; k++) {
-            const uint8_t* rec = partials + (size_t)k * stride;
-            G1::Pt q = pt_load<Fq>(rec + scaled_off, 0); G1::add(acc, q);
-            q = pt_load<Fq>(rec + scaled_off + 128, 0); G1::add(acc, q);
+            const uint8_t* rec = partials + (size_t)k * REC_BYTES;
+            G1::Pt q = pt_load<Fq>(rec + B2G_PARTIAL_BYTES, 0); G1::add(acc, q);
+            q = pt_load<Fq>(rec + B2G_PARTIAL_BYTES + 128, 0); G1::add(acc, q);
             q = pt_load<Fq>(rec + 128, 0); G1::add(acc, q);
             q = pt_load<Fq>(rec, 0); G1::add(acc, q);
         }
         G1::Aff c = G1::to_affine(acc);
         store_canon(proof, 6, c.x); store_canon(proof, 7, c.y);
-    }
-    if (lead && warp == 2) {
+    } else {
         // B2 = s*delta2 + b_g2_query[0] + msm_B2 + beta2
-        G2::Pt acc = pt_load<Fq2>(pre + 4 * 128, 0);
+        G2::Pt acc = pt_load<Fq2>(pre + 2 * 128, 0);
         G2::madd(acc, aff_load<Fq2>(consts + 5 * 64, 2));
-        for (int k = 0; k < count; k++) { G2::Pt q = pt_load<Fq2>(partials + (size_t)k * stride + 512, 0); G2::add(acc, q); }
+        for (int k = 0; k < count; k++) { G2::Pt q = pt_load<Fq2>(partials + (size_t)k * REC_BYTES + 512, 0); G2::add(acc, q); }
         G2::madd(acc, aff_load<Fq2>(consts + 5 * 64, 0));
         G2::Aff b = G2::to_affine(acc);
         store_canon(proof, 2, b.x.c0); store_canon(proof, 3, b.x.c1); store_canon(proof, 4, b.y.c0); store_canon(proof, 5, b.y.c1);
-    }
-    if (!legacy) return;
-    // host-mediated exchange (b2g_prove_partial / b2g_prove_finish): r, s may only arrive now, the scalar multiplications are done here
-    __syncthreads();
-    if (lead && warp == 0) shsA = G1::mul_scalar(shA, s.l);
-    if (lead && warp == 1) shrB1 = G1::mul_scalar(shB1, r.l);            // r == 0 -> infinity: B1 is skipped (prover.rs)
-    if (lead && warp == 3) {
-        G1::Aff a = G1::to_affine(shA);
-        store_canon(proof, 0, a.x); store_canon(proof, 1, a.y);
-    }
-    __syncthreads();
-    if (lead && warp == 0) {
-        // C = s*A + r*B1 - (r*s)*delta1 + msm_L + msm_H
-        G1::Pt acc = shsA;
-        G1::add(acc, shrB1);
-        G1::Pt rsd = G1::neg(pt_load<Fq>(pre, 2));
-        G1::add(acc, rsd);
-        for (int k = 0; k < count; k++) {
-            G1::Pt l = pt_load<Fq>(partials + (size_t)k * stride + 128, 0); G1::add(acc, l);
-            G1::Pt h = pt_load<Fq>(partials + (size_t)k * stride, 0); G1::add(acc, h);
-        }
-        G1::Aff c = G1::to_affine(acc);
-        store_canon(proof, 6, c.x); store_canon(proof, 7, c.y);
     }
 }
 
@@ -686,7 +657,7 @@ static void launch_msms(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, bool timed, bool
         msm_accumulate(pk->plan[q], on_b ? ctx->scratch[Q_B1] : ctx->scratch[Q_L], ctx->scratch[q], ctx->st[q]);
         if (scale && (q == Q_A || q == Q_B1)) {
             const Scalar256* rs = reinterpret_cast<const Scalar256*>(ctx->d_rs);
-            scale_partial_kernel<<<count, 32, 0, ctx->st[q]>>>(ctx->d_partial + PARTIAL_OFF[q], q == Q_A ? rs + 1 : rs, ctx->d_partial + B2G_PARTIAL_BYTES + (q == Q_A ? 0 : 128));
+            scale_partial_kernel<<<count, 32, 0, ctx->st[q]>>>(ctx->d_partial + PARTIAL_OFF[q], q == Q_A ? rs + 1 : rs, ctx->d_partial + B2G_PARTIAL_BYTES + (q == Q_A ? 0 : 128), 2);
             g_launch_count += 1;
         }
         if (timed) CUDA_CHECK(cudaEventRecord(ctx->ev_t[2 * q + 1], ctx->st[q]));
@@ -727,23 +698,21 @@ static void stage_rs(b2g_ctx* ctx, const void* r, const void* s, uint32_t count 
     memcpy(ctx->pre_r, r, 32); memcpy(ctx->pre_s, s, 32);
 }
 
-// r*delta1, s*delta1, rs*delta1, s*delta2 depend only on (r, s): forked from stream 0 (after d_rs is written and after the
-// previous proof's assembly has read d_pre) onto a side stream, so they overlap the MSMs
+// r*delta1, K_C and s*delta2 depend only on (r, s): forked from stream 0 (after d_rs is written and after the previous
+// proof's assembly has read d_pre) onto a side stream, so they overlap the MSMs
 static void launch_glue_pre(b2g_ctx* ctx, b2g_pk* pk, uint32_t count = 1) {
     CUDA_CHECK(cudaEventRecord(ctx->ev_fork, ctx->st[0]));
     CUDA_CHECK(cudaStreamWaitEvent(ctx->st_glue, ctx->ev_fork, 0));
-    glue_pre_kernel<<<count, 192, 0, ctx->st_glue>>>(pk->d_tab_delta1, pk->d_tab_delta2, pk->d_tab_aa, pk->d_tab_bb, reinterpret_cast<const Scalar256*>(ctx->d_rs), ctx->d_pre);
+    glue_pre_kernel<<<count, 160, 0, ctx->st_glue>>>(pk->d_tab_delta1, pk->d_tab_delta2, pk->d_tab_aa, pk->d_tab_bb, reinterpret_cast<const Scalar256*>(ctx->d_rs), ctx->d_pre);
     CUDA_CHECK(cudaEventRecord(ctx->ev_pre, ctx->st_glue));
     ctx->pre_valid = true;
     g_launch_count += 1;
 }
 
-// scaled = true: records of REC_BYTES with [s*A_k, r*B1_k] behind the partial; false: bare 768-byte partials (host-mediated exchange).
-// nproofs > 1: proofs of a batch, each assembled from its own `count` records
-static void launch_glue_post(b2g_ctx* ctx, b2g_pk* pk, const uint8_t* partials_dev, int count, bool scaled, cudaStream_t st, uint32_t nproofs = 1) {
+// partials_dev: `count` records of REC_BYTES per proof; nproofs > 1: proofs of a batch, each assembled from its own records
+static void launch_glue_post(b2g_ctx* ctx, b2g_pk* pk, const uint8_t* partials_dev, int count, cudaStream_t st, uint32_t nproofs = 1) {
     CUDA_CHECK(cudaStreamWaitEvent(st, ctx->ev_pre, 0));
-    glue_post_kernel<<<nproofs, 128, 0, st>>>(partials_dev, count, scaled ? (int)REC_BYTES : B2G_PARTIAL_BYTES, scaled ? B2G_PARTIAL_BYTES : -1, pk->d_consts, ctx->d_pre,
-                                        reinterpret_cast<const Scalar256*>(ctx->d_rs), ctx->d_proof);
+    glue_post_kernel<<<nproofs, 96, 0, st>>>(partials_dev, count, pk->d_consts, ctx->d_pre, ctx->d_proof);
     g_launch_count += 1;
     CUDA_CHECK(cudaGetLastError());
 }
@@ -763,9 +732,9 @@ static void enqueue_proof(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, int kind, bool
         xchg_publish_kernel<<<1, 64, 0, s0>>>(ctx->d_partial, ctx->d_xchg, ctx->d_epoch);
         xchg_gather_kernel<<<ctx->shard_count, 64, 0, s0>>>(ctx->d_peer_ptrs, ctx->shard_count, ctx->d_epoch, ctx->d_partials_all, p2p_timeout_ns(), d_flag);
         g_launch_count += 2;
-        launch_glue_post(ctx, pk, ctx->d_partials_all, ctx->shard_count, true, s0);
+        launch_glue_post(ctx, pk, ctx->d_partials_all, ctx->shard_count, s0);
     } else {
-        launch_glue_post(ctx, pk, ctx->d_partial, 1, true, s0, count);
+        launch_glue_post(ctx, pk, ctx->d_partial, 1, s0, count);
     }
 }
 
@@ -1073,6 +1042,7 @@ int b2g_witness_map(b2g_ctx* ctx, b2g_mat* mat, const void* w_mont, void* h_out,
     });
 }
 
+// prologue of the shard entry points (b2g_prove_partial, b2g_prove_sharded_p2p): checks, buffers of one proof, witness upload
 static void prove_common(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, const void* w_mont, bool slice_only = false) {
     check_shapes(ctx, pk, mat);
     if (!w_mont) throw_error(B2G_E_SHAPE, "null witness");
@@ -1092,23 +1062,48 @@ static double host_ms_since(const std::chrono::steady_clock::time_point& t0) {
     return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
 }
 
-// enqueue one whole proof; nothing here waits for the device (the witness must be page-locked for the upload to be
-// asynchronous too; the 256 proof bytes come back through the context's own pinned slot)
-static void prove_submit(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, const void* r_canon, const void* s_canon, const void* w_mont, uint8_t* proof_out) {
-    if (!ctx || !r_canon || !s_canon || !proof_out) throw_error(B2G_E_SHAPE, "null pointer");
-    if (ctx->shard_count != 1) throw_error(B2G_E_SHAPE, "b2g_prove needs an unsharded context; use b2g_prove_partial/finish");
+// enqueue `count` whole proofs of one circuit (r_j, s_j 32 B apart, witness j at w_mont[j]); nothing here waits for the
+// device (the witnesses must be page-locked for the upload to be asynchronous too).  The proof bytes come back through the
+// context's own pinned slot; prove_wait copies them to proofs_out.
+static void prove_submit(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, uint32_t count, const void* r_canon, const void* s_canon, const void* const* w_mont,
+                         uint8_t* proofs_out) {
+    if (!ctx || !r_canon || !s_canon || !w_mont || !proofs_out) throw_error(B2G_E_SHAPE, "null pointer");
+    if (ctx->shard_count != 1) throw_error(B2G_E_SHAPE, "a whole proof (b2g_prove, b2g_prove_many) needs an unsharded context; use b2g_prove_partial/finish");
     if (ctx->pending_out) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
+    if (count == 0 || count > MAX_BATCH) throw_error(B2G_E_SHAPE, "b2g_prove_many: count must be in [1, " + std::to_string(MAX_BATCH) + "]");
+    for (uint32_t j = 0; j < count; j++) if (!w_mont[j]) throw_error(B2G_E_SHAPE, "null witness " + std::to_string(j));
     const auto t0 = std::chrono::steady_clock::now();
     check_shapes(ctx, pk, mat);
-    prove_common(ctx, pk, mat, w_mont);
-    stage_rs(ctx, r_canon, s_canon);
-    ctx->last_ms[9] = (float)host_ms_since(t0);
+    // the sorted entries and bucket keys of a whole batch are u32 positions into one list
+    for (int q = 0; q < NQ; q++) {
+        const MsmPlan& p = pk->plan[q];
+        if (!p.table) continue;
+        if ((uint64_t)count * p.n * p.nwin >= (1ull << 32) || (uint64_t)count * p.nbuckets >= (1ull << 32))
+            throw_error(B2G_E_SHAPE, "b2g_prove_many: count x bases x windows of a query reaches 2^32 sorted entries; prove fewer per call");
+    }
+    try {
+        ensure_witness_buffers(ctx, mat->n_vars, mat->n, count);
+        ensure_batch_buffers(ctx, count);
+        ensure_scratch(ctx, pk, count);
+    } catch (const B2gError& e) {
+        if (e.code != B2G_E_DEVICE) throw;
+        cudaGetLastError();
+        throw_error(B2G_E_DEVICE, "the device buffers of " + std::to_string(count) + " proof(s) do not fit in device memory" +
+                                  (count > 1 ? "; prove fewer per call (" : " (") + e.what() + ")");
+    }
     cudaStream_t s0 = ctx->st[0];
-    run_proof(ctx, pk, mat, 0);
+    CUDA_CHECK(cudaEventRecord(ctx->ev_t[12], s0));
+    for (uint32_t j = 0; j < count; j++)
+        CUDA_CHECK(cudaMemcpyAsync(ctx->d_w + (size_t)j * mat->n_vars, w_mont[j], (size_t)mat->n_vars * 32, cudaMemcpyHostToDevice, s0));
+    CUDA_CHECK(cudaEventRecord(ctx->ev_t[13], s0));
+    stage_rs(ctx, r_canon, s_canon, count);
+    ctx->last_ms[9] = (float)host_ms_since(t0);
+    run_proof(ctx, pk, mat, 0, count);
     ctx->pre_valid = false;
-    CUDA_CHECK(cudaMemcpyAsync(ctx->h_proof, ctx->d_proof, 256, cudaMemcpyDeviceToHost, s0));
+    CUDA_CHECK(cudaMemcpyAsync(ctx->h_proof, ctx->d_proof, (size_t)count * 256, cudaMemcpyDeviceToHost, s0));
     CUDA_CHECK(cudaEventRecord(ctx->ev_t[15], s0));
-    ctx->pending_out = proof_out;
+    ctx->pending_out = proofs_out;
+    ctx->pending_count = count;
     ctx->last_ms[10] = (float)host_ms_since(t0);
 }
 
@@ -1119,7 +1114,7 @@ static void prove_wait(b2g_ctx* ctx) {
     uint8_t* out = ctx->pending_out;
     ctx->pending_out = nullptr;
     CUDA_CHECK(cudaStreamSynchronize(ctx->st[0]));
-    memcpy(out, ctx->h_proof, 256);
+    memcpy(out, ctx->h_proof, (size_t)ctx->pending_count * 256);
     ctx->last_ms[11] = (float)host_ms_since(t0);
     collect_timings(ctx);
 }
@@ -1128,7 +1123,7 @@ int b2g_prove(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, const void* r_canon, const
     return guarded([&] {
         if (!ctx) throw_error(B2G_E_SHAPE, "null pointer");
         DevGuard g(ctx->device);
-        prove_submit(ctx, pk, mat, r_canon, s_canon, w_mont, proof_out);
+        prove_submit(ctx, pk, mat, 1, r_canon, s_canon, &w_mont, proof_out);
         prove_wait(ctx);
     });
 }
@@ -1137,50 +1132,17 @@ int b2g_prove_submit(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, const void* r_canon
     return guarded([&] {
         if (!ctx) throw_error(B2G_E_SHAPE, "null pointer");
         DevGuard g(ctx->device);
-        prove_submit(ctx, pk, mat, r_canon, s_canon, w_mont, proof_out);
+        prove_submit(ctx, pk, mat, 1, r_canon, s_canon, &w_mont, proof_out);
     });
 }
 
 int b2g_prove_many(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, uint32_t count, const void* r_canon, const void* s_canon, const void* const* w_mont,
                    uint8_t* proofs_out) {
     return guarded([&] {
-        if (!ctx || !r_canon || !s_canon || !w_mont || !proofs_out) throw_error(B2G_E_SHAPE, "null pointer");
-        if (ctx->shard_count != 1) throw_error(B2G_E_SHAPE, "b2g_prove_many needs an unsharded context");
-        if (ctx->pending_out) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
-        if (count == 0 || count > MAX_BATCH) throw_error(B2G_E_SHAPE, "b2g_prove_many: count must be in [1, " + std::to_string(MAX_BATCH) + "]");
-        for (uint32_t j = 0; j < count; j++) if (!w_mont[j]) throw_error(B2G_E_SHAPE, "null witness " + std::to_string(j));
-        check_shapes(ctx, pk, mat);
-        // the sorted entries and bucket keys of a whole batch are u32 positions into one list
-        for (int q = 0; q < NQ; q++) {
-            const MsmPlan& p = pk->plan[q];
-            if (!p.table) continue;
-            if ((uint64_t)count * p.n * p.nwin >= (1ull << 32) || (uint64_t)count * p.nbuckets >= (1ull << 32))
-                throw_error(B2G_E_SHAPE, "b2g_prove_many: count x bases x windows of a query reaches 2^32 sorted entries; prove fewer per call");
-        }
+        if (!ctx) throw_error(B2G_E_SHAPE, "null pointer");
         DevGuard g(ctx->device);
-        try {
-            ensure_witness_buffers(ctx, mat->n_vars, mat->n, count);
-            ensure_batch_buffers(ctx, count);
-            ensure_scratch(ctx, pk, count);
-        } catch (const B2gError& e) {
-            if (e.code != B2G_E_DEVICE) throw;
-            cudaGetLastError();
-            throw_error(B2G_E_DEVICE, "b2g_prove_many: the device buffers of " + std::to_string(count) +
-                                      " proofs do not fit in device memory; prove fewer per call (" + e.what() + ")");
-        }
-        cudaStream_t s0 = ctx->st[0];
-        CUDA_CHECK(cudaEventRecord(ctx->ev_t[12], s0));
-        for (uint32_t j = 0; j < count; j++)
-            CUDA_CHECK(cudaMemcpyAsync(ctx->d_w + (size_t)j * mat->n_vars, w_mont[j], (size_t)mat->n_vars * 32, cudaMemcpyHostToDevice, s0));
-        CUDA_CHECK(cudaEventRecord(ctx->ev_t[13], s0));
-        stage_rs(ctx, r_canon, s_canon, count);
-        run_proof(ctx, pk, mat, 0, count);
-        ctx->pre_valid = false;
-        CUDA_CHECK(cudaMemcpyAsync(ctx->h_proof, ctx->d_proof, (size_t)count * 256, cudaMemcpyDeviceToHost, s0));
-        CUDA_CHECK(cudaEventRecord(ctx->ev_t[15], s0));
-        CUDA_CHECK(cudaStreamSynchronize(s0));
-        memcpy(proofs_out, ctx->h_proof, (size_t)count * 256);
-        collect_timings(ctx);
+        prove_submit(ctx, pk, mat, count, r_canon, s_canon, w_mont, proofs_out);
+        prove_wait(ctx);
     });
 }
 
@@ -1214,7 +1176,6 @@ int b2g_prove_partial(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, const void* r_cano
     return guarded([&] {
         if (!ctx || !pk || !partial_out) throw_error(B2G_E_SHAPE, "null pointer");
         DevGuard g(ctx->device);
-        check_shapes(ctx, pk, mat);
         ctx->pre_valid = false;
         prove_common(ctx, pk, mat, w_mont);
         if (r_canon && s_canon) { stage_rs(ctx, r_canon, s_canon); launch_glue_pre(ctx, pk); }
@@ -1238,8 +1199,19 @@ int b2g_prove_finish(b2g_ctx* ctx, b2g_pk* pk, const void* partials_all, int cou
         cudaStream_t s0 = ctx->st[0];
         if (!(ctx->pre_valid && !memcmp(ctx->pre_r, r_canon, 32) && !memcmp(ctx->pre_s, s_canon, 32))) { stage_rs(ctx, r_canon, s_canon); launch_glue_pre(ctx, pk); }
         ctx->pre_valid = false;
-        CUDA_CHECK(cudaMemcpyAsync(ctx->d_partials_all, partials_all, (size_t)count * B2G_PARTIAL_BYTES, cudaMemcpyHostToDevice, s0));
-        launch_glue_post(ctx, pk, ctx->d_partials_all, count, false, s0);
+        // the records the peer-memory gather writes: each rank's partial, then s*A_k and r*B1_k (all ranks share one (r, s)),
+        // the two products side by side on the A and B1 streams
+        CUDA_CHECK(cudaMemcpy2DAsync(ctx->d_partials_all, REC_BYTES, partials_all, B2G_PARTIAL_BYTES, B2G_PARTIAL_BYTES, count, cudaMemcpyHostToDevice, s0));
+        CUDA_CHECK(cudaEventRecord(ctx->ev_fork, s0));
+        const Scalar256* rs = reinterpret_cast<const Scalar256*>(ctx->d_rs);
+        for (int q : {Q_A, Q_B1}) {
+            CUDA_CHECK(cudaStreamWaitEvent(ctx->st[q], ctx->ev_fork, 0));
+            scale_partial_kernel<<<count, 32, 0, ctx->st[q]>>>(ctx->d_partials_all + PARTIAL_OFF[q], q == Q_A ? rs + 1 : rs, ctx->d_partials_all + B2G_PARTIAL_BYTES + (q == Q_A ? 0 : 128), 0);
+            CUDA_CHECK(cudaEventRecord(ctx->ev_done[q], ctx->st[q]));
+            CUDA_CHECK(cudaStreamWaitEvent(s0, ctx->ev_done[q], 0));
+        }
+        g_launch_count += 2;
+        launch_glue_post(ctx, pk, ctx->d_partials_all, count, s0);
         CUDA_CHECK(cudaMemcpyAsync(proof_out, ctx->d_proof, 256, cudaMemcpyDeviceToHost, s0));
         CUDA_CHECK(cudaStreamSynchronize(s0));
     });
@@ -1334,7 +1306,6 @@ int b2g_prove_sharded_p2p(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, const void* r_
         if (!ctx || !pk || !r_canon || !s_canon || !proof_out) throw_error(B2G_E_SHAPE, "null pointer");
         if (ctx->peers_imported != ctx->shard_count) throw_error(B2G_E_SHAPE, "b2g_p2p_import has not been called with every rank's handle");
         DevGuard g(ctx->device);
-        check_shapes(ctx, pk, mat);
         prove_common(ctx, pk, mat, w_mont, true);
         stage_rs(ctx, r_canon, s_canon);
         cudaStream_t s0 = ctx->st[0];

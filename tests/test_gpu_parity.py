@@ -829,13 +829,28 @@ def _prove_both(ctx, circ, w, r, s, td_seed=7):
 def test_edge_zero_witness_and_zero_blinding(ctx):
     # squaring chain with a = 0: every wire except the constant is 0 -> all MSM scalars but one vanish (empty buckets,
     # infinity partial results); r = s = 0 removes every delta term and skips B1 (prover.rs: r == 0)
-    from circom_compat_b200 import synth
+    from circom_compat_b200 import synth, Groth16, Context, fr_to_mont, release
     circ = synth.chain_circuit(1 << 10)
     w = synth.chain_witness(1 << 10, 0)
     assert w[0] == 1 and not any(w[1:])
-    for r, s in ((0, 0), (0, 5), (7, 0), (o.R_MOD - 1, o.R_MOD - 1)):
+    cases = ((0, 0), (0, 5), (7, 0), (o.R_MOD - 1, o.R_MOD - 1))
+    for r, s in cases:
         p, ref = _prove_both(ctx, circ, w, r, s)
         assert p.data == ref, (r, s)
+    # the same scalars through the host-exchange sharded route: three shard contexts, prove_finish scales every rank's
+    # A / B1 partial itself; with (r, s) given to prove_partial, prove_finish reuses the precomputation started there
+    pk, td = synth.setup(ctx, circ)
+    cm = circ.matrices()
+    wm = fr_to_mont(w)
+    shards = [Context(0, rank, 3) for rank in range(3)]
+    for r, s in cases:
+        ref = c.prove(_oracle_key(pk, cm), r, s, wm)
+        for early in ((None, None), (r, s)):
+            parts = np.stack([Groth16.prove_partial(pk, cm, wm, cx, *early) for cx in shards])
+            assert Groth16.prove_finish(pk, parts, r, s, shards[0]).data == ref, (r, s, early)
+    release(pk); release(cm)
+    for cx in shards:
+        cx.close()
 
 
 def test_edge_no_witness_variables_and_tiny_domains(ctx):
