@@ -529,6 +529,21 @@ struct Fp {
         }
         return acc;
     }
+
+    // a^((p + 1) / 4), a square root of a whenever a has one (p = 3 mod 4: Fq only); is_root tells whether it is one.  The
+    // exponent is (p >> 2) + 1, 252 bits of which 109 are set (Fq): 252 squarings and 109 products, about the cost of inv
+    static __device__ __noinline__ fe sqrt(const fe& a, bool& is_root) {
+        static_assert((P::P0 & 3u) == 3u, "sqrt needs p = 3 (mod 4)");
+        const uint32_t e[8] = {(P::P0 >> 2 | P::P1 << 30) + 1u, P::P1 >> 2 | P::P2 << 30, P::P2 >> 2 | P::P3 << 30, P::P3 >> 2 | P::P4 << 30,
+                               P::P4 >> 2 | P::P5 << 30, P::P5 >> 2 | P::P6 << 30, P::P6 >> 2 | P::P7 << 30, P::P7 >> 2};
+        fe acc = one();
+        for (int i = 251; i >= 0; i--) {
+            acc = sqr(acc);
+            if ((e[i >> 5] >> (i & 31)) & 1u) acc = mul(acc, a);
+        }
+        is_root = eq(sqr(acc), a);
+        return acc;
+    }
 };
 
 using Fq = Fp<FqParams>;
@@ -622,6 +637,31 @@ struct Fq2 {
         fe d = Fq::inv(Fq::add(Fq::sqr(a.c0), Fq::sqr(a.c1)));
         fe2 r; r.c0 = Fq::mul(a.c0, d); r.c1 = Fq::neg(Fq::mul(a.c1, d));
         return r;
+    }
+    // a square root r of a by the norm method; false (r = 0) when a has none.  With delta = (a0 + sqrt(a0^2 + a1^2)) / 2
+    // (delta = a0 when a1 = 0) and s = delta^((p + 1) / 4):
+    //     s^2 = delta    ->  r = s + a1 / (2 s) u
+    //     s^2 = -delta   ->  r = a1 / (2 s) + s u      (then (a0 - sqrt(norm)) / 2 = -a1^2 / (4 delta) is the residue)
+    // so one exponentiation serves both candidates.  A non-residue norm means no root; the result is checked by squaring.
+    // Cost: two Fq exponentiations (one when a1 = 0), one Fq inversion.
+    static __device__ __noinline__ bool sqrt(fe2& r, const fe2& a) {
+        r = zero();
+        fe d = a.c0;
+        bool direct;
+        if (!fe_is_zero(a.c1)) {
+            const fe alpha = Fq::sqrt(Fq::add(Fq::sqr(a.c0), Fq::sqr(a.c1)), direct);
+            if (!direct) return false;
+            fe half;                                                          // 1/2, Montgomery
+            half.l[0] = 0x4f060572u; half.l[1] = 0x87bee7d2u; half.l[2] = 0x2f1c6ae5u; half.l[3] = 0xd0fd2addu;
+            half.l[4] = 0xfcfd4f44u; half.l[5] = 0x8f5f7492u; half.l[6] = 0x3d9cbfacu; half.l[7] = 0x1f37631au;
+            d = Fq::mul(Fq::add(a.c0, alpha), half);
+        }
+        const fe s = Fq::sqrt(d, direct);
+        const fe t = Fq::mul(a.c1, Fq::inv(Fq::dbl(s)));
+        fe2 c; c.c0 = direct ? s : t; c.c1 = direct ? t : s;
+        if (!eq(sqr(c), a)) return false;
+        r = c;
+        return true;
     }
 };
 

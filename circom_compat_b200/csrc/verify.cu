@@ -24,6 +24,10 @@
 //   rhs      one thread: e(alpha, beta)^s_0
 //   final    one thread: one final exponentiation, compared with rhs -> one verdict byte
 // Only prepare -> miller -> product -> final run on the context's stream; the rest runs next to them on two side streams.
+// b2g_proofs_decompress, b2g_verify_many_compressed and b2g_verify_batch_compressed take arkworks' 128-byte compressed
+// proofs: a decode kernel (one proof per thread) writes the 256-byte rows the kernels above read, and a second kernel checks
+// that each decoded B lies in G2 (b2g_verify_batch leaves that to batch_g2_kernel).  The decoding rules are restated above
+// decompress_kernel.
 #include <algorithm>
 #include <cstring>
 #include <string>
@@ -60,10 +64,11 @@ namespace b2g {
 constexpr size_t REC_BYTES_V = 384, REC_OK = 320;
 
 struct VerifyBufs {
-    size_t cap_count = 0, cap_pub = 0, cap_part = 0, cap_batch = 0;
+    size_t cap_count = 0, cap_pub = 0, cap_part = 0, cap_batch = 0, cap_comp = 0;
     uint8_t *d_proofs = nullptr, *d_rec = nullptr, *d_f = nullptr, *d_verdict = nullptr;   // per proof
     uint8_t *d_pub = nullptr, *d_part = nullptr;                                            // per (proof, input)
     uint8_t* d_batch = nullptr;                   // b2g_verify_batch: weights, reduction levels, scalar sums, tail values
+    uint8_t* d_comp = nullptr;                    // compressed proofs (128 B each), then one decoded-ok byte per proof
     cudaStream_t side[2] = {nullptr, nullptr};    // b2g_verify_batch's tail pieces, next to the per-proof kernels
     cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
 };
@@ -73,7 +78,7 @@ void verify_bufs_free(VerifyBufs* v) {
     for (cudaStream_t s : v->side) if (s) cudaStreamDestroy(s);
     for (cudaEvent_t e : v->ev) if (e) cudaEventDestroy(e);
     for (void* p : {(void*)v->d_proofs, (void*)v->d_rec, (void*)v->d_f, (void*)v->d_verdict, (void*)v->d_pub, (void*)v->d_part,
-                    (void*)v->d_batch}) if (p) cudaFree(p);
+                    (void*)v->d_batch, (void*)v->d_comp}) if (p) cudaFree(p);
     delete v;
 }
 
@@ -322,6 +327,145 @@ __global__ void batch_test_kernel(int op, const uint8_t* __restrict__ a, const u
     }
 }
 
+// ---------------------------------------------------------------------------------------------- compressed proofs
+// Proof::<Bn254>::deserialize_compressed (ark-serialize, ark-ec and ark-ff 0.5, Validate::Yes), restated:
+//   layout    A = bytes 0-31, B = bytes 32-95, C = bytes 96-127, little-endian.  A G1 point is x; a G2 point is x.c0 (no
+//             flags) followed by x.c1.  The flags are the top two bits of the point's last byte (of x, or of x.c1).
+//   flags     bit 7: y is the larger of {y, -y}; bit 6: infinity; both set: invalid (SWFlags::from_u8 gives None)
+//   range     with the flags masked off, every Fq value (x, x.c0, x.c1) is below p, even when the infinity flag is set
+//   infinity  the point is infinity and x is otherwise ignored; decoded as all-zero coordinates, as b2g_prove writes it
+//   otherwise y^2 = x^3 + 3 (G1) or x^3 + 3 / (9 + u) (G2) must have a square root; of the two roots, the smaller one when
+//             bit 7 is clear and the larger one when it is set, in the order of canonical values (Fq2: c1 first, then c0)
+//   subgroup  B is in G2 (G1 has cofactor 1: A and C need no check)
+// An undecodable proof becomes a row of 0xFF bytes: every coordinate is then >= p, so proof_parse refuses it and both
+// verifiers report it invalid with their kernels unchanged.
+constexpr size_t COMP_BYTES = 128;
+
+// the coordinate that carries a point's flags: its value with the flags cleared, flags = bit 7 << 1 | bit 6
+__device__ __forceinline__ fe comp_load(const uint8_t* p, uint32_t& flags) {
+    fe x = fe_load(p);
+    flags = x.l[7] >> 30;
+    x.l[7] &= 0x3fffffffu;
+    return x;
+}
+
+// canonical a > b
+__device__ __forceinline__ bool fe_greater(const fe& a, const fe& b) {
+    for (int i = 7; i >= 0; i--) if (a.l[i] != b.l[i]) return a.l[i] > b.l[i];
+    return false;
+}
+// a canonical y is the larger of {y, -y} (Fq::neg is the same modular subtraction on canonical values)
+__device__ __forceinline__ bool y_is_larger(const fe& y) { return fe_greater(y, Fq::neg(y)); }
+__device__ __forceinline__ bool y_is_larger(const fe2& y) {
+    const fe n1 = Fq::neg(y.c1);
+    return fe_equal(y.c1, n1) ? fe_greater(y.c0, Fq::neg(y.c0)) : fe_greater(y.c1, n1);
+}
+__device__ __forceinline__ fe to_canon(const fe& a) { return Fq::to_canonical(a); }
+__device__ __forceinline__ fe2 to_canon(const fe2& a) { fe2 r; r.c0 = Fq::to_canonical(a.c0); r.c1 = Fq::to_canonical(a.c1); return r; }
+__device__ __forceinline__ fe to_mont(const fe& a) { return Fq::from_canonical(a); }
+__device__ __forceinline__ fe2 to_mont(const fe2& a) { fe2 r; r.c0 = Fq::from_canonical(a.c0); r.c1 = Fq::from_canonical(a.c1); return r; }
+__device__ __forceinline__ bool field_sqrt(fe& r, const fe& a) { bool ok; r = Fq::sqrt(a, ok); return ok; }
+__device__ __forceinline__ bool field_sqrt(fe2& r, const fe2& a) { return Fq2::sqrt(r, a); }
+
+// the canonical y of the point with canonical x on y^2 = x^3 + b, the root the sign flag picks; false when there is none
+template <class F>
+__device__ __forceinline__ bool decompress_y(typename F::elem& y, const typename F::elem& x, bool larger) {
+    const typename F::elem xm = to_mont(x);
+    typename F::elem r;
+    if (!field_sqrt(r, F::add(F::mul(F::sqr(xm), xm), curve_b((const F*)nullptr)))) return false;
+    y = to_canon(r);
+    if (y_is_larger(y) != larger) y = F::neg(y);
+    return true;
+}
+
+// a compressed G1 point (32 B) -> canonical x, y (zeros at infinity); false when it does not decode
+__device__ __forceinline__ bool g1_decompress(fe* out, const uint8_t* p) {
+    uint32_t f;
+    const fe x = comp_load(p, f);
+    if (f == 3 || !fe_below_p(x)) return false;
+    if (f & 1) { out[0] = fe_zero(); out[1] = fe_zero(); return true; }
+    out[0] = x;
+    return decompress_y<Fq>(out[1], x, f & 2);
+}
+
+// a compressed G2 point (64 B) -> canonical x.c0, x.c1, y.c0, y.c1 (zeros at infinity), without the subgroup check
+__device__ __forceinline__ bool g2_decompress(fe* out, const uint8_t* p) {
+    uint32_t f;
+    fe2 x, y;
+    x.c0 = fe_load(p);
+    x.c1 = comp_load(p + 32, f);
+    if (f == 3 || !fe_below_p(x.c0) || !fe_below_p(x.c1)) return false;
+    if (f & 1) { for (int k = 0; k < 4; k++) out[k] = fe_zero(); return true; }
+    if (!decompress_y<Fq2>(y, x, f & 2)) return false;
+    out[0] = x.c0; out[1] = x.c1; out[2] = y.c0; out[3] = y.c1;
+    return true;
+}
+
+// k canonical coordinates, or k x 32 bytes of 0xFF when !ok
+__device__ __forceinline__ void coords_store(uint8_t* p, const fe* c, int k, bool ok) {
+    fe ff;
+    for (int i = 0; i < 8; i++) ff.l[i] = 0xffffffffu;
+    for (int i = 0; i < k; i++) fe_store(p + 32 * i, ok ? c[i] : ff);
+}
+
+// one proof per thread: compressed row j -> the canonical 256-byte row j of b2g_prove and ok[j] = 1, or the 0xFF row and
+// ok[j] = 0.  No subgroup check: decompress_g2_kernel adds it where the caller needs it.
+__global__ void __launch_bounds__(128) decompress_kernel(const uint8_t* __restrict__ comp, uint32_t count, uint8_t* __restrict__ proofs,
+                                                         uint8_t* __restrict__ ok) {
+    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= count) return;
+    const uint8_t* in = comp + (size_t)j * COMP_BYTES;
+    fe c[8];
+    for (int k = 0; k < 8; k++) c[k] = fe_zero();
+    const bool good = g1_decompress(c, in) && g2_decompress(c + 2, in + 32) && g1_decompress(c + 6, in + 96);
+    coords_store(proofs + (size_t)j * 256, c, 8, good);
+    ok[j] = good;
+}
+
+// G2 membership of every decoded B, one proof per thread, in its own kernel so that the decoder does not carry
+// g2_in_subgroup's registers and stack: a row whose B is outside G2 becomes the 0xFF row and ok[j] = 0
+__global__ void __launch_bounds__(128) decompress_g2_kernel(uint32_t count, uint8_t* __restrict__ proofs, uint8_t* __restrict__ ok) {
+    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= count || !ok[j]) return;
+    uint8_t* row = proofs + (size_t)j * 256;
+    G2::Aff b;
+    b.x.c0 = to_mont(fe_load(row + 64)); b.x.c1 = to_mont(fe_load(row + 96));
+    b.y.c0 = to_mont(fe_load(row + 128)); b.y.c1 = to_mont(fe_load(row + 160));
+    if (!g2_in_subgroup(b)) { coords_store(row, nullptr, 8, false); ok[j] = 0; }
+}
+
+// b2g_test_op ops 46-48: the Fq square root (a: 32 B Montgomery; out: 64 B), the Fq2 square root (a: 64 B; out: 96 B), and
+// one compressed G2 point decoded without the subgroup check (a: 64 B; out: 160 B: the canonical affine point, or 0xFF
+// bytes).  Each result is followed by a 32-byte slot whose first word is 1 when there is a root / the point decodes.
+__global__ void decompress_test_kernel(int op, const uint8_t* __restrict__ a, uint32_t n, uint8_t* __restrict__ out) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    bool ok;
+    uint8_t* o;
+    if (op == 46) {
+        o = out + (size_t)i * 64;
+        fe_store(o, Fq::sqrt(fe_load(a + (size_t)i * 32), ok));
+        o += 32;
+    } else if (op == 47) {
+        o = out + (size_t)i * 96;
+        fe2 x, r;
+        elem_load(x, a + (size_t)i * 64);
+        ok = Fq2::sqrt(r, x);
+        elem_store(o, r);
+        o += 64;
+    } else {
+        o = out + (size_t)i * 160;
+        fe c[4];
+        for (int k = 0; k < 4; k++) c[k] = fe_zero();
+        ok = g2_decompress(c, a + (size_t)i * 64);
+        coords_store(o, c, 4, ok);
+        o += 128;
+    }
+    fe flag = fe_zero();
+    flag.l[0] = ok;
+    fe_store(o, flag);
+}
+
 // lines of -gamma (thread 0) and -delta (thread 1) for every loop step, in the order miller_loop reads them
 __global__ void vk_lines_kernel(const uint8_t* __restrict__ g2, uint8_t* __restrict__ lines) {
     const int t = threadIdx.x;
@@ -385,14 +529,17 @@ __global__ void pairing_test_kernel(int op, const uint8_t* __restrict__ a, const
 }
 
 void pairing_test_op(cudaStream_t st, int op, const void* a, const void* b, size_t n, void* out) {
-    if (op > 45 || !a || !out) throw_error(B2G_E_SHAPE, "bad arguments");
-    const bool batch_op = op >= 43;
+    if (op > 48 || !a || !out) throw_error(B2G_E_SHAPE, "bad arguments");
+    const bool batch_op = op >= 43 && op <= 45, decompress_op = op >= 46;
     size_t sa = (op == 37 || op == 40) ? 64 : ((op == 41 || op == 42) ? LINE_BYTES : F12_BYTES);
     size_t sb = op == 30 ? F12_BYTES : ((op == 37 || op == 40 || op == 42) ? 128 : (op == 39 ? LINE_BYTES : 0));
     size_t so = F12_BYTES;
     if (op == 43) { sa = 128; sb = 0; so = 8; }
     if (op == 44) { sa = 64; sb = 16; so = 64; }
     if (op == 45) { sa = F12_BYTES; sb = 32; so = F12_BYTES; }
+    if (op == 46) { sa = 32; sb = 0; so = 64; }
+    if (op == 47) { sa = 64; sb = 0; so = 96; }
+    if (op == 48) { sa = 64; sb = 0; so = 160; }
     if (sb && !b) throw_error(B2G_E_SHAPE, "this op needs operand b");
     if (n == 0) return;
     struct Bufs { uint8_t *a = nullptr, *b = nullptr, *o = nullptr; ~Bufs() { for (void* p : {(void*)a, (void*)b, (void*)o}) if (p) cudaFree(p); } } d;
@@ -400,6 +547,7 @@ void pairing_test_op(cudaStream_t st, int op, const void* a, const void* b, size
     if (sb) d.b = dev_upload<uint8_t>(b, n * sb, st);
     CUDA_CHECK(cudaMalloc(&d.o, n * so));
     if (batch_op) batch_test_kernel<<<(unsigned)((n + 63) / 64), 64, 0, st>>>(op, d.a, d.b, (uint32_t)n, d.o);
+    else if (decompress_op) decompress_test_kernel<<<(unsigned)((n + 63) / 64), 64, 0, st>>>(op, d.a, (uint32_t)n, d.o);
     else pairing_test_kernel<<<(unsigned)((n + 63) / 64), 64, 0, st>>>(op, d.a, d.b, (uint32_t)n, d.o);
     g_launch_count += 1;
     CUDA_CHECK(cudaGetLastError());
@@ -437,8 +585,9 @@ static void vbuf_grow(uint8_t*& p, size_t& cap, size_t bytes) {
 }
 
 // grows the context's verification buffers to `count` proofs, `inputs` public-input scalars, `parts` (proof, input) G1
-// records and `batch` bytes of b2g_verify_batch scratch; never shrinks them, and a failed allocation leaves them consistent
-static void vbufs_ensure(VerifyBufs*& v, size_t count, size_t inputs, size_t parts, size_t batch = 0) {
+// records, `batch` bytes of b2g_verify_batch scratch and `comp` bytes of compressed-proof staging; never shrinks them, and a
+// failed allocation leaves them consistent
+static void vbufs_ensure(VerifyBufs*& v, size_t count, size_t inputs, size_t parts, size_t batch = 0, size_t comp = 0) {
     if (!v) v = new VerifyBufs();
     if (count > v->cap_count) {
         for (uint8_t** p : {&v->d_proofs, &v->d_rec, &v->d_f, &v->d_verdict}) { if (*p) cudaFree(*p); *p = nullptr; }
@@ -452,6 +601,21 @@ static void vbufs_ensure(VerifyBufs*& v, size_t count, size_t inputs, size_t par
     vbuf_grow(v->d_pub, v->cap_pub, inputs * 32);
     vbuf_grow(v->d_part, v->cap_part, parts * 128);
     vbuf_grow(v->d_batch, v->cap_batch, batch);
+    vbuf_grow(v->d_comp, v->cap_comp, comp);
+}
+
+// the staging bytes of count compressed proofs: the rows, then one ok byte per proof
+static size_t comp_bytes(uint32_t count) { return (size_t)count * (COMP_BYTES + 1); }
+
+// uploads count compressed proofs to the staging buffer and decodes them into v.d_proofs on st; with g2_check, a decoded B
+// outside G2 also turns its row into the 0xFF row.  Returns the device ok bytes.
+static uint8_t* decompress_enqueue(VerifyBufs& v, const void* compressed, uint32_t count, bool g2_check, cudaStream_t st) {
+    uint8_t* ok = v.d_comp + (size_t)count * COMP_BYTES;
+    CUDA_CHECK(cudaMemcpyAsync(v.d_comp, compressed, (size_t)count * COMP_BYTES, cudaMemcpyHostToDevice, st));
+    decompress_kernel<<<(count + 127) / 128, 128, 0, st>>>(v.d_comp, count, v.d_proofs, ok);
+    if (g2_check) decompress_g2_kernel<<<(count + 127) / 128, 128, 0, st>>>(count, v.d_proofs, ok);
+    g_launch_count += g2_check ? 2 : 1;
+    return ok;
 }
 
 // the two side streams and five events of b2g_verify_batch, created at its first call on the context.  The side streams have
@@ -538,14 +702,21 @@ int b2g_vk_alpha_beta(b2g_vk* vk, void* out) {
     });
 }
 
-// the argument checks b2g_verify_many and b2g_verify_batch share; returns the context
+// the checks every call on a batch of proofs shares (pointers checked by the caller): count >= 1, no proof pending on the
+// context; returns the context
+static CtxView batch_args(const char* fn, b2g_ctx* ctx, uint32_t count) {
+    if (count == 0) throw_error(B2G_E_SHAPE, std::string(fn) + ": count must be at least 1");
+    const CtxView cv = ctx_view(ctx);
+    if (cv.proof_pending) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
+    return cv;
+}
+
+// the argument checks of the verifiers (b2g_verify_many, b2g_verify_batch and their compressed forms); returns the context
 static CtxView verify_args(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs,
                            const void* out) {
     if (!ctx || !vk || !proofs || !out || (vk->n_public && !public_inputs)) throw_error(B2G_E_SHAPE, "null pointer");
-    if (count == 0) throw_error(B2G_E_SHAPE, std::string(fn) + ": count must be at least 1");
-    const CtxView cv = ctx_view(ctx);
+    const CtxView cv = batch_args(fn, ctx, count);
     if (vk->device != cv.device) throw_error(B2G_E_SHAPE, "the verifying key belongs to another device");
-    if (cv.proof_pending) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
     const size_t inputs = (size_t)count * vk->n_public;
     const uint32_t* pub = (const uint32_t*)public_inputs;
     for (size_t k = 0; k < inputs; k++)
@@ -555,9 +726,10 @@ static CtxView verify_args(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t co
 }
 
 // vbufs_ensure, reporting a batch that does not fit as B2G_E_DEVICE with advice
-static void verify_bufs_ensure(const char* fn, VerifyBufs*& v, uint32_t count, size_t inputs, size_t parts, size_t batch = 0) {
+static void verify_bufs_ensure(const char* fn, VerifyBufs*& v, uint32_t count, size_t inputs, size_t parts, size_t batch = 0,
+                               size_t comp = 0) {
     try {
-        vbufs_ensure(v, count, inputs, parts, batch);
+        vbufs_ensure(v, count, inputs, parts, batch, comp);
     } catch (const B2gError& e) {
         if (e.code != B2G_E_DEVICE) throw;
         cudaGetLastError();
@@ -566,95 +738,134 @@ static void verify_bufs_ensure(const char* fn, VerifyBufs*& v, uint32_t count, s
     }
 }
 
-int b2g_verify_many(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs, uint8_t* verdicts_out) {
+int b2g_proofs_decompress(b2g_ctx* ctx, uint32_t count, const void* compressed, uint8_t* proofs_out, uint8_t* ok_out) {
     return guarded([&] {
-        const CtxView cv = verify_args("b2g_verify_many", ctx, vk, count, public_inputs, proofs, verdicts_out);
-        const size_t inputs = (size_t)count * vk->n_public;
+        if (!ctx || !compressed || !proofs_out || !ok_out) throw_error(B2G_E_SHAPE, "null pointer");
+        const CtxView cv = batch_args("b2g_proofs_decompress", ctx, count);
         DevGuard g(cv.device);
         cudaStream_t st = cv.st;
-        verify_bufs_ensure("b2g_verify_many", *cv.vbufs, count, inputs, inputs);
+        verify_bufs_ensure("b2g_proofs_decompress", *cv.vbufs, count, 0, 0, 0, comp_bytes(count));
         VerifyBufs& v = **cv.vbufs;
-        CUDA_CHECK(cudaMemcpyAsync(v.d_proofs, proofs, (size_t)count * 256, cudaMemcpyHostToDevice, st));
-        if (inputs) {
-            CUDA_CHECK(cudaMemcpyAsync(v.d_pub, public_inputs, inputs * 32, cudaMemcpyHostToDevice, st));
-            verify_inputs_kernel<<<(unsigned)((inputs + 3) / 4), 128, 0, st>>>(vk->d_tabs, (const uint32_t*)v.d_pub, vk->n_public, inputs, v.d_part);
-        }
-        verify_prepare_kernel<<<(count + 127) / 128, 128, 0, st>>>(v.d_proofs, vk->d_g1, v.d_part, vk->n_public, count, v.d_rec);
-        verify_miller_kernel<<<(count + 63) / 64, 64, 0, st>>>(v.d_rec, vk->d_lines, !vk->gamma_inf, !vk->delta_inf, count, v.d_f);
-        verify_final_kernel<<<(count + 63) / 64, 64, 0, st>>>(v.d_rec, v.d_f, vk->d_eab, count, v.d_verdict);
-        g_launch_count += 3 + (inputs ? 1 : 0);
+        const uint8_t* ok = decompress_enqueue(v, compressed, count, true, st);
         CUDA_CHECK(cudaGetLastError());
-        CUDA_CHECK(cudaMemcpyAsync(verdicts_out, v.d_verdict, count, cudaMemcpyDeviceToHost, st));
+        CUDA_CHECK(cudaMemcpyAsync(proofs_out, v.d_proofs, (size_t)count * 256, cudaMemcpyDeviceToHost, st));
+        CUDA_CHECK(cudaMemcpyAsync(ok_out, ok, count, cudaMemcpyDeviceToHost, st));
         CUDA_CHECK(cudaStreamSynchronize(st));
     });
 }
 
+// b2g_verify_many on 256-byte rows, or on compressed rows decoded on the device (G2 check included)
+static void verify_many_run(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs,
+                            bool compressed, uint8_t* verdicts_out) {
+    const CtxView cv = verify_args(fn, ctx, vk, count, public_inputs, proofs, verdicts_out);
+    const size_t inputs = (size_t)count * vk->n_public;
+    DevGuard g(cv.device);
+    cudaStream_t st = cv.st;
+    verify_bufs_ensure(fn, *cv.vbufs, count, inputs, inputs, 0, compressed ? comp_bytes(count) : 0);
+    VerifyBufs& v = **cv.vbufs;
+    if (compressed) decompress_enqueue(v, proofs, count, true, st);
+    else CUDA_CHECK(cudaMemcpyAsync(v.d_proofs, proofs, (size_t)count * 256, cudaMemcpyHostToDevice, st));
+    if (inputs) {
+        CUDA_CHECK(cudaMemcpyAsync(v.d_pub, public_inputs, inputs * 32, cudaMemcpyHostToDevice, st));
+        verify_inputs_kernel<<<(unsigned)((inputs + 3) / 4), 128, 0, st>>>(vk->d_tabs, (const uint32_t*)v.d_pub, vk->n_public, inputs, v.d_part);
+    }
+    verify_prepare_kernel<<<(count + 127) / 128, 128, 0, st>>>(v.d_proofs, vk->d_g1, v.d_part, vk->n_public, count, v.d_rec);
+    verify_miller_kernel<<<(count + 63) / 64, 64, 0, st>>>(v.d_rec, vk->d_lines, !vk->gamma_inf, !vk->delta_inf, count, v.d_f);
+    verify_final_kernel<<<(count + 63) / 64, 64, 0, st>>>(v.d_rec, v.d_f, vk->d_eab, count, v.d_verdict);
+    g_launch_count += 3 + (inputs ? 1 : 0);
+    CUDA_CHECK(cudaGetLastError());
+    CUDA_CHECK(cudaMemcpyAsync(verdicts_out, v.d_verdict, count, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaStreamSynchronize(st));
+}
+
+// b2g_verify_batch on 256-byte rows, or on compressed rows decoded on the context's stream before anything else reads them
+// (batch_g2_kernel checks the decoded B, so the decoder skips the G2 check)
+static void verify_batch_run(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs,
+                             bool compressed, const void* weights, uint8_t* verdict_out) {
+    if (!weights) throw_error(B2G_E_SHAPE, "null pointer");
+    const CtxView cv = verify_args(fn, ctx, vk, count, public_inputs, proofs, verdict_out);
+    for (uint32_t i = 0; i < count; i++)
+        if (all_zero((const uint8_t*)weights + 16 * (size_t)i, 16)) throw_error(B2G_E_INPUT, "weight " + std::to_string(i) + " is zero");
+    const uint32_t n_pts = vk->n_public + 1, chunks = (count + SCALAR_CHUNK - 1) / SCALAR_CHUNK;
+    const size_t inputs = (size_t)count * vk->n_public;
+    // scratch: weights, four reduction levels (x, y on the main stream, x2, y2 on the side streams), chunk sums of the
+    // scalars, s_j IC[j], tail values and the ok word
+    auto up = [](size_t b) { return (b + 255) & ~(size_t)255; };
+    const size_t level = up(std::max({(size_t)((count + 63) / 64) * F12_BYTES, (size_t)((count + 127) / 128) * 128,
+                                      (size_t)((n_pts + 127) / 128) * 128}));
+    const size_t o_w = 0, o_x = up((size_t)count * 16), o_y = o_x + level, o_x2 = o_y + level, o_y2 = o_x2 + level;
+    const size_t o_part = o_y2 + level, o_pts = o_part + up((size_t)n_pts * chunks * 32), o_tail = o_pts + up((size_t)n_pts * 128);
+    const size_t o_ok = o_tail + TAIL_BYTES, bytes = o_ok + 256;
+    DevGuard g(cv.device);
+    cudaStream_t st = cv.st;
+    verify_bufs_ensure(fn, *cv.vbufs, count, inputs, 0, bytes, compressed ? comp_bytes(count) : 0);
+    VerifyBufs& v = **cv.vbufs;
+    batch_streams(v);
+    cudaStream_t s2 = v.side[0], s3 = v.side[1];
+    cudaEvent_t ev_up = v.ev[0], ev_prep = v.ev[1], ev_pts = v.ev[2], ev_s2 = v.ev[3], ev_s3 = v.ev[4];
+    uint8_t* B = v.d_batch;
+    uint8_t* tail = B + o_tail;
+    const uint32_t* w = (const uint32_t*)(B + o_w);
+    uint32_t* ok = (uint32_t*)(B + o_ok);
+    auto prod = [](cudaStream_t s) {
+        return [s](uint32_t blocks, const uint8_t* src, size_t stride, uint32_t n, uint8_t* o) { f12_product_kernel<<<blocks, 64, 0, s>>>(src, stride, n, o); };
+    };
+    auto sum = [](cudaStream_t s) {
+        return [s](uint32_t blocks, const uint8_t* src, size_t stride, uint32_t n, uint8_t* o) { g1_sum_kernel<<<blocks, 128, 0, s>>>(src, stride, n, o); };
+    };
+    if (compressed) decompress_enqueue(v, proofs, count, false, st);
+    else CUDA_CHECK(cudaMemcpyAsync(v.d_proofs, proofs, (size_t)count * 256, cudaMemcpyHostToDevice, st));
+    CUDA_CHECK(cudaMemcpyAsync(B + o_w, weights, (size_t)count * 16, cudaMemcpyHostToDevice, st));
+    if (inputs) CUDA_CHECK(cudaMemcpyAsync(v.d_pub, public_inputs, inputs * 32, cudaMemcpyHostToDevice, st));
+    CUDA_CHECK(cudaMemsetAsync(ok, 0xff, 4, st));
+    CUDA_CHECK(cudaEventRecord(ev_up, st));
+    // main stream: per-proof parse and scaling, Miller loops, their product, then the verdict
+    batch_prepare_kernel<<<(count + 127) / 128, 128, 0, st>>>(v.d_proofs, w, count, v.d_rec, ok);
+    CUDA_CHECK(cudaEventRecord(ev_prep, st));
+    batch_miller_kernel<<<(count + 63) / 64, 64, 0, st>>>(v.d_rec, ok, count, v.d_f);
+    tree_reduce(v.d_f, F12_BYTES, F12_BYTES, count, 64, B + o_x, B + o_y, tail + TAIL_F, prod(st));
+    // side stream 2: the input scalars, the prepared inputs, e(alpha, beta)^s_0, the G2 membership of every B
+    CUDA_CHECK(cudaStreamWaitEvent(s2, ev_up, 0));
+    batch_scalars_kernel<<<dim3(n_pts, chunks), 128, 0, s2>>>(w, (const uint32_t*)v.d_pub, vk->n_public, count, B + o_part);
+    batch_inputs_kernel<<<(n_pts + 3) / 4, 128, 0, s2>>>(vk->d_tabs, vk->d_g1, B + o_part, chunks, vk->n_public, B + o_pts, tail);
+    tree_reduce(B + o_pts, 128, 128, n_pts, 128, B + o_x2, B + o_y2, tail + TAIL_PREP, sum(s2));
+    CUDA_CHECK(cudaEventRecord(ev_pts, s2));
+    batch_rhs_kernel<<<1, 1, 0, s2>>>(tail, vk->d_eab);
+    batch_g2_kernel<<<(count + 127) / 128, 128, 0, s2>>>(v.d_proofs, count, ok);
+    CUDA_CHECK(cudaEventRecord(ev_s2, s2));
+    // side stream 3, once the r C and the prepared inputs exist: sum r C, then the Miller loop of the prepared pairs
+    CUDA_CHECK(cudaStreamWaitEvent(s3, ev_prep, 0));
+    CUDA_CHECK(cudaStreamWaitEvent(s3, ev_pts, 0));
+    tree_reduce(v.d_rec + BREC_RC, REC_BYTES_V, 128, count, 128, B + o_x2, B + o_y2, tail + TAIL_RC, sum(s3));
+    batch_pairs_kernel<<<1, 1, 0, s3>>>(tail, vk->d_lines, !vk->gamma_inf, !vk->delta_inf);
+    CUDA_CHECK(cudaEventRecord(ev_s3, s3));
+    CUDA_CHECK(cudaStreamWaitEvent(st, ev_s2, 0));
+    CUDA_CHECK(cudaStreamWaitEvent(st, ev_s3, 0));
+    batch_final_kernel<<<1, 1, 0, st>>>(tail, ok, v.d_verdict);
+    g_launch_count += 8;
+    CUDA_CHECK(cudaGetLastError());
+    CUDA_CHECK(cudaMemcpyAsync(verdict_out, v.d_verdict, 1, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaStreamSynchronize(st));
+}
+
+int b2g_verify_many(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs, uint8_t* verdicts_out) {
+    return guarded([&] { verify_many_run("b2g_verify_many", ctx, vk, count, public_inputs, proofs, false, verdicts_out); });
+}
+
+int b2g_verify_many_compressed(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* compressed,
+                               uint8_t* verdicts_out) {
+    return guarded([&] { verify_many_run("b2g_verify_many_compressed", ctx, vk, count, public_inputs, compressed, true, verdicts_out); });
+}
+
 int b2g_verify_batch(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs, const void* weights,
                      uint8_t* verdict_out) {
+    return guarded([&] { verify_batch_run("b2g_verify_batch", ctx, vk, count, public_inputs, proofs, false, weights, verdict_out); });
+}
+
+int b2g_verify_batch_compressed(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* compressed,
+                                const void* weights, uint8_t* verdict_out) {
     return guarded([&] {
-        if (!weights) throw_error(B2G_E_SHAPE, "null pointer");
-        const CtxView cv = verify_args("b2g_verify_batch", ctx, vk, count, public_inputs, proofs, verdict_out);
-        for (uint32_t i = 0; i < count; i++)
-            if (all_zero((const uint8_t*)weights + 16 * (size_t)i, 16)) throw_error(B2G_E_INPUT, "weight " + std::to_string(i) + " is zero");
-        const uint32_t n_pts = vk->n_public + 1, chunks = (count + SCALAR_CHUNK - 1) / SCALAR_CHUNK;
-        const size_t inputs = (size_t)count * vk->n_public;
-        // scratch: weights, four reduction levels (x, y on the main stream, x2, y2 on the side streams), chunk sums of the
-        // scalars, s_j IC[j], tail values and the ok word
-        auto up = [](size_t b) { return (b + 255) & ~(size_t)255; };
-        const size_t level = up(std::max({(size_t)((count + 63) / 64) * F12_BYTES, (size_t)((count + 127) / 128) * 128,
-                                          (size_t)((n_pts + 127) / 128) * 128}));
-        const size_t o_w = 0, o_x = up((size_t)count * 16), o_y = o_x + level, o_x2 = o_y + level, o_y2 = o_x2 + level;
-        const size_t o_part = o_y2 + level, o_pts = o_part + up((size_t)n_pts * chunks * 32), o_tail = o_pts + up((size_t)n_pts * 128);
-        const size_t o_ok = o_tail + TAIL_BYTES, bytes = o_ok + 256;
-        DevGuard g(cv.device);
-        cudaStream_t st = cv.st;
-        verify_bufs_ensure("b2g_verify_batch", *cv.vbufs, count, inputs, 0, bytes);
-        VerifyBufs& v = **cv.vbufs;
-        batch_streams(v);
-        cudaStream_t s2 = v.side[0], s3 = v.side[1];
-        cudaEvent_t ev_up = v.ev[0], ev_prep = v.ev[1], ev_pts = v.ev[2], ev_s2 = v.ev[3], ev_s3 = v.ev[4];
-        uint8_t* B = v.d_batch;
-        uint8_t* tail = B + o_tail;
-        const uint32_t* w = (const uint32_t*)(B + o_w);
-        uint32_t* ok = (uint32_t*)(B + o_ok);
-        auto prod = [](cudaStream_t s) {
-            return [s](uint32_t blocks, const uint8_t* src, size_t stride, uint32_t n, uint8_t* o) { f12_product_kernel<<<blocks, 64, 0, s>>>(src, stride, n, o); };
-        };
-        auto sum = [](cudaStream_t s) {
-            return [s](uint32_t blocks, const uint8_t* src, size_t stride, uint32_t n, uint8_t* o) { g1_sum_kernel<<<blocks, 128, 0, s>>>(src, stride, n, o); };
-        };
-        CUDA_CHECK(cudaMemcpyAsync(v.d_proofs, proofs, (size_t)count * 256, cudaMemcpyHostToDevice, st));
-        CUDA_CHECK(cudaMemcpyAsync(B + o_w, weights, (size_t)count * 16, cudaMemcpyHostToDevice, st));
-        if (inputs) CUDA_CHECK(cudaMemcpyAsync(v.d_pub, public_inputs, inputs * 32, cudaMemcpyHostToDevice, st));
-        CUDA_CHECK(cudaMemsetAsync(ok, 0xff, 4, st));
-        CUDA_CHECK(cudaEventRecord(ev_up, st));
-        // main stream: per-proof parse and scaling, Miller loops, their product, then the verdict
-        batch_prepare_kernel<<<(count + 127) / 128, 128, 0, st>>>(v.d_proofs, w, count, v.d_rec, ok);
-        CUDA_CHECK(cudaEventRecord(ev_prep, st));
-        batch_miller_kernel<<<(count + 63) / 64, 64, 0, st>>>(v.d_rec, ok, count, v.d_f);
-        tree_reduce(v.d_f, F12_BYTES, F12_BYTES, count, 64, B + o_x, B + o_y, tail + TAIL_F, prod(st));
-        // side stream 2: the input scalars, the prepared inputs, e(alpha, beta)^s_0, the G2 membership of every B
-        CUDA_CHECK(cudaStreamWaitEvent(s2, ev_up, 0));
-        batch_scalars_kernel<<<dim3(n_pts, chunks), 128, 0, s2>>>(w, (const uint32_t*)v.d_pub, vk->n_public, count, B + o_part);
-        batch_inputs_kernel<<<(n_pts + 3) / 4, 128, 0, s2>>>(vk->d_tabs, vk->d_g1, B + o_part, chunks, vk->n_public, B + o_pts, tail);
-        tree_reduce(B + o_pts, 128, 128, n_pts, 128, B + o_x2, B + o_y2, tail + TAIL_PREP, sum(s2));
-        CUDA_CHECK(cudaEventRecord(ev_pts, s2));
-        batch_rhs_kernel<<<1, 1, 0, s2>>>(tail, vk->d_eab);
-        batch_g2_kernel<<<(count + 127) / 128, 128, 0, s2>>>(v.d_proofs, count, ok);
-        CUDA_CHECK(cudaEventRecord(ev_s2, s2));
-        // side stream 3, once the r C and the prepared inputs exist: sum r C, then the Miller loop of the prepared pairs
-        CUDA_CHECK(cudaStreamWaitEvent(s3, ev_prep, 0));
-        CUDA_CHECK(cudaStreamWaitEvent(s3, ev_pts, 0));
-        tree_reduce(v.d_rec + BREC_RC, REC_BYTES_V, 128, count, 128, B + o_x2, B + o_y2, tail + TAIL_RC, sum(s3));
-        batch_pairs_kernel<<<1, 1, 0, s3>>>(tail, vk->d_lines, !vk->gamma_inf, !vk->delta_inf);
-        CUDA_CHECK(cudaEventRecord(ev_s3, s3));
-        CUDA_CHECK(cudaStreamWaitEvent(st, ev_s2, 0));
-        CUDA_CHECK(cudaStreamWaitEvent(st, ev_s3, 0));
-        batch_final_kernel<<<1, 1, 0, st>>>(tail, ok, v.d_verdict);
-        g_launch_count += 8;
-        CUDA_CHECK(cudaGetLastError());
-        CUDA_CHECK(cudaMemcpyAsync(verdict_out, v.d_verdict, 1, cudaMemcpyDeviceToHost, st));
-        CUDA_CHECK(cudaStreamSynchronize(st));
+        verify_batch_run("b2g_verify_batch_compressed", ctx, vk, count, public_inputs, compressed, true, weights, verdict_out);
     });
 }
 

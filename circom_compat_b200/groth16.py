@@ -14,6 +14,10 @@
            (b2g_verify_many, with the key prepared on the device by b2g_vk_load <- process_vk).
     Groth16.verify_batch(vk, public_inputs, proofs)
         <- the same check for a whole batch at once: one random-linear-combination pairing check (b2g_verify_batch).
+    Groth16.decompress_proofs(blobs)
+        <- Proof::<Bn254>::deserialize_compressed (ark-serialize 0.5, Validate::Yes) for many 128-byte proofs, on the device.
+    Groth16.verify_many_compressed / verify_batch_compressed(vk, public_inputs, blobs)
+        <- deserialize_compressed followed by verify_many / verify_batch, decoded on the device.
 Arguments keep the reference's meaning; field elements are (n, 4) uint64 Montgomery limb arrays (fr_to_mont).
 """
 from __future__ import annotations
@@ -45,7 +49,9 @@ _TEST_OP_WORDS = {**{op: (4, 4, 4) for op in (0, 1, 2, 3, 4, 5, 14, 15, 16)}, 6:
                   30: (48, 48, 48), **{op: (48, 0, 48) for op in (31, 32, 33, 34, 35, 36, 38)}, 37: (8, 16, 48), 39: (48, 24, 48),
                   40: (8, 16, 48), 41: (24, 0, 48), 42: (24, 16, 48),
                   # the batch check's pieces: G2 membership, 128-bit G1 product, cyclotomic exponentiation
-                  43: (16, 0, 1), 44: (8, 2, 8), 45: (48, 4, 48)}
+                  43: (16, 0, 1), 44: (8, 2, 8), 45: (48, 4, 48),
+                  # the compressed-proof decoder's pieces: Fq and Fq2 square roots, one compressed G2 point (result, then a flag slot)
+                  46: (4, 0, 8), 47: (8, 0, 12), 48: (8, 0, 20)}
 TEST_PAIR_RUN = 16            # entries per row of op 27; an entry is 16 words of affine point + 4 words whose bit 0 is the sign
 
 
@@ -268,15 +274,29 @@ class PendingProof:
         return Proof(self._out.tobytes())
 
 
-def _verify_args(fn, vk, public_inputs, proofs, ctx):
-    """the argument checks and encoding verify_many and verify_batch share: None for an empty batch, else (ctx, device key,
-    count, public inputs as 32 B words or None, proofs as 256 B rows)"""
+COMPRESSED_PROOF_BYTES = 128
+
+
+def _proof_rows(fn, proofs, compressed) -> bytes:
+    """proofs as back-to-back rows: 256-byte Proof.data, or (compressed) 128-byte blobs of any other length refused"""
+    if not compressed:
+        return b''.join(p.data for p in proofs)
+    for b in proofs:
+        if not isinstance(b, (bytes, bytearray, memoryview)) or len(b) != COMPRESSED_PROOF_BYTES:
+            raise ValueError(f"{fn}: a compressed proof is {COMPRESSED_PROOF_BYTES} bytes")
+    return b''.join(bytes(b) for b in proofs)
+
+
+def _verify_args(fn, vk, public_inputs, proofs, ctx, compressed=False):
+    """the argument checks and encoding the verifiers share: None for an empty batch, else (ctx, device key, count, public
+    inputs as 32 B words or None, proofs as 256 B rows, or as 128 B rows when compressed)"""
     from . import verifier
     public_inputs, proofs = [list(x) for x in public_inputs], list(proofs)
     if len(public_inputs) != len(proofs):
         raise ValueError(f"{fn}: one public-input list per proof")
     if not proofs:
         return None
+    rows = _proof_rows(fn, proofs, compressed)
     base = vk.vk if isinstance(vk, verifier.PreparedVerifyingKey) else vk
     n_public = len(base.gamma_abc_g1) - 1
     for xs in public_inputs:
@@ -289,8 +309,48 @@ def _verify_args(fn, vk, public_inputs, proofs, ctx):
     vh = ctx.vk_handle(vk)
     pub = b''.join(int(x).to_bytes(32, 'little') for xs in public_inputs for x in xs)
     pub_arr = np.frombuffer(pub, dtype=np.uint8).copy() if pub else None
-    data = np.frombuffer(b''.join(p.data for p in proofs), dtype=np.uint8).copy()
+    data = np.frombuffer(rows, dtype=np.uint8).copy()
     return ctx, vh, len(proofs), pub_arr, data
+
+
+def _verify_many(fn, vk, public_inputs, proofs, ctx, compressed) -> list:
+    """Groth16.verify_many and verify_many_compressed"""
+    args = _verify_args(fn, vk, public_inputs, proofs, ctx, compressed)
+    if args is None:
+        return []
+    ctx, vh, count, pub_arr, data = args
+    out = np.zeros(count, dtype=np.uint8)
+    entry = N.lib().b2g_verify_many_compressed if compressed else N.lib().b2g_verify_many
+    N.check(entry(ctx._h, vh, count, _ptr(pub_arr) if pub_arr is not None else None, _ptr(data), _ptr(out)))
+    return [bool(v) for v in out]
+
+
+def _verify_batch(fn, vk, public_inputs, proofs, ctx, weights, compressed) -> bool:
+    """Groth16.verify_batch and verify_batch_compressed"""
+    import secrets
+    proofs = list(proofs)
+    if weights is not None:                    # checked before the key is loaded on the device
+        weights = [int(w) for w in weights]
+        if len(weights) != len(proofs):
+            raise ValueError(f"{fn}: one weight per proof")
+        for w in weights:
+            if not 0 < w < 1 << 128:
+                raise N.B2gError(N.B2G_E_INPUT, f"weight {w} is not in [1, 2^128)")
+    args = _verify_args(fn, vk, public_inputs, proofs, ctx, compressed)
+    if args is None:
+        return True
+    ctx, vh, count, pub_arr, data = args
+    if weights is None:
+        weights = []
+        while len(weights) < count:
+            w = secrets.randbits(128)
+            if w:
+                weights.append(w)
+    wb = np.frombuffer(b''.join(w.to_bytes(16, 'little') for w in weights), dtype=np.uint8).copy()
+    out = np.zeros(1, dtype=np.uint8)
+    entry = N.lib().b2g_verify_batch_compressed if compressed else N.lib().b2g_verify_batch
+    N.check(entry(ctx._h, vh, count, _ptr(pub_arr) if pub_arr is not None else None, _ptr(data), _ptr(wb), _ptr(out)))
+    return bool(out[0])
 
 
 def _scalar_bytes(v) -> np.ndarray:
@@ -456,13 +516,7 @@ class Groth16:
         sequence of ints per proof, proofs = [Proof].  Returns [bool].  Verdicts equal the host call's, except that a proof
         coordinate >= p is invalid here (arkworks cannot deserialise it) where the host verifier reduces it.  A public input
         outside [0, r) raises B2gError (B2G_E_INPUT); an input count that does not match the key raises MalformedVerifyingKey."""
-        args = _verify_args('verify_many', vk, public_inputs, proofs, ctx)
-        if args is None:
-            return []
-        ctx, vh, count, pub_arr, data = args
-        out = np.zeros(count, dtype=np.uint8)
-        N.check(N.lib().b2g_verify_many(ctx._h, vh, count, _ptr(pub_arr) if pub_arr is not None else None, _ptr(data), _ptr(out)))
-        return [bool(v) for v in out]
+        return _verify_many('verify_many', vk, public_inputs, proofs, ctx, False)
 
     @staticmethod
     def verify_batch(vk, public_inputs, proofs, ctx: Context = None, weights=None) -> bool:
@@ -473,29 +527,39 @@ class Groth16:
         batch is True.  `weights` (one int in [1, 2^128) per proof) are drawn with secrets.randbits(128) when not given;
         weights a prover could know or choose before fixing its proofs make the check unsound.  A zero or too large weight
         raises B2gError (B2G_E_INPUT)."""
-        import secrets
-        proofs = list(proofs)
-        if weights is not None:                    # checked before the key is loaded on the device
-            weights = [int(w) for w in weights]
-            if len(weights) != len(proofs):
-                raise ValueError("verify_batch: one weight per proof")
-            for w in weights:
-                if not 0 < w < 1 << 128:
-                    raise N.B2gError(N.B2G_E_INPUT, f"weight {w} is not in [1, 2^128)")
-        args = _verify_args('verify_batch', vk, public_inputs, proofs, ctx)
-        if args is None:
-            return True
-        ctx, vh, count, pub_arr, data = args
-        if weights is None:
-            weights = []
-            while len(weights) < count:
-                w = secrets.randbits(128)
-                if w:
-                    weights.append(w)
-        wb = np.frombuffer(b''.join(w.to_bytes(16, 'little') for w in weights), dtype=np.uint8).copy()
-        out = np.zeros(1, dtype=np.uint8)
-        N.check(N.lib().b2g_verify_batch(ctx._h, vh, count, _ptr(pub_arr) if pub_arr is not None else None, _ptr(data), _ptr(wb), _ptr(out)))
-        return bool(out[0])
+        return _verify_batch('verify_batch', vk, public_inputs, proofs, ctx, weights, False)
+
+    # ---- compressed proofs: Proof::<Bn254>::serialize_compressed (ethereum.serialize_compressed), decoded on the device
+    @staticmethod
+    def decompress_proofs(blobs, ctx: Context = None) -> list:
+        """Proof::<Bn254>::deserialize_compressed (ark-serialize 0.5, Validate::Yes) for many proofs in one device pass
+        (b2g_proofs_decompress): blobs = 128-byte bytes each.  Returns [Proof | None]: None where arkworks would refuse the
+        blob (both flag bits set, a coordinate >= p, an x without a y, or a B outside G2).  A blob of another length raises
+        ValueError."""
+        blobs = list(blobs)
+        rows = _proof_rows('decompress_proofs', blobs, True)
+        if not blobs:
+            return []
+        ctx = ctx or default_context()
+        data = np.frombuffer(rows, dtype=np.uint8).copy()
+        out = np.zeros((len(blobs), 256), dtype=np.uint8)
+        ok = np.zeros(len(blobs), dtype=np.uint8)
+        N.check(N.lib().b2g_proofs_decompress(ctx._h, len(blobs), _ptr(data), _ptr(out), _ptr(ok)))
+        return [Proof(row.tobytes()) if k else None for row, k in zip(out, ok)]
+
+    @staticmethod
+    def verify_many_compressed(vk, public_inputs, blobs, ctx: Context = None) -> list:
+        """verify_many on compressed proofs (b2g_verify_many_compressed), decoded on the device: a verdict is True exactly
+        when the blob decodes as decompress_proofs decodes it (G2 check of B included) and the decoded proof passes
+        verify_many.  Arguments and errors as verify_many; a blob that is not 128 bytes raises ValueError."""
+        return _verify_many('verify_many_compressed', vk, public_inputs, blobs, ctx, True)
+
+    @staticmethod
+    def verify_batch_compressed(vk, public_inputs, blobs, ctx: Context = None, weights=None) -> bool:
+        """verify_batch on compressed proofs (b2g_verify_batch_compressed), decoded on the device: True exactly when every
+        blob decodes and verify_batch with the same weights is True on the decoded proofs.  Arguments, weights and errors as
+        verify_batch; a blob that is not 128 bytes raises ValueError."""
+        return _verify_batch('verify_batch_compressed', vk, public_inputs, blobs, ctx, weights, True)
 
     # base-range sharded variant: every rank calls prove_partial, the 768-byte partials are all-gathered by the caller
     # (torch.distributed / NCCL), then every rank calls prove_finish and obtains the same proof.

@@ -12,6 +12,9 @@
 //   ark_circom::Groth16::verify_many          <- verify_with_processed_vk for many proofs of one key, in one device pass
 //                                                         (host pairing, ark_circom_verifier.hpp; no GPU involved)
 //   ark_circom::Groth16::verify_batch         <- the same for a whole batch at once: one random-linear-combination check
+//   ark_circom::Groth16::decompress_proofs    <- Proof::<Bn254>::deserialize_compressed (ark-serialize 0.5) for many proofs
+//   ark_circom::Groth16::verify_many_compressed / verify_batch_compressed <- deserialize_compressed, then the two above
+//   ark_circom::serialize_compressed          <- Proof::<Bn254>::serialize_compressed (ark_circom_ethereum.hpp)
 //   ark_circom::read_wtns                              <- snarkjs .wtns (test-vectors/circuit2_js/witness.wtns; the reference
 //                                                         computes witnesses with WASM instead, out of scope here)
 // Parsing and key handling stay on the host; every field/curve operation of the proof runs in libb2groth.so.
@@ -22,6 +25,7 @@
 #include <istream>
 #include <map>
 #include <memory>
+#include <optional>
 #include <random>
 #include <stdexcept>
 #include <string>
@@ -368,16 +372,19 @@ typedef Reduction<B2G_REDUCTION_LIBSNARK> LibsnarkReduction;   // ark-groth16's 
 #include "ark_circom_ethereum.hpp"
 namespace ark_circom {
 
-// what Groth16::verify_many and verify_batch share: the argument checks, the key prepared on the device at first use
-// (b2g_vk_load, kept in pvk.device) and the encoded public inputs and proofs
+// what the Groth16 verifiers (verify_many, verify_batch and their compressed forms) share: the argument checks, the key
+// prepared on the device at first use (b2g_vk_load, kept in pvk.device) and the encoded public inputs and proofs (P = Proof,
+// 256-byte rows, or CompressedProof, 128-byte rows)
 struct VerifyCall {
     size_t n = 0;
     Gpu* gpu = nullptr;
     b2g_vk* vk = nullptr;
     std::vector<BigInt256> pub;
     std::vector<uint8_t> bytes;
+    template <class P>
     VerifyCall(const char* fn, const PreparedVerifyingKey& pvk, const std::vector<std::vector<Fr>>& public_inputs,
-               const std::vector<Proof>& proofs, int device) {
+               const std::vector<P>& proofs, int device) {
+        static_assert(sizeof(P) == 256 || sizeof(P) == 128, "a proof row is 256 bytes, or 128 compressed");
         if (public_inputs.size() != proofs.size()) throw SynthesisError(std::string(fn) + ": one public-input list per proof");
         const size_t n_public = pvk.vk.gamma_abc_g1.size() - 1;
         if (proofs.empty()) return;
@@ -395,10 +402,20 @@ struct VerifyCall {
         }
         pub.resize(n * n_public);
         for (size_t i = 0; i < n; i++) for (size_t k = 0; k < n_public; k++) pub[i * n_public + k] = public_inputs[i][k].into_bigint();
-        bytes.resize(n * 256);
-        for (size_t i = 0; i < n; i++) memcpy(&bytes[i * 256], proofs[i].bytes, 256);
+        bytes.resize(n * sizeof(P));
+        for (size_t i = 0; i < n; i++) memcpy(&bytes[i * sizeof(P)], &proofs[i], sizeof(P));
     }
 };
+
+// n nonzero 128-bit weights of the batch check (4 little-endian words each) from std::random_device
+inline std::vector<uint32_t> batch_weights(size_t n) {
+    std::random_device rd;
+    std::vector<uint32_t> w(4 * n);
+    for (size_t i = 0; i < n; i++) {
+        do { for (int t = 0; t < 4; t++) w[4 * i + t] = (uint32_t)rd(); } while (!(w[4 * i] | w[4 * i + 1] | w[4 * i + 2] | w[4 * i + 3]));
+    }
+    return w;
+}
 
 template <class QAP = CircomReduction>
 struct Groth16T {                                       // Groth16::<Bn254, QAP>
@@ -429,13 +446,43 @@ struct Groth16T {                                       // Groth16::<Bn254, QAP>
                              const std::vector<Proof>& proofs, int device = 0) {
         VerifyCall c("verify_batch", pvk, public_inputs, proofs, device);
         if (c.n == 0) return true;
-        std::random_device rd;
-        std::vector<uint32_t> w(4 * c.n);
-        for (size_t i = 0; i < c.n; i++) {
-            do { for (int t = 0; t < 4; t++) w[4 * i + t] = (uint32_t)rd(); } while (!(w[4 * i] | w[4 * i + 1] | w[4 * i + 2] | w[4 * i + 3]));
-        }
+        const std::vector<uint32_t> w = batch_weights(c.n);
         uint8_t verdict = 0;
         check(b2g_verify_batch(c.gpu->ctx(), c.vk, (uint32_t)c.n, c.pub.empty() ? nullptr : c.pub.data(), c.bytes.data(), w.data(), &verdict));
+        return verdict != 0;
+    }
+    // Proof::<Bn254>::deserialize_compressed (ark-serialize 0.5, Validate::Yes) for many proofs in one device pass
+    // (b2g_proofs_decompress): an empty optional where arkworks would refuse the bytes (both flag bits set, a coordinate
+    // >= p, an x without a y, or a B outside G2)
+    static std::vector<std::optional<Proof>> decompress_proofs(const std::vector<CompressedProof>& blobs, int device = 0) {
+        if (blobs.empty()) return {};
+        Gpu& gpu = Gpu::on(device);
+        std::vector<Proof> rows(blobs.size());
+        std::vector<uint8_t> ok(blobs.size());
+        check(b2g_proofs_decompress(gpu.ctx(), (uint32_t)blobs.size(), blobs.data(), rows[0].bytes, ok.data()));
+        std::vector<std::optional<Proof>> out(blobs.size());
+        for (size_t i = 0; i < blobs.size(); i++) if (ok[i]) out[i] = rows[i];
+        return out;
+    }
+    // verify_many on compressed proofs, decoded on the device (b2g_verify_many_compressed): a verdict is true exactly when
+    // the proof decodes (G2 check included) and the decoded proof passes verify_many
+    static std::vector<bool> verify_many_compressed(const PreparedVerifyingKey& pvk, const std::vector<std::vector<Fr>>& public_inputs,
+                                                    const std::vector<CompressedProof>& blobs, int device = 0) {
+        VerifyCall c("verify_many_compressed", pvk, public_inputs, blobs, device);
+        if (c.n == 0) return {};
+        std::vector<uint8_t> verdicts(c.n);
+        check(b2g_verify_many_compressed(c.gpu->ctx(), c.vk, (uint32_t)c.n, c.pub.empty() ? nullptr : c.pub.data(), c.bytes.data(), verdicts.data()));
+        return std::vector<bool>(verdicts.begin(), verdicts.end());
+    }
+    // verify_batch on compressed proofs, decoded on the device (b2g_verify_batch_compressed): true exactly when every proof
+    // decodes and verify_batch would be true on the decoded proofs with the same weights
+    static bool verify_batch_compressed(const PreparedVerifyingKey& pvk, const std::vector<std::vector<Fr>>& public_inputs,
+                                        const std::vector<CompressedProof>& blobs, int device = 0) {
+        VerifyCall c("verify_batch_compressed", pvk, public_inputs, blobs, device);
+        if (c.n == 0) return true;
+        const std::vector<uint32_t> w = batch_weights(c.n);
+        uint8_t verdict = 0;
+        check(b2g_verify_batch_compressed(c.gpu->ctx(), c.vk, (uint32_t)c.n, c.pub.empty() ? nullptr : c.pub.data(), c.bytes.data(), w.data(), &verdict));
         return verdict != 0;
     }
     static Proof create_proof_with_reduction_and_matrices(const ProvingKey& pk, const Fr& r, const Fr& s, const ConstraintMatrices& matrices,

@@ -5,6 +5,7 @@
 // like the reference (`From<&G1Affine> for G1` and `From<G1> for G1Affine`, ...).  A U256 is the canonical integer of a
 // coordinate as 32 big-endian bytes (what `U256::from(&bytes_be[..])` holds and what the Solidity verifier of
 // tests/solidity.rs receives).  The point at infinity is (0, 0), as in the reference (:26-39, :61-80).
+// ark_circom::serialize_compressed mirrors ethereum.py's encoder of arkworks' 128-byte compressed proof.
 // Host-side formatting of a handful of points; included by ark_circom_b200.hpp after the verifier (needs pairing::Fq).
 #pragma once
 
@@ -134,4 +135,41 @@ struct VerifyingKey {
 };
 
 }  // namespace ethereum
+
+// ---------------------------------------------------------------------------------------------- ark-serialize
+// Proof::<Bn254>::serialize_compressed (ark-serialize 0.5, restated like ethereum.py's serialize_compressed, byte for byte
+// equal to it): A.x (32 B), B.x.c0, B.x.c1, C.x, little-endian; the flags of each point ride in the top two bits of its last
+// byte: bit 6 = infinity, bit 7 = y is the larger of {y, -y} (Fq2: c1 compared first, then c0).
+typedef std::array<uint8_t, 128> CompressedProof;
+
+namespace detail_eth {
+// canonical little-endian coordinate y (32 B) against p - y (0 for y = 0): -1, 0 or 1
+inline int cmp_neg(const uint8_t* yb) {
+    uint64_t y[4], n[4] = {0, 0, 0, 0};
+    memcpy(y, yb, 32);
+    if (y[0] | y[1] | y[2] | y[3]) {
+        unsigned __int128 br = 0;
+        for (int i = 0; i < 4; i++) { unsigned __int128 t = (unsigned __int128)detail::FQ_P[i] - y[i] - (uint64_t)br; n[i] = (uint64_t)t; br = (t >> 64) & 1; }
+    }
+    for (int i = 3; i >= 0; i--) if (y[i] != n[i]) return y[i] > n[i] ? 1 : -1;
+    return 0;
+}
+inline bool all_zero(const uint8_t* b, size_t n) { for (size_t i = 0; i < n; i++) if (b[i]) return false; return true; }
+}  // namespace detail_eth
+
+inline CompressedProof serialize_compressed(const Proof& p) {
+    CompressedProof out;
+    const uint8_t* b = p.bytes;
+    auto g1 = [&](uint8_t* o, const uint8_t* xy) {
+        memcpy(o, xy, 32);
+        o[31] |= detail_eth::all_zero(xy, 64) ? 0x40 : (detail_eth::cmp_neg(xy + 32) > 0 ? 0x80 : 0);
+    };
+    g1(out.data(), b);
+    memcpy(out.data() + 32, b + 64, 64);                                   // B.x.c0, B.x.c1
+    const int c1 = detail_eth::cmp_neg(b + 160);
+    out[95] |= detail_eth::all_zero(b + 64, 128) ? 0x40 : ((c1 ? c1 : detail_eth::cmp_neg(b + 128)) > 0 ? 0x80 : 0);
+    g1(out.data() + 96, b + 192);
+    return out;
+}
+
 }  // namespace ark_circom

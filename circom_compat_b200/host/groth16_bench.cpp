@@ -3,13 +3,17 @@
 //
 //   groth16_bench --parse-only <circuit.zkey> [--dump-key]         host-only: print what read_zkey produced (no GPU)
 //   groth16_bench --verify <circuit.zkey> <proof_hex> [inputs...]  host-only: process_vk + verify_with_processed_vk
-//   groth16_bench --ethereum <circuit.zkey> <proof_hex> [inputs...] host-only: src/ethereum.rs views of vk / proof / inputs, both directions
+//   groth16_bench --ethereum <circuit.zkey> <proof_hex> [inputs...] host-only: src/ethereum.rs views of vk / proof / inputs, both directions,
+//                                                                   and the proof's ark-serialize compressed bytes
 //   groth16_bench <circuit.zkey> chain:<a>|<witness.wtns> [iters] [r_hex s_hex]
 //       B2G_MANY=K: also K proofs in one device pass (Groth16::create_proofs)
 //       B2G_VERIFY_MANY=K: also prove K proofs, negate A in every other one, and compare Groth16::verify_many's verdicts with
 //       verify_with_processed_vk called per proof (timing both)
 //       B2G_VERIFY_BATCH=K: also prove K proofs and compare Groth16::verify_batch's verdict, on them and with the last
 //       proof's A negated, with verify_with_processed_vk over every proof (timing the batch call)
+//       B2G_VERIFY_COMPRESSED=K: also prove K proofs, serialize them compressed, flip the sign bit of A in every other one,
+//       compare Groth16::verify_many_compressed's verdicts with the host verifier, decode the untouched ones back, and print
+//       Groth16::verify_batch_compressed's verdict on the untouched and on the flipped set
 //       chain:<a> = the witness of the reference's squaring-chain bench family for input a
 //       (test-vectors/complex-circuit/input.json has a = 3), computed on the host instead of by WASM.
 #include <chrono>
@@ -134,7 +138,9 @@ int main(int argc, char** argv) {
             std::vector<Fr> in2;
             for (const eth::U256& w : ein) in2.push_back(eth::u256_to_fr(w));
             for (size_t i = 0; i < inputs.size(); i++) rt = rt && in2[i] == inputs[i];
-            std::printf("roundtrip=%d\n", rt ? 1 : 0);
+            std::printf("roundtrip=%d\ncompressed=", rt ? 1 : 0);            // Proof::serialize_compressed
+            for (uint8_t b : serialize_compressed(proof)) std::printf("%02x", b);
+            std::printf("\n");
             std::printf("verified=%d\n", Groth16::verify_with_processed_vk(Groth16::process_vk(vk2), in2, p2) ? 1 : 0);
             return 0;
         }
@@ -263,6 +269,46 @@ int main(int argc, char** argv) {
             }
             std::printf("verify_batch %d proofs: valid=%d tampered=%d host=%d/%d agree=%d, device %.3f ms/batch (%.1f proofs/s)\n", k,
                         valid && again, tampered, host, host_bad, (valid && again) == host && tampered == host_bad, dev_ms, k / (dev_ms / 1e3));
+        }
+        if (const char* vc = std::getenv("B2G_VERIFY_COMPRESSED")) {     // compressed proofs decoded on the device, against the host
+            const int k = std::atoi(vc);
+            if (k < 1) throw SynthesisError("B2G_VERIFY_COMPRESSED must be >= 1");
+            std::vector<std::vector<Fr>> wv((size_t)k, full_assignment);
+            if (wsrc.rfind("chain:", 0) == 0)
+                for (int i = 1; i < k; i++) wv[(size_t)i] = chain_witness(params.a_query.size(), std::stoull(wsrc.substr(6)) + (unsigned long long)i);
+            std::vector<const std::vector<Fr>*> ws;
+            for (const auto& w : wv) ws.push_back(&w);
+            std::mt19937_64 rng(0xC0C0);
+            std::vector<std::pair<Fr, Fr>> rs;
+            for (int i = 0; i < k; i++) rs.push_back({Fr::rand(rng), Fr::rand(rng)});
+            const std::vector<Proof> proofs = Groth16::create_proofs(params, matrices, rs, ws);
+            std::vector<std::vector<Fr>> inputs;
+            for (const auto& w : wv) inputs.emplace_back(w.begin() + 1, w.begin() + num_inputs);
+            std::vector<CompressedProof> blobs, flipped;
+            for (const Proof& p : proofs) blobs.push_back(serialize_compressed(p));
+            flipped = blobs;
+            for (int i = 1; i < k; i += 2) flipped[(size_t)i][31] ^= 0x80;  // the sign bit of A: A -> -A
+            std::vector<Proof> negated = proofs;                          // the same proofs uncompressed: y -> p - y
+            for (int i = 1; i < k; i += 2) {
+                uint64_t y[4], d[4]; memcpy(y, negated[(size_t)i].bytes + 32, 32);
+                unsigned __int128 borrow = 0;
+                for (int j = 0; j < 4; j++) { unsigned __int128 t = (unsigned __int128)detail::FQ_P[j] - y[j] - borrow; d[j] = (uint64_t)t; borrow = (t >> 64) & 1; }
+                memcpy(negated[(size_t)i].bytes + 32, d, 32);
+            }
+            auto pvk = Groth16::process_vk(params.vk);
+            const std::vector<bool> got = Groth16::verify_many_compressed(pvk, inputs, flipped);
+            int agree = 1, valid = 0;
+            for (int i = 0; i < k; i++) {
+                const bool host = Groth16::verify_with_processed_vk(pvk, inputs[(size_t)i], negated[(size_t)i]);
+                agree &= host == got[(size_t)i];
+                valid += host;
+            }
+            const auto decoded = Groth16::decompress_proofs(blobs);
+            int round_trip = 1;
+            for (int i = 0; i < k; i++) round_trip &= decoded[(size_t)i].has_value() && !memcmp(decoded[(size_t)i]->bytes, proofs[(size_t)i].bytes, 256);
+            const bool batch = Groth16::verify_batch_compressed(pvk, inputs, blobs), batch_flipped = Groth16::verify_batch_compressed(pvk, inputs, flipped);
+            std::printf("verify_compressed %d proofs (%d valid): many agree=%d, batch valid=%d flipped=%d, round trip=%d\n", k, valid, agree,
+                        batch, batch_flipped, round_trip);
         }
         return 0;
     } catch (const std::exception& e) {

@@ -18,6 +18,8 @@
  *   b2g_verify_many        <- GrothBn::verify_with_processed_vk(&pvk, &inputs, &proof) (src/zkey.rs:869-870, 915-916), called
  *                             for many proofs of one key in one device pass
  *   b2g_verify_batch       <- the same check for a whole batch at once, as one random linear combination of the proofs
+ *   b2g_proofs_decompress  <- Proof::<Bn254>::deserialize_compressed (ark-serialize 0.5, Validate::Yes), for many proofs
+ *   b2g_verify_many_compressed / b2g_verify_batch_compressed <- deserialize_compressed followed by the two calls above
  *   b2g_fixed_base_g1/g2   <- the batch fixed-base multiplications of generate_random_parameters_with_reduction
  *                             (tests/groth16.rs:25); used to manufacture synthetic proving keys
  *
@@ -243,6 +245,31 @@ B2G_API int b2g_verify_many(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void
 B2G_API int b2g_verify_batch(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs,
                              const void* weights, uint8_t* verdict_out);
 
+/* Compressed proofs: the 128-byte form of Proof::<Bn254>::serialize_compressed (ark-serialize 0.5) that arkworks-based
+ * systems store and send: A.x (32 B), B.x.c0 (32 B), B.x.c1 (32 B), C.x (32 B), little-endian, each point's flags in the top
+ * two bits of its last byte (bit 7: y is the larger of {y, -y}; bit 6: infinity).  A proof decodes as
+ * Proof::<Bn254>::deserialize_compressed (Validate::Yes) decodes it: both flag bits set, a value >= p with the flags masked
+ * off (infinity flag or not), an x whose y^2 has no square root, or a B outside G2 make it undecodable.  An undecodable proof
+ * is never an error: it is invalid.  The decoding runs on the device, one proof per thread (csrc/verify.cu restates the rules).
+ *
+ * b2g_proofs_decompress <- Proof::<Bn254>::deserialize_compressed (ark-serialize 0.5, Validate::Yes) for count proofs in one
+ * device pass.  compressed = count x 128 B; proofs_out = count x 256 B in the b2g_prove layout (a point at infinity = zeros);
+ * ok_out = count bytes (1 decoded, 0 not; the row of an undecodable proof is 256 bytes of 0xFF, which b2g_verify_many reports
+ * invalid).  Synchronous.  Errors: B2G_E_SHAPE for count == 0, null pointers or a proof pending on the context;
+ * B2G_E_DEVICE when the buffers do not fit (the context stays usable). */
+B2G_API int b2g_proofs_decompress(b2g_ctx* ctx, uint32_t count, const void* compressed, uint8_t* proofs_out, uint8_t* ok_out);
+/* b2g_verify_many_compressed <- deserialize_compressed followed by GrothBn::verify_with_processed_vk (src/zkey.rs:869-870,
+ * 915-916), for count proofs of one key; b2g_verify_many on compressed proofs, decoded on the device without a round trip
+ * through the host.  compressed = count x 128 B; the other arguments, the errors and the buffers as b2g_verify_many.  A verdict
+ * is 1 exactly when the proof decodes (G2 check of B included) and the decoded proof passes b2g_verify_many. */
+B2G_API int b2g_verify_many_compressed(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs,
+                                       const void* compressed, uint8_t* verdicts_out);
+/* b2g_verify_batch_compressed <- deserialize_compressed followed by the batch check of b2g_verify_batch.  compressed = count x
+ * 128 B; the other arguments, the errors and the soundness statement as b2g_verify_batch.  The verdict is 1 exactly when every
+ * proof decodes and b2g_verify_batch with the same weights gives 1 on the decoded rows. */
+B2G_API int b2g_verify_batch_compressed(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs,
+                                        const void* compressed, const void* weights, uint8_t* verdict_out);
+
 /* Kernel-level entry points (parity tests, benchmarks). All pointers host. */
 B2G_API int b2g_msm_g1(b2g_ctx* ctx, const void* bases, const void* scalars, size_t n, int scalars_mont, void* out_xy_mont);
 B2G_API int b2g_msm_g2(b2g_ctx* ctx, const void* bases, const void* scalars, size_t n, int scalars_mont, void* out_xy_mont);
@@ -275,6 +302,12 @@ B2G_API int b2g_fixed_base_g2(b2g_ctx* ctx, const void* scalars_canon, size_t n,
  *     43 G2 membership of a (128 B G2 affine, on the twist): out = 8 B, 1 if a is in G2 (or infinity), else 0,
  *     44 r * a for a G1 affine a (64 B) and a 128-bit r (b: 16 B little-endian): out = 64 B affine,
  *     45 a^k for a cyclotomic Fq12 a and a canonical 256-bit k (b: 32 B): out = 384 B.
+ * Ops 46-48 are the compressed-proof decoder's pieces (b ignored); each result is followed by a 32 B slot whose first 64-bit
+ * word is 1 when there is a root / the point decodes, else 0:
+ *     46 a square root of a (32 B Fq, mont): out = 64 B, the root (mont) then the slot,
+ *     47 a square root of a (64 B Fq2, mont): out = 96 B,
+ *     48 one compressed G2 point a (64 B: x.c0, then x.c1 with the flags) decoded without the G2 check: out = 160 B, the
+ *        canonical affine point (zeros at infinity, 0xFF bytes when it does not decode) then the slot.
  * Operand and result sizes per row therefore differ by op; b may be NULL where the op does not read it. */
 B2G_API int b2g_test_op(b2g_ctx* ctx, int op, const void* a, const void* b, size_t n, void* out);
 
