@@ -361,7 +361,8 @@ __device__ __noinline__ void ell_fixed(fe12& f, int i, int nfix, const Affine<Fq
 // (f = 1 there); every line of a step is multiplied in for all pairs.  The pair counts are template parameters: one
 // specialised loop per shape keeps the absent pairs' code out of it.  A single loop taking the counts at run time, and
 // this loop with ell_fixed inlined, both gave values that differ from the model on sm_90a (CUDA 12.9), while this form
-// matches it bit for bit (tests/test_verify_many.py); the cause was not found.
+// matches it bit for bit; the cause was not found.  Each kernel gets its own compiled copy of these calls, so the tests run
+// the shipped kernels themselves: verify_miller_kernel (test op 49) and batch_pairs_kernel (op 53), tests/test_verify_stages.py.
 template <bool V_ON, int NFIX>
 __device__ __noinline__ void miller_loop_t(fe12& f, const Affine<Fq>& vp, const Affine<Fq2>& vq, const Affine<Fq>* fp,
                                            const uint8_t* const* lines) {

@@ -528,8 +528,91 @@ __global__ void pairing_test_kernel(int op, const uint8_t* __restrict__ a, const
     Fq12::store(out + (size_t)i * F12_BYTES, r);
 }
 
+static bool all_zero(const void* p, size_t n);
+
+// ops 49-53 (see include/b2groth.h) run the kernels the verifier runs, not test copies of them: ptxas compiles each kernel
+// with its own copy of the __noinline__ calls it reaches (miller_loop_t, ell_fixed, the tower), so only a launch of the
+// shipped kernel tests the shipped machine code.  Per row of ops 49 and 53, a staging region holds the key's G2 points for
+// vk_lines_kernel (an unused slot, gamma, delta), then the row's proof record (op 49) or batch tail (op 53), then the lines
+// of -gamma and -delta; a point given as zeros is infinity and drops its pair, as in b2g_vk_load.
+constexpr size_t STAGE_G2 = 0, STAGE_REC = 384, STAGE_LINES = STAGE_REC + TAIL_BYTES, STAGE_BYTES = STAGE_LINES + 2 * ATE_LINES * LINE_BYTES;
+
+static void verify_stage_test_op(cudaStream_t st, int op, const void* a, const void* b, size_t n, void* out) {
+    if (op == 51 && !b) throw_error(B2G_E_SHAPE, "this op needs operand b");
+    const size_t sa = op == 49 ? 576 : (op == 50 ? 128 : (op == 51 ? 32 : (op == 52 ? 64 : 512)));
+    const size_t so = (op == 49 || op == 53) ? F12_BYTES : (op == 50 ? ATE_LINES * LINE_BYTES : (op == 51 ? 128 : TABLE_BYTES));
+    if (n == 0) return;
+    struct Bufs { uint8_t *a = nullptr, *s = nullptr, *o = nullptr; ~Bufs() { for (void* p : {(void*)a, (void*)s, (void*)o}) if (p) cudaFree(p); } } d;
+    const uint8_t* in = (const uint8_t*)a;
+    if (op == 49 || op == 53) {
+        // op 49 row: A (64 B), B (128 B), the prepared inputs (64 B), C (64 B), gamma, delta (128 B each) -> a verify_many
+        // record; op 53 row: the prepared inputs and sum r C (XYZZ, 128 B each), gamma, delta -> a verify_batch tail
+        std::vector<uint8_t> stage(n * STAGE_BYTES, 0);
+        std::vector<uint8_t> on(2 * n);
+        for (size_t i = 0; i < n; i++) {
+            const uint8_t* row = in + i * sa;
+            uint8_t* g = stage.data() + i * STAGE_BYTES;
+            const uint8_t* q = row + (op == 49 ? 320 : 256);
+            memcpy(g + STAGE_G2 + 128, q, 256);
+            on[2 * i] = !all_zero(q, 128);
+            on[2 * i + 1] = !all_zero(q + 128, 128);
+            uint8_t* r = g + STAGE_REC;
+            if (op == 49) {
+                memcpy(r, row, 64);                             // A
+                memcpy(r + 64, row + 64, 128);                  // B
+                memcpy(r + 192, row + 256, 64);                 // C
+                memcpy(r + 256, row + 192, 64);                 // the prepared inputs
+                *reinterpret_cast<uint32_t*>(r + REC_OK) = 1;
+            } else {
+                memcpy(r + TAIL_PREP, row, 128);
+                memcpy(r + TAIL_RC, row + 128, 128);
+            }
+        }
+        d.s = dev_upload<uint8_t>(stage.data(), stage.size(), st);
+        CUDA_CHECK(cudaMalloc(&d.o, n * so));
+        for (size_t i = 0; i < n; i++) {
+            uint8_t* g = d.s + i * STAGE_BYTES;
+            vk_lines_kernel<<<1, 32, 0, st>>>(g + STAGE_G2, g + STAGE_LINES);
+            if (op == 49) {
+                verify_miller_kernel<<<1, 64, 0, st>>>(g + STAGE_REC, g + STAGE_LINES, on[2 * i], on[2 * i + 1], 1, d.o + i * F12_BYTES);
+            } else {
+                batch_pairs_kernel<<<1, 1, 0, st>>>(g + STAGE_REC, g + STAGE_LINES, on[2 * i], on[2 * i + 1]);
+                CUDA_CHECK(cudaMemcpyAsync(d.o + i * F12_BYTES, g + STAGE_REC + TAIL_G, F12_BYTES, cudaMemcpyDeviceToDevice, st));
+            }
+        }
+        g_launch_count += 2 * n;
+    } else if (op == 50) {
+        // the lines of -a: rows 2k and 2k + 1 are the gamma and delta of one vk_lines_kernel launch
+        const size_t pairs = (n + 1) / 2;
+        std::vector<uint8_t> g2(pairs * 384, 0);
+        for (size_t i = 0; i < n; i++) memcpy(g2.data() + (i / 2) * 384 + 128 * (1 + i % 2), in + i * 128, 128);
+        d.a = dev_upload<uint8_t>(g2.data(), g2.size(), st);
+        CUDA_CHECK(cudaMalloc(&d.o, 2 * pairs * so));
+        for (size_t k = 0; k < pairs; k++) vk_lines_kernel<<<1, 32, 0, st>>>(d.a + k * 384, d.o + 2 * k * so);
+        g_launch_count += pairs;
+    } else if (op == 51) {
+        d.a = dev_upload<uint8_t>(a, n * sa, st);
+        CUDA_CHECK(cudaMalloc(&d.o, n * so));
+        CUDA_CHECK(cudaMalloc(&d.s, 256 + TABLE_BYTES));                // the point, then its table
+        CUDA_CHECK(cudaMemcpyAsync(d.s, b, 64, cudaMemcpyHostToDevice, st));
+        fixed_table_kernel<G1, Fq><<<(32 * 255 + 63) / 64, 64, 0, st>>>(d.s + 256, d.s);
+        verify_inputs_kernel<<<(unsigned)((n + 3) / 4), 128, 0, st>>>(d.s + 256, (const uint32_t*)d.a, 1, n, d.o);
+        g_launch_count += 2;
+    } else {
+        d.a = dev_upload<uint8_t>(a, n * sa, st);
+        CUDA_CHECK(cudaMalloc(&d.o, n * so));
+        for (size_t i = 0; i < n; i++)
+            fixed_table_kernel<G1, Fq><<<(32 * 255 + 63) / 64, 64, 0, st>>>(d.o + i * TABLE_BYTES, d.a + i * 64);
+        g_launch_count += n;
+    }
+    CUDA_CHECK(cudaGetLastError());
+    CUDA_CHECK(cudaMemcpyAsync(out, d.o, n * so, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaStreamSynchronize(st));
+}
+
 void pairing_test_op(cudaStream_t st, int op, const void* a, const void* b, size_t n, void* out) {
-    if (op > 48 || !a || !out) throw_error(B2G_E_SHAPE, "bad arguments");
+    if (op > 53 || !a || !out) throw_error(B2G_E_SHAPE, "bad arguments");
+    if (op >= 49) { verify_stage_test_op(st, op, a, b, n, out); return; }
     const bool batch_op = op >= 43 && op <= 45, decompress_op = op >= 46;
     size_t sa = (op == 37 || op == 40) ? 64 : ((op == 41 || op == 42) ? LINE_BYTES : F12_BYTES);
     size_t sb = op == 30 ? F12_BYTES : ((op == 37 || op == 40 || op == 42) ? 128 : (op == 39 ? LINE_BYTES : 0));

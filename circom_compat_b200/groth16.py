@@ -51,7 +51,11 @@ _TEST_OP_WORDS = {**{op: (4, 4, 4) for op in (0, 1, 2, 3, 4, 5, 14, 15, 16)}, 6:
                   # the batch check's pieces: G2 membership, 128-bit G1 product, cyclotomic exponentiation
                   43: (16, 0, 1), 44: (8, 2, 8), 45: (48, 4, 48),
                   # the compressed-proof decoder's pieces: Fq and Fq2 square roots, one compressed G2 point (result, then a flag slot)
-                  46: (4, 0, 8), 47: (8, 0, 12), 48: (8, 0, 20)}
+                  46: (4, 0, 8), 47: (8, 0, 12), 48: (8, 0, 20),
+                  # the verifier's stages: a verify_many Miller value, prepared lines, the window-table product (b: one
+                  # G1 point for every row), the window table and verify_batch's prepared-pair Miller value
+                  49: (72, 0, 48), 50: (16, 0, 88 * 24), 51: (4, 8, 16), 52: (8, 0, 32 * 255 * 8), 53: (64, 0, 48)}
+_TEST_OP_B_ONCE = {51}        # ops whose operand b is one row for all rows of a
 TEST_PAIR_RUN = 16            # entries per row of op 27; an entry is 16 words of affine point + 4 words whose bit 0 is the sign
 
 
@@ -224,8 +228,9 @@ class Context:
         a = _c(a); b = _c(b) if b is not None else None
         a_words, b_words, out_words = _TEST_OP_WORDS.get(op, (4, 4, 4))    # an unknown op is refused by the library
         n = a.size // a_words
-        if b is not None and b_words and b.size < n * b_words:
-            raise ValueError(f"test op {op}: operand b holds fewer than {n} rows of {b_words} words")
+        b_rows = 1 if op in _TEST_OP_B_ONCE else n
+        if b is not None and b_words and b.size < b_rows * b_words:
+            raise ValueError(f"test op {op}: operand b holds fewer than {b_rows} rows of {b_words} words")
         out = np.zeros((n, out_words), dtype=np.uint64)
         N.check(N.lib().b2g_test_op(self._h, op, _ptr(a), _ptr(b) if b is not None else None, n, _ptr(out)))
         return out

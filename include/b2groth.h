@@ -308,6 +308,17 @@ B2G_API int b2g_fixed_base_g2(b2g_ctx* ctx, const void* scalars_canon, size_t n,
  *     47 a square root of a (64 B Fq2, mont): out = 96 B,
  *     48 one compressed G2 point a (64 B: x.c0, then x.c1 with the flags) decoded without the G2 check: out = 160 B, the
  *        canonical affine point (zeros at infinity, 0xFF bytes when it does not decode) then the slot.
+ * Ops 49-53 are the verifier's stages, each a launch of the kernel b2g_vk_load, b2g_verify_many or b2g_verify_batch runs
+ * (b ignored unless stated; gamma and delta are G2 affine, 128 B, zeros = infinity, and their lines are those of -gamma and
+ * -delta, prepared as b2g_vk_load prepares them):
+ *     49 the Miller value of one verify_many proof record: a = 576 B, A (G1 64 B), B (G2 128 B), the prepared inputs and C
+ *        (G1 64 B each), gamma, delta; a pair with a point at infinity contributes 1: out = 384 B,
+ *     50 the prepared lines of -a for a G2 affine a (128 B, not infinity): out = 88 lines of c0 || c1 || c2 (88 x 192 B),
+ *     51 x * P from the 8-bit window table of P as the public-input kernel computes it: a = x (32 B canonical), b = one G1
+ *        affine P for all rows (64 B): out = 128 B XYZZ,
+ *     52 the 8-bit window table of a G1 affine a (64 B): out = 32 x 255 affine points d * 256^w * a (w-major),
+ *     53 the Miller value of verify_batch's two prepared pairs: a = 512 B, the prepared inputs and sum r C (G1 XYZZ, 128 B
+ *        each), gamma, delta: out = 384 B.
  * Operand and result sizes per row therefore differ by op; b may be NULL where the op does not read it. */
 B2G_API int b2g_test_op(b2g_ctx* ctx, int op, const void* a, const void* b, size_t n, void* out);
 
