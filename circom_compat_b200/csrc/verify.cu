@@ -70,7 +70,7 @@ struct VerifyBufs {
     uint8_t* d_batch = nullptr;                   // b2g_verify_batch: weights, reduction levels, scalar sums, tail values
     uint8_t* d_comp = nullptr;                    // compressed proofs (128 B each), then one decoded-ok byte per proof
     cudaStream_t side[2] = {nullptr, nullptr};    // b2g_verify_batch's tail pieces, next to the per-proof kernels
-    cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
+    cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
 };
 
 void verify_bufs_free(VerifyBufs* v) {
@@ -277,7 +277,7 @@ __global__ void __launch_bounds__(128) g1_sum_kernel(const uint8_t* __restrict__
 }
 
 // the Miller value of the prepared pairs (prepared inputs, -gamma) and (sum r C, -delta); 1 when both drop out
-__global__ void batch_pairs_kernel(uint8_t* __restrict__ tail, const uint8_t* __restrict__ lines, bool gamma_on, bool delta_on) {
+__device__ __forceinline__ void tail_pairs(uint8_t* tail, const uint8_t* lines, bool gamma_on, bool delta_on) {
     const G1::Aff prep = G1::to_affine(pt_load<Fq>(tail + TAIL_PREP, 0)), c = G1::to_affine(pt_load<Fq>(tail + TAIL_RC, 0));
     G1::Aff fp[2];
     const uint8_t* fl[2];
@@ -290,6 +290,10 @@ __global__ void batch_pairs_kernel(uint8_t* __restrict__ tail, const uint8_t* __
     Fq12::store(tail + TAIL_G, g);
 }
 
+__global__ void batch_pairs_kernel(uint8_t* __restrict__ tail, const uint8_t* __restrict__ lines, bool gamma_on, bool delta_on) {
+    tail_pairs(tail, lines, gamma_on, delta_on);
+}
+
 // e(alpha, beta)^s_0
 __global__ void batch_rhs_kernel(uint8_t* __restrict__ tail, const uint8_t* __restrict__ eab) {
     fe12 rhs;
@@ -298,7 +302,16 @@ __global__ void batch_rhs_kernel(uint8_t* __restrict__ tail, const uint8_t* __re
     Fq12::store(tail + TAIL_RHS, rhs);
 }
 
-// the verdict: ok, and the final exponentiation of (per-proof product) x (prepared pairs) equals e(alpha, beta)^s_0
+// the final exponentiation of (per-proof product) x (prepared pairs) equals e(alpha, beta)^s_0 (batch_final_kernel keeps
+// its own copy of these lines: calling this from it changes its register count)
+__device__ __forceinline__ bool tail_holds(const uint8_t* tail) {
+    fe12 f = Fq12::load(tail + TAIL_F), e;
+    Fq12::mul(f, f, Fq12::load(tail + TAIL_G));
+    Fq12::final_exponentiation(e, f);
+    return Fq12::eq(e, Fq12::load(tail + TAIL_RHS));
+}
+
+// the verdict: ok, and the batch equation holds
 __global__ void batch_final_kernel(const uint8_t* __restrict__ tail, const uint32_t* __restrict__ ok_all, uint8_t* __restrict__ verdict) {
     if (!*ok_all) { *verdict = 0; return; }
     fe12 f = Fq12::load(tail + TAIL_F), e;
@@ -325,6 +338,119 @@ __global__ void batch_test_kernel(int op, const uint8_t* __restrict__ a, const u
         Fq12::cyclotomic_exp(r, Fq12::load(a + (size_t)i * F12_BYTES), k.l);
         Fq12::store(out + (size_t)i * F12_BYTES, r);
     }
+}
+
+// ---------------------------------------------------------------------------------------------- b2g_verify_batch_locate kernels
+// The batch check above, once per group of LOCATE_GROUP consecutive proofs, over the group's well-formed proofs only.  The
+// per-proof work is batch_prepare_kernel on a zeroed record area, so that a malformed proof keeps r A and r C at infinity,
+// and batch_miller_kernel with an ok word nothing clears, so that every proof gets its Miller value.  wf[i] is 1 when proof
+// i parses and its B lies in G2; every group product and sum below leaves out the proofs with wf[i] = 0.  Group g's tail
+// values (the TAIL_* offsets) sit at tails + g * TAIL_BYTES.
+constexpr uint32_t LOCATE_GROUP = 64;              // proofs per group: one CTA of locate_product_kernel
+static_assert(TAIL_BYTES % 256 == 0, "group tails stay 256-byte aligned");
+
+// one proof per thread, on a side stream next to the per-proof chain: wf[j] = the proof parses and its B lies in G2
+__global__ void __launch_bounds__(128) locate_g2_kernel(const uint8_t* __restrict__ proofs, uint32_t count, uint8_t* __restrict__ wf) {
+    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= count) return;
+    G1::Aff a, cc; G2::Aff b;
+    wf[j] = proof_parse(proofs + (size_t)j * 256, a, b, cc) && g2_in_subgroup(b);
+}
+
+// one warp per (group g, j = 0..n_public), t = g * (n_public + 1) + j: s_gj = the sum of r_i x_ij over the group's well-formed
+// proofs (x_i0 = 1), then pts[t] = s_gj IC[j] (IC[0]: a variable-base product of a scalar below 64 x 2^128); s_g0 to the tail
+__global__ void __launch_bounds__(128) locate_inputs_kernel(const uint8_t* __restrict__ tabs, const uint8_t* __restrict__ g1,
+                                                            const uint32_t* __restrict__ w, const uint32_t* __restrict__ pub,
+                                                            const uint8_t* __restrict__ wf, uint32_t n_public, uint32_t count,
+                                                            uint32_t groups, uint8_t* __restrict__ pts, uint8_t* __restrict__ tails) {
+    __shared__ G1::Pt sh[4][32];
+    __shared__ fe s[4];
+    const uint32_t wid = threadIdx.x >> 5, lane = threadIdx.x & 31, n_pts = n_public + 1;
+    const size_t t = (size_t)blockIdx.x * 4 + wid;
+    if (t >= (size_t)groups * n_pts) return;               // whole warps leave together
+    const uint32_t g = (uint32_t)(t / n_pts), j = (uint32_t)(t % n_pts);
+    fe acc = Fr::zero();
+    for (uint32_t k = lane; k < LOCATE_GROUP; k += 32) {
+        const uint32_t i = g * LOCATE_GROUP + k;
+        if (i >= count || !wf[i]) continue;
+        fe wi = fe_zero();
+        weight_load(wi.l, w, i);
+        acc = Fr::add(acc, j ? Fr::mul(wi, fe_load(pub + 8 * ((size_t)i * n_public + j - 1))) : wi);
+    }
+    for (int d = 16; d > 0; d >>= 1) {
+        fe o;
+        for (int q = 0; q < 8; q++) o.l[q] = __shfl_down_sync(0xffffffffu, acc.l[q], d);
+        acc = Fr::add(acc, o);
+    }
+    if (lane == 0) s[wid] = j ? Fr::from_canonical(acc) : acc;   // from_canonical cancels the products' 1 / R
+    __syncwarp();
+    if (j) {
+        const G1::Pt p = warp_fixed_mul<G1, Fq>(tabs + (size_t)(j - 1) * TABLE_BYTES, s[wid].l, sh[wid]);
+        if (lane == 0) pt_store<Fq>(pts, t, p);
+    } else if (lane == 0) {
+        pt_store<Fq>(pts, t, G1::mul_scalar(G1::from_affine(aff_load<Fq>(g1, 1)), s[wid].l));
+        fe_store(tails + (size_t)g * TAIL_BYTES + TAIL_S0, s[wid]);
+    }
+}
+
+// CTA b: dst + b * dst_stride = the sum of src[seg * b .. seg * b + seg - 1] below n (G1 XYZZ, `stride` bytes apart), leaving
+// out record i when mask[i] = 0 (no mask: every record)
+__global__ void __launch_bounds__(128) g1_segment_sum_kernel(const uint8_t* __restrict__ src, size_t stride, uint32_t seg, size_t n,
+                                                             const uint8_t* __restrict__ mask, uint8_t* __restrict__ dst, size_t dst_stride) {
+    __shared__ G1::Pt sh[128];
+    const uint32_t t = threadIdx.x;
+    G1::Pt acc = G1::infinity();
+    for (uint32_t k = t; k < seg; k += 128) {
+        const size_t i = (size_t)blockIdx.x * seg + k;
+        if (i < n && (!mask || mask[i])) G1::add(acc, pt_load<Fq>(src + i * stride, 0));
+    }
+    sh[t] = acc;
+    __syncthreads();
+    for (uint32_t d = 64; d > 0; d >>= 1) {
+        if (t < d) { G1::Pt x = sh[t]; G1::add(x, sh[t + d]); sh[t] = x; }
+        __syncthreads();
+    }
+    if (t == 0) pt_store<Fq>(dst + (size_t)blockIdx.x * dst_stride, 0, sh[0]);
+}
+
+// CTA g: the product of the group's Miller values, 1 for a proof with wf[i] = 0
+__global__ void __launch_bounds__(64) locate_product_kernel(const uint8_t* __restrict__ f, const uint8_t* __restrict__ wf, uint32_t count,
+                                                            uint8_t* __restrict__ tails) {
+    static_assert(LOCATE_GROUP == 64, "one thread per proof of a group");
+    __shared__ fe12 sh[64];
+    const uint32_t t = threadIdx.x, i = blockIdx.x * 64 + t;
+    sh[t] = i < count && wf[i] ? Fq12::load(f + (size_t)i * F12_BYTES) : Fq12::one();
+    __syncthreads();
+    for (uint32_t d = 32; d > 0; d >>= 1) {
+        if (t < d) { fe12 x = sh[t]; Fq12::mul(x, x, sh[t + d]); sh[t] = x; }
+        __syncthreads();
+    }
+    if (t == 0) Fq12::store(tails + (size_t)blockIdx.x * TAIL_BYTES + TAIL_F, sh[0]);
+}
+
+// one group per thread: the Miller value of the group's prepared pairs
+__global__ void __launch_bounds__(64) locate_pairs_kernel(uint8_t* __restrict__ tails, uint32_t groups, const uint8_t* __restrict__ lines,
+                                                          bool gamma_on, bool delta_on) {
+    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g < groups) tail_pairs(tails + (size_t)g * TAIL_BYTES, lines, gamma_on, delta_on);
+}
+
+// one group per thread: e(alpha, beta)^s_g0
+__global__ void __launch_bounds__(64) locate_rhs_kernel(uint8_t* __restrict__ tails, uint32_t groups, const uint8_t* __restrict__ eab) {
+    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= groups) return;
+    uint8_t* tail = tails + (size_t)g * TAIL_BYTES;
+    fe12 rhs;
+    const fe s0 = fe_load(tail + TAIL_S0);
+    Fq12::cyclotomic_exp(rhs, Fq12::load(eab), s0.l);
+    Fq12::store(tail + TAIL_RHS, rhs);
+}
+
+// one group per thread: verdict[g] = the group's batch equation holds.  A group without a well-formed proof has every
+// value at 1 (product, pairs and e(alpha, beta)^0), so it holds.
+__global__ void __launch_bounds__(64) locate_final_kernel(const uint8_t* __restrict__ tails, uint32_t groups, uint8_t* __restrict__ verdict) {
+    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g < groups) verdict[g] = tail_holds(tails + (size_t)g * TAIL_BYTES);
 }
 
 // ---------------------------------------------------------------------------------------------- compressed proofs
@@ -701,10 +827,11 @@ static uint8_t* decompress_enqueue(VerifyBufs& v, const void* compressed, uint32
     return ok;
 }
 
-// the two side streams and five events of b2g_verify_batch, created at its first call on the context.  The side streams have
-// the greatest priority, so that their one-thread tail kernels are scheduled ahead of queued per-proof CTAs.
+// the two side streams and six events of b2g_verify_batch and b2g_verify_batch_locate, created at the first such call on the
+// context.  The side streams have the greatest priority, so that their tail kernels are scheduled ahead of queued per-proof
+// CTAs.
 static void batch_streams(VerifyBufs& v) {
-    if (v.ev[4]) return;
+    if (v.ev[5]) return;
     int least = 0, greatest = 0;
     CUDA_CHECK(cudaDeviceGetStreamPriorityRange(&least, &greatest));
     for (cudaStream_t& s : v.side) if (!s) CUDA_CHECK(cudaStreamCreateWithPriority(&s, cudaStreamNonBlocking, greatest));
@@ -837,15 +964,11 @@ int b2g_proofs_decompress(b2g_ctx* ctx, uint32_t count, const void* compressed, 
     });
 }
 
-// b2g_verify_many on 256-byte rows, or on compressed rows decoded on the device (G2 check included)
-static void verify_many_run(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs,
-                            bool compressed, uint8_t* verdicts_out) {
-    const CtxView cv = verify_args(fn, ctx, vk, count, public_inputs, proofs, verdicts_out);
+// b2g_verify_many's uploads and four kernels on st, on 256-byte rows or on compressed rows decoded first (G2 check
+// included); the verdicts go to v.d_verdict
+static void verify_many_enqueue(VerifyBufs& v, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs,
+                                bool compressed, cudaStream_t st) {
     const size_t inputs = (size_t)count * vk->n_public;
-    DevGuard g(cv.device);
-    cudaStream_t st = cv.st;
-    verify_bufs_ensure(fn, *cv.vbufs, count, inputs, inputs, 0, compressed ? comp_bytes(count) : 0);
-    VerifyBufs& v = **cv.vbufs;
     if (compressed) decompress_enqueue(v, proofs, count, true, st);
     else CUDA_CHECK(cudaMemcpyAsync(v.d_proofs, proofs, (size_t)count * 256, cudaMemcpyHostToDevice, st));
     if (inputs) {
@@ -857,8 +980,26 @@ static void verify_many_run(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t c
     verify_final_kernel<<<(count + 63) / 64, 64, 0, st>>>(v.d_rec, v.d_f, vk->d_eab, count, v.d_verdict);
     g_launch_count += 3 + (inputs ? 1 : 0);
     CUDA_CHECK(cudaGetLastError());
+}
+
+// b2g_verify_many on 256-byte rows, or on compressed rows decoded on the device (G2 check included)
+static void verify_many_run(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs,
+                            bool compressed, uint8_t* verdicts_out) {
+    const CtxView cv = verify_args(fn, ctx, vk, count, public_inputs, proofs, verdicts_out);
+    const size_t inputs = (size_t)count * vk->n_public;
+    DevGuard g(cv.device);
+    cudaStream_t st = cv.st;
+    verify_bufs_ensure(fn, *cv.vbufs, count, inputs, inputs, 0, compressed ? comp_bytes(count) : 0);
+    VerifyBufs& v = **cv.vbufs;
+    verify_many_enqueue(v, vk, count, public_inputs, proofs, compressed, st);
     CUDA_CHECK(cudaMemcpyAsync(verdicts_out, v.d_verdict, count, cudaMemcpyDeviceToHost, st));
     CUDA_CHECK(cudaStreamSynchronize(st));
+}
+
+// the batch verifiers' weight check: no weight is zero
+static void weights_check(const void* weights, uint32_t count) {
+    for (uint32_t i = 0; i < count; i++)
+        if (all_zero((const uint8_t*)weights + 16 * (size_t)i, 16)) throw_error(B2G_E_INPUT, "weight " + std::to_string(i) + " is zero");
 }
 
 // b2g_verify_batch on 256-byte rows, or on compressed rows decoded on the context's stream before anything else reads them
@@ -867,8 +1008,7 @@ static void verify_batch_run(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t 
                              bool compressed, const void* weights, uint8_t* verdict_out) {
     if (!weights) throw_error(B2G_E_SHAPE, "null pointer");
     const CtxView cv = verify_args(fn, ctx, vk, count, public_inputs, proofs, verdict_out);
-    for (uint32_t i = 0; i < count; i++)
-        if (all_zero((const uint8_t*)weights + 16 * (size_t)i, 16)) throw_error(B2G_E_INPUT, "weight " + std::to_string(i) + " is zero");
+    weights_check(weights, count);
     const uint32_t n_pts = vk->n_public + 1, chunks = (count + SCALAR_CHUNK - 1) / SCALAR_CHUNK;
     const size_t inputs = (size_t)count * vk->n_public;
     // scratch: weights, four reduction levels (x, y on the main stream, x2, y2 on the side streams), chunk sums of the
@@ -931,6 +1071,97 @@ static void verify_batch_run(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t 
     CUDA_CHECK(cudaStreamSynchronize(st));
 }
 
+// b2g_verify_batch_locate on 256-byte rows, or on compressed rows decoded on the context's stream first.  The batch check
+// runs once per group of LOCATE_GROUP proofs; the well-formed proofs of the groups that fail it then go through
+// b2g_verify_many's kernels, compacted on the host from the caller's rows.
+static void verify_locate_run(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs,
+                              bool compressed, const void* weights, uint8_t* verdicts_out) {
+    if (!weights) throw_error(B2G_E_SHAPE, "null pointer");
+    const CtxView cv = verify_args(fn, ctx, vk, count, public_inputs, proofs, verdicts_out);
+    weights_check(weights, count);
+    const uint32_t n_public = vk->n_public, n_pts = n_public + 1, groups = (count + LOCATE_GROUP - 1) / LOCATE_GROUP;
+    const size_t inputs = (size_t)count * n_public, comp = compressed ? comp_bytes(count) : 0;
+    // scratch: weights, s_gj IC[j] per (group, j), the group tails, wf per proof, the group verdicts and two ok words (the
+    // one batch_prepare_kernel clears, and the one batch_miller_kernel reads, which stays set)
+    auto up = [](size_t b) { return (b + 255) & ~(size_t)255; };
+    const size_t o_w = 0, o_pts = up((size_t)count * 16), o_tail = o_pts + up((size_t)groups * n_pts * 128);
+    const size_t o_wf = o_tail + (size_t)groups * TAIL_BYTES, o_gv = o_wf + up(count), o_ok = o_gv + up(groups), bytes = o_ok + 256;
+    DevGuard g(cv.device);
+    cudaStream_t st = cv.st;
+    verify_bufs_ensure(fn, *cv.vbufs, count, inputs, 0, bytes, comp);
+    VerifyBufs& v = **cv.vbufs;
+    batch_streams(v);
+    cudaStream_t s2 = v.side[0], s3 = v.side[1];
+    cudaEvent_t ev_up = v.ev[0], ev_prep = v.ev[1], ev_g2 = v.ev[2], ev_pts = v.ev[3], ev_s2 = v.ev[4], ev_s3 = v.ev[5];
+    uint8_t* B = v.d_batch;
+    uint8_t *tails = B + o_tail, *wf = B + o_wf, *gv = B + o_gv;
+    const uint32_t* w = (const uint32_t*)(B + o_w);
+    uint32_t* ok = (uint32_t*)(B + o_ok);
+    if (compressed) decompress_enqueue(v, proofs, count, false, st);
+    else CUDA_CHECK(cudaMemcpyAsync(v.d_proofs, proofs, (size_t)count * 256, cudaMemcpyHostToDevice, st));
+    CUDA_CHECK(cudaMemcpyAsync(B + o_w, weights, (size_t)count * 16, cudaMemcpyHostToDevice, st));
+    if (inputs) CUDA_CHECK(cudaMemcpyAsync(v.d_pub, public_inputs, inputs * 32, cudaMemcpyHostToDevice, st));
+    CUDA_CHECK(cudaMemsetAsync(ok, 0xff, 8, st));
+    CUDA_CHECK(cudaMemsetAsync(v.d_rec, 0, (size_t)count * REC_BYTES_V, st));
+    CUDA_CHECK(cudaEventRecord(ev_up, st));
+    // main stream: per-proof parse and scaling, every proof's Miller value, the group products, then the group verdicts
+    batch_prepare_kernel<<<(count + 127) / 128, 128, 0, st>>>(v.d_proofs, w, count, v.d_rec, ok);
+    CUDA_CHECK(cudaEventRecord(ev_prep, st));
+    batch_miller_kernel<<<(count + 63) / 64, 64, 0, st>>>(v.d_rec, ok + 1, count, v.d_f);
+    // side stream 2: the G2 membership of every B, the group scalars and prepared inputs, e(alpha, beta)^s_g0
+    CUDA_CHECK(cudaStreamWaitEvent(s2, ev_up, 0));
+    locate_g2_kernel<<<(count + 127) / 128, 128, 0, s2>>>(v.d_proofs, count, wf);
+    CUDA_CHECK(cudaEventRecord(ev_g2, s2));
+    locate_inputs_kernel<<<(unsigned)(((size_t)groups * n_pts + 3) / 4), 128, 0, s2>>>(vk->d_tabs, vk->d_g1, w, (const uint32_t*)v.d_pub, wf,
+                                                                                      n_public, count, groups, B + o_pts, tails);
+    g1_segment_sum_kernel<<<groups, 128, 0, s2>>>(B + o_pts, 128, n_pts, (size_t)groups * n_pts, nullptr, tails + TAIL_PREP, TAIL_BYTES);
+    CUDA_CHECK(cudaEventRecord(ev_pts, s2));
+    locate_rhs_kernel<<<(groups + 63) / 64, 64, 0, s2>>>(tails, groups, vk->d_eab);
+    CUDA_CHECK(cudaEventRecord(ev_s2, s2));
+    // side stream 3, once the r C and the G2 checks exist: the group sums of r C, then the groups' prepared pairs
+    CUDA_CHECK(cudaStreamWaitEvent(s3, ev_prep, 0));
+    CUDA_CHECK(cudaStreamWaitEvent(s3, ev_g2, 0));
+    g1_segment_sum_kernel<<<groups, 128, 0, s3>>>(v.d_rec + BREC_RC, REC_BYTES_V, LOCATE_GROUP, count, wf, tails + TAIL_RC, TAIL_BYTES);
+    CUDA_CHECK(cudaStreamWaitEvent(s3, ev_pts, 0));
+    locate_pairs_kernel<<<(groups + 63) / 64, 64, 0, s3>>>(tails, groups, vk->d_lines, !vk->gamma_inf, !vk->delta_inf);
+    CUDA_CHECK(cudaEventRecord(ev_s3, s3));
+    CUDA_CHECK(cudaStreamWaitEvent(st, ev_g2, 0));
+    locate_product_kernel<<<groups, 64, 0, st>>>(v.d_f, wf, count, tails);
+    CUDA_CHECK(cudaStreamWaitEvent(st, ev_s2, 0));
+    CUDA_CHECK(cudaStreamWaitEvent(st, ev_s3, 0));
+    locate_final_kernel<<<(groups + 63) / 64, 64, 0, st>>>(tails, groups, gv);
+    g_launch_count += 10;
+    CUDA_CHECK(cudaGetLastError());
+    std::vector<uint8_t> ok_h(count), gv_h(groups);
+    CUDA_CHECK(cudaMemcpyAsync(ok_h.data(), wf, count, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaMemcpyAsync(gv_h.data(), gv, groups, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    // the verdicts: 0 for a malformed proof, 1 in a group that holds, else b2g_verify_many's verdict
+    std::vector<uint8_t> out(count);
+    std::vector<uint32_t> idx;
+    for (uint32_t i = 0; i < count; i++) {
+        out[i] = ok_h[i] && gv_h[i / LOCATE_GROUP];
+        if (ok_h[i] && !gv_h[i / LOCATE_GROUP]) idx.push_back(i);
+    }
+    if (!idx.empty()) {
+        // when every proof is checked again, the caller's rows are already the compact ones
+        const uint32_t m = (uint32_t)idx.size();
+        const bool whole = m == count;
+        const size_t row = compressed ? COMP_BYTES : 256, pub_row = (size_t)n_public * 32;
+        std::vector<uint8_t> rows(whole ? 0 : (size_t)m * row), pubs(whole ? 0 : (size_t)m * pub_row), many(m);
+        for (uint32_t k = 0; k < m && !whole; k++) {
+            memcpy(rows.data() + k * row, (const uint8_t*)proofs + idx[k] * row, row);
+            if (pub_row) memcpy(pubs.data() + k * pub_row, (const uint8_t*)public_inputs + idx[k] * pub_row, pub_row);
+        }
+        verify_bufs_ensure(fn, *cv.vbufs, count, inputs, (size_t)m * n_public, bytes, comp);
+        verify_many_enqueue(**cv.vbufs, vk, m, whole ? public_inputs : pubs.data(), whole ? proofs : rows.data(), compressed, st);
+        CUDA_CHECK(cudaMemcpyAsync(many.data(), (*cv.vbufs)->d_verdict, m, cudaMemcpyDeviceToHost, st));
+        CUDA_CHECK(cudaStreamSynchronize(st));
+        for (uint32_t k = 0; k < m; k++) out[idx[k]] = many[k];
+    }
+    memcpy(verdicts_out, out.data(), count);
+}
+
 int b2g_verify_many(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs, uint8_t* verdicts_out) {
     return guarded([&] { verify_many_run("b2g_verify_many", ctx, vk, count, public_inputs, proofs, false, verdicts_out); });
 }
@@ -949,6 +1180,18 @@ int b2g_verify_batch_compressed(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const 
                                 const void* weights, uint8_t* verdict_out) {
     return guarded([&] {
         verify_batch_run("b2g_verify_batch_compressed", ctx, vk, count, public_inputs, compressed, true, weights, verdict_out);
+    });
+}
+
+int b2g_verify_batch_locate(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs, const void* weights,
+                            uint8_t* verdicts_out) {
+    return guarded([&] { verify_locate_run("b2g_verify_batch_locate", ctx, vk, count, public_inputs, proofs, false, weights, verdicts_out); });
+}
+
+int b2g_verify_batch_locate_compressed(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* compressed,
+                                       const void* weights, uint8_t* verdicts_out) {
+    return guarded([&] {
+        verify_locate_run("b2g_verify_batch_locate_compressed", ctx, vk, count, public_inputs, compressed, true, weights, verdicts_out);
     });
 }
 

@@ -14,6 +14,8 @@
            (b2g_verify_many, with the key prepared on the device by b2g_vk_load <- process_vk).
     Groth16.verify_batch(vk, public_inputs, proofs)
         <- the same check for a whole batch at once: one random-linear-combination pairing check (b2g_verify_batch).
+    Groth16.verify_batch_locate(vk, public_inputs, proofs)
+        <- verify_with_processed_vk for every proof, from one batch check per group of 64 proofs (b2g_verify_batch_locate).
     Groth16.decompress_proofs(blobs)
         <- Proof::<Bn254>::deserialize_compressed (ark-serialize 0.5, Validate::Yes) for many 128-byte proofs, on the device.
     Groth16.verify_many_compressed / verify_batch_compressed(vk, public_inputs, blobs)
@@ -330,8 +332,8 @@ def _verify_many(fn, vk, public_inputs, proofs, ctx, compressed) -> list:
     return [bool(v) for v in out]
 
 
-def _verify_batch(fn, vk, public_inputs, proofs, ctx, weights, compressed) -> bool:
-    """Groth16.verify_batch and verify_batch_compressed"""
+def _verify_batch(fn, vk, public_inputs, proofs, ctx, weights, compressed, locate=False):
+    """Groth16.verify_batch, verify_batch_locate and their compressed forms: one bool, or one bool per proof when locate"""
     import secrets
     proofs = list(proofs)
     if weights is not None:                    # checked before the key is loaded on the device
@@ -343,7 +345,7 @@ def _verify_batch(fn, vk, public_inputs, proofs, ctx, weights, compressed) -> bo
                 raise N.B2gError(N.B2G_E_INPUT, f"weight {w} is not in [1, 2^128)")
     args = _verify_args(fn, vk, public_inputs, proofs, ctx, compressed)
     if args is None:
-        return True
+        return [] if locate else True
     ctx, vh, count, pub_arr, data = args
     if weights is None:
         weights = []
@@ -352,10 +354,14 @@ def _verify_batch(fn, vk, public_inputs, proofs, ctx, weights, compressed) -> bo
             if w:
                 weights.append(w)
     wb = np.frombuffer(b''.join(w.to_bytes(16, 'little') for w in weights), dtype=np.uint8).copy()
-    out = np.zeros(1, dtype=np.uint8)
-    entry = N.lib().b2g_verify_batch_compressed if compressed else N.lib().b2g_verify_batch
+    out = np.zeros(count if locate else 1, dtype=np.uint8)
+    L = N.lib()
+    if locate:
+        entry = L.b2g_verify_batch_locate_compressed if compressed else L.b2g_verify_batch_locate
+    else:
+        entry = L.b2g_verify_batch_compressed if compressed else L.b2g_verify_batch
     N.check(entry(ctx._h, vh, count, _ptr(pub_arr) if pub_arr is not None else None, _ptr(data), _ptr(wb), _ptr(out)))
-    return bool(out[0])
+    return [bool(v) for v in out] if locate else bool(out[0])
 
 
 def _scalar_bytes(v) -> np.ndarray:
@@ -526,13 +532,24 @@ class Groth16:
     @staticmethod
     def verify_batch(vk, public_inputs, proofs, ctx: Context = None, weights=None) -> bool:
         """Whether ALL proofs are valid, from one random-linear-combination pairing check on the device (b2g_verify_batch):
-        cheaper per proof than verify_many, but one verdict for the batch.  On False, call verify_many to find the invalid
-        proofs.  True iff every proof would pass verify_many, every B lies in G2 (verify_many does not check that), except
+        cheaper per proof than verify_many, but one verdict for the batch.  On False, call verify_batch_locate to find the
+        invalid proofs.  True iff every proof would pass verify_many, every B lies in G2 (verify_many does not check that), except
         with probability at most 1 / (2^128 - 1) when the weights are uniform.  Arguments and errors as verify_many; an empty
         batch is True.  `weights` (one int in [1, 2^128) per proof) are drawn with secrets.randbits(128) when not given;
         weights a prover could know or choose before fixing its proofs make the check unsound.  A zero or too large weight
         raises B2gError (B2G_E_INPUT)."""
         return _verify_batch('verify_batch', vk, public_inputs, proofs, ctx, weights, False)
+
+    @staticmethod
+    def verify_batch_locate(vk, public_inputs, proofs, ctx: Context = None, weights=None) -> list:
+        """One verdict per proof at about verify_batch's cost when few proofs are invalid (b2g_verify_batch_locate).  The
+        batch check runs once per group of 64 consecutive proofs, over the group's well-formed proofs (every coordinate
+        below p, every point on its curve, B at infinity or in G2); the well-formed proofs of a group that fails it are
+        then checked one by one as verify_many checks them.  A proof that is not well-formed is False.  A proof that
+        verify_many accepts and whose B is in G2 is always True; any other proof is False except with probability at most
+        (groups holding such a proof) / (2^128 - 1) when the weights are uniform.  Arguments, weights and errors as
+        verify_batch; an empty batch gives []."""
+        return _verify_batch('verify_batch_locate', vk, public_inputs, proofs, ctx, weights, False, True)
 
     # ---- compressed proofs: Proof::<Bn254>::serialize_compressed (ethereum.serialize_compressed), decoded on the device
     @staticmethod
@@ -565,6 +582,13 @@ class Groth16:
         blob decodes and verify_batch with the same weights is True on the decoded proofs.  Arguments, weights and errors as
         verify_batch; a blob that is not 128 bytes raises ValueError."""
         return _verify_batch('verify_batch_compressed', vk, public_inputs, blobs, ctx, weights, True)
+
+    @staticmethod
+    def verify_batch_locate_compressed(vk, public_inputs, blobs, ctx: Context = None, weights=None) -> list:
+        """verify_batch_locate on compressed proofs (b2g_verify_batch_locate_compressed), decoded on the device: a blob that
+        does not decode is False, and the other verdicts are those of verify_batch_locate on the decoded proofs.  Arguments,
+        weights and errors as verify_batch; a blob that is not 128 bytes raises ValueError."""
+        return _verify_batch('verify_batch_locate_compressed', vk, public_inputs, blobs, ctx, weights, True, True)
 
     # base-range sharded variant: every rank calls prove_partial, the 768-byte partials are all-gathered by the caller
     # (torch.distributed / NCCL), then every rank calls prove_finish and obtains the same proof.

@@ -14,6 +14,8 @@
 //   ark_circom::Groth16::verify_batch         <- the same for a whole batch at once: one random-linear-combination check
 //   ark_circom::Groth16::decompress_proofs    <- Proof::<Bn254>::deserialize_compressed (ark-serialize 0.5) for many proofs
 //   ark_circom::Groth16::verify_many_compressed / verify_batch_compressed <- deserialize_compressed, then the two above
+//   ark_circom::Groth16::verify_batch_locate (+ _compressed) <- verify_with_processed_vk for every proof, at about the batch
+//                                              check's cost when few proofs are invalid
 //   ark_circom::serialize_compressed          <- Proof::<Bn254>::serialize_compressed (ark_circom_ethereum.hpp)
 //   ark_circom::read_wtns                              <- snarkjs .wtns (test-vectors/circuit2_js/witness.wtns; the reference
 //                                                         computes witnesses with WASM instead, out of scope here)
@@ -440,7 +442,7 @@ struct Groth16T {                                       // Groth16::<Bn254, QAP>
     }
     // whether ALL proofs are valid, from one random-linear-combination pairing check (b2g_verify_batch): true iff every
     // proof passes verify_many and every B lies in G2, except with probability <= 1 / (2^128 - 1).  The 128-bit weights
-    // come from std::random_device, drawn after the proofs are fixed.  On false, call verify_many to find the invalid
+    // come from std::random_device, drawn after the proofs are fixed.  On false, call verify_batch_locate to find the invalid
     // proofs.  An empty batch is true.
     static bool verify_batch(const PreparedVerifyingKey& pvk, const std::vector<std::vector<Fr>>& public_inputs,
                              const std::vector<Proof>& proofs, int device = 0) {
@@ -450,6 +452,20 @@ struct Groth16T {                                       // Groth16::<Bn254, QAP>
         uint8_t verdict = 0;
         check(b2g_verify_batch(c.gpu->ctx(), c.vk, (uint32_t)c.n, c.pub.empty() ? nullptr : c.pub.data(), c.bytes.data(), w.data(), &verdict));
         return verdict != 0;
+    }
+    // one verdict per proof at about verify_batch's cost when few proofs are invalid (b2g_verify_batch_locate): the batch
+    // check runs once per group of 64 proofs over the group's well-formed proofs, and the well-formed proofs of a failing
+    // group are checked as verify_many checks them.  A proof with a coordinate >= p, a point off its curve or a B outside
+    // G2 is false.  A proof that verify_many accepts and whose B is in G2 is always true; any other proof is false except
+    // with probability <= (groups holding such a proof) / (2^128 - 1).  Weights from std::random_device, as verify_batch.
+    static std::vector<bool> verify_batch_locate(const PreparedVerifyingKey& pvk, const std::vector<std::vector<Fr>>& public_inputs,
+                                                 const std::vector<Proof>& proofs, int device = 0) {
+        VerifyCall c("verify_batch_locate", pvk, public_inputs, proofs, device);
+        if (c.n == 0) return {};
+        const std::vector<uint32_t> w = batch_weights(c.n);
+        std::vector<uint8_t> verdicts(c.n);
+        check(b2g_verify_batch_locate(c.gpu->ctx(), c.vk, (uint32_t)c.n, c.pub.empty() ? nullptr : c.pub.data(), c.bytes.data(), w.data(), verdicts.data()));
+        return std::vector<bool>(verdicts.begin(), verdicts.end());
     }
     // Proof::<Bn254>::deserialize_compressed (ark-serialize 0.5, Validate::Yes) for many proofs in one device pass
     // (b2g_proofs_decompress): an empty optional where arkworks would refuse the bytes (both flag bits set, a coordinate
@@ -484,6 +500,18 @@ struct Groth16T {                                       // Groth16::<Bn254, QAP>
         uint8_t verdict = 0;
         check(b2g_verify_batch_compressed(c.gpu->ctx(), c.vk, (uint32_t)c.n, c.pub.empty() ? nullptr : c.pub.data(), c.bytes.data(), w.data(), &verdict));
         return verdict != 0;
+    }
+    // verify_batch_locate on compressed proofs, decoded on the device (b2g_verify_batch_locate_compressed): a proof that does
+    // not decode is false, the others as verify_batch_locate on the decoded proofs
+    static std::vector<bool> verify_batch_locate_compressed(const PreparedVerifyingKey& pvk, const std::vector<std::vector<Fr>>& public_inputs,
+                                                            const std::vector<CompressedProof>& blobs, int device = 0) {
+        VerifyCall c("verify_batch_locate_compressed", pvk, public_inputs, blobs, device);
+        if (c.n == 0) return {};
+        const std::vector<uint32_t> w = batch_weights(c.n);
+        std::vector<uint8_t> verdicts(c.n);
+        check(b2g_verify_batch_locate_compressed(c.gpu->ctx(), c.vk, (uint32_t)c.n, c.pub.empty() ? nullptr : c.pub.data(), c.bytes.data(),
+                                                 w.data(), verdicts.data()));
+        return std::vector<bool>(verdicts.begin(), verdicts.end());
     }
     static Proof create_proof_with_reduction_and_matrices(const ProvingKey& pk, const Fr& r, const Fr& s, const ConstraintMatrices& matrices,
                                                           size_t num_inputs, size_t num_constraints, const std::vector<Fr>& full_assignment,

@@ -14,8 +14,11 @@
 //       B2G_VERIFY_COMPRESSED=K: also prove K proofs, serialize them compressed, flip the sign bit of A in every other one,
 //       compare Groth16::verify_many_compressed's verdicts with the host verifier, decode the untouched ones back, and print
 //       Groth16::verify_batch_compressed's verdict on the untouched and on the flipped set
+//       B2G_VERIFY_LOCATE=K: also prove K proofs, negate A in proofs 0, K / 2 and K - 1, and compare
+//       Groth16::verify_batch_locate's verdicts with verify_with_processed_vk called per proof (timing the locate call)
 //       chain:<a> = the witness of the reference's squaring-chain bench family for input a
 //       (test-vectors/complex-circuit/input.json has a = 3), computed on the host instead of by WASM.
+#include <algorithm>
 #include <chrono>
 #include <cstdlib>
 #include <cstdio>
@@ -309,6 +312,43 @@ int main(int argc, char** argv) {
             const bool batch = Groth16::verify_batch_compressed(pvk, inputs, blobs), batch_flipped = Groth16::verify_batch_compressed(pvk, inputs, flipped);
             std::printf("verify_compressed %d proofs (%d valid): many agree=%d, batch valid=%d flipped=%d, round trip=%d\n", k, valid, agree,
                         batch, batch_flipped, round_trip);
+        }
+        if (const char* vl = std::getenv("B2G_VERIFY_LOCATE")) {         // per-proof verdicts of the grouped batch check, against the host
+            const int k = std::atoi(vl);
+            if (k < 1) throw SynthesisError("B2G_VERIFY_LOCATE must be >= 1");
+            std::vector<std::vector<Fr>> wv((size_t)k, full_assignment);
+            if (wsrc.rfind("chain:", 0) == 0)
+                for (int i = 1; i < k; i++) wv[(size_t)i] = chain_witness(params.a_query.size(), std::stoull(wsrc.substr(6)) + (unsigned long long)i);
+            std::vector<const std::vector<Fr>*> ws;
+            for (const auto& w : wv) ws.push_back(&w);
+            std::mt19937_64 rng(0x10CA);
+            std::vector<std::pair<Fr, Fr>> rs;
+            for (int i = 0; i < k; i++) rs.push_back({Fr::rand(rng), Fr::rand(rng)});
+            std::vector<Proof> proofs = Groth16::create_proofs(params, matrices, rs, ws);
+            std::vector<std::vector<Fr>> inputs;
+            for (const auto& w : wv) inputs.emplace_back(w.begin() + 1, w.begin() + num_inputs);
+            std::vector<size_t> at = {0, (size_t)k / 2, (size_t)k - 1};
+            std::sort(at.begin(), at.end());
+            at.erase(std::unique(at.begin(), at.end()), at.end());
+            for (size_t i : at) {                                         // A -> -A: y -> p - y
+                uint64_t y[4], d[4]; memcpy(y, proofs[i].bytes + 32, 32);
+                unsigned __int128 borrow = 0;
+                for (int j = 0; j < 4; j++) { unsigned __int128 t = (unsigned __int128)detail::FQ_P[j] - y[j] - borrow; d[j] = (uint64_t)t; borrow = (t >> 64) & 1; }
+                memcpy(proofs[i].bytes + 32, d, 32);
+            }
+            auto pvk = Groth16::process_vk(params.vk);
+            std::vector<bool> got = Groth16::verify_batch_locate(pvk, inputs, proofs);   // also loads the key on the device
+            auto t1 = std::chrono::steady_clock::now();
+            got = Groth16::verify_batch_locate(pvk, inputs, proofs);
+            const double dev_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t1).count();
+            int agree = 1, valid = 0;
+            for (int i = 0; i < k; i++) {
+                const bool host = Groth16::verify_with_processed_vk(pvk, inputs[(size_t)i], proofs[(size_t)i]);
+                agree &= host == got[(size_t)i];
+                valid += host;
+            }
+            std::printf("verify_locate %d proofs (%d valid, %d tampered): agree=%d, device %.3f ms/batch (%.1f proofs/s)\n", k, valid,
+                        (int)at.size(), agree, dev_ms, k / (dev_ms / 1e3));
         }
         return 0;
     } catch (const std::exception& e) {

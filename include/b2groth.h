@@ -20,6 +20,8 @@
  *   b2g_verify_batch       <- the same check for a whole batch at once, as one random linear combination of the proofs
  *   b2g_proofs_decompress  <- Proof::<Bn254>::deserialize_compressed (ark-serialize 0.5, Validate::Yes), for many proofs
  *   b2g_verify_many_compressed / b2g_verify_batch_compressed <- deserialize_compressed followed by the two calls above
+ *   b2g_verify_batch_locate (+ _compressed) <- GrothBn::verify_with_processed_vk for every proof of a batch, at about the
+ *                             batch check's cost when few proofs are invalid
  *   b2g_fixed_base_g1/g2   <- the batch fixed-base multiplications of generate_random_parameters_with_reduction
  *                             (tests/groth16.rs:25); used to manufacture synthetic proving keys
  *
@@ -226,7 +228,8 @@ B2G_API int b2g_verify_many(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void
                             uint8_t* verdicts_out);
 
 /* b2g_verify_batch: whether ALL count proofs are valid, from one random-linear-combination pairing check, for callers that
- * only need the batch's verdict (an aggregator, a rollup node, a bridge) and fall back to b2g_verify_many when it is 0.
+ * only need the batch's verdict (an aggregator, a rollup node, a bridge).  When it is 0, b2g_verify_batch_locate finds the
+ * invalid proofs.
  * public_inputs and proofs are laid out as for b2g_verify_many; weights = count x 16 B little-endian 128-bit weights r_i;
  * *verdict_out = 1 or 0.  The verdict is 1 iff every coordinate is below p, every point is on its curve, every B_i not at
  * infinity lies in G2 (the order-r subgroup of the twist; a proof whose B is outside G2 makes the batch invalid), and
@@ -269,6 +272,38 @@ B2G_API int b2g_verify_many_compressed(b2g_ctx* ctx, b2g_vk* vk, uint32_t count,
  * proof decodes and b2g_verify_batch with the same weights gives 1 on the decoded rows. */
 B2G_API int b2g_verify_batch_compressed(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs,
                                         const void* compressed, const void* weights, uint8_t* verdict_out);
+
+/* b2g_verify_batch_locate: one verdict per proof at about the cost of b2g_verify_batch when few proofs are invalid, for callers
+ * that take proofs from untrusted submitters and must find the invalid ones.  The arguments, their layouts and the buffers are
+ * those of b2g_verify_batch, except that verdicts_out = count bytes.
+ * Proofs are split into groups of 64 consecutive proofs (the last group may be shorter).  Proof i is well-formed when every
+ * coordinate is below p, every point is on its curve, and B is at infinity or lies in G2.  Its verdict is
+ *   0 if it is not well-formed;
+ *   else 1 if its group passes the batch equation of b2g_verify_batch taken over the group's well-formed proofs only, with the
+ *     caller's weights for them (malformed proofs are left out of the product, of the sums and of s_0, s_j; a group without a
+ *     well-formed proof has nothing left to check);
+ *   else the b2g_verify_many verdict of the proof (the well-formed proofs of every failing group go through b2g_verify_many's
+ *     kernels in one more device pass).
+ * Completeness: a proof that b2g_verify_many accepts and whose B is in G2 always gets 1.
+ * Soundness: any other proof gets 0, except with probability at most (the number of groups holding such a proof) / (2^128 - 1)
+ * over uniformly drawn nonzero weights.  As for b2g_verify_batch, the weights must be drawn AFTER the proofs are fixed, from a
+ * source the prover cannot predict or influence.
+ * Determinism: for given weights the verdicts are deterministic.
+ * Relation to b2g_verify_batch: every verdict is 1 exactly when b2g_verify_batch with the same weights gives 1, except in the
+ * same low-probability event.  The two are not equal bit for bit: weights that make invalid proofs of different groups cancel
+ * in the whole batch's equation do not make them cancel in their groups' equations.
+ * Cost: b2g_verify_batch's per-proof work, plus per group one two-pair Miller loop, one final exponentiation, e(alpha, beta)^s_0
+ * and the public-input products; plus b2g_verify_many on the well-formed proofs of the groups that fail.
+ * Synchronous.  Errors as b2g_verify_batch: B2G_E_SHAPE for count == 0, null pointers, a key of another device or a pending
+ * proof; B2G_E_INPUT for a public input >= r or a zero weight; B2G_E_DEVICE when the buffers do not fit.  Every error leaves
+ * the context usable. */
+B2G_API int b2g_verify_batch_locate(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs,
+                                    const void* weights, uint8_t* verdicts_out);
+/* b2g_verify_batch_locate_compressed: b2g_verify_batch_locate on compressed proofs, decoded on the device.  compressed = count x
+ * 128 B; the other arguments, the rules and the errors as b2g_verify_batch_locate, where a proof that does not decode is not
+ * well-formed.  The verdicts equal those of b2g_proofs_decompress followed by b2g_verify_batch_locate on the decoded rows. */
+B2G_API int b2g_verify_batch_locate_compressed(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs,
+                                               const void* compressed, const void* weights, uint8_t* verdicts_out);
 
 /* Kernel-level entry points (parity tests, benchmarks). All pointers host. */
 B2G_API int b2g_msm_g1(b2g_ctx* ctx, const void* bases, const void* scalars, size_t n, int scalars_mont, void* out_xy_mont);
