@@ -11,23 +11,27 @@
 //   prepare  parse the proof (canonical coordinates; >= p or off the curve -> invalid), sum the prepared inputs, affine
 //   miller   one multi-Miller loop over (A, B), (prepared, -gamma), (C, -delta) sharing one f; only B is stepped here
 //   final    the final exponentiation, compared with e(alpha, beta) -> one verdict byte
-// b2g_verify_batch checks the whole batch with one random linear combination instead (weights r_i from the caller):
+// b2g_verify_batch and b2g_verify_batch_locate check a random linear combination instead (weights r_i from the caller), once
+// per group of `group` consecutive proofs:
 //     prod e(r_i A_i, B_i) * e(sum r_i C_i, -delta) * e(s_0 IC[0] + sum_j s_j IC[j], -gamma) == e(alpha, beta)^s_0,
-//     s_0 = sum r_i, s_j = sum r_i x_ij (mod r), x_ij the j-th public input of proof i (j = 1..n_public)
+//     s_0 = sum r_i, s_j = sum r_i x_ij (mod r), x_ij the j-th public input of proof i (j = 1..n_public), sums over the group
+// b2g_verify_batch runs it with one group of the whole batch; b2g_verify_batch_locate with groups of LOCATE_GROUP proofs whose
+// sums leave out the malformed proofs (a mask), then b2g_verify_many on the well-formed proofs of the groups that fail.
 //   prepare  one proof per thread: the parse and on-curve checks above, r_i A_i (affine) and r_i C_i (XYZZ)
-//   g2       one proof per thread: B in G2
-//   scalars  one CTA per (j, chunk of proofs): partial sums of r_i x_ij (x_i0 = 1)
-//   inputs   one warp per j: s_j from the partial sums, then s_j IC[j] from the window table (IC[0]: a variable-base product)
+//   g2       one proof per thread: the proof parses and its B lies in G2 (the mask)
+//   scalars  one CTA per (chunk of the group or of SCALAR_CHUNK proofs, j): partial sums of r_i x_ij (x_i0 = 1)
+//   inputs   one warp per (group, j): s_j from the group's partial sums, then s_j IC[j] from the window table (IC[0]: a
+//            variable-base product)
 //   miller   one proof per thread: the one-pair Miller loop of (r_i A_i, B_i)
-//   reduce   tree products of the Miller values, tree sums of the r_i C_i and of the s_j IC[j], one CTA level per launch
-//   pairs    one thread: the Miller loop of the two prepared pairs
-//   rhs      one thread: e(alpha, beta)^s_0
-//   final    one thread: one final exponentiation, compared with rhs -> one verdict byte
+//   reduce   per group: the product of the Miller values and the sums of the r_i C_i and of the s_j IC[j]; one CTA per group,
+//            or tree levels of one CTA per 64 or 128 records when the one group is larger
+//   pairs    one group per thread: the Miller loop of the two prepared pairs
+//   rhs      one group per thread: e(alpha, beta)^s_0
+//   final    one group per thread: one final exponentiation, compared with rhs -> one verdict byte per group
 // Only prepare -> miller -> product -> final run on the context's stream; the rest runs next to them on two side streams.
-// b2g_proofs_decompress, b2g_verify_many_compressed and b2g_verify_batch_compressed take arkworks' 128-byte compressed
-// proofs: a decode kernel (one proof per thread) writes the 256-byte rows the kernels above read, and a second kernel checks
-// that each decoded B lies in G2 (b2g_verify_batch leaves that to batch_g2_kernel).  The decoding rules are restated above
-// decompress_kernel.
+// b2g_proofs_decompress and the _compressed verifiers take arkworks' 128-byte compressed proofs: a decode kernel (one proof
+// per thread) writes the 256-byte rows the kernels above read, and a second kernel checks that each decoded B lies in G2 (the
+// batch check leaves that to batch_g2_kernel).  The decoding rules are restated above decompress_kernel.
 #include <algorithm>
 #include <cstring>
 #include <string>
@@ -67,9 +71,9 @@ struct VerifyBufs {
     size_t cap_count = 0, cap_pub = 0, cap_part = 0, cap_batch = 0, cap_comp = 0;
     uint8_t *d_proofs = nullptr, *d_rec = nullptr, *d_f = nullptr, *d_verdict = nullptr;   // per proof
     uint8_t *d_pub = nullptr, *d_part = nullptr;                                            // per (proof, input)
-    uint8_t* d_batch = nullptr;                   // b2g_verify_batch: weights, reduction levels, scalar sums, tail values
+    uint8_t* d_batch = nullptr;                   // the batch check's scratch: weights, reduction levels, group tails, ...
     uint8_t* d_comp = nullptr;                    // compressed proofs (128 B each), then one decoded-ok byte per proof
-    cudaStream_t side[2] = {nullptr, nullptr};    // b2g_verify_batch's tail pieces, next to the per-proof kernels
+    cudaStream_t side[2] = {nullptr, nullptr};    // the batch check's tail pieces, next to the per-proof kernels
     cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
 };
 
@@ -155,14 +159,19 @@ __global__ void __launch_bounds__(64) verify_final_kernel(const uint8_t* __restr
     verdict[j] = Fq12::eq(e, Fq12::load(eab));
 }
 
-// ---------------------------------------------------------------------------------------------- b2g_verify_batch kernels
-// Per-proof record of the batch check, REC_BYTES_V apart: r A (affine, 64 B), B (affine, 128 B), r C (XYZZ, 128 B).  The
-// batch's ok word starts all ones and any failed parse, on-curve or G2 check clears it.
+// ---------------------------------------------------------------------------------------------- batch check kernels
+// b2g_verify_batch and b2g_verify_batch_locate: the batch equation once per group of `group` consecutive proofs, each group's
+// products and sums optionally masked by wf (wf[i] = 1 when proof i parses and its B lies in G2).
+// Per-proof record, REC_BYTES_V apart: r A (affine, 64 B), B (affine, 128 B), r C (XYZZ, 128 B).  The record area is zeroed
+// first, so a proof that does not parse keeps r A and r C at infinity.  The ok word starts all ones and any failed parse,
+// on-curve or G2 check clears it.
 constexpr size_t BREC_B = 64, BREC_RC = 192;
-constexpr uint32_t SCALAR_CHUNK = 2048;            // proofs per CTA of batch_scalars_kernel
-// tail values (Fq12 384 B, G1 XYZZ 128 B): the product of the per-proof Miller values, the Miller value of the prepared
-// pairs, e(alpha, beta)^s_0, sum r C, the prepared inputs, s_0
+// tail values of a group, group g's at tails + g * TAIL_BYTES (Fq12 384 B, G1 XYZZ 128 B): the product of the per-proof
+// Miller values, the Miller value of the prepared pairs, e(alpha, beta)^s_0, sum r C, the prepared inputs, s_0
 constexpr size_t TAIL_F = 0, TAIL_G = 384, TAIL_RHS = 768, TAIL_RC = 1152, TAIL_PREP = 1280, TAIL_S0 = 1408, TAIL_BYTES = 1536;
+static_assert(TAIL_BYTES % 256 == 0, "group tails stay 256-byte aligned");
+constexpr uint32_t LOCATE_GROUP = 64;              // proofs per group of b2g_verify_batch_locate: one CTA of f12_product_kernel
+constexpr uint32_t SCALAR_CHUNK = 2048;            // at most this many proofs per CTA of batch_scalars_kernel
 
 __device__ __forceinline__ void weight_load(uint32_t* k, const uint32_t* w, size_t i) {
     for (int t = 0; t < 4; t++) k[t] = w[4 * i + t];
@@ -173,8 +182,8 @@ __global__ void __launch_bounds__(128) batch_prepare_kernel(const uint8_t* __res
     const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= count) return;
     G1::Aff a, cc; G2::Aff b;
-    // a failed proof's record is not written: the Miller kernel skips every proof once the ok word is cleared, the r C sum
-    // still reads the stale record, and batch_final_kernel discards what was computed from it
+    // a failed proof's record is not written: it stays zeroed, so its r A and r C are at infinity, and the cleared ok word
+    // fails a batch verdict (a group verdict leaves the proof out through wf instead)
     if (!proof_parse(proofs + (size_t)j * 256, a, b, cc)) { atomicAnd(ok_all, 0u); return; }
     uint32_t k[4];
     weight_load(k, w, j);
@@ -184,22 +193,28 @@ __global__ void __launch_bounds__(128) batch_prepare_kernel(const uint8_t* __res
     pt_store<Fq>(r + BREC_RC, 0, G1::mul_affine(cc, k, 4));
 }
 
-// G2 membership of every B, one proof per thread, on a side stream next to the Miller kernel (only the ok word needs it)
-__global__ void __launch_bounds__(128) batch_g2_kernel(const uint8_t* __restrict__ proofs, uint32_t count, uint32_t* __restrict__ ok_all) {
+// one proof per thread, on a side stream next to the per-proof chain: wf[j] = the proof parses and its B lies in G2; clears
+// the ok word when it does not
+__global__ void __launch_bounds__(128) batch_g2_kernel(const uint8_t* __restrict__ proofs, uint32_t count, uint8_t* __restrict__ wf,
+                                                       uint32_t* __restrict__ ok_all) {
     const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= count) return;
     G1::Aff a, cc; G2::Aff b;
-    if (proof_parse(proofs + (size_t)j * 256, a, b, cc) && !g2_in_subgroup(b)) atomicAnd(ok_all, 0u);
+    const bool good = proof_parse(proofs + (size_t)j * 256, a, b, cc) && g2_in_subgroup(b);
+    wf[j] = good;
+    if (!good) atomicAnd(ok_all, 0u);
 }
 
-// CTA (j, chunk): part[j * gridDim.y + chunk] = the sum over the chunk's proofs i of r_i (j = 0) or of
-// Fr::mul(r_i, x_ij) = r_i x_ij / R (j >= 1)
+// CTA (c, j): part[j * gridDim.x + c] = the sum over the proofs i of chunk c (`chunk` proofs) of r_i (j = 0) or of
+// Fr::mul(r_i, x_ij) = r_i x_ij / R (j >= 1), leaving out proof i when mask[i] = 0 (no mask: every proof)
 __global__ void __launch_bounds__(128) batch_scalars_kernel(const uint32_t* __restrict__ w, const uint32_t* __restrict__ pub,
-                                                            uint32_t n_public, uint32_t count, uint8_t* __restrict__ part) {
+                                                            const uint8_t* __restrict__ mask, uint32_t n_public, uint32_t count,
+                                                            uint32_t chunk, uint8_t* __restrict__ part) {
     __shared__ fe sh[128];
-    const uint32_t j = blockIdx.x, end = min(count, (blockIdx.y + 1) * SCALAR_CHUNK);
+    const uint32_t j = blockIdx.y, end = min(count, (blockIdx.x + 1) * chunk);
     fe acc = Fr::zero();
-    for (uint32_t i = blockIdx.y * SCALAR_CHUNK + threadIdx.x; i < end; i += 128) {
+    for (uint32_t i = blockIdx.x * chunk + threadIdx.x; i < end; i += 128) {
+        if (mask && !mask[i]) continue;
         fe wi = fe_zero();
         weight_load(wi.l, w, i);
         acc = Fr::add(acc, j ? Fr::mul(wi, fe_load(pub + 8 * ((size_t)i * n_public + j - 1))) : wi);
@@ -210,29 +225,39 @@ __global__ void __launch_bounds__(128) batch_scalars_kernel(const uint32_t* __re
         if ((int)threadIdx.x < d) sh[threadIdx.x] = Fr::add(sh[threadIdx.x], sh[threadIdx.x + d]);
         __syncthreads();
     }
-    if (threadIdx.x == 0) fe_store(part + ((size_t)j * gridDim.y + blockIdx.y) * 32, sh[0]);
+    if (threadIdx.x == 0) fe_store(part + ((size_t)j * gridDim.x + blockIdx.x) * 32, sh[0]);
 }
 
-// one warp per j = 0..n_public: s_j from the chunk sums, pts[j] = s_j IC[j]; also s_0 to the tail
+// one warp per (group g, j = 0..n_public), t = g * (n_public + 1) + j: s_gj = the sum of the group's `per` chunk sums of
+// batch_scalars_kernel (`chunks` in all), then pts[t] = s_gj IC[j] (IC[0]: a variable-base product); s_g0 to the group's tail
 __global__ void __launch_bounds__(128) batch_inputs_kernel(const uint8_t* __restrict__ tabs, const uint8_t* __restrict__ g1,
-                                                           const uint8_t* __restrict__ part, uint32_t chunks, uint32_t n_public,
-                                                           uint8_t* __restrict__ pts, uint8_t* __restrict__ tail) {
+                                                           const uint8_t* __restrict__ part, uint32_t per, uint32_t chunks,
+                                                           uint32_t n_public, uint32_t groups, uint8_t* __restrict__ pts,
+                                                           uint8_t* __restrict__ tails) {
     __shared__ G1::Pt sh[4][32];
     __shared__ fe s[4];
-    const uint32_t wid = threadIdx.x >> 5, lane = threadIdx.x & 31, j = blockIdx.x * 4 + wid;
-    if (j > n_public) return;                              // whole warps leave together
-    if (lane == 0) {
-        fe acc = Fr::zero();
-        for (uint32_t c = 0; c < chunks; c++) acc = Fr::add(acc, fe_load(part + ((size_t)j * chunks + c) * 32));
-        s[wid] = j ? Fr::from_canonical(acc) : acc;       // from_canonical multiplies by R, cancelling the products' 1 / R
+    const uint32_t wid = threadIdx.x >> 5, lane = threadIdx.x & 31, n_pts = n_public + 1;
+    const size_t t = (size_t)blockIdx.x * 4 + wid;
+    if (t >= (size_t)groups * n_pts) return;               // whole warps leave together
+    const uint32_t g = (uint32_t)(t / n_pts), j = (uint32_t)(t % n_pts);
+    fe acc = Fr::zero();
+    for (uint32_t k = lane; k < per; k += 32) {
+        const uint32_t c = g * per + k;
+        if (c < chunks) acc = Fr::add(acc, fe_load(part + ((size_t)j * chunks + c) * 32));
     }
+    for (int d = 16; d > 0; d >>= 1) {
+        fe o;
+        for (int q = 0; q < 8; q++) o.l[q] = __shfl_down_sync(0xffffffffu, acc.l[q], d);
+        acc = Fr::add(acc, o);
+    }
+    if (lane == 0) s[wid] = j ? Fr::from_canonical(acc) : acc;   // from_canonical cancels the products' 1 / R
     __syncwarp();
     if (j) {
         const G1::Pt p = warp_fixed_mul<G1, Fq>(tabs + (size_t)(j - 1) * TABLE_BYTES, s[wid].l, sh[wid]);
-        if (lane == 0) pt_store<Fq>(pts, j, p);
+        if (lane == 0) pt_store<Fq>(pts, t, p);
     } else if (lane == 0) {
-        pt_store<Fq>(pts, 0, G1::mul_scalar(G1::from_affine(aff_load<Fq>(g1, 1)), s[wid].l));
-        fe_store(tail + TAIL_S0, s[wid]);
+        pt_store<Fq>(pts, t, G1::mul_scalar(G1::from_affine(aff_load<Fq>(g1, 1)), s[wid].l));
+        fe_store(tails + (size_t)g * TAIL_BYTES + TAIL_S0, s[wid]);
     }
 }
 
@@ -250,30 +275,37 @@ __global__ void __launch_bounds__(64) batch_miller_kernel(const uint8_t* __restr
     Fq12::store(fout + (size_t)j * F12_BYTES, f);
 }
 
-// one level of a tree product: dst[b] = the product of src[64 b .. 64 b + 63] (Fq12, `stride` bytes apart)
-__global__ void __launch_bounds__(64) f12_product_kernel(const uint8_t* __restrict__ src, size_t stride, uint32_t n, uint8_t* __restrict__ dst) {
+// CTA b: dst + b * dst_stride = the product of src[64 b .. 64 b + 63] below n (Fq12, `stride` bytes apart), taking 1 for
+// record i when mask[i] = 0 (no mask: every record)
+__global__ void __launch_bounds__(64) f12_product_kernel(const uint8_t* __restrict__ src, size_t stride, uint32_t n,
+                                                         const uint8_t* __restrict__ mask, uint8_t* __restrict__ dst, size_t dst_stride) {
     __shared__ fe12 sh[64];
     const uint32_t t = threadIdx.x, i = blockIdx.x * 64 + t;
-    sh[t] = i < n ? Fq12::load(src + (size_t)i * stride) : Fq12::one();
+    sh[t] = i < n && (!mask || mask[i]) ? Fq12::load(src + (size_t)i * stride) : Fq12::one();
     __syncthreads();
     for (uint32_t d = 32; d > 0; d >>= 1) {
         if (t < d) { fe12 x = sh[t]; Fq12::mul(x, x, sh[t + d]); sh[t] = x; }
         __syncthreads();
     }
-    if (t == 0) Fq12::store(dst + (size_t)blockIdx.x * F12_BYTES, sh[0]);
+    if (t == 0) Fq12::store(dst + (size_t)blockIdx.x * dst_stride, sh[0]);
 }
 
-// one level of a tree sum: dst[b] = the sum of src[128 b .. 128 b + 127] (G1 XYZZ, `stride` bytes apart)
-__global__ void __launch_bounds__(128) g1_sum_kernel(const uint8_t* __restrict__ src, size_t stride, uint32_t n, uint8_t* __restrict__ dst) {
+// CTA b: dst + b * dst_stride = the sum of src[seg * b .. seg * b + seg - 1] below n (G1 XYZZ, `stride` bytes apart), leaving
+// out record i when mask[i] = 0 (no mask: every record)
+__global__ void __launch_bounds__(128) g1_sum_kernel(const uint8_t* __restrict__ src, size_t stride, uint32_t seg, size_t n,
+                                                     const uint8_t* __restrict__ mask, uint8_t* __restrict__ dst, size_t dst_stride) {
     __shared__ G1::Pt sh[128];
-    const uint32_t t = threadIdx.x, i = blockIdx.x * 128 + t;
-    sh[t] = i < n ? pt_load<Fq>(src + (size_t)i * stride, 0) : G1::infinity();
+    const uint32_t t = threadIdx.x;
+    const size_t base = (size_t)blockIdx.x * seg, end = min(n, base + seg);
+    sh[t] = G1::infinity();                                // accumulated in shared memory: a register sum spills
+    for (size_t i = base + t; i < end; i += 128)
+        if (!mask || mask[i]) { G1::Pt x = sh[t]; G1::add(x, pt_load<Fq>(src + i * stride, 0)); sh[t] = x; }
     __syncthreads();
     for (uint32_t d = 64; d > 0; d >>= 1) {
         if (t < d) { G1::Pt x = sh[t]; G1::add(x, sh[t + d]); sh[t] = x; }
         __syncthreads();
     }
-    if (t == 0) pt_store<Fq>(dst, blockIdx.x, sh[0]);
+    if (t == 0) pt_store<Fq>(dst + (size_t)blockIdx.x * dst_stride, 0, sh[0]);
 }
 
 // the Miller value of the prepared pairs (prepared inputs, -gamma) and (sum r C, -delta); 1 when both drop out
@@ -290,20 +322,25 @@ __device__ __forceinline__ void tail_pairs(uint8_t* tail, const uint8_t* lines, 
     Fq12::store(tail + TAIL_G, g);
 }
 
-__global__ void batch_pairs_kernel(uint8_t* __restrict__ tail, const uint8_t* __restrict__ lines, bool gamma_on, bool delta_on) {
-    tail_pairs(tail, lines, gamma_on, delta_on);
+// one group per thread: the Miller value of the group's prepared pairs
+__global__ void __launch_bounds__(64) batch_pairs_kernel(uint8_t* __restrict__ tails, uint32_t groups, const uint8_t* __restrict__ lines,
+                                                         bool gamma_on, bool delta_on) {
+    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g < groups) tail_pairs(tails + (size_t)g * TAIL_BYTES, lines, gamma_on, delta_on);
 }
 
-// e(alpha, beta)^s_0
-__global__ void batch_rhs_kernel(uint8_t* __restrict__ tail, const uint8_t* __restrict__ eab) {
+// one group per thread: e(alpha, beta)^s_g0
+__global__ void __launch_bounds__(64) batch_rhs_kernel(uint8_t* __restrict__ tails, uint32_t groups, const uint8_t* __restrict__ eab) {
+    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= groups) return;
+    uint8_t* tail = tails + (size_t)g * TAIL_BYTES;
     fe12 rhs;
     const fe s0 = fe_load(tail + TAIL_S0);
     Fq12::cyclotomic_exp(rhs, Fq12::load(eab), s0.l);
     Fq12::store(tail + TAIL_RHS, rhs);
 }
 
-// the final exponentiation of (per-proof product) x (prepared pairs) equals e(alpha, beta)^s_0 (batch_final_kernel keeps
-// its own copy of these lines: calling this from it changes its register count)
+// the final exponentiation of (per-proof product) x (prepared pairs) equals e(alpha, beta)^s_0
 __device__ __forceinline__ bool tail_holds(const uint8_t* tail) {
     fe12 f = Fq12::load(tail + TAIL_F), e;
     Fq12::mul(f, f, Fq12::load(tail + TAIL_G));
@@ -311,13 +348,12 @@ __device__ __forceinline__ bool tail_holds(const uint8_t* tail) {
     return Fq12::eq(e, Fq12::load(tail + TAIL_RHS));
 }
 
-// the verdict: ok, and the batch equation holds
-__global__ void batch_final_kernel(const uint8_t* __restrict__ tail, const uint32_t* __restrict__ ok_all, uint8_t* __restrict__ verdict) {
-    if (!*ok_all) { *verdict = 0; return; }
-    fe12 f = Fq12::load(tail + TAIL_F), e;
-    Fq12::mul(f, f, Fq12::load(tail + TAIL_G));
-    Fq12::final_exponentiation(e, f);
-    *verdict = Fq12::eq(e, Fq12::load(tail + TAIL_RHS));
+// one group per thread: verdict[g] = the ok word is set (no ok word: always) and the group's batch equation holds.  A group
+// whose proofs are all masked out has every value at 1 (product, pairs and e(alpha, beta)^0), so it holds.
+__global__ void __launch_bounds__(64) batch_final_kernel(const uint8_t* __restrict__ tails, uint32_t groups, const uint32_t* __restrict__ ok_all,
+                                                         uint8_t* __restrict__ verdict) {
+    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g < groups) verdict[g] = (!ok_all || *ok_all) && tail_holds(tails + (size_t)g * TAIL_BYTES);
 }
 
 // b2g_test_op ops 43-45: G2 membership of a G2 affine point (out: 8 B, 1 or 0), r * P for a G1 affine P and a 128-bit r
@@ -338,119 +374,6 @@ __global__ void batch_test_kernel(int op, const uint8_t* __restrict__ a, const u
         Fq12::cyclotomic_exp(r, Fq12::load(a + (size_t)i * F12_BYTES), k.l);
         Fq12::store(out + (size_t)i * F12_BYTES, r);
     }
-}
-
-// ---------------------------------------------------------------------------------------------- b2g_verify_batch_locate kernels
-// The batch check above, once per group of LOCATE_GROUP consecutive proofs, over the group's well-formed proofs only.  The
-// per-proof work is batch_prepare_kernel on a zeroed record area, so that a malformed proof keeps r A and r C at infinity,
-// and batch_miller_kernel with an ok word nothing clears, so that every proof gets its Miller value.  wf[i] is 1 when proof
-// i parses and its B lies in G2; every group product and sum below leaves out the proofs with wf[i] = 0.  Group g's tail
-// values (the TAIL_* offsets) sit at tails + g * TAIL_BYTES.
-constexpr uint32_t LOCATE_GROUP = 64;              // proofs per group: one CTA of locate_product_kernel
-static_assert(TAIL_BYTES % 256 == 0, "group tails stay 256-byte aligned");
-
-// one proof per thread, on a side stream next to the per-proof chain: wf[j] = the proof parses and its B lies in G2
-__global__ void __launch_bounds__(128) locate_g2_kernel(const uint8_t* __restrict__ proofs, uint32_t count, uint8_t* __restrict__ wf) {
-    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= count) return;
-    G1::Aff a, cc; G2::Aff b;
-    wf[j] = proof_parse(proofs + (size_t)j * 256, a, b, cc) && g2_in_subgroup(b);
-}
-
-// one warp per (group g, j = 0..n_public), t = g * (n_public + 1) + j: s_gj = the sum of r_i x_ij over the group's well-formed
-// proofs (x_i0 = 1), then pts[t] = s_gj IC[j] (IC[0]: a variable-base product of a scalar below 64 x 2^128); s_g0 to the tail
-__global__ void __launch_bounds__(128) locate_inputs_kernel(const uint8_t* __restrict__ tabs, const uint8_t* __restrict__ g1,
-                                                            const uint32_t* __restrict__ w, const uint32_t* __restrict__ pub,
-                                                            const uint8_t* __restrict__ wf, uint32_t n_public, uint32_t count,
-                                                            uint32_t groups, uint8_t* __restrict__ pts, uint8_t* __restrict__ tails) {
-    __shared__ G1::Pt sh[4][32];
-    __shared__ fe s[4];
-    const uint32_t wid = threadIdx.x >> 5, lane = threadIdx.x & 31, n_pts = n_public + 1;
-    const size_t t = (size_t)blockIdx.x * 4 + wid;
-    if (t >= (size_t)groups * n_pts) return;               // whole warps leave together
-    const uint32_t g = (uint32_t)(t / n_pts), j = (uint32_t)(t % n_pts);
-    fe acc = Fr::zero();
-    for (uint32_t k = lane; k < LOCATE_GROUP; k += 32) {
-        const uint32_t i = g * LOCATE_GROUP + k;
-        if (i >= count || !wf[i]) continue;
-        fe wi = fe_zero();
-        weight_load(wi.l, w, i);
-        acc = Fr::add(acc, j ? Fr::mul(wi, fe_load(pub + 8 * ((size_t)i * n_public + j - 1))) : wi);
-    }
-    for (int d = 16; d > 0; d >>= 1) {
-        fe o;
-        for (int q = 0; q < 8; q++) o.l[q] = __shfl_down_sync(0xffffffffu, acc.l[q], d);
-        acc = Fr::add(acc, o);
-    }
-    if (lane == 0) s[wid] = j ? Fr::from_canonical(acc) : acc;   // from_canonical cancels the products' 1 / R
-    __syncwarp();
-    if (j) {
-        const G1::Pt p = warp_fixed_mul<G1, Fq>(tabs + (size_t)(j - 1) * TABLE_BYTES, s[wid].l, sh[wid]);
-        if (lane == 0) pt_store<Fq>(pts, t, p);
-    } else if (lane == 0) {
-        pt_store<Fq>(pts, t, G1::mul_scalar(G1::from_affine(aff_load<Fq>(g1, 1)), s[wid].l));
-        fe_store(tails + (size_t)g * TAIL_BYTES + TAIL_S0, s[wid]);
-    }
-}
-
-// CTA b: dst + b * dst_stride = the sum of src[seg * b .. seg * b + seg - 1] below n (G1 XYZZ, `stride` bytes apart), leaving
-// out record i when mask[i] = 0 (no mask: every record)
-__global__ void __launch_bounds__(128) g1_segment_sum_kernel(const uint8_t* __restrict__ src, size_t stride, uint32_t seg, size_t n,
-                                                             const uint8_t* __restrict__ mask, uint8_t* __restrict__ dst, size_t dst_stride) {
-    __shared__ G1::Pt sh[128];
-    const uint32_t t = threadIdx.x;
-    G1::Pt acc = G1::infinity();
-    for (uint32_t k = t; k < seg; k += 128) {
-        const size_t i = (size_t)blockIdx.x * seg + k;
-        if (i < n && (!mask || mask[i])) G1::add(acc, pt_load<Fq>(src + i * stride, 0));
-    }
-    sh[t] = acc;
-    __syncthreads();
-    for (uint32_t d = 64; d > 0; d >>= 1) {
-        if (t < d) { G1::Pt x = sh[t]; G1::add(x, sh[t + d]); sh[t] = x; }
-        __syncthreads();
-    }
-    if (t == 0) pt_store<Fq>(dst + (size_t)blockIdx.x * dst_stride, 0, sh[0]);
-}
-
-// CTA g: the product of the group's Miller values, 1 for a proof with wf[i] = 0
-__global__ void __launch_bounds__(64) locate_product_kernel(const uint8_t* __restrict__ f, const uint8_t* __restrict__ wf, uint32_t count,
-                                                            uint8_t* __restrict__ tails) {
-    static_assert(LOCATE_GROUP == 64, "one thread per proof of a group");
-    __shared__ fe12 sh[64];
-    const uint32_t t = threadIdx.x, i = blockIdx.x * 64 + t;
-    sh[t] = i < count && wf[i] ? Fq12::load(f + (size_t)i * F12_BYTES) : Fq12::one();
-    __syncthreads();
-    for (uint32_t d = 32; d > 0; d >>= 1) {
-        if (t < d) { fe12 x = sh[t]; Fq12::mul(x, x, sh[t + d]); sh[t] = x; }
-        __syncthreads();
-    }
-    if (t == 0) Fq12::store(tails + (size_t)blockIdx.x * TAIL_BYTES + TAIL_F, sh[0]);
-}
-
-// one group per thread: the Miller value of the group's prepared pairs
-__global__ void __launch_bounds__(64) locate_pairs_kernel(uint8_t* __restrict__ tails, uint32_t groups, const uint8_t* __restrict__ lines,
-                                                          bool gamma_on, bool delta_on) {
-    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
-    if (g < groups) tail_pairs(tails + (size_t)g * TAIL_BYTES, lines, gamma_on, delta_on);
-}
-
-// one group per thread: e(alpha, beta)^s_g0
-__global__ void __launch_bounds__(64) locate_rhs_kernel(uint8_t* __restrict__ tails, uint32_t groups, const uint8_t* __restrict__ eab) {
-    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
-    if (g >= groups) return;
-    uint8_t* tail = tails + (size_t)g * TAIL_BYTES;
-    fe12 rhs;
-    const fe s0 = fe_load(tail + TAIL_S0);
-    Fq12::cyclotomic_exp(rhs, Fq12::load(eab), s0.l);
-    Fq12::store(tail + TAIL_RHS, rhs);
-}
-
-// one group per thread: verdict[g] = the group's batch equation holds.  A group without a well-formed proof has every
-// value at 1 (product, pairs and e(alpha, beta)^0), so it holds.
-__global__ void __launch_bounds__(64) locate_final_kernel(const uint8_t* __restrict__ tails, uint32_t groups, uint8_t* __restrict__ verdict) {
-    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
-    if (g < groups) verdict[g] = tail_holds(tails + (size_t)g * TAIL_BYTES);
 }
 
 // ---------------------------------------------------------------------------------------------- compressed proofs
@@ -702,7 +625,7 @@ static void verify_stage_test_op(cudaStream_t st, int op, const void* a, const v
             if (op == 49) {
                 verify_miller_kernel<<<1, 64, 0, st>>>(g + STAGE_REC, g + STAGE_LINES, on[2 * i], on[2 * i + 1], 1, d.o + i * F12_BYTES);
             } else {
-                batch_pairs_kernel<<<1, 1, 0, st>>>(g + STAGE_REC, g + STAGE_LINES, on[2 * i], on[2 * i + 1]);
+                batch_pairs_kernel<<<1, 1, 0, st>>>(g + STAGE_REC, 1, g + STAGE_LINES, on[2 * i], on[2 * i + 1]);
                 CUDA_CHECK(cudaMemcpyAsync(d.o + i * F12_BYTES, g + STAGE_REC + TAIL_G, F12_BYTES, cudaMemcpyDeviceToDevice, st));
             }
         }
@@ -827,9 +750,8 @@ static uint8_t* decompress_enqueue(VerifyBufs& v, const void* compressed, uint32
     return ok;
 }
 
-// the two side streams and six events of b2g_verify_batch and b2g_verify_batch_locate, created at the first such call on the
-// context.  The side streams have the greatest priority, so that their tail kernels are scheduled ahead of queued per-proof
-// CTAs.
+// the two side streams and six events of the batch check (batch_enqueue), created at the first such call on the context.  The
+// side streams have the greatest priority, so that their tail kernels are scheduled ahead of queued per-proof CTAs.
 static void batch_streams(VerifyBufs& v) {
     if (v.ev[5]) return;
     int least = 0, greatest = 0;
@@ -838,18 +760,20 @@ static void batch_streams(VerifyBufs& v) {
     for (cudaEvent_t& e : v.ev) if (!e) CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
 }
 
-// one tree reduction of n records of `src` (`stride` bytes apart) into `dst`: a launch per level of `per` records per CTA,
-// the levels alternating between the scratch areas x and y
+// reduces n records of `src` (`stride` bytes apart) to one value per group of `group` records, group g's at dst +
+// g * TAIL_BYTES.  A group of at most `per` records takes one CTA of one launch; a larger group, which must then be the only
+// one, takes a tree of launches of `per` records per CTA, the levels alternating between the scratch areas x and y.  Only
+// the first level reads the mask.  level(blocks, src, stride, seg, n, mask, dst, dst_stride) launches one level.
 template <class Level>
-static void tree_reduce(const uint8_t* src, size_t stride, size_t rec_bytes, uint32_t n, uint32_t per, uint8_t* x, uint8_t* y,
-                        uint8_t* dst, Level&& level) {
+static void group_reduce(const uint8_t* src, size_t stride, size_t rec_bytes, uint32_t n, uint32_t group, uint32_t per,
+                         const uint8_t* mask, uint8_t* x, uint8_t* y, uint8_t* dst, Level&& level) {
     for (;;) {
-        const uint32_t blocks = (n + per - 1) / per;
-        uint8_t* out = blocks == 1 ? dst : x;
-        level(blocks, src, stride, n, out);
+        const uint32_t seg = std::min(group, per), blocks = (n + seg - 1) / seg;
+        const bool last = seg == group;
+        level(blocks, src, stride, seg, n, mask, last ? dst : x, last ? TAIL_BYTES : rec_bytes);
         g_launch_count += 1;
-        if (blocks == 1) return;
-        src = out; stride = rec_bytes; n = blocks;
+        if (last) return;
+        src = x; stride = rec_bytes; n = group = blocks; mask = nullptr;
         std::swap(x, y);
     }
 }
@@ -1002,99 +926,39 @@ static void weights_check(const void* weights, uint32_t count) {
         if (all_zero((const uint8_t*)weights + 16 * (size_t)i, 16)) throw_error(B2G_E_INPUT, "weight " + std::to_string(i) + " is zero");
 }
 
-// b2g_verify_batch on 256-byte rows, or on compressed rows decoded on the context's stream before anything else reads them
-// (batch_g2_kernel checks the decoded B, so the decoder skips the G2 check)
-static void verify_batch_run(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs,
-                             bool compressed, const void* weights, uint8_t* verdict_out) {
-    if (!weights) throw_error(B2G_E_SHAPE, "null pointer");
-    const CtxView cv = verify_args(fn, ctx, vk, count, public_inputs, proofs, verdict_out);
-    weights_check(weights, count);
-    const uint32_t n_pts = vk->n_public + 1, chunks = (count + SCALAR_CHUNK - 1) / SCALAR_CHUNK;
+// the device results of batch_enqueue: wf (one byte per proof: it parses and its B lies in G2) and one verdict per group
+struct BatchOut { const uint8_t* wf; const uint8_t* verdict; };
+
+// the batch check of b2g_verify_batch (group = count, no mask) and b2g_verify_batch_locate (group = LOCATE_GROUP, masked by
+// wf), on 256-byte rows or on compressed rows decoded on the context's stream before anything else reads them
+// (batch_g2_kernel checks the decoded B, so the decoder skips the G2 check).  The results are ready once the context's stream
+// is.
+static BatchOut batch_enqueue(const char* fn, const CtxView& cv, b2g_vk* vk, uint32_t count, uint32_t group, bool masked,
+                              const void* public_inputs, const void* proofs, bool compressed, const void* weights) {
+    const uint32_t n_pts = vk->n_public + 1, groups = (count + group - 1) / group;
+    // the scalar sums in chunks of a group, or of SCALAR_CHUNK proofs when the one group is larger: per chunks per group
+    const uint32_t chunk = std::min(group, SCALAR_CHUNK), chunks = (count + chunk - 1) / chunk, per = (group + chunk - 1) / chunk;
     const size_t inputs = (size_t)count * vk->n_public;
-    // scratch: weights, four reduction levels (x, y on the main stream, x2, y2 on the side streams), chunk sums of the
-    // scalars, s_j IC[j], tail values and the ok word
+    // scratch: weights, four tree levels (x, y for the Miller values on the main stream, x2, y2 for the r C on side stream
+    // 3; a group of more than one CTA needs them), chunk sums of the scalars, s_gj IC[j] per (group, j), the group tails,
+    // wf, the group verdicts and two ok words (the one batch_prepare_kernel and batch_g2_kernel clear, and one that stays set)
     auto up = [](size_t b) { return (b + 255) & ~(size_t)255; };
-    const size_t level = up(std::max({(size_t)((count + 63) / 64) * F12_BYTES, (size_t)((count + 127) / 128) * 128,
-                                      (size_t)((n_pts + 127) / 128) * 128}));
+    const size_t level = up(std::max((size_t)((count + 63) / 64) * F12_BYTES, (size_t)((count + 127) / 128) * 128));
     const size_t o_w = 0, o_x = up((size_t)count * 16), o_y = o_x + level, o_x2 = o_y + level, o_y2 = o_x2 + level;
-    const size_t o_part = o_y2 + level, o_pts = o_part + up((size_t)n_pts * chunks * 32), o_tail = o_pts + up((size_t)n_pts * 128);
-    const size_t o_ok = o_tail + TAIL_BYTES, bytes = o_ok + 256;
-    DevGuard g(cv.device);
-    cudaStream_t st = cv.st;
+    const size_t o_part = o_y2 + level, o_pts = o_part + up((size_t)n_pts * chunks * 32);
+    const size_t o_tail = o_pts + up((size_t)groups * n_pts * 128), o_wf = o_tail + (size_t)groups * TAIL_BYTES;
+    const size_t o_gv = o_wf + up(count), o_ok = o_gv + up(groups), bytes = o_ok + 256;
     verify_bufs_ensure(fn, *cv.vbufs, count, inputs, 0, bytes, compressed ? comp_bytes(count) : 0);
     VerifyBufs& v = **cv.vbufs;
     batch_streams(v);
-    cudaStream_t s2 = v.side[0], s3 = v.side[1];
-    cudaEvent_t ev_up = v.ev[0], ev_prep = v.ev[1], ev_pts = v.ev[2], ev_s2 = v.ev[3], ev_s3 = v.ev[4];
-    uint8_t* B = v.d_batch;
-    uint8_t* tail = B + o_tail;
-    const uint32_t* w = (const uint32_t*)(B + o_w);
-    uint32_t* ok = (uint32_t*)(B + o_ok);
-    auto prod = [](cudaStream_t s) {
-        return [s](uint32_t blocks, const uint8_t* src, size_t stride, uint32_t n, uint8_t* o) { f12_product_kernel<<<blocks, 64, 0, s>>>(src, stride, n, o); };
-    };
-    auto sum = [](cudaStream_t s) {
-        return [s](uint32_t blocks, const uint8_t* src, size_t stride, uint32_t n, uint8_t* o) { g1_sum_kernel<<<blocks, 128, 0, s>>>(src, stride, n, o); };
-    };
-    if (compressed) decompress_enqueue(v, proofs, count, false, st);
-    else CUDA_CHECK(cudaMemcpyAsync(v.d_proofs, proofs, (size_t)count * 256, cudaMemcpyHostToDevice, st));
-    CUDA_CHECK(cudaMemcpyAsync(B + o_w, weights, (size_t)count * 16, cudaMemcpyHostToDevice, st));
-    if (inputs) CUDA_CHECK(cudaMemcpyAsync(v.d_pub, public_inputs, inputs * 32, cudaMemcpyHostToDevice, st));
-    CUDA_CHECK(cudaMemsetAsync(ok, 0xff, 4, st));
-    CUDA_CHECK(cudaEventRecord(ev_up, st));
-    // main stream: per-proof parse and scaling, Miller loops, their product, then the verdict
-    batch_prepare_kernel<<<(count + 127) / 128, 128, 0, st>>>(v.d_proofs, w, count, v.d_rec, ok);
-    CUDA_CHECK(cudaEventRecord(ev_prep, st));
-    batch_miller_kernel<<<(count + 63) / 64, 64, 0, st>>>(v.d_rec, ok, count, v.d_f);
-    tree_reduce(v.d_f, F12_BYTES, F12_BYTES, count, 64, B + o_x, B + o_y, tail + TAIL_F, prod(st));
-    // side stream 2: the input scalars, the prepared inputs, e(alpha, beta)^s_0, the G2 membership of every B
-    CUDA_CHECK(cudaStreamWaitEvent(s2, ev_up, 0));
-    batch_scalars_kernel<<<dim3(n_pts, chunks), 128, 0, s2>>>(w, (const uint32_t*)v.d_pub, vk->n_public, count, B + o_part);
-    batch_inputs_kernel<<<(n_pts + 3) / 4, 128, 0, s2>>>(vk->d_tabs, vk->d_g1, B + o_part, chunks, vk->n_public, B + o_pts, tail);
-    tree_reduce(B + o_pts, 128, 128, n_pts, 128, B + o_x2, B + o_y2, tail + TAIL_PREP, sum(s2));
-    CUDA_CHECK(cudaEventRecord(ev_pts, s2));
-    batch_rhs_kernel<<<1, 1, 0, s2>>>(tail, vk->d_eab);
-    batch_g2_kernel<<<(count + 127) / 128, 128, 0, s2>>>(v.d_proofs, count, ok);
-    CUDA_CHECK(cudaEventRecord(ev_s2, s2));
-    // side stream 3, once the r C and the prepared inputs exist: sum r C, then the Miller loop of the prepared pairs
-    CUDA_CHECK(cudaStreamWaitEvent(s3, ev_prep, 0));
-    CUDA_CHECK(cudaStreamWaitEvent(s3, ev_pts, 0));
-    tree_reduce(v.d_rec + BREC_RC, REC_BYTES_V, 128, count, 128, B + o_x2, B + o_y2, tail + TAIL_RC, sum(s3));
-    batch_pairs_kernel<<<1, 1, 0, s3>>>(tail, vk->d_lines, !vk->gamma_inf, !vk->delta_inf);
-    CUDA_CHECK(cudaEventRecord(ev_s3, s3));
-    CUDA_CHECK(cudaStreamWaitEvent(st, ev_s2, 0));
-    CUDA_CHECK(cudaStreamWaitEvent(st, ev_s3, 0));
-    batch_final_kernel<<<1, 1, 0, st>>>(tail, ok, v.d_verdict);
-    g_launch_count += 8;
-    CUDA_CHECK(cudaGetLastError());
-    CUDA_CHECK(cudaMemcpyAsync(verdict_out, v.d_verdict, 1, cudaMemcpyDeviceToHost, st));
-    CUDA_CHECK(cudaStreamSynchronize(st));
-}
-
-// b2g_verify_batch_locate on 256-byte rows, or on compressed rows decoded on the context's stream first.  The batch check
-// runs once per group of LOCATE_GROUP proofs; the well-formed proofs of the groups that fail it then go through
-// b2g_verify_many's kernels, compacted on the host from the caller's rows.
-static void verify_locate_run(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs,
-                              bool compressed, const void* weights, uint8_t* verdicts_out) {
-    if (!weights) throw_error(B2G_E_SHAPE, "null pointer");
-    const CtxView cv = verify_args(fn, ctx, vk, count, public_inputs, proofs, verdicts_out);
-    weights_check(weights, count);
-    const uint32_t n_public = vk->n_public, n_pts = n_public + 1, groups = (count + LOCATE_GROUP - 1) / LOCATE_GROUP;
-    const size_t inputs = (size_t)count * n_public, comp = compressed ? comp_bytes(count) : 0;
-    // scratch: weights, s_gj IC[j] per (group, j), the group tails, wf per proof, the group verdicts and two ok words (the
-    // one batch_prepare_kernel clears, and the one batch_miller_kernel reads, which stays set)
-    auto up = [](size_t b) { return (b + 255) & ~(size_t)255; };
-    const size_t o_w = 0, o_pts = up((size_t)count * 16), o_tail = o_pts + up((size_t)groups * n_pts * 128);
-    const size_t o_wf = o_tail + (size_t)groups * TAIL_BYTES, o_gv = o_wf + up(count), o_ok = o_gv + up(groups), bytes = o_ok + 256;
-    DevGuard g(cv.device);
-    cudaStream_t st = cv.st;
-    verify_bufs_ensure(fn, *cv.vbufs, count, inputs, 0, bytes, comp);
-    VerifyBufs& v = **cv.vbufs;
-    batch_streams(v);
-    cudaStream_t s2 = v.side[0], s3 = v.side[1];
+    cudaStream_t st = cv.st, s2 = v.side[0], s3 = v.side[1];
+    // ev_up: the uploads, before both side streams; ev_prep: the r C records, before side stream 3 sums them; ev_g2: wf,
+    // before the masked product and r C sums (with a mask only); ev_pts: the prepared inputs, before the prepared pairs;
+    // ev_s2, ev_s3: the end of each side stream, before the final kernel
     cudaEvent_t ev_up = v.ev[0], ev_prep = v.ev[1], ev_g2 = v.ev[2], ev_pts = v.ev[3], ev_s2 = v.ev[4], ev_s3 = v.ev[5];
     uint8_t* B = v.d_batch;
     uint8_t *tails = B + o_tail, *wf = B + o_wf, *gv = B + o_gv;
+    const uint8_t* mask = masked ? wf : nullptr;
     const uint32_t* w = (const uint32_t*)(B + o_w);
     uint32_t* ok = (uint32_t*)(B + o_ok);
     if (compressed) decompress_enqueue(v, proofs, count, false, st);
@@ -1104,37 +968,80 @@ static void verify_locate_run(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t
     CUDA_CHECK(cudaMemsetAsync(ok, 0xff, 8, st));
     CUDA_CHECK(cudaMemsetAsync(v.d_rec, 0, (size_t)count * REC_BYTES_V, st));
     CUDA_CHECK(cudaEventRecord(ev_up, st));
-    // main stream: per-proof parse and scaling, every proof's Miller value, the group products, then the group verdicts
+    // main stream: per-proof parse and scaling, then the Miller values.  Without a mask the Miller kernel reads the ok word
+    // and skips a batch that has already failed; with one, every proof needs its Miller value, so it reads the word that
+    // stays set.
     batch_prepare_kernel<<<(count + 127) / 128, 128, 0, st>>>(v.d_proofs, w, count, v.d_rec, ok);
     CUDA_CHECK(cudaEventRecord(ev_prep, st));
-    batch_miller_kernel<<<(count + 63) / 64, 64, 0, st>>>(v.d_rec, ok + 1, count, v.d_f);
-    // side stream 2: the G2 membership of every B, the group scalars and prepared inputs, e(alpha, beta)^s_g0
+    batch_miller_kernel<<<(count + 63) / 64, 64, 0, st>>>(v.d_rec, masked ? ok + 1 : ok, count, v.d_f);
+    // side stream 2: the group scalars and prepared inputs, e(alpha, beta)^s_g0, and the G2 membership of every B: first when
+    // wf masks the sums, last when only the verdict needs it
+    auto g2 = [&] {
+        batch_g2_kernel<<<(count + 127) / 128, 128, 0, s2>>>(v.d_proofs, count, wf, ok);
+        CUDA_CHECK(cudaEventRecord(ev_g2, s2));
+    };
     CUDA_CHECK(cudaStreamWaitEvent(s2, ev_up, 0));
-    locate_g2_kernel<<<(count + 127) / 128, 128, 0, s2>>>(v.d_proofs, count, wf);
-    CUDA_CHECK(cudaEventRecord(ev_g2, s2));
-    locate_inputs_kernel<<<(unsigned)(((size_t)groups * n_pts + 3) / 4), 128, 0, s2>>>(vk->d_tabs, vk->d_g1, w, (const uint32_t*)v.d_pub, wf,
-                                                                                      n_public, count, groups, B + o_pts, tails);
-    g1_segment_sum_kernel<<<groups, 128, 0, s2>>>(B + o_pts, 128, n_pts, (size_t)groups * n_pts, nullptr, tails + TAIL_PREP, TAIL_BYTES);
+    if (masked) g2();
+    batch_scalars_kernel<<<dim3(chunks, n_pts), 128, 0, s2>>>(w, (const uint32_t*)v.d_pub, mask, vk->n_public, count, chunk, B + o_part);
+    batch_inputs_kernel<<<(unsigned)(((size_t)groups * n_pts + 3) / 4), 128, 0, s2>>>(vk->d_tabs, vk->d_g1, B + o_part, per, chunks,
+                                                                                     vk->n_public, groups, B + o_pts, tails);
+    g1_sum_kernel<<<groups, 128, 0, s2>>>(B + o_pts, 128, n_pts, (size_t)groups * n_pts, nullptr, tails + TAIL_PREP, TAIL_BYTES);
     CUDA_CHECK(cudaEventRecord(ev_pts, s2));
-    locate_rhs_kernel<<<(groups + 63) / 64, 64, 0, s2>>>(tails, groups, vk->d_eab);
+    batch_rhs_kernel<<<(groups + 63) / 64, 64, 0, s2>>>(tails, groups, vk->d_eab);
+    if (!masked) g2();
     CUDA_CHECK(cudaEventRecord(ev_s2, s2));
-    // side stream 3, once the r C and the G2 checks exist: the group sums of r C, then the groups' prepared pairs
+    // side stream 3, once the r C (and wf, with a mask) exist: the group sums of r C, then, once the prepared inputs exist,
+    // the groups' prepared pairs
     CUDA_CHECK(cudaStreamWaitEvent(s3, ev_prep, 0));
-    CUDA_CHECK(cudaStreamWaitEvent(s3, ev_g2, 0));
-    g1_segment_sum_kernel<<<groups, 128, 0, s3>>>(v.d_rec + BREC_RC, REC_BYTES_V, LOCATE_GROUP, count, wf, tails + TAIL_RC, TAIL_BYTES);
+    if (masked) CUDA_CHECK(cudaStreamWaitEvent(s3, ev_g2, 0));
+    group_reduce(v.d_rec + BREC_RC, REC_BYTES_V, 128, count, group, 128, mask, B + o_x2, B + o_y2, tails + TAIL_RC,
+                 [&](uint32_t blocks, const uint8_t* src, size_t stride, uint32_t seg, uint32_t n, const uint8_t* m, uint8_t* dst,
+                     size_t dst_stride) { g1_sum_kernel<<<blocks, 128, 0, s3>>>(src, stride, seg, n, m, dst, dst_stride); });
     CUDA_CHECK(cudaStreamWaitEvent(s3, ev_pts, 0));
-    locate_pairs_kernel<<<(groups + 63) / 64, 64, 0, s3>>>(tails, groups, vk->d_lines, !vk->gamma_inf, !vk->delta_inf);
+    batch_pairs_kernel<<<(groups + 63) / 64, 64, 0, s3>>>(tails, groups, vk->d_lines, !vk->gamma_inf, !vk->delta_inf);
     CUDA_CHECK(cudaEventRecord(ev_s3, s3));
-    CUDA_CHECK(cudaStreamWaitEvent(st, ev_g2, 0));
-    locate_product_kernel<<<groups, 64, 0, st>>>(v.d_f, wf, count, tails);
+    // main stream: the group products of the Miller values (f12_product_kernel's CTA always spans 64 records, which is seg
+    // whenever there is more than one CTA), then the group verdicts; the ok word decides a batch verdict only
+    if (masked) CUDA_CHECK(cudaStreamWaitEvent(st, ev_g2, 0));
+    group_reduce(v.d_f, F12_BYTES, F12_BYTES, count, group, 64, mask, B + o_x, B + o_y, tails + TAIL_F,
+                 [&](uint32_t blocks, const uint8_t* src, size_t stride, uint32_t, uint32_t n, const uint8_t* m, uint8_t* dst,
+                     size_t dst_stride) { f12_product_kernel<<<blocks, 64, 0, st>>>(src, stride, n, m, dst, dst_stride); });
     CUDA_CHECK(cudaStreamWaitEvent(st, ev_s2, 0));
     CUDA_CHECK(cudaStreamWaitEvent(st, ev_s3, 0));
-    locate_final_kernel<<<(groups + 63) / 64, 64, 0, st>>>(tails, groups, gv);
-    g_launch_count += 10;
+    batch_final_kernel<<<(groups + 63) / 64, 64, 0, st>>>(tails, groups, masked ? nullptr : ok, gv);
+    g_launch_count += 9;
     CUDA_CHECK(cudaGetLastError());
+    return {wf, gv};
+}
+
+// b2g_verify_batch on 256-byte rows, or on compressed rows: the batch check with one group of the whole batch
+static void verify_batch_run(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs,
+                             bool compressed, const void* weights, uint8_t* verdict_out) {
+    if (!weights) throw_error(B2G_E_SHAPE, "null pointer");
+    const CtxView cv = verify_args(fn, ctx, vk, count, public_inputs, proofs, verdict_out);
+    weights_check(weights, count);
+    DevGuard g(cv.device);
+    const BatchOut r = batch_enqueue(fn, cv, vk, count, count, false, public_inputs, proofs, compressed, weights);
+    CUDA_CHECK(cudaMemcpyAsync(verdict_out, r.verdict, 1, cudaMemcpyDeviceToHost, cv.st));
+    CUDA_CHECK(cudaStreamSynchronize(cv.st));
+}
+
+// b2g_verify_batch_locate on 256-byte rows, or on compressed rows.  The batch check runs once per group of LOCATE_GROUP
+// proofs; the well-formed proofs of the groups that fail it then go through b2g_verify_many's kernels, compacted on the host
+// from the caller's rows.
+static void verify_locate_run(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs,
+                              bool compressed, const void* weights, uint8_t* verdicts_out) {
+    if (!weights) throw_error(B2G_E_SHAPE, "null pointer");
+    const CtxView cv = verify_args(fn, ctx, vk, count, public_inputs, proofs, verdicts_out);
+    weights_check(weights, count);
+    const uint32_t n_public = vk->n_public, groups = (count + LOCATE_GROUP - 1) / LOCATE_GROUP;
+    const size_t inputs = (size_t)count * n_public;
+    DevGuard g(cv.device);
+    cudaStream_t st = cv.st;
+    const BatchOut r = batch_enqueue(fn, cv, vk, count, LOCATE_GROUP, true, public_inputs, proofs, compressed, weights);
     std::vector<uint8_t> ok_h(count), gv_h(groups);
-    CUDA_CHECK(cudaMemcpyAsync(ok_h.data(), wf, count, cudaMemcpyDeviceToHost, st));
-    CUDA_CHECK(cudaMemcpyAsync(gv_h.data(), gv, groups, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaMemcpyAsync(ok_h.data(), r.wf, count, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaMemcpyAsync(gv_h.data(), r.verdict, groups, cudaMemcpyDeviceToHost, st));
     CUDA_CHECK(cudaStreamSynchronize(st));
     // the verdicts: 0 for a malformed proof, 1 in a group that holds, else b2g_verify_many's verdict
     std::vector<uint8_t> out(count);
@@ -1153,7 +1060,7 @@ static void verify_locate_run(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t
             memcpy(rows.data() + k * row, (const uint8_t*)proofs + idx[k] * row, row);
             if (pub_row) memcpy(pubs.data() + k * pub_row, (const uint8_t*)public_inputs + idx[k] * pub_row, pub_row);
         }
-        verify_bufs_ensure(fn, *cv.vbufs, count, inputs, (size_t)m * n_public, bytes, comp);
+        verify_bufs_ensure(fn, *cv.vbufs, count, inputs, (size_t)m * n_public, 0, compressed ? comp_bytes(count) : 0);
         verify_many_enqueue(**cv.vbufs, vk, m, whole ? public_inputs : pubs.data(), whole ? proofs : rows.data(), compressed, st);
         CUDA_CHECK(cudaMemcpyAsync(many.data(), (*cv.vbufs)->d_verdict, m, cudaMemcpyDeviceToHost, st));
         CUDA_CHECK(cudaStreamSynchronize(st));
