@@ -94,17 +94,44 @@ def test_sparse_b_batches(ctx, monkeypatch, compact):
     release(pk); release(cm)
 
 
+def _resolved_witness(circ, w, rng):
+    """another satisfying assignment of a circuit whose rows each set one wire (C = one term, rows in dependency order, as
+    synth.circomlike_circuit builds them): every wire no row sets is redrawn, then each row's target is recomputed, the
+    public output included"""
+    v = list(w)
+    targets = set(np.asarray(circ.C[1]).tolist())
+    for i in range(1, len(v)):
+        if i not in targets:
+            v[i] = rng.randrange(o.R_MOD)
+    terms = {}
+    for name, (rows, cols, vals) in zip('ABC', (circ.A, circ.B, circ.C)):
+        for r_, c_, x in zip(np.asarray(rows).tolist(), np.asarray(cols).tolist(), vals):
+            terms.setdefault((name, r_), []).append((c_, x))
+    for k in range(circ.num_constraints):
+        a = sum(x * v[c_] for c_, x in terms.get(('A', k), ())) % o.R_MOD
+        b = sum(x * v[c_] for c_, x in terms.get(('B', k), ())) % o.R_MOD
+        (col, x), = terms[('C', k)]
+        v[col] = a * b * pow(x, -1, o.R_MOD) % o.R_MOD
+    return v
+
+
 def test_libsnark_reduction_batch_verifies(ctx):
+    """five distinct satisfying witnesses (distinct public outputs) of a circom-like 2^12 circuit under LibsnarkReduction:
+    a proof that reads another proof's a, b, c or h slice no longer equals its single proof nor verifies"""
     from circom_compat_b200 import Groth16, LibsnarkReduction, fr_to_mont, synth, release, Proof
     circ, w = synth.circomlike_circuit(12)
     pk, td = synth.setup(ctx, circ, flavour='libsnark')
     cm = circ.matrices(with_c=True)
-    wm = fr_to_mont(w)
-    rs = _random_rs(random.Random(12), 5)
-    got = _many(pk, cm, rs, [wm] * 5, ctx, LibsnarkReduction)
-    assert got == _singles(pk, cm, rs, [wm] * 5, ctx, LibsnarkReduction)
-    for d in got:
-        assert Groth16.verify(pk, w[1:circ.num_inputs], Proof(d))
+    rng = random.Random(12)
+    ws = [list(w)] + [_resolved_witness(circ, w, rng) for _ in range(4)]
+    assert len({v[1] for v in ws}) == 5
+    wms = [fr_to_mont(v) for v in ws]
+    rs = _random_rs(rng, 5)
+    got = _many(pk, cm, rs, wms, ctx, LibsnarkReduction)
+    assert got == _singles(pk, cm, rs, wms, ctx, LibsnarkReduction)
+    for d, v in zip(got, ws):
+        assert Groth16.verify(pk, v[1:circ.num_inputs], Proof(d))
+    assert not Groth16.verify(pk, ws[1][1:circ.num_inputs], Proof(got[0]))
     release(pk); release(cm)
 
 
