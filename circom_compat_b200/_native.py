@@ -18,6 +18,7 @@ class B2gError(RuntimeError):
     def __init__(self, code: int, msg: str):
         super().__init__(f"b2groth error {code}: {msg}")
         self.code = code
+        self.msg = msg
 
 
 class PolynomialDegreeTooLarge(B2gError):
@@ -40,12 +41,19 @@ class VkDesc(C.Structure):
                [(k, C.c_void_p) for k in ('alpha_g1', 'beta_g2', 'gamma_g2', 'delta_g2', 'gamma_abc_g1')]
 
 
+class KeyBatch(C.Structure):
+    """b2g_key_batch: one batch of proofs under one verifying key (b2g_verify_batch_keys)"""
+    _fields_ = [('vk', C.c_void_p), ('count', C.c_uint32), ('reserved', C.c_uint32)] + \
+               [(k, C.c_void_p) for k in ('public_inputs', 'proofs', 'weights')]
+
+
 EXPORTS = ['b2g_last_error', 'b2g_version', 'b2g_device_count', 'b2g_ctx_create', 'b2g_ctx_destroy', 'b2g_ctx_prepare', 'b2g_pk_load', 'b2g_pk_free',
            'b2g_matrices_load', 'b2g_matrices_free', 'b2g_witness_map', 'b2g_prove', 'b2g_prove_many', 'b2g_prove_submit', 'b2g_prove_wait', 'b2g_host_register', 'b2g_host_unregister', 'b2g_prove_partial', 'b2g_prove_finish',
            'b2g_p2p_export', 'b2g_p2p_import', 'b2g_p2p_connect_local', 'b2g_prove_sharded_p2p', 'b2g_msm_g1', 'b2g_msm_g2', 'b2g_ntt', 'b2g_fixed_base_g1', 'b2g_fixed_base_g2', 'b2g_test_op', 'b2g_last_timings',
            'b2g_bench_device', 'b2g_bench_msm', 'b2g_launch_count', 'b2g_vk_load', 'b2g_vk_free', 'b2g_vk_alpha_beta', 'b2g_verify_many',
            'b2g_verify_batch', 'b2g_proofs_decompress', 'b2g_verify_many_compressed', 'b2g_verify_batch_compressed',
-           'b2g_verify_batch_locate', 'b2g_verify_batch_locate_compressed']
+           'b2g_verify_batch_locate', 'b2g_verify_batch_locate_compressed', 'b2g_verify_batch_keys',
+           'b2g_verify_batch_keys_compressed']
 
 _lib = None
 
@@ -103,6 +111,8 @@ def lib():
         L.b2g_verify_batch_compressed.argtypes = [vp, vp, C.c_uint32, vp, vp, vp, vp]
         L.b2g_verify_batch_locate.argtypes = [vp, vp, C.c_uint32, vp, vp, vp, vp]
         L.b2g_verify_batch_locate_compressed.argtypes = [vp, vp, C.c_uint32, vp, vp, vp, vp]
+        L.b2g_verify_batch_keys.argtypes = [vp, C.c_uint32, C.POINTER(KeyBatch), vp]
+        L.b2g_verify_batch_keys_compressed.argtypes = [vp, C.c_uint32, C.POINTER(KeyBatch), vp]
         _lib = L
     return _lib
 

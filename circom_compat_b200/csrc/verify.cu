@@ -11,23 +11,24 @@
 //   prepare  parse the proof (canonical coordinates; >= p or off the curve -> invalid), sum the prepared inputs, affine
 //   miller   one multi-Miller loop over (A, B), (prepared, -gamma), (C, -delta) sharing one f; only B is stepped here
 //   final    the final exponentiation, compared with e(alpha, beta) -> one verdict byte
-// b2g_verify_batch and b2g_verify_batch_locate check a random linear combination instead (weights r_i from the caller), once
-// per group of `group` consecutive proofs:
+// b2g_verify_batch, b2g_verify_batch_locate and b2g_verify_batch_keys check a random linear combination instead (weights r_i
+// from the caller), once per segment of consecutive proofs under one key:
 //     prod e(r_i A_i, B_i) * e(sum r_i C_i, -delta) * e(s_0 IC[0] + sum_j s_j IC[j], -gamma) == e(alpha, beta)^s_0,
-//     s_0 = sum r_i, s_j = sum r_i x_ij (mod r), x_ij the j-th public input of proof i (j = 1..n_public), sums over the group
-// b2g_verify_batch runs it with one group of the whole batch; b2g_verify_batch_locate with groups of LOCATE_GROUP proofs whose
-// sums leave out the malformed proofs (a mask), then b2g_verify_many on the well-formed proofs of the groups that fail.
+//     s_0 = sum r_i, s_j = sum r_i x_ij (mod r), x_ij the j-th public input of proof i (j = 1..n_public), sums over the segment
+// b2g_verify_batch runs it with one segment of the whole batch; b2g_verify_batch_locate with segments of LOCATE_GROUP proofs
+// whose sums leave out the malformed proofs (a mask), then b2g_verify_many on the well-formed proofs of the segments that
+// fail; b2g_verify_batch_keys with one segment per key.  A segment table and a table of key records drive every stage below.
 //   prepare  one proof per thread: the parse and on-curve checks above, r_i A_i (affine) and r_i C_i (XYZZ)
 //   g2       one proof per thread: the proof parses and its B lies in G2 (the mask)
-//   scalars  one CTA per (chunk of the group or of SCALAR_CHUNK proofs, j): partial sums of r_i x_ij (x_i0 = 1)
-//   inputs   one warp per (group, j): s_j from the group's partial sums, then s_j IC[j] from the window table (IC[0]: a
-//            variable-base product)
+//   scalars  one CTA per (chunk of at most SCALAR_CHUNK proofs of a segment, j): partial sums of r_i x_ij (x_i0 = 1)
+//   inputs   one warp per (segment, j): s_j from the segment's partial sums, then s_j IC[j] from the key's window table
+//            (IC[0]: a variable-base product)
 //   miller   one proof per thread: the one-pair Miller loop of (r_i A_i, B_i)
-//   reduce   per group: the product of the Miller values and the sums of the r_i C_i and of the s_j IC[j]; one CTA per group,
-//            or tree levels of one CTA per 64 or 128 records when the one group is larger
-//   pairs    one group per thread: the Miller loop of the two prepared pairs
-//   rhs      one group per thread: e(alpha, beta)^s_0
-//   final    one group per thread: one final exponentiation, compared with rhs -> one verdict byte per group
+//   reduce   per segment: the product of the Miller values and the sums of the r_i C_i and of the s_j IC[j], in levels of
+//            one CTA per at most 64 or 128 records of one segment, until each segment has one value
+//   pairs    one segment per thread: the Miller loop of the two prepared pairs
+//   rhs      one segment per thread: e(alpha, beta)^s_0
+//   final    one segment per thread: one final exponentiation, compared with rhs -> one verdict byte per segment
 // Only prepare -> miller -> product -> final run on the context's stream; the rest runs next to them on two side streams.
 // b2g_proofs_decompress and the _compressed verifiers take arkworks' 128-byte compressed proofs: a decode kernel (one proof
 // per thread) writes the 256-byte rows the kernels above read, and a second kernel checks that each decoded B lies in G2 (the
@@ -75,6 +76,7 @@ struct VerifyBufs {
     uint8_t* d_comp = nullptr;                    // compressed proofs (128 B each), then one decoded-ok byte per proof
     cudaStream_t side[2] = {nullptr, nullptr};    // the batch check's tail pieces, next to the per-proof kernels
     cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+    std::vector<uint8_t> h_meta;                  // the batch check's key records, segment table and reduction spans (host)
 };
 
 void verify_bufs_free(VerifyBufs* v) {
@@ -160,18 +162,52 @@ __global__ void __launch_bounds__(64) verify_final_kernel(const uint8_t* __restr
 }
 
 // ---------------------------------------------------------------------------------------------- batch check kernels
-// b2g_verify_batch and b2g_verify_batch_locate: the batch equation once per group of `group` consecutive proofs, each group's
-// products and sums optionally masked by wf (wf[i] = 1 when proof i parses and its B lies in G2).
+// b2g_verify_batch, b2g_verify_batch_locate and b2g_verify_batch_keys: the batch equation once per segment of consecutive
+// proofs under one key, each segment's products and sums optionally masked by wf (wf[i] = 1 when proof i parses and its B
+// lies in G2).
 // Per-proof record, REC_BYTES_V apart: r A (affine, 64 B), B (affine, 128 B), r C (XYZZ, 128 B).  The record area is zeroed
 // first, so a proof that does not parse keeps r A and r C at infinity.  The ok word starts all ones and any failed parse,
 // on-curve or G2 check clears it.
 constexpr size_t BREC_B = 64, BREC_RC = 192;
-// tail values of a group, group g's at tails + g * TAIL_BYTES (Fq12 384 B, G1 XYZZ 128 B): the product of the per-proof
+// tail values of a segment, segment g's at tails + g * TAIL_BYTES (Fq12 384 B, G1 XYZZ 128 B): the product of the per-proof
 // Miller values, the Miller value of the prepared pairs, e(alpha, beta)^s_0, sum r C, the prepared inputs, s_0
 constexpr size_t TAIL_F = 0, TAIL_G = 384, TAIL_RHS = 768, TAIL_RC = 1152, TAIL_PREP = 1280, TAIL_S0 = 1408, TAIL_BYTES = 1536;
-static_assert(TAIL_BYTES % 256 == 0, "group tails stay 256-byte aligned");
-constexpr uint32_t LOCATE_GROUP = 64;              // proofs per group of b2g_verify_batch_locate: one CTA of f12_product_kernel
+static_assert(TAIL_BYTES % 256 == 0, "segment tails stay 256-byte aligned");
+constexpr uint32_t LOCATE_GROUP = 64;              // proofs per segment of b2g_verify_batch_locate: one CTA of f12_product_kernel
 constexpr uint32_t SCALAR_CHUNK = 2048;            // at most this many proofs per CTA of batch_scalars_kernel
+
+// the key a segment is checked under: its prepared lines of -gamma and -delta, e(alpha, beta), the window tables of
+// IC[1..n_public], alpha and IC (b2g_vk's arrays), and whether each prepared pair takes part (gamma, delta not at infinity)
+struct KeyRec {
+    const uint8_t *lines, *eab, *tabs, *g1;
+    uint32_t n_public, gamma_on, delta_on, pad;
+};
+// a segment: proofs first .. first + count - 1 under key record `key`; its public inputs start at scalar `pub`, its
+// (chunk, j) work items of batch_scalars_kernel at `part` (chunks of them, chunk-major: chunk q's item j is part + q *
+// (n_public + 1) + j), its prepared-input points at `pt`.  first, part and pt increase along the table.
+struct Seg {
+    uint64_t pub;
+    uint32_t key, first, count, part, chunks, pt;
+};
+// one CTA of a segmented reduction: records first .. first + n - 1 of one segment, to value `out` of the next level, or to
+// the tail of segment out & ~TO_TAIL when TO_TAIL is set
+struct Span { uint32_t first, n, out; };
+constexpr uint32_t TO_TAIL = 0x80000000u;
+
+// the last segment k < n with s[k].*M <= v, for a field that is nondecreasing along the table
+template <uint32_t Seg::*M>
+__device__ __forceinline__ uint32_t seg_find(const Seg* __restrict__ s, uint32_t n, uint32_t v) {
+    uint32_t lo = 0, hi = n;
+    while (hi - lo > 1) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (s[mid].*M <= v) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+
+__device__ __forceinline__ uint8_t* span_out(const Span& s, uint8_t* dst, size_t rec_bytes, uint8_t* tails) {
+    return s.out & TO_TAIL ? tails + (size_t)(s.out & ~TO_TAIL) * TAIL_BYTES : dst + (size_t)s.out * rec_bytes;
+}
 
 __device__ __forceinline__ void weight_load(uint32_t* k, const uint32_t* w, size_t i) {
     for (int t = 0; t < 4; t++) k[t] = w[4 * i + t];
@@ -205,19 +241,22 @@ __global__ void __launch_bounds__(128) batch_g2_kernel(const uint8_t* __restrict
     if (!good) atomicAnd(ok_all, 0u);
 }
 
-// CTA (c, j): part[j * gridDim.x + c] = the sum over the proofs i of chunk c (`chunk` proofs) of r_i (j = 0) or of
-// Fr::mul(r_i, x_ij) = r_i x_ij / R (j >= 1), leaving out proof i when mask[i] = 0 (no mask: every proof)
+// CTA t, the work item (chunk q of segment s, j): part[t] = the sum over the proofs i of the chunk (SCALAR_CHUNK proofs
+// from s.first + q * SCALAR_CHUNK, fewer at the segment's end) of r_i (j = 0) or of Fr::mul(r_i, x_ij) = r_i x_ij / R
+// (j >= 1), leaving out proof i when mask[i] = 0 (no mask: every proof)
 __global__ void __launch_bounds__(128) batch_scalars_kernel(const uint32_t* __restrict__ w, const uint32_t* __restrict__ pub,
-                                                            const uint8_t* __restrict__ mask, uint32_t n_public, uint32_t count,
-                                                            uint32_t chunk, uint8_t* __restrict__ part) {
+                                                            const uint8_t* __restrict__ mask, const Seg* __restrict__ segs,
+                                                            uint32_t n_segs, const KeyRec* __restrict__ keys, uint8_t* __restrict__ part) {
     __shared__ fe sh[128];
-    const uint32_t j = blockIdx.y, end = min(count, (blockIdx.x + 1) * chunk);
+    const Seg s = segs[seg_find<&Seg::part>(segs, n_segs, blockIdx.x)];
+    const uint32_t n_public = keys[s.key].n_public, q = (blockIdx.x - s.part) / (n_public + 1), j = (blockIdx.x - s.part) % (n_public + 1);
+    const uint32_t end = s.first + min(s.count, (q + 1) * SCALAR_CHUNK);
     fe acc = Fr::zero();
-    for (uint32_t i = blockIdx.x * chunk + threadIdx.x; i < end; i += 128) {
+    for (uint32_t i = s.first + q * SCALAR_CHUNK + threadIdx.x; i < end; i += 128) {
         if (mask && !mask[i]) continue;
         fe wi = fe_zero();
         weight_load(wi.l, w, i);
-        acc = Fr::add(acc, j ? Fr::mul(wi, fe_load(pub + 8 * ((size_t)i * n_public + j - 1))) : wi);
+        acc = Fr::add(acc, j ? Fr::mul(wi, fe_load(pub + 8 * (s.pub + (size_t)(i - s.first) * n_public + j - 1))) : wi);
     }
     sh[threadIdx.x] = acc;
     __syncthreads();
@@ -225,26 +264,27 @@ __global__ void __launch_bounds__(128) batch_scalars_kernel(const uint32_t* __re
         if ((int)threadIdx.x < d) sh[threadIdx.x] = Fr::add(sh[threadIdx.x], sh[threadIdx.x + d]);
         __syncthreads();
     }
-    if (threadIdx.x == 0) fe_store(part + ((size_t)j * gridDim.x + blockIdx.x) * 32, sh[0]);
+    if (threadIdx.x == 0) fe_store(part + (size_t)blockIdx.x * 32, sh[0]);
 }
 
-// one warp per (group g, j = 0..n_public), t = g * (n_public + 1) + j: s_gj = the sum of the group's `per` chunk sums of
-// batch_scalars_kernel (`chunks` in all), then pts[t] = s_gj IC[j] (IC[0]: a variable-base product); s_g0 to the group's tail
-__global__ void __launch_bounds__(128) batch_inputs_kernel(const uint8_t* __restrict__ tabs, const uint8_t* __restrict__ g1,
-                                                           const uint8_t* __restrict__ part, uint32_t per, uint32_t chunks,
-                                                           uint32_t n_public, uint32_t groups, uint8_t* __restrict__ pts,
-                                                           uint8_t* __restrict__ tails) {
+// one warp per prepared-input point t < n_pts_all, point j = t - seg.pt of segment g (j = 0..n_public of its key): s_gj = the
+// sum of the segment's chunk sums of batch_scalars_kernel, then pts[t] = s_gj IC[j] (IC[0]: a variable-base product); s_g0
+// to the segment's tail
+__global__ void __launch_bounds__(128) batch_inputs_kernel(const uint8_t* __restrict__ part, const Seg* __restrict__ segs, uint32_t n_segs,
+                                                           const KeyRec* __restrict__ keys, uint32_t n_pts_all,
+                                                           uint8_t* __restrict__ pts, uint8_t* __restrict__ tails) {
     __shared__ G1::Pt sh[4][32];
     __shared__ fe s[4];
-    const uint32_t wid = threadIdx.x >> 5, lane = threadIdx.x & 31, n_pts = n_public + 1;
+    const uint32_t wid = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const size_t t = (size_t)blockIdx.x * 4 + wid;
-    if (t >= (size_t)groups * n_pts) return;               // whole warps leave together
-    const uint32_t g = (uint32_t)(t / n_pts), j = (uint32_t)(t % n_pts);
+    if (t >= n_pts_all) return;                            // whole warps leave together
+    const uint32_t g = seg_find<&Seg::pt>(segs, n_segs, (uint32_t)t);
+    const Seg sg = segs[g];
+    const KeyRec& key = keys[sg.key];
+    const uint32_t n_pts = key.n_public + 1, j = (uint32_t)t - sg.pt;
+    const uint8_t *tabs = key.tabs, *g1 = key.g1;
     fe acc = Fr::zero();
-    for (uint32_t k = lane; k < per; k += 32) {
-        const uint32_t c = g * per + k;
-        if (c < chunks) acc = Fr::add(acc, fe_load(part + ((size_t)j * chunks + c) * 32));
-    }
+    for (uint32_t q = lane; q < sg.chunks; q += 32) acc = Fr::add(acc, fe_load(part + ((size_t)sg.part + (size_t)q * n_pts + j) * 32));
     for (int d = 16; d > 0; d >>= 1) {
         fe o;
         for (int q = 0; q < 8; q++) o.l[q] = __shfl_down_sync(0xffffffffu, acc.l[q], d);
@@ -275,37 +315,38 @@ __global__ void __launch_bounds__(64) batch_miller_kernel(const uint8_t* __restr
     Fq12::store(fout + (size_t)j * F12_BYTES, f);
 }
 
-// CTA b: dst + b * dst_stride = the product of src[64 b .. 64 b + 63] below n (Fq12, `stride` bytes apart), taking 1 for
-// record i when mask[i] = 0 (no mask: every record)
-__global__ void __launch_bounds__(64) f12_product_kernel(const uint8_t* __restrict__ src, size_t stride, uint32_t n,
-                                                         const uint8_t* __restrict__ mask, uint8_t* __restrict__ dst, size_t dst_stride) {
+// CTA b, span sp = spans[b] (n <= 64): the product of src[sp.first .. sp.first + sp.n - 1] (Fq12, `stride` bytes apart),
+// taking 1 for record i when mask[i] = 0 (no mask: every record), to dst (F12_BYTES apart) or to a tail (at tails)
+__global__ void __launch_bounds__(64) f12_product_kernel(const uint8_t* __restrict__ src, size_t stride, const Span* __restrict__ spans,
+                                                         const uint8_t* __restrict__ mask, uint8_t* __restrict__ dst, uint8_t* __restrict__ tails) {
     __shared__ fe12 sh[64];
-    const uint32_t t = threadIdx.x, i = blockIdx.x * 64 + t;
-    sh[t] = i < n && (!mask || mask[i]) ? Fq12::load(src + (size_t)i * stride) : Fq12::one();
+    const Span sp = spans[blockIdx.x];
+    const uint32_t t = threadIdx.x, i = sp.first + t;
+    sh[t] = t < sp.n && (!mask || mask[i]) ? Fq12::load(src + (size_t)i * stride) : Fq12::one();
     __syncthreads();
     for (uint32_t d = 32; d > 0; d >>= 1) {
         if (t < d) { fe12 x = sh[t]; Fq12::mul(x, x, sh[t + d]); sh[t] = x; }
         __syncthreads();
     }
-    if (t == 0) Fq12::store(dst + (size_t)blockIdx.x * dst_stride, sh[0]);
+    if (t == 0) Fq12::store(span_out(sp, dst, F12_BYTES, tails), sh[0]);
 }
 
-// CTA b: dst + b * dst_stride = the sum of src[seg * b .. seg * b + seg - 1] below n (G1 XYZZ, `stride` bytes apart), leaving
-// out record i when mask[i] = 0 (no mask: every record)
-__global__ void __launch_bounds__(128) g1_sum_kernel(const uint8_t* __restrict__ src, size_t stride, uint32_t seg, size_t n,
-                                                     const uint8_t* __restrict__ mask, uint8_t* __restrict__ dst, size_t dst_stride) {
+// CTA b, span sp = spans[b]: the sum of src[sp.first .. sp.first + sp.n - 1] (G1 XYZZ, `stride` bytes apart), leaving out
+// record i when mask[i] = 0 (no mask: every record), to dst (128 B apart) or to a tail (at tails)
+__global__ void __launch_bounds__(128) g1_sum_kernel(const uint8_t* __restrict__ src, size_t stride, const Span* __restrict__ spans,
+                                                     const uint8_t* __restrict__ mask, uint8_t* __restrict__ dst, uint8_t* __restrict__ tails) {
     __shared__ G1::Pt sh[128];
-    const uint32_t t = threadIdx.x;
-    const size_t base = (size_t)blockIdx.x * seg, end = min(n, base + seg);
+    const Span sp = spans[blockIdx.x];
+    const uint32_t t = threadIdx.x, end = sp.first + sp.n;
     sh[t] = G1::infinity();                                // accumulated in shared memory: a register sum spills
-    for (size_t i = base + t; i < end; i += 128)
-        if (!mask || mask[i]) { G1::Pt x = sh[t]; G1::add(x, pt_load<Fq>(src + i * stride, 0)); sh[t] = x; }
+    for (uint32_t i = sp.first + t; i < end; i += 128)
+        if (!mask || mask[i]) { G1::Pt x = sh[t]; G1::add(x, pt_load<Fq>(src + (size_t)i * stride, 0)); sh[t] = x; }
     __syncthreads();
     for (uint32_t d = 64; d > 0; d >>= 1) {
         if (t < d) { G1::Pt x = sh[t]; G1::add(x, sh[t + d]); sh[t] = x; }
         __syncthreads();
     }
-    if (t == 0) pt_store<Fq>(dst + (size_t)blockIdx.x * dst_stride, 0, sh[0]);
+    if (t == 0) pt_store<Fq>(span_out(sp, dst, 128, tails), 0, sh[0]);
 }
 
 // the Miller value of the prepared pairs (prepared inputs, -gamma) and (sum r C, -delta); 1 when both drop out
@@ -322,21 +363,24 @@ __device__ __forceinline__ void tail_pairs(uint8_t* tail, const uint8_t* lines, 
     Fq12::store(tail + TAIL_G, g);
 }
 
-// one group per thread: the Miller value of the group's prepared pairs
-__global__ void __launch_bounds__(64) batch_pairs_kernel(uint8_t* __restrict__ tails, uint32_t groups, const uint8_t* __restrict__ lines,
-                                                         bool gamma_on, bool delta_on) {
+// one segment per thread: the Miller value of the segment's prepared pairs, with the lines of the segment's key
+__global__ void __launch_bounds__(64) batch_pairs_kernel(uint8_t* __restrict__ tails, uint32_t n_segs, const Seg* __restrict__ segs,
+                                                         const KeyRec* __restrict__ keys) {
     const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
-    if (g < groups) tail_pairs(tails + (size_t)g * TAIL_BYTES, lines, gamma_on, delta_on);
+    if (g >= n_segs) return;
+    const KeyRec& key = keys[segs[g].key];
+    tail_pairs(tails + (size_t)g * TAIL_BYTES, key.lines, key.gamma_on, key.delta_on);
 }
 
-// one group per thread: e(alpha, beta)^s_g0
-__global__ void __launch_bounds__(64) batch_rhs_kernel(uint8_t* __restrict__ tails, uint32_t groups, const uint8_t* __restrict__ eab) {
+// one segment per thread: e(alpha, beta)^s_g0 of the segment's key
+__global__ void __launch_bounds__(64) batch_rhs_kernel(uint8_t* __restrict__ tails, uint32_t n_segs, const Seg* __restrict__ segs,
+                                                       const KeyRec* __restrict__ keys) {
     const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
-    if (g >= groups) return;
+    if (g >= n_segs) return;
     uint8_t* tail = tails + (size_t)g * TAIL_BYTES;
     fe12 rhs;
     const fe s0 = fe_load(tail + TAIL_S0);
-    Fq12::cyclotomic_exp(rhs, Fq12::load(eab), s0.l);
+    Fq12::cyclotomic_exp(rhs, Fq12::load(keys[segs[g].key].eab), s0.l);
     Fq12::store(tail + TAIL_RHS, rhs);
 }
 
@@ -348,12 +392,21 @@ __device__ __forceinline__ bool tail_holds(const uint8_t* tail) {
     return Fq12::eq(e, Fq12::load(tail + TAIL_RHS));
 }
 
-// one group per thread: verdict[g] = the ok word is set (no ok word: always) and the group's batch equation holds.  A group
-// whose proofs are all masked out has every value at 1 (product, pairs and e(alpha, beta)^0), so it holds.
-__global__ void __launch_bounds__(64) batch_final_kernel(const uint8_t* __restrict__ tails, uint32_t groups, const uint32_t* __restrict__ ok_all,
-                                                         uint8_t* __restrict__ verdict) {
+// one segment per thread: verdict[g] = the ok word is set (no ok word: always), the segment's ok byte is set (no ok bytes:
+// always) and the segment's batch equation holds.  A segment whose proofs are all masked out has every value at 1 (product,
+// pairs and e(alpha, beta)^0), so it holds.
+__global__ void __launch_bounds__(64) batch_final_kernel(const uint8_t* __restrict__ tails, uint32_t n_segs, const uint32_t* __restrict__ ok_all,
+                                                         const uint8_t* __restrict__ seg_ok, uint8_t* __restrict__ verdict) {
     const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
-    if (g < groups) verdict[g] = (!ok_all || *ok_all) && tail_holds(tails + (size_t)g * TAIL_BYTES);
+    if (g < n_segs) verdict[g] = (!ok_all || *ok_all) && (!seg_ok || seg_ok[g]) && tail_holds(tails + (size_t)g * TAIL_BYTES);
+}
+
+// one proof per thread, after batch_g2_kernel: clears the ok byte of the segment that holds a proof with wf[j] = 0, so that
+// a malformed proof fails its own segment only (b2g_verify_batch_keys)
+__global__ void __launch_bounds__(128) batch_segment_ok_kernel(const uint8_t* __restrict__ wf, const Seg* __restrict__ segs, uint32_t n_segs,
+                                                               uint32_t count, uint8_t* __restrict__ seg_ok) {
+    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j < count && !wf[j]) seg_ok[seg_find<&Seg::first>(segs, n_segs, j)] = 0;
 }
 
 // b2g_test_op ops 43-45: G2 membership of a G2 affine point (out: 8 B, 1 or 0), r * P for a G1 affine P and a 128-bit r
@@ -619,13 +672,24 @@ static void verify_stage_test_op(cudaStream_t st, int op, const void* a, const v
         }
         d.s = dev_upload<uint8_t>(stage.data(), stage.size(), st);
         CUDA_CHECK(cudaMalloc(&d.o, n * so));
+        // op 53: per row, a key record with the row's lines and a one-segment table, as batch_enqueue builds them
+        if (op == 53) {
+            std::vector<uint8_t> meta(n * sizeof(KeyRec) + sizeof(Seg));
+            KeyRec* keys = reinterpret_cast<KeyRec*>(meta.data());
+            for (size_t i = 0; i < n; i++)
+                keys[i] = {d.s + i * STAGE_BYTES + STAGE_LINES, nullptr, nullptr, nullptr, 0, on[2 * i], on[2 * i + 1], 0};
+            const Seg seg = {0, 0, 0, 1, 0, 1, 0};
+            memcpy(meta.data() + n * sizeof(KeyRec), &seg, sizeof(Seg));
+            d.a = dev_upload<uint8_t>(meta.data(), meta.size(), st);
+            CUDA_CHECK(cudaStreamSynchronize(st));         // meta is pageable and leaves scope here
+        }
         for (size_t i = 0; i < n; i++) {
             uint8_t* g = d.s + i * STAGE_BYTES;
             vk_lines_kernel<<<1, 32, 0, st>>>(g + STAGE_G2, g + STAGE_LINES);
             if (op == 49) {
                 verify_miller_kernel<<<1, 64, 0, st>>>(g + STAGE_REC, g + STAGE_LINES, on[2 * i], on[2 * i + 1], 1, d.o + i * F12_BYTES);
             } else {
-                batch_pairs_kernel<<<1, 1, 0, st>>>(g + STAGE_REC, 1, g + STAGE_LINES, on[2 * i], on[2 * i + 1]);
+                batch_pairs_kernel<<<1, 1, 0, st>>>(g + STAGE_REC, 1, (const Seg*)(d.a + n * sizeof(KeyRec)), (const KeyRec*)d.a + i);
                 CUDA_CHECK(cudaMemcpyAsync(d.o + i * F12_BYTES, g + STAGE_REC + TAIL_G, F12_BYTES, cudaMemcpyDeviceToDevice, st));
             }
         }
@@ -760,23 +824,45 @@ static void batch_streams(VerifyBufs& v) {
     for (cudaEvent_t& e : v.ev) if (!e) CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
 }
 
-// reduces n records of `src` (`stride` bytes apart) to one value per group of `group` records, group g's at dst +
-// g * TAIL_BYTES.  A group of at most `per` records takes one CTA of one launch; a larger group, which must then be the only
-// one, takes a tree of launches of `per` records per CTA, the levels alternating between the scratch areas x and y.  Only
-// the first level reads the mask.  level(blocks, src, stride, seg, n, mask, dst, dst_stride) launches one level.
+// the CTAs of a segmented reduction to one value per segment, `per` records per CTA, level by level: the first level reads
+// each segment's records (segs[k].first .. + count), each later level the values the previous level wrote for the segments
+// that still have more than one, and a segment's last value goes to its tail.  Appends the spans of every level to `spans`
+// and returns the number of CTAs per level; *scratch = the most values one level writes below the tails.
+static std::vector<uint32_t> reduce_plan(const std::vector<Seg>& segs, uint32_t per, std::vector<Span>& spans, size_t* scratch) {
+    std::vector<uint32_t> first(segs.size()), len(segs.size()), levels;
+    for (size_t k = 0; k < segs.size(); k++) { first[k] = segs[k].first; len[k] = segs[k].count; }
+    for (uint32_t out = 1; out;) {
+        const size_t before = spans.size();
+        out = 0;
+        for (uint32_t k = 0; k < (uint32_t)segs.size(); k++) {
+            if (!len[k]) continue;                         // done at an earlier level
+            const uint32_t blocks = (len[k] + per - 1) / per;
+            for (uint32_t b = 0; b < blocks; b++)
+                spans.push_back({first[k] + b * per, std::min(per, len[k] - b * per), blocks == 1 ? TO_TAIL | k : out + b});
+            if (blocks == 1) { len[k] = 0; continue; }
+            first[k] = out; len[k] = blocks; out += blocks;
+        }
+        levels.push_back((uint32_t)(spans.size() - before));
+        *scratch = std::max(*scratch, (size_t)out);
+    }
+    return levels;
+}
+
+// launches the levels of a reduce_plan: the first reads `src` (`stride` bytes apart) under the mask, the later ones the
+// scratch areas x and y in turn (rec_bytes apart); level(blocks, src, stride, spans, mask, dst) launches one level
 template <class Level>
-static void group_reduce(const uint8_t* src, size_t stride, size_t rec_bytes, uint32_t n, uint32_t group, uint32_t per,
-                         const uint8_t* mask, uint8_t* x, uint8_t* y, uint8_t* dst, Level&& level) {
-    for (;;) {
-        const uint32_t seg = std::min(group, per), blocks = (n + seg - 1) / seg;
-        const bool last = seg == group;
-        level(blocks, src, stride, seg, n, mask, last ? dst : x, last ? TAIL_BYTES : rec_bytes);
+static void reduce_run(const std::vector<uint32_t>& levels, const Span* spans, const uint8_t* src, size_t stride, size_t rec_bytes,
+                       const uint8_t* mask, uint8_t* x, uint8_t* y, Level&& level) {
+    for (uint32_t blocks : levels) {
+        level(blocks, src, stride, spans, mask, x);
         g_launch_count += 1;
-        if (last) return;
-        src = x; stride = rec_bytes; n = group = blocks; mask = nullptr;
+        spans += blocks; src = x; stride = rec_bytes; mask = nullptr;
         std::swap(x, y);
     }
 }
+
+// one segment of the batch check: `count` consecutive proofs under key record `key`
+struct SegIn { uint32_t key, count; };
 
 }  // namespace b2g
 
@@ -926,109 +1012,147 @@ static void weights_check(const void* weights, uint32_t count) {
         if (all_zero((const uint8_t*)weights + 16 * (size_t)i, 16)) throw_error(B2G_E_INPUT, "weight " + std::to_string(i) + " is zero");
 }
 
-// the device results of batch_enqueue: wf (one byte per proof: it parses and its B lies in G2) and one verdict per group
+// the device results of batch_enqueue: wf (one byte per proof: it parses and its B lies in G2) and one verdict per segment
 struct BatchOut { const uint8_t* wf; const uint8_t* verdict; };
 
-// the batch check of b2g_verify_batch (group = count, no mask) and b2g_verify_batch_locate (group = LOCATE_GROUP, masked by
-// wf), on 256-byte rows or on compressed rows decoded on the context's stream before anything else reads them
-// (batch_g2_kernel checks the decoded B, so the decoder skips the G2 check).  The results are ready once the context's stream
-// is.
-static BatchOut batch_enqueue(const char* fn, const CtxView& cv, b2g_vk* vk, uint32_t count, uint32_t group, bool masked,
-                              const void* public_inputs, const void* proofs, bool compressed, const void* weights) {
-    const uint32_t n_pts = vk->n_public + 1, groups = (count + group - 1) / group;
-    // the scalar sums in chunks of a group, or of SCALAR_CHUNK proofs when the one group is larger: per chunks per group
-    const uint32_t chunk = std::min(group, SCALAR_CHUNK), chunks = (count + chunk - 1) / chunk, per = (group + chunk - 1) / chunk;
-    const size_t inputs = (size_t)count * vk->n_public;
-    // scratch: weights, four tree levels (x, y for the Miller values on the main stream, x2, y2 for the r C on side stream
-    // 3; a group of more than one CTA needs them), chunk sums of the scalars, s_gj IC[j] per (group, j), the group tails,
-    // wf, the group verdicts and two ok words (the one batch_prepare_kernel and batch_g2_kernel clear, and one that stays set)
+// the batch check over a segment table: segment g holds the next segs_in[g].count proofs, checked under vks[segs_in[g].key].
+//   b2g_verify_batch         one segment, no mask; the verdict ANDs the ok word
+//   b2g_verify_batch_locate  segments of LOCATE_GROUP proofs under one key, masked by wf
+//   b2g_verify_batch_keys    one segment per key (keyed), no mask; each verdict ANDs its segment's ok byte
+// on 256-byte rows or on compressed rows decoded on the context's stream before anything else reads them (batch_g2_kernel
+// checks the decoded B, so the decoder skips the G2 check).  The results are ready once the context's stream is.
+static BatchOut batch_enqueue(const char* fn, const CtxView& cv, const std::vector<b2g_vk*>& vks, const std::vector<SegIn>& segs_in,
+                              bool masked, bool keyed, const void* public_inputs, const void* proofs, bool compressed,
+                              const void* weights) {
+    // the per-call tables: key records, segments, then the spans of the Miller-value products, of the r C sums and of the
+    // prepared-input sums (one CTA per segment)
+    std::vector<KeyRec> keys(vks.size());
+    for (size_t k = 0; k < vks.size(); k++) {
+        const b2g_vk* vk = vks[k];
+        keys[k] = {vk->d_lines, vk->d_eab, vk->d_tabs, vk->d_g1, vk->n_public, !vk->gamma_inf, !vk->delta_inf, 0};
+    }
+    const uint32_t n_segs = (uint32_t)segs_in.size();
+    std::vector<Seg> segs(n_segs);
+    uint32_t count = 0, items = 0, n_pts_all = 0;
+    size_t inputs = 0;
+    for (uint32_t g = 0; g < n_segs; g++) {
+        const SegIn& in = segs_in[g];
+        const uint32_t n_public = keys[in.key].n_public, chunks = (in.count + SCALAR_CHUNK - 1) / SCALAR_CHUNK;
+        segs[g] = {inputs, in.key, count, in.count, items, chunks, n_pts_all};
+        count += in.count; inputs += (size_t)in.count * n_public; items += chunks * (n_public + 1); n_pts_all += n_public + 1;
+    }
+    std::vector<Span> spans;
+    size_t lvl_f = 0, lvl_g = 0;
+    const std::vector<uint32_t> levels_f = reduce_plan(segs, 64, spans, &lvl_f);
+    const size_t sp_g = spans.size();
+    const std::vector<uint32_t> levels_g = reduce_plan(segs, 128, spans, &lvl_g);
+    const size_t sp_p = spans.size();
+    for (uint32_t g = 0; g < n_segs; g++) spans.push_back({segs[g].pt, keys[segs_in[g].key].n_public + 1, TO_TAIL | g});
     auto up = [](size_t b) { return (b + 255) & ~(size_t)255; };
-    const size_t level = up(std::max((size_t)((count + 63) / 64) * F12_BYTES, (size_t)((count + 127) / 128) * 128));
+    const size_t m_segs = up(keys.size() * sizeof(KeyRec)), m_spans = m_segs + up(segs.size() * sizeof(Seg));
+    const size_t meta = m_spans + spans.size() * sizeof(Span);
+    // scratch: weights, four reduction levels (x, y for the Miller values on the main stream, x2, y2 for the r C on side
+    // stream 3; a segment of more than one CTA needs them), the chunk sums of the scalars, s_gj IC[j] per (segment, j), the
+    // segment tails, wf, the segment verdicts, the segment ok bytes (keyed), two ok words (the one batch_prepare_kernel and
+    // batch_g2_kernel clear, and one that stays set), the tables
+    const size_t level = up(std::max(lvl_f * F12_BYTES, lvl_g * 128));
     const size_t o_w = 0, o_x = up((size_t)count * 16), o_y = o_x + level, o_x2 = o_y + level, o_y2 = o_x2 + level;
-    const size_t o_part = o_y2 + level, o_pts = o_part + up((size_t)n_pts * chunks * 32);
-    const size_t o_tail = o_pts + up((size_t)groups * n_pts * 128), o_wf = o_tail + (size_t)groups * TAIL_BYTES;
-    const size_t o_gv = o_wf + up(count), o_ok = o_gv + up(groups), bytes = o_ok + 256;
+    const size_t o_part = o_y2 + level, o_pts = o_part + up((size_t)items * 32);
+    const size_t o_tail = o_pts + up((size_t)n_pts_all * 128), o_wf = o_tail + (size_t)n_segs * TAIL_BYTES;
+    const size_t o_gv = o_wf + up(count), o_sok = o_gv + up(n_segs), o_ok = o_sok + up(n_segs), o_meta = o_ok + 256;
+    const size_t bytes = o_meta + up(meta);
     verify_bufs_ensure(fn, *cv.vbufs, count, inputs, 0, bytes, compressed ? comp_bytes(count) : 0);
     VerifyBufs& v = **cv.vbufs;
     batch_streams(v);
+    // the tables go up in one copy from a host buffer that outlives the call
+    v.h_meta.assign(meta, 0);
+    memcpy(v.h_meta.data(), keys.data(), keys.size() * sizeof(KeyRec));
+    memcpy(v.h_meta.data() + m_segs, segs.data(), segs.size() * sizeof(Seg));
+    memcpy(v.h_meta.data() + m_spans, spans.data(), spans.size() * sizeof(Span));
     cudaStream_t st = cv.st, s2 = v.side[0], s3 = v.side[1];
     // ev_up: the uploads, before both side streams; ev_prep: the r C records, before side stream 3 sums them; ev_g2: wf,
     // before the masked product and r C sums (with a mask only); ev_pts: the prepared inputs, before the prepared pairs;
     // ev_s2, ev_s3: the end of each side stream, before the final kernel
     cudaEvent_t ev_up = v.ev[0], ev_prep = v.ev[1], ev_g2 = v.ev[2], ev_pts = v.ev[3], ev_s2 = v.ev[4], ev_s3 = v.ev[5];
     uint8_t* B = v.d_batch;
-    uint8_t *tails = B + o_tail, *wf = B + o_wf, *gv = B + o_gv;
+    uint8_t *tails = B + o_tail, *wf = B + o_wf, *gv = B + o_gv, *seg_ok = B + o_sok;
     const uint8_t* mask = masked ? wf : nullptr;
     const uint32_t* w = (const uint32_t*)(B + o_w);
     uint32_t* ok = (uint32_t*)(B + o_ok);
+    const KeyRec* d_keys = (const KeyRec*)(B + o_meta);
+    const Seg* d_segs = (const Seg*)(B + o_meta + m_segs);
+    const Span* d_spans = (const Span*)(B + o_meta + m_spans);
     if (compressed) decompress_enqueue(v, proofs, count, false, st);
     else CUDA_CHECK(cudaMemcpyAsync(v.d_proofs, proofs, (size_t)count * 256, cudaMemcpyHostToDevice, st));
     CUDA_CHECK(cudaMemcpyAsync(B + o_w, weights, (size_t)count * 16, cudaMemcpyHostToDevice, st));
     if (inputs) CUDA_CHECK(cudaMemcpyAsync(v.d_pub, public_inputs, inputs * 32, cudaMemcpyHostToDevice, st));
+    CUDA_CHECK(cudaMemcpyAsync(B + o_meta, v.h_meta.data(), meta, cudaMemcpyHostToDevice, st));
     CUDA_CHECK(cudaMemsetAsync(ok, 0xff, 8, st));
+    if (keyed) CUDA_CHECK(cudaMemsetAsync(seg_ok, 1, n_segs, st));
     CUDA_CHECK(cudaMemsetAsync(v.d_rec, 0, (size_t)count * REC_BYTES_V, st));
     CUDA_CHECK(cudaEventRecord(ev_up, st));
-    // main stream: per-proof parse and scaling, then the Miller values.  Without a mask the Miller kernel reads the ok word
-    // and skips a batch that has already failed; with one, every proof needs its Miller value, so it reads the word that
-    // stays set.
+    // main stream: per-proof parse and scaling, then the Miller values.  With one verdict for the batch the Miller kernel
+    // reads the ok word and skips a batch that has already failed; with a verdict per segment, every proof needs its Miller
+    // value, so it reads the word that stays set.
     batch_prepare_kernel<<<(count + 127) / 128, 128, 0, st>>>(v.d_proofs, w, count, v.d_rec, ok);
     CUDA_CHECK(cudaEventRecord(ev_prep, st));
-    batch_miller_kernel<<<(count + 63) / 64, 64, 0, st>>>(v.d_rec, masked ? ok + 1 : ok, count, v.d_f);
-    // side stream 2: the group scalars and prepared inputs, e(alpha, beta)^s_g0, and the G2 membership of every B: first when
-    // wf masks the sums, last when only the verdict needs it
+    batch_miller_kernel<<<(count + 63) / 64, 64, 0, st>>>(v.d_rec, masked || keyed ? ok + 1 : ok, count, v.d_f);
+    // side stream 2: the segment scalars and prepared inputs, e(alpha, beta)^s_g0, and the G2 membership of every B: first
+    // when wf masks the sums, last when only the verdicts need it (keyed: then the segment ok bytes)
     auto g2 = [&] {
         batch_g2_kernel<<<(count + 127) / 128, 128, 0, s2>>>(v.d_proofs, count, wf, ok);
         CUDA_CHECK(cudaEventRecord(ev_g2, s2));
     };
     CUDA_CHECK(cudaStreamWaitEvent(s2, ev_up, 0));
     if (masked) g2();
-    batch_scalars_kernel<<<dim3(chunks, n_pts), 128, 0, s2>>>(w, (const uint32_t*)v.d_pub, mask, vk->n_public, count, chunk, B + o_part);
-    batch_inputs_kernel<<<(unsigned)(((size_t)groups * n_pts + 3) / 4), 128, 0, s2>>>(vk->d_tabs, vk->d_g1, B + o_part, per, chunks,
-                                                                                     vk->n_public, groups, B + o_pts, tails);
-    g1_sum_kernel<<<groups, 128, 0, s2>>>(B + o_pts, 128, n_pts, (size_t)groups * n_pts, nullptr, tails + TAIL_PREP, TAIL_BYTES);
+    batch_scalars_kernel<<<items, 128, 0, s2>>>(w, (const uint32_t*)v.d_pub, mask, d_segs, n_segs, d_keys, B + o_part);
+    batch_inputs_kernel<<<(n_pts_all + 3) / 4, 128, 0, s2>>>(B + o_part, d_segs, n_segs, d_keys, n_pts_all, B + o_pts, tails);
+    g1_sum_kernel<<<n_segs, 128, 0, s2>>>(B + o_pts, 128, d_spans + sp_p, nullptr, nullptr, tails + TAIL_PREP);
     CUDA_CHECK(cudaEventRecord(ev_pts, s2));
-    batch_rhs_kernel<<<(groups + 63) / 64, 64, 0, s2>>>(tails, groups, vk->d_eab);
+    batch_rhs_kernel<<<(n_segs + 63) / 64, 64, 0, s2>>>(tails, n_segs, d_segs, d_keys);
     if (!masked) g2();
+    if (keyed) batch_segment_ok_kernel<<<(count + 127) / 128, 128, 0, s2>>>(wf, d_segs, n_segs, count, seg_ok);
     CUDA_CHECK(cudaEventRecord(ev_s2, s2));
-    // side stream 3, once the r C (and wf, with a mask) exist: the group sums of r C, then, once the prepared inputs exist,
-    // the groups' prepared pairs
+    // side stream 3, once the r C (and wf, with a mask) exist: the segment sums of r C, then, once the prepared inputs exist,
+    // the segments' prepared pairs
     CUDA_CHECK(cudaStreamWaitEvent(s3, ev_prep, 0));
     if (masked) CUDA_CHECK(cudaStreamWaitEvent(s3, ev_g2, 0));
-    group_reduce(v.d_rec + BREC_RC, REC_BYTES_V, 128, count, group, 128, mask, B + o_x2, B + o_y2, tails + TAIL_RC,
-                 [&](uint32_t blocks, const uint8_t* src, size_t stride, uint32_t seg, uint32_t n, const uint8_t* m, uint8_t* dst,
-                     size_t dst_stride) { g1_sum_kernel<<<blocks, 128, 0, s3>>>(src, stride, seg, n, m, dst, dst_stride); });
+    reduce_run(levels_g, d_spans + sp_g, v.d_rec + BREC_RC, REC_BYTES_V, 128, mask, B + o_x2, B + o_y2,
+               [&](uint32_t blocks, const uint8_t* src, size_t stride, const Span* sp, const uint8_t* m, uint8_t* dst) {
+                   g1_sum_kernel<<<blocks, 128, 0, s3>>>(src, stride, sp, m, dst, tails + TAIL_RC);
+               });
     CUDA_CHECK(cudaStreamWaitEvent(s3, ev_pts, 0));
-    batch_pairs_kernel<<<(groups + 63) / 64, 64, 0, s3>>>(tails, groups, vk->d_lines, !vk->gamma_inf, !vk->delta_inf);
+    batch_pairs_kernel<<<(n_segs + 63) / 64, 64, 0, s3>>>(tails, n_segs, d_segs, d_keys);
     CUDA_CHECK(cudaEventRecord(ev_s3, s3));
-    // main stream: the group products of the Miller values (f12_product_kernel's CTA always spans 64 records, which is seg
-    // whenever there is more than one CTA), then the group verdicts; the ok word decides a batch verdict only
+    // main stream: the segment products of the Miller values, then the segment verdicts
     if (masked) CUDA_CHECK(cudaStreamWaitEvent(st, ev_g2, 0));
-    group_reduce(v.d_f, F12_BYTES, F12_BYTES, count, group, 64, mask, B + o_x, B + o_y, tails + TAIL_F,
-                 [&](uint32_t blocks, const uint8_t* src, size_t stride, uint32_t, uint32_t n, const uint8_t* m, uint8_t* dst,
-                     size_t dst_stride) { f12_product_kernel<<<blocks, 64, 0, st>>>(src, stride, n, m, dst, dst_stride); });
+    reduce_run(levels_f, d_spans, v.d_f, F12_BYTES, F12_BYTES, mask, B + o_x, B + o_y,
+               [&](uint32_t blocks, const uint8_t* src, size_t stride, const Span* sp, const uint8_t* m, uint8_t* dst) {
+                   f12_product_kernel<<<blocks, 64, 0, st>>>(src, stride, sp, m, dst, tails + TAIL_F);
+               });
     CUDA_CHECK(cudaStreamWaitEvent(st, ev_s2, 0));
     CUDA_CHECK(cudaStreamWaitEvent(st, ev_s3, 0));
-    batch_final_kernel<<<(groups + 63) / 64, 64, 0, st>>>(tails, groups, masked ? nullptr : ok, gv);
-    g_launch_count += 9;
+    batch_final_kernel<<<(n_segs + 63) / 64, 64, 0, st>>>(tails, n_segs, masked || keyed ? nullptr : ok, keyed ? seg_ok : nullptr, gv);
+    g_launch_count += keyed ? 10 : 9;
     CUDA_CHECK(cudaGetLastError());
     return {wf, gv};
 }
 
-// b2g_verify_batch on 256-byte rows, or on compressed rows: the batch check with one group of the whole batch
+// b2g_verify_batch on 256-byte rows, or on compressed rows: the batch check with one segment of the whole batch
 static void verify_batch_run(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs,
                              bool compressed, const void* weights, uint8_t* verdict_out) {
     if (!weights) throw_error(B2G_E_SHAPE, "null pointer");
     const CtxView cv = verify_args(fn, ctx, vk, count, public_inputs, proofs, verdict_out);
     weights_check(weights, count);
     DevGuard g(cv.device);
-    const BatchOut r = batch_enqueue(fn, cv, vk, count, count, false, public_inputs, proofs, compressed, weights);
+    const BatchOut r = batch_enqueue(fn, cv, {vk}, {{0, count}}, false, false, public_inputs, proofs, compressed, weights);
     CUDA_CHECK(cudaMemcpyAsync(verdict_out, r.verdict, 1, cudaMemcpyDeviceToHost, cv.st));
     CUDA_CHECK(cudaStreamSynchronize(cv.st));
 }
 
-// b2g_verify_batch_locate on 256-byte rows, or on compressed rows.  The batch check runs once per group of LOCATE_GROUP
-// proofs; the well-formed proofs of the groups that fail it then go through b2g_verify_many's kernels, compacted on the host
-// from the caller's rows.
+// b2g_verify_batch_locate on 256-byte rows, or on compressed rows.  The batch check runs once per segment of LOCATE_GROUP
+// proofs; the well-formed proofs of the segments that fail it then go through b2g_verify_many's kernels, compacted on the
+// host from the caller's rows.
 static void verify_locate_run(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs,
                               bool compressed, const void* weights, uint8_t* verdicts_out) {
     if (!weights) throw_error(B2G_E_SHAPE, "null pointer");
@@ -1038,7 +1162,9 @@ static void verify_locate_run(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t
     const size_t inputs = (size_t)count * n_public;
     DevGuard g(cv.device);
     cudaStream_t st = cv.st;
-    const BatchOut r = batch_enqueue(fn, cv, vk, count, LOCATE_GROUP, true, public_inputs, proofs, compressed, weights);
+    std::vector<SegIn> segs(groups);
+    for (uint32_t k = 0; k < groups; k++) segs[k] = {0, std::min(LOCATE_GROUP, count - k * LOCATE_GROUP)};
+    const BatchOut r = batch_enqueue(fn, cv, {vk}, segs, true, false, public_inputs, proofs, compressed, weights);
     std::vector<uint8_t> ok_h(count), gv_h(groups);
     CUDA_CHECK(cudaMemcpyAsync(ok_h.data(), r.wf, count, cudaMemcpyDeviceToHost, st));
     CUDA_CHECK(cudaMemcpyAsync(gv_h.data(), r.verdict, groups, cudaMemcpyDeviceToHost, st));
@@ -1067,6 +1193,62 @@ static void verify_locate_run(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t
         for (uint32_t k = 0; k < m; k++) out[idx[k]] = many[k];
     }
     memcpy(verdicts_out, out.data(), count);
+}
+
+// b2g_verify_batch_keys on 256-byte rows, or on compressed rows: the batch check with one segment per key batch that holds
+// proofs; a batch without proofs gets 1.  The batches' proofs, public inputs and weights are packed into one host array each,
+// so that each goes up in one copy.
+static void verify_keys_run(const char* fn, b2g_ctx* ctx, uint32_t n_keys, const b2g_key_batch* batches, bool compressed,
+                            uint8_t* verdicts_out) {
+    if (!ctx || !batches || !verdicts_out) throw_error(B2G_E_SHAPE, "null pointer");
+    if (n_keys == 0) throw_error(B2G_E_SHAPE, std::string(fn) + ": n_keys must be at least 1");
+    auto at = [&](uint32_t k) { return std::string(fn) + ": key " + std::to_string(k) + ": "; };
+    uint64_t total = 0, inputs = 0;
+    for (uint32_t k = 0; k < n_keys; k++) {
+        const b2g_key_batch& b = batches[k];
+        if (!b.vk) throw_error(B2G_E_SHAPE, at(k) + "null verifying key");
+        if (b.count && (!b.proofs || !b.weights || (b.vk->n_public && !b.public_inputs))) throw_error(B2G_E_SHAPE, at(k) + "null pointer");
+        total += b.count;
+        inputs += (uint64_t)b.count * b.vk->n_public;
+    }
+    if (total == 0) throw_error(B2G_E_SHAPE, std::string(fn) + ": every key batch is empty; at least one proof is needed");
+    if (total > UINT32_MAX) throw_error(B2G_E_SHAPE, std::string(fn) + ": more than 2^32 - 1 proofs in all");
+    const CtxView cv = batch_args(fn, ctx, (uint32_t)total);
+    for (uint32_t k = 0; k < n_keys; k++) {
+        const b2g_key_batch& b = batches[k];
+        if (b.vk->device != cv.device) throw_error(B2G_E_SHAPE, at(k) + "the verifying key belongs to another device");
+        const uint32_t n_public = b.vk->n_public;
+        const uint32_t* pub = (const uint32_t*)b.public_inputs;
+        for (size_t i = 0; i < (size_t)b.count * n_public; i++)
+            if (!below_r(pub + 8 * i)) throw_error(B2G_E_INPUT, at(k) + "public input " + std::to_string(i % n_public) + " of proof " +
+                                                                std::to_string(i / n_public) + " is not below the scalar field modulus r");
+        for (uint32_t i = 0; i < b.count; i++)
+            if (all_zero((const uint8_t*)b.weights + 16 * (size_t)i, 16)) throw_error(B2G_E_INPUT, at(k) + "weight " + std::to_string(i) + " is zero");
+    }
+    const size_t row = compressed ? COMP_BYTES : 256;
+    std::vector<uint8_t> rows(total * row), pubs(inputs * 32), ws(total * 16);
+    std::vector<b2g_vk*> vks;
+    std::vector<SegIn> segs;
+    std::vector<uint32_t> seg_of(n_keys, UINT32_MAX);
+    size_t p = 0, x = 0;
+    for (uint32_t k = 0; k < n_keys; k++) {
+        const b2g_key_batch& b = batches[k];
+        if (!b.count) continue;
+        const size_t nx = (size_t)b.count * b.vk->n_public * 32;
+        memcpy(rows.data() + p * row, b.proofs, b.count * row);
+        memcpy(ws.data() + p * 16, b.weights, (size_t)b.count * 16);
+        if (nx) memcpy(pubs.data() + x, b.public_inputs, nx);
+        seg_of[k] = (uint32_t)segs.size();
+        segs.push_back({(uint32_t)vks.size(), b.count});
+        vks.push_back(b.vk);
+        p += b.count; x += nx;
+    }
+    DevGuard g(cv.device);
+    const BatchOut r = batch_enqueue(fn, cv, vks, segs, false, true, pubs.data(), rows.data(), compressed, ws.data());
+    std::vector<uint8_t> gv(segs.size());
+    CUDA_CHECK(cudaMemcpyAsync(gv.data(), r.verdict, segs.size(), cudaMemcpyDeviceToHost, cv.st));
+    CUDA_CHECK(cudaStreamSynchronize(cv.st));
+    for (uint32_t k = 0; k < n_keys; k++) verdicts_out[k] = seg_of[k] == UINT32_MAX ? 1 : gv[seg_of[k]];
 }
 
 int b2g_verify_many(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs, uint8_t* verdicts_out) {
@@ -1100,6 +1282,14 @@ int b2g_verify_batch_locate_compressed(b2g_ctx* ctx, b2g_vk* vk, uint32_t count,
     return guarded([&] {
         verify_locate_run("b2g_verify_batch_locate_compressed", ctx, vk, count, public_inputs, compressed, true, weights, verdicts_out);
     });
+}
+
+int b2g_verify_batch_keys(b2g_ctx* ctx, uint32_t n_keys, const b2g_key_batch* batches, uint8_t* verdicts_out) {
+    return guarded([&] { verify_keys_run("b2g_verify_batch_keys", ctx, n_keys, batches, false, verdicts_out); });
+}
+
+int b2g_verify_batch_keys_compressed(b2g_ctx* ctx, uint32_t n_keys, const b2g_key_batch* batches, uint8_t* verdicts_out) {
+    return guarded([&] { verify_keys_run("b2g_verify_batch_keys_compressed", ctx, n_keys, batches, true, verdicts_out); });
 }
 
 }  // extern "C"

@@ -16,6 +16,8 @@
         <- the same check for a whole batch at once: one random-linear-combination pairing check (b2g_verify_batch).
     Groth16.verify_batch_locate(vk, public_inputs, proofs)
         <- verify_with_processed_vk for every proof, from one batch check per group of 64 proofs (b2g_verify_batch_locate).
+    Groth16.verify_batch_keys([(vk, public_inputs, proofs), ...])
+        <- verify_batch for many keys in one device pass, one verdict per key (b2g_verify_batch_keys).
     Groth16.decompress_proofs(blobs)
         <- Proof::<Bn254>::deserialize_compressed (ark-serialize 0.5, Validate::Yes) for many 128-byte proofs, on the device.
     Groth16.verify_many_compressed / verify_batch_compressed(vk, public_inputs, blobs)
@@ -364,6 +366,60 @@ def _verify_batch(fn, vk, public_inputs, proofs, ctx, weights, compressed, locat
     return [bool(v) for v in out] if locate else bool(out[0])
 
 
+def _verify_batch_keys(fn, batches, ctx, weights, compressed) -> list:
+    """Groth16.verify_batch_keys and verify_batch_keys_compressed: one bool per (vk, public_inputs, proofs) batch"""
+    import secrets
+    from . import verifier
+    batches = [tuple(b) for b in batches]
+    for k, b in enumerate(batches):
+        if len(b) != 3:
+            raise ValueError(f"{fn}: key {k}: a batch is (vk, public_inputs, proofs)")
+    if weights is not None:
+        weights = [None if w is None else [int(x) for x in w] for w in weights]
+        if len(weights) != len(batches):
+            raise ValueError(f"{fn}: one weight list per key batch")
+    ctx = ctx or default_context()
+    verdicts, rows, keep = [True] * len(batches), [], []
+    for k, (vk, public_inputs, proofs) in enumerate(batches):
+        where = f"{fn}: key {k}"
+        proofs = list(proofs)
+        ws = None if weights is None else weights[k]
+        if ws is not None:                     # checked before the key is loaded on the device
+            if len(ws) != len(proofs):
+                raise ValueError(f"{where}: one weight per proof")
+            for w in ws:
+                if not 0 < w < 1 << 128:
+                    raise N.B2gError(N.B2G_E_INPUT, f"{where}: weight {w} is not in [1, 2^128)")
+        try:
+            args = _verify_args(where, vk, public_inputs, proofs, ctx, compressed)
+        except N.B2gError as e:
+            raise N.B2gError(e.code, f"{where}: {e.msg}") from e
+        except verifier.MalformedVerifyingKey as e:
+            raise verifier.MalformedVerifyingKey(f"{where}: {e}") from e
+        if args is None:                       # an empty batch is True
+            continue
+        _, vh, count, pub_arr, data = args
+        if ws is None:
+            ws = []
+            while len(ws) < count:
+                w = secrets.randbits(128)
+                if w:
+                    ws.append(w)
+        wb = np.frombuffer(b''.join(w.to_bytes(16, 'little') for w in ws), dtype=np.uint8).copy()
+        keep += [pub_arr, data, wb]
+        rows.append((k, N.KeyBatch(vh.value, count, 0, _ptr(pub_arr).value if pub_arr is not None else None, _ptr(data).value,
+                                   _ptr(wb).value)))
+    if not rows:
+        return verdicts
+    table = (N.KeyBatch * len(rows))(*[r for _, r in rows])
+    out = np.zeros(len(rows), dtype=np.uint8)
+    entry = N.lib().b2g_verify_batch_keys_compressed if compressed else N.lib().b2g_verify_batch_keys
+    N.check(entry(ctx._h, len(rows), table, _ptr(out)))
+    for (k, _), v in zip(rows, out):
+        verdicts[k] = bool(v)
+    return verdicts
+
+
 def _scalar_bytes(v) -> np.ndarray:
     if isinstance(v, (int, np.integer)):
         return np.frombuffer((int(v) % R_MOD).to_bytes(32, 'little'), dtype='<u8').copy()
@@ -550,6 +606,23 @@ class Groth16:
         (groups holding such a proof) / (2^128 - 1) when the weights are uniform.  Arguments, weights and errors as
         verify_batch; an empty batch gives []."""
         return _verify_batch('verify_batch_locate', vk, public_inputs, proofs, ctx, weights, False, True)
+
+    @staticmethod
+    def verify_batch_keys(batches, ctx: Context = None, weights=None) -> list:
+        """verify_batch for many keys in ONE device pass (b2g_verify_batch_keys): batches = a sequence of (vk, public_inputs,
+        proofs), each as verify_batch takes them (keys are prepared on the device once and cached per object, and one key
+        may appear in several batches).  Returns one bool per batch, equal to verify_batch on that batch with the same
+        weights; an invalid proof changes its own batch's verdict only, and an empty batch is True.  `weights` is None
+        (drawn with secrets.randbits(128)) or one list per batch (None in it: drawn).  Argument checks and errors as
+        verify_batch, with the batch's index in the message."""
+        return _verify_batch_keys('verify_batch_keys', batches, ctx, weights, False)
+
+    @staticmethod
+    def verify_batch_keys_compressed(batches, ctx: Context = None, weights=None) -> list:
+        """verify_batch_keys on compressed proofs (b2g_verify_batch_keys_compressed), decoded on the device: a batch with a
+        blob that does not decode is False, and the other verdicts are those of verify_batch_keys on the decoded proofs.
+        Arguments, weights and errors as verify_batch_keys; a blob that is not 128 bytes raises ValueError."""
+        return _verify_batch_keys('verify_batch_keys_compressed', batches, ctx, weights, True)
 
     # ---- compressed proofs: Proof::<Bn254>::serialize_compressed (ethereum.serialize_compressed), decoded on the device
     @staticmethod

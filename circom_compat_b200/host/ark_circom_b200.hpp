@@ -14,6 +14,7 @@
 //   ark_circom::Groth16::verify_batch         <- the same for a whole batch at once: one random-linear-combination check
 //   ark_circom::Groth16::decompress_proofs    <- Proof::<Bn254>::deserialize_compressed (ark-serialize 0.5) for many proofs
 //   ark_circom::Groth16::verify_many_compressed / verify_batch_compressed <- deserialize_compressed, then the two above
+//   ark_circom::Groth16::verify_batch_keys (+ _compressed) <- verify_batch for many keys in one device pass, a verdict per key
 //   ark_circom::Groth16::verify_batch_locate (+ _compressed) <- verify_with_processed_vk for every proof, at about the batch
 //                                              check's cost when few proofs are invalid
 //   ark_circom::serialize_compressed          <- Proof::<Bn254>::serialize_compressed (ark_circom_ethereum.hpp)
@@ -419,6 +420,49 @@ inline std::vector<uint32_t> batch_weights(size_t n) {
     return w;
 }
 
+// one batch of Groth16::verify_batch_keys: a prepared key with its proofs (P = Proof, or CompressedProof) and their public
+// inputs; the same key may appear in several batches
+template <class P>
+struct KeyBatchOf {
+    const PreparedVerifyingKey& pvk;
+    const std::vector<std::vector<Fr>>& public_inputs;
+    const std::vector<P>& proofs;
+};
+typedef KeyBatchOf<Proof> KeyBatch;
+typedef KeyBatchOf<CompressedProof> CompressedKeyBatch;
+
+// verify_batch_keys and its compressed form: one b2g_verify_batch_keys call over the batches that hold proofs, true for
+// the others
+template <class P>
+inline std::vector<bool> verify_keys_call(const char* fn, const std::vector<KeyBatchOf<P>>& batches, int device) {
+    std::vector<VerifyCall> calls;
+    calls.reserve(batches.size());
+    std::vector<std::vector<uint32_t>> weights;
+    std::vector<b2g_key_batch> table;
+    std::vector<size_t> at;
+    for (size_t k = 0; k < batches.size(); k++) {
+        const std::string where = std::string(fn) + ": key " + std::to_string(k);
+        calls.emplace_back(where.c_str(), batches[k].pvk, batches[k].public_inputs, batches[k].proofs, device);
+        const VerifyCall& c = calls.back();
+        if (c.n == 0) continue;
+        weights.push_back(batch_weights(c.n));
+        b2g_key_batch b; memset(&b, 0, sizeof b);
+        b.vk = c.vk; b.count = (uint32_t)c.n;
+        b.public_inputs = c.pub.empty() ? nullptr : c.pub.data();
+        b.proofs = c.bytes.data(); b.weights = weights.back().data();
+        table.push_back(b);
+        at.push_back(k);
+    }
+    std::vector<bool> out(batches.size(), true);
+    if (table.empty()) return out;
+    std::vector<uint8_t> verdicts(table.size());
+    b2g_ctx* ctx = Gpu::on(device).ctx();
+    check(sizeof(P) == 256 ? b2g_verify_batch_keys(ctx, (uint32_t)table.size(), table.data(), verdicts.data())
+                           : b2g_verify_batch_keys_compressed(ctx, (uint32_t)table.size(), table.data(), verdicts.data()));
+    for (size_t i = 0; i < at.size(); i++) out[at[i]] = verdicts[i] != 0;
+    return out;
+}
+
 template <class QAP = CircomReduction>
 struct Groth16T {                                       // Groth16::<Bn254, QAP>
     // verification (host pairing, ark_circom_verifier.hpp): src/zkey.rs:868-870, 914-916; tests/groth16.rs:33-35
@@ -466,6 +510,17 @@ struct Groth16T {                                       // Groth16::<Bn254, QAP>
         std::vector<uint8_t> verdicts(c.n);
         check(b2g_verify_batch_locate(c.gpu->ctx(), c.vk, (uint32_t)c.n, c.pub.empty() ? nullptr : c.pub.data(), c.bytes.data(), w.data(), verdicts.data()));
         return std::vector<bool>(verdicts.begin(), verdicts.end());
+    }
+    // verify_batch for many keys in ONE device pass (b2g_verify_batch_keys): one verdict per batch, equal to verify_batch on
+    // that batch with the same weights; an invalid proof changes its own batch's verdict only, and an empty batch is true.
+    // Each key is prepared on the device at first use and kept in its pvk.device.  Weights from std::random_device.
+    static std::vector<bool> verify_batch_keys(const std::vector<KeyBatch>& batches, int device = 0) {
+        return verify_keys_call("verify_batch_keys", batches, device);
+    }
+    // verify_batch_keys on compressed proofs, decoded on the device (b2g_verify_batch_keys_compressed): a batch with a proof
+    // that does not decode is false, the others as verify_batch_keys on the decoded proofs
+    static std::vector<bool> verify_batch_keys_compressed(const std::vector<CompressedKeyBatch>& batches, int device = 0) {
+        return verify_keys_call("verify_batch_keys_compressed", batches, device);
     }
     // Proof::<Bn254>::deserialize_compressed (ark-serialize 0.5, Validate::Yes) for many proofs in one device pass
     // (b2g_proofs_decompress): an empty optional where arkworks would refuse the bytes (both flag bits set, a coordinate

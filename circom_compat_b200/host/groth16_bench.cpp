@@ -16,6 +16,9 @@
 //       Groth16::verify_batch_compressed's verdict on the untouched and on the flipped set
 //       B2G_VERIFY_LOCATE=K: also prove K proofs, negate A in proofs 0, K / 2 and K - 1, and compare
 //       Groth16::verify_batch_locate's verdicts with verify_with_processed_vk called per proof (timing the locate call)
+//       B2G_VERIFY_KEYS=K: also prove K proofs, split them into up to four batches of the key plus an empty one, negate A in
+//       the last proof of the second batch, and compare Groth16::verify_batch_keys's verdicts with the host verifier per
+//       batch (timing the keyed call)
 //       chain:<a> = the witness of the reference's squaring-chain bench family for input a
 //       (test-vectors/complex-circuit/input.json has a = 3), computed on the host instead of by WASM.
 #include <algorithm>
@@ -349,6 +352,50 @@ int main(int argc, char** argv) {
             }
             std::printf("verify_locate %d proofs (%d valid, %d tampered): agree=%d, device %.3f ms/batch (%.1f proofs/s)\n", k, valid,
                         (int)at.size(), agree, dev_ms, k / (dev_ms / 1e3));
+        }
+        if (const char* vk_env = std::getenv("B2G_VERIFY_KEYS")) {       // one verdict per key batch, against the host
+            const int k = std::atoi(vk_env);
+            if (k < 1) throw SynthesisError("B2G_VERIFY_KEYS must be >= 1");
+            std::vector<std::vector<Fr>> wv((size_t)k, full_assignment);
+            if (wsrc.rfind("chain:", 0) == 0)
+                for (int i = 1; i < k; i++) wv[(size_t)i] = chain_witness(params.a_query.size(), std::stoull(wsrc.substr(6)) + (unsigned long long)i);
+            std::vector<const std::vector<Fr>*> ws;
+            for (const auto& w : wv) ws.push_back(&w);
+            std::mt19937_64 rng(0x4E75);
+            std::vector<std::pair<Fr, Fr>> rs;
+            for (int i = 0; i < k; i++) rs.push_back({Fr::rand(rng), Fr::rand(rng)});
+            const std::vector<Proof> proofs = Groth16::create_proofs(params, matrices, rs, ws);
+            // the proofs split into up to four batches of the bench key (sizes about k/4, the rest in the last), plus an empty
+            // one; the last proof of the second batch (or of the first, with one batch) gets A -> -A
+            const size_t nb = std::min<size_t>(4, (size_t)k), per = (size_t)k / nb;
+            std::vector<std::vector<std::vector<Fr>>> inputs(nb + 1);
+            std::vector<std::vector<Proof>> parts(nb + 1);
+            for (size_t i = 0; i < (size_t)k; i++) {
+                const size_t b = std::min(i / per, nb - 1);
+                inputs[b].emplace_back(wv[i].begin() + 1, wv[i].begin() + num_inputs);
+                parts[b].push_back(proofs[i]);
+            }
+            Proof& bad = parts[nb > 1 ? 1 : 0].back();
+            uint64_t y[4], d[4]; memcpy(y, bad.bytes + 32, 32);
+            unsigned __int128 borrow = 0;
+            for (int j = 0; j < 4; j++) { unsigned __int128 t = (unsigned __int128)detail::FQ_P[j] - y[j] - borrow; d[j] = (uint64_t)t; borrow = (t >> 64) & 1; }
+            memcpy(bad.bytes + 32, d, 32);
+            auto pvk = Groth16::process_vk(params.vk);
+            std::vector<KeyBatch> batches;
+            for (size_t b = 0; b <= nb; b++) batches.push_back({pvk, inputs[b], parts[b]});
+            std::vector<bool> got = Groth16::verify_batch_keys(batches);        // also loads the key on the device
+            auto t1 = std::chrono::steady_clock::now();
+            got = Groth16::verify_batch_keys(batches);
+            const double dev_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t1).count();
+            std::string dev, host;
+            for (size_t b = 0; b <= nb; b++) {
+                bool h = true;
+                for (size_t i = 0; i < parts[b].size(); i++) h = h && Groth16::verify_with_processed_vk(pvk, inputs[b][i], parts[b][i]);
+                dev += got[b] ? '1' : '0';
+                host += h ? '1' : '0';
+            }
+            std::printf("verify_keys %d proofs in %d batches: device=%s host=%s agree=%d, device %.3f ms/call (%.1f proofs/s)\n", k,
+                        (int)nb + 1, dev.c_str(), host.c_str(), dev == host, dev_ms, k / (dev_ms / 1e3));
         }
         return 0;
     } catch (const std::exception& e) {

@@ -22,7 +22,8 @@
  *   b2g_verify_many_compressed / b2g_verify_batch_compressed <- deserialize_compressed followed by the two calls above
  *   b2g_verify_batch_locate (+ _compressed) <- GrothBn::verify_with_processed_vk for every proof of a batch, at about the
  *                             batch check's cost when few proofs are invalid
- *   b2g_fixed_base_g1/g2   <- the batch fixed-base multiplications of generate_random_parameters_with_reduction
+ *   b2g_verify_batch_keys (+ _compressed) <- b2g_verify_batch for many keys, one verdict per key, in one device pass
+ *   b2g_fixed_base_g1/g2  <- the batch fixed-base multiplications of generate_random_parameters_with_reduction
  *                             (tests/groth16.rs:25); used to manufacture synthetic proving keys
  *
  * Conventions
@@ -304,6 +305,33 @@ B2G_API int b2g_verify_batch_locate(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, co
  * well-formed.  The verdicts equal those of b2g_proofs_decompress followed by b2g_verify_batch_locate on the decoded rows. */
 B2G_API int b2g_verify_batch_locate_compressed(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs,
                                                const void* compressed, const void* weights, uint8_t* verdicts_out);
+
+/* One batch of proofs under one verifying key, for b2g_verify_batch_keys. */
+typedef struct {
+    b2g_vk* vk;
+    uint32_t count;              /* proofs under this key (0 allowed) */
+    uint32_t reserved;
+    const void* public_inputs;   /* count x vk's n_public canonical 32 B scalars (NULL when n_public == 0 or count == 0) */
+    const void* proofs;          /* count x 256 B (b2g_prove layout), or count x 128 B for the _compressed form */
+    const void* weights;         /* count x 16 B nonzero 128-bit weights */
+} b2g_key_batch;
+
+/* b2g_verify_batch_keys: b2g_verify_batch for n_keys batches, each under its own key, in one device pass, for callers that
+ * see many circuits with a few to a few hundred proofs each (rollup and bridge nodes, aggregators).  verdicts_out = n_keys
+ * bytes.  verdicts_out[k] equals, bit for bit, *verdict_out of b2g_verify_batch(batches[k].vk, batches[k].count, the same
+ * public inputs, proofs and weights): 1 iff every proof of batch k is well-formed (coordinates below p, points on their
+ * curves, B at infinity or in G2) and batch k's equation of b2g_verify_batch holds.  A batch with count == 0 gets 1.  The
+ * batches are independent: an invalid proof of batch k changes verdicts_out[k] only.  Each verdict keeps b2g_verify_batch's
+ * soundness statement, with weights drawn after the proofs are fixed.  The same key may appear in several batches.
+ * Cost: b2g_verify_batch's per-proof work over all proofs, plus per batch one two-pair Miller loop, e(alpha, beta)^s_0, one
+ * final exponentiation and the public-input products; one device pass whatever the number of keys.
+ * Synchronous.  Errors as b2g_verify_batch, with the key index in the message: B2G_E_SHAPE for n_keys == 0, a total count of
+ * 0, null pointers, a key of another device or a pending proof; B2G_E_INPUT for a public input >= r or a zero weight;
+ * B2G_E_DEVICE when the buffers do not fit.  Every error leaves the context usable. */
+B2G_API int b2g_verify_batch_keys(b2g_ctx* ctx, uint32_t n_keys, const b2g_key_batch* batches, uint8_t* verdicts_out);
+/* b2g_verify_batch_keys_compressed: b2g_verify_batch_keys on compressed proofs (128 B each), decoded on the device.  A proof
+ * that does not decode is malformed: verdicts_out[k] equals b2g_proofs_decompress followed by b2g_verify_batch_keys. */
+B2G_API int b2g_verify_batch_keys_compressed(b2g_ctx* ctx, uint32_t n_keys, const b2g_key_batch* batches, uint8_t* verdicts_out);
 
 /* Kernel-level entry points (parity tests, benchmarks). All pointers host. */
 B2G_API int b2g_msm_g1(b2g_ctx* ctx, const void* bases, const void* scalars, size_t n, int scalars_mont, void* out_xy_mont);
