@@ -42,7 +42,7 @@ class VkDesc(C.Structure):
 
 
 class KeyBatch(C.Structure):
-    """b2g_key_batch: one batch of proofs under one verifying key (b2g_verify_batch_keys)"""
+    """b2g_key_batch: one batch of proofs under one verifying key (b2g_verify_batch_keys, b2g_verify_batch_keys_locate)"""
     _fields_ = [('vk', C.c_void_p), ('count', C.c_uint32), ('reserved', C.c_uint32)] + \
                [(k, C.c_void_p) for k in ('public_inputs', 'proofs', 'weights')]
 
@@ -53,7 +53,7 @@ EXPORTS = ['b2g_last_error', 'b2g_version', 'b2g_device_count', 'b2g_ctx_create'
            'b2g_bench_device', 'b2g_bench_msm', 'b2g_launch_count', 'b2g_vk_load', 'b2g_vk_free', 'b2g_vk_alpha_beta', 'b2g_verify_many',
            'b2g_verify_batch', 'b2g_proofs_decompress', 'b2g_verify_many_compressed', 'b2g_verify_batch_compressed',
            'b2g_verify_batch_locate', 'b2g_verify_batch_locate_compressed', 'b2g_verify_batch_keys',
-           'b2g_verify_batch_keys_compressed']
+           'b2g_verify_batch_keys_compressed', 'b2g_verify_batch_keys_locate', 'b2g_verify_batch_keys_locate_compressed']
 
 _lib = None
 
@@ -113,6 +113,8 @@ def lib():
         L.b2g_verify_batch_locate_compressed.argtypes = [vp, vp, C.c_uint32, vp, vp, vp, vp]
         L.b2g_verify_batch_keys.argtypes = [vp, C.c_uint32, C.POINTER(KeyBatch), vp]
         L.b2g_verify_batch_keys_compressed.argtypes = [vp, C.c_uint32, C.POINTER(KeyBatch), vp]
+        L.b2g_verify_batch_keys_locate.argtypes = [vp, C.c_uint32, C.POINTER(KeyBatch), vp]
+        L.b2g_verify_batch_keys_locate_compressed.argtypes = [vp, C.c_uint32, C.POINTER(KeyBatch), vp]
         _lib = L
     return _lib
 

@@ -17,7 +17,9 @@
 //     s_0 = sum r_i, s_j = sum r_i x_ij (mod r), x_ij the j-th public input of proof i (j = 1..n_public), sums over the segment
 // b2g_verify_batch runs it with one segment of the whole batch; b2g_verify_batch_locate with segments of LOCATE_GROUP proofs
 // whose sums leave out the malformed proofs (a mask), then b2g_verify_many on the well-formed proofs of the segments that
-// fail; b2g_verify_batch_keys with one segment per key.  A segment table and a table of key records drive every stage below.
+// fail; b2g_verify_batch_keys with one segment per key; b2g_verify_batch_keys_locate with segments of LOCATE_GROUP proofs of
+// one key, then one b2g_verify_many pass whose kernels check each proof under its own key.  A segment table and a table of
+// key records drive every stage below.
 //   prepare  one proof per thread: the parse and on-curve checks above, r_i A_i (affine) and r_i C_i (XYZZ)
 //   g2       one proof per thread: the proof parses and its B lies in G2 (the mask)
 //   scalars  one CTA per (chunk of at most SCALAR_CHUNK proofs of a segment, j): partial sums of r_i x_ij (x_i0 = 1)
@@ -69,14 +71,15 @@ namespace b2g {
 constexpr size_t REC_BYTES_V = 384, REC_OK = 320;
 
 struct VerifyBufs {
-    size_t cap_count = 0, cap_pub = 0, cap_part = 0, cap_batch = 0, cap_comp = 0;
+    size_t cap_count = 0, cap_pub = 0, cap_part = 0, cap_batch = 0, cap_comp = 0, cap_meta = 0;
     uint8_t *d_proofs = nullptr, *d_rec = nullptr, *d_f = nullptr, *d_verdict = nullptr;   // per proof
     uint8_t *d_pub = nullptr, *d_part = nullptr;                                            // per (proof, input)
     uint8_t* d_batch = nullptr;                   // the batch check's scratch: weights, reduction levels, group tails, ...
     uint8_t* d_comp = nullptr;                    // compressed proofs (128 B each), then one decoded-ok byte per proof
+    uint8_t* d_meta = nullptr;                    // b2g_verify_many's key records and segment table
     cudaStream_t side[2] = {nullptr, nullptr};    // the batch check's tail pieces, next to the per-proof kernels
     cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-    std::vector<uint8_t> h_meta;                  // the batch check's key records, segment table and reduction spans (host)
+    std::vector<uint8_t> h_meta;                  // the key records, segment table and reduction spans of the last call (host)
 };
 
 void verify_bufs_free(VerifyBufs* v) {
@@ -84,19 +87,54 @@ void verify_bufs_free(VerifyBufs* v) {
     for (cudaStream_t s : v->side) if (s) cudaStreamDestroy(s);
     for (cudaEvent_t e : v->ev) if (e) cudaEventDestroy(e);
     for (void* p : {(void*)v->d_proofs, (void*)v->d_rec, (void*)v->d_f, (void*)v->d_verdict, (void*)v->d_pub, (void*)v->d_part,
-                    (void*)v->d_batch, (void*)v->d_comp}) if (p) cudaFree(p);
+                    (void*)v->d_batch, (void*)v->d_comp, (void*)v->d_meta}) if (p) cudaFree(p);
     delete v;
 }
 
+// ------------------------------------------------------------------------------------------------ key and segment tables
+// the key a segment is checked under: its prepared lines of -gamma and -delta, e(alpha, beta), the window tables of
+// IC[1..n_public], alpha and IC (b2g_vk's arrays), and whether each prepared pair takes part (gamma, delta not at infinity)
+struct KeyRec {
+    const uint8_t *lines, *eab, *tabs, *g1;
+    uint32_t n_public, gamma_on, delta_on, pad;
+};
+// a segment: proofs first .. first + count - 1 under key record `key`; its public inputs start at scalar `pub`.  In the batch
+// check, its (chunk, j) work items of batch_scalars_kernel start at `part` (chunks of them, chunk-major: chunk q's item j is
+// part + q * (n_public + 1) + j) and its prepared-input points at `pt`; b2g_verify_many's kernels leave those three at 0.
+// first, pub, part and pt never decrease along the table.
+struct Seg {
+    uint64_t pub;
+    uint32_t key, first, count, part, chunks, pt;
+};
+
+// the last segment k < n with s[k].*M <= v, for a field that is nondecreasing along the table (first, part, pt, or the 64-bit
+// pub)
+template <auto M, class T>
+__device__ __forceinline__ uint32_t seg_find(const Seg* __restrict__ s, uint32_t n, T v) {
+    uint32_t lo = 0, hi = n;
+    while (hi - lo > 1) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (s[mid].*M <= v) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+
 // ------------------------------------------------------------------------------------------------ kernels
-// x * IC[i + 1] for one (proof, input) per warp: w = proof * n_public + i; pub = canonical scalars, part = G1 XYZZ records
-__global__ void __launch_bounds__(128) verify_inputs_kernel(const uint8_t* __restrict__ tabs, const uint32_t* __restrict__ pub,
-                                                            uint32_t n_public, size_t total, uint8_t* __restrict__ part) {
+// b2g_verify_many's kernels check each proof under its own key: proof j belongs to the segment whose first .. first + count -
+// 1 holds it, and its public inputs (and their G1 records in part) start at seg.pub + (j - seg.first) * n_public.  A call
+// under one key is a table of one segment.
+// x * IC[i + 1] for one (proof, input) per warp: w indexes the public-input scalars of every proof back to back, input i of
+// proof j of the segment whose inputs hold w; pub = canonical scalars, part = G1 XYZZ records (both w-indexed)
+__global__ void __launch_bounds__(128) verify_inputs_kernel(const KeyRec* __restrict__ keys, const Seg* __restrict__ segs, uint32_t n_segs,
+                                                            const uint32_t* __restrict__ pub, size_t total, uint8_t* __restrict__ part) {
     __shared__ G1::Pt sh[4][32];
     const size_t w = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (w >= total) return;                                // whole warps leave together
-    const uint32_t i = (uint32_t)(w % n_public);
-    G1::Pt p = warp_fixed_mul<G1, Fq>(tabs + (size_t)i * TABLE_BYTES, pub + 8 * w, sh[threadIdx.x >> 5]);
+    // a segment without inputs shares its pub with the next one, so the last segment with pub <= w is the one that holds w
+    const Seg s = segs[seg_find<&Seg::pub>(segs, n_segs, (uint64_t)w)];
+    const KeyRec& key = keys[s.key];
+    const uint32_t i = (uint32_t)((w - s.pub) % key.n_public);
+    G1::Pt p = warp_fixed_mul<G1, Fq>(key.tabs + (size_t)i * TABLE_BYTES, pub + 8 * w, sh[threadIdx.x >> 5]);
     if ((threadIdx.x & 31) == 0) pt_store<Fq>(part, w, p);
 }
 
@@ -116,15 +154,19 @@ __device__ __forceinline__ bool proof_parse(const uint8_t* pr, G1::Aff& a, G2::A
     return ok && aff_on_curve<G1, Fq>(a) && aff_on_curve<G1, Fq>(cc) && aff_on_curve<G2, Fq2>(b);
 }
 
-__global__ void __launch_bounds__(128) verify_prepare_kernel(const uint8_t* __restrict__ proofs, const uint8_t* __restrict__ g1,
-                                                             const uint8_t* __restrict__ part, uint32_t n_public, uint32_t count,
-                                                             uint8_t* __restrict__ rec) {
+__global__ void __launch_bounds__(128) verify_prepare_kernel(const uint8_t* __restrict__ proofs, const KeyRec* __restrict__ keys,
+                                                             const Seg* __restrict__ segs, uint32_t n_segs, const uint8_t* __restrict__ part,
+                                                             uint32_t count, uint8_t* __restrict__ rec) {
     const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= count) return;
     G1::Aff a, cc; G2::Aff b;
     const bool ok = proof_parse(proofs + (size_t)j * 256, a, b, cc);
-    G1::Pt acc = G1::from_affine(aff_load<Fq>(g1, 1));   // IC[0]
-    for (uint32_t i = 0; i < n_public; i++) G1::add(acc, pt_load<Fq>(part, (size_t)j * n_public + i));
+    const Seg s = segs[seg_find<&Seg::first>(segs, n_segs, j)];
+    const KeyRec& key = keys[s.key];
+    const uint32_t n_public = key.n_public;
+    const size_t p0 = s.pub + (size_t)(j - s.first) * n_public;
+    G1::Pt acc = G1::from_affine(aff_load<Fq>(key.g1, 1));   // IC[0]
+    for (uint32_t i = 0; i < n_public; i++) G1::add(acc, pt_load<Fq>(part, p0 + i));
     uint8_t* r = rec + (size_t)j * REC_BYTES_V;
     aff_store<Fq>(r, 0, a);
     aff_store<Fq2>(r + 64, 0, b);
@@ -133,32 +175,36 @@ __global__ void __launch_bounds__(128) verify_prepare_kernel(const uint8_t* __re
     *reinterpret_cast<uint32_t*>(r + REC_OK) = ok;
 }
 
-__global__ void __launch_bounds__(64) verify_miller_kernel(const uint8_t* __restrict__ rec, const uint8_t* __restrict__ lines,
-                                                           bool gamma_on, bool delta_on, uint32_t count, uint8_t* __restrict__ fout) {
+__global__ void __launch_bounds__(64) verify_miller_kernel(const uint8_t* __restrict__ rec, const KeyRec* __restrict__ keys,
+                                                           const Seg* __restrict__ segs, uint32_t n_segs, uint32_t count,
+                                                           uint8_t* __restrict__ fout) {
     const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= count) return;
     const uint8_t* r = rec + (size_t)j * REC_BYTES_V;
     if (!*reinterpret_cast<const uint32_t*>(r + REC_OK)) return;
+    const KeyRec& key = keys[segs[seg_find<&Seg::first>(segs, n_segs, j)].key];
+    const uint8_t* lines = key.lines;
     const G1::Aff a = aff_load<Fq>(r, 0), c = aff_load<Fq>(r + 192, 0), prep = aff_load<Fq>(r + 256, 0);
     const G2::Aff b = aff_load<Fq2>(r + 64, 0);
     G1::Aff fp[2];
     const uint8_t* fl[2];
     int nfix = 0;
-    if (gamma_on && !G1::aff_is_inf(prep)) { fp[nfix] = prep; fl[nfix++] = lines; }
-    if (delta_on && !G1::aff_is_inf(c)) { fp[nfix] = c; fl[nfix++] = lines + ATE_LINES * LINE_BYTES; }
+    if (key.gamma_on && !G1::aff_is_inf(prep)) { fp[nfix] = prep; fl[nfix++] = lines; }
+    if (key.delta_on && !G1::aff_is_inf(c)) { fp[nfix] = c; fl[nfix++] = lines + ATE_LINES * LINE_BYTES; }
     fe12 f;
     miller_loop(f, !G1::aff_is_inf(a) && !G2::aff_is_inf(b), a, b, nfix, fp, fl);
     Fq12::store(fout + (size_t)j * F12_BYTES, f);
 }
 
 __global__ void __launch_bounds__(64) verify_final_kernel(const uint8_t* __restrict__ rec, const uint8_t* __restrict__ fin,
-                                                          const uint8_t* __restrict__ eab, uint32_t count, uint8_t* __restrict__ verdict) {
+                                                          const KeyRec* __restrict__ keys, const Seg* __restrict__ segs, uint32_t n_segs,
+                                                          uint32_t count, uint8_t* __restrict__ verdict) {
     const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= count) return;
     if (!*reinterpret_cast<const uint32_t*>(rec + (size_t)j * REC_BYTES_V + REC_OK)) { verdict[j] = 0; return; }
     fe12 e;
     Fq12::final_exponentiation(e, Fq12::load(fin + (size_t)j * F12_BYTES));
-    verdict[j] = Fq12::eq(e, Fq12::load(eab));
+    verdict[j] = Fq12::eq(e, Fq12::load(keys[segs[seg_find<&Seg::first>(segs, n_segs, j)].key].eab));
 }
 
 // ---------------------------------------------------------------------------------------------- batch check kernels
@@ -176,34 +222,10 @@ static_assert(TAIL_BYTES % 256 == 0, "segment tails stay 256-byte aligned");
 constexpr uint32_t LOCATE_GROUP = 64;              // proofs per segment of b2g_verify_batch_locate: one CTA of f12_product_kernel
 constexpr uint32_t SCALAR_CHUNK = 2048;            // at most this many proofs per CTA of batch_scalars_kernel
 
-// the key a segment is checked under: its prepared lines of -gamma and -delta, e(alpha, beta), the window tables of
-// IC[1..n_public], alpha and IC (b2g_vk's arrays), and whether each prepared pair takes part (gamma, delta not at infinity)
-struct KeyRec {
-    const uint8_t *lines, *eab, *tabs, *g1;
-    uint32_t n_public, gamma_on, delta_on, pad;
-};
-// a segment: proofs first .. first + count - 1 under key record `key`; its public inputs start at scalar `pub`, its
-// (chunk, j) work items of batch_scalars_kernel at `part` (chunks of them, chunk-major: chunk q's item j is part + q *
-// (n_public + 1) + j), its prepared-input points at `pt`.  first, part and pt increase along the table.
-struct Seg {
-    uint64_t pub;
-    uint32_t key, first, count, part, chunks, pt;
-};
 // one CTA of a segmented reduction: records first .. first + n - 1 of one segment, to value `out` of the next level, or to
 // the tail of segment out & ~TO_TAIL when TO_TAIL is set
 struct Span { uint32_t first, n, out; };
 constexpr uint32_t TO_TAIL = 0x80000000u;
-
-// the last segment k < n with s[k].*M <= v, for a field that is nondecreasing along the table
-template <uint32_t Seg::*M>
-__device__ __forceinline__ uint32_t seg_find(const Seg* __restrict__ s, uint32_t n, uint32_t v) {
-    uint32_t lo = 0, hi = n;
-    while (hi - lo > 1) {
-        const uint32_t mid = (lo + hi) >> 1;
-        if (s[mid].*M <= v) lo = mid; else hi = mid;
-    }
-    return lo;
-}
 
 __device__ __forceinline__ uint8_t* span_out(const Span& s, uint8_t* dst, size_t rec_bytes, uint8_t* tails) {
     return s.out & TO_TAIL ? tails + (size_t)(s.out & ~TO_TAIL) * TAIL_BYTES : dst + (size_t)s.out * rec_bytes;
@@ -672,24 +694,24 @@ static void verify_stage_test_op(cudaStream_t st, int op, const void* a, const v
         }
         d.s = dev_upload<uint8_t>(stage.data(), stage.size(), st);
         CUDA_CHECK(cudaMalloc(&d.o, n * so));
-        // op 53: per row, a key record with the row's lines and a one-segment table, as batch_enqueue builds them
-        if (op == 53) {
-            std::vector<uint8_t> meta(n * sizeof(KeyRec) + sizeof(Seg));
-            KeyRec* keys = reinterpret_cast<KeyRec*>(meta.data());
-            for (size_t i = 0; i < n; i++)
-                keys[i] = {d.s + i * STAGE_BYTES + STAGE_LINES, nullptr, nullptr, nullptr, 0, on[2 * i], on[2 * i + 1], 0};
-            const Seg seg = {0, 0, 0, 1, 0, 1, 0};
-            memcpy(meta.data() + n * sizeof(KeyRec), &seg, sizeof(Seg));
-            d.a = dev_upload<uint8_t>(meta.data(), meta.size(), st);
-            CUDA_CHECK(cudaStreamSynchronize(st));         // meta is pageable and leaves scope here
-        }
+        // per row, a key record with the row's lines and a one-segment table, as verify_many_enqueue and batch_enqueue build
+        // them
+        std::vector<uint8_t> meta(n * sizeof(KeyRec) + sizeof(Seg));
+        KeyRec* keys = reinterpret_cast<KeyRec*>(meta.data());
+        for (size_t i = 0; i < n; i++)
+            keys[i] = {d.s + i * STAGE_BYTES + STAGE_LINES, nullptr, nullptr, nullptr, 0, on[2 * i], on[2 * i + 1], 0};
+        const Seg seg = {0, 0, 0, 1, 0, 1, 0};
+        memcpy(meta.data() + n * sizeof(KeyRec), &seg, sizeof(Seg));
+        d.a = dev_upload<uint8_t>(meta.data(), meta.size(), st);
+        CUDA_CHECK(cudaStreamSynchronize(st));             // meta is pageable and leaves scope here
+        const Seg* d_seg = (const Seg*)(d.a + n * sizeof(KeyRec));
         for (size_t i = 0; i < n; i++) {
             uint8_t* g = d.s + i * STAGE_BYTES;
             vk_lines_kernel<<<1, 32, 0, st>>>(g + STAGE_G2, g + STAGE_LINES);
             if (op == 49) {
-                verify_miller_kernel<<<1, 64, 0, st>>>(g + STAGE_REC, g + STAGE_LINES, on[2 * i], on[2 * i + 1], 1, d.o + i * F12_BYTES);
+                verify_miller_kernel<<<1, 64, 0, st>>>(g + STAGE_REC, (const KeyRec*)d.a + i, d_seg, 1, 1, d.o + i * F12_BYTES);
             } else {
-                batch_pairs_kernel<<<1, 1, 0, st>>>(g + STAGE_REC, 1, (const Seg*)(d.a + n * sizeof(KeyRec)), (const KeyRec*)d.a + i);
+                batch_pairs_kernel<<<1, 1, 0, st>>>(g + STAGE_REC, 1, d_seg, (const KeyRec*)d.a + i);
                 CUDA_CHECK(cudaMemcpyAsync(d.o + i * F12_BYTES, g + STAGE_REC + TAIL_G, F12_BYTES, cudaMemcpyDeviceToDevice, st));
             }
         }
@@ -706,10 +728,20 @@ static void verify_stage_test_op(cudaStream_t st, int op, const void* a, const v
     } else if (op == 51) {
         d.a = dev_upload<uint8_t>(a, n * sa, st);
         CUDA_CHECK(cudaMalloc(&d.o, n * so));
-        CUDA_CHECK(cudaMalloc(&d.s, 256 + TABLE_BYTES));                // the point, then its table
-        CUDA_CHECK(cudaMemcpyAsync(d.s, b, 64, cudaMemcpyHostToDevice, st));
+        // the point, a one-input key record and a one-segment table over the n rows, then the point's table
+        CUDA_CHECK(cudaMalloc(&d.s, 256 + TABLE_BYTES));
+        static_assert(128 + sizeof(KeyRec) + sizeof(Seg) <= 256, "the op 51 tables fit between the point and its table");
+        uint8_t meta[256] = {};
+        memcpy(meta, b, 64);
+        const KeyRec key = {nullptr, nullptr, d.s + 256, nullptr, 1, 0, 0, 0};
+        const Seg seg = {0, 0, 0, (uint32_t)n, 0, 0, 0};
+        memcpy(meta + 128, &key, sizeof(KeyRec));
+        memcpy(meta + 128 + sizeof(KeyRec), &seg, sizeof(Seg));
+        CUDA_CHECK(cudaMemcpyAsync(d.s, meta, 256, cudaMemcpyHostToDevice, st));
+        CUDA_CHECK(cudaStreamSynchronize(st));             // meta is pageable and leaves scope here
         fixed_table_kernel<G1, Fq><<<(32 * 255 + 63) / 64, 64, 0, st>>>(d.s + 256, d.s);
-        verify_inputs_kernel<<<(unsigned)((n + 3) / 4), 128, 0, st>>>(d.s + 256, (const uint32_t*)d.a, 1, n, d.o);
+        verify_inputs_kernel<<<(unsigned)((n + 3) / 4), 128, 0, st>>>((const KeyRec*)(d.s + 128), (const Seg*)(d.s + 128 + sizeof(KeyRec)), 1,
+                                                                      (const uint32_t*)d.a, n, d.o);
         g_launch_count += 2;
     } else {
         d.a = dev_upload<uint8_t>(a, n * sa, st);
@@ -781,9 +813,9 @@ static void vbuf_grow(uint8_t*& p, size_t& cap, size_t bytes) {
 }
 
 // grows the context's verification buffers to `count` proofs, `inputs` public-input scalars, `parts` (proof, input) G1
-// records, `batch` bytes of b2g_verify_batch scratch and `comp` bytes of compressed-proof staging; never shrinks them, and a
-// failed allocation leaves them consistent
-static void vbufs_ensure(VerifyBufs*& v, size_t count, size_t inputs, size_t parts, size_t batch = 0, size_t comp = 0) {
+// records, `batch` bytes of b2g_verify_batch scratch, `comp` bytes of compressed-proof staging and `meta` bytes of
+// b2g_verify_many tables; never shrinks them, and a failed allocation leaves them consistent
+static void vbufs_ensure(VerifyBufs*& v, size_t count, size_t inputs, size_t parts, size_t batch = 0, size_t comp = 0, size_t meta = 0) {
     if (!v) v = new VerifyBufs();
     if (count > v->cap_count) {
         for (uint8_t** p : {&v->d_proofs, &v->d_rec, &v->d_f, &v->d_verdict}) { if (*p) cudaFree(*p); *p = nullptr; }
@@ -798,6 +830,7 @@ static void vbufs_ensure(VerifyBufs*& v, size_t count, size_t inputs, size_t par
     vbuf_grow(v->d_part, v->cap_part, parts * 128);
     vbuf_grow(v->d_batch, v->cap_batch, batch);
     vbuf_grow(v->d_comp, v->cap_comp, comp);
+    vbuf_grow(v->d_meta, v->cap_meta, meta);
 }
 
 // the staging bytes of count compressed proofs: the rows, then one ok byte per proof
@@ -947,9 +980,9 @@ static CtxView verify_args(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t co
 
 // vbufs_ensure, reporting a batch that does not fit as B2G_E_DEVICE with advice
 static void verify_bufs_ensure(const char* fn, VerifyBufs*& v, uint32_t count, size_t inputs, size_t parts, size_t batch = 0,
-                               size_t comp = 0) {
+                               size_t comp = 0, size_t meta = 0) {
     try {
-        vbufs_ensure(v, count, inputs, parts, batch, comp);
+        vbufs_ensure(v, count, inputs, parts, batch, comp, meta);
     } catch (const B2gError& e) {
         if (e.code != B2G_E_DEVICE) throw;
         cudaGetLastError();
@@ -974,34 +1007,58 @@ int b2g_proofs_decompress(b2g_ctx* ctx, uint32_t count, const void* compressed, 
     });
 }
 
-// b2g_verify_many's uploads and four kernels on st, on 256-byte rows or on compressed rows decoded first (G2 check
-// included); the verdicts go to v.d_verdict
-static void verify_many_enqueue(VerifyBufs& v, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs,
-                                bool compressed, cudaStream_t st) {
-    const size_t inputs = (size_t)count * vk->n_public;
+// the key record of a loaded key
+static KeyRec key_rec(const b2g_vk* vk) {
+    return {vk->d_lines, vk->d_eab, vk->d_tabs, vk->d_g1, vk->n_public, !vk->gamma_inf, !vk->delta_inf, 0};
+}
+
+// the device bytes of b2g_verify_many's tables for n_keys keys: the key records, then one segment per key
+static size_t many_meta_bytes(size_t n_keys) { return n_keys * (sizeof(KeyRec) + sizeof(Seg)); }
+
+// b2g_verify_many's uploads and four kernels on st, every proof under its own key: segment k holds the next counts[k]
+// proofs, checked under vks[k] (counts[k] >= 1), and the public inputs of all proofs lie back to back.  On 256-byte rows, or
+// on compressed rows decoded first (G2 check included); the verdicts go to v.d_verdict.  v.d_meta holds at least
+// many_meta_bytes(vks.size()) bytes.
+static void verify_many_enqueue(VerifyBufs& v, const std::vector<b2g_vk*>& vks, const std::vector<uint32_t>& counts,
+                                const void* public_inputs, const void* proofs, bool compressed, cudaStream_t st) {
+    const uint32_t n_segs = (uint32_t)vks.size();
+    // the tables go up from a host buffer that outlives the call, as in batch_enqueue
+    v.h_meta.assign(many_meta_bytes(n_segs), 0);
+    KeyRec* keys = reinterpret_cast<KeyRec*>(v.h_meta.data());
+    Seg* segs = reinterpret_cast<Seg*>(v.h_meta.data() + n_segs * sizeof(KeyRec));
+    uint32_t count = 0;
+    size_t inputs = 0;
+    for (uint32_t k = 0; k < n_segs; k++) {
+        keys[k] = key_rec(vks[k]);
+        segs[k] = {inputs, k, count, counts[k], 0, 0, 0};
+        count += counts[k]; inputs += (size_t)counts[k] * vks[k]->n_public;
+    }
+    const KeyRec* d_keys = reinterpret_cast<const KeyRec*>(v.d_meta);
+    const Seg* d_segs = reinterpret_cast<const Seg*>(v.d_meta + n_segs * sizeof(KeyRec));
+    CUDA_CHECK(cudaMemcpyAsync(v.d_meta, v.h_meta.data(), v.h_meta.size(), cudaMemcpyHostToDevice, st));
     if (compressed) decompress_enqueue(v, proofs, count, true, st);
     else CUDA_CHECK(cudaMemcpyAsync(v.d_proofs, proofs, (size_t)count * 256, cudaMemcpyHostToDevice, st));
     if (inputs) {
         CUDA_CHECK(cudaMemcpyAsync(v.d_pub, public_inputs, inputs * 32, cudaMemcpyHostToDevice, st));
-        verify_inputs_kernel<<<(unsigned)((inputs + 3) / 4), 128, 0, st>>>(vk->d_tabs, (const uint32_t*)v.d_pub, vk->n_public, inputs, v.d_part);
+        verify_inputs_kernel<<<(unsigned)((inputs + 3) / 4), 128, 0, st>>>(d_keys, d_segs, n_segs, (const uint32_t*)v.d_pub, inputs, v.d_part);
     }
-    verify_prepare_kernel<<<(count + 127) / 128, 128, 0, st>>>(v.d_proofs, vk->d_g1, v.d_part, vk->n_public, count, v.d_rec);
-    verify_miller_kernel<<<(count + 63) / 64, 64, 0, st>>>(v.d_rec, vk->d_lines, !vk->gamma_inf, !vk->delta_inf, count, v.d_f);
-    verify_final_kernel<<<(count + 63) / 64, 64, 0, st>>>(v.d_rec, v.d_f, vk->d_eab, count, v.d_verdict);
+    verify_prepare_kernel<<<(count + 127) / 128, 128, 0, st>>>(v.d_proofs, d_keys, d_segs, n_segs, v.d_part, count, v.d_rec);
+    verify_miller_kernel<<<(count + 63) / 64, 64, 0, st>>>(v.d_rec, d_keys, d_segs, n_segs, count, v.d_f);
+    verify_final_kernel<<<(count + 63) / 64, 64, 0, st>>>(v.d_rec, v.d_f, d_keys, d_segs, n_segs, count, v.d_verdict);
     g_launch_count += 3 + (inputs ? 1 : 0);
     CUDA_CHECK(cudaGetLastError());
 }
 
-// b2g_verify_many on 256-byte rows, or on compressed rows decoded on the device (G2 check included)
+// b2g_verify_many on 256-byte rows, or on compressed rows decoded on the device (G2 check included): a table of one key
 static void verify_many_run(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs,
                             bool compressed, uint8_t* verdicts_out) {
     const CtxView cv = verify_args(fn, ctx, vk, count, public_inputs, proofs, verdicts_out);
     const size_t inputs = (size_t)count * vk->n_public;
     DevGuard g(cv.device);
     cudaStream_t st = cv.st;
-    verify_bufs_ensure(fn, *cv.vbufs, count, inputs, inputs, 0, compressed ? comp_bytes(count) : 0);
+    verify_bufs_ensure(fn, *cv.vbufs, count, inputs, inputs, 0, compressed ? comp_bytes(count) : 0, many_meta_bytes(1));
     VerifyBufs& v = **cv.vbufs;
-    verify_many_enqueue(v, vk, count, public_inputs, proofs, compressed, st);
+    verify_many_enqueue(v, {vk}, {count}, public_inputs, proofs, compressed, st);
     CUDA_CHECK(cudaMemcpyAsync(verdicts_out, v.d_verdict, count, cudaMemcpyDeviceToHost, st));
     CUDA_CHECK(cudaStreamSynchronize(st));
 }
@@ -1027,10 +1084,7 @@ static BatchOut batch_enqueue(const char* fn, const CtxView& cv, const std::vect
     // the per-call tables: key records, segments, then the spans of the Miller-value products, of the r C sums and of the
     // prepared-input sums (one CTA per segment)
     std::vector<KeyRec> keys(vks.size());
-    for (size_t k = 0; k < vks.size(); k++) {
-        const b2g_vk* vk = vks[k];
-        keys[k] = {vk->d_lines, vk->d_eab, vk->d_tabs, vk->d_g1, vk->n_public, !vk->gamma_inf, !vk->delta_inf, 0};
-    }
+    for (size_t k = 0; k < vks.size(); k++) keys[k] = key_rec(vks[k]);
     const uint32_t n_segs = (uint32_t)segs_in.size();
     std::vector<Seg> segs(n_segs);
     uint32_t count = 0, items = 0, n_pts_all = 0;
@@ -1150,66 +1204,39 @@ static void verify_batch_run(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t 
     CUDA_CHECK(cudaStreamSynchronize(cv.st));
 }
 
-// b2g_verify_batch_locate on 256-byte rows, or on compressed rows.  The batch check runs once per segment of LOCATE_GROUP
-// proofs; the well-formed proofs of the segments that fail it then go through b2g_verify_many's kernels, compacted on the
-// host from the caller's rows.
-static void verify_locate_run(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs,
-                              bool compressed, const void* weights, uint8_t* verdicts_out) {
-    if (!weights) throw_error(B2G_E_SHAPE, "null pointer");
-    const CtxView cv = verify_args(fn, ctx, vk, count, public_inputs, proofs, verdicts_out);
-    weights_check(weights, count);
-    const uint32_t n_public = vk->n_public, groups = (count + LOCATE_GROUP - 1) / LOCATE_GROUP;
-    const size_t inputs = (size_t)count * n_public;
-    DevGuard g(cv.device);
-    cudaStream_t st = cv.st;
-    std::vector<SegIn> segs(groups);
-    for (uint32_t k = 0; k < groups; k++) segs[k] = {0, std::min(LOCATE_GROUP, count - k * LOCATE_GROUP)};
-    const BatchOut r = batch_enqueue(fn, cv, {vk}, segs, true, false, public_inputs, proofs, compressed, weights);
-    std::vector<uint8_t> ok_h(count), gv_h(groups);
-    CUDA_CHECK(cudaMemcpyAsync(ok_h.data(), r.wf, count, cudaMemcpyDeviceToHost, st));
-    CUDA_CHECK(cudaMemcpyAsync(gv_h.data(), r.verdict, groups, cudaMemcpyDeviceToHost, st));
-    CUDA_CHECK(cudaStreamSynchronize(st));
-    // the verdicts: 0 for a malformed proof, 1 in a group that holds, else b2g_verify_many's verdict
-    std::vector<uint8_t> out(count);
-    std::vector<uint32_t> idx;
-    for (uint32_t i = 0; i < count; i++) {
-        out[i] = ok_h[i] && gv_h[i / LOCATE_GROUP];
-        if (ok_h[i] && !gv_h[i / LOCATE_GROUP]) idx.push_back(i);
-    }
-    if (!idx.empty()) {
-        // when every proof is checked again, the caller's rows are already the compact ones
-        const uint32_t m = (uint32_t)idx.size();
-        const bool whole = m == count;
-        const size_t row = compressed ? COMP_BYTES : 256, pub_row = (size_t)n_public * 32;
-        std::vector<uint8_t> rows(whole ? 0 : (size_t)m * row), pubs(whole ? 0 : (size_t)m * pub_row), many(m);
-        for (uint32_t k = 0; k < m && !whole; k++) {
-            memcpy(rows.data() + k * row, (const uint8_t*)proofs + idx[k] * row, row);
-            if (pub_row) memcpy(pubs.data() + k * pub_row, (const uint8_t*)public_inputs + idx[k] * pub_row, pub_row);
-        }
-        verify_bufs_ensure(fn, *cv.vbufs, count, inputs, (size_t)m * n_public, 0, compressed ? comp_bytes(count) : 0);
-        verify_many_enqueue(**cv.vbufs, vk, m, whole ? public_inputs : pubs.data(), whole ? proofs : rows.data(), compressed, st);
-        CUDA_CHECK(cudaMemcpyAsync(many.data(), (*cv.vbufs)->d_verdict, m, cudaMemcpyDeviceToHost, st));
-        CUDA_CHECK(cudaStreamSynchronize(st));
-        for (uint32_t k = 0; k < m; k++) out[idx[k]] = many[k];
-    }
-    memcpy(verdicts_out, out.data(), count);
+// key batches as one run of proofs: one entry per batch that holds proofs (vks, counts, and its index among the caller's
+// batches in `at`), and their proofs, public inputs and weights back to back.  With one such batch these are the caller's
+// arrays; with more they are packed into one host array each, so that each goes up in one copy.
+struct KeysPacked {
+    std::vector<b2g_vk*> vks;
+    std::vector<uint32_t> counts, at;
+    uint32_t total = 0;
+    size_t inputs = 0;
+    const void *proofs = nullptr, *public_inputs = nullptr, *weights = nullptr;
+    std::vector<uint8_t> rows_h, pubs_h, ws_h;
+};
+
+// one key's proofs as a KeysPacked of one entry (b2g_verify_batch_locate)
+static KeysPacked keys_one(b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs, const void* weights) {
+    KeysPacked p;
+    p.vks = {vk}; p.counts = {count}; p.at = {0};
+    p.total = count; p.inputs = (size_t)count * vk->n_public;
+    p.proofs = proofs; p.public_inputs = public_inputs; p.weights = weights;
+    return p;
 }
 
-// b2g_verify_batch_keys on 256-byte rows, or on compressed rows: the batch check with one segment per key batch that holds
-// proofs; a batch without proofs gets 1.  The batches' proofs, public inputs and weights are packed into one host array each,
-// so that each goes up in one copy.
-static void verify_keys_run(const char* fn, b2g_ctx* ctx, uint32_t n_keys, const b2g_key_batch* batches, bool compressed,
-                            uint8_t* verdicts_out) {
+// the argument checks of b2g_verify_batch_keys and b2g_verify_batch_keys_locate (and their compressed forms), each message
+// naming the key index; returns the context
+static CtxView keys_args(const char* fn, b2g_ctx* ctx, uint32_t n_keys, const b2g_key_batch* batches, const uint8_t* verdicts_out) {
     if (!ctx || !batches || !verdicts_out) throw_error(B2G_E_SHAPE, "null pointer");
     if (n_keys == 0) throw_error(B2G_E_SHAPE, std::string(fn) + ": n_keys must be at least 1");
     auto at = [&](uint32_t k) { return std::string(fn) + ": key " + std::to_string(k) + ": "; };
-    uint64_t total = 0, inputs = 0;
+    uint64_t total = 0;
     for (uint32_t k = 0; k < n_keys; k++) {
         const b2g_key_batch& b = batches[k];
         if (!b.vk) throw_error(B2G_E_SHAPE, at(k) + "null verifying key");
         if (b.count && (!b.proofs || !b.weights || (b.vk->n_public && !b.public_inputs))) throw_error(B2G_E_SHAPE, at(k) + "null pointer");
         total += b.count;
-        inputs += (uint64_t)b.count * b.vk->n_public;
     }
     if (total == 0) throw_error(B2G_E_SHAPE, std::string(fn) + ": every key batch is empty; at least one proof is needed");
     if (total > UINT32_MAX) throw_error(B2G_E_SHAPE, std::string(fn) + ": more than 2^32 - 1 proofs in all");
@@ -1225,30 +1252,132 @@ static void verify_keys_run(const char* fn, b2g_ctx* ctx, uint32_t n_keys, const
         for (uint32_t i = 0; i < b.count; i++)
             if (all_zero((const uint8_t*)b.weights + 16 * (size_t)i, 16)) throw_error(B2G_E_INPUT, at(k) + "weight " + std::to_string(i) + " is zero");
     }
+    return cv;
+}
+
+// the key batches (checked by keys_args) as one run of proofs
+static KeysPacked keys_pack(uint32_t n_keys, const b2g_key_batch* batches, bool compressed) {
+    uint32_t used = 0, last = 0;
+    for (uint32_t k = 0; k < n_keys; k++) if (batches[k].count) { used++; last = k; }
+    if (used == 1) {
+        const b2g_key_batch& b = batches[last];
+        KeysPacked p = keys_one(b.vk, b.count, b.public_inputs, b.proofs, b.weights);
+        p.at = {last};
+        return p;
+    }
+    KeysPacked p;
+    for (uint32_t k = 0; k < n_keys; k++) {
+        p.total += batches[k].count;
+        p.inputs += (size_t)batches[k].count * batches[k].vk->n_public;
+    }
     const size_t row = compressed ? COMP_BYTES : 256;
-    std::vector<uint8_t> rows(total * row), pubs(inputs * 32), ws(total * 16);
-    std::vector<b2g_vk*> vks;
-    std::vector<SegIn> segs;
-    std::vector<uint32_t> seg_of(n_keys, UINT32_MAX);
-    size_t p = 0, x = 0;
+    p.rows_h.resize((size_t)p.total * row); p.pubs_h.resize(p.inputs * 32); p.ws_h.resize((size_t)p.total * 16);
+    size_t n = 0, x = 0;
     for (uint32_t k = 0; k < n_keys; k++) {
         const b2g_key_batch& b = batches[k];
         if (!b.count) continue;
         const size_t nx = (size_t)b.count * b.vk->n_public * 32;
-        memcpy(rows.data() + p * row, b.proofs, b.count * row);
-        memcpy(ws.data() + p * 16, b.weights, (size_t)b.count * 16);
-        if (nx) memcpy(pubs.data() + x, b.public_inputs, nx);
-        seg_of[k] = (uint32_t)segs.size();
-        segs.push_back({(uint32_t)vks.size(), b.count});
-        vks.push_back(b.vk);
-        p += b.count; x += nx;
+        memcpy(p.rows_h.data() + n * row, b.proofs, b.count * row);
+        memcpy(p.ws_h.data() + n * 16, b.weights, (size_t)b.count * 16);
+        if (nx) memcpy(p.pubs_h.data() + x, b.public_inputs, nx);
+        p.vks.push_back(b.vk); p.counts.push_back(b.count); p.at.push_back(k);
+        n += b.count; x += nx;
     }
+    p.proofs = p.rows_h.data(); p.public_inputs = p.pubs_h.data(); p.weights = p.ws_h.data();
+    return p;
+}
+
+// the per-proof verdicts of b2g_verify_batch_locate and b2g_verify_batch_keys_locate, p.total bytes in p's order.  The batch
+// check runs once per segment of at most LOCATE_GROUP consecutive proofs of one key (a key's segments start at its first
+// proof), masked by wf; the well-formed proofs of the segments that fail it then go through b2g_verify_many's kernels in one
+// pass, each under its own key, compacted on the host from p's rows.
+static void locate_run(const char* fn, const CtxView& cv, const KeysPacked& p, bool compressed, uint8_t* verdicts_out) {
+    cudaStream_t st = cv.st;
+    std::vector<SegIn> segs;
+    for (uint32_t k = 0; k < (uint32_t)p.vks.size(); k++)
+        for (uint32_t f = 0; f < p.counts[k]; f += LOCATE_GROUP) segs.push_back({k, std::min(LOCATE_GROUP, p.counts[k] - f)});
+    const BatchOut r = batch_enqueue(fn, cv, p.vks, segs, true, false, p.public_inputs, p.proofs, compressed, p.weights);
+    std::vector<uint8_t> ok_h(p.total), gv_h(segs.size());
+    CUDA_CHECK(cudaMemcpyAsync(ok_h.data(), r.wf, p.total, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaMemcpyAsync(gv_h.data(), r.verdict, segs.size(), cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    // the verdicts: 0 for a malformed proof, 1 in a segment that holds, else b2g_verify_many's verdict.  The proofs checked
+    // again (idx, with their first public-input scalar in xs) keep the keys' order: one b2g_verify_many segment per key
+    // among them (vks2, counts2).
+    std::vector<uint8_t> out(p.total);
+    std::vector<uint32_t> idx, counts2;
+    std::vector<size_t> xs;
+    std::vector<b2g_vk*> vks2;
+    uint32_t i = 0, prev = UINT32_MAX;
+    size_t x = 0, inputs2 = 0;
+    for (uint32_t g = 0; g < (uint32_t)segs.size(); g++) {
+        const uint32_t key = segs[g].key, n_public = p.vks[key]->n_public;
+        for (uint32_t t = 0; t < segs[g].count; t++, i++, x += n_public) {
+            out[i] = ok_h[i] && gv_h[g];
+            if (!ok_h[i] || gv_h[g]) continue;
+            if (key != prev) { vks2.push_back(p.vks[key]); counts2.push_back(0); prev = key; }
+            counts2.back()++;
+            idx.push_back(i); xs.push_back(x); inputs2 += n_public;
+        }
+    }
+    if (!idx.empty()) {
+        // when every proof is checked again, p's rows are already the compact ones
+        const uint32_t m = (uint32_t)idx.size();
+        const bool whole = m == p.total;
+        const size_t row = compressed ? COMP_BYTES : 256;
+        std::vector<uint8_t> rows(whole ? 0 : (size_t)m * row), pubs(whole ? 0 : inputs2 * 32), many(m);
+        size_t y = 0;
+        for (uint32_t k = 0, s = 0, in_s = 0; k < m && !whole; k++) {            // proof k is the in_s-th of segment s
+            memcpy(rows.data() + (size_t)k * row, (const uint8_t*)p.proofs + (size_t)idx[k] * row, row);
+            const size_t pub_row = (size_t)vks2[s]->n_public * 32;
+            if (pub_row) memcpy(pubs.data() + y, (const uint8_t*)p.public_inputs + xs[k] * 32, pub_row);
+            y += pub_row;
+            if (++in_s == counts2[s]) { s++; in_s = 0; }
+        }
+        verify_bufs_ensure(fn, *cv.vbufs, p.total, p.inputs, inputs2, 0, compressed ? comp_bytes(p.total) : 0, many_meta_bytes(vks2.size()));
+        verify_many_enqueue(**cv.vbufs, vks2, counts2, whole ? p.public_inputs : pubs.data(), whole ? p.proofs : rows.data(), compressed, st);
+        CUDA_CHECK(cudaMemcpyAsync(many.data(), (*cv.vbufs)->d_verdict, m, cudaMemcpyDeviceToHost, st));
+        CUDA_CHECK(cudaStreamSynchronize(st));
+        for (uint32_t k = 0; k < m; k++) out[idx[k]] = many[k];
+    }
+    memcpy(verdicts_out, out.data(), p.total);
+}
+
+// b2g_verify_batch_locate on 256-byte rows, or on compressed rows: the locate pipeline with one key
+static void verify_locate_run(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs,
+                              bool compressed, const void* weights, uint8_t* verdicts_out) {
+    if (!weights) throw_error(B2G_E_SHAPE, "null pointer");
+    const CtxView cv = verify_args(fn, ctx, vk, count, public_inputs, proofs, verdicts_out);
+    weights_check(weights, count);
     DevGuard g(cv.device);
-    const BatchOut r = batch_enqueue(fn, cv, vks, segs, false, true, pubs.data(), rows.data(), compressed, ws.data());
+    locate_run(fn, cv, keys_one(vk, count, public_inputs, proofs, weights), compressed, verdicts_out);
+}
+
+// b2g_verify_batch_keys_locate on 256-byte rows, or on compressed rows: the locate pipeline over every key batch, whose
+// verdicts lie back to back in batch order (an empty batch has none)
+static void verify_keys_locate_run(const char* fn, b2g_ctx* ctx, uint32_t n_keys, const b2g_key_batch* batches, bool compressed,
+                                   uint8_t* verdicts_out) {
+    const CtxView cv = keys_args(fn, ctx, n_keys, batches, verdicts_out);
+    const KeysPacked p = keys_pack(n_keys, batches, compressed);
+    DevGuard g(cv.device);
+    locate_run(fn, cv, p, compressed, verdicts_out);
+}
+
+// b2g_verify_batch_keys on 256-byte rows, or on compressed rows: the batch check with one segment per key batch that holds
+// proofs; a batch without proofs gets 1
+static void verify_keys_run(const char* fn, b2g_ctx* ctx, uint32_t n_keys, const b2g_key_batch* batches, bool compressed,
+                            uint8_t* verdicts_out) {
+    const CtxView cv = keys_args(fn, ctx, n_keys, batches, verdicts_out);
+    const KeysPacked p = keys_pack(n_keys, batches, compressed);
+    std::vector<SegIn> segs;
+    for (uint32_t k = 0; k < (uint32_t)p.vks.size(); k++) segs.push_back({k, p.counts[k]});
+    DevGuard g(cv.device);
+    const BatchOut r = batch_enqueue(fn, cv, p.vks, segs, false, true, p.public_inputs, p.proofs, compressed, p.weights);
     std::vector<uint8_t> gv(segs.size());
     CUDA_CHECK(cudaMemcpyAsync(gv.data(), r.verdict, segs.size(), cudaMemcpyDeviceToHost, cv.st));
     CUDA_CHECK(cudaStreamSynchronize(cv.st));
-    for (uint32_t k = 0; k < n_keys; k++) verdicts_out[k] = seg_of[k] == UINT32_MAX ? 1 : gv[seg_of[k]];
+    std::fill(verdicts_out, verdicts_out + n_keys, 1);
+    for (size_t k = 0; k < segs.size(); k++) verdicts_out[p.at[k]] = gv[k];
 }
 
 int b2g_verify_many(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs, uint8_t* verdicts_out) {
@@ -1290,6 +1419,16 @@ int b2g_verify_batch_keys(b2g_ctx* ctx, uint32_t n_keys, const b2g_key_batch* ba
 
 int b2g_verify_batch_keys_compressed(b2g_ctx* ctx, uint32_t n_keys, const b2g_key_batch* batches, uint8_t* verdicts_out) {
     return guarded([&] { verify_keys_run("b2g_verify_batch_keys_compressed", ctx, n_keys, batches, true, verdicts_out); });
+}
+
+int b2g_verify_batch_keys_locate(b2g_ctx* ctx, uint32_t n_keys, const b2g_key_batch* batches, uint8_t* verdicts_out) {
+    return guarded([&] { verify_keys_locate_run("b2g_verify_batch_keys_locate", ctx, n_keys, batches, false, verdicts_out); });
+}
+
+int b2g_verify_batch_keys_locate_compressed(b2g_ctx* ctx, uint32_t n_keys, const b2g_key_batch* batches, uint8_t* verdicts_out) {
+    return guarded([&] {
+        verify_keys_locate_run("b2g_verify_batch_keys_locate_compressed", ctx, n_keys, batches, true, verdicts_out);
+    });
 }
 
 }  // extern "C"

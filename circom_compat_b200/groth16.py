@@ -18,6 +18,8 @@
         <- verify_with_processed_vk for every proof, from one batch check per group of 64 proofs (b2g_verify_batch_locate).
     Groth16.verify_batch_keys([(vk, public_inputs, proofs), ...])
         <- verify_batch for many keys in one device pass, one verdict per key (b2g_verify_batch_keys).
+    Groth16.verify_batch_keys_locate([(vk, public_inputs, proofs), ...])
+        <- verify_batch_locate for many keys in one device pass, one verdict per proof (b2g_verify_batch_keys_locate).
     Groth16.decompress_proofs(blobs)
         <- Proof::<Bn254>::deserialize_compressed (ark-serialize 0.5, Validate::Yes) for many 128-byte proofs, on the device.
     Groth16.verify_many_compressed / verify_batch_compressed(vk, public_inputs, blobs)
@@ -366,8 +368,9 @@ def _verify_batch(fn, vk, public_inputs, proofs, ctx, weights, compressed, locat
     return [bool(v) for v in out] if locate else bool(out[0])
 
 
-def _verify_batch_keys(fn, batches, ctx, weights, compressed) -> list:
-    """Groth16.verify_batch_keys and verify_batch_keys_compressed: one bool per (vk, public_inputs, proofs) batch"""
+def _key_batches(fn, batches, ctx, weights, compressed):
+    """the argument checks and encoding of the keyed verifiers: (ctx, number of batches, [(batch index, KeyBatch)] for the
+    batches that hold proofs, the arrays the KeyBatch rows point into)"""
     import secrets
     from . import verifier
     batches = [tuple(b) for b in batches]
@@ -379,7 +382,7 @@ def _verify_batch_keys(fn, batches, ctx, weights, compressed) -> list:
         if len(weights) != len(batches):
             raise ValueError(f"{fn}: one weight list per key batch")
     ctx = ctx or default_context()
-    verdicts, rows, keep = [True] * len(batches), [], []
+    rows, keep = [], []
     for k, (vk, public_inputs, proofs) in enumerate(batches):
         where = f"{fn}: key {k}"
         proofs = list(proofs)
@@ -396,7 +399,7 @@ def _verify_batch_keys(fn, batches, ctx, weights, compressed) -> list:
             raise N.B2gError(e.code, f"{where}: {e.msg}") from e
         except verifier.MalformedVerifyingKey as e:
             raise verifier.MalformedVerifyingKey(f"{where}: {e}") from e
-        if args is None:                       # an empty batch is True
+        if args is None:                       # an empty batch is not passed on
             continue
         _, vh, count, pub_arr, data = args
         if ws is None:
@@ -409,6 +412,13 @@ def _verify_batch_keys(fn, batches, ctx, weights, compressed) -> list:
         keep += [pub_arr, data, wb]
         rows.append((k, N.KeyBatch(vh.value, count, 0, _ptr(pub_arr).value if pub_arr is not None else None, _ptr(data).value,
                                    _ptr(wb).value)))
+    return ctx, len(batches), rows, keep
+
+
+def _verify_batch_keys(fn, batches, ctx, weights, compressed) -> list:
+    """Groth16.verify_batch_keys and verify_batch_keys_compressed: one bool per (vk, public_inputs, proofs) batch"""
+    ctx, n, rows, keep = _key_batches(fn, batches, ctx, weights, compressed)
+    verdicts = [True] * n                      # an empty batch is True
     if not rows:
         return verdicts
     table = (N.KeyBatch * len(rows))(*[r for _, r in rows])
@@ -417,6 +427,24 @@ def _verify_batch_keys(fn, batches, ctx, weights, compressed) -> list:
     N.check(entry(ctx._h, len(rows), table, _ptr(out)))
     for (k, _), v in zip(rows, out):
         verdicts[k] = bool(v)
+    return verdicts
+
+
+def _verify_batch_keys_locate(fn, batches, ctx, weights, compressed) -> list:
+    """Groth16.verify_batch_keys_locate and verify_batch_keys_locate_compressed: one list of bools per (vk, public_inputs,
+    proofs) batch"""
+    ctx, n, rows, keep = _key_batches(fn, batches, ctx, weights, compressed)
+    verdicts = [[] for _ in range(n)]          # an empty batch has no verdicts
+    if not rows:
+        return verdicts
+    table = (N.KeyBatch * len(rows))(*[r for _, r in rows])
+    out = np.zeros(sum(r.count for _, r in rows), dtype=np.uint8)
+    entry = N.lib().b2g_verify_batch_keys_locate_compressed if compressed else N.lib().b2g_verify_batch_keys_locate
+    N.check(entry(ctx._h, len(rows), table, _ptr(out)))
+    at = 0
+    for k, r in rows:
+        verdicts[k] = [bool(v) for v in out[at:at + r.count]]
+        at += r.count
     return verdicts
 
 
@@ -623,6 +651,21 @@ class Groth16:
         blob that does not decode is False, and the other verdicts are those of verify_batch_keys on the decoded proofs.
         Arguments, weights and errors as verify_batch_keys; a blob that is not 128 bytes raises ValueError."""
         return _verify_batch_keys('verify_batch_keys_compressed', batches, ctx, weights, True)
+
+    @staticmethod
+    def verify_batch_keys_locate(batches, ctx: Context = None, weights=None) -> list:
+        """verify_batch_locate for many keys in ONE device pass (b2g_verify_batch_keys_locate): batches as verify_batch_keys
+        takes them.  Returns one list of bools per batch, equal to verify_batch_locate on that batch with the same weights
+        (groups of 64 start at each batch's first proof); an empty batch gives [].  Weights, argument checks and errors as
+        verify_batch_keys."""
+        return _verify_batch_keys_locate('verify_batch_keys_locate', batches, ctx, weights, False)
+
+    @staticmethod
+    def verify_batch_keys_locate_compressed(batches, ctx: Context = None, weights=None) -> list:
+        """verify_batch_keys_locate on compressed proofs (b2g_verify_batch_keys_locate_compressed), decoded on the device: a
+        blob that does not decode is False, and each batch's verdicts equal verify_batch_locate_compressed on that batch.
+        Arguments, weights and errors as verify_batch_keys_locate; a blob that is not 128 bytes raises ValueError."""
+        return _verify_batch_keys_locate('verify_batch_keys_locate_compressed', batches, ctx, weights, True)
 
     # ---- compressed proofs: Proof::<Bn254>::serialize_compressed (ethereum.serialize_compressed), decoded on the device
     @staticmethod

@@ -15,6 +15,8 @@
 //   ark_circom::Groth16::decompress_proofs    <- Proof::<Bn254>::deserialize_compressed (ark-serialize 0.5) for many proofs
 //   ark_circom::Groth16::verify_many_compressed / verify_batch_compressed <- deserialize_compressed, then the two above
 //   ark_circom::Groth16::verify_batch_keys (+ _compressed) <- verify_batch for many keys in one device pass, a verdict per key
+//   ark_circom::Groth16::verify_batch_keys_locate (+ _compressed) <- verify_batch_locate for many keys in one device pass, a
+//                             verdict per proof
 //   ark_circom::Groth16::verify_batch_locate (+ _compressed) <- verify_with_processed_vk for every proof, at about the batch
 //                                              check's cost when few proofs are invalid
 //   ark_circom::serialize_compressed          <- Proof::<Bn254>::serialize_compressed (ark_circom_ethereum.hpp)
@@ -431,35 +433,65 @@ struct KeyBatchOf {
 typedef KeyBatchOf<Proof> KeyBatch;
 typedef KeyBatchOf<CompressedProof> CompressedKeyBatch;
 
+// the b2g_key_batch rows of the keyed verifiers for the batches that hold proofs (row i is batch at[i]), with the arrays
+// they point into; weights from std::random_device
+struct KeysTable {
+    std::vector<VerifyCall> calls;
+    std::vector<std::vector<uint32_t>> weights;
+    std::vector<b2g_key_batch> table;
+    std::vector<size_t> at;
+    size_t total = 0;
+    template <class P>
+    KeysTable(const char* fn, const std::vector<KeyBatchOf<P>>& batches, int device) {
+        calls.reserve(batches.size());
+        for (size_t k = 0; k < batches.size(); k++) {
+            const std::string where = std::string(fn) + ": key " + std::to_string(k);
+            calls.emplace_back(where.c_str(), batches[k].pvk, batches[k].public_inputs, batches[k].proofs, device);
+            const VerifyCall& c = calls.back();
+            if (c.n == 0) continue;
+            weights.push_back(batch_weights(c.n));
+            b2g_key_batch b; memset(&b, 0, sizeof b);
+            b.vk = c.vk; b.count = (uint32_t)c.n;
+            b.public_inputs = c.pub.empty() ? nullptr : c.pub.data();
+            b.proofs = c.bytes.data(); b.weights = weights.back().data();
+            table.push_back(b);
+            at.push_back(k);
+            total += c.n;
+        }
+    }
+};
+
 // verify_batch_keys and its compressed form: one b2g_verify_batch_keys call over the batches that hold proofs, true for
 // the others
 template <class P>
 inline std::vector<bool> verify_keys_call(const char* fn, const std::vector<KeyBatchOf<P>>& batches, int device) {
-    std::vector<VerifyCall> calls;
-    calls.reserve(batches.size());
-    std::vector<std::vector<uint32_t>> weights;
-    std::vector<b2g_key_batch> table;
-    std::vector<size_t> at;
-    for (size_t k = 0; k < batches.size(); k++) {
-        const std::string where = std::string(fn) + ": key " + std::to_string(k);
-        calls.emplace_back(where.c_str(), batches[k].pvk, batches[k].public_inputs, batches[k].proofs, device);
-        const VerifyCall& c = calls.back();
-        if (c.n == 0) continue;
-        weights.push_back(batch_weights(c.n));
-        b2g_key_batch b; memset(&b, 0, sizeof b);
-        b.vk = c.vk; b.count = (uint32_t)c.n;
-        b.public_inputs = c.pub.empty() ? nullptr : c.pub.data();
-        b.proofs = c.bytes.data(); b.weights = weights.back().data();
-        table.push_back(b);
-        at.push_back(k);
-    }
+    const KeysTable t(fn, batches, device);
     std::vector<bool> out(batches.size(), true);
-    if (table.empty()) return out;
-    std::vector<uint8_t> verdicts(table.size());
+    if (t.table.empty()) return out;
+    std::vector<uint8_t> verdicts(t.table.size());
     b2g_ctx* ctx = Gpu::on(device).ctx();
-    check(sizeof(P) == 256 ? b2g_verify_batch_keys(ctx, (uint32_t)table.size(), table.data(), verdicts.data())
-                           : b2g_verify_batch_keys_compressed(ctx, (uint32_t)table.size(), table.data(), verdicts.data()));
-    for (size_t i = 0; i < at.size(); i++) out[at[i]] = verdicts[i] != 0;
+    check(sizeof(P) == 256 ? b2g_verify_batch_keys(ctx, (uint32_t)t.table.size(), t.table.data(), verdicts.data())
+                           : b2g_verify_batch_keys_compressed(ctx, (uint32_t)t.table.size(), t.table.data(), verdicts.data()));
+    for (size_t i = 0; i < t.at.size(); i++) out[t.at[i]] = verdicts[i] != 0;
+    return out;
+}
+
+// verify_batch_keys_locate and its compressed form: one b2g_verify_batch_keys_locate call over the batches that hold proofs,
+// one verdict list per batch (empty for an empty batch)
+template <class P>
+inline std::vector<std::vector<bool>> verify_keys_locate_call(const char* fn, const std::vector<KeyBatchOf<P>>& batches, int device) {
+    const KeysTable t(fn, batches, device);
+    std::vector<std::vector<bool>> out(batches.size());
+    if (t.table.empty()) return out;
+    std::vector<uint8_t> verdicts(t.total);
+    b2g_ctx* ctx = Gpu::on(device).ctx();
+    check(sizeof(P) == 256 ? b2g_verify_batch_keys_locate(ctx, (uint32_t)t.table.size(), t.table.data(), verdicts.data())
+                           : b2g_verify_batch_keys_locate_compressed(ctx, (uint32_t)t.table.size(), t.table.data(), verdicts.data()));
+    size_t v = 0;
+    for (size_t i = 0; i < t.at.size(); i++) {
+        out[t.at[i]].assign(verdicts.begin() + v, verdicts.begin() + v + t.table[i].count);
+        v += t.table[i].count;
+    }
     return out;
 }
 
@@ -521,6 +553,17 @@ struct Groth16T {                                       // Groth16::<Bn254, QAP>
     // that does not decode is false, the others as verify_batch_keys on the decoded proofs
     static std::vector<bool> verify_batch_keys_compressed(const std::vector<CompressedKeyBatch>& batches, int device = 0) {
         return verify_keys_call("verify_batch_keys_compressed", batches, device);
+    }
+    // verify_batch_locate for many keys in ONE device pass (b2g_verify_batch_keys_locate): one verdict list per batch, equal
+    // to verify_batch_locate on that batch with the same weights (groups of 64 start at each batch's first proof); an empty
+    // batch gives an empty list.  Weights from std::random_device.
+    static std::vector<std::vector<bool>> verify_batch_keys_locate(const std::vector<KeyBatch>& batches, int device = 0) {
+        return verify_keys_locate_call("verify_batch_keys_locate", batches, device);
+    }
+    // verify_batch_keys_locate on compressed proofs, decoded on the device (b2g_verify_batch_keys_locate_compressed): a proof
+    // that does not decode is false, the others as verify_batch_keys_locate on the decoded proofs
+    static std::vector<std::vector<bool>> verify_batch_keys_locate_compressed(const std::vector<CompressedKeyBatch>& batches, int device = 0) {
+        return verify_keys_locate_call("verify_batch_keys_locate_compressed", batches, device);
     }
     // Proof::<Bn254>::deserialize_compressed (ark-serialize 0.5, Validate::Yes) for many proofs in one device pass
     // (b2g_proofs_decompress): an empty optional where arkworks would refuse the bytes (both flag bits set, a coordinate

@@ -19,6 +19,10 @@
 //       B2G_VERIFY_KEYS=K: also prove K proofs, split them into up to four batches of the key plus an empty one, negate A in
 //       the last proof of the second batch, and compare Groth16::verify_batch_keys's verdicts with the host verifier per
 //       batch (timing the keyed call)
+//       B2G_VERIFY_KEYS_LOCATE=K: also prove K proofs, split them into up to four batches of the key with an empty one after
+//       the first, negate A in the first proof of the first batch, the last proof of the others and proofs 63 and 64 of each
+//       batch that has them, and compare Groth16::verify_batch_keys_locate's verdicts with the host verifier per proof
+//       (timing the keyed locate call)
 //       chain:<a> = the witness of the reference's squaring-chain bench family for input a
 //       (test-vectors/complex-circuit/input.json has a = 3), computed on the host instead of by WASM.
 #include <algorithm>
@@ -396,6 +400,65 @@ int main(int argc, char** argv) {
             }
             std::printf("verify_keys %d proofs in %d batches: device=%s host=%s agree=%d, device %.3f ms/call (%.1f proofs/s)\n", k,
                         (int)nb + 1, dev.c_str(), host.c_str(), dev == host, dev_ms, k / (dev_ms / 1e3));
+        }
+        if (const char* kl = std::getenv("B2G_VERIFY_KEYS_LOCATE")) {    // one verdict per proof over key batches, against the host
+            const int k = std::atoi(kl);
+            if (k < 1) throw SynthesisError("B2G_VERIFY_KEYS_LOCATE must be >= 1");
+            std::vector<std::vector<Fr>> wv((size_t)k, full_assignment);
+            if (wsrc.rfind("chain:", 0) == 0)
+                for (int i = 1; i < k; i++) wv[(size_t)i] = chain_witness(params.a_query.size(), std::stoull(wsrc.substr(6)) + (unsigned long long)i);
+            std::vector<const std::vector<Fr>*> ws;
+            for (const auto& w : wv) ws.push_back(&w);
+            std::mt19937_64 rng(0x4C0C);
+            std::vector<std::pair<Fr, Fr>> rs;
+            for (int i = 0; i < k; i++) rs.push_back({Fr::rand(rng), Fr::rand(rng)});
+            const std::vector<Proof> proofs = Groth16::create_proofs(params, matrices, rs, ws);
+            // up to four batches of the bench key (sizes about k/4, the rest in the last) with an empty one after the first;
+            // A -> -A in the first proof of the first batch, the last proof of every other batch, and proofs 63 and 64 (the
+            // edge of its first two groups) of every batch that has them
+            const size_t nb = std::min<size_t>(4, (size_t)k), per = (size_t)k / nb;
+            std::vector<std::vector<std::vector<Fr>>> inputs(nb + 1);
+            std::vector<std::vector<Proof>> parts(nb + 1);
+            for (size_t i = 0; i < (size_t)k; i++) {
+                const size_t b = std::min(i / per, nb - 1);
+                const size_t slot = b == 0 ? 0 : b + 1;                    // slot 1 stays empty
+                inputs[slot].emplace_back(wv[i].begin() + 1, wv[i].begin() + num_inputs);
+                parts[slot].push_back(proofs[i]);
+            }
+            int tampered = 0;
+            for (size_t b = 0; b <= nb; b++) {
+                std::vector<size_t> at;
+                if (parts[b].empty()) continue;
+                at.push_back(b == 0 ? 0 : parts[b].size() - 1);
+                if (parts[b].size() > 64) { at.push_back(63); at.push_back(64); }
+                std::sort(at.begin(), at.end());
+                at.erase(std::unique(at.begin(), at.end()), at.end());
+                for (size_t i : at) {                                     // A -> -A: y -> p - y
+                    uint64_t y[4], d[4]; memcpy(y, parts[b][i].bytes + 32, 32);
+                    unsigned __int128 borrow = 0;
+                    for (int j = 0; j < 4; j++) { unsigned __int128 t = (unsigned __int128)detail::FQ_P[j] - y[j] - borrow; d[j] = (uint64_t)t; borrow = (t >> 64) & 1; }
+                    memcpy(parts[b][i].bytes + 32, d, 32);
+                    tampered++;
+                }
+            }
+            auto pvk = Groth16::process_vk(params.vk);
+            std::vector<KeyBatch> batches;
+            for (size_t b = 0; b <= nb; b++) batches.push_back({pvk, inputs[b], parts[b]});
+            std::vector<std::vector<bool>> got = Groth16::verify_batch_keys_locate(batches);   // also loads the key on the device
+            auto t1 = std::chrono::steady_clock::now();
+            got = Groth16::verify_batch_keys_locate(batches);
+            const double dev_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t1).count();
+            int agree = got.size() == nb + 1, valid = 0;
+            for (size_t b = 0; b <= nb && agree; b++) {
+                agree &= got[b].size() == parts[b].size();
+                for (size_t i = 0; i < parts[b].size() && agree; i++) {
+                    const bool host = Groth16::verify_with_processed_vk(pvk, inputs[b][i], parts[b][i]);
+                    agree &= host == got[b][i];
+                    valid += host;
+                }
+            }
+            std::printf("verify_keys_locate %d proofs in %d batches (%d valid, %d tampered): agree=%d, device %.3f ms/call (%.1f proofs/s)\n",
+                        k, (int)nb + 1, valid, tampered, agree, dev_ms, k / (dev_ms / 1e3));
         }
         return 0;
     } catch (const std::exception& e) {

@@ -23,6 +23,8 @@
  *   b2g_verify_batch_locate (+ _compressed) <- GrothBn::verify_with_processed_vk for every proof of a batch, at about the
  *                             batch check's cost when few proofs are invalid
  *   b2g_verify_batch_keys (+ _compressed) <- b2g_verify_batch for many keys, one verdict per key, in one device pass
+ *   b2g_verify_batch_keys_locate (+ _compressed) <- b2g_verify_batch_locate for many keys, one verdict per proof, in one
+ *                             device pass
  *   b2g_fixed_base_g1/g2  <- the batch fixed-base multiplications of generate_random_parameters_with_reduction
  *                             (tests/groth16.rs:25); used to manufacture synthetic proving keys
  *
@@ -306,7 +308,7 @@ B2G_API int b2g_verify_batch_locate(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, co
 B2G_API int b2g_verify_batch_locate_compressed(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs,
                                                const void* compressed, const void* weights, uint8_t* verdicts_out);
 
-/* One batch of proofs under one verifying key, for b2g_verify_batch_keys. */
+/* One batch of proofs under one verifying key, for b2g_verify_batch_keys and b2g_verify_batch_keys_locate. */
 typedef struct {
     b2g_vk* vk;
     uint32_t count;              /* proofs under this key (0 allowed) */
@@ -332,6 +334,27 @@ B2G_API int b2g_verify_batch_keys(b2g_ctx* ctx, uint32_t n_keys, const b2g_key_b
 /* b2g_verify_batch_keys_compressed: b2g_verify_batch_keys on compressed proofs (128 B each), decoded on the device.  A proof
  * that does not decode is malformed: verdicts_out[k] equals b2g_proofs_decompress followed by b2g_verify_batch_keys. */
 B2G_API int b2g_verify_batch_keys_compressed(b2g_ctx* ctx, uint32_t n_keys, const b2g_key_batch* batches, uint8_t* verdicts_out);
+
+/* b2g_verify_batch_keys_locate: b2g_verify_batch_locate for n_keys batches, each under its own key, in one device pass, for
+ * callers that see many circuits and take their proofs from untrusted submitters (rollup and bridge nodes, aggregators).
+ * verdicts_out = one byte per proof, sum of batches[k].count bytes in batch order: batch k's verdicts start at the sum of
+ * count_j over j < k, and a batch with count == 0 has none.  Batch k's verdicts equal, bit for bit, verdicts_out of
+ * b2g_verify_batch_locate(batches[k].vk, batches[k].count, the same public inputs, proofs and weights).  Groups never cross
+ * keys: a batch's groups of 64 start at its first proof and its last group may be shorter.  The completeness, soundness and
+ * determinism statements of b2g_verify_batch_locate hold per batch.  The same key may appear in several batches.
+ * Cost: b2g_verify_batch's per-proof work over all proofs, plus per group one two-pair Miller loop, one final exponentiation,
+ * e(alpha, beta)^s_0 and the public-input products; plus b2g_verify_many's work on the well-formed proofs of the failing
+ * groups, all keys in one more device pass.  The number of kernel launches does not depend on n_keys or on how many keys
+ * fail.
+ * Synchronous.  Errors as b2g_verify_batch_keys, with the key index in the message: B2G_E_SHAPE for n_keys == 0, a total
+ * count of 0 or above 2^32 - 1, null pointers, a key of another device or a pending proof; B2G_E_INPUT for a public input >= r
+ * or a zero weight; B2G_E_DEVICE when the buffers do not fit.  Every error leaves the context usable. */
+B2G_API int b2g_verify_batch_keys_locate(b2g_ctx* ctx, uint32_t n_keys, const b2g_key_batch* batches, uint8_t* verdicts_out);
+/* b2g_verify_batch_keys_locate_compressed: b2g_verify_batch_keys_locate on compressed proofs (128 B each), decoded on the
+ * device.  A proof that does not decode is not well-formed: batch k's verdicts equal those of
+ * b2g_verify_batch_locate_compressed on batch k alone. */
+B2G_API int b2g_verify_batch_keys_locate_compressed(b2g_ctx* ctx, uint32_t n_keys, const b2g_key_batch* batches,
+                                                    uint8_t* verdicts_out);
 
 /* Kernel-level entry points (parity tests, benchmarks). All pointers host. */
 B2G_API int b2g_msm_g1(b2g_ctx* ctx, const void* bases, const void* scalars, size_t n, int scalars_mont, void* out_xy_mont);
