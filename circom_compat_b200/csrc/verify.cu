@@ -964,20 +964,6 @@ static CtxView batch_args(const char* fn, b2g_ctx* ctx, uint32_t count) {
     return cv;
 }
 
-// the argument checks of the verifiers (b2g_verify_many, b2g_verify_batch and their compressed forms); returns the context
-static CtxView verify_args(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs,
-                           const void* out) {
-    if (!ctx || !vk || !proofs || !out || (vk->n_public && !public_inputs)) throw_error(B2G_E_SHAPE, "null pointer");
-    const CtxView cv = batch_args(fn, ctx, count);
-    if (vk->device != cv.device) throw_error(B2G_E_SHAPE, "the verifying key belongs to another device");
-    const size_t inputs = (size_t)count * vk->n_public;
-    const uint32_t* pub = (const uint32_t*)public_inputs;
-    for (size_t k = 0; k < inputs; k++)
-        if (!below_r(pub + 8 * k)) throw_error(B2G_E_INPUT, "public input " + std::to_string(k % vk->n_public) + " of proof " +
-                                                             std::to_string(k / vk->n_public) + " is not below the scalar field modulus r");
-    return cv;
-}
-
 // vbufs_ensure, reporting a batch that does not fit as B2G_E_DEVICE with advice
 static void verify_bufs_ensure(const char* fn, VerifyBufs*& v, uint32_t count, size_t inputs, size_t parts, size_t batch = 0,
                                size_t comp = 0, size_t meta = 0) {
@@ -1047,26 +1033,6 @@ static void verify_many_enqueue(VerifyBufs& v, const std::vector<b2g_vk*>& vks, 
     verify_final_kernel<<<(count + 63) / 64, 64, 0, st>>>(v.d_rec, v.d_f, d_keys, d_segs, n_segs, count, v.d_verdict);
     g_launch_count += 3 + (inputs ? 1 : 0);
     CUDA_CHECK(cudaGetLastError());
-}
-
-// b2g_verify_many on 256-byte rows, or on compressed rows decoded on the device (G2 check included): a table of one key
-static void verify_many_run(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs,
-                            bool compressed, uint8_t* verdicts_out) {
-    const CtxView cv = verify_args(fn, ctx, vk, count, public_inputs, proofs, verdicts_out);
-    const size_t inputs = (size_t)count * vk->n_public;
-    DevGuard g(cv.device);
-    cudaStream_t st = cv.st;
-    verify_bufs_ensure(fn, *cv.vbufs, count, inputs, inputs, 0, compressed ? comp_bytes(count) : 0, many_meta_bytes(1));
-    VerifyBufs& v = **cv.vbufs;
-    verify_many_enqueue(v, {vk}, {count}, public_inputs, proofs, compressed, st);
-    CUDA_CHECK(cudaMemcpyAsync(verdicts_out, v.d_verdict, count, cudaMemcpyDeviceToHost, st));
-    CUDA_CHECK(cudaStreamSynchronize(st));
-}
-
-// the batch verifiers' weight check: no weight is zero
-static void weights_check(const void* weights, uint32_t count) {
-    for (uint32_t i = 0; i < count; i++)
-        if (all_zero((const uint8_t*)weights + 16 * (size_t)i, 16)) throw_error(B2G_E_INPUT, "weight " + std::to_string(i) + " is zero");
 }
 
 // the device results of batch_enqueue: wf (one byte per proof: it parses and its B lies in G2) and one verdict per segment
@@ -1192,18 +1158,6 @@ static BatchOut batch_enqueue(const char* fn, const CtxView& cv, const std::vect
     return {wf, gv};
 }
 
-// b2g_verify_batch on 256-byte rows, or on compressed rows: the batch check with one segment of the whole batch
-static void verify_batch_run(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs,
-                             bool compressed, const void* weights, uint8_t* verdict_out) {
-    if (!weights) throw_error(B2G_E_SHAPE, "null pointer");
-    const CtxView cv = verify_args(fn, ctx, vk, count, public_inputs, proofs, verdict_out);
-    weights_check(weights, count);
-    DevGuard g(cv.device);
-    const BatchOut r = batch_enqueue(fn, cv, {vk}, {{0, count}}, false, false, public_inputs, proofs, compressed, weights);
-    CUDA_CHECK(cudaMemcpyAsync(verdict_out, r.verdict, 1, cudaMemcpyDeviceToHost, cv.st));
-    CUDA_CHECK(cudaStreamSynchronize(cv.st));
-}
-
 // key batches as one run of proofs: one entry per batch that holds proofs (vks, counts, and its index among the caller's
 // batches in `at`), and their proofs, public inputs and weights back to back.  With one such batch these are the caller's
 // arrays; with more they are packed into one host array each, so that each goes up in one copy.
@@ -1216,18 +1170,17 @@ struct KeysPacked {
     std::vector<uint8_t> rows_h, pubs_h, ws_h;
 };
 
-// one key's proofs as a KeysPacked of one entry (b2g_verify_batch_locate)
-static KeysPacked keys_one(b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs, const void* weights) {
-    KeysPacked p;
-    p.vks = {vk}; p.counts = {count}; p.at = {0};
-    p.total = count; p.inputs = (size_t)count * vk->n_public;
-    p.proofs = proofs; p.public_inputs = public_inputs; p.weights = weights;
-    return p;
+// the shape checks of a one-key verifier (b2g_verify_many, b2g_verify_batch, b2g_verify_batch_locate and their compressed
+// forms) on the key batch made of its arguments, the weights only when its kind takes them; returns the number of proofs
+static uint32_t one_key_shape(b2g_ctx* ctx, const b2g_key_batch& b, bool weighted, const uint8_t* verdicts_out) {
+    if (!ctx || !b.vk || !b.proofs || !verdicts_out || (weighted && !b.weights) || (b.vk->n_public && !b.public_inputs))
+        throw_error(B2G_E_SHAPE, "null pointer");
+    return b.count;
 }
 
-// the argument checks of b2g_verify_batch_keys and b2g_verify_batch_keys_locate (and their compressed forms), each message
-// naming the key index; returns the context
-static CtxView keys_args(const char* fn, b2g_ctx* ctx, uint32_t n_keys, const b2g_key_batch* batches, const uint8_t* verdicts_out) {
+// the shape checks of a key-table verifier (b2g_verify_batch_keys, b2g_verify_batch_keys_locate and their compressed forms),
+// each message about a row naming the key index; returns the number of proofs
+static uint32_t keys_shape(const char* fn, b2g_ctx* ctx, uint32_t n_keys, const b2g_key_batch* batches, const uint8_t* verdicts_out) {
     if (!ctx || !batches || !verdicts_out) throw_error(B2G_E_SHAPE, "null pointer");
     if (n_keys == 0) throw_error(B2G_E_SHAPE, std::string(fn) + ": n_keys must be at least 1");
     auto at = [&](uint32_t k) { return std::string(fn) + ": key " + std::to_string(k) + ": "; };
@@ -1240,32 +1193,37 @@ static CtxView keys_args(const char* fn, b2g_ctx* ctx, uint32_t n_keys, const b2
     }
     if (total == 0) throw_error(B2G_E_SHAPE, std::string(fn) + ": every key batch is empty; at least one proof is needed");
     if (total > UINT32_MAX) throw_error(B2G_E_SHAPE, std::string(fn) + ": more than 2^32 - 1 proofs in all");
-    const CtxView cv = batch_args(fn, ctx, (uint32_t)total);
-    for (uint32_t k = 0; k < n_keys; k++) {
-        const b2g_key_batch& b = batches[k];
-        if (b.vk->device != cv.device) throw_error(B2G_E_SHAPE, at(k) + "the verifying key belongs to another device");
-        const uint32_t n_public = b.vk->n_public;
-        const uint32_t* pub = (const uint32_t*)b.public_inputs;
-        for (size_t i = 0; i < (size_t)b.count * n_public; i++)
-            if (!below_r(pub + 8 * i)) throw_error(B2G_E_INPUT, at(k) + "public input " + std::to_string(i % n_public) + " of proof " +
-                                                                std::to_string(i / n_public) + " is not below the scalar field modulus r");
-        for (uint32_t i = 0; i < b.count; i++)
-            if (all_zero((const uint8_t*)b.weights + 16 * (size_t)i, 16)) throw_error(B2G_E_INPUT, at(k) + "weight " + std::to_string(i) + " is zero");
-    }
-    return cv;
+    return (uint32_t)total;
 }
 
-// the key batches (checked by keys_args) as one run of proofs
+// the content checks of one key batch, for every verifier: its key lies on the context's device, every public input is
+// below r and, when the kind takes weights, no weight is zero.  In a key table (key >= 0) each message names the key index.
+static void batch_check(const char* fn, int64_t key, const CtxView& cv, const b2g_key_batch& b, bool weighted) {
+    auto fail = [&](int code, const std::string& what) {
+        throw_error(code, key < 0 ? what : std::string(fn) + ": key " + std::to_string(key) + ": " + what);
+    };
+    if (b.vk->device != cv.device) fail(B2G_E_SHAPE, "the verifying key belongs to another device");
+    const uint32_t n_public = b.vk->n_public;
+    const uint32_t* pub = (const uint32_t*)b.public_inputs;
+    for (size_t i = 0; i < (size_t)b.count * n_public; i++)
+        if (!below_r(pub + 8 * i)) fail(B2G_E_INPUT, "public input " + std::to_string(i % n_public) + " of proof " + std::to_string(i / n_public) +
+                                                     " is not below the scalar field modulus r");
+    for (uint32_t i = 0; weighted && i < b.count; i++)
+        if (all_zero((const uint8_t*)b.weights + 16 * (size_t)i, 16)) fail(B2G_E_INPUT, "weight " + std::to_string(i) + " is zero");
+}
+
+// the key batches (checked) as one run of proofs
 static KeysPacked keys_pack(uint32_t n_keys, const b2g_key_batch* batches, bool compressed) {
     uint32_t used = 0, last = 0;
     for (uint32_t k = 0; k < n_keys; k++) if (batches[k].count) { used++; last = k; }
+    KeysPacked p;
     if (used == 1) {
         const b2g_key_batch& b = batches[last];
-        KeysPacked p = keys_one(b.vk, b.count, b.public_inputs, b.proofs, b.weights);
-        p.at = {last};
+        p.vks = {b.vk}; p.counts = {b.count}; p.at = {last};
+        p.total = b.count; p.inputs = (size_t)b.count * b.vk->n_public;
+        p.proofs = b.proofs; p.public_inputs = b.public_inputs; p.weights = b.weights;
         return p;
     }
-    KeysPacked p;
     for (uint32_t k = 0; k < n_keys; k++) {
         p.total += batches[k].count;
         p.inputs += (size_t)batches[k].count * batches[k].vk->n_public;
@@ -1343,91 +1301,96 @@ static void locate_run(const char* fn, const CtxView& cv, const KeysPacked& p, b
     memcpy(verdicts_out, out.data(), p.total);
 }
 
-// b2g_verify_batch_locate on 256-byte rows, or on compressed rows: the locate pipeline with one key
-static void verify_locate_run(const char* fn, b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs,
-                              bool compressed, const void* weights, uint8_t* verdicts_out) {
-    if (!weights) throw_error(B2G_E_SHAPE, "null pointer");
-    const CtxView cv = verify_args(fn, ctx, vk, count, public_inputs, proofs, verdicts_out);
-    weights_check(weights, count);
-    DevGuard g(cv.device);
-    locate_run(fn, cv, keys_one(vk, count, public_inputs, proofs, weights), compressed, verdicts_out);
-}
+// how a verifier call runs its key batches:
+//   VERIFY_MANY    b2g_verify_many's kernels, one verdict per proof
+//   VERIFY_BATCH   the batch check with one segment, unmasked: b2g_verify_batch's one verdict
+//   VERIFY_KEYS    the batch check with one segment per key batch that holds proofs (keyed): one verdict per key batch
+//   VERIFY_LOCATE  locate_run, one verdict per proof
+// VERIFY_BATCH stays apart from VERIFY_KEYS on one key: it has one launch fewer, and its Miller kernel skips a batch that
+// has already failed.
+enum VerifyKind { VERIFY_MANY, VERIFY_BATCH, VERIFY_KEYS, VERIFY_LOCATE };
 
-// b2g_verify_batch_keys_locate on 256-byte rows, or on compressed rows: the locate pipeline over every key batch, whose
-// verdicts lie back to back in batch order (an empty batch has none)
-static void verify_keys_locate_run(const char* fn, b2g_ctx* ctx, uint32_t n_keys, const b2g_key_batch* batches, bool compressed,
-                                   uint8_t* verdicts_out) {
-    const CtxView cv = keys_args(fn, ctx, n_keys, batches, verdicts_out);
+// every verifier on 256-byte rows, or on compressed rows: the checks, then kind's run over the key batches, whose verdicts
+// go to verdicts_out (a key batch without proofs gets 1 under VERIFY_KEYS, and none under VERIFY_LOCATE).  `table`: the
+// batches are the caller's key table, not the one batch made of a one-key verifier's arguments.
+static void verify_run(const char* fn, b2g_ctx* ctx, VerifyKind kind, bool table, uint32_t n_keys, const b2g_key_batch* batches,
+                       bool compressed, uint8_t* verdicts_out) {
+    const bool weighted = kind != VERIFY_MANY;
+    const uint32_t total = table ? keys_shape(fn, ctx, n_keys, batches, verdicts_out) : one_key_shape(ctx, batches[0], weighted, verdicts_out);
+    const CtxView cv = batch_args(fn, ctx, total);
+    for (uint32_t k = 0; k < n_keys; k++) batch_check(fn, table ? (int64_t)k : -1, cv, batches[k], weighted);
     const KeysPacked p = keys_pack(n_keys, batches, compressed);
     DevGuard g(cv.device);
-    locate_run(fn, cv, p, compressed, verdicts_out);
-}
-
-// b2g_verify_batch_keys on 256-byte rows, or on compressed rows: the batch check with one segment per key batch that holds
-// proofs; a batch without proofs gets 1
-static void verify_keys_run(const char* fn, b2g_ctx* ctx, uint32_t n_keys, const b2g_key_batch* batches, bool compressed,
-                            uint8_t* verdicts_out) {
-    const CtxView cv = keys_args(fn, ctx, n_keys, batches, verdicts_out);
-    const KeysPacked p = keys_pack(n_keys, batches, compressed);
-    std::vector<SegIn> segs;
-    for (uint32_t k = 0; k < (uint32_t)p.vks.size(); k++) segs.push_back({k, p.counts[k]});
-    DevGuard g(cv.device);
-    const BatchOut r = batch_enqueue(fn, cv, p.vks, segs, false, true, p.public_inputs, p.proofs, compressed, p.weights);
-    std::vector<uint8_t> gv(segs.size());
-    CUDA_CHECK(cudaMemcpyAsync(gv.data(), r.verdict, segs.size(), cudaMemcpyDeviceToHost, cv.st));
-    CUDA_CHECK(cudaStreamSynchronize(cv.st));
-    std::fill(verdicts_out, verdicts_out + n_keys, 1);
-    for (size_t k = 0; k < segs.size(); k++) verdicts_out[p.at[k]] = gv[k];
+    cudaStream_t st = cv.st;
+    if (kind == VERIFY_LOCATE) {
+        locate_run(fn, cv, p, compressed, verdicts_out);
+    } else if (kind == VERIFY_MANY) {
+        verify_bufs_ensure(fn, *cv.vbufs, p.total, p.inputs, p.inputs, 0, compressed ? comp_bytes(p.total) : 0, many_meta_bytes(p.vks.size()));
+        verify_many_enqueue(**cv.vbufs, p.vks, p.counts, p.public_inputs, p.proofs, compressed, st);
+        CUDA_CHECK(cudaMemcpyAsync(verdicts_out, (*cv.vbufs)->d_verdict, p.total, cudaMemcpyDeviceToHost, st));
+        CUDA_CHECK(cudaStreamSynchronize(st));
+    } else {
+        std::vector<SegIn> segs;
+        for (uint32_t k = 0; k < (uint32_t)p.vks.size(); k++) segs.push_back({k, p.counts[k]});
+        const BatchOut r = batch_enqueue(fn, cv, p.vks, segs, false, kind == VERIFY_KEYS, p.public_inputs, p.proofs, compressed, p.weights);
+        std::vector<uint8_t> gv(segs.size());
+        CUDA_CHECK(cudaMemcpyAsync(gv.data(), r.verdict, segs.size(), cudaMemcpyDeviceToHost, st));
+        CUDA_CHECK(cudaStreamSynchronize(st));
+        std::fill(verdicts_out, verdicts_out + n_keys, 1);
+        for (size_t k = 0; k < segs.size(); k++) verdicts_out[p.at[k]] = gv[k];
+    }
 }
 
 int b2g_verify_many(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs, uint8_t* verdicts_out) {
-    return guarded([&] { verify_many_run("b2g_verify_many", ctx, vk, count, public_inputs, proofs, false, verdicts_out); });
+    const b2g_key_batch b = {vk, count, 0, public_inputs, proofs, nullptr};
+    return guarded([&] { verify_run("b2g_verify_many", ctx, VERIFY_MANY, false, 1, &b, false, verdicts_out); });
 }
 
 int b2g_verify_many_compressed(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* compressed,
                                uint8_t* verdicts_out) {
-    return guarded([&] { verify_many_run("b2g_verify_many_compressed", ctx, vk, count, public_inputs, compressed, true, verdicts_out); });
+    const b2g_key_batch b = {vk, count, 0, public_inputs, compressed, nullptr};
+    return guarded([&] { verify_run("b2g_verify_many_compressed", ctx, VERIFY_MANY, false, 1, &b, true, verdicts_out); });
 }
 
 int b2g_verify_batch(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs, const void* weights,
                      uint8_t* verdict_out) {
-    return guarded([&] { verify_batch_run("b2g_verify_batch", ctx, vk, count, public_inputs, proofs, false, weights, verdict_out); });
+    const b2g_key_batch b = {vk, count, 0, public_inputs, proofs, weights};
+    return guarded([&] { verify_run("b2g_verify_batch", ctx, VERIFY_BATCH, false, 1, &b, false, verdict_out); });
 }
 
 int b2g_verify_batch_compressed(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* compressed,
                                 const void* weights, uint8_t* verdict_out) {
-    return guarded([&] {
-        verify_batch_run("b2g_verify_batch_compressed", ctx, vk, count, public_inputs, compressed, true, weights, verdict_out);
-    });
+    const b2g_key_batch b = {vk, count, 0, public_inputs, compressed, weights};
+    return guarded([&] { verify_run("b2g_verify_batch_compressed", ctx, VERIFY_BATCH, false, 1, &b, true, verdict_out); });
 }
 
 int b2g_verify_batch_locate(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* proofs, const void* weights,
                             uint8_t* verdicts_out) {
-    return guarded([&] { verify_locate_run("b2g_verify_batch_locate", ctx, vk, count, public_inputs, proofs, false, weights, verdicts_out); });
+    const b2g_key_batch b = {vk, count, 0, public_inputs, proofs, weights};
+    return guarded([&] { verify_run("b2g_verify_batch_locate", ctx, VERIFY_LOCATE, false, 1, &b, false, verdicts_out); });
 }
 
 int b2g_verify_batch_locate_compressed(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs, const void* compressed,
                                        const void* weights, uint8_t* verdicts_out) {
-    return guarded([&] {
-        verify_locate_run("b2g_verify_batch_locate_compressed", ctx, vk, count, public_inputs, compressed, true, weights, verdicts_out);
-    });
+    const b2g_key_batch b = {vk, count, 0, public_inputs, compressed, weights};
+    return guarded([&] { verify_run("b2g_verify_batch_locate_compressed", ctx, VERIFY_LOCATE, false, 1, &b, true, verdicts_out); });
 }
 
 int b2g_verify_batch_keys(b2g_ctx* ctx, uint32_t n_keys, const b2g_key_batch* batches, uint8_t* verdicts_out) {
-    return guarded([&] { verify_keys_run("b2g_verify_batch_keys", ctx, n_keys, batches, false, verdicts_out); });
+    return guarded([&] { verify_run("b2g_verify_batch_keys", ctx, VERIFY_KEYS, true, n_keys, batches, false, verdicts_out); });
 }
 
 int b2g_verify_batch_keys_compressed(b2g_ctx* ctx, uint32_t n_keys, const b2g_key_batch* batches, uint8_t* verdicts_out) {
-    return guarded([&] { verify_keys_run("b2g_verify_batch_keys_compressed", ctx, n_keys, batches, true, verdicts_out); });
+    return guarded([&] { verify_run("b2g_verify_batch_keys_compressed", ctx, VERIFY_KEYS, true, n_keys, batches, true, verdicts_out); });
 }
 
 int b2g_verify_batch_keys_locate(b2g_ctx* ctx, uint32_t n_keys, const b2g_key_batch* batches, uint8_t* verdicts_out) {
-    return guarded([&] { verify_keys_locate_run("b2g_verify_batch_keys_locate", ctx, n_keys, batches, false, verdicts_out); });
+    return guarded([&] { verify_run("b2g_verify_batch_keys_locate", ctx, VERIFY_LOCATE, true, n_keys, batches, false, verdicts_out); });
 }
 
 int b2g_verify_batch_keys_locate_compressed(b2g_ctx* ctx, uint32_t n_keys, const b2g_key_batch* batches, uint8_t* verdicts_out) {
     return guarded([&] {
-        verify_keys_locate_run("b2g_verify_batch_keys_locate_compressed", ctx, n_keys, batches, true, verdicts_out);
+        verify_run("b2g_verify_batch_keys_locate_compressed", ctx, VERIFY_LOCATE, true, n_keys, batches, true, verdicts_out);
     });
 }
 

@@ -324,54 +324,55 @@ def _verify_args(fn, vk, public_inputs, proofs, ctx, compressed=False):
     return ctx, vh, len(proofs), pub_arr, data
 
 
-def _verify_many(fn, vk, public_inputs, proofs, ctx, compressed) -> list:
-    """Groth16.verify_many and verify_many_compressed"""
-    args = _verify_args(fn, vk, public_inputs, proofs, ctx, compressed)
-    if args is None:
-        return []
-    ctx, vh, count, pub_arr, data = args
-    out = np.zeros(count, dtype=np.uint8)
-    entry = N.lib().b2g_verify_many_compressed if compressed else N.lib().b2g_verify_many
-    N.check(entry(ctx._h, vh, count, _ptr(pub_arr) if pub_arr is not None else None, _ptr(data), _ptr(out)))
-    return [bool(v) for v in out]
+# the library entry of each verifier, by (kind, compressed)
+_VERIFY_ENTRY = {(kind, compressed): f"b2g_verify_{kind}{'_compressed' if compressed else ''}"
+                 for kind in ('many', 'batch', 'batch_locate', 'batch_keys', 'batch_keys_locate') for compressed in (False, True)}
 
 
-def _verify_batch(fn, vk, public_inputs, proofs, ctx, weights, compressed, locate=False):
-    """Groth16.verify_batch, verify_batch_locate and their compressed forms: one bool, or one bool per proof when locate"""
+def _check_weights(where, weights, count, at=''):
+    """caller-given weights as ints, one per proof and each in [1, 2^128), checked before the key is loaded on the device;
+    `at` starts the message of a weight out of range"""
+    weights = [int(w) for w in weights]
+    if len(weights) != count:
+        raise ValueError(f"{where}: one weight per proof")
+    for w in weights:
+        if not 0 < w < 1 << 128:
+            raise N.B2gError(N.B2G_E_INPUT, f"{at}weight {w} is not in [1, 2^128)")
+    return weights
+
+
+def _weight_bytes(weights, count) -> np.ndarray:
+    """the weights as 16-byte little-endian words, drawn with secrets.randbits(128) (never 0) when None"""
     import secrets
-    proofs = list(proofs)
-    if weights is not None:                    # checked before the key is loaded on the device
-        weights = [int(w) for w in weights]
-        if len(weights) != len(proofs):
-            raise ValueError(f"{fn}: one weight per proof")
-        for w in weights:
-            if not 0 < w < 1 << 128:
-                raise N.B2gError(N.B2G_E_INPUT, f"weight {w} is not in [1, 2^128)")
-    args = _verify_args(fn, vk, public_inputs, proofs, ctx, compressed)
-    if args is None:
-        return [] if locate else True
-    ctx, vh, count, pub_arr, data = args
     if weights is None:
         weights = []
         while len(weights) < count:
             w = secrets.randbits(128)
             if w:
                 weights.append(w)
-    wb = np.frombuffer(b''.join(w.to_bytes(16, 'little') for w in weights), dtype=np.uint8).copy()
-    out = np.zeros(count if locate else 1, dtype=np.uint8)
-    L = N.lib()
-    if locate:
-        entry = L.b2g_verify_batch_locate_compressed if compressed else L.b2g_verify_batch_locate
-    else:
-        entry = L.b2g_verify_batch_compressed if compressed else L.b2g_verify_batch
-    N.check(entry(ctx._h, vh, count, _ptr(pub_arr) if pub_arr is not None else None, _ptr(data), _ptr(wb), _ptr(out)))
-    return [bool(v) for v in out] if locate else bool(out[0])
+    return np.frombuffer(b''.join(w.to_bytes(16, 'little') for w in weights), dtype=np.uint8).copy()
+
+
+def _verify_one_key(fn, kind, vk, public_inputs, proofs, ctx, compressed, weights=None):
+    """Groth16.verify_many, verify_batch, verify_batch_locate and their compressed forms (kind 'many', 'batch' or
+    'batch_locate'): one bool for 'batch', else one bool per proof"""
+    proofs = list(proofs)
+    if weights is not None:
+        weights = _check_weights(fn, weights, len(proofs))
+    args = _verify_args(fn, vk, public_inputs, proofs, ctx, compressed)
+    if args is None:
+        return True if kind == 'batch' else []
+    ctx, vh, count, pub_arr, data = args
+    wb = None if kind == 'many' else _weight_bytes(weights, count)
+    out = np.zeros(1 if kind == 'batch' else count, dtype=np.uint8)
+    ws = () if wb is None else (_ptr(wb),)
+    N.check(getattr(N.lib(), _VERIFY_ENTRY[kind, compressed])(ctx._h, vh, count, _ptr(pub_arr), _ptr(data), *ws, _ptr(out)))
+    return bool(out[0]) if kind == 'batch' else [bool(v) for v in out]
 
 
 def _key_batches(fn, batches, ctx, weights, compressed):
     """the argument checks and encoding of the keyed verifiers: (ctx, number of batches, [(batch index, KeyBatch)] for the
     batches that hold proofs, the arrays the KeyBatch rows point into)"""
-    import secrets
     from . import verifier
     batches = [tuple(b) for b in batches]
     for k, b in enumerate(batches):
@@ -387,12 +388,8 @@ def _key_batches(fn, batches, ctx, weights, compressed):
         where = f"{fn}: key {k}"
         proofs = list(proofs)
         ws = None if weights is None else weights[k]
-        if ws is not None:                     # checked before the key is loaded on the device
-            if len(ws) != len(proofs):
-                raise ValueError(f"{where}: one weight per proof")
-            for w in ws:
-                if not 0 < w < 1 << 128:
-                    raise N.B2gError(N.B2G_E_INPUT, f"{where}: weight {w} is not in [1, 2^128)")
+        if ws is not None:
+            _check_weights(where, ws, len(proofs), f"{where}: ")
         try:
             args = _verify_args(where, vk, public_inputs, proofs, ctx, compressed)
         except N.B2gError as e:
@@ -402,48 +399,27 @@ def _key_batches(fn, batches, ctx, weights, compressed):
         if args is None:                       # an empty batch is not passed on
             continue
         _, vh, count, pub_arr, data = args
-        if ws is None:
-            ws = []
-            while len(ws) < count:
-                w = secrets.randbits(128)
-                if w:
-                    ws.append(w)
-        wb = np.frombuffer(b''.join(w.to_bytes(16, 'little') for w in ws), dtype=np.uint8).copy()
+        wb = _weight_bytes(ws, count)
         keep += [pub_arr, data, wb]
         rows.append((k, N.KeyBatch(vh.value, count, 0, _ptr(pub_arr).value if pub_arr is not None else None, _ptr(data).value,
                                    _ptr(wb).value)))
     return ctx, len(batches), rows, keep
 
 
-def _verify_batch_keys(fn, batches, ctx, weights, compressed) -> list:
-    """Groth16.verify_batch_keys and verify_batch_keys_compressed: one bool per (vk, public_inputs, proofs) batch"""
+def _verify_batch_keys(fn, batches, ctx, weights, compressed, locate) -> list:
+    """Groth16.verify_batch_keys, verify_batch_keys_locate and their compressed forms: per (vk, public_inputs, proofs)
+    batch one bool, or one list of bools when locate"""
     ctx, n, rows, keep = _key_batches(fn, batches, ctx, weights, compressed)
-    verdicts = [True] * n                      # an empty batch is True
+    verdicts = [[] if locate else True for _ in range(n)]      # an empty batch has no verdicts, or is True
     if not rows:
         return verdicts
     table = (N.KeyBatch * len(rows))(*[r for _, r in rows])
-    out = np.zeros(len(rows), dtype=np.uint8)
-    entry = N.lib().b2g_verify_batch_keys_compressed if compressed else N.lib().b2g_verify_batch_keys
-    N.check(entry(ctx._h, len(rows), table, _ptr(out)))
-    for (k, _), v in zip(rows, out):
-        verdicts[k] = bool(v)
-    return verdicts
-
-
-def _verify_batch_keys_locate(fn, batches, ctx, weights, compressed) -> list:
-    """Groth16.verify_batch_keys_locate and verify_batch_keys_locate_compressed: one list of bools per (vk, public_inputs,
-    proofs) batch"""
-    ctx, n, rows, keep = _key_batches(fn, batches, ctx, weights, compressed)
-    verdicts = [[] for _ in range(n)]          # an empty batch has no verdicts
-    if not rows:
-        return verdicts
-    table = (N.KeyBatch * len(rows))(*[r for _, r in rows])
-    out = np.zeros(sum(r.count for _, r in rows), dtype=np.uint8)
-    entry = N.lib().b2g_verify_batch_keys_locate_compressed if compressed else N.lib().b2g_verify_batch_keys_locate
+    out = np.zeros(sum(r.count for _, r in rows) if locate else len(rows), dtype=np.uint8)
+    entry = getattr(N.lib(), _VERIFY_ENTRY['batch_keys_locate' if locate else 'batch_keys', compressed])
     N.check(entry(ctx._h, len(rows), table, _ptr(out)))
     at = 0
-    for k, r in rows:
-        verdicts[k] = [bool(v) for v in out[at:at + r.count]]
+    for i, (k, r) in enumerate(rows):
+        verdicts[k] = [bool(v) for v in out[at:at + r.count]] if locate else bool(out[i])
         at += r.count
     return verdicts
 
@@ -611,7 +587,7 @@ class Groth16:
         sequence of ints per proof, proofs = [Proof].  Returns [bool].  Verdicts equal the host call's, except that a proof
         coordinate >= p is invalid here (arkworks cannot deserialise it) where the host verifier reduces it.  A public input
         outside [0, r) raises B2gError (B2G_E_INPUT); an input count that does not match the key raises MalformedVerifyingKey."""
-        return _verify_many('verify_many', vk, public_inputs, proofs, ctx, False)
+        return _verify_one_key('verify_many', 'many', vk, public_inputs, proofs, ctx, False)
 
     @staticmethod
     def verify_batch(vk, public_inputs, proofs, ctx: Context = None, weights=None) -> bool:
@@ -622,7 +598,7 @@ class Groth16:
         batch is True.  `weights` (one int in [1, 2^128) per proof) are drawn with secrets.randbits(128) when not given;
         weights a prover could know or choose before fixing its proofs make the check unsound.  A zero or too large weight
         raises B2gError (B2G_E_INPUT)."""
-        return _verify_batch('verify_batch', vk, public_inputs, proofs, ctx, weights, False)
+        return _verify_one_key('verify_batch', 'batch', vk, public_inputs, proofs, ctx, False, weights)
 
     @staticmethod
     def verify_batch_locate(vk, public_inputs, proofs, ctx: Context = None, weights=None) -> list:
@@ -633,7 +609,7 @@ class Groth16:
         verify_many accepts and whose B is in G2 is always True; any other proof is False except with probability at most
         (groups holding such a proof) / (2^128 - 1) when the weights are uniform.  Arguments, weights and errors as
         verify_batch; an empty batch gives []."""
-        return _verify_batch('verify_batch_locate', vk, public_inputs, proofs, ctx, weights, False, True)
+        return _verify_one_key('verify_batch_locate', 'batch_locate', vk, public_inputs, proofs, ctx, False, weights)
 
     @staticmethod
     def verify_batch_keys(batches, ctx: Context = None, weights=None) -> list:
@@ -643,14 +619,14 @@ class Groth16:
         weights; an invalid proof changes its own batch's verdict only, and an empty batch is True.  `weights` is None
         (drawn with secrets.randbits(128)) or one list per batch (None in it: drawn).  Argument checks and errors as
         verify_batch, with the batch's index in the message."""
-        return _verify_batch_keys('verify_batch_keys', batches, ctx, weights, False)
+        return _verify_batch_keys('verify_batch_keys', batches, ctx, weights, False, False)
 
     @staticmethod
     def verify_batch_keys_compressed(batches, ctx: Context = None, weights=None) -> list:
         """verify_batch_keys on compressed proofs (b2g_verify_batch_keys_compressed), decoded on the device: a batch with a
         blob that does not decode is False, and the other verdicts are those of verify_batch_keys on the decoded proofs.
         Arguments, weights and errors as verify_batch_keys; a blob that is not 128 bytes raises ValueError."""
-        return _verify_batch_keys('verify_batch_keys_compressed', batches, ctx, weights, True)
+        return _verify_batch_keys('verify_batch_keys_compressed', batches, ctx, weights, True, False)
 
     @staticmethod
     def verify_batch_keys_locate(batches, ctx: Context = None, weights=None) -> list:
@@ -658,14 +634,14 @@ class Groth16:
         takes them.  Returns one list of bools per batch, equal to verify_batch_locate on that batch with the same weights
         (groups of 64 start at each batch's first proof); an empty batch gives [].  Weights, argument checks and errors as
         verify_batch_keys."""
-        return _verify_batch_keys_locate('verify_batch_keys_locate', batches, ctx, weights, False)
+        return _verify_batch_keys('verify_batch_keys_locate', batches, ctx, weights, False, True)
 
     @staticmethod
     def verify_batch_keys_locate_compressed(batches, ctx: Context = None, weights=None) -> list:
         """verify_batch_keys_locate on compressed proofs (b2g_verify_batch_keys_locate_compressed), decoded on the device: a
         blob that does not decode is False, and each batch's verdicts equal verify_batch_locate_compressed on that batch.
         Arguments, weights and errors as verify_batch_keys_locate; a blob that is not 128 bytes raises ValueError."""
-        return _verify_batch_keys_locate('verify_batch_keys_locate_compressed', batches, ctx, weights, True)
+        return _verify_batch_keys('verify_batch_keys_locate_compressed', batches, ctx, weights, True, True)
 
     # ---- compressed proofs: Proof::<Bn254>::serialize_compressed (ethereum.serialize_compressed), decoded on the device
     @staticmethod
@@ -690,21 +666,21 @@ class Groth16:
         """verify_many on compressed proofs (b2g_verify_many_compressed), decoded on the device: a verdict is True exactly
         when the blob decodes as decompress_proofs decodes it (G2 check of B included) and the decoded proof passes
         verify_many.  Arguments and errors as verify_many; a blob that is not 128 bytes raises ValueError."""
-        return _verify_many('verify_many_compressed', vk, public_inputs, blobs, ctx, True)
+        return _verify_one_key('verify_many_compressed', 'many', vk, public_inputs, blobs, ctx, True)
 
     @staticmethod
     def verify_batch_compressed(vk, public_inputs, blobs, ctx: Context = None, weights=None) -> bool:
         """verify_batch on compressed proofs (b2g_verify_batch_compressed), decoded on the device: True exactly when every
         blob decodes and verify_batch with the same weights is True on the decoded proofs.  Arguments, weights and errors as
         verify_batch; a blob that is not 128 bytes raises ValueError."""
-        return _verify_batch('verify_batch_compressed', vk, public_inputs, blobs, ctx, weights, True)
+        return _verify_one_key('verify_batch_compressed', 'batch', vk, public_inputs, blobs, ctx, True, weights)
 
     @staticmethod
     def verify_batch_locate_compressed(vk, public_inputs, blobs, ctx: Context = None, weights=None) -> list:
         """verify_batch_locate on compressed proofs (b2g_verify_batch_locate_compressed), decoded on the device: a blob that
         does not decode is False, and the other verdicts are those of verify_batch_locate on the decoded proofs.  Arguments,
         weights and errors as verify_batch; a blob that is not 128 bytes raises ValueError."""
-        return _verify_batch('verify_batch_locate_compressed', vk, public_inputs, blobs, ctx, weights, True, True)
+        return _verify_one_key('verify_batch_locate_compressed', 'batch_locate', vk, public_inputs, blobs, ctx, True, weights)
 
     # base-range sharded variant: every rank calls prove_partial, the 768-byte partials are all-gathered by the caller
     # (torch.distributed / NCCL), then every rank calls prove_finish and obtains the same proof.

@@ -377,9 +377,8 @@ typedef Reduction<B2G_REDUCTION_LIBSNARK> LibsnarkReduction;   // ark-groth16's 
 #include "ark_circom_ethereum.hpp"
 namespace ark_circom {
 
-// what the Groth16 verifiers (verify_many, verify_batch and their compressed forms) share: the argument checks, the key
-// prepared on the device at first use (b2g_vk_load, kept in pvk.device) and the encoded public inputs and proofs (P = Proof,
-// 256-byte rows, or CompressedProof, 128-byte rows)
+// what the Groth16 verifiers share: the argument checks, the key prepared on the device at first use (b2g_vk_load, kept in
+// pvk.device) and the encoded public inputs and proofs (P = Proof, 256-byte rows, or CompressedProof, 128-byte rows)
 struct VerifyCall {
     size_t n = 0;
     Gpu* gpu = nullptr;
@@ -461,37 +460,57 @@ struct KeysTable {
     }
 };
 
-// verify_batch_keys and its compressed form: one b2g_verify_batch_keys call over the batches that hold proofs, true for
-// the others
+// the one-key verifiers' kinds
+enum class VerifyKind { many, batch, locate };
+
+// verify_many, verify_batch, verify_batch_locate and their compressed forms (P = Proof, or CompressedProof): one ABI call,
+// with weights from std::random_device when the kind takes them; the verdicts (one for batch, else one per proof), none
+// for an empty batch
 template <class P>
-inline std::vector<bool> verify_keys_call(const char* fn, const std::vector<KeyBatchOf<P>>& batches, int device) {
-    const KeysTable t(fn, batches, device);
-    std::vector<bool> out(batches.size(), true);
-    if (t.table.empty()) return out;
-    std::vector<uint8_t> verdicts(t.table.size());
-    b2g_ctx* ctx = Gpu::on(device).ctx();
-    check(sizeof(P) == 256 ? b2g_verify_batch_keys(ctx, (uint32_t)t.table.size(), t.table.data(), verdicts.data())
-                           : b2g_verify_batch_keys_compressed(ctx, (uint32_t)t.table.size(), t.table.data(), verdicts.data()));
-    for (size_t i = 0; i < t.at.size(); i++) out[t.at[i]] = verdicts[i] != 0;
-    return out;
+inline std::vector<bool> verify_one_key(const char* fn, VerifyKind kind, const PreparedVerifyingKey& pvk,
+                                        const std::vector<std::vector<Fr>>& public_inputs, const std::vector<P>& proofs, int device) {
+    VerifyCall c(fn, pvk, public_inputs, proofs, device);
+    if (c.n == 0) return {};
+    std::vector<uint8_t> verdicts(kind == VerifyKind::batch ? 1 : c.n);
+    b2g_ctx* ctx = c.gpu->ctx();
+    const void* pub = c.pub.empty() ? nullptr : c.pub.data();
+    const bool z = sizeof(P) == 128;
+    if (kind == VerifyKind::many) {
+        check((z ? b2g_verify_many_compressed : b2g_verify_many)(ctx, c.vk, (uint32_t)c.n, pub, c.bytes.data(), verdicts.data()));
+    } else {
+        const std::vector<uint32_t> w = batch_weights(c.n);
+        auto entry = kind == VerifyKind::batch ? (z ? b2g_verify_batch_compressed : b2g_verify_batch)
+                                               : (z ? b2g_verify_batch_locate_compressed : b2g_verify_batch_locate);
+        check(entry(ctx, c.vk, (uint32_t)c.n, pub, c.bytes.data(), w.data(), verdicts.data()));
+    }
+    return std::vector<bool>(verdicts.begin(), verdicts.end());
 }
 
-// verify_batch_keys_locate and its compressed form: one b2g_verify_batch_keys_locate call over the batches that hold proofs,
-// one verdict list per batch (empty for an empty batch)
+// verify_batch_keys, verify_batch_keys_locate and their compressed forms: one ABI call over the batches that hold proofs;
+// per batch its verdicts (one per proof when locate, else one), none for an empty batch
 template <class P>
-inline std::vector<std::vector<bool>> verify_keys_locate_call(const char* fn, const std::vector<KeyBatchOf<P>>& batches, int device) {
+inline std::vector<std::vector<bool>> verify_keys_call(const char* fn, const std::vector<KeyBatchOf<P>>& batches, bool locate, int device) {
     const KeysTable t(fn, batches, device);
     std::vector<std::vector<bool>> out(batches.size());
     if (t.table.empty()) return out;
-    std::vector<uint8_t> verdicts(t.total);
+    std::vector<uint8_t> verdicts(locate ? t.total : t.table.size());
     b2g_ctx* ctx = Gpu::on(device).ctx();
-    check(sizeof(P) == 256 ? b2g_verify_batch_keys_locate(ctx, (uint32_t)t.table.size(), t.table.data(), verdicts.data())
-                           : b2g_verify_batch_keys_locate_compressed(ctx, (uint32_t)t.table.size(), t.table.data(), verdicts.data()));
-    size_t v = 0;
-    for (size_t i = 0; i < t.at.size(); i++) {
-        out[t.at[i]].assign(verdicts.begin() + v, verdicts.begin() + v + t.table[i].count);
-        v += t.table[i].count;
+    const bool z = sizeof(P) == 128;
+    auto entry = locate ? (z ? b2g_verify_batch_keys_locate_compressed : b2g_verify_batch_keys_locate)
+                        : (z ? b2g_verify_batch_keys_compressed : b2g_verify_batch_keys);
+    check(entry(ctx, (uint32_t)t.table.size(), t.table.data(), verdicts.data()));
+    for (size_t i = 0, v = 0; i < t.at.size(); i++) {
+        const size_t m = locate ? t.table[i].count : 1;
+        out[t.at[i]].assign(verdicts.begin() + v, verdicts.begin() + v + m);
+        v += m;
     }
+    return out;
+}
+
+// one verdict per batch from verify_keys_call's lists: an empty batch is true
+inline std::vector<bool> batch_verdicts(const std::vector<std::vector<bool>>& lists) {
+    std::vector<bool> out;
+    for (const auto& l : lists) out.push_back(l.empty() || l[0]);
     return out;
 }
 
@@ -510,11 +529,7 @@ struct Groth16T {                                       // Groth16::<Bn254, QAP>
     // coordinate >= p: the host call throws SerializationError there, the batch reports the proof invalid.
     static std::vector<bool> verify_many(const PreparedVerifyingKey& pvk, const std::vector<std::vector<Fr>>& public_inputs,
                                          const std::vector<Proof>& proofs, int device = 0) {
-        VerifyCall c("verify_many", pvk, public_inputs, proofs, device);
-        if (c.n == 0) return {};
-        std::vector<uint8_t> verdicts(c.n);
-        check(b2g_verify_many(c.gpu->ctx(), c.vk, (uint32_t)c.n, c.pub.empty() ? nullptr : c.pub.data(), c.bytes.data(), verdicts.data()));
-        return std::vector<bool>(verdicts.begin(), verdicts.end());
+        return verify_one_key("verify_many", VerifyKind::many, pvk, public_inputs, proofs, device);
     }
     // whether ALL proofs are valid, from one random-linear-combination pairing check (b2g_verify_batch): true iff every
     // proof passes verify_many and every B lies in G2, except with probability <= 1 / (2^128 - 1).  The 128-bit weights
@@ -522,12 +537,8 @@ struct Groth16T {                                       // Groth16::<Bn254, QAP>
     // proofs.  An empty batch is true.
     static bool verify_batch(const PreparedVerifyingKey& pvk, const std::vector<std::vector<Fr>>& public_inputs,
                              const std::vector<Proof>& proofs, int device = 0) {
-        VerifyCall c("verify_batch", pvk, public_inputs, proofs, device);
-        if (c.n == 0) return true;
-        const std::vector<uint32_t> w = batch_weights(c.n);
-        uint8_t verdict = 0;
-        check(b2g_verify_batch(c.gpu->ctx(), c.vk, (uint32_t)c.n, c.pub.empty() ? nullptr : c.pub.data(), c.bytes.data(), w.data(), &verdict));
-        return verdict != 0;
+        const std::vector<bool> v = verify_one_key("verify_batch", VerifyKind::batch, pvk, public_inputs, proofs, device);
+        return v.empty() || v[0];
     }
     // one verdict per proof at about verify_batch's cost when few proofs are invalid (b2g_verify_batch_locate): the batch
     // check runs once per group of 64 proofs over the group's well-formed proofs, and the well-formed proofs of a failing
@@ -536,34 +547,29 @@ struct Groth16T {                                       // Groth16::<Bn254, QAP>
     // with probability <= (groups holding such a proof) / (2^128 - 1).  Weights from std::random_device, as verify_batch.
     static std::vector<bool> verify_batch_locate(const PreparedVerifyingKey& pvk, const std::vector<std::vector<Fr>>& public_inputs,
                                                  const std::vector<Proof>& proofs, int device = 0) {
-        VerifyCall c("verify_batch_locate", pvk, public_inputs, proofs, device);
-        if (c.n == 0) return {};
-        const std::vector<uint32_t> w = batch_weights(c.n);
-        std::vector<uint8_t> verdicts(c.n);
-        check(b2g_verify_batch_locate(c.gpu->ctx(), c.vk, (uint32_t)c.n, c.pub.empty() ? nullptr : c.pub.data(), c.bytes.data(), w.data(), verdicts.data()));
-        return std::vector<bool>(verdicts.begin(), verdicts.end());
+        return verify_one_key("verify_batch_locate", VerifyKind::locate, pvk, public_inputs, proofs, device);
     }
     // verify_batch for many keys in ONE device pass (b2g_verify_batch_keys): one verdict per batch, equal to verify_batch on
     // that batch with the same weights; an invalid proof changes its own batch's verdict only, and an empty batch is true.
     // Each key is prepared on the device at first use and kept in its pvk.device.  Weights from std::random_device.
     static std::vector<bool> verify_batch_keys(const std::vector<KeyBatch>& batches, int device = 0) {
-        return verify_keys_call("verify_batch_keys", batches, device);
+        return batch_verdicts(verify_keys_call("verify_batch_keys", batches, false, device));
     }
     // verify_batch_keys on compressed proofs, decoded on the device (b2g_verify_batch_keys_compressed): a batch with a proof
     // that does not decode is false, the others as verify_batch_keys on the decoded proofs
     static std::vector<bool> verify_batch_keys_compressed(const std::vector<CompressedKeyBatch>& batches, int device = 0) {
-        return verify_keys_call("verify_batch_keys_compressed", batches, device);
+        return batch_verdicts(verify_keys_call("verify_batch_keys_compressed", batches, false, device));
     }
     // verify_batch_locate for many keys in ONE device pass (b2g_verify_batch_keys_locate): one verdict list per batch, equal
     // to verify_batch_locate on that batch with the same weights (groups of 64 start at each batch's first proof); an empty
     // batch gives an empty list.  Weights from std::random_device.
     static std::vector<std::vector<bool>> verify_batch_keys_locate(const std::vector<KeyBatch>& batches, int device = 0) {
-        return verify_keys_locate_call("verify_batch_keys_locate", batches, device);
+        return verify_keys_call("verify_batch_keys_locate", batches, true, device);
     }
     // verify_batch_keys_locate on compressed proofs, decoded on the device (b2g_verify_batch_keys_locate_compressed): a proof
     // that does not decode is false, the others as verify_batch_keys_locate on the decoded proofs
     static std::vector<std::vector<bool>> verify_batch_keys_locate_compressed(const std::vector<CompressedKeyBatch>& batches, int device = 0) {
-        return verify_keys_locate_call("verify_batch_keys_locate_compressed", batches, device);
+        return verify_keys_call("verify_batch_keys_locate_compressed", batches, true, device);
     }
     // Proof::<Bn254>::deserialize_compressed (ark-serialize 0.5, Validate::Yes) for many proofs in one device pass
     // (b2g_proofs_decompress): an empty optional where arkworks would refuse the bytes (both flag bits set, a coordinate
@@ -582,34 +588,20 @@ struct Groth16T {                                       // Groth16::<Bn254, QAP>
     // the proof decodes (G2 check included) and the decoded proof passes verify_many
     static std::vector<bool> verify_many_compressed(const PreparedVerifyingKey& pvk, const std::vector<std::vector<Fr>>& public_inputs,
                                                     const std::vector<CompressedProof>& blobs, int device = 0) {
-        VerifyCall c("verify_many_compressed", pvk, public_inputs, blobs, device);
-        if (c.n == 0) return {};
-        std::vector<uint8_t> verdicts(c.n);
-        check(b2g_verify_many_compressed(c.gpu->ctx(), c.vk, (uint32_t)c.n, c.pub.empty() ? nullptr : c.pub.data(), c.bytes.data(), verdicts.data()));
-        return std::vector<bool>(verdicts.begin(), verdicts.end());
+        return verify_one_key("verify_many_compressed", VerifyKind::many, pvk, public_inputs, blobs, device);
     }
     // verify_batch on compressed proofs, decoded on the device (b2g_verify_batch_compressed): true exactly when every proof
     // decodes and verify_batch would be true on the decoded proofs with the same weights
     static bool verify_batch_compressed(const PreparedVerifyingKey& pvk, const std::vector<std::vector<Fr>>& public_inputs,
                                         const std::vector<CompressedProof>& blobs, int device = 0) {
-        VerifyCall c("verify_batch_compressed", pvk, public_inputs, blobs, device);
-        if (c.n == 0) return true;
-        const std::vector<uint32_t> w = batch_weights(c.n);
-        uint8_t verdict = 0;
-        check(b2g_verify_batch_compressed(c.gpu->ctx(), c.vk, (uint32_t)c.n, c.pub.empty() ? nullptr : c.pub.data(), c.bytes.data(), w.data(), &verdict));
-        return verdict != 0;
+        const std::vector<bool> v = verify_one_key("verify_batch_compressed", VerifyKind::batch, pvk, public_inputs, blobs, device);
+        return v.empty() || v[0];
     }
     // verify_batch_locate on compressed proofs, decoded on the device (b2g_verify_batch_locate_compressed): a proof that does
     // not decode is false, the others as verify_batch_locate on the decoded proofs
     static std::vector<bool> verify_batch_locate_compressed(const PreparedVerifyingKey& pvk, const std::vector<std::vector<Fr>>& public_inputs,
                                                             const std::vector<CompressedProof>& blobs, int device = 0) {
-        VerifyCall c("verify_batch_locate_compressed", pvk, public_inputs, blobs, device);
-        if (c.n == 0) return {};
-        const std::vector<uint32_t> w = batch_weights(c.n);
-        std::vector<uint8_t> verdicts(c.n);
-        check(b2g_verify_batch_locate_compressed(c.gpu->ctx(), c.vk, (uint32_t)c.n, c.pub.empty() ? nullptr : c.pub.data(), c.bytes.data(),
-                                                 w.data(), verdicts.data()));
-        return std::vector<bool>(verdicts.begin(), verdicts.end());
+        return verify_one_key("verify_batch_locate_compressed", VerifyKind::locate, pvk, public_inputs, blobs, device);
     }
     static Proof create_proof_with_reduction_and_matrices(const ProvingKey& pk, const Fr& r, const Fr& s, const ConstraintMatrices& matrices,
                                                           size_t num_inputs, size_t num_constraints, const std::vector<Fr>& full_assignment,

@@ -271,12 +271,16 @@ def test_errors_leave_the_context_usable(ctx, golden, test_zkey_bytes):
         pub_r = (C.c_uint8 * 128).from_buffer_copy(R.to_bytes(32, 'little') + bytes(96))
         out = (C.c_uint8 * 2)()
         assert entry(ctx._h, h, 2, pub, buf, w0, out) == -4                      # a zero weight
+        assert L.b2g_last_error() == b'weight 1 is zero'
         assert entry(ctx._h, h, 2, pub_r, buf, w, out) == -4                     # an input >= r
+        assert L.b2g_last_error() == b'public input 0 of proof 0 is not below the scalar field modulus r'
         assert entry(ctx._h, h, 0, pub, buf, w, out) == -2
-        for args in ((None, buf, w, out), (pub, None, w, out), (pub, buf, None, out), (pub, buf, w, None)):
-            assert entry(ctx._h, h, 2, *args) == -2
-        assert entry(None, h, 2, pub, buf, w, out) == -2
-        assert entry(ctx._h, None, 2, pub, buf, w, out) == -2
+        assert L.b2g_last_error() == entry.__name__.encode() + b': count must be at least 1'
+        for args in ((ctx._h, h, 0, pub, None, w, out), (ctx._h, h, 2, None, buf, w, out), (ctx._h, h, 2, pub, None, w, out),
+                     (ctx._h, h, 2, pub, buf, None, out), (ctx._h, h, 2, pub, buf, w, None), (None, h, 2, pub, buf, w, out),
+                     (ctx._h, None, 2, pub, buf, w, out)):
+            assert entry(*args) == -2
+            assert L.b2g_last_error() == b'null pointer'
         assert entry(ctx._h, h, 2, pub, buf, w, out) == 0 and list(out) == [1, 1]
     # a proof pending on the context
     pk, cm = read_zkey(test_zkey_bytes)
@@ -286,6 +290,7 @@ def test_errors_leave_the_context_usable(ctx, golden, test_zkey_bytes):
     with pytest.raises(B2gError) as e:
         Groth16.verify_batch_locate(vk, inputs, proofs, ctx)
     assert e.value.code == -2
+    assert e.value.msg == 'a submitted proof is still pending on this context: call b2g_prove_wait first'
     assert pending.wait().data.hex() == case['proof_hex']
     release(vk); release(pk); release(cm)
 

@@ -316,20 +316,31 @@ def test_errors_leave_the_context_usable(ctx, golden, test_zkey_bytes):
     w = (C.c_uint8 * 32).from_buffer_copy((5).to_bytes(16, 'little') + (7).to_bytes(16, 'little'))
     w0 = (C.c_uint8 * 32).from_buffer_copy((5).to_bytes(16, 'little') + bytes(16))
     rows, ok, out = (C.c_uint8 * 512)(), (C.c_uint8 * 2)(), (C.c_uint8 * 2)()
+    pub_r_text = b'public input 0 of proof 0 is not below the scalar field modulus r'
     assert L.b2g_proofs_decompress(ctx._h, 0, buf, rows, ok) == -2
+    assert L.b2g_last_error() == b'b2g_proofs_decompress: count must be at least 1'
     for args in ((None, rows, ok), (buf, None, ok), (buf, rows, None)):
         assert L.b2g_proofs_decompress(ctx._h, 2, *args) == -2
+        assert L.b2g_last_error() == b'null pointer'
     assert L.b2g_proofs_decompress(None, 2, buf, rows, ok) == -2
+    assert L.b2g_last_error() == b'null pointer'
     assert L.b2g_verify_many_compressed(ctx._h, h, 0, pub, buf, out) == -2
+    assert L.b2g_last_error() == b'b2g_verify_many_compressed: count must be at least 1'
     assert L.b2g_verify_many_compressed(ctx._h, h, 2, pub_r, buf, out) == -4
-    for args in ((None, buf, out), (pub, None, out), (pub, buf, None)):
-        assert L.b2g_verify_many_compressed(ctx._h, h, 2, *args) == -2
-    assert L.b2g_verify_many_compressed(ctx._h, None, 2, pub, buf, out) == -2
+    assert L.b2g_last_error() == pub_r_text
+    for args in ((h, 0, pub, None, out), (h, 2, None, buf, out), (h, 2, pub, None, out), (h, 2, pub, buf, None), (None, 2, pub, buf, out)):
+        assert L.b2g_verify_many_compressed(ctx._h, *args) == -2
+        assert L.b2g_last_error() == b'null pointer'
     assert L.b2g_verify_batch_compressed(ctx._h, h, 2, pub, buf, w0, out) == -4
+    assert L.b2g_last_error() == b'weight 1 is zero'
     assert L.b2g_verify_batch_compressed(ctx._h, h, 2, pub_r, buf, w, out) == -4
+    assert L.b2g_last_error() == pub_r_text
     assert L.b2g_verify_batch_compressed(ctx._h, h, 0, pub, buf, w, out) == -2
-    for args in ((None, buf, w, out), (pub, None, w, out), (pub, buf, None, out), (pub, buf, w, None)):
-        assert L.b2g_verify_batch_compressed(ctx._h, h, 2, *args) == -2
+    assert L.b2g_last_error() == b'b2g_verify_batch_compressed: count must be at least 1'
+    for args in ((h, 0, pub, None, w, out), (h, 2, None, buf, w, out), (h, 2, pub, None, w, out), (h, 2, pub, buf, None, out),
+                 (h, 2, pub, buf, w, None)):
+        assert L.b2g_verify_batch_compressed(ctx._h, *args) == -2
+        assert L.b2g_last_error() == b'null pointer'
     assert L.b2g_proofs_decompress(ctx._h, 2, buf, rows, ok) == 0 and list(ok) == [1, 1]
     assert bytes(rows) == proofs[0].data + proofs[1].data
     assert L.b2g_verify_many_compressed(ctx._h, h, 2, pub, buf, out) == 0 and list(out) == [1, 1]
@@ -344,6 +355,7 @@ def test_errors_leave_the_context_usable(ctx, golden, test_zkey_bytes):
         with pytest.raises(B2gError) as e:
             call()
         assert e.value.code == -2
+        assert e.value.msg == 'a submitted proof is still pending on this context: call b2g_prove_wait first'
     assert pending.wait().data.hex() == case['proof_hex']
     for k in (5, 1, 5):
         assert [p.data for p in Groth16.decompress_proofs(blobs[:k], ctx)] == [p.data for p in proofs[:k]]

@@ -281,14 +281,15 @@ def test_errors_leave_the_context_usable(ctx):
     pub_r = (C.c_uint8 * 64).from_buffer_copy(R.to_bytes(32, 'little') + (1).to_bytes(32, 'little'))
     buf1 = (C.c_uint8 * 256).from_buffer_copy(proofs[0].data)
     assert L.b2g_verify_many(ctx._h, h, 1, pub_r, buf1, (C.c_uint8 * 1)()) == -4      # >= r refused by the library itself
+    assert L.b2g_last_error() == b'public input 0 of proof 0 is not below the scalar field modulus r'
     buf = (C.c_uint8 * 256)()
     out = (C.c_uint8 * 8)()
     pub = (C.c_uint8 * 64)()
     assert L.b2g_verify_many(ctx._h, h, 0, pub, buf, out) == -2
-    assert L.b2g_verify_many(ctx._h, h, 1, None, buf, out) == -2
-    assert L.b2g_verify_many(ctx._h, h, 1, pub, None, out) == -2
-    assert L.b2g_verify_many(ctx._h, None, 1, pub, buf, out) == -2
-    assert L.b2g_verify_many(ctx._h, h, 1, pub, buf, None) == -2
+    assert L.b2g_last_error() == b'b2g_verify_many: count must be at least 1'
+    for args in ((h, 0, pub, None, out), (h, 1, None, buf, out), (h, 1, pub, None, out), (None, 1, pub, buf, out), (h, 1, pub, buf, None)):
+        assert L.b2g_verify_many(ctx._h, *args) == -2
+        assert L.b2g_last_error() == b'null pointer'
     tampered = [_proof(p.a, p.b, o.G1.add(p.c, o.G1_GEN)) for p in proofs]
     for k in (5, 1, 5):
         assert Groth16.verify_many(vk, inputs[:k], proofs[:k], ctx) == [True] * k
