@@ -53,7 +53,8 @@ EXPORTS = ['b2g_last_error', 'b2g_version', 'b2g_device_count', 'b2g_ctx_create'
            'b2g_bench_device', 'b2g_bench_msm', 'b2g_launch_count', 'b2g_vk_load', 'b2g_vk_free', 'b2g_vk_alpha_beta', 'b2g_verify_many',
            'b2g_verify_batch', 'b2g_proofs_decompress', 'b2g_verify_many_compressed', 'b2g_verify_batch_compressed',
            'b2g_verify_batch_locate', 'b2g_verify_batch_locate_compressed', 'b2g_verify_batch_keys',
-           'b2g_verify_batch_keys_compressed', 'b2g_verify_batch_keys_locate', 'b2g_verify_batch_keys_locate_compressed']
+           'b2g_verify_batch_keys_compressed', 'b2g_verify_batch_keys_locate', 'b2g_verify_batch_keys_locate_compressed',
+           'b2g_rerandomize_many']
 
 _lib = None
 
@@ -115,6 +116,7 @@ def lib():
         L.b2g_verify_batch_keys_compressed.argtypes = [vp, C.c_uint32, C.POINTER(KeyBatch), vp]
         L.b2g_verify_batch_keys_locate.argtypes = [vp, C.c_uint32, C.POINTER(KeyBatch), vp]
         L.b2g_verify_batch_keys_locate_compressed.argtypes = [vp, C.c_uint32, C.POINTER(KeyBatch), vp]
+        L.b2g_rerandomize_many.argtypes = [vp, vp, C.c_uint32, vp, vp, vp, vp, vp]
         _lib = L
     return _lib
 

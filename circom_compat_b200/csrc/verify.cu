@@ -35,6 +35,8 @@
 // b2g_proofs_decompress and the _compressed verifiers take arkworks' 128-byte compressed proofs: a decode kernel (one proof
 // per thread) writes the 256-byte rows the kernels above read, and a second kernel checks that each decoded B lies in G2 (the
 // batch check leaves that to batch_g2_kernel).  The decoding rules are restated above decompress_kernel.
+// b2g_rerandomize_many (ark-groth16's rerandomize_proof) parses rows with the verifiers' proof_parse and runs one kernel, one
+// proof per thread: rerandomize_kernel.
 #include <algorithm>
 #include <cstring>
 #include <string>
@@ -590,6 +592,57 @@ __global__ void decompress_test_kernel(int op, const uint8_t* __restrict__ a, ui
     fe_store(o, flag);
 }
 
+// ---------------------------------------------------------------------------------------------- rerandomization
+// b2g_rerandomize_many: ark-groth16 0.5.0's Groth16::rerandomize_proof for a proof (A, B, C) and nonzero factors r1, r2:
+//     A' = r1^-1 A,   B' = r1 B + (r1 r2) delta_2,   C' = C + r2 A
+// A scalar below r has at most RERAND_BITS bits.
+constexpr int RERAND_BITS = 254;
+
+// k1 b + k2 d for scalars below r (canonical): one doubling chain over both scalars (Shamir's trick), each step adding b, d
+// or b + d, all three affine so that every addition is a mixed one; every exceptional case is left to madd
+__device__ __noinline__ G2::Pt g2_joint_mul(const G2::Aff& b, const G2::Aff& d, const uint32_t* k1, const uint32_t* k2) {
+    G2::Pt t = G2::from_affine(b);
+    G2::madd(t, d);
+    const G2::Aff bd = G2::to_affine(t);
+    G2::Pt acc = G2::infinity();
+    #pragma unroll 1
+    for (int i = RERAND_BITS - 1; i >= 0; i--) {
+        acc = G2::dbl(acc);
+        const uint32_t u = (k1[i >> 5] >> (i & 31)) & 1u, v = (k2[i >> 5] >> (i & 31)) & 1u;
+        if (u & v) G2::madd(acc, bd);
+        else if (u) G2::madd(acc, b);
+        else if (v) G2::madd(acc, d);
+    }
+    return acc;
+}
+
+// one proof per thread: row j of proofs (b2g_prove layout) with the factors r1[j], r2[j] (canonical, nonzero, below r: the
+// host checks them) -> the canonical rerandomized row j of out and ok[j] = 1, or the 0xFF row and ok[j] = 0 when row j does
+// not parse (a coordinate >= p or a point off its curve: proof_parse, the rule of b2g_verify_many).  delta = delta_2 (affine
+// Montgomery, zeros = infinity).  No G2 subgroup check, as in arkworks.
+__global__ void __launch_bounds__(64) rerandomize_kernel(const uint8_t* __restrict__ proofs, const uint8_t* __restrict__ r1s,
+                                                         const uint8_t* __restrict__ r2s, const uint8_t* __restrict__ delta,
+                                                         uint32_t count, uint8_t* __restrict__ out, uint8_t* __restrict__ ok) {
+    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= count) return;
+    G1::Aff a, cc; G2::Aff b;
+    const bool good = proof_parse(proofs + (size_t)j * 256, a, b, cc);
+    ok[j] = good;
+    if (!good) { coords_store(out + (size_t)j * 256, nullptr, 8, false); return; }
+    const fe r1 = fe_load(r1s + (size_t)j * 32), r2 = fe_load(r2s + (size_t)j * 32);
+    const fe r1m = Fr::from_canonical(r1);
+    const fe r1_inv = Fr::to_canonical(Fr::inv(r1m));
+    const fe r12 = Fr::mul(r1m, r2);                     // r1 R r2 / R: canonical r1 r2 mod r
+    const G1::Aff a2 = G1::to_affine(G1::mul_affine(a, r1_inv.l, 8));
+    G1::Pt c2 = G1::mul_affine(a, r2.l, 8);
+    G1::madd(c2, cc);
+    const G2::Aff b2 = G2::to_affine(g2_joint_mul(b, aff_load<Fq2>(delta, 0), r1.l, r12.l));
+    const G1::Aff c2a = G1::to_affine(c2);
+    fe c[8] = {a2.x, a2.y, b2.x.c0, b2.x.c1, b2.y.c0, b2.y.c1, c2a.x, c2a.y};
+    for (int k = 0; k < 8; k++) c[k] = Fq::to_canonical(c[k]);
+    coords_store(out + (size_t)j * 256, c, 8, true);
+}
+
 // lines of -gamma (thread 0) and -delta (thread 1) for every loop step, in the order miller_loop reads them
 __global__ void vk_lines_kernel(const uint8_t* __restrict__ g2, uint8_t* __restrict__ lines) {
     const int t = threadIdx.x;
@@ -989,6 +1042,40 @@ int b2g_proofs_decompress(b2g_ctx* ctx, uint32_t count, const void* compressed, 
         CUDA_CHECK(cudaGetLastError());
         CUDA_CHECK(cudaMemcpyAsync(proofs_out, v.d_proofs, (size_t)count * 256, cudaMemcpyDeviceToHost, st));
         CUDA_CHECK(cudaMemcpyAsync(ok_out, ok, count, cudaMemcpyDeviceToHost, st));
+        CUDA_CHECK(cudaStreamSynchronize(st));
+    });
+}
+
+int b2g_rerandomize_many(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* proofs, const void* r1_canon, const void* r2_canon,
+                         uint8_t* proofs_out, uint8_t* ok_out) {
+    return guarded([&] {
+        static const char* fn = "b2g_rerandomize_many";
+        if (!ctx || !vk || !proofs || !r1_canon || !r2_canon || !proofs_out || !ok_out) throw_error(B2G_E_SHAPE, "null pointer");
+        const CtxView cv = batch_args(fn, ctx, count);
+        if (vk->device != cv.device) throw_error(B2G_E_SHAPE, "the verifying key belongs to another device");
+        DevGuard g(cv.device);
+        cudaStream_t st = cv.st;
+        // the buffers before the factors: a count whose buffers cannot fit is refused without reading count factors
+        verify_bufs_ensure(fn, *cv.vbufs, count, 0, 0);
+        VerifyBufs& v = **cv.vbufs;
+        for (uint32_t i = 0; i < count; i++)
+            for (const auto& [name, r] : {std::pair{"r1", r1_canon}, std::pair{"r2", r2_canon}}) {
+                const uint32_t* k = (const uint32_t*)r + 8 * (size_t)i;
+                if (all_zero(k, 32) || !below_r(k))
+                    throw_error(B2G_E_INPUT, std::string(fn) + ": factor " + name + " of proof " + std::to_string(i) +
+                                             " is not in [1, r)");
+            }
+        // the factors and the output rows share the record area
+        static_assert(REC_BYTES_V >= 2 * 32 + 256, "r1, r2 and the output row fit in a proof's record");
+        uint8_t *d_r1 = v.d_rec, *d_r2 = v.d_rec + (size_t)count * 32, *d_out = v.d_rec + (size_t)count * 64;
+        CUDA_CHECK(cudaMemcpyAsync(v.d_proofs, proofs, (size_t)count * 256, cudaMemcpyHostToDevice, st));
+        CUDA_CHECK(cudaMemcpyAsync(d_r1, r1_canon, (size_t)count * 32, cudaMemcpyHostToDevice, st));
+        CUDA_CHECK(cudaMemcpyAsync(d_r2, r2_canon, (size_t)count * 32, cudaMemcpyHostToDevice, st));
+        rerandomize_kernel<<<(count + 63) / 64, 64, 0, st>>>(v.d_proofs, d_r1, d_r2, vk->d_g2 + 2 * 128, count, d_out, v.d_verdict);
+        g_launch_count += 1;
+        CUDA_CHECK(cudaGetLastError());
+        CUDA_CHECK(cudaMemcpyAsync(proofs_out, d_out, (size_t)count * 256, cudaMemcpyDeviceToHost, st));
+        CUDA_CHECK(cudaMemcpyAsync(ok_out, v.d_verdict, count, cudaMemcpyDeviceToHost, st));
         CUDA_CHECK(cudaStreamSynchronize(st));
     });
 }

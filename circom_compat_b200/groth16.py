@@ -24,6 +24,8 @@
         <- Proof::<Bn254>::deserialize_compressed (ark-serialize 0.5, Validate::Yes) for many 128-byte proofs, on the device.
     Groth16.verify_many_compressed / verify_batch_compressed(vk, public_inputs, blobs)
         <- deserialize_compressed followed by verify_many / verify_batch, decoded on the device.
+    Groth16.rerandomize_proof(vk, proof, rng) / Groth16.rerandomize_proofs(vk, proofs)
+        <- Groth16::rerandomize_proof (ark-groth16 0.5.0), for one or many proofs of one key in one device pass.
 Arguments keep the reference's meaning; field elements are (n, 4) uint64 Montgomery limb arrays (fr_to_mont).
 """
 from __future__ import annotations
@@ -451,6 +453,16 @@ def fr_rand(rng) -> int:
 _R_INV_R = pow(1 << 256, -1, R_MOD)
 
 
+def _rerandomize_factors(rng) -> tuple:
+    """(r1, r2) as Groth16::rerandomize_proof (ark-groth16 0.5.0) draws them: r1 = Fr::rand, then r2 = Fr::rand (fr_rand),
+    both drawn again while either is zero"""
+    r1 = r2 = 0
+    while r1 == 0 or r2 == 0:
+        r1 = fr_rand(rng)
+        r2 = fr_rand(rng)
+    return r1, r2
+
+
 def _mont_points(points, g2: bool) -> np.ndarray:
     """canonical affine points (None = infinity) -> rows of Montgomery words, all-zero = infinity"""
     from .zkey import Q_MOD
@@ -681,6 +693,55 @@ class Groth16:
         does not decode is False, and the other verdicts are those of verify_batch_locate on the decoded proofs.  Arguments,
         weights and errors as verify_batch; a blob that is not 128 bytes raises ValueError."""
         return _verify_one_key('verify_batch_locate_compressed', 'batch_locate', vk, public_inputs, blobs, ctx, True, weights)
+
+    # ---- rerandomization: Groth16::rerandomize_proof (ark-groth16 0.5.0), on the device (b2g_rerandomize_many)
+    @staticmethod
+    def rerandomize_proof(vk, proof: Proof, rng, ctx: Context = None) -> Proof:
+        """Groth16::rerandomize_proof(vk, proof, rng): a new proof of the same statement, statistically indistinguishable
+        from a fresh honest proof and unlinkable to `proof`; no witness is needed.  The factors are drawn as arkworks draws
+        them (r1 = Fr::rand, r2 = Fr::rand, both again while either is zero, with fr_rand's limb rule), then
+            A' = r1^-1 A,  B' = r1 B + (r1 r2) delta_2,  C' = C + r2 A.
+        `vk` is a VerifyingKey, PreparedVerifyingKey or ProvingKey (prepared on the device once and cached per object, as for
+        verify_many).  Raises ValueError when the proof is malformed (a coordinate >= p or a point off its curve); B is not
+        checked for membership in G2, as in arkworks."""
+        out = Groth16.rerandomize_proofs(vk, [proof], ctx=ctx, factors=[_rerandomize_factors(rng)])[0]
+        if out is None:
+            raise ValueError("rerandomize_proof: the proof is malformed (a coordinate >= p or a point off its curve)")
+        return out
+
+    @staticmethod
+    def rerandomize_proofs(vk, proofs, rng=None, ctx: Context = None, factors=None) -> list:
+        """rerandomize_proof for many proofs of one key in ONE device pass (b2g_rerandomize_many).  Proof i's factors are
+        drawn from `rng` in order, as rerandomize_proof called on each proof in turn would draw them; the default rng is
+        secrets.SystemRandom().  `factors` = one (r1, r2) per proof, each in [1, r), replaces the draw (a factor out of
+        range raises B2gError, B2G_E_INPUT).  Returns [Proof | None]: None in place of a malformed proof, whose neighbours
+        are unaffected."""
+        proofs = list(proofs)
+        for p in proofs:
+            if len(p.data) != 256:
+                raise ValueError("rerandomize_proofs: a proof is 256 bytes")
+        if factors is None:
+            import secrets
+            rng = rng or secrets.SystemRandom()
+            factors = [_rerandomize_factors(rng) for _ in proofs]
+        factors = [(int(r1), int(r2)) for r1, r2 in factors]
+        if len(factors) != len(proofs):
+            raise ValueError("rerandomize_proofs: one (r1, r2) per proof")
+        for i, pair in enumerate(factors):
+            for name, f in zip(('r1', 'r2'), pair):
+                if not 0 < f < R_MOD:
+                    raise N.B2gError(N.B2G_E_INPUT, f"factor {name} of proof {i} is not in [1, r)")
+        if not proofs:
+            return []
+        ctx = ctx or default_context()
+        vh = ctx.vk_handle(vk)
+        rows = np.frombuffer(b''.join(p.data for p in proofs), dtype=np.uint8).copy()
+        r1 = np.frombuffer(b''.join(f.to_bytes(32, 'little') for f, _ in factors), dtype=np.uint8).copy()
+        r2 = np.frombuffer(b''.join(f.to_bytes(32, 'little') for _, f in factors), dtype=np.uint8).copy()
+        out = np.zeros((len(proofs), 256), dtype=np.uint8)
+        ok = np.zeros(len(proofs), dtype=np.uint8)
+        N.check(N.lib().b2g_rerandomize_many(ctx._h, vh, len(proofs), _ptr(rows), _ptr(r1), _ptr(r2), _ptr(out), _ptr(ok)))
+        return [Proof(row.tobytes()) if k else None for row, k in zip(out, ok)]
 
     # base-range sharded variant: every rank calls prove_partial, the 768-byte partials are all-gathered by the caller
     # (torch.distributed / NCCL), then every rank calls prove_finish and obtains the same proof.

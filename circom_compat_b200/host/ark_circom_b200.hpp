@@ -19,6 +19,8 @@
 //                             verdict per proof
 //   ark_circom::Groth16::verify_batch_locate (+ _compressed) <- verify_with_processed_vk for every proof, at about the batch
 //                                              check's cost when few proofs are invalid
+//   ark_circom::Groth16::rerandomize_proof / rerandomize_many <- Groth16::rerandomize_proof (ark-groth16 0.5.0), many
+//                                              proofs of one key in one device pass
 //   ark_circom::serialize_compressed          <- Proof::<Bn254>::serialize_compressed (ark_circom_ethereum.hpp)
 //   ark_circom::read_wtns                              <- snarkjs .wtns (test-vectors/circuit2_js/witness.wtns; the reference
 //                                                         computes witnesses with WASM instead, out of scope here)
@@ -377,8 +379,21 @@ typedef Reduction<B2G_REDUCTION_LIBSNARK> LibsnarkReduction;   // ark-groth16's 
 #include "ark_circom_ethereum.hpp"
 namespace ark_circom {
 
-// what the Groth16 verifiers share: the argument checks, the key prepared on the device at first use (b2g_vk_load, kept in
-// pvk.device) and the encoded public inputs and proofs (P = Proof, 256-byte rows, or CompressedProof, 128-byte rows)
+// the key prepared on the device at first use (b2g_vk_load), kept in pvk.device
+inline b2g_vk* device_vk(const PreparedVerifyingKey& pvk, Gpu& gpu) {
+    if (void* h = pvk.device.find(gpu.ctx(), 0)) return (b2g_vk*)h;
+    b2g_vk_desc d; memset(&d, 0, sizeof d);
+    d.n_public = (uint32_t)(pvk.vk.gamma_abc_g1.size() - 1);
+    d.alpha_g1 = &pvk.vk.alpha_g1; d.beta_g2 = &pvk.vk.beta_g2; d.gamma_g2 = &pvk.vk.gamma_g2; d.delta_g2 = &pvk.vk.delta_g2;
+    d.gamma_abc_g1 = pvk.vk.gamma_abc_g1.data();
+    b2g_vk* vk = nullptr;
+    check(b2g_vk_load(gpu.ctx(), &d, &vk));
+    pvk.device.put(gpu.ctx(), 0, vk, [](void* p) { b2g_vk_free((b2g_vk*)p); });
+    return vk;
+}
+
+// what the Groth16 verifiers share: the argument checks, the key on the device (device_vk) and the encoded public inputs
+// and proofs (P = Proof, 256-byte rows, or CompressedProof, 128-byte rows)
 struct VerifyCall {
     size_t n = 0;
     Gpu* gpu = nullptr;
@@ -395,15 +410,7 @@ struct VerifyCall {
         for (const auto& xs : public_inputs) if (xs.size() != n_public) throw MalformedVerifyingKey();
         n = proofs.size();
         gpu = &Gpu::on(device);
-        vk = (b2g_vk*)pvk.device.find(gpu->ctx(), 0);
-        if (!vk) {
-            b2g_vk_desc d; memset(&d, 0, sizeof d);
-            d.n_public = (uint32_t)n_public;
-            d.alpha_g1 = &pvk.vk.alpha_g1; d.beta_g2 = &pvk.vk.beta_g2; d.gamma_g2 = &pvk.vk.gamma_g2; d.delta_g2 = &pvk.vk.delta_g2;
-            d.gamma_abc_g1 = pvk.vk.gamma_abc_g1.data();
-            check(b2g_vk_load(gpu->ctx(), &d, &vk));
-            pvk.device.put(gpu->ctx(), 0, vk, [](void* p) { b2g_vk_free((b2g_vk*)p); });
-        }
+        vk = device_vk(pvk, *gpu);
         pub.resize(n * n_public);
         for (size_t i = 0; i < n; i++) for (size_t k = 0; k < n_public; k++) pub[i * n_public + k] = public_inputs[i][k].into_bigint();
         bytes.resize(n * sizeof(P));
@@ -602,6 +609,37 @@ struct Groth16T {                                       // Groth16::<Bn254, QAP>
     static std::vector<bool> verify_batch_locate_compressed(const PreparedVerifyingKey& pvk, const std::vector<std::vector<Fr>>& public_inputs,
                                                             const std::vector<CompressedProof>& blobs, int device = 0) {
         return verify_one_key("verify_batch_locate_compressed", VerifyKind::locate, pvk, public_inputs, blobs, device);
+    }
+    // Groth16::rerandomize_proof (ark-groth16 0.5.0) for many proofs of one key in ONE device pass (b2g_rerandomize_many): a
+    // new proof of the same statement per proof, unlinkable to it, with no witness.  Proof i's factors are drawn from rng as
+    // rerandomize_proof called on each proof in turn draws them.  An empty optional in place of a malformed proof (a
+    // coordinate >= p or a point off its curve); B is not checked for membership in G2, as in arkworks.
+    template <class Rng>
+    static std::vector<std::optional<Proof>> rerandomize_many(const PreparedVerifyingKey& pvk, const std::vector<Proof>& proofs, Rng& rng,
+                                                              int device = 0) {
+        if (proofs.empty()) return {};
+        Gpu& gpu = Gpu::on(device);
+        const size_t n = proofs.size();
+        std::vector<BigInt256> r1(n), r2(n);
+        for (size_t i = 0; i < n; i++) {
+            Fr a, b;
+            while (a.is_zero() || b.is_zero()) { a = Fr::rand(rng); b = Fr::rand(rng); }   // r1, then r2, again while either is 0
+            r1[i] = a.into_bigint(); r2[i] = b.into_bigint();
+        }
+        std::vector<Proof> rows(n);
+        std::vector<uint8_t> ok(n);
+        check(b2g_rerandomize_many(gpu.ctx(), device_vk(pvk, gpu), (uint32_t)n, proofs.data(), r1.data(), r2.data(), rows[0].bytes, ok.data()));
+        std::vector<std::optional<Proof>> out(n);
+        for (size_t i = 0; i < n; i++) if (ok[i]) out[i] = rows[i];
+        return out;
+    }
+    // Groth16::rerandomize_proof(vk, proof, rng): A' = r1^-1 A, B' = r1 B + (r1 r2) delta_2, C' = C + r2 A with r1, r2 drawn
+    // as arkworks draws them; throws SerializationError for a malformed proof
+    template <class Rng>
+    static Proof rerandomize_proof(const PreparedVerifyingKey& pvk, const Proof& proof, Rng& rng, int device = 0) {
+        const std::optional<Proof> p = rerandomize_many(pvk, std::vector<Proof>{proof}, rng, device)[0];
+        if (!p) throw SerializationError("rerandomize_proof: the proof is malformed (a coordinate >= p or a point off its curve)");
+        return *p;
     }
     static Proof create_proof_with_reduction_and_matrices(const ProvingKey& pk, const Fr& r, const Fr& s, const ConstraintMatrices& matrices,
                                                           size_t num_inputs, size_t num_constraints, const std::vector<Fr>& full_assignment,

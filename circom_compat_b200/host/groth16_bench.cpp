@@ -23,6 +23,8 @@
 //       the first, negate A in the first proof of the first batch, the last proof of the others and proofs 63 and 64 of each
 //       batch that has them, and compare Groth16::verify_batch_keys_locate's verdicts with the host verifier per proof
 //       (timing the keyed locate call)
+//       B2G_RERANDOMIZE=K: also prove K proofs, rerandomize them with Groth16::rerandomize_many (factors from std::mt19937_64
+//       seeded with 0x5EED), print every input and output row in hex, and check the outputs with the host verifier
 //       chain:<a> = the witness of the reference's squaring-chain bench family for input a
 //       (test-vectors/complex-circuit/input.json has a = 3), computed on the host instead of by WASM.
 #include <algorithm>
@@ -459,6 +461,33 @@ int main(int argc, char** argv) {
             }
             std::printf("verify_keys_locate %d proofs in %d batches (%d valid, %d tampered): agree=%d, device %.3f ms/call (%.1f proofs/s)\n",
                         k, (int)nb + 1, valid, tampered, agree, dev_ms, k / (dev_ms / 1e3));
+        }
+        if (const char* rr = std::getenv("B2G_RERANDOMIZE")) {           // rerandomized proofs, rows printed for the Python mirror
+            const int k = std::atoi(rr);
+            if (k < 1) throw SynthesisError("B2G_RERANDOMIZE must be >= 1");
+            std::vector<std::vector<Fr>> wv((size_t)k, full_assignment);
+            if (wsrc.rfind("chain:", 0) == 0)
+                for (int i = 1; i < k; i++) wv[(size_t)i] = chain_witness(params.a_query.size(), std::stoull(wsrc.substr(6)) + (unsigned long long)i);
+            std::vector<const std::vector<Fr>*> ws;
+            for (const auto& w : wv) ws.push_back(&w);
+            std::mt19937_64 prng(0x4E4D);
+            std::vector<std::pair<Fr, Fr>> rs;
+            for (int i = 0; i < k; i++) rs.push_back({Fr::rand(prng), Fr::rand(prng)});
+            const std::vector<Proof> proofs = Groth16::create_proofs(params, matrices, rs, ws);
+            auto pvk = Groth16::process_vk(params.vk);
+            std::mt19937_64 rng(0x5EED);
+            auto t1 = std::chrono::steady_clock::now();
+            const std::vector<std::optional<Proof>> out = Groth16::rerandomize_many(pvk, proofs, rng);   // includes the key load
+            const double dev_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t1).count();
+            int valid = 0, changed = 0;
+            for (int i = 0; i < k; i++) {
+                const Proof& q = *out[(size_t)i];
+                std::printf("rerand_in[%d]=%s\nrerand[%d]=%s\n", i, proofs[(size_t)i].hex().c_str(), i, q.hex().c_str());
+                const std::vector<Fr> inputs(wv[(size_t)i].begin() + 1, wv[(size_t)i].begin() + num_inputs);
+                valid += Groth16::verify_with_processed_vk(pvk, inputs, q);
+                changed += memcmp(q.bytes, proofs[(size_t)i].bytes, 256) != 0;
+            }
+            std::printf("rerandomize %d proofs: valid=%d changed=%d, device %.3f ms/call (with the key load)\n", k, valid, changed, dev_ms);
         }
         return 0;
     } catch (const std::exception& e) {

@@ -25,6 +25,7 @@
  *   b2g_verify_batch_keys (+ _compressed) <- b2g_verify_batch for many keys, one verdict per key, in one device pass
  *   b2g_verify_batch_keys_locate (+ _compressed) <- b2g_verify_batch_locate for many keys, one verdict per proof, in one
  *                             device pass
+ *   b2g_rerandomize_many   <- Groth16::rerandomize_proof (ark-groth16 0.5.0) for many proofs of one key, in one device pass
  *   b2g_fixed_base_g1/g2  <- the batch fixed-base multiplications of generate_random_parameters_with_reduction
  *                             (tests/groth16.rs:25); used to manufacture synthetic proving keys
  *
@@ -355,6 +356,27 @@ B2G_API int b2g_verify_batch_keys_locate(b2g_ctx* ctx, uint32_t n_keys, const b2
  * b2g_verify_batch_locate_compressed on batch k alone. */
 B2G_API int b2g_verify_batch_keys_locate_compressed(b2g_ctx* ctx, uint32_t n_keys, const b2g_key_batch* batches,
                                                     uint8_t* verdicts_out);
+
+/* b2g_rerandomize_many <- Groth16::rerandomize_proof(vk, proof, rng) (ark-groth16 0.5.0, src/prover.rs) for count proofs in one
+ * device pass, for callers that hand stored proofs out again (relayers, credential services): each output is a proof of the
+ * same statement, statistically indistinguishable from a fresh honest proof and unlinkable to its input (BKSV20, eprint
+ * 2020/811, theorem 3).  No witness is needed.  For proof i = (A, B, C) and its factors r1 = r1_canon[i], r2 = r2_canon[i]:
+ *     A' = r1^-1 A,   B' = r1 B + (r1 r2) delta_2,   C' = C + r2 A       (delta_2 = the key's delta_g2, r1^-1 and r1 r2 mod r)
+ * Points at infinity follow the group law: A = infinity gives A' = infinity and C' = C, C = -r2 A gives C' = infinity.  As in
+ * arkworks, B is not checked for membership in G2: a B outside G2 is transformed like any other point.
+ * proofs = count x 256 B in the layout b2g_prove writes; r1_canon, r2_canon = count x 32 B canonical factors, each in
+ * [1, r); proofs_out = count x 256 B, canonical affine (all zeros = infinity); ok_out = count bytes.  Row i is well-formed when
+ * every coordinate is below p and every point not at infinity lies on its curve (the rule of b2g_verify_many).  A malformed
+ * row is not an error: ok_out[i] = 0 and its output row is 256 bytes of 0xFF, which b2g_verify_many reports invalid; the other
+ * rows are unaffected.  ok_out[i] = 1 otherwise.  The key's memory is used as b2g_vk_load left it (delta_2 only).
+ * Cost: per proof one Fr inversion, two 254-bit G1 products of A, one joint 254-bit G2 chain over B and delta_2, and three
+ * conversions to affine; one kernel, one proof per thread.
+ * Synchronous.  Errors (checked before anything runs): B2G_E_SHAPE for count == 0, null pointers, a key of another device or a
+ * proof pending on the context; B2G_E_INPUT for a factor that is zero or >= r (the message names the proof); B2G_E_DEVICE when
+ * the buffers do not fit.  Every error leaves the context usable.  The buffers are the context's verification buffers: they
+ * grow to the largest batch seen and are kept. */
+B2G_API int b2g_rerandomize_many(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* proofs, const void* r1_canon,
+                                 const void* r2_canon, uint8_t* proofs_out, uint8_t* ok_out);
 
 /* Kernel-level entry points (parity tests, benchmarks). All pointers host. */
 B2G_API int b2g_msm_g1(b2g_ctx* ctx, const void* bases, const void* scalars, size_t n, int scalars_mont, void* out_xy_mont);
