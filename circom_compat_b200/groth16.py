@@ -746,10 +746,12 @@ class Groth16:
     # base-range sharded variant: every rank calls prove_partial, the 768-byte partials are all-gathered by the caller
     # (torch.distributed / NCCL), then every rank calls prove_finish and obtains the same proof.
     @staticmethod
-    def prove_partial(pk: ProvingKey, matrices: ConstraintMatrices, full_assignment, ctx: Context, r=None, s=None) -> np.ndarray:
-        """r, s are optional here: when given, the (r, s)-only scalar multiplications start alongside the MSMs."""
+    def prove_partial(pk: ProvingKey, matrices: ConstraintMatrices, full_assignment, ctx: Context, r=None, s=None,
+                      reduction=CircomReduction) -> np.ndarray:
+        """r, s are optional here: when given, the (r, s)-only scalar multiplications start alongside the MSMs.  reduction:
+        the key's R1CSToQAP, as for create_proof_with_reduction_and_matrices (LibsnarkReduction needs matrices with C)."""
         w = _c(full_assignment)
-        ph, mh = ctx.pk_handle(pk), ctx.mat_handle(matrices, pk.n_vars)
+        ph, mh = ctx.pk_handle(pk), ctx.mat_handle(matrices, pk.n_vars, reduction.ID)
         out = np.zeros(N.PARTIAL_BYTES, dtype=np.uint8)
         rr = _scalar_bytes(r) if r is not None else None
         ss = _scalar_bytes(s) if s is not None else None

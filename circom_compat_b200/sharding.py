@@ -8,6 +8,8 @@ from __future__ import annotations
 
 import numpy as np
 
+from .groth16 import CircomReduction, Groth16
+
 PARTIAL_BYTES = 768
 # offsets inside a partial: [H, L, A, B1] as G1 XYZZ (128 B) then B2 as G2 XYZZ (256 B)
 PARTIAL_LAYOUT = {'h': (0, 128), 'l': (128, 128), 'a': (256, 128), 'b1': (384, 128), 'b2': (512, 256)}
@@ -36,10 +38,9 @@ def all_gather_partials(partial: np.ndarray, dist, device=None, group=None) -> n
     return out.cpu().numpy().reshape(world, PARTIAL_BYTES)
 
 
-def prove_sharded(ctx, pk, matrices, w_mont, r, s, dist, device=None, group=None):
+def prove_sharded(ctx, pk, matrices, w_mont, r, s, dist, device=None, group=None, reduction=CircomReduction):
     """One proof on a sharded context: partial MSMs -> all-gather -> identical fold on every rank."""
-    from .groth16 import Groth16
-    part = Groth16.prove_partial(pk, matrices, w_mont, ctx, r, s)
+    part = Groth16.prove_partial(pk, matrices, w_mont, ctx, r, s, reduction)
     allp = all_gather_partials(part, dist, device, group)
     return Groth16.prove_finish(pk, allp, r, s, ctx)
 

@@ -8,6 +8,7 @@ import pytest
 
 from oracle import cref as c
 from oracle import pyref as o
+from proof_model import CpuFixedBase
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -69,12 +70,6 @@ def test_montgomery_helpers_roundtrip():
     assert np.array_equal(m, c.fr_to_mont(c.ints_to_limbs(vals)))
 
 
-class _CpuFixedBase:
-    """stands in for Context in synth.setup on a CPU-only box (group elements from the oracle)"""
-    def fixed_base_g1(self, s): return c.fixed_base_g1(s)
-    def fixed_base_g2(self, s): return c.fixed_base_g2(s)
-
-
 @pytest.mark.parametrize('kind', ['chain', 'circomlike'])
 def test_synthetic_setup_is_a_valid_groth16_key(kind, tmp_path):
     from circom_compat_b200 import synth, read_zkey, fr_to_mont, fr_from_mont
@@ -82,7 +77,7 @@ def test_synthetic_setup_is_a_valid_groth16_key(kind, tmp_path):
         circ = synth.chain_circuit(64); w = synth.chain_witness(64)
     else:
         circ, w = synth.circomlike_circuit(9)
-    pk, td = synth.setup(_CpuFixedBase(), circ)
+    pk, td = synth.setup(CpuFixedBase(), circ)
     assert td.h_t == o.h_query_scalars(circ.domain_size - 1, td.tau, pow(td.delta, -1, o.R_MOD))   # qap.rs:90-105 literally
     path = str(tmp_path / 'syn.zkey')
     synth.write_zkey(path, pk, circ)

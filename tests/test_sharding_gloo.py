@@ -11,61 +11,26 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _worker(rank, world, port, q):
-    sys.path.insert(0, ROOT)
+    sys.path[:0] = [ROOT, os.path.join(ROOT, 'tests')]
     os.environ['MASTER_ADDR'] = '127.0.0.1'; os.environ['MASTER_PORT'] = str(port)
     import torch.distributed as dist
     dist.init_process_group('gloo', rank=rank, world_size=world)
     try:
         from circom_compat_b200 import read_zkey, fr_to_mont, sharding
         from oracle import cref as c, pyref as o
+        from proof_model import assemble, fold, partial_points, partial_record, rank_partials, shard_bases, shard_scalars
         g = json.load(open(os.path.join(ROOT, 'tests', 'golden', 'golden_vectors.json')))['complex_zkey']
         data = open(os.path.join(ROOT, 'tests', 'golden', 'complex-circuit-10000-10000.zkey'), 'rb').read()
         pk, cm = read_zkey(data)
         za = c.zkey_arrays(data)
-        w = o.chain_witness(pk.n_vars, g['a'])
-        wm = fr_to_mont(w)
+        wm = fr_to_mont(o.chain_witness(pk.n_vars, g['a']))
         h = c.witness_map(cm.num_constraints, cm.num_instance_variables, pk.n_vars, za['a_csr'], za['b_csr'], wm, nthreads=2)
-        wc, hc = c.fr_from_mont(wm), c.fr_from_mont(h)
-        li = pk.n_public + 1
-        l_padded = np.concatenate([np.zeros((li - 1, 8), dtype=np.uint64), pk.l_query])      # L re-indexed onto w[1..]
-        bases = {'h': pk.h_query, 'l': l_padded, 'a': pk.a_query[1:], 'b1': pk.b_g1_query[1:], 'b2': pk.b_g2_query[1:]}
-        scal = {'h': hc, 'w': wc}
-        one = c.fq_to_mont(c.ints_to_limbs([1]))[0]
-        part = np.zeros(sharding.PARTIAL_BYTES, dtype=np.uint8)
-        for q_, (total, sv, soff) in sharding.query_totals(pk.n_vars, pk.n_public, pk.domain_size).items():
-            lo, hi = sharding.shard_range(total, rank, world)
-            f = c.msm_g2 if q_ == 'b2' else c.msm_g1
-            aff = f(bases[q_][lo:hi], scal[sv][soff + lo: soff + hi], nthreads=2)
-            off, size = sharding.PARTIAL_LAYOUT[q_]
-            if aff.any():                                   # affine -> XYZZ with ZZ = ZZZ = 1
-                ones = np.concatenate([one, np.zeros(4, dtype=np.uint64)]) if q_ == 'b2' else one
-                xyzz = np.concatenate([aff, ones, ones])
-                part[off:off + size] = np.frombuffer(xyzz.tobytes(), dtype=np.uint8)
+        part = partial_record(rank_partials(pk, shard_bases(pk), shard_scalars(wm, h), rank, world, nthreads=2))
         allp = sharding.all_gather_partials(part, dist)
         assert allp.shape == (world, sharding.PARTIAL_BYTES) and np.array_equal(allp[rank], part)
-
         # fold in rank order and assemble (ark-groth16 create_proof_with_assignment) with the big-int oracle
-        def g1(buf):
-            v = c.limbs_to_ints(c.fq_from_mont(np.frombuffer(buf.tobytes(), dtype='<u8')))
-            return None if v[2] == 0 else (v[0], v[1])      # ZZ = ZZZ = 1 here
-
-        def g2(buf):
-            v = c.limbs_to_ints(c.fq_from_mont(np.frombuffer(buf.tobytes(), dtype='<u8')))
-            return None if (v[4], v[5]) == (0, 0) else ((v[0], v[1]), (v[2], v[3]))
-        acc = {k: None for k in sharding.PARTIAL_LAYOUT}
-        for rk in range(world):
-            for k, (off, size) in sharding.PARTIAL_LAYOUT.items():
-                buf = allp[rk, off:off + size]
-                acc[k] = o.G2.add(acc[k], g2(buf)) if k == 'b2' else o.G1.add(acc[k], g1(buf))
-        z = o.read_zkey(data, decode_points=False)
-        def pt1(arr): return o._g1_from(np.ascontiguousarray(arr).tobytes())
-        def pt2(arr): return o._g2_from(np.ascontiguousarray(arr).tobytes())
-        r, s = int(g['r']), int(g['s'])
-        A = o.G1.sum([o.G1.mul(z.delta_g1, r), pt1(pk.a_query[0]), acc['a'], z.alpha_g1])
-        B1 = o.G1.sum([o.G1.mul(z.delta_g1, s), pt1(pk.b_g1_query[0]), acc['b1'], z.beta_g1])
-        B2 = o.G2.sum([o.G2.mul(z.delta_g2, s), pt2(pk.b_g2_query[0]), acc['b2'], z.beta_g2])
-        C = o.G1.sum([o.G1.mul(A, s), o.G1.mul(B1, r), o.G1.neg(o.G1.mul(z.delta_g1, r * s % o.R_MOD)), acc['l'], acc['h']])
-        q.put((rank, o.proof_to_bytes(A, B2, C).hex() == g['proof_hex']))
+        proof = assemble(pk, fold([partial_points(p) for p in allp]), int(g['r']), int(g['s']))
+        q.put((rank, proof.hex() == g['proof_hex']))
     finally:
         dist.destroy_process_group()
 
