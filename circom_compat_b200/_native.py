@@ -50,7 +50,7 @@ class KeyBatch(C.Structure):
 EXPORTS = ['b2g_last_error', 'b2g_version', 'b2g_device_count', 'b2g_ctx_create', 'b2g_ctx_destroy', 'b2g_ctx_prepare', 'b2g_pk_load', 'b2g_pk_free',
            'b2g_matrices_load', 'b2g_matrices_free', 'b2g_witness_map', 'b2g_prove', 'b2g_prove_many', 'b2g_prove_submit', 'b2g_prove_wait', 'b2g_host_register', 'b2g_host_unregister', 'b2g_prove_partial', 'b2g_prove_finish',
            'b2g_p2p_export', 'b2g_p2p_import', 'b2g_p2p_connect_local', 'b2g_prove_sharded_p2p', 'b2g_msm_g1', 'b2g_msm_g2', 'b2g_ntt', 'b2g_fixed_base_g1', 'b2g_fixed_base_g2', 'b2g_test_op', 'b2g_last_timings',
-           'b2g_bench_device', 'b2g_bench_msm', 'b2g_launch_count', 'b2g_vk_load', 'b2g_vk_free', 'b2g_vk_alpha_beta', 'b2g_verify_many',
+           'b2g_bench_device', 'b2g_bench_msm', 'b2g_launch_count', 'b2g_vk_load', 'b2g_vk_load_many', 'b2g_vk_free', 'b2g_vk_alpha_beta', 'b2g_verify_many',
            'b2g_verify_batch', 'b2g_proofs_decompress', 'b2g_verify_many_compressed', 'b2g_verify_batch_compressed',
            'b2g_verify_batch_locate', 'b2g_verify_batch_locate_compressed', 'b2g_verify_batch_keys',
            'b2g_verify_batch_keys_compressed', 'b2g_verify_batch_keys_locate', 'b2g_verify_batch_keys_locate_compressed',
@@ -103,6 +103,7 @@ def lib():
         L.b2g_launch_count.argtypes = [vp, C.POINTER(C.c_uint64)]
         L.b2g_device_count.argtypes = [C.POINTER(C.c_int)]
         L.b2g_vk_load.argtypes = [vp, C.POINTER(VkDesc), C.POINTER(vp)]
+        L.b2g_vk_load_many.argtypes = [vp, C.c_uint32, C.POINTER(VkDesc), C.POINTER(vp)]
         L.b2g_vk_free.argtypes = [vp]
         L.b2g_vk_alpha_beta.argtypes = [vp, vp]
         L.b2g_verify_many.argtypes = [vp, vp, C.c_uint32, vp, vp, vp]

@@ -40,18 +40,24 @@ template <class C> struct Gen;
 template <> struct Gen<G1> { static __device__ __forceinline__ G1::Aff get() { return g1_generator(); } };
 template <> struct Gen<G2> { static __device__ __forceinline__ G2::Aff get() { return g2_generator(); } };
 
-// table[w][d-1] = d * 256^w * G (affine), w < 32, d = 1..255
+// entry i < 32 x 255 of a window table: table[w][d-1] = d * 256^w * G (affine), w = i / 255, d = i % 255 + 1
 // base = nullptr: the group generator; else the affine point at `base` (e.g. delta of a proving key)
 template <class C, class F>
-__global__ void fixed_table_kernel(void* __restrict__ table, const void* __restrict__ base) {
-    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= 32u * 255u) return;
+__device__ __forceinline__ void fixed_table_entry(void* __restrict__ table, const void* __restrict__ base, uint32_t i) {
     uint32_t w = i / 255u, d = i % 255u + 1u;
     uint32_t k[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     k[w >> 2] = d << (8 * (w & 3));
     typename C::Aff g = base ? aff_load<F>(base, 0) : Gen<C>::get();
     typename C::Pt p = C::mul_scalar(C::from_affine(g), k);
     aff_store<F>(table, i, C::to_affine(p));
+}
+
+// the whole window table of G, one entry per thread
+template <class C, class F>
+__global__ void fixed_table_kernel(void* __restrict__ table, const void* __restrict__ base) {
+    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= 32u * 255u) return;
+    fixed_table_entry<C, F>(table, base, i);
 }
 
 }  // namespace b2g

@@ -4,8 +4,9 @@
 // verify_with_processed_vk, /root/reference/src/zkey.rs:868-870, 914-916; ark-groth16 0.5.0): a proof (A, B, C) with public
 // inputs x is valid iff
 //     e(A, B) * e(IC[0] + sum_i x_i IC[i + 1], -gamma) * e(C, -delta) == e(alpha, beta).
-// The key is prepared once on the device (b2g_vk_load): on-curve checks, e(alpha, beta), the line coefficients of the two
-// fixed G2 arguments -gamma and -delta for every loop step (ark's G2Prepared), and an 8-bit window table per IC[i + 1].
+// The key is prepared once on the device (b2g_vk_load, or b2g_vk_load_many for many keys in the same four launches): on-curve
+// checks, e(alpha, beta), the line coefficients of the two fixed G2 arguments -gamma and -delta for every loop step (ark's
+// G2Prepared), and an 8-bit window table per IC[i + 1].
 // A batch then runs four kernels, one proof per thread (the parallelism comes from the batch):
 //   inputs   one warp per (proof, input): x_i IC[i + 1] from the window table (32 look-ups and a warp tree)
 //   prepare  parse the proof (canonical coordinates; >= p or off the curve -> invalid), sum the prepared inputs, affine
@@ -39,6 +40,7 @@
 // proof per thread: rerandomize_kernel.
 #include <algorithm>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <vector>
 #include "../../include/b2groth.h"
@@ -47,22 +49,28 @@
 #include "util.cuh"
 #include "verify.cuh"
 
-namespace b2g {
-void msm_validate_points(const void* pts_dev, uint32_t n, bool g2, cudaStream_t st, const char* what);   // msm.cu
-}
 using namespace b2g;
 
-constexpr size_t TABLE_BYTES = 32 * 255 * 64;       // one 8-bit window table of a G1 point
+constexpr uint32_t TABLE_POINTS = 32 * 255;         // entries of one 8-bit window table
+constexpr size_t TABLE_BYTES = TABLE_POINTS * 64;    // one 8-bit window table of a G1 point
 constexpr size_t F12_BYTES = 384;
+
+// the device memory of one b2g_vk_load_many call: every key's arrays, carved out of one allocation.  Each handle the call
+// made holds a reference; the last one to be freed frees the allocation.
+struct VkArena {
+    uint8_t* base = nullptr;
+    ~VkArena() { if (base) cudaFree(base); }
+};
 
 struct b2g_vk {
     int device = 0;
     uint32_t n_public = 0;
+    std::shared_ptr<VkArena> arena;   // the memory the arrays below lie in
     uint8_t* d_g1 = nullptr;       // alpha, IC[0..n_public] (G1 affine, Montgomery, 64 B each)
     uint8_t* d_g2 = nullptr;       // beta, gamma, delta (G2 affine, 128 B each)
     uint8_t* d_lines = nullptr;    // prepared lines of -gamma, then of -delta: 2 x ATE_LINES x LINE_BYTES
     uint8_t* d_eab = nullptr;      // e(alpha, beta), 384 B
-    uint8_t* d_tabs = nullptr;     // window tables of IC[1..n_public], TABLE_BYTES apart
+    uint8_t* d_tabs = nullptr;     // window tables of IC[1..n_public], TABLE_BYTES apart (none when n_public == 0)
     bool gamma_inf = false, delta_inf = false;
 };
 
@@ -109,10 +117,18 @@ struct Seg {
     uint32_t key, first, count, part, chunks, pt;
 };
 
-// the last segment k < n with s[k].*M <= v, for a field that is nondecreasing along the table (first, part, pt, or the 64-bit
-// pub)
-template <auto M, class T>
-__device__ __forceinline__ uint32_t seg_find(const Seg* __restrict__ s, uint32_t n, T v) {
+// one key of a b2g_vk_load_many call as its kernels read it: where its arrays lie in the call's allocation, its first point
+// of vk_validate_kernel and its first window table of vk_tables_kernel (pt and tab never decrease along the table)
+struct VkRec {
+    uint64_t pt, tab;
+    uint8_t *g1, *g2, *eab, *lines, *tabs;
+    uint32_t n_public, pad;
+};
+
+// the last record k < n with s[k].*M <= v, for a field that is nondecreasing along the table (a Seg's first, part, pt, or the
+// 64-bit pub; a VkRec's pt or tab)
+template <auto M, class R, class T>
+__device__ __forceinline__ uint32_t seg_find(const R* __restrict__ s, uint32_t n, T v) {
     uint32_t lo = 0, hi = n;
     while (hi - lo > 1) {
         const uint32_t mid = (lo + hi) >> 1;
@@ -643,23 +659,63 @@ __global__ void __launch_bounds__(64) rerandomize_kernel(const uint8_t* __restri
     coords_store(out + (size_t)j * 256, c, 8, true);
 }
 
-// lines of -gamma (thread 0) and -delta (thread 1) for every loop step, in the order miller_loop reads them
-__global__ void vk_lines_kernel(const uint8_t* __restrict__ g2, uint8_t* __restrict__ lines) {
-    const int t = threadIdx.x;
-    if (t > 1) return;
-    const G2::Aff q = aff_load<Fq2>(g2, 1 + t);
+// ---------------------------------------------------------------------------------------------- key preparation
+// b2g_vk_load_many (b2g_vk_load is its call of one key) prepares every key of a call in four launches, whatever the number
+// of keys and of public inputs; each kernel finds its key in the call's VkRec table.
+
+// one thread per point of every key: key k's points are its G1 points alpha, IC[0..n_public], then its G2 points beta,
+// gamma, delta.  bad[2k] (G1) and bad[2k + 1] (G2) receive 1 + the greatest index of an off-curve point among them, the
+// index msm_validate_points reports.
+__global__ void __launch_bounds__(256) vk_validate_kernel(const VkRec* __restrict__ keys, uint32_t n_keys, uint64_t n_pts,
+                                                          uint32_t* __restrict__ bad) {
+    const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n_pts) return;
+    const uint32_t k = seg_find<&VkRec::pt>(keys, n_keys, t);
+    const VkRec& key = keys[k];
+    const uint32_t j = (uint32_t)(t - key.pt), n_g1 = key.n_public + 2;
+    if (j < n_g1) {
+        if (!aff_on_curve<G1, Fq>(aff_load<Fq>(key.g1, j))) atomicMax(bad + 2 * k, j + 1);
+    } else if (!aff_on_curve<G2, Fq2>(aff_load<Fq2>(key.g2, j - n_g1))) {
+        atomicMax(bad + 2 * k + 1, j - n_g1 + 1);
+    }
+}
+
+// e(alpha, beta) of every key, one key per thread
+__global__ void __launch_bounds__(64) vk_pairing_kernel(const VkRec* __restrict__ keys, uint32_t n_keys) {
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n_keys) return;
+    fe12 e;
+    pairing(e, aff_load<Fq>(keys[k].g1, 0), aff_load<Fq2>(keys[k].g2, 0));
+    Fq12::store(keys[k].eab, e);
+}
+
+// the lines of -gamma (thread 2k) and -delta (thread 2k + 1) of key k for every loop step, in the order miller_loop reads
+// them; nothing for a point at infinity, whose pair drops out
+__global__ void __launch_bounds__(64) vk_lines_kernel(const VkRec* __restrict__ keys, uint32_t n_keys) {
+    const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= 2 * (uint64_t)n_keys) return;
+    const VkRec& key = keys[t >> 1];
+    const uint32_t s = (uint32_t)(t & 1);
+    const G2::Aff q = aff_load<Fq2>(key.g2, 1 + s);
     if (G2::aff_is_inf(q)) return;
-    uint8_t* out = lines + (size_t)t * ATE_LINES * LINE_BYTES;
+    uint8_t* out = key.lines + (size_t)s * ATE_LINES * LINE_BYTES;
     g2_line_walk(q.x, Fq2::neg(q.y), [&](const fe2* c) {
         elem_store(out, c[0]); elem_store(out + 64, c[1]); elem_store(out + 128, c[2]);
         out += LINE_BYTES;
     });
 }
 
-__global__ void vk_pairing_kernel(const uint8_t* __restrict__ g1, const uint8_t* __restrict__ g2, uint8_t* __restrict__ eab) {
-    fe12 e;
-    pairing(e, aff_load<Fq>(g1, 0), aff_load<Fq2>(g2, 0));
-    Fq12::store(eab, e);
+// every window table of every key, one entry per thread: the tables of all keys are numbered back to back, and table t
+// (key k's IC[j + 1], j = t - keys[k].tab) gets its entry e % TABLE_POINTS.  The points are indexed on grid.x, so the
+// number of tables is not bound by a grid dimension.
+__global__ void __launch_bounds__(64) vk_tables_kernel(const VkRec* __restrict__ keys, uint32_t n_keys, uint64_t n_entries) {
+    const uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n_entries) return;
+    const uint64_t t = e / TABLE_POINTS;
+    // a key without inputs shares its tab with the next key, so the last key with tab <= t is the one that holds t
+    const VkRec& key = keys[seg_find<&VkRec::tab>(keys, n_keys, t)];
+    const uint64_t j = t - key.tab;
+    fixed_table_entry<G1, Fq>(key.tabs + j * TABLE_BYTES, key.g1 + (2 + j) * 64, (uint32_t)(e % TABLE_POINTS));
 }
 
 // b2g_test_op ops 30-42 on Fq12 values (384 B), G1 / G2 affine points (64 / 128 B), lines (3 Fq2, 192 B) and projective
@@ -711,7 +767,8 @@ static bool all_zero(const void* p, size_t n);
 // with its own copy of the __noinline__ calls it reaches (miller_loop_t, ell_fixed, the tower), so only a launch of the
 // shipped kernel tests the shipped machine code.  Per row of ops 49 and 53, a staging region holds the key's G2 points for
 // vk_lines_kernel (an unused slot, gamma, delta), then the row's proof record (op 49) or batch tail (op 53), then the lines
-// of -gamma and -delta; a point given as zeros is infinity and drops its pair, as in b2g_vk_load.
+// of -gamma and -delta; a point given as zeros is infinity and drops its pair, as in b2g_vk_load.  Ops 49, 50 and 52 make
+// each row (or pair of rows) a key of one b2g_vk_load_many kernel launch.
 constexpr size_t STAGE_G2 = 0, STAGE_REC = 384, STAGE_LINES = STAGE_REC + TAIL_BYTES, STAGE_BYTES = STAGE_LINES + 2 * ATE_LINES * LINE_BYTES;
 
 static void verify_stage_test_op(cudaStream_t st, int op, const void* a, const void* b, size_t n, void* out) {
@@ -748,19 +805,23 @@ static void verify_stage_test_op(cudaStream_t st, int op, const void* a, const v
         d.s = dev_upload<uint8_t>(stage.data(), stage.size(), st);
         CUDA_CHECK(cudaMalloc(&d.o, n * so));
         // per row, a key record with the row's lines and a one-segment table, as verify_many_enqueue and batch_enqueue build
-        // them
-        std::vector<uint8_t> meta(n * sizeof(KeyRec) + sizeof(Seg));
+        // them, then the rows as the keys of one vk_lines_kernel launch, as b2g_vk_load_many builds them
+        std::vector<uint8_t> meta(n * sizeof(KeyRec) + sizeof(Seg) + n * sizeof(VkRec));
         KeyRec* keys = reinterpret_cast<KeyRec*>(meta.data());
-        for (size_t i = 0; i < n; i++)
-            keys[i] = {d.s + i * STAGE_BYTES + STAGE_LINES, nullptr, nullptr, nullptr, 0, on[2 * i], on[2 * i + 1], 0};
+        VkRec* vks = reinterpret_cast<VkRec*>(meta.data() + n * sizeof(KeyRec) + sizeof(Seg));
+        for (size_t i = 0; i < n; i++) {
+            uint8_t* g = d.s + i * STAGE_BYTES;
+            keys[i] = {g + STAGE_LINES, nullptr, nullptr, nullptr, 0, on[2 * i], on[2 * i + 1], 0};
+            vks[i] = {0, 0, nullptr, g + STAGE_G2, nullptr, g + STAGE_LINES, nullptr, 0, 0};
+        }
         const Seg seg = {0, 0, 0, 1, 0, 1, 0};
         memcpy(meta.data() + n * sizeof(KeyRec), &seg, sizeof(Seg));
         d.a = dev_upload<uint8_t>(meta.data(), meta.size(), st);
         CUDA_CHECK(cudaStreamSynchronize(st));             // meta is pageable and leaves scope here
         const Seg* d_seg = (const Seg*)(d.a + n * sizeof(KeyRec));
+        vk_lines_kernel<<<(unsigned)((2 * n + 63) / 64), 64, 0, st>>>((const VkRec*)(d.a + n * sizeof(KeyRec) + sizeof(Seg)), (uint32_t)n);
         for (size_t i = 0; i < n; i++) {
             uint8_t* g = d.s + i * STAGE_BYTES;
-            vk_lines_kernel<<<1, 32, 0, st>>>(g + STAGE_G2, g + STAGE_LINES);
             if (op == 49) {
                 verify_miller_kernel<<<1, 64, 0, st>>>(g + STAGE_REC, (const KeyRec*)d.a + i, d_seg, 1, 1, d.o + i * F12_BYTES);
             } else {
@@ -768,16 +829,20 @@ static void verify_stage_test_op(cudaStream_t st, int op, const void* a, const v
                 CUDA_CHECK(cudaMemcpyAsync(d.o + i * F12_BYTES, g + STAGE_REC + TAIL_G, F12_BYTES, cudaMemcpyDeviceToDevice, st));
             }
         }
-        g_launch_count += 2 * n;
+        g_launch_count += 1 + n;
     } else if (op == 50) {
-        // the lines of -a: rows 2k and 2k + 1 are the gamma and delta of one vk_lines_kernel launch
+        // the lines of -a: rows 2k and 2k + 1 are the gamma and delta of key k of one vk_lines_kernel launch
         const size_t pairs = (n + 1) / 2;
         std::vector<uint8_t> g2(pairs * 384, 0);
         for (size_t i = 0; i < n; i++) memcpy(g2.data() + (i / 2) * 384 + 128 * (1 + i % 2), in + i * 128, 128);
         d.a = dev_upload<uint8_t>(g2.data(), g2.size(), st);
         CUDA_CHECK(cudaMalloc(&d.o, 2 * pairs * so));
-        for (size_t k = 0; k < pairs; k++) vk_lines_kernel<<<1, 32, 0, st>>>(d.a + k * 384, d.o + 2 * k * so);
-        g_launch_count += pairs;
+        std::vector<VkRec> vks(pairs);
+        for (size_t k = 0; k < pairs; k++) vks[k] = {0, 0, nullptr, d.a + k * 384, nullptr, d.o + 2 * k * so, nullptr, 0, 0};
+        d.s = dev_upload<uint8_t>(vks.data(), pairs * sizeof(VkRec), st);
+        CUDA_CHECK(cudaStreamSynchronize(st));             // vks is pageable and leaves scope here
+        vk_lines_kernel<<<(unsigned)((2 * pairs + 63) / 64), 64, 0, st>>>((const VkRec*)d.s, (uint32_t)pairs);
+        g_launch_count += 1;
     } else if (op == 51) {
         d.a = dev_upload<uint8_t>(a, n * sa, st);
         CUDA_CHECK(cudaMalloc(&d.o, n * so));
@@ -797,11 +862,17 @@ static void verify_stage_test_op(cudaStream_t st, int op, const void* a, const v
                                                                       (const uint32_t*)d.a, n, d.o);
         g_launch_count += 2;
     } else {
-        d.a = dev_upload<uint8_t>(a, n * sa, st);
+        // row i is IC[1] of key i of one vk_tables_kernel launch: its G1 slots are (unused alpha, unused IC[0], the row)
+        std::vector<uint8_t> g1(n * 192, 0);
+        for (size_t i = 0; i < n; i++) memcpy(g1.data() + i * 192 + 128, in + i * 64, 64);
+        d.a = dev_upload<uint8_t>(g1.data(), g1.size(), st);
         CUDA_CHECK(cudaMalloc(&d.o, n * so));
-        for (size_t i = 0; i < n; i++)
-            fixed_table_kernel<G1, Fq><<<(32 * 255 + 63) / 64, 64, 0, st>>>(d.o + i * TABLE_BYTES, d.a + i * 64);
-        g_launch_count += n;
+        std::vector<VkRec> vks(n);
+        for (size_t i = 0; i < n; i++) vks[i] = {0, i, d.a + i * 192, nullptr, nullptr, nullptr, d.o + i * TABLE_BYTES, 1, 0};
+        d.s = dev_upload<uint8_t>(vks.data(), n * sizeof(VkRec), st);
+        CUDA_CHECK(cudaStreamSynchronize(st));             // g1 and vks are pageable and leave scope here
+        vk_tables_kernel<<<(unsigned)((n * TABLE_POINTS + 63) / 64), 64, 0, st>>>((const VkRec*)d.s, (uint32_t)n, (uint64_t)n * TABLE_POINTS);
+        g_launch_count += 1;
     }
     CUDA_CHECK(cudaGetLastError());
     CUDA_CHECK(cudaMemcpyAsync(out, d.o, n * so, cudaMemcpyDeviceToHost, st));
@@ -837,11 +908,6 @@ void pairing_test_op(cudaStream_t st, int op, const void* a, const void* b, size
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-static void vk_release(b2g_vk* vk) {
-    for (void* p : {(void*)vk->d_g1, (void*)vk->d_g2, (void*)vk->d_lines, (void*)vk->d_eab, (void*)vk->d_tabs}) if (p) cudaFree(p);
-    delete vk;
-}
-
 static bool all_zero(const void* p, size_t n) {
     const uint8_t* b = (const uint8_t*)p;
     for (size_t i = 0; i < n; i++) if (b[i]) return false;
@@ -950,45 +1016,113 @@ static void reduce_run(const std::vector<uint32_t>& levels, const Span* spans, c
 // one segment of the batch check: `count` consecutive proofs under key record `key`
 struct SegIn { uint32_t key, count; };
 
+// b2g_vk_load_many: the checks, one allocation carved into every key's arrays (each 256-byte aligned), one upload of every
+// key's points and of the VkRec table, the on-curve checks and one synchronise, then e(alpha, beta), the lines and the window
+// tables of every key in three launches and a second synchronise.  The handles are made only once everything succeeded.
+// b2g_vk_load is the call of one key (`one`): its messages keep their form without a key index.
+static void vk_load_many(b2g_ctx* ctx, uint32_t n_keys, const b2g_vk_desc* descs, b2g_vk** out, bool one) {
+    static const char* fn = "b2g_vk_load_many";
+    auto at = [&](uint32_t k) { return one ? std::string() : std::string(fn) + ": key " + std::to_string(k) + ": "; };
+    if (!ctx || !descs || !out) throw_error(B2G_E_SHAPE, one ? "null pointer" : std::string(fn) + ": null pointer");
+    if (n_keys == 0) throw_error(B2G_E_SHAPE, std::string(fn) + ": n_keys must be at least 1");
+    for (uint32_t k = 0; k < n_keys; k++) {
+        const b2g_vk_desc& d = descs[k];
+        if (!d.alpha_g1 || !d.beta_g2 || !d.gamma_g2 || !d.delta_g2 || !d.gamma_abc_g1) throw_error(B2G_E_SHAPE, at(k) + "null verifying-key field");
+    }
+    const CtxView cv = ctx_view(ctx);
+    DevGuard g(cv.device);
+    cudaStream_t st = cv.st;
+    // the layout: the uploaded part first (per key its G1 points alpha, IC[0..n_public] and its G2 points beta, gamma, delta;
+    // then the VkRec table), then the on-curve status words, then per key e(alpha, beta), the lines and the window tables
+    auto up = [](size_t b) { return (b + 255) & ~(size_t)255; };
+    static_assert(TABLE_BYTES % 256 == 0, "window tables stay 256-byte aligned");
+    std::vector<size_t> o_g1(n_keys), o_g2(n_keys), o_eab(n_keys);
+    size_t o = 0;
+    uint64_t n_pts = 0, n_tabs = 0;
+    for (uint32_t k = 0; k < n_keys; k++) {
+        o_g1[k] = o; o += up(((size_t)descs[k].n_public + 2) * 64);
+        o_g2[k] = o; o += up(3 * 128);
+        n_pts += (uint64_t)descs[k].n_public + 5; n_tabs += descs[k].n_public;
+    }
+    const size_t o_recs = o, n_up = o + (size_t)n_keys * sizeof(VkRec);
+    const size_t o_bad = up(n_up);
+    o = o_bad + up((size_t)n_keys * 8);
+    for (uint32_t k = 0; k < n_keys; k++) { o_eab[k] = o; o += up(F12_BYTES) + up(2 * ATE_LINES * LINE_BYTES) + descs[k].n_public * TABLE_BYTES; }
+    auto arena = std::make_shared<VkArena>();
+    if (cudaMalloc(&arena->base, o) != cudaSuccess) {
+        cudaGetLastError();
+        arena->base = nullptr;
+        throw_error(B2G_E_DEVICE, std::string(fn) + ": the device state of " + std::to_string(n_keys) + (n_keys == 1 ? " key (" : " keys (") +
+                                  std::to_string((o + (1 << 20) - 1) >> 20) + " MiB) does not fit in device memory");
+    }
+    uint8_t* base = arena->base;
+    std::vector<uint8_t> h(n_up, 0);
+    VkRec* recs = reinterpret_cast<VkRec*>(h.data() + o_recs);
+    uint64_t pt = 0, tab = 0;
+    for (uint32_t k = 0; k < n_keys; k++) {
+        const b2g_vk_desc& d = descs[k];
+        uint8_t *g1 = h.data() + o_g1[k], *g2 = h.data() + o_g2[k];
+        memcpy(g1, d.alpha_g1, 64);
+        memcpy(g1 + 64, d.gamma_abc_g1, ((size_t)d.n_public + 1) * 64);
+        memcpy(g2, d.beta_g2, 128); memcpy(g2 + 128, d.gamma_g2, 128); memcpy(g2 + 256, d.delta_g2, 128);
+        uint8_t* eab = base + o_eab[k];
+        recs[k] = {pt, tab, base + o_g1[k], base + o_g2[k], eab, eab + up(F12_BYTES),
+                   d.n_public ? eab + up(F12_BYTES) + up(2 * ATE_LINES * LINE_BYTES) : nullptr, d.n_public, 0};
+        pt += (uint64_t)d.n_public + 5; tab += d.n_public;
+    }
+    const VkRec* d_recs = reinterpret_cast<const VkRec*>(base + o_recs);
+    uint32_t* d_bad = reinterpret_cast<uint32_t*>(base + o_bad);
+    std::vector<uint32_t> bad(2 * (size_t)n_keys);
+    try {
+        // prepare_verifying_key checks every point (verifier.py): an off-curve point fails the call with B2G_E_INPUT, naming the
+        // lowest key that holds one and, as msm_validate_points does, its G1 points before its G2 points
+        CUDA_CHECK(cudaMemcpyAsync(base, h.data(), n_up, cudaMemcpyHostToDevice, st));
+        CUDA_CHECK(cudaMemsetAsync(d_bad, 0, (size_t)n_keys * 8, st));
+        vk_validate_kernel<<<(unsigned)((n_pts + 255) / 256), 256, 0, st>>>(d_recs, n_keys, n_pts, d_bad);
+        g_launch_count += 1;
+        CUDA_CHECK(cudaGetLastError());
+        CUDA_CHECK(cudaMemcpyAsync(bad.data(), d_bad, (size_t)n_keys * 8, cudaMemcpyDeviceToHost, st));
+        CUDA_CHECK(cudaStreamSynchronize(st));
+        for (uint32_t k = 0; k < n_keys; k++) {
+            if (bad[2 * k]) throw_error(B2G_E_INPUT, at(k) + "G1 point " + std::to_string(bad[2 * k] - 1) + " of alpha_g1 / gamma_abc_g1 is not on the curve");
+            if (bad[2 * k + 1]) throw_error(B2G_E_INPUT, at(k) + "G2 point " + std::to_string(bad[2 * k + 1] - 1) + " of beta_g2 / gamma_g2 / delta_g2 is not on the curve");
+        }
+        // the table kernel is launched without tables too (one CTA that does nothing), so that the launches do not depend on
+        // the public-input counts
+        const uint64_t entries = n_tabs * TABLE_POINTS;
+        vk_pairing_kernel<<<(n_keys + 63) / 64, 64, 0, st>>>(d_recs, n_keys);
+        vk_lines_kernel<<<(unsigned)((2 * (uint64_t)n_keys + 63) / 64), 64, 0, st>>>(d_recs, n_keys);
+        vk_tables_kernel<<<(unsigned)std::max<uint64_t>(1, (entries + 63) / 64), 64, 0, st>>>(d_recs, n_keys, entries);
+        g_launch_count += 3;
+        CUDA_CHECK(cudaGetLastError());
+        CUDA_CHECK(cudaStreamSynchronize(st));
+    } catch (...) {
+        cudaDeviceSynchronize();                           // nothing may still use the allocation when it is freed
+        throw;
+    }
+    std::vector<std::unique_ptr<b2g_vk>> vks(n_keys);
+    for (uint32_t k = 0; k < n_keys; k++) {
+        const VkRec& r = recs[k];
+        vks[k].reset(new b2g_vk());
+        b2g_vk* vk = vks[k].get();
+        vk->device = cv.device; vk->n_public = descs[k].n_public; vk->arena = arena;
+        vk->d_g1 = r.g1; vk->d_g2 = r.g2; vk->d_eab = r.eab; vk->d_lines = r.lines; vk->d_tabs = r.tabs;
+        vk->gamma_inf = all_zero(descs[k].gamma_g2, 128);
+        vk->delta_inf = all_zero(descs[k].delta_g2, 128);
+    }
+    for (uint32_t k = 0; k < n_keys; k++) out[k] = vks[k].release();
+}
+
 }  // namespace b2g
 
 extern "C" {
 
 int b2g_vk_load(b2g_ctx* ctx, const b2g_vk_desc* d, b2g_vk** out) {
-    return guarded([&] {
-        if (!ctx || !d || !out) throw_error(B2G_E_SHAPE, "null pointer");
-        if (!d->alpha_g1 || !d->beta_g2 || !d->gamma_g2 || !d->delta_g2 || !d->gamma_abc_g1) throw_error(B2G_E_SHAPE, "null verifying-key field");
-        const CtxView cv = ctx_view(ctx);
-        DevGuard g(cv.device);
-        cudaStream_t st = cv.st;
-        struct VkGuard { b2g_vk* vk = new b2g_vk(); ~VkGuard() { if (vk) { cudaDeviceSynchronize(); vk_release(vk); } } } guard;
-        b2g_vk* vk = guard.vk;
-        vk->device = cv.device; vk->n_public = d->n_public;
-        const size_t n1 = (size_t)d->n_public + 1;
-        std::vector<uint8_t> g1((1 + n1) * 64), g2(3 * 128);
-        memcpy(g1.data(), d->alpha_g1, 64);
-        memcpy(g1.data() + 64, d->gamma_abc_g1, n1 * 64);
-        memcpy(g2.data(), d->beta_g2, 128); memcpy(g2.data() + 128, d->gamma_g2, 128); memcpy(g2.data() + 256, d->delta_g2, 128);
-        vk->gamma_inf = all_zero(d->gamma_g2, 128);
-        vk->delta_inf = all_zero(d->delta_g2, 128);
-        vk->d_g1 = dev_upload<uint8_t>(g1.data(), g1.size(), st);
-        vk->d_g2 = dev_upload<uint8_t>(g2.data(), g2.size(), st);
-        // prepare_verifying_key checks every point (verifier.py); an off-curve point fails the load with B2G_E_INPUT
-        msm_validate_points(vk->d_g1, (uint32_t)(1 + n1), false, st, "alpha_g1 / gamma_abc_g1");
-        msm_validate_points(vk->d_g2, 3, true, st, "beta_g2 / gamma_g2 / delta_g2");
-        CUDA_CHECK(cudaMalloc(&vk->d_eab, F12_BYTES));
-        CUDA_CHECK(cudaMalloc(&vk->d_lines, 2 * ATE_LINES * LINE_BYTES));
-        CUDA_CHECK(cudaMalloc(&vk->d_tabs, d->n_public ? d->n_public * TABLE_BYTES : 1));
-        vk_pairing_kernel<<<1, 1, 0, st>>>(vk->d_g1, vk->d_g2, vk->d_eab);
-        vk_lines_kernel<<<1, 32, 0, st>>>(vk->d_g2, vk->d_lines);
-        for (uint32_t i = 0; i < d->n_public; i++)
-            fixed_table_kernel<G1, Fq><<<(32 * 255 + 63) / 64, 64, 0, st>>>(vk->d_tabs + i * TABLE_BYTES, vk->d_g1 + (size_t)(2 + i) * 64);
-        g_launch_count += 2 + d->n_public;
-        CUDA_CHECK(cudaGetLastError());
-        CUDA_CHECK(cudaStreamSynchronize(st));
-        guard.vk = nullptr;
-        *out = vk;
-    });
+    return guarded([&] { vk_load_many(ctx, 1, d, out, true); });
+}
+
+int b2g_vk_load_many(b2g_ctx* ctx, uint32_t n_keys, const b2g_vk_desc* descs, b2g_vk** out) {
+    return guarded([&] { vk_load_many(ctx, n_keys, descs, out, false); });
 }
 
 int b2g_vk_free(b2g_vk* vk) {
@@ -996,7 +1130,7 @@ int b2g_vk_free(b2g_vk* vk) {
         if (!vk) return;
         DevGuard g(vk->device);
         cudaDeviceSynchronize();
-        vk_release(vk);
+        delete vk;                                         // the last handle of a b2g_vk_load_many call frees its allocation
     });
 }
 

@@ -16,6 +16,8 @@
         <- the same check for a whole batch at once: one random-linear-combination pairing check (b2g_verify_batch).
     Groth16.verify_batch_locate(vk, public_inputs, proofs)
         <- verify_with_processed_vk for every proof, from one batch check per group of 64 proofs (b2g_verify_batch_locate).
+    Groth16.load_verifying_keys(vks)
+        <- process_vk for many keys in one device pass (b2g_vk_load_many); the keyed verifiers below load their new keys so.
     Groth16.verify_batch_keys([(vk, public_inputs, proofs), ...])
         <- verify_batch for many keys in one device pass, one verdict per key (b2g_verify_batch_keys).
     Groth16.verify_batch_keys_locate([(vk, public_inputs, proofs), ...])
@@ -31,6 +33,7 @@ Arguments keep the reference's meaning; field elements are (n, 4) uint64 Montgom
 from __future__ import annotations
 
 import ctypes as C
+import re
 from dataclasses import dataclass
 
 import numpy as np
@@ -73,6 +76,32 @@ TEST_PAIR_RUN = 16            # entries per row of op 27; an entry is 16 words o
 # release(obj) / release_all() free them.
 _PK_HANDLES, _MAT_HANDLES, _VK_HANDLES = {}, {}, {}
 _CACHES = ((_PK_HANDLES, 'b2g_pk_free'), (_MAT_HANDLES, 'b2g_matrices_free'), (_VK_HANDLES, 'b2g_vk_free'))
+
+
+def _vk_desc(key):
+    """(b2g_vk_desc, the arrays it points into) of a verifier.VerifyingKey, PreparedVerifyingKey or ProvingKey"""
+    from . import verifier
+    vk = key.vk if isinstance(key, verifier.PreparedVerifyingKey) else key
+    if not isinstance(vk, verifier.VerifyingKey):
+        vk = verifier.VerifyingKey.from_proving_key(vk)
+    keep = {'alpha_g1': _mont_points([vk.alpha_g1], False), 'beta_g2': _mont_points([vk.beta_g2], True),
+            'gamma_g2': _mont_points([vk.gamma_g2], True), 'delta_g2': _mont_points([vk.delta_g2], True),
+            'gamma_abc_g1': _mont_points(vk.gamma_abc_g1, False)}
+    d = N.VkDesc()
+    d.n_public = len(vk.gamma_abc_g1) - 1
+    for name, arr in keep.items():
+        setattr(d, name, arr.ctypes.data)
+    return d, keep
+
+
+_LOAD_MANY_KEY = re.compile(r'b2g_vk_load_many: key (\d+): (.*)', re.S)
+
+
+def _refused_key(e):
+    """(the key's index in the call, the message b2g_vk_load gives for that key alone) of a b2g_vk_load_many error that names
+    a key, else (None, the message)"""
+    m = _LOAD_MANY_KEY.fullmatch(e.msg)
+    return (int(m.group(1)), m.group(2)) if m else (None, e.msg)
 
 
 def release(obj):
@@ -141,23 +170,42 @@ class Context:
 
     def vk_handle(self, key):
         """device verifying key for a verifier.VerifyingKey, PreparedVerifyingKey or ProvingKey (cached per host object)"""
-        from . import verifier
         cache_key = (id(key), self.device)
         if cache_key not in _VK_HANDLES:
-            vk = key.vk if isinstance(key, verifier.PreparedVerifyingKey) else key
-            if not isinstance(vk, verifier.VerifyingKey):
-                vk = verifier.VerifyingKey.from_proving_key(vk)
-            keep = {'alpha_g1': _mont_points([vk.alpha_g1], False), 'beta_g2': _mont_points([vk.beta_g2], True),
-                    'gamma_g2': _mont_points([vk.gamma_g2], True), 'delta_g2': _mont_points([vk.delta_g2], True),
-                    'gamma_abc_g1': _mont_points(vk.gamma_abc_g1, False)}
-            d = N.VkDesc()
-            d.n_public = len(vk.gamma_abc_g1) - 1
-            for name, arr in keep.items():
-                setattr(d, name, arr.ctypes.data)
+            d, keep = _vk_desc(key)
             h = C.c_void_p()
             N.check(N.lib().b2g_vk_load(self._h, C.byref(d), C.byref(h)))
             _VK_HANDLES[cache_key] = (h, key)
         return _VK_HANDLES[cache_key][0]
+
+    def vk_handles(self, keys) -> list:
+        """device verifying keys for many keys, each as vk_handle takes it: every key not yet cached on this device is loaded
+        in ONE b2g_vk_load_many call and cached as vk_handle caches it.  Returns the handles in the order of `keys`.  A key
+        the library refuses raises B2gError naming its first index in `keys`; then no key of the call is loaded."""
+        keys = list(keys)
+        loads, at = {}, []
+        for i, key in enumerate(keys):
+            cache_key = (id(key), self.device)
+            if cache_key not in _VK_HANDLES and cache_key not in loads:
+                loads[cache_key] = (key,) + _vk_desc(key)
+                at.append(i)
+        try:
+            self._vk_load_many(list(loads.values()))
+        except N.B2gError as e:
+            i, msg = _refused_key(e)
+            raise N.B2gError(e.code, msg if i is None else f"key {at[i]}: {msg}") from e
+        return [_VK_HANDLES[(id(key), self.device)][0] for key in keys]
+
+    def _vk_load_many(self, loads):
+        """loads = [(key, b2g_vk_desc, the arrays it points into)] of keys not cached on this device: one b2g_vk_load_many
+        call, then each handle cached as vk_handle caches it"""
+        if not loads:
+            return
+        descs = (N.VkDesc * len(loads))(*[d for _, d, _ in loads])
+        hs = (C.c_void_p * len(loads))()
+        N.check(N.lib().b2g_vk_load_many(self._h, len(loads), descs, hs))
+        for (key, _, _), h in zip(loads, hs):
+            _VK_HANDLES[(id(key), self.device)] = (C.c_void_p(h), key)
 
     def prepare(self, pk: ProvingKey, matrices: ConstraintMatrices, reduction_id: int = N.REDUCTION_CIRCOM) -> None:
         """load (pk, matrices) and allocate this context's scratch now instead of inside the first proof"""
@@ -303,6 +351,15 @@ def _proof_rows(fn, proofs, compressed) -> bytes:
 def _verify_args(fn, vk, public_inputs, proofs, ctx, compressed=False):
     """the argument checks and encoding the verifiers share: None for an empty batch, else (ctx, device key, count, public
     inputs as 32 B words or None, proofs as 256 B rows, or as 128 B rows when compressed)"""
+    args = _batch_args(fn, vk, public_inputs, proofs, compressed)
+    if args is None:
+        return None
+    ctx = ctx or default_context()
+    return (ctx, ctx.vk_handle(vk)) + args
+
+
+def _batch_args(fn, vk, public_inputs, proofs, compressed):
+    """_verify_args without the device key: None for an empty batch, else (count, public inputs, proof rows)"""
     from . import verifier
     public_inputs, proofs = [list(x) for x in public_inputs], list(proofs)
     if len(public_inputs) != len(proofs):
@@ -318,12 +375,10 @@ def _verify_args(fn, vk, public_inputs, proofs, ctx, compressed=False):
         for x in xs:
             if not 0 <= int(x) < R_MOD:        # the library refuses >= r too; this also covers values no 32 B word holds
                 raise N.B2gError(N.B2G_E_INPUT, f"public input {int(x)} is not in [0, r)")
-    ctx = ctx or default_context()
-    vh = ctx.vk_handle(vk)
     pub = b''.join(int(x).to_bytes(32, 'little') for xs in public_inputs for x in xs)
     pub_arr = np.frombuffer(pub, dtype=np.uint8).copy() if pub else None
     data = np.frombuffer(rows, dtype=np.uint8).copy()
-    return ctx, vh, len(proofs), pub_arr, data
+    return len(proofs), pub_arr, data
 
 
 # the library entry of each verifier, by (kind, compressed)
@@ -374,7 +429,11 @@ def _verify_one_key(fn, kind, vk, public_inputs, proofs, ctx, compressed, weight
 
 def _key_batches(fn, batches, ctx, weights, compressed):
     """the argument checks and encoding of the keyed verifiers: (ctx, number of batches, [(batch index, KeyBatch)] for the
-    batches that hold proofs, the arrays the KeyBatch rows point into)"""
+    batches that hold proofs, the arrays the KeyBatch rows point into).
+    Every batch's checks run first, in batch order, up to the first batch j that fails them (j = the number of batches when
+    none fails).  The keys of the batches before j that hold proofs and are not yet on the device then load in ONE
+    b2g_vk_load_many call.  A key the library refuses raises under the lowest batch that uses it; otherwise batch j raises
+    its own error.  So the errors, and which of them wins, are those of loading each batch's key as the batch is reached."""
     from . import verifier
     batches = [tuple(b) for b in batches]
     for k, b in enumerate(batches):
@@ -385,22 +444,40 @@ def _key_batches(fn, batches, ctx, weights, compressed):
         if len(weights) != len(batches):
             raise ValueError(f"{fn}: one weight list per key batch")
     ctx = ctx or default_context()
-    rows, keep = [], []
+    checked, loads, first_use, failure = [], {}, {}, None
     for k, (vk, public_inputs, proofs) in enumerate(batches):
         where = f"{fn}: key {k}"
-        proofs = list(proofs)
-        ws = None if weights is None else weights[k]
-        if ws is not None:
-            _check_weights(where, ws, len(proofs), f"{where}: ")
         try:
-            args = _verify_args(where, vk, public_inputs, proofs, ctx, compressed)
-        except N.B2gError as e:
-            raise N.B2gError(e.code, f"{where}: {e.msg}") from e
-        except verifier.MalformedVerifyingKey as e:
-            raise verifier.MalformedVerifyingKey(f"{where}: {e}") from e
-        if args is None:                       # an empty batch is not passed on
-            continue
-        _, vh, count, pub_arr, data = args
+            proofs = list(proofs)
+            ws = None if weights is None else weights[k]
+            if ws is not None:
+                _check_weights(where, ws, len(proofs), f"{where}: ")
+            try:
+                args = _batch_args(where, vk, public_inputs, proofs, compressed)
+                cache_key = (id(vk), ctx.device)
+                if args is not None and cache_key not in _VK_HANDLES and cache_key not in loads:
+                    loads[cache_key] = (vk,) + _vk_desc(vk)
+                    first_use[cache_key] = k
+            except N.B2gError as e:
+                raise N.B2gError(e.code, f"{where}: {e.msg}") from e
+            except verifier.MalformedVerifyingKey as e:
+                raise verifier.MalformedVerifyingKey(f"{where}: {e}") from e
+        except Exception as e:                 # raised once the keys of the batches before this one are loaded
+            failure = e
+            break
+        if args is not None:                   # an empty batch is not passed on
+            checked.append((k, vk, ws, args))
+    try:
+        ctx._vk_load_many(list(loads.values()))
+    except N.B2gError as e:
+        i, msg = _refused_key(e)
+        k = first_use[list(loads)[i or 0]]
+        raise N.B2gError(e.code, f"{fn}: key {k}: {msg}") from e
+    if failure is not None:
+        raise failure
+    rows, keep = [], []
+    for k, vk, ws, (count, pub_arr, data) in checked:
+        vh = _VK_HANDLES[(id(vk), ctx.device)][0]
         wb = _weight_bytes(ws, count)
         keep += [pub_arr, data, wb]
         rows.append((k, N.KeyBatch(vh.value, count, 0, _ptr(pub_arr).value if pub_arr is not None else None, _ptr(data).value,
@@ -622,6 +699,14 @@ class Groth16:
         (groups holding such a proof) / (2^128 - 1) when the weights are uniform.  Arguments, weights and errors as
         verify_batch; an empty batch gives []."""
         return _verify_one_key('verify_batch_locate', 'batch_locate', vk, public_inputs, proofs, ctx, False, weights)
+
+    @staticmethod
+    def load_verifying_keys(vks, ctx: Context = None) -> None:
+        """Prepare many verifying keys on the device in ONE device pass (b2g_vk_load_many), e.g. when a node starts: every key
+        (a VerifyingKey, PreparedVerifyingKey or ProvingKey) not yet on ctx's device is loaded and cached per object, as the
+        verifiers cache it, so that no verifier call has to load it.  A key with a point off its curve raises B2gError
+        (B2G_E_INPUT) naming its index in `vks`; then none of the keys is loaded.  release(vk) frees a key."""
+        (ctx or default_context()).vk_handles(vks)
 
     @staticmethod
     def verify_batch_keys(batches, ctx: Context = None, weights=None) -> list:

@@ -27,8 +27,10 @@
 // Parsing and key handling stay on the host; every field/curve operation of the proof runs in libb2groth.so.
 // Header-only; link with -lb2groth.
 #pragma once
+#include <algorithm>
 #include <cstdint>
 #include <cstring>
+#include <exception>
 #include <istream>
 #include <map>
 #include <memory>
@@ -379,21 +381,58 @@ typedef Reduction<B2G_REDUCTION_LIBSNARK> LibsnarkReduction;   // ark-groth16's 
 #include "ark_circom_ethereum.hpp"
 namespace ark_circom {
 
-// the key prepared on the device at first use (b2g_vk_load), kept in pvk.device
-inline b2g_vk* device_vk(const PreparedVerifyingKey& pvk, Gpu& gpu) {
-    if (void* h = pvk.device.find(gpu.ctx(), 0)) return (b2g_vk*)h;
+// the b2g_vk_desc of a prepared key (pointing into pvk.vk)
+inline b2g_vk_desc vk_desc(const PreparedVerifyingKey& pvk) {
     b2g_vk_desc d; memset(&d, 0, sizeof d);
     d.n_public = (uint32_t)(pvk.vk.gamma_abc_g1.size() - 1);
     d.alpha_g1 = &pvk.vk.alpha_g1; d.beta_g2 = &pvk.vk.beta_g2; d.gamma_g2 = &pvk.vk.gamma_g2; d.delta_g2 = &pvk.vk.delta_g2;
     d.gamma_abc_g1 = pvk.vk.gamma_abc_g1.data();
+    return d;
+}
+
+// the key prepared on the device at first use (b2g_vk_load), kept in pvk.device
+inline b2g_vk* device_vk(const PreparedVerifyingKey& pvk, Gpu& gpu) {
+    if (void* h = pvk.device.find(gpu.ctx(), 0)) return (b2g_vk*)h;
+    const b2g_vk_desc d = vk_desc(pvk);
     b2g_vk* vk = nullptr;
     check(b2g_vk_load(gpu.ctx(), &d, &vk));
     pvk.device.put(gpu.ctx(), 0, vk, [](void* p) { b2g_vk_free((b2g_vk*)p); });
     return vk;
 }
 
-// what the Groth16 verifiers share: the argument checks, the key on the device (device_vk) and the encoded public inputs
-// and proofs (P = Proof, 256-byte rows, or CompressedProof, 128-byte rows)
+// the keys of pvks not yet on gpu's device, prepared in ONE b2g_vk_load_many call and kept in each pvk.device as device_vk
+// keeps them (a key given twice loads once).  When the library refuses a key, nothing is loaded and a DeviceError carries
+// the message b2g_vk_load gives for that key alone, after "key i: " (i = its first index in pvks) when name_key is set.
+inline void device_vks(const std::vector<const PreparedVerifyingKey*>& pvks, Gpu& gpu, bool name_key) {
+    std::vector<const PreparedVerifyingKey*> todo;
+    std::vector<size_t> at;
+    std::vector<b2g_vk_desc> descs;
+    for (size_t i = 0; i < pvks.size(); i++) {
+        const PreparedVerifyingKey* p = pvks[i];
+        if (p->device.find(gpu.ctx(), 0) || std::find(todo.begin(), todo.end(), p) != todo.end()) continue;
+        todo.push_back(p); at.push_back(i); descs.push_back(vk_desc(*p));
+    }
+    if (todo.empty()) return;
+    std::vector<b2g_vk*> vks(todo.size());
+    const int rc = b2g_vk_load_many(gpu.ctx(), (uint32_t)todo.size(), descs.data(), vks.data());
+    if (rc != B2G_OK) {
+        // "b2g_vk_load_many: key k: <b2g_vk_load's message>" names the key; other messages name none
+        std::string msg = b2g_last_error();
+        const std::string head = "b2g_vk_load_many: key ";
+        size_t k = 0;
+        if (msg.compare(0, head.size(), head) == 0) {
+            size_t len = 0;
+            k = std::stoul(msg.substr(head.size()), &len);
+            msg = msg.substr(head.size() + len + 2);
+            if (name_key) msg = "key " + std::to_string(at[k]) + ": " + msg;
+        }
+        throw DeviceError(std::string("b2groth error ") + std::to_string(rc) + ": " + msg);
+    }
+    for (size_t i = 0; i < todo.size(); i++) todo[i]->device.put(gpu.ctx(), 0, vks[i], [](void* p) { b2g_vk_free((b2g_vk*)p); });
+}
+
+// what the Groth16 verifiers share: the argument checks, the key on the device (device_vk; left to the caller unless
+// `load`) and the encoded public inputs and proofs (P = Proof, 256-byte rows, or CompressedProof, 128-byte rows)
 struct VerifyCall {
     size_t n = 0;
     Gpu* gpu = nullptr;
@@ -402,7 +441,7 @@ struct VerifyCall {
     std::vector<uint8_t> bytes;
     template <class P>
     VerifyCall(const char* fn, const PreparedVerifyingKey& pvk, const std::vector<std::vector<Fr>>& public_inputs,
-               const std::vector<P>& proofs, int device) {
+               const std::vector<P>& proofs, int device, bool load = true) {
         static_assert(sizeof(P) == 256 || sizeof(P) == 128, "a proof row is 256 bytes, or 128 compressed");
         if (public_inputs.size() != proofs.size()) throw SynthesisError(std::string(fn) + ": one public-input list per proof");
         const size_t n_public = pvk.vk.gamma_abc_g1.size() - 1;
@@ -410,7 +449,7 @@ struct VerifyCall {
         for (const auto& xs : public_inputs) if (xs.size() != n_public) throw MalformedVerifyingKey();
         n = proofs.size();
         gpu = &Gpu::on(device);
-        vk = device_vk(pvk, *gpu);
+        if (load) vk = device_vk(pvk, *gpu);
         pub.resize(n * n_public);
         for (size_t i = 0; i < n; i++) for (size_t k = 0; k < n_public; k++) pub[i * n_public + k] = public_inputs[i][k].into_bigint();
         bytes.resize(n * sizeof(P));
@@ -440,7 +479,10 @@ typedef KeyBatchOf<Proof> KeyBatch;
 typedef KeyBatchOf<CompressedProof> CompressedKeyBatch;
 
 // the b2g_key_batch rows of the keyed verifiers for the batches that hold proofs (row i is batch at[i]), with the arrays
-// they point into; weights from std::random_device
+// they point into; weights from std::random_device.  Every batch's checks run first, in batch order, up to the first batch
+// that fails them; the keys of the batches before it that hold proofs then load in ONE b2g_vk_load_many call (device_vks).
+// A refused key throws; otherwise the failing batch throws its own error: the errors, and which of them wins, are those of
+// loading each batch's key as the batch is reached.
 struct KeysTable {
     std::vector<VerifyCall> calls;
     std::vector<std::vector<uint32_t>> weights;
@@ -450,11 +492,23 @@ struct KeysTable {
     template <class P>
     KeysTable(const char* fn, const std::vector<KeyBatchOf<P>>& batches, int device) {
         calls.reserve(batches.size());
-        for (size_t k = 0; k < batches.size(); k++) {
+        std::exception_ptr failure;
+        std::vector<const PreparedVerifyingKey*> pvks;
+        for (size_t k = 0; k < batches.size() && !failure; k++) {
             const std::string where = std::string(fn) + ": key " + std::to_string(k);
-            calls.emplace_back(where.c_str(), batches[k].pvk, batches[k].public_inputs, batches[k].proofs, device);
-            const VerifyCall& c = calls.back();
+            try {
+                calls.emplace_back(where.c_str(), batches[k].pvk, batches[k].public_inputs, batches[k].proofs, device, false);
+                if (calls.back().n) pvks.push_back(&batches[k].pvk);
+            } catch (...) {
+                failure = std::current_exception();
+            }
+        }
+        if (!pvks.empty()) device_vks(pvks, Gpu::on(device), false);
+        if (failure) std::rethrow_exception(failure);
+        for (size_t k = 0; k < batches.size(); k++) {
+            VerifyCall& c = calls[k];
             if (c.n == 0) continue;
+            c.vk = device_vk(batches[k].pvk, *c.gpu);     // loaded above
             weights.push_back(batch_weights(c.n));
             b2g_key_batch b; memset(&b, 0, sizeof b);
             b.vk = c.vk; b.count = (uint32_t)c.n;
@@ -556,9 +610,18 @@ struct Groth16T {                                       // Groth16::<Bn254, QAP>
                                                  const std::vector<Proof>& proofs, int device = 0) {
         return verify_one_key("verify_batch_locate", VerifyKind::locate, pvk, public_inputs, proofs, device);
     }
+    // process_vk on the device for many keys in ONE device pass (b2g_vk_load_many), e.g. when a node starts: every key not
+    // yet on the device is prepared and kept in its pvk.device, so that no verifier call has to prepare it.  A key with a point
+    // off its curve throws DeviceError naming its index in pvks; then none of the keys is loaded.
+    static void load_verifying_keys(const std::vector<PreparedVerifyingKey>& pvks, int device = 0) {
+        std::vector<const PreparedVerifyingKey*> ptrs;
+        for (const PreparedVerifyingKey& p : pvks) ptrs.push_back(&p);
+        if (!ptrs.empty()) device_vks(ptrs, Gpu::on(device), true);
+    }
     // verify_batch for many keys in ONE device pass (b2g_verify_batch_keys): one verdict per batch, equal to verify_batch on
     // that batch with the same weights; an invalid proof changes its own batch's verdict only, and an empty batch is true.
-    // Each key is prepared on the device at first use and kept in its pvk.device.  Weights from std::random_device.
+    // The keys not yet on the device are prepared in one b2g_vk_load_many call and kept in their pvk.device.  Weights from
+    // std::random_device.
     static std::vector<bool> verify_batch_keys(const std::vector<KeyBatch>& batches, int device = 0) {
         return batch_verdicts(verify_keys_call("verify_batch_keys", batches, false, device));
     }

@@ -19,6 +19,9 @@
 //       B2G_VERIFY_KEYS=K: also prove K proofs, split them into up to four batches of the key plus an empty one, negate A in
 //       the last proof of the second batch, and compare Groth16::verify_batch_keys's verdicts with the host verifier per
 //       batch (timing the keyed call)
+//       B2G_LOAD_KEYS=K: also prove K proofs, prepare K copies of the key on the device with Groth16::load_verifying_keys,
+//       negate A in every third proof, and compare Groth16::verify_batch_keys's verdicts (proof i under copy i) with the host
+//       verifier, printing the launches of both calls
 //       B2G_VERIFY_KEYS_LOCATE=K: also prove K proofs, split them into up to four batches of the key with an empty one after
 //       the first, negate A in the first proof of the first batch, the last proof of the others and proofs 63 and 64 of each
 //       batch that has them, and compare Groth16::verify_batch_keys_locate's verdicts with the host verifier per proof
@@ -402,6 +405,55 @@ int main(int argc, char** argv) {
             }
             std::printf("verify_keys %d proofs in %d batches: device=%s host=%s agree=%d, device %.3f ms/call (%.1f proofs/s)\n", k,
                         (int)nb + 1, dev.c_str(), host.c_str(), dev == host, dev_ms, k / (dev_ms / 1e3));
+        }
+        if (const char* lk = std::getenv("B2G_LOAD_KEYS")) {             // K keys prepared in one call, then verified, against the host
+            const int k = std::atoi(lk);
+            if (k < 1) throw SynthesisError("B2G_LOAD_KEYS must be >= 1");
+            std::vector<std::vector<Fr>> wv((size_t)k, full_assignment);
+            if (wsrc.rfind("chain:", 0) == 0)
+                for (int i = 1; i < k; i++) wv[(size_t)i] = chain_witness(params.a_query.size(), std::stoull(wsrc.substr(6)) + (unsigned long long)i);
+            std::vector<const std::vector<Fr>*> ws;
+            for (const auto& w : wv) ws.push_back(&w);
+            std::mt19937_64 rng(0x10AD);
+            std::vector<std::pair<Fr, Fr>> rs;
+            for (int i = 0; i < k; i++) rs.push_back({Fr::rand(rng), Fr::rand(rng)});
+            const std::vector<Proof> proofs = Groth16::create_proofs(params, matrices, rs, ws);
+            // k prepared copies of the bench key, each a separate device key; batch i holds proof i under copy i, with A -> -A
+            // in every third proof
+            const std::vector<PreparedVerifyingKey> pvks((size_t)k, Groth16::process_vk(params.vk));
+            std::vector<std::vector<std::vector<Fr>>> inputs((size_t)k);
+            std::vector<std::vector<Proof>> parts((size_t)k);
+            std::vector<KeyBatch> batches;
+            for (size_t i = 0; i < (size_t)k; i++) {
+                inputs[i].emplace_back(wv[i].begin() + 1, wv[i].begin() + num_inputs);
+                parts[i].push_back(proofs[i]);
+                if (i % 3 == 1) {
+                    Proof& bad = parts[i].back();
+                    uint64_t y[4], d[4]; memcpy(y, bad.bytes + 32, 32);
+                    unsigned __int128 borrow = 0;
+                    for (int j = 0; j < 4; j++) { unsigned __int128 t = (unsigned __int128)detail::FQ_P[j] - y[j] - borrow; d[j] = (uint64_t)t; borrow = (t >> 64) & 1; }
+                    memcpy(bad.bytes + 32, d, 32);
+                }
+            }
+            for (size_t i = 0; i < (size_t)k; i++) batches.push_back({pvks[i], inputs[i], parts[i]});
+            uint64_t l0 = 0, l1 = 0, l2 = 0;
+            check(b2g_launch_count(Gpu::instance().ctx(), &l0));
+            auto t1 = std::chrono::steady_clock::now();
+            Groth16::load_verifying_keys(pvks);
+            const double load_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t1).count();
+            check(b2g_launch_count(Gpu::instance().ctx(), &l1));
+            bool held = true;
+            for (const auto& p : pvks) held = held && p.device.find(Gpu::instance().ctx(), 0);
+            const std::vector<bool> got = Groth16::verify_batch_keys(batches);
+            check(b2g_launch_count(Gpu::instance().ctx(), &l2));
+            std::string dev, host;
+            for (size_t i = 0; i < (size_t)k; i++) {
+                dev += got[i] ? '1' : '0';
+                host += Groth16::verify_with_processed_vk(pvks[i], inputs[i][0], parts[i][0]) ? '1' : '0';
+            }
+            // the keyed call after load_verifying_keys loads nothing: it issues the launches of a call with preloaded keys
+            std::printf("load_keys %d keys: held=%d load_launches=%llu verify_launches=%llu device=%s host=%s agree=%d, load %.3f ms\n", k,
+                        held, (unsigned long long)(l1 - l0), (unsigned long long)(l2 - l1), dev.c_str(), host.c_str(), dev == host, load_ms);
         }
         if (const char* kl = std::getenv("B2G_VERIFY_KEYS_LOCATE")) {    // one verdict per proof over key batches, against the host
             const int k = std::atoi(kl);

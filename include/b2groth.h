@@ -15,6 +15,7 @@
  *   b2g_prove_many         <- the same function called for many witnesses of one circuit, in one device pass
  *   b2g_prove_partial / b2g_prove_finish : the same proof split for base-range sharding over several GPUs
  *   b2g_vk_load            <- GrothBn::process_vk(&params.vk) (src/zkey.rs:868, 914): the prepared verifying key, on the device
+ *   b2g_vk_load_many       <- the same for many keys in one device pass
  *   b2g_verify_many        <- GrothBn::verify_with_processed_vk(&pvk, &inputs, &proof) (src/zkey.rs:869-870, 915-916), called
  *                             for many proofs of one key in one device pass
  *   b2g_verify_batch       <- the same check for a whole batch at once, as one random linear combination of the proofs
@@ -213,6 +214,21 @@ typedef struct {
  * -delta for every Miller-loop step, and an 8-bit window table per gamma_abc_g1[i + 1] (510 KiB each).  Like b2g_pk, the key is
  * a device object any context of the same device can use. */
 B2G_API int b2g_vk_load(b2g_ctx* ctx, const b2g_vk_desc* desc, b2g_vk** out);
+/* b2g_vk_load_many <- process_vk for n_keys keys in one device pass, for nodes that see many circuits (rollup and bridge nodes,
+ * aggregators, verification layers whose clients send their keys with their proofs).  descs = n_keys descriptors (host);
+ * out = n_keys handles.  out[k] holds, byte for byte, the device state b2g_vk_load(ctx, &descs[k]) builds (the points,
+ * e(alpha, beta), the lines of -gamma and -delta, the window tables, which of gamma and delta are at infinity), and every call
+ * that takes a b2g_vk takes it.  The same desc may appear more than once; each occurrence gets its own handle.
+ * Memory: one device allocation per call, carved into every key's arrays (256-byte aligned).  Each handle holds a reference to
+ * it: b2g_vk_free frees the handles one at a time, in any order, and the last one frees the allocation.
+ * Cost: four kernel launches and two synchronises, whatever n_keys and the public-input counts: the on-curve checks of every
+ * point, e(alpha, beta) one key per thread, the lines two threads per key, and every window table of every key in one launch.
+ * b2g_vk_load is this call with one key.
+ * All or nothing: on any error no handle is created, out is not written and the context stays usable.  Errors: B2G_E_SHAPE for
+ * n_keys == 0 or a null pointer or field (the message names the key); B2G_E_INPUT for a point off its curve (the message
+ * names the lowest key that holds one, and the point as b2g_vk_load names it); B2G_E_DEVICE when the keys do not fit in device
+ * memory. */
+B2G_API int b2g_vk_load_many(b2g_ctx* ctx, uint32_t n_keys, const b2g_vk_desc* descs, b2g_vk** out);
 B2G_API int b2g_vk_free(b2g_vk* vk);
 /* e(alpha, beta) as the loaded key holds it (PreparedVerifyingKey::alpha_g1_beta_g2): 384 B, twelve Montgomery Fq in the
  * order c0.c0.c0, c0.c0.c1, c0.c1.c0, ..., c1.c2.c1 (host pointer) */
