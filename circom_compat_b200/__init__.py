@@ -10,3 +10,5 @@ from .r1cs import R1CSFile, R1CS, read_wtns  # noqa: F401
 from .builder import CircomConfig, CircomBuilder, CircomCircuit  # noqa: F401
 from .verifier import VerifyingKey, PreparedVerifyingKey, MalformedVerifyingKey  # noqa: F401
 from ._native import B2gError, PolynomialDegreeTooLarge  # noqa: F401
+from .ark_serialize import (serialize_proving_key, deserialize_proving_key, serialize_verifying_key,  # noqa: F401
+                            deserialize_verifying_key, deserialize_verifying_keys)

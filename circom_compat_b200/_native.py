@@ -54,7 +54,7 @@ EXPORTS = ['b2g_last_error', 'b2g_version', 'b2g_device_count', 'b2g_ctx_create'
            'b2g_verify_batch', 'b2g_proofs_decompress', 'b2g_verify_many_compressed', 'b2g_verify_batch_compressed',
            'b2g_verify_batch_locate', 'b2g_verify_batch_locate_compressed', 'b2g_verify_batch_keys',
            'b2g_verify_batch_keys_compressed', 'b2g_verify_batch_keys_locate', 'b2g_verify_batch_keys_locate_compressed',
-           'b2g_rerandomize_many']
+           'b2g_rerandomize_many', 'b2g_points_serialize', 'b2g_points_deserialize']
 
 _lib = None
 
@@ -118,6 +118,8 @@ def lib():
         L.b2g_verify_batch_keys_locate.argtypes = [vp, C.c_uint32, C.POINTER(KeyBatch), vp]
         L.b2g_verify_batch_keys_locate_compressed.argtypes = [vp, C.c_uint32, C.POINTER(KeyBatch), vp]
         L.b2g_rerandomize_many.argtypes = [vp, vp, C.c_uint32, vp, vp, vp, vp, vp]
+        L.b2g_points_serialize.argtypes = [vp, i, i, sz, vp, vp]
+        L.b2g_points_deserialize.argtypes = [vp, i, i, sz, vp, vp, C.POINTER(C.c_uint64)]
         _lib = L
     return _lib
 

@@ -608,6 +608,93 @@ __global__ void decompress_test_kernel(int op, const uint8_t* __restrict__ a, ui
     fe_store(o, flag);
 }
 
+// ---------------------------------------------------------------------------------------------- key points
+// b2g_points_serialize / b2g_points_deserialize: CanonicalSerialize / CanonicalDeserialize (Validate::Yes) of bare G1 or G2
+// affine points, the elements of a serialized ProvingKey<Bn254> or VerifyingKey<Bn254> (ark-groth16 0.5).  The compressed
+// form and its rules are those above COMP_BYTES.  The uncompressed form is x then y (G2: x.c0, x.c1, y.c0, y.c1) with the
+// point's flags on the last byte of y (of y.c1): bit 7 is written for the larger y and ignored on read, bit 6 = infinity
+// (zero coordinates on write), both set is invalid.  On read, every coordinate with the flags masked off must be below p,
+// even under the infinity flag; a point without the infinity flag must lie on its curve; a G2 point not at infinity must lie
+// in G2, in both forms (points_g2_subgroup_kernel).  One point per thread, in slices of at most KEY_SLICE points.
+constexpr size_t KEY_SLICE = size_t(1) << 20;
+
+__device__ __forceinline__ void as_elem(fe& r, const fe* c) { r = c[0]; }
+__device__ __forceinline__ void as_elem(fe2& r, const fe* c) { r.c0 = c[0]; r.c1 = c[1]; }
+
+// one point per thread: Montgomery point i (all zero = infinity) -> its canonical bytes with flags; a coordinate >= p lowers
+// *bad to base + i
+template <class F>
+__global__ void __launch_bounds__(128) points_serialize_kernel(const uint8_t* __restrict__ pts, uint32_t n, int compress, uint64_t base,
+                                                               uint8_t* __restrict__ out, unsigned long long* __restrict__ bad) {
+    constexpr int K = Bytes<F>::ELEM / 32;                 // Fq coordinates of one of x, y
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    fe c[2 * K];
+    bool ok = true, inf = true;
+    for (int k = 0; k < 2 * K; k++) {
+        c[k] = fe_load(pts + ((size_t)i * 2 * K + k) * 32);
+        ok &= fe_below_p(c[k]);
+        inf &= fe_equal(c[k], fe_zero());
+        c[k] = to_canon(c[k]);
+    }
+    if (!ok) { atomicMin(bad, (unsigned long long)(base + i)); return; }
+    typename F::elem y;
+    as_elem(y, c + K);
+    const int last = compress ? K - 1 : 2 * K - 1;         // the coordinate that carries the flags
+    c[last].l[7] |= inf ? 0x40000000u : (y_is_larger(y) ? 0x80000000u : 0u);
+    uint8_t* o = out + (size_t)i * (last + 1) * 32;
+    for (int k = 0; k <= last; k++) fe_store(o + 32 * k, c[k]);
+}
+
+// one point per thread: serialized point i -> Montgomery point i (all zero = infinity), or zeros and *bad lowered to base + i
+// when it does not decode.  No subgroup check: points_g2_subgroup_kernel adds it for G2.
+template <class C, class F, bool COMPRESS>
+__global__ void __launch_bounds__(128) points_deserialize_kernel(const uint8_t* __restrict__ in, uint32_t n, uint64_t base,
+                                                                 uint8_t* __restrict__ pts, unsigned long long* __restrict__ bad) {
+    constexpr int K = Bytes<F>::ELEM / 32;
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    fe c[2 * K];
+    for (int k = 0; k < 2 * K; k++) c[k] = fe_zero();
+    const uint8_t* p = in + (size_t)i * (COMPRESS ? K : 2 * K) * 32;
+    bool ok;
+    if constexpr (COMPRESS) {
+        if constexpr (K == 1) ok = g1_decompress(c, p); else ok = g2_decompress(c, p);
+        for (int k = 0; k < 2 * K; k++) c[k] = to_mont(c[k]);
+    } else {
+        uint32_t f;
+        for (int k = 0; k < 2 * K - 1; k++) c[k] = fe_load(p + 32 * k);
+        c[2 * K - 1] = comp_load(p + 32 * (2 * K - 1), f);
+        ok = f != 3;
+        for (int k = 0; k < 2 * K; k++) ok &= fe_below_p(c[k]);
+        if (ok && (f & 1)) {
+            for (int k = 0; k < 2 * K; k++) c[k] = fe_zero();
+        } else if (ok) {
+            Affine<F> a;
+            for (int k = 0; k < 2 * K; k++) c[k] = to_mont(c[k]);
+            as_elem(a.x, c); as_elem(a.y, c + K);
+            ok = !C::aff_is_inf(a) && aff_on_curve<C, F>(a);   // (0, 0) without the infinity flag is off the curve
+        }
+    }
+    if (!ok) {
+        atomicMin(bad, (unsigned long long)(base + i));
+        for (int k = 0; k < 2 * K; k++) c[k] = fe_zero();
+    }
+    for (int k = 0; k < 2 * K; k++) fe_store(pts + ((size_t)i * 2 * K + k) * 32, c[k]);
+}
+
+// G2 membership of every decoded point, one point per thread, in its own kernel so that the decoder does not carry
+// g2_in_subgroup's registers and stack (as decompress_g2_kernel); points that did not decode are zeros and are skipped
+__global__ void __launch_bounds__(128) points_g2_subgroup_kernel(const uint8_t* __restrict__ pts, uint32_t n, uint64_t base,
+                                                                 unsigned long long* __restrict__ bad) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const G2::Aff q = aff_load<Fq2>(pts, i);
+    if (G2::aff_is_inf(q) || g2_in_subgroup(q)) return;
+    // the index again from the special registers, so that no value has to live across the call
+    atomicMin(bad, (unsigned long long)(base + blockIdx.x * blockDim.x + threadIdx.x));
+}
+
 // ---------------------------------------------------------------------------------------------- rerandomization
 // b2g_rerandomize_many: ark-groth16 0.5.0's Groth16::rerandomize_proof for a proof (A, B, C) and nonzero factors r1, r2:
 //     A' = r1^-1 A,   B' = r1 B + (r1 r2) delta_2,   C' = C + r2 A
@@ -1113,6 +1200,46 @@ static void vk_load_many(b2g_ctx* ctx, uint32_t n_keys, const b2g_vk_desc* descs
     for (uint32_t k = 0; k < n_keys; k++) out[k] = vks[k].release();
 }
 
+// the slice loop of b2g_points_serialize / b2g_points_deserialize: one device allocation of min(n, KEY_SLICE) input rows,
+// as many output rows and the bad-index word, reused by every slice.  Per slice: the upload, run(d_in, d_out, count, base,
+// d_bad, st), the download and one synchronise; a slice with a bad point ends the loop, as no later point can be lower.
+// Returns the lowest bad index, or n.
+template <class Run>
+static uint64_t points_slices(const char* fn, b2g_ctx* ctx, size_t n, size_t in_row, size_t out_row, const void* in, void* out, Run&& run) {
+    const CtxView cv = ctx_view(ctx);
+    if (cv.proof_pending) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
+    if (n == 0) return 0;
+    DevGuard g(cv.device);
+    cudaStream_t st = cv.st;
+    const size_t slice = std::min(n, KEY_SLICE), bytes = slice * (in_row + out_row) + 8;
+    struct Buf { uint8_t* p = nullptr; ~Buf() { if (p) cudaFree(p); } } b;
+    if (cudaMalloc(&b.p, bytes) != cudaSuccess) {
+        cudaGetLastError();
+        b.p = nullptr;
+        throw_error(B2G_E_DEVICE, std::string(fn) + ": the device buffer of " + std::to_string(slice) + " points (" +
+                                  std::to_string((bytes + (1 << 20) - 1) >> 20) + " MiB) does not fit in device memory");
+    }
+    uint8_t *d_in = b.p, *d_out = b.p + slice * in_row;
+    unsigned long long* d_bad = reinterpret_cast<unsigned long long*>(d_out + slice * out_row);
+    uint64_t bad = n;
+    try {
+        CUDA_CHECK(cudaMemcpyAsync(d_bad, &bad, 8, cudaMemcpyHostToDevice, st));
+        for (size_t base = 0; base < n && bad == n; base += slice) {
+            const size_t m = std::min(slice, n - base);
+            CUDA_CHECK(cudaMemcpyAsync(d_in, (const uint8_t*)in + base * in_row, m * in_row, cudaMemcpyHostToDevice, st));
+            run(d_in, d_out, (uint32_t)m, (uint64_t)base, d_bad, st);
+            CUDA_CHECK(cudaGetLastError());
+            CUDA_CHECK(cudaMemcpyAsync((uint8_t*)out + base * out_row, d_out, m * out_row, cudaMemcpyDeviceToHost, st));
+            CUDA_CHECK(cudaMemcpyAsync(&bad, d_bad, 8, cudaMemcpyDeviceToHost, st));
+            CUDA_CHECK(cudaStreamSynchronize(st));
+        }
+    } catch (...) {
+        cudaStreamSynchronize(st);                         // nothing may still use the buffer when it is freed
+        throw;
+    }
+    return bad;
+}
+
 }  // namespace b2g
 
 extern "C" {
@@ -1177,6 +1304,39 @@ int b2g_proofs_decompress(b2g_ctx* ctx, uint32_t count, const void* compressed, 
         CUDA_CHECK(cudaMemcpyAsync(proofs_out, v.d_proofs, (size_t)count * 256, cudaMemcpyDeviceToHost, st));
         CUDA_CHECK(cudaMemcpyAsync(ok_out, ok, count, cudaMemcpyDeviceToHost, st));
         CUDA_CHECK(cudaStreamSynchronize(st));
+    });
+}
+
+int b2g_points_serialize(b2g_ctx* ctx, int g2, int compress, size_t n, const void* points_mont, void* out) {
+    return guarded([&] {
+        static const char* fn = "b2g_points_serialize";
+        if (!ctx || !points_mont || !out) throw_error(B2G_E_SHAPE, std::string(fn) + ": null pointer");
+        const size_t e = g2 ? 64 : 32;                     // bytes of one of x, y
+        const uint64_t bad = points_slices(fn, ctx, n, 2 * e, compress ? e : 2 * e, points_mont, out,
+            [&](const uint8_t* d_in, uint8_t* d_out, uint32_t m, uint64_t base, unsigned long long* d_bad, cudaStream_t st) {
+                if (g2) points_serialize_kernel<Fq2><<<(m + 127) / 128, 128, 0, st>>>(d_in, m, compress, base, d_out, d_bad);
+                else points_serialize_kernel<Fq><<<(m + 127) / 128, 128, 0, st>>>(d_in, m, compress, base, d_out, d_bad);
+                g_launch_count += 1;
+            });
+        if (bad < n) throw_error(B2G_E_INPUT, std::string(fn) + ": point " + std::to_string(bad) + " has a coordinate >= p");
+    });
+}
+
+int b2g_points_deserialize(b2g_ctx* ctx, int g2, int compress, size_t n, const void* in, void* points_out, uint64_t* first_bad_out) {
+    return guarded([&] {
+        static const char* fn = "b2g_points_deserialize";
+        if (!ctx || !in || !points_out || !first_bad_out) throw_error(B2G_E_SHAPE, std::string(fn) + ": null pointer");
+        const size_t e = g2 ? 64 : 32;
+        *first_bad_out = points_slices(fn, ctx, n, compress ? e : 2 * e, 2 * e, in, points_out,
+            [&](const uint8_t* d_in, uint8_t* d_out, uint32_t m, uint64_t base, unsigned long long* d_bad, cudaStream_t st) {
+                const unsigned blocks = (m + 127) / 128;
+                if (g2 && compress) points_deserialize_kernel<G2, Fq2, true><<<blocks, 128, 0, st>>>(d_in, m, base, d_out, d_bad);
+                else if (g2) points_deserialize_kernel<G2, Fq2, false><<<blocks, 128, 0, st>>>(d_in, m, base, d_out, d_bad);
+                else if (compress) points_deserialize_kernel<G1, Fq, true><<<blocks, 128, 0, st>>>(d_in, m, base, d_out, d_bad);
+                else points_deserialize_kernel<G1, Fq, false><<<blocks, 128, 0, st>>>(d_in, m, base, d_out, d_bad);
+                if (g2) points_g2_subgroup_kernel<<<blocks, 128, 0, st>>>(d_out, m, base, d_bad);
+                g_launch_count += g2 ? 2 : 1;
+            });
     });
 }
 

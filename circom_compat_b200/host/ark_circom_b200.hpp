@@ -22,6 +22,9 @@
 //   ark_circom::Groth16::rerandomize_proof / rerandomize_many <- Groth16::rerandomize_proof (ark-groth16 0.5.0), many
 //                                              proofs of one key in one device pass
 //   ark_circom::serialize_compressed          <- Proof::<Bn254>::serialize_compressed (ark_circom_ethereum.hpp)
+//   ark_circom::serialize_proving_key / deserialize_proving_key / serialize_verifying_key / deserialize_verifying_key(s)
+//                                             <- CanonicalSerialize / CanonicalDeserialize (ark-serialize 0.5, Validate::Yes)
+//                                                of ProvingKey<Bn254> / VerifyingKey<Bn254>, points decoded on the device
 //   ark_circom::read_wtns                              <- snarkjs .wtns (test-vectors/circuit2_js/witness.wtns; the reference
 //                                                         computes witnesses with WASM instead, out of scope here)
 // Parsing and key handling stay on the host; every field/curve operation of the proof runs in libb2groth.so.
@@ -36,8 +39,10 @@
 #include <memory>
 #include <optional>
 #include <random>
+#include <sstream>
 #include <stdexcept>
 #include <string>
+#include <tuple>
 #include <utility>
 #include <vector>
 
@@ -846,5 +851,197 @@ struct R1CS {
         return m;
     }
 };
+
+// ---------------------------------------------------------------------------------------------- ark-serialize keys
+// serialize_proving_key / serialize_verifying_key    <- pk.serialize_compressed(&mut w) / serialize_uncompressed (ark-serialize 0.5)
+// deserialize_proving_key / deserialize_verifying_key <- ProvingKey / VerifyingKey::<Bn254>::deserialize_compressed(&mut r) /
+//                                                      deserialize_uncompressed (Validate::Yes)
+// deserialize_verifying_keys                          <- the same for many keys, decoded in two device calls
+// The layout is ark_serialize.py's (fields in declaration order, h_query before l_query, a Vec = u64 length then its
+// elements); the host parses lengths only, and every point is encoded or decoded on the device (b2g_points_serialize /
+// b2g_points_deserialize): all G1 points of a call in one device call, all G2 points in one more.  A refusal throws
+// SerializationError naming the field and index ("b_g2_query[17]: ...").
+namespace detail {
+struct KeyField { const char* name; bool vec, g2; };
+static const KeyField VK_FIELDS[] = {{"alpha_g1", false, false}, {"beta_g2", false, true}, {"gamma_g2", false, true},
+                                     {"delta_g2", false, true}, {"gamma_abc_g1", true, false}};
+static const KeyField PK_FIELDS[] = {{"alpha_g1", false, false}, {"beta_g2", false, true}, {"gamma_g2", false, true},
+                                     {"delta_g2", false, true}, {"gamma_abc_g1", true, false}, {"beta_g1", false, false},
+                                     {"delta_g1", false, false}, {"a_query", true, false}, {"b_g1_query", true, false},
+                                     {"b_g2_query", true, true}, {"h_query", true, false}, {"l_query", true, false}};
+inline size_t point_size(bool g2, bool compress) { return (g2 ? 64 : 32) * (compress ? 1 : 2); }
+
+// the points of one field of one key: Montgomery rows (on write) or serialized bytes (on read), and their number
+struct FieldPoints { const KeyField* f; const uint8_t* data; size_t count; };
+
+inline std::vector<FieldPoints> vk_points(const VerifyingKey& vk) {
+    return {{&VK_FIELDS[0], (const uint8_t*)&vk.alpha_g1, 1}, {&VK_FIELDS[1], (const uint8_t*)&vk.beta_g2, 1},
+            {&VK_FIELDS[2], (const uint8_t*)&vk.gamma_g2, 1}, {&VK_FIELDS[3], (const uint8_t*)&vk.delta_g2, 1},
+            {&VK_FIELDS[4], (const uint8_t*)vk.gamma_abc_g1.data(), vk.gamma_abc_g1.size()}};
+}
+
+inline std::vector<uint8_t> encode_key(const std::vector<FieldPoints>& fields, bool compress, int device) {
+    std::vector<uint8_t> enc[2];
+    for (int g2 = 0; g2 < 2; g2++) {
+        std::vector<uint8_t> pts;
+        for (const FieldPoints& fp : fields) if (fp.f->g2 == (bool)g2) pts.insert(pts.end(), fp.data, fp.data + fp.count * (g2 ? 128 : 64));
+        const size_t n = pts.size() / (g2 ? 128 : 64);
+        enc[g2].resize(n * point_size(g2, compress));
+        if (n) check(b2g_points_serialize(Gpu::on(device).ctx(), g2, compress, n, pts.data(), enc[g2].data()));
+    }
+    std::vector<uint8_t> out;
+    size_t at[2] = {0, 0};
+    for (const FieldPoints& fp : fields) {
+        const int g2 = fp.f->g2;
+        if (fp.f->vec) { const uint64_t c = fp.count; const uint8_t* b = (const uint8_t*)&c; out.insert(out.end(), b, b + 8); }
+        const size_t bytes = fp.count * point_size(g2, compress);
+        out.insert(out.end(), enc[g2].begin() + at[g2], enc[g2].begin() + at[g2] + bytes);
+        at[g2] += bytes;
+    }
+    return out;
+}
+
+// the serialized points of every field, length prefixes parsed; the input is read in chunks, so a huge length prefix
+// never allocates its size
+inline std::vector<std::pair<uint64_t, std::vector<uint8_t>>> parse_key(std::istream& r, const KeyField* fields, size_t n_fields,
+                                                                       bool compress, const std::string& at) {
+    std::vector<std::pair<uint64_t, std::vector<uint8_t>>> out;
+    for (size_t k = 0; k < n_fields; k++) {
+        const KeyField& f = fields[k];
+        uint64_t count = 1;
+        if (f.vec) {
+            r.read(reinterpret_cast<char*>(&count), 8);
+            if (r.gcount() != 8) throw SerializationError(at + f.name + ": the input ends in the length");
+        }
+        const size_t size = point_size(f.g2, compress);
+        std::vector<uint8_t> raw;
+        for (uint64_t left = count; left;) {
+            const uint64_t m = std::min<uint64_t>(left, (1u << 26) / size);
+            const size_t have = raw.size();
+            raw.resize(have + m * size);
+            r.read(reinterpret_cast<char*>(raw.data() + have), (std::streamsize)(m * size));
+            if ((size_t)r.gcount() != m * size) throw SerializationError(at + f.name + ": the input ends before its " + std::to_string(count) + " points");
+            left -= m;
+        }
+        out.push_back({count, std::move(raw)});
+    }
+    return out;
+}
+
+// decodes the points of every key (keys[k][field] from parse_key) in two device calls: decoded[k][field] = Montgomery rows.
+// The refused point that comes first in serialized order throws.
+inline std::vector<std::vector<std::vector<uint8_t>>> decode_keys(const std::vector<std::vector<std::pair<uint64_t, std::vector<uint8_t>>>>& keys,
+                                                                  const KeyField* fields, size_t n_fields, bool compress,
+                                                                  const std::vector<std::string>& ats, int device) {
+    std::vector<std::vector<std::vector<uint8_t>>> out(keys.size(), std::vector<std::vector<uint8_t>>(n_fields));
+    std::tuple<size_t, size_t, uint64_t> first_bad{SIZE_MAX, 0, 0};
+    for (int g2 = 0; g2 < 2; g2++) {
+        std::vector<uint8_t> raw;
+        size_t n = 0;
+        for (const auto& key : keys)
+            for (size_t f = 0; f < n_fields; f++)
+                if (fields[f].g2 == (bool)g2) { raw.insert(raw.end(), key[f].second.begin(), key[f].second.end()); n += key[f].first; }
+        if (!n) continue;
+        const size_t row = g2 ? 128 : 64;
+        std::vector<uint8_t> pts(n * row);
+        uint64_t bad = n;
+        check(b2g_points_deserialize(Gpu::on(device).ctx(), g2, compress, n, raw.data(), pts.data(), &bad));
+        size_t o = 0;
+        for (size_t k = 0; k < keys.size(); k++)
+            for (size_t f = 0; f < n_fields; f++) {
+                if (fields[f].g2 != (bool)g2) continue;
+                const uint64_t c = keys[k][f].first;
+                if (bad >= o && bad < o + c) first_bad = std::min(first_bad, std::make_tuple(k, f, bad - o));
+                out[k][f].assign(pts.begin() + o * row, pts.begin() + (o + c) * row);
+                o += c;
+            }
+    }
+    if (std::get<0>(first_bad) != SIZE_MAX) {
+        const auto [k, f, i] = first_bad;
+        throw SerializationError(ats[k] + fields[f].name + (fields[f].vec ? "[" + std::to_string(i) + "]" : std::string()) +
+                                 ": not a valid " + (compress ? "compressed " : "uncompressed ") + (fields[f].g2 ? "G2" : "G1") + " point (Validate::Yes)");
+    }
+    return out;
+}
+
+template <class T> inline void rows_into(T& dst, const std::vector<uint8_t>& rows) { memcpy(&dst, rows.data(), sizeof(T)); }
+template <class T> inline void rows_into(std::vector<T>& dst, const std::vector<uint8_t>& rows) {
+    dst.resize(rows.size() / sizeof(T));
+    if (!dst.empty()) memcpy(dst.data(), rows.data(), rows.size());
+}
+
+inline VerifyingKey vk_from(const std::vector<std::vector<uint8_t>>& d) {
+    VerifyingKey vk;
+    rows_into(vk.alpha_g1, d[0]); rows_into(vk.beta_g2, d[1]); rows_into(vk.gamma_g2, d[2]); rows_into(vk.delta_g2, d[3]);
+    rows_into(vk.gamma_abc_g1, d[4]);
+    return vk;
+}
+
+inline void check_gamma_abc(uint64_t count, const std::string& at) {
+    if (count == 0) throw SerializationError(at + "gamma_abc_g1: empty (a key has at least the constant term's point)");
+}
+}  // namespace detail
+
+inline std::vector<uint8_t> serialize_verifying_key(const VerifyingKey& vk, bool compress = true, int device = 0) {
+    return detail::encode_key(detail::vk_points(vk), compress, device);
+}
+
+inline std::vector<uint8_t> serialize_proving_key(const ProvingKey& pk, bool compress = true, int device = 0) {
+    std::vector<detail::FieldPoints> f = detail::vk_points(pk.vk);
+    const detail::KeyField* F = detail::PK_FIELDS;
+    f.push_back({&F[5], (const uint8_t*)&pk.beta_g1, 1});
+    f.push_back({&F[6], (const uint8_t*)&pk.delta_g1, 1});
+    f.push_back({&F[7], (const uint8_t*)pk.a_query.data(), pk.a_query.size()});
+    f.push_back({&F[8], (const uint8_t*)pk.b_g1_query.data(), pk.b_g1_query.size()});
+    f.push_back({&F[9], (const uint8_t*)pk.b_g2_query.data(), pk.b_g2_query.size()});
+    f.push_back({&F[10], (const uint8_t*)pk.h_query.data(), pk.h_query.size()});
+    f.push_back({&F[11], (const uint8_t*)pk.l_query.data(), pk.l_query.size()});
+    return detail::encode_key(f, compress, device);
+}
+
+// the reader is left just past the key; gamma_abc_g1 must hold at least one point
+inline VerifyingKey deserialize_verifying_key(std::istream& r, bool compress = true, int device = 0) {
+    auto key = detail::parse_key(r, detail::VK_FIELDS, 5, compress, "");
+    detail::check_gamma_abc(key[4].first, "");
+    return detail::vk_from(detail::decode_keys({key}, detail::VK_FIELDS, 5, compress, {""}, device)[0]);
+}
+
+// many keys, every G1 point in one device call and every G2 point in one more; a refusal names the key ("key 3: ...")
+inline std::vector<VerifyingKey> deserialize_verifying_keys(const std::vector<std::vector<uint8_t>>& blobs, bool compress = true, int device = 0) {
+    std::vector<std::vector<std::pair<uint64_t, std::vector<uint8_t>>>> keys;
+    std::vector<std::string> ats;
+    for (size_t k = 0; k < blobs.size(); k++) {
+        std::istringstream r(std::string(blobs[k].begin(), blobs[k].end()));
+        ats.push_back("key " + std::to_string(k) + ": ");
+        keys.push_back(detail::parse_key(r, detail::VK_FIELDS, 5, compress, ats.back()));
+        detail::check_gamma_abc(keys.back()[4].first, ats.back());
+    }
+    std::vector<VerifyingKey> out;
+    if (keys.empty()) return out;
+    for (const auto& d : detail::decode_keys(keys, detail::VK_FIELDS, 5, compress, ats, device)) out.push_back(detail::vk_from(d));
+    return out;
+}
+
+// the reader is left just past the key.  Keys whose vector lengths disagree (b_g1_query or b_g2_query not of a_query's
+// length, l_query not of len(a_query) - len(gamma_abc_g1) points, an empty gamma_abc_g1) are refused although arkworks
+// reads them: no proof can be made with such a key.  The key carries no reduction; it proves under the one the caller picks.
+inline ProvingKey deserialize_proving_key(std::istream& r, bool compress = true, int device = 0) {
+    auto key = detail::parse_key(r, detail::PK_FIELDS, 12, compress, "");
+    detail::check_gamma_abc(key[4].first, "");
+    const uint64_t n_vars = key[7].first, n_ic = key[4].first;
+    if (n_ic > n_vars) throw SerializationError("gamma_abc_g1: " + std::to_string(n_ic) + " points, more than a_query's " + std::to_string(n_vars));
+    const std::pair<size_t, uint64_t> want[] = {{8, n_vars}, {9, n_vars}, {11, n_vars - n_ic}};
+    for (const auto& [f, n] : want)
+        if (key[f].first != n)
+            throw SerializationError(std::string(detail::PK_FIELDS[f].name) + ": " + std::to_string(key[f].first) +
+                                     " points, the key's a_query and gamma_abc_g1 need " + std::to_string(n));
+    const auto d = detail::decode_keys({key}, detail::PK_FIELDS, 12, compress, {""}, device)[0];
+    ProvingKey pk;
+    pk.vk = detail::vk_from(d);
+    detail::rows_into(pk.beta_g1, d[5]); detail::rows_into(pk.delta_g1, d[6]);
+    detail::rows_into(pk.a_query, d[7]); detail::rows_into(pk.b_g1_query, d[8]); detail::rows_into(pk.b_g2_query, d[9]);
+    detail::rows_into(pk.h_query, d[10]); detail::rows_into(pk.l_query, d[11]);
+    return pk;
+}
 
 }  // namespace ark_circom

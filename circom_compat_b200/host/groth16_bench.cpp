@@ -28,6 +28,9 @@
 //       (timing the keyed locate call)
 //       B2G_RERANDOMIZE=K: also prove K proofs, rerandomize them with Groth16::rerandomize_many (factors from std::mt19937_64
 //       seeded with 0x5EED), print every input and output row in hex, and check the outputs with the host verifier
+//       B2G_ARK_KEYS=path: also write the key with serialize_proving_key, compressed to path.compressed and uncompressed to
+//       path.uncompressed, read each back with deserialize_proving_key, and print its size, its FNV-1a digest and whether
+//       the key read back is identical
 //       chain:<a> = the witness of the reference's squaring-chain bench family for input a
 //       (test-vectors/complex-circuit/input.json has a = 3), computed on the host instead of by WASM.
 #include <algorithm>
@@ -540,6 +543,32 @@ int main(int argc, char** argv) {
                 changed += memcmp(q.bytes, proofs[(size_t)i].bytes, 256) != 0;
             }
             std::printf("rerandomize %d proofs: valid=%d changed=%d, device %.3f ms/call (with the key load)\n", k, valid, changed, dev_ms);
+        }
+        if (const char* ak = std::getenv("B2G_ARK_KEYS")) {              // the key in both ark-serialize forms, written and read back
+            auto same = [](const auto& a, const auto& b) { return a.size() == b.size() && (a.empty() || !memcmp(a.data(), b.data(), a.size() * sizeof(a[0]))); };
+            for (int z = 1; z >= 0; z--) {
+                const std::string path = std::string(ak) + (z ? ".compressed" : ".uncompressed");
+                auto t1 = std::chrono::steady_clock::now();
+                const std::vector<uint8_t> bytes = serialize_proving_key(params, z);
+                {
+                    std::ofstream of(path, std::ios::binary);
+                    of.write((const char*)bytes.data(), (std::streamsize)bytes.size());
+                    if (!of) throw SerializationError("cannot write " + path);
+                }
+                std::ifstream in(path, std::ios::binary);
+                const ProvingKey back = deserialize_proving_key(in, z);
+                const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t1).count();
+                const VerifyingKey &v1 = params.vk, &v2 = back.vk;
+                const bool identical = !memcmp(&v1.alpha_g1, &v2.alpha_g1, 64) && !memcmp(&v1.beta_g2, &v2.beta_g2, 128) &&
+                                       !memcmp(&v1.gamma_g2, &v2.gamma_g2, 128) && !memcmp(&v1.delta_g2, &v2.delta_g2, 128) &&
+                                       same(v1.gamma_abc_g1, v2.gamma_abc_g1) && !memcmp(&params.beta_g1, &back.beta_g1, 64) &&
+                                       !memcmp(&params.delta_g1, &back.delta_g1, 64) && same(params.a_query, back.a_query) &&
+                                       same(params.b_g1_query, back.b_g1_query) && same(params.b_g2_query, back.b_g2_query) &&
+                                       same(params.h_query, back.h_query) && same(params.l_query, back.l_query) &&
+                                       in.tellg() == (std::streampos)bytes.size();
+                std::printf("ark_keys %s bytes=%zu fnv=%016llx identical=%d, write + read %.1f ms\n", z ? "compressed" : "uncompressed",
+                            bytes.size(), (unsigned long long)fnv(bytes.data(), bytes.size()), identical ? 1 : 0, ms);
+            }
         }
         return 0;
     } catch (const std::exception& e) {

@@ -27,6 +27,8 @@
  *   b2g_verify_batch_keys_locate (+ _compressed) <- b2g_verify_batch_locate for many keys, one verdict per proof, in one
  *                             device pass
  *   b2g_rerandomize_many   <- Groth16::rerandomize_proof (ark-groth16 0.5.0) for many proofs of one key, in one device pass
+ *   b2g_points_serialize / b2g_points_deserialize <- CanonicalSerialize / CanonicalDeserialize (ark-serialize 0.5,
+ *                             Validate::Yes) of the G1 / G2 points of a ProvingKey<Bn254> or VerifyingKey<Bn254>
  *   b2g_fixed_base_g1/g2  <- the batch fixed-base multiplications of generate_random_parameters_with_reduction
  *                             (tests/groth16.rs:25); used to manufacture synthetic proving keys
  *
@@ -292,6 +294,30 @@ B2G_API int b2g_verify_many_compressed(b2g_ctx* ctx, b2g_vk* vk, uint32_t count,
  * proof decodes and b2g_verify_batch with the same weights gives 1 on the decoded rows. */
 B2G_API int b2g_verify_batch_compressed(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* public_inputs,
                                         const void* compressed, const void* weights, uint8_t* verdict_out);
+
+/* Key points: the points of an arkworks-serialized ProvingKey<Bn254> / VerifyingKey<Bn254> (ark-groth16 0.5), for callers
+ * that load or store such keys; the lengths and field order of the keys are parsed on the host (ark_serialize.py).  A
+ * compressed point follows the rules of the compressed proofs above: G1 = x (32 B), G2 = x.c0, x.c1 (64 B), flags on the
+ * last byte of x (of x.c1).  An uncompressed point is G1 = x, y (64 B) or G2 = x.c0, x.c1, y.c0, y.c1 (128 B), flags on the
+ * last byte of y (of y.c1); bit 7 is written for the larger y and ignored on read.  A point at infinity is written as zero
+ * coordinates with bit 6 set.  Both calls work in slices of a fixed number of points through one device buffer, so a key of
+ * any size needs a bounded amount of device memory; they are synchronous, and every error leaves the context usable.
+ *
+ * b2g_points_serialize <- G1Affine / G2Affine::serialize_with_mode (ark-ec 0.5, CanonicalSerialize) for n points.  g2 = 0:
+ * G1, 1: G2; compress = 0 or 1.  points_mont = n x 64 / 128 B (the b2g_pk_desc layout, all-zero = infinity); out = n x 32 /
+ * 64 B (compressed) or 64 / 128 B (uncompressed).  Errors: B2G_E_SHAPE for null pointers or a proof pending on the context;
+ * B2G_E_INPUT for a coordinate >= p (the message names the lowest such point); B2G_E_DEVICE when the buffer does not fit.
+ *
+ * b2g_points_deserialize <- G1Affine / G2Affine::deserialize_with_mode (ark-ec 0.5, CanonicalDeserialize, Validate::Yes) for
+ * n points without any length prefix.  in = n points of the form above; points_out = n x 64 / 128 B Montgomery (all-zero =
+ * infinity).  A point does not decode when both flag bits are set, a coordinate with its flags masked off is >= p (with the
+ * infinity flag too), a compressed x has no y, an uncompressed point without the infinity flag is off its curve, or a G2
+ * point not at infinity lies outside the order-r subgroup (G1 has cofactor 1).  *first_bad_out = the index of the lowest
+ * point that does not decode, or n; such a point is not an error code.  points_out[i] is defined for i < *first_bad_out.
+ * Errors: B2G_E_SHAPE for null pointers or a proof pending on the context; B2G_E_DEVICE when the buffer does not fit. */
+B2G_API int b2g_points_serialize(b2g_ctx* ctx, int g2, int compress, size_t n, const void* points_mont, void* out);
+B2G_API int b2g_points_deserialize(b2g_ctx* ctx, int g2, int compress, size_t n, const void* in, void* points_out,
+                                   uint64_t* first_bad_out);
 
 /* b2g_verify_batch_locate: one verdict per proof at about the cost of b2g_verify_batch when few proofs are invalid, for callers
  * that take proofs from untrusted submitters and must find the invalid ones.  The arguments, their layouts and the buffers are
