@@ -41,6 +41,17 @@ class VkDesc(C.Structure):
                [(k, C.c_void_p) for k in ('alpha_g1', 'beta_g2', 'gamma_g2', 'delta_g2', 'gamma_abc_g1')]
 
 
+class SetupSecrets(C.Structure):
+    """b2g_setup_secrets: 32-byte canonical scalars; g1 / g2 affine Montgomery generators or NULL for the standard ones"""
+    _fields_ = [(k, C.c_void_p) for k in ('alpha', 'beta', 'gamma', 'delta', 'tau', 'g1', 'g2')]
+
+
+class SetupOut(C.Structure):
+    """b2g_setup_out: host buffers in the b2g_pk_desc layout"""
+    _fields_ = [(k, C.c_void_p) for k in ('alpha_g1', 'beta_g1', 'delta_g1', 'beta_g2', 'gamma_g2', 'delta_g2', 'gamma_abc_g1',
+                                          'a_query', 'b_g1_query', 'b_g2_query', 'l_query', 'h_query')]
+
+
 class KeyBatch(C.Structure):
     """b2g_key_batch: one batch of proofs under one verifying key (b2g_verify_batch_keys, b2g_verify_batch_keys_locate)"""
     _fields_ = [('vk', C.c_void_p), ('count', C.c_uint32), ('reserved', C.c_uint32)] + \
@@ -54,7 +65,7 @@ EXPORTS = ['b2g_last_error', 'b2g_version', 'b2g_device_count', 'b2g_ctx_create'
            'b2g_verify_batch', 'b2g_proofs_decompress', 'b2g_verify_many_compressed', 'b2g_verify_batch_compressed',
            'b2g_verify_batch_locate', 'b2g_verify_batch_locate_compressed', 'b2g_verify_batch_keys',
            'b2g_verify_batch_keys_compressed', 'b2g_verify_batch_keys_locate', 'b2g_verify_batch_keys_locate_compressed',
-           'b2g_rerandomize_many', 'b2g_points_serialize', 'b2g_points_deserialize']
+           'b2g_rerandomize_many', 'b2g_points_serialize', 'b2g_points_deserialize', 'b2g_setup']
 
 _lib = None
 
@@ -96,6 +107,7 @@ def lib():
         L.b2g_ntt.argtypes = [vp, vp, i, i]
         L.b2g_fixed_base_g1.argtypes = [vp, vp, sz, vp]
         L.b2g_fixed_base_g2.argtypes = [vp, vp, sz, vp]
+        L.b2g_setup.argtypes = [vp, C.POINTER(MatDesc), C.POINTER(SetupSecrets), C.POINTER(SetupOut)]
         L.b2g_test_op.argtypes = [vp, i, vp, vp, sz, vp]
         L.b2g_last_timings.argtypes = [vp, vp]
         L.b2g_bench_device.argtypes = [vp, vp, vp, i, C.POINTER(C.c_float)]

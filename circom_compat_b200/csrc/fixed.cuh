@@ -60,4 +60,18 @@ __global__ void fixed_table_kernel(void* __restrict__ table, const void* __restr
     fixed_table_entry<C, F>(table, base, i);
 }
 
+// out[i] = scalars[i] * G (affine) for the window table of G and canonical scalars, one product per thread
+template <class C, class F>
+__global__ void __launch_bounds__(128) fixed_base_kernel(const void* __restrict__ table, const fe* __restrict__ scalars, uint32_t n, void* __restrict__ out) {
+    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    fe k = fe_load_nc(&scalars[i]);
+    typename C::Pt acc = C::infinity();
+    for (int w = 0; w < 32; w++) {
+        uint32_t byte = (k.l[w >> 2] >> (8 * (w & 3))) & 255u;
+        if (byte) C::madd(acc, aff_load<F>(table, (size_t)w * 255u + byte - 1u));
+    }
+    aff_store<F>(out, i, C::to_affine(acc));
+}
+
 }  // namespace b2g

@@ -507,6 +507,13 @@ void ntt_plain(const NttDomain& d, fe* data, fe* tmp, bool inverse, cudaStream_t
     CUDA_CHECK(cudaGetLastError());
 }
 
+void ntt_powers(int logn, const fe* pw, const fe* scale, fe* out, cudaStream_t st) {
+    const size_t n = (size_t)1 << logn;
+    ntt_powers_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(logn, pw, scale, out);
+    g_launch_count += 1;
+    CUDA_CHECK(cudaGetLastError());
+}
+
 void spmv_launch(uint32_t n, uint32_t m, uint32_t num_inputs, const uint32_t* a_rowptr, const uint32_t* a_col, const fe* a_val,
                  const uint32_t* b_rowptr, const uint32_t* b_col, const fe* b_val, const fe* w, fe* a, fe* b, fe* c, cudaStream_t st,
                  const uint32_t* c_rowptr, const uint32_t* c_col, const fe* c_val, uint32_t count, uint32_t w_stride) {

@@ -22,6 +22,8 @@ void ntt_witness_transform(const NttDomain& d, fe* a, fe* b, fe* c, fe* out, cud
 void ntt_transform_single(const NttDomain& d, fe* v, cudaStream_t st);
 void ntt_witness_transform_libsnark(const NttDomain& d, fe* a, fe* b, fe* c, fe* scratch, fe* out, cudaStream_t st, uint32_t count = 1);
 void ntt_plain(const NttDomain& d, fe* data, fe* tmp, bool inverse, cudaStream_t st);
+// out[k] = *scale * x^k for k < 2^logn, from pw[b] = x^(2^b), b < logn (device pointers)
+void ntt_powers(int logn, const fe* pw, const fe* scale, fe* out, cudaStream_t st);
 void spmv_launch(uint32_t n, uint32_t m, uint32_t num_inputs, const uint32_t* a_rowptr, const uint32_t* a_col, const fe* a_val,
                  const uint32_t* b_rowptr, const uint32_t* b_col, const fe* b_val, const fe* w, fe* a, fe* b, fe* c, cudaStream_t st,
                  const uint32_t* c_rowptr = nullptr, const uint32_t* c_col = nullptr, const fe* c_val = nullptr,

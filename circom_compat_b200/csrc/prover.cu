@@ -15,6 +15,7 @@
 #include "msm.cuh"
 #include "fixed.cuh"
 #include "ntt.cuh"
+#include "setup.cuh"
 #include "util.cuh"
 #include "verify.cuh"
 
@@ -341,19 +342,6 @@ __global__ void affine_sum_kernel(const uint8_t* __restrict__ pts, int i, int j,
     G1::Pt acc = G1::from_affine(aff_load<Fq>(pts, (size_t)i));
     G1::madd(acc, aff_load<Fq>(pts, (size_t)j));
     aff_store<Fq>(out, 0, G1::to_affine(acc));
-}
-
-template <class C, class F>
-__global__ void __launch_bounds__(128) fixed_base_kernel(const void* __restrict__ table, const fe* __restrict__ scalars, uint32_t n, void* __restrict__ out) {
-    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    fe k = fe_load_nc(&scalars[i]);
-    typename C::Pt acc = C::infinity();
-    for (int w = 0; w < 32; w++) {
-        uint32_t byte = (k.l[w >> 2] >> (8 * (w & 3))) & 255u;
-        if (byte) C::madd(acc, aff_load<F>(table, (size_t)w * 255u + byte - 1u));
-    }
-    aff_store<F>(out, i, C::to_affine(acc));
 }
 
 // Bytes per row of each test op's operands and result (0: operand not read).  XYZZ records are 4 coordinates (G1 128 B,
@@ -959,6 +947,43 @@ int b2g_pk_free(b2g_pk* pk) {
     });
 }
 
+}  // extern "C"
+namespace b2g {
+
+int mat_desc_check(const b2g_mat_desc* d, bool with_c) {
+    if (!d->a_rowptr || !d->b_rowptr) throw_error(B2G_E_SHAPE, "null row pointer array");
+    if (d->num_inputs == 0 || d->num_inputs > d->n_vars) throw_error(B2G_E_SHAPE, "num_inputs out of range");
+    const uint64_t need = (uint64_t)d->num_constraints + d->num_inputs;
+    int logn = 0;
+    while ((1ull << logn) < need) logn++;
+    if (logn > 27) throw_error(B2G_E_DOMAIN, "PolynomialDegreeTooLarge: domain (and its double) must fit 2^28");
+    const uint32_t m = d->num_constraints;
+    const uint32_t annz = d->a_rowptr[m], bnnz = d->b_rowptr[m];
+    if ((annz && (!d->a_col || !d->a_val)) || (bnnz && (!d->b_col || !d->b_val))) throw_error(B2G_E_SHAPE, "null matrix arrays");
+    if (d->reduction > B2G_REDUCTION_LIBSNARK) throw_error(B2G_E_SHAPE, "unknown reduction");
+    const bool libsnark = d->reduction == B2G_REDUCTION_LIBSNARK;
+    if (with_c && !d->c_rowptr) throw_error(B2G_E_SHAPE, "b2g_setup needs the C matrix (it may have no nonzeros)");
+    if (libsnark && !d->c_rowptr) throw_error(B2G_E_SHAPE, "LibsnarkReduction needs the C matrix");
+    with_c = with_c || libsnark;
+    const uint32_t cnnz = with_c ? d->c_rowptr[m] : 0;
+    if (cnnz && (!d->c_col || !d->c_val)) throw_error(B2G_E_SHAPE, "null matrix arrays");
+    // row pointers index col / val on the device: must start at 0 and never decrease (the last one is the nnz used above)
+    auto check_rowptr = [&](const uint32_t* rp, const char* name) {
+        if (rp[0] != 0) throw_error(B2G_E_SHAPE, std::string("matrix ") + name + ": rowptr[0] != 0");
+        for (uint32_t i = 0; i < m; i++) if (rp[i + 1] < rp[i]) throw_error(B2G_E_SHAPE, std::string("matrix ") + name + ": row pointers decrease at row " + std::to_string(i));
+    };
+    check_rowptr(d->a_rowptr, "A"); check_rowptr(d->b_rowptr, "B");
+    if (with_c) check_rowptr(d->c_rowptr, "C");
+    for (uint32_t k = 0; k < cnnz; k++) if (d->c_col[k] >= d->n_vars) throw_error(B2G_E_SHAPE, "matrix C column index out of range");
+    for (uint32_t k = 0; k < annz; k++) if (d->a_col[k] >= d->n_vars) throw_error(B2G_E_SHAPE, "matrix A column index out of range");
+    for (uint32_t k = 0; k < bnnz; k++) if (d->b_col[k] >= d->n_vars) throw_error(B2G_E_SHAPE, "matrix B column index out of range");
+    return logn;
+}
+
+}  // namespace b2g
+
+extern "C" {
+
 static void mat_release(b2g_mat* mat) {
     ntt_domain_destroy(mat->dom);
     for (void* p : {(void*)mat->a_rowptr, (void*)mat->a_col, (void*)mat->b_rowptr, (void*)mat->b_col, (void*)mat->a_val, (void*)mat->b_val,
@@ -969,30 +994,10 @@ static void mat_release(b2g_mat* mat) {
 int b2g_matrices_load(b2g_ctx* ctx, const b2g_mat_desc* d, b2g_mat** out) {
     return guarded([&] {
         if (!ctx || !d || !out) throw_error(B2G_E_SHAPE, "null pointer");
-        if (!d->a_rowptr || !d->b_rowptr) throw_error(B2G_E_SHAPE, "null row pointer array");
-        if (d->num_inputs == 0 || d->num_inputs > d->n_vars) throw_error(B2G_E_SHAPE, "num_inputs out of range");
-        const uint64_t need = (uint64_t)d->num_constraints + d->num_inputs;
-        int logn = 0;
-        while ((1ull << logn) < need) logn++;
-        if (logn > 27) throw_error(B2G_E_DOMAIN, "PolynomialDegreeTooLarge: domain (and its double) must fit 2^28");
+        const int logn = mat_desc_check(d, false);
         const uint32_t m = d->num_constraints;
-        const uint32_t annz = d->a_rowptr[m], bnnz = d->b_rowptr[m];
-        if ((annz && (!d->a_col || !d->a_val)) || (bnnz && (!d->b_col || !d->b_val))) throw_error(B2G_E_SHAPE, "null matrix arrays");
-        if (d->reduction > B2G_REDUCTION_LIBSNARK) throw_error(B2G_E_SHAPE, "unknown reduction");
         const bool libsnark = d->reduction == B2G_REDUCTION_LIBSNARK;
-        if (libsnark && !d->c_rowptr) throw_error(B2G_E_SHAPE, "LibsnarkReduction needs the C matrix");
-        const uint32_t cnnz = libsnark ? d->c_rowptr[m] : 0;
-        if (cnnz && (!d->c_col || !d->c_val)) throw_error(B2G_E_SHAPE, "null matrix arrays");
-        // row pointers index col / val on the device: must start at 0 and never decrease (the last one is the nnz used above)
-        auto check_rowptr = [&](const uint32_t* rp, const char* name) {
-            if (rp[0] != 0) throw_error(B2G_E_SHAPE, std::string("matrix ") + name + ": rowptr[0] != 0");
-            for (uint32_t i = 0; i < m; i++) if (rp[i + 1] < rp[i]) throw_error(B2G_E_SHAPE, std::string("matrix ") + name + ": row pointers decrease at row " + std::to_string(i));
-        };
-        check_rowptr(d->a_rowptr, "A"); check_rowptr(d->b_rowptr, "B");
-        if (libsnark) check_rowptr(d->c_rowptr, "C");
-        for (uint32_t k = 0; k < cnnz; k++) if (d->c_col[k] >= d->n_vars) throw_error(B2G_E_SHAPE, "matrix C column index out of range");
-        for (uint32_t k = 0; k < annz; k++) if (d->a_col[k] >= d->n_vars) throw_error(B2G_E_SHAPE, "matrix A column index out of range");
-        for (uint32_t k = 0; k < bnnz; k++) if (d->b_col[k] >= d->n_vars) throw_error(B2G_E_SHAPE, "matrix B column index out of range");
+        const uint32_t annz = d->a_rowptr[m], bnnz = d->b_rowptr[m], cnnz = libsnark ? d->c_rowptr[m] : 0;
         DevGuard g(ctx->device);
         cudaStream_t st = ctx->st[0];
         b2g_mat* mat = new b2g_mat();

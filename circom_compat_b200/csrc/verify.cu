@@ -1240,6 +1240,31 @@ static uint64_t points_slices(const char* fn, b2g_ctx* ctx, size_t n, size_t in_
     return bad;
 }
 
+// b2g_setup's generators: bad[0] for g1 (thread 0), bad[1] for g2 (thread 1), with the codes of setup_generators_check
+__global__ void setup_generators_kernel(const void* __restrict__ g1, const void* __restrict__ g2, uint32_t* __restrict__ bad) {
+    if (threadIdx.x == 0 && g1) {
+        const G1::Aff p = aff_load<Fq>(g1, 0);
+        bad[0] = G1::aff_is_inf(p) || !aff_on_curve<G1, Fq>(p) ? 1u : 0u;
+    } else if (threadIdx.x == 1 && g2) {
+        const G2::Aff q = aff_load<Fq2>(g2, 0);
+        bad[1] = G2::aff_is_inf(q) || !aff_on_curve<G2, Fq2>(q) ? 2u : (g2_in_subgroup(q) ? 0u : 3u);
+    }
+}
+
+int setup_generators_check(const void* g1, const void* g2, cudaStream_t st) {
+    if (!g1 && !g2) return 0;
+    uint32_t* d_bad = nullptr;
+    CUDA_CHECK(cudaMalloc(&d_bad, 2 * sizeof(uint32_t)));
+    uint32_t bad[2] = {0, 0};
+    cudaError_t e = cudaMemsetAsync(d_bad, 0, sizeof(bad), st);
+    if (e == cudaSuccess) { setup_generators_kernel<<<1, 32, 0, st>>>(g1, g2, d_bad); g_launch_count += 1; e = cudaGetLastError(); }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(bad, d_bad, sizeof(bad), cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    cudaFree(d_bad);
+    CUDA_CHECK(e);
+    return bad[0] ? (int)bad[0] : (int)bad[1];
+}
+
 }  // namespace b2g
 
 extern "C" {

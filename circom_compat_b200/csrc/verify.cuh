@@ -18,4 +18,9 @@ CtxView ctx_view(b2g_ctx* ctx);
 constexpr int PAIRING_TEST_OP0 = 30;
 void pairing_test_op(cudaStream_t st, int op, const void* a, const void* b, size_t n, void* out);
 
+// b2g_setup's generator checks on a device buffer of a G1 (64 B) and a G2 (128 B) affine Montgomery point; a NULL pointer is
+// not checked.  Returns 0, or 1 for a G1 point at infinity or off its curve, 2 for a G2 point at infinity or off its twist, 3 for
+// a G2 point outside G2.  Synchronises the stream.
+int setup_generators_check(const void* g1, const void* g2, cudaStream_t st);
+
 }  // namespace b2g

@@ -28,6 +28,9 @@
         <- deserialize_compressed followed by verify_many / verify_batch, decoded on the device.
     Groth16.rerandomize_proof(vk, proof, rng) / Groth16.rerandomize_proofs(vk, proofs)
         <- Groth16::rerandomize_proof (ark-groth16 0.5.0), for one or many proofs of one key in one device pass.
+    Groth16.generate_parameters_with_qap(circuit, alpha, beta, gamma, delta, g1, g2, tau=tau)
+        <- Groth16::generate_parameters_with_qap (ark-groth16 0.5): the whole setup on the device (b2g_setup);
+           generate_random_parameters_with_reduction(circuit, rng) draws the toxic waste and calls it.
 Arguments keep the reference's meaning; field elements are (n, 4) uint64 Montgomery limb arrays (fr_to_mont).
 """
 from __future__ import annotations
@@ -94,6 +97,23 @@ def _vk_desc(key):
     return d, keep
 
 
+def _mat_desc(m: ConstraintMatrices, n_vars: int, reduction: int, with_c: bool = False):
+    """(b2g_mat_desc, the arrays it points into) of ConstraintMatrices; with_c: pass the C matrix whatever the reduction
+    (b2g_setup reads it for both)"""
+    d = N.MatDesc()
+    d.num_constraints, d.num_inputs, d.n_vars, d.reduction = m.num_constraints, m.num_instance_variables, n_vars, reduction
+    keep = [_c(m.a[0], np.uint32), _c(m.a[1], np.uint32), _c(m.a[2]), _c(m.b[0], np.uint32), _c(m.b[1], np.uint32), _c(m.b[2])]
+    names = ['a_rowptr', 'a_col', 'a_val', 'b_rowptr', 'b_col', 'b_val']
+    if with_c or reduction == N.REDUCTION_LIBSNARK:
+        if m.c is None:
+            raise ValueError(("the setup" if with_c else "LibsnarkReduction") + " needs the C matrix (R1CS route); zkey matrices have none")
+        keep += [_c(m.c[0], np.uint32), _c(m.c[1], np.uint32), _c(m.c[2])]
+        names += ['c_rowptr', 'c_col', 'c_val']
+    for name, arr in zip(names, keep):
+        setattr(d, name, arr.ctypes.data if arr.size else None)
+    return d, keep
+
+
 _LOAD_MANY_KEY = re.compile(r'b2g_vk_load_many: key (\d+): (.*)', re.S)
 
 
@@ -152,17 +172,7 @@ class Context:
     def mat_handle(self, m: ConstraintMatrices, n_vars: int, reduction: int = N.REDUCTION_CIRCOM):
         key = (id(m), self.device, n_vars, reduction)
         if key not in _MAT_HANDLES:
-            d = N.MatDesc()
-            d.num_constraints, d.num_inputs, d.n_vars, d.reduction = m.num_constraints, m.num_instance_variables, n_vars, reduction
-            keep = [_c(m.a[0], np.uint32), _c(m.a[1], np.uint32), _c(m.a[2]), _c(m.b[0], np.uint32), _c(m.b[1], np.uint32), _c(m.b[2])]
-            names = ['a_rowptr', 'a_col', 'a_val', 'b_rowptr', 'b_col', 'b_val']
-            if reduction == N.REDUCTION_LIBSNARK:
-                if m.c is None:
-                    raise ValueError("LibsnarkReduction needs the C matrix (R1CS route); zkey matrices have none")
-                keep += [_c(m.c[0], np.uint32), _c(m.c[1], np.uint32), _c(m.c[2])]
-                names += ['c_rowptr', 'c_col', 'c_val']
-            for name, arr in zip(names, keep):
-                setattr(d, name, arr.ctypes.data if arr.size else None)
+            d, keep = _mat_desc(m, n_vars, reduction)
             h = C.c_void_p()
             N.check(N.lib().b2g_matrices_load(self._h, C.byref(d), C.byref(h)))
             _MAT_HANDLES[key] = (h, m)
@@ -645,10 +655,59 @@ class Groth16:
 
     @staticmethod
     def generate_random_parameters_with_reduction(circuit, rng, ctx: Context = None, reduction=CircomReduction) -> ProvingKey:
-        """Setup on the GPU (tests/groth16.rs:25 flow); `circuit` is a synth.Circuit (R1CS as coordinate lists)."""
-        from . import synth
-        flavour = 'libsnark' if reduction.ID == N.REDUCTION_LIBSNARK else 'circom'
-        return synth.generate_random_parameters_with_reduction(circuit, rng, ctx or default_context(), flavour)
+        """Setup on the GPU (tests/groth16.rs:25 flow): the toxic waste alpha, beta, gamma, delta, tau is drawn in that order
+        with rng.randrange(1, r), the key is built on the standard generators by one b2g_setup call, and the toxic waste is
+        dropped.  `circuit` is a synth.Circuit (R1CS as coordinate lists) or ConstraintMatrices with C."""
+        alpha, beta, gamma, delta, tau = (rng.randrange(1, R_MOD) for _ in range(5))
+        return Groth16.generate_parameters_with_qap(circuit, alpha, beta, gamma, delta, tau=tau, ctx=ctx, reduction=reduction)
+
+    @staticmethod
+    def generate_parameters_with_qap(circuit, alpha, beta, gamma, delta, g1_generator=None, g2_generator=None, *, tau,
+                                     ctx: Context = None, reduction=CircomReduction) -> ProvingKey:
+        """Groth16::generate_parameters_with_qap(circuit, alpha, beta, gamma, delta, g1_generator, g2_generator, rng)
+        (ark-groth16 0.5) with tau given instead of drawn from the rng; every scalar and point is computed on the GPU by
+        b2g_setup.  Scalars are ints in [0, r) (gamma, delta nonzero); generators are in the ProvingKey point-array layout
+        (8 / 16 uint64 words, affine Montgomery), None for the standard ones.  `circuit` is a synth.Circuit or
+        ConstraintMatrices with C (the R1CS route); its n_vars is then the matrices' own."""
+        ctx = ctx or default_context()
+        if hasattr(circuit, 'matrices'):
+            m, n_vars = circuit.matrices(with_c=True), circuit.n_vars
+        else:
+            m, n_vars = circuit, circuit.n_vars
+        d, keep = _mat_desc(m, n_vars, reduction.ID, with_c=True)
+        ni = m.num_instance_variables
+        if ni == 0 or ni > n_vars:
+            raise N.B2gError(N.B2G_E_SHAPE, "num_inputs out of range")
+        size = 1
+        while size < m.num_constraints + ni:
+            size <<= 1
+        nh = size - 1 if reduction.ID == N.REDUCTION_LIBSNARK else size
+        secrets = np.frombuffer(b''.join(int(v).to_bytes(32, 'little') for v in (alpha, beta, gamma, delta, tau)), dtype=np.uint8).copy()
+        sec = N.SetupSecrets()
+        for i, name in enumerate(('alpha', 'beta', 'gamma', 'delta', 'tau')):
+            setattr(sec, name, secrets.ctypes.data + 32 * i)
+        gens = []
+        for name, gen, words in (('g1', g1_generator, 8), ('g2', g2_generator, 16)):
+            if gen is not None:
+                g = _c(gen).reshape(-1)
+                if g.size != words:
+                    raise ValueError(f"{name}_generator must be {words} uint64 words (affine Montgomery)")
+                gens.append(g)
+                setattr(sec, name, g.ctypes.data)
+        shapes = {'alpha_g1': (1, 8), 'beta_g1': (1, 8), 'delta_g1': (1, 8), 'beta_g2': (1, 16), 'gamma_g2': (1, 16), 'delta_g2': (1, 16),
+                  'gamma_abc_g1': (ni, 8), 'a_query': (n_vars, 8), 'b_g1_query': (n_vars, 8), 'b_g2_query': (n_vars, 16),
+                  'l_query': (n_vars - ni, 8), 'h_query': (nh, 8)}
+        arrs = {k: np.zeros(v, dtype=np.uint64) for k, v in shapes.items()}
+        out = N.SetupOut()
+        for k, a in arrs.items():
+            setattr(out, k, a.ctypes.data if a.size else None)
+        try:
+            N.check(N.lib().b2g_setup(ctx._h, C.byref(d), C.byref(sec), C.byref(out)))
+        finally:
+            secrets[:] = 0
+        return ProvingKey(n_vars, ni - 1, nh, arrs['alpha_g1'], arrs['beta_g1'], arrs['beta_g2'], arrs['gamma_g2'], arrs['delta_g1'],
+                          arrs['delta_g2'], arrs['gamma_abc_g1'], arrs['a_query'], arrs['b_g1_query'], arrs['b_g2_query'],
+                          arrs['l_query'], arrs['h_query'])
 
     # ---- verification (host pairing; circom_compat_b200/verifier.py).  Call sites in the reference: src/zkey.rs:868-870,
     # 914-916 (process_vk + verify_with_processed_vk), tests/groth16.rs:33-35 (SNARK::verify).

@@ -337,27 +337,37 @@ public:
     b2g_mat* mat(const ConstraintMatrices& m, size_t n_vars, uint32_t reduction = B2G_REDUCTION_CIRCOM) {
         const uint32_t tag = reduction | (uint32_t)(n_vars << 1);     // a matrices handle is specific to (reduction, n_vars)
         if (void* h = m.device.find(ctx_, tag)) return (b2g_mat*)h;
-        std::vector<uint32_t> rp[3], col[3]; std::vector<Fr> val[3];
-        const Matrix* src[3] = {&m.a, &m.b, &m.c};
-        const int nmat = reduction == B2G_REDUCTION_LIBSNARK ? 3 : 2;
-        for (int k = 0; k < nmat; k++) {
-            rp[k].assign(m.num_constraints + 1, 0);
-            for (size_t i = 0; i < m.num_constraints; i++) {
-                const auto& row = i < src[k]->size() ? (*src[k])[i] : Matrix::value_type();
-                for (const auto& e : row) { val[k].push_back(e.first); col[k].push_back((uint32_t)e.second); }
-                rp[k][i + 1] = (uint32_t)col[k].size();
-            }
-        }
-        b2g_mat_desc d; memset(&d, 0, sizeof d);
-        d.num_constraints = (uint32_t)m.num_constraints; d.num_inputs = (uint32_t)m.num_instance_variables; d.n_vars = (uint32_t)n_vars;
-        d.reduction = reduction;
-        d.a_rowptr = rp[0].data(); d.a_col = col[0].data(); d.a_val = val[0].data();
-        d.b_rowptr = rp[1].data(); d.b_col = col[1].data(); d.b_val = val[1].data();
-        if (nmat == 3) { d.c_rowptr = rp[2].data(); d.c_col = col[2].data(); d.c_val = val[2].data(); }
-        b2g_mat* h = nullptr; check(b2g_matrices_load(ctx_, &d, &h));
+        const MatDesc md(m, n_vars, reduction);
+        b2g_mat* h = nullptr; check(b2g_matrices_load(ctx_, &md.d, &h));
         m.device.put(ctx_, tag, h, [](void* p) { b2g_matrices_free((b2g_mat*)p); });
         return h;
     }
+
+    // the b2g_mat_desc of matrices and the CSR arrays it points into; with_c: C whatever the reduction (b2g_setup reads it for both)
+    struct MatDesc {
+        std::vector<uint32_t> rp[3], col[3]; std::vector<Fr> val[3];
+        b2g_mat_desc d;
+        MatDesc(const ConstraintMatrices& m, size_t n_vars, uint32_t reduction, bool with_c = false) {
+            const Matrix* src[3] = {&m.a, &m.b, &m.c};
+            const int nmat = with_c || reduction == B2G_REDUCTION_LIBSNARK ? 3 : 2;
+            for (int k = 0; k < nmat; k++) {
+                rp[k].assign(m.num_constraints + 1, 0);
+                for (size_t i = 0; i < m.num_constraints; i++) {
+                    const auto& row = i < src[k]->size() ? (*src[k])[i] : Matrix::value_type();
+                    for (const auto& e : row) { val[k].push_back(e.first); col[k].push_back((uint32_t)e.second); }
+                    rp[k][i + 1] = (uint32_t)col[k].size();
+                }
+            }
+            memset(&d, 0, sizeof d);
+            d.num_constraints = (uint32_t)m.num_constraints; d.num_inputs = (uint32_t)m.num_instance_variables; d.n_vars = (uint32_t)n_vars;
+            d.reduction = reduction;
+            d.a_rowptr = rp[0].data(); d.a_col = col[0].data(); d.a_val = val[0].data();
+            d.b_rowptr = rp[1].data(); d.b_col = col[1].data(); d.b_val = val[1].data();
+            if (nmat == 3) { d.c_rowptr = rp[2].data(); d.c_col = col[2].data(); d.c_val = val[2].data(); }
+        }
+        MatDesc(const MatDesc&) = delete;
+        MatDesc& operator=(const MatDesc&) = delete;
+    };
 
 private:
     b2g_ctx* ctx_ = nullptr;
@@ -780,6 +790,43 @@ struct Groth16T {                                       // Groth16::<Bn254, QAP>
         check(b2g_prove_many(gpu.ctx(), gpu.pk(pk), gpu.mat(matrices, pk.a_query.size(), QAP::ID), (uint32_t)n, rb.data(), sb.data(), ws.data(), bytes.data()));
         for (size_t i = 0; i < n; i++) memcpy(out[i].bytes, bytes.data() + 256 * i, 256);
         return out;
+    }
+
+    // Groth16::generate_parameters_with_qap(circuit, alpha, beta, gamma, delta, g1, g2, rng) (ark-groth16 0.5) with tau given
+    // instead of drawn: every scalar and point of the key on the device (b2g_setup).  g1 / g2 = nullptr: the standard
+    // generators.  The matrices must carry C, as R1CS::to_matrices gives them; n_vars = num_instance + num_witness variables.
+    static ProvingKey generate_parameters_with_qap(const ConstraintMatrices& matrices, const Fr& alpha, const Fr& beta, const Fr& gamma,
+                                                   const Fr& delta, const G1Affine* g1, const G2Affine* g2, const Fr& tau,
+                                                   Gpu& gpu = Gpu::instance()) {
+        const size_t ni = matrices.num_instance_variables, nv = ni + matrices.num_witness_variables;
+        if (ni == 0) throw SynthesisError("generate_parameters_with_qap: no instance variable");
+        if (matrices.num_constraints && matrices.c.empty())
+            throw SynthesisError("generate_parameters_with_qap needs the C matrix (R1CS route); zkey matrices have none");
+        size_t n = 1;
+        while (n < matrices.num_constraints + ni) n <<= 1;
+        ProvingKey pk;
+        pk.vk.gamma_abc_g1.resize(ni); pk.a_query.resize(nv); pk.b_g1_query.resize(nv); pk.b_g2_query.resize(nv);
+        pk.l_query.resize(nv - ni); pk.h_query.resize(QAP::ID == B2G_REDUCTION_LIBSNARK ? n - 1 : n);
+        BigInt256 k[5] = {alpha.into_bigint(), beta.into_bigint(), gamma.into_bigint(), delta.into_bigint(), tau.into_bigint()};
+        const b2g_setup_secrets sec = {k[0].l, k[1].l, k[2].l, k[3].l, k[4].l, g1, g2};
+        b2g_setup_out out = {&pk.vk.alpha_g1, &pk.beta_g1, &pk.delta_g1, &pk.vk.beta_g2, &pk.vk.gamma_g2, &pk.vk.delta_g2,
+                             pk.vk.gamma_abc_g1.data(), pk.a_query.data(), pk.b_g1_query.data(), pk.b_g2_query.data(),
+                             pk.l_query.data(), pk.h_query.data()};
+        const Gpu::MatDesc md(matrices, nv, QAP::ID, true);
+        const int rc = b2g_setup(gpu.ctx(), &md.d, &sec, &out);
+        for (BigInt256& b : k) {                                // the toxic waste does not outlive the call on the host either
+            volatile uint64_t* wipe = b.l;
+            for (int i = 0; i < 4; i++) wipe[i] = 0;
+        }
+        check(rc);
+        return pk;
+    }
+    // Groth16::generate_random_parameters_with_reduction(circuit, rng): alpha, beta, gamma, delta, tau drawn with Fr::rand in that
+    // order, on the standard generators
+    template <class Rng>
+    static ProvingKey generate_random_parameters_with_reduction(const ConstraintMatrices& matrices, Rng& rng, Gpu& gpu = Gpu::instance()) {
+        const Fr alpha = Fr::rand(rng), beta = Fr::rand(rng), gamma = Fr::rand(rng), delta = Fr::rand(rng), tau = Fr::rand(rng);
+        return generate_parameters_with_qap(matrices, alpha, beta, gamma, delta, nullptr, nullptr, tau, gpu);
     }
 
     template <class Rng>

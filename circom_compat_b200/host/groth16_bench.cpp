@@ -31,6 +31,10 @@
 //       B2G_ARK_KEYS=path: also write the key with serialize_proving_key, compressed to path.compressed and uncompressed to
 //       path.uncompressed, read each back with deserialize_proving_key, and print its size, its FNV-1a digest and whether
 //       the key read back is identical
+//   B2G_SETUP=<seed> groth16_bench <circuit.r1cs> <witness.wtns>
+//       tests/groth16.rs:75-105 in C++: draw the toxic waste with std::mt19937_64(seed), make the key with
+//       Groth16T<LibsnarkReduction>::generate_random_parameters_with_reduction (b2g_setup), print the five secrets, the key
+//       (serialize_proving_key, compressed, hex), the proof of the witness under the same rng and the host verifier's verdict
 //       chain:<a> = the witness of the reference's squaring-chain bench family for input a
 //       (test-vectors/complex-circuit/input.json has a = 3), computed on the host instead of by WASM.
 #include <algorithm>
@@ -160,6 +164,34 @@ int main(int argc, char** argv) {
             for (uint8_t b : serialize_compressed(proof)) std::printf("%02x", b);
             std::printf("\n");
             std::printf("verified=%d\n", Groth16::verify_with_processed_vk(Groth16::process_vk(vk2), in2, p2) ? 1 : 0);
+            return 0;
+        }
+        if (const char* seed = std::getenv("B2G_SETUP")) {                  // R1CS -> setup on the GPU -> prove -> verify
+            if (argc < 3) { std::fprintf(stderr, "usage: B2G_SETUP=<seed> %s <circuit.r1cs> <witness.wtns>\n", argv[0]); return 2; }
+            typedef Groth16T<LibsnarkReduction> G;                           // Groth16<Bn254> (tests/groth16.rs:9)
+            std::ifstream rf(argv[1], std::ios::binary);
+            if (!rf) throw SerializationError("cannot open r1cs");
+            const R1CS r1cs = R1CS::read(rf);
+            const ConstraintMatrices matrices = r1cs.to_matrices();
+            std::ifstream wf(argv[2], std::ios::binary);
+            if (!wf) throw SerializationError("cannot open wtns");
+            const std::vector<Fr> w = read_wtns(wf);
+            std::mt19937_64 rng(std::stoull(seed, nullptr, 0));
+            std::mt19937_64 replay = rng;                                    // the same draws, to print the secrets
+            const char* names[5] = {"alpha", "beta", "gamma", "delta", "tau"};
+            for (const char* name : names) {
+                const BigInt256 b = Fr::rand(replay).into_bigint();
+                std::printf("%s=0x%016llx%016llx%016llx%016llx\n", name, (unsigned long long)b.l[3], (unsigned long long)b.l[2],
+                            (unsigned long long)b.l[1], (unsigned long long)b.l[0]);
+            }
+            const ProvingKey pk = G::generate_random_parameters_with_reduction(matrices, rng);
+            std::printf("key=");
+            for (uint8_t b : serialize_proving_key(pk)) std::printf("%02x", b);
+            std::printf("\n");
+            const Proof proof = G::prove(pk, matrices, w, rng);
+            std::printf("proof=%s\n", proof.hex().c_str());
+            const std::vector<Fr> inputs(w.begin() + 1, w.begin() + matrices.num_instance_variables);
+            std::printf("verified=%d\n", G::verify_with_processed_vk(G::process_vk(pk.vk), inputs, proof) ? 1 : 0);
             return 0;
         }
         if (argc < 3) { std::fprintf(stderr, "usage: %s [--parse-only] <zkey> chain:<a>|<wtns> [iters] [r_hex s_hex]\n", argv[0]); return 2; }

@@ -251,17 +251,6 @@ def setup(ctx, circ: Circuit, seed: int = 0xB200, trapdoor=None, flavour: str = 
     return pk, td
 
 
-def generate_random_parameters_with_reduction(circ: Circuit, rng, ctx, flavour: str = 'circom'):
-    """Groth16::<Bn254, CircomReduction>::generate_random_parameters_with_reduction(circuit, rng) as the reference's
-    tests call it (tests/groth16.rs:25): toxic waste (alpha, beta, gamma, delta, tau) drawn from `rng` (any object with
-    randrange), Lagrange evaluations on the host, every group element by fixed-base multiplication on the GPU, H query
-    from CircomReduction::h_query_scalars (src/circom/qap.rs:90-105).  Returns the ProvingKey only (the trapdoor is dropped)."""
-    trap = [rng.randrange(1, R_MOD) for _ in range(5)]
-    alpha, beta, gamma, delta, tau = trap
-    pk, _ = setup(ctx, circ, trapdoor=(tau, alpha, beta, gamma, delta), flavour=flavour)
-    return pk
-
-
 def qap_numerator_at_tau(td: Trapdoor, circ: Circuit, w):
     """(a*b - c)(tau) computed WITHOUT any transform and without the C matrix: a, b are the interpolants of the row
     evaluations <A_row, w>, <B_row, w> (plus the public-input rows of A, qap.rs:46-50) and c interpolates their

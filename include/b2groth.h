@@ -29,8 +29,9 @@
  *   b2g_rerandomize_many   <- Groth16::rerandomize_proof (ark-groth16 0.5.0) for many proofs of one key, in one device pass
  *   b2g_points_serialize / b2g_points_deserialize <- CanonicalSerialize / CanonicalDeserialize (ark-serialize 0.5,
  *                             Validate::Yes) of the G1 / G2 points of a ProvingKey<Bn254> or VerifyingKey<Bn254>
- *   b2g_fixed_base_g1/g2  <- the batch fixed-base multiplications of generate_random_parameters_with_reduction
- *                             (tests/groth16.rs:25); used to manufacture synthetic proving keys
+ *   b2g_setup              <- Groth16::generate_parameters_with_qap (ark-groth16 0.5), which
+ *                             generate_random_parameters_with_reduction calls (tests/groth16.rs:25): a whole proving key
+ *   b2g_fixed_base_g1/g2  <- the batch fixed-base multiplications of that setup, for the standard generators only
  *
  * Conventions
  *   - every function returns 0 (B2G_OK) or a negative error code; b2g_last_error() gives a thread-local message.
@@ -419,6 +420,50 @@ B2G_API int b2g_verify_batch_keys_locate_compressed(b2g_ctx* ctx, uint32_t n_key
  * grow to the largest batch seen and are kept. */
 B2G_API int b2g_rerandomize_many(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* proofs, const void* r1_canon,
                                  const void* r2_canon, uint8_t* proofs_out, uint8_t* ok_out);
+
+/* The toxic waste of one setup: alpha, beta, gamma, delta, tau are 32 B canonical scalars; g1 / g2 are the generators the key
+ * is built on, affine Montgomery (64 B / 128 B), or NULL for the standard ones (G1 = (1, 2), G2 = src/zkey.rs:443-463). */
+typedef struct {
+    const void* alpha; const void* beta; const void* gamma; const void* delta; const void* tau;
+    const void* g1;
+    const void* g2;
+} b2g_setup_secrets;
+
+/* HOST buffers the caller sized, in the b2g_pk_desc layout (affine Montgomery, all-zero = infinity). */
+typedef struct {
+    void *alpha_g1, *beta_g1, *delta_g1;            /* 64 B each */
+    void *beta_g2, *gamma_g2, *delta_g2;            /* 128 B each */
+    void *gamma_abc_g1;                             /* num_inputs G1 */
+    void *a_query, *b_g1_query;                     /* n_vars G1 */
+    void *b_g2_query;                               /* n_vars G2 */
+    void *l_query;                                  /* n_vars - num_inputs G1 (may be NULL when that is 0) */
+    void *h_query;                                  /* n G1 (CircomReduction) or n - 1 (LibsnarkReduction) */
+} b2g_setup_out;
+
+/* b2g_setup <- Groth16::generate_parameters_with_qap(circuit, alpha, beta, gamma, delta, g1, g2) (ark-groth16 0.5) with tau given
+ * instead of drawn, i.e. the key generate_random_parameters_with_reduction makes (tests/groth16.rs:25).  The circuit is a
+ * b2g_mat_desc as b2g_matrices_load reads it: m rows in CSR form with Montgomery values, without the public-input rows (the
+ * setup appends them, as the witness map does); `reduction` selects the H query; the C matrix is required for both reductions
+ * (it may have no nonzeros).  With n the least power of two >= m + num_inputs and L_i = L_i(tau) the Lagrange coefficients of
+ * the domain of size n:
+ *     a_j = sum_rows A[r][j] L_r (+ L_(m+j) for j < num_inputs), b_j and c_j likewise without the extra term,
+ *     a_query[j] = a_j g1, b_g1_query[j] = b_j g1, b_g2_query[j] = b_j g2 (j < n_vars),
+ *     gamma_abc_g1[j] = (beta a_j + alpha b_j + c_j) / gamma g1 (j < num_inputs), l_query[j - num_inputs] = the same / delta,
+ *     alpha_g1 = alpha g1, beta_g1 = beta g1, delta_g1 = delta g1, beta_g2 = beta g2, gamma_g2 = gamma g2, delta_g2 = delta g2,
+ *     h_query (LibsnarkReduction) = tau^i (tau^n - 1) / delta g1, i < n - 1,
+ *     h_query (CircomReduction)   = the odd entries of the inverse NTT over 2n points of (tau^i / delta, i < 2n - 1, then 0),
+ *                                   times g1 (CircomReduction::h_query_scalars, src/circom/qap.rs:90-105).
+ * Every scalar is computed on the device: the Lagrange coefficients as one inverse NTT of the powers of tau, the column sums by
+ * a radix sort of the nonzeros by column and a reduce-by-key (no column is summed by one thread), the points by fixed-base
+ * multiplication from window tables of g1 and g2, in slices through bounded device buffers.  Every device buffer that held a
+ * secret or a value derived from one is zeroed before it is freed, and so is the library's host copy of the secrets.
+ * Synchronous.  Errors (every error leaves the context usable; the content of the output buffers is then unspecified):
+ * B2G_E_SHAPE for null pointers or fields, a missing C matrix, num_inputs of 0 or above n_vars, row pointers that do not start
+ * at 0 or that decrease, a column index >= n_vars, an unknown reduction or a proof pending on the context (the matrix checks and
+ * their messages are b2g_matrices_load's); B2G_E_DOMAIN for n above 2^27 (LibsnarkReduction) or 2^26 (CircomReduction, whose H
+ * query needs the domain of 2n points); B2G_E_INPUT for a secret >= r, gamma or delta equal to 0, a generator coordinate >= p,
+ * a generator at infinity or off its curve, or a g2 outside G2; B2G_E_DEVICE when the buffers do not fit in device memory. */
+B2G_API int b2g_setup(b2g_ctx* ctx, const b2g_mat_desc* circuit, const b2g_setup_secrets* secrets, b2g_setup_out* out);
 
 /* Kernel-level entry points (parity tests, benchmarks). All pointers host. */
 B2G_API int b2g_msm_g1(b2g_ctx* ctx, const void* bases, const void* scalars, size_t n, int scalars_mont, void* out_xy_mont);
