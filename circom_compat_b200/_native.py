@@ -52,6 +52,17 @@ class SetupOut(C.Structure):
                                           'a_query', 'b_g1_query', 'b_g2_query', 'l_query', 'h_query')]
 
 
+class PowersDesc(C.Structure):
+    """b2g_powers_desc: the host arrays of a powers-of-tau ceremony of size 2^log_size (affine Montgomery, all-zero = infinity)"""
+    _fields_ = [('log_size', C.c_uint32), ('reserved', C.c_uint32)] + \
+               [(k, C.c_void_p) for k in ('tau_g1', 'tau_g2', 'alpha_tau_g1', 'beta_tau_g1', 'beta_g2')]
+
+
+class DeltaKey(C.Structure):
+    """b2g_delta_key: the fields of a proving key a delta contribution changes (host buffers)"""
+    _fields_ = [('n_l', C.c_uint32), ('n_h', C.c_uint32)] + [(k, C.c_void_p) for k in ('delta_g1', 'delta_g2', 'l_query', 'h_query')]
+
+
 class KeyBatch(C.Structure):
     """b2g_key_batch: one batch of proofs under one verifying key (b2g_verify_batch_keys, b2g_verify_batch_keys_locate)"""
     _fields_ = [('vk', C.c_void_p), ('count', C.c_uint32), ('reserved', C.c_uint32)] + \
@@ -65,7 +76,8 @@ EXPORTS = ['b2g_last_error', 'b2g_version', 'b2g_device_count', 'b2g_ctx_create'
            'b2g_verify_batch', 'b2g_proofs_decompress', 'b2g_verify_many_compressed', 'b2g_verify_batch_compressed',
            'b2g_verify_batch_locate', 'b2g_verify_batch_locate_compressed', 'b2g_verify_batch_keys',
            'b2g_verify_batch_keys_compressed', 'b2g_verify_batch_keys_locate', 'b2g_verify_batch_keys_locate_compressed',
-           'b2g_rerandomize_many', 'b2g_points_serialize', 'b2g_points_deserialize', 'b2g_setup']
+           'b2g_rerandomize_many', 'b2g_points_serialize', 'b2g_points_deserialize', 'b2g_setup',
+           'b2g_setup_from_powers', 'b2g_delta_update', 'b2g_delta_update_check', 'b2g_points_intt']
 
 _lib = None
 
@@ -108,6 +120,10 @@ def lib():
         L.b2g_fixed_base_g1.argtypes = [vp, vp, sz, vp]
         L.b2g_fixed_base_g2.argtypes = [vp, vp, sz, vp]
         L.b2g_setup.argtypes = [vp, C.POINTER(MatDesc), C.POINTER(SetupSecrets), C.POINTER(SetupOut)]
+        L.b2g_setup_from_powers.argtypes = [vp, C.POINTER(MatDesc), C.POINTER(PowersDesc), C.POINTER(SetupOut)]
+        L.b2g_delta_update.argtypes = [vp, C.POINTER(DeltaKey), vp, C.POINTER(DeltaKey)]
+        L.b2g_delta_update_check.argtypes = [vp, C.POINTER(DeltaKey), C.POINTER(DeltaKey), vp, vp]
+        L.b2g_points_intt.argtypes = [vp, i, i, vp]
         L.b2g_test_op.argtypes = [vp, i, vp, vp, sz, vp]
         L.b2g_last_timings.argtypes = [vp, vp]
         L.b2g_bench_device.argtypes = [vp, vp, vp, i, C.POINTER(C.c_float)]

@@ -12,6 +12,20 @@
 //   group elements         fixed_base_kernel from the 8-bit window tables of the given generators, in slices through one
 //                          bounded device buffer
 // Every device buffer is zeroed before it is freed: all of them hold the toxic waste or values derived from it.
+//
+// b2g_setup_from_powers makes the same key (gamma = delta = 1) from the points of a powers-of-tau ceremony instead, with no
+// scalar known to anyone:
+//   Lagrange points        [L_r] = iNTT_n(tau^i G)_r over points (points_intt: one launch per radix-2 DIF stage, one butterfly
+//                          per thread, the twiddle product a variable-base double-and-add on an XYZZ record; then a gather
+//                          from bit-reversed order that scales by n^-1 and converts to affine), for tau G1, tau G2, alpha tau G1
+//                          and beta tau G1
+//   column sums            the nonzeros sorted by column as above, then products coefficient x Lagrange point summed in pieces
+//                          of PIECE_PRODUCTS per thread and reduced by column, PIECE_SUMS points per thread and level, until each
+//                          column has one point; a coefficient above r / 2 multiplies the negated point by r - k
+//   H query                LibsnarkReduction: tau^(i + n) G - tau^i G; CircomReduction: 1/2 iNTT_n of
+//                          y_i = omega_2n^-i (tau^i G - tau^(i + n) G), the odd entries of the 2n-point transform folded
+//                          into one n-point transform
+// b2g_delta_update multiplies delta by x and the L and H queries by x^-1, one point per thread.
 #include <cub/cub.cuh>
 #include <algorithm>
 #include <cstring>
@@ -316,6 +330,520 @@ static void setup_run(b2g_ctx* ctx, const b2g_mat_desc* d, const b2g_setup_secre
     CUDA_CHECK(cudaStreamSynchronize(st));
 }
 
+// ---------------------------------------------------------------------------------------------- points of a ceremony
+constexpr uint32_t PIECE_PRODUCTS = 4;                  // products one thread sums at the first level of a column sum
+constexpr uint32_t PIECE_SUMS = 32;                     // points one thread sums at each later level
+
+// k P for an affine P and a canonical 256-bit k: mixed double-and-add from the top set bit; every exceptional case is madd's
+template <class C>
+__device__ __noinline__ typename C::Pt aff_mul(const typename C::Aff& p, const uint32_t* k) {
+    typename C::Pt acc = C::infinity();
+    if (C::aff_is_inf(p)) return acc;
+    int top = 255;
+    while (top >= 0 && !((k[top >> 5] >> (top & 31)) & 1u)) top--;
+    #pragma unroll 1
+    for (int i = top; i >= 0; i--) {
+        acc = C::dbl(acc);
+        if ((k[i >> 5] >> (i & 31)) & 1u) C::madd(acc, p);
+    }
+    return acc;
+}
+
+template <class C, class F>
+__global__ void __launch_bounds__(128) pts_from_affine_kernel(const void* __restrict__ aff, uint32_t n, void* __restrict__ pts) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) pt_store<F>(pts, i, C::from_affine(aff_load<F>(aff, i)));
+}
+
+// one radix-2 DIF stage of the inverse transform over n = 2^logn points, half-size h = 2^s, one butterfly per thread:
+//   (u, v) -> (u + v, (u - v) omega_n^-e),  e = j 2^(logn - 1 - s) for the butterfly's offset j < h in its block
+// with omega_n^-e = -tw[n - 2e] for e > 0 (tw[k] = omega_2n^k, NttDomain), so the product is (v - u) tw[n - 2e]
+template <class C, class F>
+__global__ void __launch_bounds__(128) pts_intt_stage_kernel(void* __restrict__ pts, int logn, int s, const fe* __restrict__ tw) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= (1u << (logn - 1))) return;
+    const uint32_t h = 1u << s, j = t & (h - 1), i0 = ((t >> s) << (s + 1)) | j, i1 = i0 + h;
+    const uint32_t e = j << (logn - 1 - s);
+    const typename C::Pt u = pt_load<F>(pts, i0);
+    typename C::Pt v = pt_load<F>(pts, i1), sum = u;
+    C::add(sum, v);
+    C::add(v, C::neg(u));                                                  // v - u
+    if (e) {
+        const fe k = Fr::to_canonical(fe_load_nc(&tw[(1u << logn) - 2 * e]));
+        v = C::mul_scalar(v, k.l);
+    } else {
+        v = C::neg(v);
+    }
+    pt_store<F>(pts, i0, sum);
+    pt_store<F>(pts, i1, v);
+}
+
+// out[k] = scale x pts[bitrev(k)] in affine form: the natural order of the DIF output, times n^-1 (or (2n)^-1)
+template <class C, class F>
+__global__ void __launch_bounds__(128) pts_intt_finish_kernel(const void* __restrict__ pts, int logn, const fe* __restrict__ scale,
+                                                              void* __restrict__ out) {
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= (1u << logn)) return;
+    const uint32_t src = logn ? __brev(k) >> (32 - logn) : 0u;
+    const fe sc = *scale;
+    aff_store<F>(out, k, C::to_affine(C::mul_scalar(pt_load<F>(pts, src), sc.l)));
+}
+
+// sc[0] = n^-1, sc[1] = (2n)^-1 (canonical) from ninv = n^-1 (Montgomery)
+__global__ void pts_scale_kernel(const fe* __restrict__ ninv, fe* __restrict__ sc) {
+    if (threadIdx.x != 0 || blockIdx.x != 0) return;
+    fe two = fe_zero(); two.l[0] = 2;
+    sc[0] = Fr::to_canonical(*ninv);
+    sc[1] = Fr::to_canonical(Fr::mul(*ninv, Fr::inv(Fr::from_canonical(two))));
+}
+
+// the natural-order inverse transform of the XYZZ records at pts (n = 2^logn >= 2, in place through the DIF stages), times
+// *scale, to the affine points at out
+template <class C, class F>
+static void points_intt(const NttDomain& dom, void* pts, const fe* scale, void* out, cudaStream_t st) {
+    const int logn = dom.logn;
+    const uint32_t n = 1u << logn;
+    for (int s = logn - 1; s >= 0; s--)
+        pts_intt_stage_kernel<C, F><<<(n / 2 + 127) / 128, 128, 0, st>>>(pts, logn, s, dom.tw);
+    pts_intt_finish_kernel<C, F><<<(n + 127) / 128, 128, 0, st>>>(pts, logn, scale, out);
+    g_launch_count += logn + 1;
+    CUDA_CHECK(cudaGetLastError());
+}
+
+// LibsnarkReduction's H query: out[i] = tau[i + n] - tau[i], i < n - 1
+__global__ void __launch_bounds__(128) hq_libsnark_kernel(const void* __restrict__ tau, uint32_t n, void* __restrict__ out) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i + 1 >= n) return;
+    G1::Aff a = aff_load<Fq>(tau, i);
+    if (!G1::aff_is_inf(a)) a.y = Fq::neg(a.y);
+    G1::Pt p = G1::from_affine(aff_load<Fq>(tau, i + n));
+    G1::madd(p, a);
+    aff_store<Fq>(out, i, G1::to_affine(p));
+}
+
+// CircomReduction's folded input: pts[i] = omega_2n^-i (tau[i] - tau[i + n]) = tw[n - i] (tau[i + n] - tau[i]) for i > 0,
+// tau[0] - tau[n] for i = 0, with tau[2n - 1] taken as infinity
+__global__ void __launch_bounds__(128) hq_circom_kernel(const void* __restrict__ tau, uint32_t n, const fe* __restrict__ tw,
+                                                        void* __restrict__ pts) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    G1::Aff a = aff_load<Fq>(tau, i);
+    if (!G1::aff_is_inf(a)) a.y = Fq::neg(a.y);
+    G1::Pt p = i + n < 2 * n - 1 ? G1::from_affine(aff_load<Fq>(tau, i + n)) : G1::infinity();
+    G1::madd(p, a);
+    if (i) {
+        const fe k = Fr::to_canonical(fe_load_nc(&tw[n - i]));
+        p = G1::mul_scalar(p, k.l);
+    } else {
+        p = G1::neg(p);
+    }
+    pt_store<Fq>(pts, i, p);
+}
+
+// colptr[j] = the first k with keys[k] >= j, j <= nv (keys sorted)
+__global__ void __launch_bounds__(256) colptr_kernel(uint32_t nnz, uint32_t nv, const uint32_t* __restrict__ keys, uint32_t* __restrict__ colptr) {
+    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j > nv) return;
+    uint32_t lo = 0, hi = nnz;
+    while (lo < hi) {
+        const uint32_t mid = lo + (hi - lo) / 2;
+        if (keys[mid] < j) lo = mid + 1; else hi = mid;
+    }
+    colptr[j] = lo;
+}
+
+// the column j < nv whose pieces ptr[j] .. ptr[j + 1] - 1 hold piece q (ptr nondecreasing, ptr[nv] > q)
+__device__ __forceinline__ uint32_t piece_column(const uint32_t* __restrict__ ptr, uint32_t nv, uint32_t q) {
+    uint32_t lo = 0, hi = nv - 1;
+    while (lo < hi) {
+        const uint32_t mid = lo + (hi - lo + 1) / 2;
+        if (ptr[mid] <= q) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+}
+
+// first level of a column sum: piece q of column j sums up to PIECE_PRODUCTS products val[p] base[row of p] of the
+// column's nonzeros in sorted order (p = perm[k]); a coefficient k > r - k multiplies the negated point by r - k
+template <class C, class F>
+__global__ void __launch_bounds__(128) colsum_products_kernel(uint32_t pieces, uint32_t nv, uint32_t m, const uint32_t* __restrict__ rowptr,
+                                                              const fe* __restrict__ val, const uint32_t* __restrict__ perm,
+                                                              const uint32_t* __restrict__ colptr, const uint32_t* __restrict__ ptr,
+                                                              const void* __restrict__ base, void* __restrict__ out) {
+    const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= pieces) return;
+    const uint32_t j = piece_column(ptr, nv, q);
+    const uint32_t start = colptr[j] + (q - ptr[j]) * PIECE_PRODUCTS, end = min(start + PIECE_PRODUCTS, colptr[j + 1]);
+    typename C::Pt acc = C::infinity();
+    for (uint32_t k = start; k < end; k++) {
+        const uint32_t p = perm[k];
+        uint32_t lo = 0, hi = m - 1;                     // the last row r with rowptr[r] <= p
+        while (lo < hi) {
+            const uint32_t mid = lo + (hi - lo + 1) / 2;
+            if (rowptr[mid] <= p) lo = mid; else hi = mid - 1;
+        }
+        fe c = Fr::to_canonical(fe_load_nc(&val[p]));
+        typename C::Aff b = aff_load<F>(base, lo);
+        const fe nc = Fr::neg(c);
+        bool big = false;
+        for (int w = 7; w >= 0; w--) if (c.l[w] != nc.l[w]) { big = c.l[w] > nc.l[w]; break; }
+        if (big && !C::aff_is_inf(b)) { c = nc; b.y = F::neg(b.y); }
+        C::add(acc, aff_mul<C>(b, c.l));
+    }
+    pt_store<F>(out, q, acc);
+}
+
+// a later level: piece q of column j sums up to PIECE_SUMS of the column's records of the level below (ptr_in)
+template <class C, class F>
+__global__ void __launch_bounds__(128) colsum_reduce_kernel(uint32_t pieces, uint32_t nv, const uint32_t* __restrict__ ptr_in,
+                                                            const uint32_t* __restrict__ ptr, const void* __restrict__ in, void* __restrict__ out) {
+    const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= pieces) return;
+    const uint32_t j = piece_column(ptr, nv, q);
+    const uint32_t start = ptr_in[j] + (q - ptr[j]) * PIECE_SUMS, end = min(start + PIECE_SUMS, ptr_in[j + 1]);
+    typename C::Pt acc = pt_load<F>(in, start);
+    for (uint32_t k = start + 1; k < end; k++) C::add(acc, pt_load<F>(in, k));
+    pt_store<F>(out, q, acc);
+}
+
+// acc[j] += in[ptr[j]] for the columns with a piece at the last level (at most one each)
+template <class C, class F>
+__global__ void __launch_bounds__(128) colsum_accumulate_kernel(uint32_t nv, const uint32_t* __restrict__ ptr, const void* __restrict__ in,
+                                                                void* __restrict__ acc) {
+    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= nv || ptr[j + 1] == ptr[j]) return;
+    typename C::Pt a = pt_load<F>(acc, j);
+    C::add(a, pt_load<F>(in, ptr[j]));
+    pt_store<F>(acc, j, a);
+}
+
+// out[j] = acc[j] (+ extra[m + j] for j < ni when extra is given), affine
+template <class C, class F>
+__global__ void __launch_bounds__(128) colsum_finish_kernel(uint32_t nv, uint32_t ni, uint32_t m, const void* __restrict__ acc,
+                                                            const void* __restrict__ extra, void* __restrict__ out) {
+    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= nv) return;
+    typename C::Pt a = pt_load<F>(acc, j);
+    if (extra && j < ni) C::madd(a, aff_load<F>(extra, (size_t)m + j));
+    aff_store<F>(out, j, C::to_affine(a));
+}
+
+// one matrix on the device with its nonzeros in column order (perm) and the pieces of every level of its column sums: level
+// l >= 1 gives column j the pieces ptr[l][j] .. ptr[l][j + 1] - 1; ptr[0] is the column pointer of the sorted nonzeros.  The
+// last level has at most one piece per column.
+struct ColPlan {
+    uint32_t nnz = 0;
+    const uint32_t* rowptr = nullptr;
+    const fe* val = nullptr;
+    const uint32_t* perm = nullptr;
+    std::vector<const uint32_t*> ptr;
+    std::vector<uint32_t> pieces;
+};
+
+static ColPlan col_plan(SetupMem& mem, const b2g_mat_desc* d, int x, uint32_t nv, cudaStream_t st) {
+    const uint32_t m = d->num_constraints;
+    const uint32_t* rowptrs[3] = {d->a_rowptr, d->b_rowptr, d->c_rowptr};
+    const uint32_t* cols[3] = {d->a_col, d->b_col, d->c_col};
+    const void* vals[3] = {d->a_val, d->b_val, d->c_val};
+    ColPlan cp;
+    cp.nnz = rowptrs[x][m];
+    if (!cp.nnz) return cp;
+    const uint32_t nnz = cp.nnz;
+    const unsigned blocks = (nnz + 255) / 256;
+    int end_bit = 1;
+    while (end_bit < 32 && (1ull << end_bit) < nv) end_bit++;
+    uint32_t* d_rowptr = mem.alloc<uint32_t>(((size_t)m + 1) * 4);
+    uint32_t* d_col = mem.alloc<uint32_t>((size_t)nnz * 4);
+    fe* d_val = mem.alloc<fe>((size_t)nnz * sizeof(fe));
+    uint32_t* d_keys = mem.alloc<uint32_t>((size_t)nnz * 4);
+    uint32_t* d_idx = mem.alloc<uint32_t>((size_t)nnz * 4);
+    uint32_t* d_perm = mem.alloc<uint32_t>((size_t)nnz * 4);
+    uint32_t* d_colptr = mem.alloc<uint32_t>(((size_t)nv + 1) * 4);
+    size_t sort_bytes = 0;
+    CUDA_CHECK(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, d_col, d_keys, d_idx, d_perm, (int)nnz, 0, end_bit, st));
+    void* d_temp = mem.alloc<void>(sort_bytes);
+    CUDA_CHECK(cudaMemcpyAsync(d_rowptr, rowptrs[x], ((size_t)m + 1) * 4, cudaMemcpyHostToDevice, st));
+    CUDA_CHECK(cudaMemcpyAsync(d_col, cols[x], (size_t)nnz * 4, cudaMemcpyHostToDevice, st));
+    CUDA_CHECK(cudaMemcpyAsync(d_val, vals[x], (size_t)nnz * sizeof(fe), cudaMemcpyHostToDevice, st));
+    setup_iota_kernel<<<blocks, 256, 0, st>>>(nnz, d_idx);
+    CUDA_CHECK(cub::DeviceRadixSort::SortPairs(d_temp, sort_bytes, d_col, d_keys, d_idx, d_perm, (int)nnz, 0, end_bit, st));
+    colptr_kernel<<<(nv + 256) / 256, 256, 0, st>>>(nnz, nv, d_keys, d_colptr);
+    g_launch_count += 2;
+    CUDA_CHECK(cudaGetLastError());
+    std::vector<uint32_t> cur(nv + 1);
+    CUDA_CHECK(cudaMemcpyAsync(cur.data(), d_colptr, ((size_t)nv + 1) * 4, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    cp.rowptr = d_rowptr; cp.val = d_val; cp.perm = d_perm;
+    cp.ptr.push_back(d_colptr);
+    cp.pieces.push_back(nnz);
+    // the pieces of each level on the host, from the counts of the level below, until no column has more than one
+    for (uint32_t per = PIECE_PRODUCTS, most = 2; most > 1; per = PIECE_SUMS) {
+        std::vector<uint32_t> next(nv + 1, 0);
+        most = 0;
+        for (uint32_t j = 0; j < nv; j++) {
+            const uint32_t c = (cur[j + 1] - cur[j] + per - 1) / per;
+            next[j + 1] = next[j] + c;
+            most = std::max(most, c);
+        }
+        uint32_t* d_ptr = mem.alloc<uint32_t>(((size_t)nv + 1) * 4);
+        CUDA_CHECK(cudaMemcpyAsync(d_ptr, next.data(), ((size_t)nv + 1) * 4, cudaMemcpyHostToDevice, st));
+        CUDA_CHECK(cudaStreamSynchronize(st));                         // `next` is freed at the end of this iteration
+        cp.ptr.push_back(d_ptr);
+        cp.pieces.push_back(next[nv]);
+        cur.swap(next);
+    }
+    return cp;
+}
+
+// acc[j] += sum over the nonzeros (r, j, k) of the plan's matrix of k base[r] (XYZZ accumulators, one per column), through
+// the scratch areas x and y (each at least cp.pieces[1] records)
+template <class C, class F>
+static void col_sums(const ColPlan& cp, uint32_t nv, uint32_t m, const void* base, uint8_t* x, uint8_t* y, void* acc, cudaStream_t st) {
+    if (!cp.nnz) return;
+    colsum_products_kernel<C, F><<<(cp.pieces[1] + 127) / 128, 128, 0, st>>>(cp.pieces[1], nv, m, cp.rowptr, cp.val, cp.perm, cp.ptr[0],
+                                                                              cp.ptr[1], base, x);
+    for (size_t l = 2; l < cp.ptr.size(); l++) {
+        colsum_reduce_kernel<C, F><<<(cp.pieces[l] + 127) / 128, 128, 0, st>>>(cp.pieces[l], nv, cp.ptr[l - 1], cp.ptr[l], x, y);
+        std::swap(x, y);
+    }
+    colsum_accumulate_kernel<C, F><<<(nv + 127) / 128, 128, 0, st>>>(nv, cp.ptr.back(), x, acc);
+    g_launch_count += cp.ptr.size();
+    CUDA_CHECK(cudaGetLastError());
+}
+
+// uploads n affine points (row bytes each) and refuses the array when one of them is off its curve, has a coordinate >= p
+// or (subgroup) lies outside G2; `name` names the array in the message
+static uint8_t* powers_upload(SetupMem& mem, const char* name, const void* host, size_t n, bool g2, bool subgroup, cudaStream_t st) {
+    const size_t row = g2 ? 128 : 64;
+    uint8_t* d = mem.alloc<uint8_t>(n * row);
+    CUDA_CHECK(cudaMemcpyAsync(d, host, n * row, cudaMemcpyHostToDevice, st));
+    int why = 0;
+    const uint64_t bad = points_check(g2, d, n, subgroup, st, &why);
+    if (bad < n)
+        throw_error(B2G_E_INPUT, std::string(name) + "[" + std::to_string(bad) + "]: " +
+                                     (why == 2 ? "not in G2" : g2 ? "off the twist or a coordinate >= p" : "off the curve or a coordinate >= p"));
+    return d;
+}
+
+static void setup_from_powers_run(b2g_ctx* ctx, const b2g_mat_desc* d, const b2g_powers_desc* pw, const b2g_setup_out* o) {
+    if (!ctx || !d || !pw || !o) throw_error(B2G_E_SHAPE, "null pointer");
+    const CtxView cv = ctx_view(ctx);
+    if (cv.proof_pending) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
+    const int logn = mat_desc_check(d, true);
+    const bool libsnark = d->reduction == B2G_REDUCTION_LIBSNARK;
+    if (!libsnark && logn > 26) throw_error(B2G_E_DOMAIN, "PolynomialDegreeTooLarge: a CircomReduction setup transforms over 2n points, so n must fit 2^26");
+    if (pw->log_size > 28 || logn > (int)pw->log_size)
+        throw_error(B2G_E_DOMAIN, "PolynomialDegreeTooLarge: the circuit's domain of 2^" + std::to_string(logn) +
+                                      " points exceeds the ceremony's 2^" + std::to_string(pw->log_size) + " powers");
+    if (!pw->tau_g1 || !pw->tau_g2 || !pw->alpha_tau_g1 || !pw->beta_tau_g1 || !pw->beta_g2) throw_error(B2G_E_SHAPE, "null powers array");
+    const uint32_t m = d->num_constraints, ni = d->num_inputs, nv = d->n_vars;
+    const size_t n = (size_t)1 << logn, nh = libsnark ? n - 1 : n;
+    if (!o->alpha_g1 || !o->beta_g1 || !o->delta_g1 || !o->beta_g2 || !o->gamma_g2 || !o->delta_g2 || !o->gamma_abc_g1 || !o->a_query ||
+        !o->b_g1_query || !o->b_g2_query || (nv > ni && !o->l_query) || (nh && !o->h_query))
+        throw_error(B2G_E_SHAPE, "null output buffer");
+    const uint32_t maxnnz = std::max(d->a_rowptr[m], std::max(d->b_rowptr[m], d->c_rowptr[m]));
+    if (maxnnz > (uint32_t)INT32_MAX) throw_error(B2G_E_DEVICE, "b2g_setup_from_powers: more than 2^31 - 1 nonzeros in one matrix");
+
+    DevGuard g(cv.device);
+    cudaStream_t st = cv.st;
+    SetupMem mem{st, {}};
+    uint8_t* d_tau1 = powers_upload(mem, "tau_g1", pw->tau_g1, 2 * n - 1, false, false, st);
+    uint8_t* d_tau2 = powers_upload(mem, "tau_g2", pw->tau_g2, n, true, true, st);
+    uint8_t* d_atau = powers_upload(mem, "alpha_tau_g1", pw->alpha_tau_g1, n, false, false, st);
+    uint8_t* d_btau = powers_upload(mem, "beta_tau_g1", pw->beta_tau_g1, n, false, false, st);
+    powers_upload(mem, "beta_g2", pw->beta_g2, 1, true, true, st);
+    if (all_zero32((const uint8_t*)pw->tau_g1) && all_zero32((const uint8_t*)pw->tau_g1 + 32)) throw_error(B2G_E_INPUT, "tau_g1[0]: at infinity");
+    {
+        bool inf = true;
+        for (int i = 0; i < 4; i++) inf = inf && all_zero32((const uint8_t*)pw->tau_g2 + 32 * i);
+        if (inf) throw_error(B2G_E_INPUT, "tau_g2[0]: at infinity");
+    }
+
+    // the Lagrange points: four transforms through one XYZZ work area
+    NttDomain dom;
+    struct DomGuard { NttDomain& d; ~DomGuard() { ntt_domain_destroy(d); } } dg{dom};
+    ntt_domain_create(dom, logn, st);
+    fe* d_sc = mem.alloc<fe>(2 * sizeof(fe));
+    pts_scale_kernel<<<1, 1, 0, st>>>(dom.ct, d_sc);                       // ct[0] = n^-1
+    g_launch_count += 1;
+    uint8_t* d_work = mem.alloc<uint8_t>(n * 256);
+    uint8_t* d_L1 = mem.alloc<uint8_t>(n * 64);
+    uint8_t* d_L2 = mem.alloc<uint8_t>(n * 128);
+    uint8_t* d_aL = mem.alloc<uint8_t>(n * 64);
+    uint8_t* d_bL = mem.alloc<uint8_t>(n * 64);
+    const unsigned pblocks = (unsigned)((n + 127) / 128);
+    const std::pair<const uint8_t*, uint8_t*> g1_sets[3] = {{d_tau1, d_L1}, {d_atau, d_aL}, {d_btau, d_bL}};
+    for (const auto& s : g1_sets) {
+        pts_from_affine_kernel<G1, Fq><<<pblocks, 128, 0, st>>>(s.first, (uint32_t)n, d_work);
+        points_intt<G1, Fq>(dom, d_work, d_sc, s.second, st);
+    }
+    pts_from_affine_kernel<G2, Fq2><<<pblocks, 128, 0, st>>>(d_tau2, (uint32_t)n, d_work);
+    points_intt<G2, Fq2>(dom, d_work, d_sc, d_L2, st);
+    g_launch_count += 4;
+
+    // the H query
+    uint8_t* d_h = mem.alloc<uint8_t>(n * 64);
+    if (libsnark) {
+        hq_libsnark_kernel<<<pblocks, 128, 0, st>>>(d_tau1, (uint32_t)n, d_h);
+        g_launch_count += 1;
+    } else {
+        hq_circom_kernel<<<pblocks, 128, 0, st>>>(d_tau1, (uint32_t)n, dom.tw, d_work);
+        g_launch_count += 1;
+        points_intt<G1, Fq>(dom, d_work, d_sc + 1, d_h, st);
+    }
+    CUDA_CHECK(cudaGetLastError());
+
+    // column sums: a = A L, b1 = B L, b2 = B L2, k = A beta L + B alpha L + C L, then the public-input rows and affine form
+    const ColPlan plans[3] = {col_plan(mem, d, 0, nv, st), col_plan(mem, d, 1, nv, st), col_plan(mem, d, 2, nv, st)};
+    size_t scratch = 1;
+    for (const ColPlan& cp : plans) if (cp.nnz) scratch = std::max(scratch, (size_t)cp.pieces[1]);
+    uint8_t* d_x = mem.alloc<uint8_t>(scratch * 256);
+    uint8_t* d_y = mem.alloc<uint8_t>(scratch * 256);
+    uint8_t* d_acc = mem.alloc<uint8_t>((size_t)nv * (128 * 3 + 256));
+    CUDA_CHECK(cudaMemsetAsync(d_acc, 0, (size_t)nv * (128 * 3 + 256), st));
+    uint8_t *acc_a = d_acc, *acc_b1 = acc_a + (size_t)nv * 128, *acc_k = acc_b1 + (size_t)nv * 128, *acc_b2 = acc_k + (size_t)nv * 128;
+    col_sums<G1, Fq>(plans[0], nv, m, d_L1, d_x, d_y, acc_a, st);
+    col_sums<G1, Fq>(plans[1], nv, m, d_L1, d_x, d_y, acc_b1, st);
+    col_sums<G2, Fq2>(plans[1], nv, m, d_L2, d_x, d_y, acc_b2, st);
+    col_sums<G1, Fq>(plans[0], nv, m, d_bL, d_x, d_y, acc_k, st);
+    col_sums<G1, Fq>(plans[1], nv, m, d_aL, d_x, d_y, acc_k, st);
+    col_sums<G1, Fq>(plans[2], nv, m, d_L1, d_x, d_y, acc_k, st);
+    uint8_t* d_out = mem.alloc<uint8_t>((size_t)nv * (64 * 3 + 128));
+    uint8_t *out_a = d_out, *out_b1 = out_a + (size_t)nv * 64, *out_k = out_b1 + (size_t)nv * 64, *out_b2 = out_k + (size_t)nv * 64;
+    const unsigned vblocks = (nv + 127) / 128;
+    colsum_finish_kernel<G1, Fq><<<vblocks, 128, 0, st>>>(nv, ni, m, acc_a, d_L1, out_a);
+    colsum_finish_kernel<G1, Fq><<<vblocks, 128, 0, st>>>(nv, ni, m, acc_b1, nullptr, out_b1);
+    colsum_finish_kernel<G1, Fq><<<vblocks, 128, 0, st>>>(nv, ni, m, acc_k, d_bL, out_k);
+    colsum_finish_kernel<G2, Fq2><<<vblocks, 128, 0, st>>>(nv, ni, m, acc_b2, nullptr, out_b2);
+    g_launch_count += 4;
+    CUDA_CHECK(cudaGetLastError());
+
+    CUDA_CHECK(cudaMemcpyAsync(o->a_query, out_a, (size_t)nv * 64, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaMemcpyAsync(o->b_g1_query, out_b1, (size_t)nv * 64, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaMemcpyAsync(o->b_g2_query, out_b2, (size_t)nv * 128, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaMemcpyAsync(o->gamma_abc_g1, out_k, (size_t)ni * 64, cudaMemcpyDeviceToHost, st));
+    if (nv > ni) CUDA_CHECK(cudaMemcpyAsync(o->l_query, out_k + (size_t)ni * 64, (size_t)(nv - ni) * 64, cudaMemcpyDeviceToHost, st));
+    if (nh) CUDA_CHECK(cudaMemcpyAsync(o->h_query, d_h, nh * 64, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    memcpy(o->alpha_g1, pw->alpha_tau_g1, 64);
+    memcpy(o->beta_g1, pw->beta_tau_g1, 64);
+    memcpy(o->delta_g1, pw->tau_g1, 64);
+    memcpy(o->beta_g2, pw->beta_g2, 128);
+    memcpy(o->gamma_g2, pw->tau_g2, 128);
+    memcpy(o->delta_g2, pw->tau_g2, 128);
+}
+
+// b2g_points_intt: n = 2^logn affine points in place (host buffer)
+static void points_intt_run(b2g_ctx* ctx, int g2, int logn, void* pts) {
+    if (!ctx || !pts) throw_error(B2G_E_SHAPE, "null pointer");
+    const CtxView cv = ctx_view(ctx);
+    if (cv.proof_pending) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
+    if (logn < 1 || logn > 27) throw_error(B2G_E_DOMAIN, "b2g_points_intt: log_n must be in 1..27");
+    const size_t n = (size_t)1 << logn, row = g2 ? 128 : 64;
+    DevGuard g(cv.device);
+    cudaStream_t st = cv.st;
+    SetupMem mem{st, {}};
+    uint8_t* d_in = mem.alloc<uint8_t>(n * row);
+    uint8_t* d_work = mem.alloc<uint8_t>(n * row * 2);
+    fe* d_sc = mem.alloc<fe>(2 * sizeof(fe));
+    NttDomain dom;
+    struct DomGuard { NttDomain& d; ~DomGuard() { ntt_domain_destroy(d); } } dg{dom};
+    ntt_domain_create(dom, logn, st);
+    pts_scale_kernel<<<1, 1, 0, st>>>(dom.ct, d_sc);
+    g_launch_count += 2;
+    CUDA_CHECK(cudaMemcpyAsync(d_in, pts, n * row, cudaMemcpyHostToDevice, st));
+    const unsigned blocks = (unsigned)((n + 127) / 128);
+    if (g2) {
+        pts_from_affine_kernel<G2, Fq2><<<blocks, 128, 0, st>>>(d_in, (uint32_t)n, d_work);
+        points_intt<G2, Fq2>(dom, d_work, d_sc, d_in, st);
+    } else {
+        pts_from_affine_kernel<G1, Fq><<<blocks, 128, 0, st>>>(d_in, (uint32_t)n, d_work);
+        points_intt<G1, Fq>(dom, d_work, d_sc, d_in, st);
+    }
+    CUDA_CHECK(cudaMemcpyAsync(pts, d_in, n * row, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaStreamSynchronize(st));
+}
+
+// ---------------------------------------------------------------------------------------------- delta contributions
+// k[1] = x^-1 (canonical) from k[0] = x (canonical, nonzero, below r)
+__global__ void delta_inverse_kernel(fe* __restrict__ k) {
+    if (threadIdx.x != 0 || blockIdx.x != 0) return;
+    k[1] = Fr::to_canonical(Fr::inv(Fr::from_canonical(k[0])));
+}
+
+// out[i] = k pts[i] (affine), one point per thread
+template <class C, class F>
+__global__ void __launch_bounds__(128) pts_scale_by_kernel(const void* __restrict__ pts, uint32_t n, const fe* __restrict__ k,
+                                                           void* __restrict__ out) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const fe s = *k;
+    aff_store<F>(out, i, C::to_affine(aff_mul<C>(aff_load<F>(pts, i), s.l)));
+}
+
+static void delta_update_run(b2g_ctx* ctx, const b2g_delta_key* a, const void* x_canon, b2g_delta_key* b) {
+    if (!ctx || !a || !x_canon || !b) throw_error(B2G_E_SHAPE, "null pointer");
+    if (!a->delta_g1 || !a->delta_g2 || !b->delta_g1 || !b->delta_g2 || (a->n_l && (!a->l_query || !b->l_query)) ||
+        (a->n_h && (!a->h_query || !b->h_query)))
+        throw_error(B2G_E_SHAPE, "null key buffer");
+    if (a->n_l != b->n_l || a->n_h != b->n_h) throw_error(B2G_E_SHAPE, "b2g_delta_update: the two keys' n_l / n_h differ");
+    const CtxView cv = ctx_view(ctx);
+    if (cv.proof_pending) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
+    if (!below((const uint8_t*)x_canon, R_WORDS)) throw_error(B2G_E_INPUT, "x is not below r");
+    if (all_zero32((const uint8_t*)x_canon)) throw_error(B2G_E_INPUT, "x is zero");
+    DevGuard g(cv.device);
+    cudaStream_t st = cv.st;
+    SetupMem mem{st, {}};
+    uint8_t* d_d1 = powers_upload(mem, "delta_g1", a->delta_g1, 1, false, false, st);
+    uint8_t* d_d2 = powers_upload(mem, "delta_g2", a->delta_g2, 1, true, true, st);
+    uint8_t* d_l = powers_upload(mem, "l_query", a->l_query, a->n_l, false, false, st);
+    uint8_t* d_h = powers_upload(mem, "h_query", a->h_query, a->n_h, false, false, st);
+    fe* d_k = mem.alloc<fe>(2 * sizeof(fe));
+    {
+        uint8_t h_x[32];
+        memcpy(h_x, x_canon, 32);
+        // on the call's stream; h_x is wiped once the copy is done
+        cudaError_t e = cudaMemcpyAsync(d_k, h_x, 32, cudaMemcpyHostToDevice, st);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+        secure_zero(h_x, sizeof(h_x));
+        CUDA_CHECK(e);
+    }
+    delta_inverse_kernel<<<1, 1, 0, st>>>(d_k);
+    const size_t most = std::max((size_t)std::max(a->n_l, a->n_h), (size_t)2);
+    uint8_t* d_out = mem.alloc<uint8_t>(most * 64);
+    uint8_t* d_out2 = mem.alloc<uint8_t>(128);
+    pts_scale_by_kernel<G1, Fq><<<1, 128, 0, st>>>(d_d1, 1, d_k, d_out);
+    pts_scale_by_kernel<G2, Fq2><<<1, 128, 0, st>>>(d_d2, 1, d_k, d_out2);
+    g_launch_count += 3;
+    CUDA_CHECK(cudaMemcpyAsync(b->delta_g1, d_out, 64, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaMemcpyAsync(b->delta_g2, d_out2, 128, cudaMemcpyDeviceToHost, st));
+    const std::pair<const uint8_t*, std::pair<uint32_t, void*>> qs[2] = {{d_l, {a->n_l, b->l_query}}, {d_h, {a->n_h, b->h_query}}};
+    for (const auto& q : qs) {
+        const uint32_t n = q.second.first;
+        if (!n) continue;
+        CUDA_CHECK(cudaStreamSynchronize(st));                             // d_out is reused
+        pts_scale_by_kernel<G1, Fq><<<(n + 127) / 128, 128, 0, st>>>(q.first, n, d_k + 1, d_out);
+        g_launch_count += 1;
+        CUDA_CHECK(cudaGetLastError());
+        CUDA_CHECK(cudaMemcpyAsync(q.second.second, d_out, (size_t)n * 64, cudaMemcpyDeviceToHost, st));
+    }
+    CUDA_CHECK(cudaGetLastError());
+    CUDA_CHECK(cudaStreamSynchronize(st));
+}
+
+// runs the body of a C entry point; a buffer that did not fit leaves cudaErrorMemoryAllocation as the thread's last error:
+// it is cleared, so that the context's next call does not fail on it
+template <class Fn>
+static int setup_guarded(Fn&& fn) {
+    return guarded([&] {
+        try {
+            fn();
+        } catch (const B2gError& e) {
+            if (e.code == B2G_E_DEVICE) cudaGetLastError();
+            throw;
+        }
+    });
+}
+
 }  // namespace b2g
 
 extern "C" {
@@ -331,6 +859,18 @@ int b2g_setup(b2g_ctx* ctx, const b2g_mat_desc* circuit, const b2g_setup_secrets
             throw;
         }
     });
+}
+
+int b2g_setup_from_powers(b2g_ctx* ctx, const b2g_mat_desc* circuit, const b2g_powers_desc* powers, b2g_setup_out* out) {
+    return b2g::setup_guarded([&] { b2g::setup_from_powers_run(ctx, circuit, powers, out); });
+}
+
+int b2g_points_intt(b2g_ctx* ctx, int g2, int log_n, void* points_mont) {
+    return b2g::setup_guarded([&] { b2g::points_intt_run(ctx, g2, log_n, points_mont); });
+}
+
+int b2g_delta_update(b2g_ctx* ctx, const b2g_delta_key* before, const void* x_canon, b2g_delta_key* after) {
+    return b2g::setup_guarded([&] { b2g::delta_update_run(ctx, before, x_canon, after); });
 }
 
 }  // extern "C"

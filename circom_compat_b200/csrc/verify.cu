@@ -1251,6 +1251,160 @@ __global__ void setup_generators_kernel(const void* __restrict__ g1, const void*
     }
 }
 
+// bad = the lowest point with a coordinate >= p or off its curve (infinity = zeros passes)
+template <class C, class F>
+__global__ void __launch_bounds__(128) points_curve_kernel(const uint8_t* __restrict__ pts, uint32_t n, unsigned long long* __restrict__ bad) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    constexpr int WORDS = 2 * Bytes<F>::ELEM / 32;
+    bool ok = true;
+    for (int k = 0; k < WORDS; k++) ok &= fe_below_p(fe_load(pts + ((size_t)i * WORDS + k) * 32));
+    if (!ok || !aff_on_curve<C, F>(aff_load<F>(pts, i))) atomicMin(bad, (unsigned long long)i);
+}
+
+uint64_t points_check(bool g2, const void* pts, size_t n, bool subgroup, cudaStream_t st, int* why) {
+    *why = 0;
+    if (n == 0) return 0;
+    unsigned long long* d_bad = nullptr;
+    CUDA_CHECK(cudaMalloc(&d_bad, 2 * sizeof(unsigned long long)));
+    uint64_t bad[2] = {n, n};
+    const unsigned blocks = (unsigned)((n + 127) / 128);
+    cudaError_t e = cudaMemcpyAsync(d_bad, bad, sizeof(bad), cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) {
+        if (g2) points_curve_kernel<G2, Fq2><<<blocks, 128, 0, st>>>((const uint8_t*)pts, (uint32_t)n, d_bad);
+        else points_curve_kernel<G1, Fq><<<blocks, 128, 0, st>>>((const uint8_t*)pts, (uint32_t)n, d_bad);
+        if (g2 && subgroup) points_g2_subgroup_kernel<<<blocks, 128, 0, st>>>((const uint8_t*)pts, (uint32_t)n, 0, d_bad + 1);
+        g_launch_count += g2 && subgroup ? 2 : 1;
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(bad, d_bad, sizeof(bad), cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    cudaFree(d_bad);
+    CUDA_CHECK(e);
+    // a point off its curve is also tested for G2 membership: the curve failure names it
+    if (bad[0] < n && bad[0] <= bad[1]) { *why = 1; return bad[0]; }
+    if (bad[1] < n) { *why = 2; return bad[1]; }
+    return n;
+}
+
+// ---------------------------------------------------------------------------------------------- delta update check
+// b2g_delta_update_check: rec[i] = w_i after[i], rec[N + i] = w_i before[i] for the N = n_l + n_h points L || H of each key
+// (G1 XYZZ); clears *ok when an after point has a coordinate >= p or lies off its curve
+__global__ void __launch_bounds__(128) delta_weigh_kernel(const uint8_t* __restrict__ after, const uint8_t* __restrict__ before,
+                                                          const uint32_t* __restrict__ w, uint32_t n, uint8_t* __restrict__ rec,
+                                                          uint32_t* __restrict__ ok) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    bool good = true;
+    for (int k = 0; k < 2; k++) good &= fe_below_p(fe_load(after + ((size_t)i * 2 + k) * 32));
+    const G1::Aff a = aff_load<Fq>(after, i), b = aff_load<Fq>(before, i);
+    if (!good || !aff_on_curve<G1, Fq>(a)) atomicAnd(ok, 0u);
+    uint32_t k[4];
+    weight_load(k, w, i);
+    pt_store<Fq>(rec, i, G1::mul_affine(a, k, 4));
+    pt_store<Fq>(rec, (size_t)n + i, G1::mul_affine(b, k, 4));
+}
+
+// one block of 32 threads: threads 0-3 compute the four pairings e(d1', d2), e(d1, d2'), e(S', d2'), e(S, d2), thread 4
+// checks the point rules, and thread 0 then gives the verdict.
+// d = before d1 (64 B), before d2 (128 B), after d1, after d2; S' and S are the XYZZ sums at the first two tails.
+__global__ void __launch_bounds__(32) delta_verdict_kernel(const uint8_t* __restrict__ d, const uint8_t* __restrict__ tails,
+                                                           const uint32_t* __restrict__ ok, uint8_t* __restrict__ verdict) {
+    __shared__ fe12 e[4];
+    __shared__ uint32_t good;
+    const uint32_t t = threadIdx.x;
+    const G1::Aff d1 = aff_load<Fq>(d, 0), d1a = aff_load<Fq>(d + 192, 0);
+    const G2::Aff d2 = aff_load<Fq2>(d + 64, 0), d2a = aff_load<Fq2>(d + 256, 0);
+    if (t == 4) {
+        bool g = *ok != 0;
+        for (int k = 0; k < 6; k++) g &= fe_below_p(fe_load(d + 192 + 32 * k));
+        g = g && aff_on_curve<G1, Fq>(d1a) && aff_on_curve<G2, Fq2>(d2a) && !G1::aff_is_inf(d1a) && !G2::aff_is_inf(d2a) &&
+            !G2::aff_is_inf(d2) && g2_in_subgroup(d2a);
+        good = g;
+    } else if (t < 4) {
+        G1::Aff p;
+        if (t == 0) p = d1a;
+        else if (t == 1) p = d1;
+        else p = G1::to_affine(pt_load<Fq>(tails + (size_t)(t - 2) * TAIL_BYTES, 0));
+        fe12 r;
+        pairing(r, p, t == 0 || t == 3 ? d2 : d2a);
+        e[t] = r;
+    }
+    __syncthreads();
+    if (t == 0) *verdict = good && Fq12::eq(e[0], e[1]) && Fq12::eq(e[2], e[3]);
+}
+
+static void delta_check_run(b2g_ctx* ctx, const b2g_delta_key* a, const b2g_delta_key* b, const void* weights, uint8_t* verdict_out) {
+    if (!ctx || !a || !b || !verdict_out) throw_error(B2G_E_SHAPE, "null pointer");
+    if (!a->delta_g1 || !a->delta_g2 || !b->delta_g1 || !b->delta_g2 || (a->n_l && !a->l_query) || (a->n_h && !a->h_query) ||
+        (b->n_l && !b->l_query) || (b->n_h && !b->h_query))
+        throw_error(B2G_E_SHAPE, "null key buffer");
+    const CtxView cv = ctx_view(ctx);
+    if (cv.proof_pending) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
+    *verdict_out = 0;
+    const uint64_t n64 = (uint64_t)a->n_l + a->n_h;
+    if (n64 && !weights) throw_error(B2G_E_SHAPE, "null pointer");
+    if (n64 >= (1ull << 31)) throw_error(B2G_E_DEVICE, "b2g_delta_update_check: more than 2^31 - 1 points");
+    const uint32_t n = (uint32_t)n64;
+    for (uint32_t i = 0; i < n; i++)
+        if (all_zero((const uint8_t*)weights + 16 * (size_t)i, 16)) throw_error(B2G_E_INPUT, "weight " + std::to_string(i) + " is zero");
+    if (a->n_l != b->n_l || a->n_h != b->n_h) return;
+    DevGuard g(cv.device);
+    cudaStream_t st = cv.st;
+    // one allocation: the four delta points, after L || H, before L || H, the weights, 2n records, two scratch areas, the
+    // tails of the two sums, the spans, the ok word and the verdict
+    std::vector<Seg> segs(2);
+    segs[0].first = 0; segs[0].count = n; segs[1].first = n; segs[1].count = n;
+    std::vector<Span> spans;
+    size_t scratch = 0;
+    const std::vector<uint32_t> levels = n ? reduce_plan(segs, 128, spans, &scratch) : std::vector<uint32_t>();
+    const size_t o_pts = 384, o_before = o_pts + (size_t)n * 64, o_w = o_before + (size_t)n * 64, o_rec = o_w + (size_t)n * 16;
+    const size_t o_x = o_rec + (size_t)n * 256, o_y = o_x + std::max(scratch, (size_t)1) * 128;
+    const size_t o_tails = (o_y + std::max(scratch, (size_t)1) * 128 + 255) & ~(size_t)255, o_spans = o_tails + 2 * TAIL_BYTES;
+    const size_t o_ok = o_spans + std::max(spans.size(), (size_t)1) * sizeof(Span), bytes = o_ok + 8;
+    struct Buf { uint8_t* p = nullptr; ~Buf() { if (p) cudaFree(p); } } buf;
+    if (cudaMalloc(&buf.p, bytes) != cudaSuccess) {
+        cudaGetLastError();
+        buf.p = nullptr;
+        throw_error(B2G_E_DEVICE, "b2g_delta_update_check: the device buffers (" + std::to_string((bytes + (1 << 20) - 1) >> 20) +
+                                      " MiB) do not fit in device memory");
+    }
+    uint8_t* D = buf.p;
+    try {
+        const uint32_t one = 1;
+        CUDA_CHECK(cudaMemsetAsync(D + o_tails, 0, 2 * TAIL_BYTES, st));
+        CUDA_CHECK(cudaMemcpyAsync(D + o_ok, &one, 4, cudaMemcpyHostToDevice, st));
+        CUDA_CHECK(cudaMemcpyAsync(D, a->delta_g1, 64, cudaMemcpyHostToDevice, st));
+        CUDA_CHECK(cudaMemcpyAsync(D + 64, a->delta_g2, 128, cudaMemcpyHostToDevice, st));
+        CUDA_CHECK(cudaMemcpyAsync(D + 192, b->delta_g1, 64, cudaMemcpyHostToDevice, st));
+        CUDA_CHECK(cudaMemcpyAsync(D + 256, b->delta_g2, 128, cudaMemcpyHostToDevice, st));
+        if (n) {
+            const size_t nl = a->n_l, nh = a->n_h;
+            if (nl) CUDA_CHECK(cudaMemcpyAsync(D + o_pts, b->l_query, nl * 64, cudaMemcpyHostToDevice, st));
+            if (nh) CUDA_CHECK(cudaMemcpyAsync(D + o_pts + nl * 64, b->h_query, nh * 64, cudaMemcpyHostToDevice, st));
+            if (nl) CUDA_CHECK(cudaMemcpyAsync(D + o_before, a->l_query, nl * 64, cudaMemcpyHostToDevice, st));
+            if (nh) CUDA_CHECK(cudaMemcpyAsync(D + o_before + nl * 64, a->h_query, nh * 64, cudaMemcpyHostToDevice, st));
+            CUDA_CHECK(cudaMemcpyAsync(D + o_w, weights, (size_t)n * 16, cudaMemcpyHostToDevice, st));
+            CUDA_CHECK(cudaMemcpyAsync(D + o_spans, spans.data(), spans.size() * sizeof(Span), cudaMemcpyHostToDevice, st));
+            delta_weigh_kernel<<<(n + 127) / 128, 128, 0, st>>>(D + o_pts, D + o_before, (const uint32_t*)(D + o_w), n, D + o_rec,
+                                                                (uint32_t*)(D + o_ok));
+            g_launch_count += 1;
+            reduce_run(levels, (const Span*)(D + o_spans), D + o_rec, 128, 128, nullptr, D + o_x, D + o_y,
+                       [&](uint32_t blocks, const uint8_t* src, size_t stride, const Span* sp, const uint8_t* mask, uint8_t* dst) {
+                           g1_sum_kernel<<<blocks, 128, 0, st>>>(src, stride, sp, mask, dst, D + o_tails);
+                       });
+        }
+        delta_verdict_kernel<<<1, 32, 0, st>>>(D, D + o_tails, (const uint32_t*)(D + o_ok), D + o_ok + 4);
+        g_launch_count += 1;
+        CUDA_CHECK(cudaGetLastError());
+        CUDA_CHECK(cudaMemcpyAsync(verdict_out, D + o_ok + 4, 1, cudaMemcpyDeviceToHost, st));
+        CUDA_CHECK(cudaStreamSynchronize(st));
+    } catch (...) {
+        cudaStreamSynchronize(st);                         // nothing may still use the buffer when it is freed
+        throw;
+    }
+}
+
 int setup_generators_check(const void* g1, const void* g2, cudaStream_t st) {
     if (!g1 && !g2) return 0;
     uint32_t* d_bad = nullptr;
@@ -1268,6 +1422,11 @@ int setup_generators_check(const void* g1, const void* g2, cudaStream_t st) {
 }  // namespace b2g
 
 extern "C" {
+
+int b2g_delta_update_check(b2g_ctx* ctx, const b2g_delta_key* before, const b2g_delta_key* after, const void* weights,
+                           uint8_t* verdict_out) {
+    return guarded([&] { delta_check_run(ctx, before, after, weights, verdict_out); });
+}
 
 int b2g_vk_load(b2g_ctx* ctx, const b2g_vk_desc* d, b2g_vk** out) {
     return guarded([&] { vk_load_many(ctx, 1, d, out, true); });

@@ -23,4 +23,9 @@ void pairing_test_op(cudaStream_t st, int op, const void* a, const void* b, size
 // a G2 point outside G2.  Synchronises the stream.
 int setup_generators_check(const void* g1, const void* g2, cudaStream_t st);
 
+// The lowest i < n whose point in the device buffer pts (n affine Montgomery G1 or G2 points, zeros = infinity) has a coordinate
+// >= p or lies off its curve (*why = 1), or, with `subgroup`, is a G2 point outside G2 (*why = 2); n when every point passes.
+// Synchronises the stream.
+uint64_t points_check(bool g2, const void* pts, size_t n, bool subgroup, cudaStream_t st, int* why);
+
 }  // namespace b2g

@@ -31,6 +31,10 @@
     Groth16.generate_parameters_with_qap(circuit, alpha, beta, gamma, delta, g1, g2, tau=tau)
         <- Groth16::generate_parameters_with_qap (ark-groth16 0.5): the whole setup on the device (b2g_setup);
            generate_random_parameters_with_reduction(circuit, rng) draws the toxic waste and calls it.
+    Groth16.generate_parameters_from_powers_of_tau(circuit, powers)
+        <- snarkjs groth16 setup: a key from a powers-of-tau ceremony (ptau.read_ptau), gamma = delta = 1.
+    Groth16.contribute(pk) / Groth16.verify_contribution(before, after)
+        <- snarkjs zkey contribute / the delta checks of snarkjs zkey verify.
 Arguments keep the reference's meaning; field elements are (n, 4) uint64 Montgomery limb arrays (fr_to_mont).
 """
 from __future__ import annotations
@@ -275,6 +279,16 @@ class Context:
         if n == 0 or (1 << log_n) != n:
             raise ValueError("ntt length must be a power of two")
         N.check(N.lib().b2g_ntt(self._h, _ptr(d), log_n, int(inverse)))
+        return d
+
+    def points_intt(self, points_mont, g2=False) -> np.ndarray:
+        """b2g_points_intt: the inverse transform (scaled by n^-1) of 2^k affine Montgomery points, rows of 8 / 16 words"""
+        d = _c(points_mont).reshape(-1, 16 if g2 else 8).copy()
+        n = d.shape[0]
+        log_n = n.bit_length() - 1
+        if n == 0 or (1 << log_n) != n:
+            raise ValueError("points_intt length must be a power of two")
+        N.check(N.lib().b2g_points_intt(self._h, int(bool(g2)), log_n, _ptr(d)))
         return d
 
     def fixed_base_g1(self, scalars_canon) -> np.ndarray:
@@ -561,6 +575,21 @@ def _mont_points(points, g2: bool) -> np.ndarray:
     return np.frombuffer(b''.join(v.to_bytes(32, 'little') for v in vals), dtype='<u8').copy()
 
 
+def _delta_desc(arrs) -> 'N.DeltaKey':
+    d = N.DeltaKey()
+    d.n_l, d.n_h = arrs['l_query'].size // 8, arrs['h_query'].size // 8
+    for name, a in arrs.items():
+        setattr(d, name, a.ctypes.data if a.size else None)
+    return d
+
+
+def _delta_key(pk: ProvingKey):
+    """(b2g_delta_key of the key's delta, L and H fields, the arrays it points into)"""
+    keep = {name: _c(getattr(pk, name)).reshape(-1, 16 if name == 'delta_g2' else 8)
+            for name in ('delta_g1', 'delta_g2', 'l_query', 'h_query')}
+    return _delta_desc(keep), keep
+
+
 class CircomReduction:
     """R1CSToQAP implementation selected by Groth16<Bn254, CircomReduction> (src/circom/qap.rs:12-14)."""
     ID = N.REDUCTION_CIRCOM
@@ -708,6 +737,99 @@ class Groth16:
         return ProvingKey(n_vars, ni - 1, nh, arrs['alpha_g1'], arrs['beta_g1'], arrs['beta_g2'], arrs['gamma_g2'], arrs['delta_g1'],
                           arrs['delta_g2'], arrs['gamma_abc_g1'], arrs['a_query'], arrs['b_g1_query'], arrs['b_g2_query'],
                           arrs['l_query'], arrs['h_query'])
+
+    @staticmethod
+    def generate_parameters_from_powers_of_tau(circuit, powers, ctx: Context = None, reduction=CircomReduction) -> ProvingKey:
+        """`snarkjs groth16 setup circuit.r1cs pot.ptau` on the GPU (b2g_setup_from_powers): the proving key of `circuit` (as
+        generate_parameters_with_qap takes it) from a powers-of-tau ceremony (ptau.read_ptau, or any object with the same
+        fields), with gamma = delta = 1.  Only the prefix of each array the circuit's domain needs is read."""
+        ctx = ctx or default_context()
+        m, n_vars = (circuit.matrices(with_c=True), circuit.n_vars) if hasattr(circuit, 'matrices') else (circuit, circuit.n_vars)
+        d, keep = _mat_desc(m, n_vars, reduction.ID, with_c=True)
+        ni = m.num_instance_variables
+        if ni == 0 or ni > n_vars:
+            raise N.B2gError(N.B2G_E_SHAPE, "num_inputs out of range")
+        size = 1
+        while size < m.num_constraints + ni:
+            size <<= 1
+        nh = size - 1 if reduction.ID == N.REDUCTION_LIBSNARK else size
+        from .ptau import Powers
+        log_n = size.bit_length() - 1
+        pd = N.PowersDesc()
+        pd.log_size = int(powers.power)
+        arrays = {}
+        if log_n <= pd.log_size:                  # else the library refuses the domain before it reads any point
+            # checks that each array holds what the domain reads (ValueError otherwise), as views where they can be
+            pre = Powers(int(powers.power), int(getattr(powers, 'ceremony_power', powers.power)),
+                         *(np.asarray(getattr(powers, k)) for k in ('tau_g1', 'tau_g2', 'alpha_tau_g1', 'beta_tau_g1', 'beta_g2')))
+            pre = pre.prefix(log_n)
+            for name in ('tau_g1', 'tau_g2', 'alpha_tau_g1', 'beta_tau_g1', 'beta_g2'):
+                a = _c(getattr(pre, name))
+                arrays[name] = a
+                setattr(pd, name, a.ctypes.data)
+        shapes = {'alpha_g1': (1, 8), 'beta_g1': (1, 8), 'delta_g1': (1, 8), 'beta_g2': (1, 16), 'gamma_g2': (1, 16), 'delta_g2': (1, 16),
+                  'gamma_abc_g1': (ni, 8), 'a_query': (n_vars, 8), 'b_g1_query': (n_vars, 8), 'b_g2_query': (n_vars, 16),
+                  'l_query': (n_vars - ni, 8), 'h_query': (nh, 8)}
+        arrs = {k: np.zeros(v, dtype=np.uint64) for k, v in shapes.items()}
+        out = N.SetupOut()
+        for k, a in arrs.items():
+            setattr(out, k, a.ctypes.data if a.size else None)
+        N.check(N.lib().b2g_setup_from_powers(ctx._h, C.byref(d), C.byref(pd), C.byref(out)))
+        return ProvingKey(n_vars, ni - 1, nh, arrs['alpha_g1'], arrs['beta_g1'], arrs['beta_g2'], arrs['gamma_g2'], arrs['delta_g1'],
+                          arrs['delta_g2'], arrs['gamma_abc_g1'], arrs['a_query'], arrs['b_g1_query'], arrs['b_g2_query'],
+                          arrs['l_query'], arrs['h_query'])
+
+    @staticmethod
+    def contribute(pk: ProvingKey, rng=None, ctx: Context = None, x=None) -> ProvingKey:
+        """`snarkjs zkey contribute` on the GPU (b2g_delta_update): a new key with delta multiplied by a secret x and the L and
+        H queries divided by it.  x is drawn in [1, r) with `secrets` (or rng.randrange when an rng is given) unless given;
+        it is not returned, and the library's copies of it are wiped."""
+        import secrets
+        ctx = ctx or default_context()
+        if x is None:
+            x = rng.randrange(1, R_MOD) if rng is not None else 1 + secrets.randbelow(R_MOD - 1)
+        x = int(x)
+        if not 0 <= x < 1 << 256:
+            raise N.B2gError(N.B2G_E_INPUT, "x is not below r")
+        xb = np.frombuffer(x.to_bytes(32, 'little'), dtype=np.uint8).copy()
+        before, keep = _delta_key(pk)
+        after_arrs = {'delta_g1': np.zeros((1, 8), dtype=np.uint64), 'delta_g2': np.zeros((1, 16), dtype=np.uint64),
+                      'l_query': np.zeros_like(keep['l_query']), 'h_query': np.zeros_like(keep['h_query'])}
+        after = _delta_desc(after_arrs)
+        try:
+            N.check(N.lib().b2g_delta_update(ctx._h, C.byref(before), _ptr(xb), C.byref(after)))
+        finally:
+            xb[:] = 0
+        return ProvingKey(pk.n_vars, pk.n_public, pk.domain_size, np.array(pk.alpha_g1, copy=True), np.array(pk.beta_g1, copy=True),
+                          np.array(pk.beta_g2, copy=True), np.array(pk.gamma_g2, copy=True), after_arrs['delta_g1'], after_arrs['delta_g2'],
+                          np.array(pk.gamma_abc_g1, copy=True), np.array(pk.a_query, copy=True), np.array(pk.b_g1_query, copy=True),
+                          np.array(pk.b_g2_query, copy=True), after_arrs['l_query'], after_arrs['h_query'])
+
+    @staticmethod
+    def verify_contribution(before: ProvingKey, after: ProvingKey, ctx: Context = None, weights=None) -> bool:
+        """The delta checks of `snarkjs zkey verify` (b2g_delta_update_check): whether `after` is `before` with one or more
+        delta contributions.  The fields a contribution leaves alone are compared on the host; the weights (one per L point,
+        then one per H point, in [1, 2^128)) are drawn with `secrets` unless given.  A False verdict is wrong with probability
+        at most 1 / (2^128 - 1) per equation when the weights are drawn after both keys are fixed."""
+        ctx = ctx or default_context()
+        for name in ('n_vars', 'n_public', 'domain_size'):
+            if getattr(before, name) != getattr(after, name):
+                return False
+        for name in ('alpha_g1', 'beta_g1', 'beta_g2', 'gamma_g2', 'gamma_abc_g1', 'a_query', 'b_g1_query', 'b_g2_query'):
+            a, b = _c(getattr(before, name)), _c(getattr(after, name))
+            if a.shape != b.shape or a.tobytes() != b.tobytes():
+                return False
+        d0, k0 = _delta_key(before)
+        d1, k1 = _delta_key(after)
+        if (d0.n_l, d0.n_h) != (d1.n_l, d1.n_h):
+            return False
+        count = d0.n_l + d0.n_h
+        if weights is not None:
+            weights = _check_weights("verify_contribution", weights, count)
+        wb = _weight_bytes(weights, count)
+        out = np.zeros(1, dtype=np.uint8)
+        N.check(N.lib().b2g_delta_update_check(ctx._h, C.byref(d0), C.byref(d1), _ptr(wb), _ptr(out)))
+        return bool(out[0])
 
     # ---- verification (host pairing; circom_compat_b200/verifier.py).  Call sites in the reference: src/zkey.rs:868-870,
     # 914-916 (process_vk + verify_with_processed_vk), tests/groth16.rs:33-35 (SNARK::verify).

@@ -25,6 +25,8 @@
 //   ark_circom::serialize_proving_key / deserialize_proving_key / serialize_verifying_key / deserialize_verifying_key(s)
 //                                             <- CanonicalSerialize / CanonicalDeserialize (ark-serialize 0.5, Validate::Yes)
 //                                                of ProvingKey<Bn254> / VerifyingKey<Bn254>, points decoded on the device
+//   ark_circom::read_ptau + Groth16::generate_parameters_from_powers_of_tau <- snarkjs groth16 setup (a key from a ceremony)
+//   ark_circom::Groth16::contribute / verify_contribution <- snarkjs zkey contribute / the delta checks of snarkjs zkey verify
 //   ark_circom::read_wtns                              <- snarkjs .wtns (test-vectors/circuit2_js/witness.wtns; the reference
 //                                                         computes witnesses with WASM instead, out of scope here)
 // Parsing and key handling stay on the host; every field/curve operation of the proof runs in libb2groth.so.
@@ -40,6 +42,7 @@
 #include <optional>
 #include <random>
 #include <sstream>
+#include <type_traits>
 #include <stdexcept>
 #include <string>
 #include <tuple>
@@ -301,6 +304,76 @@ inline std::vector<Fr> read_wtns(std::istream& r) {
         r.seekg(pos + (std::streamoff)len);
     }
     return out;
+}
+
+// ---------------------------------------------------------------------------------------------- .ptau reader (host)
+// The points of a powers-of-tau ceremony of size 2^power (snarkjs .ptau sections 2-6; layout restated in ptau.py), affine
+// Montgomery as in a zkey.  The vectors may hold only a prefix of the ceremony: see read_ptau.
+struct Powers {
+    uint32_t power = 0, ceremony_power = 0;
+    std::vector<G1Affine> tau_g1, alpha_tau_g1, beta_tau_g1;    // 2^(power+1) - 1, 2^power, 2^power points in the file
+    std::vector<G2Affine> tau_g2;                               // 2^power
+    G2Affine beta_g2;
+};
+
+// Parses a .ptau container with the checks of ptau.read_ptau (magic, version 1, BN254's field, sections 1-6 present, not
+// truncated, sizes that agree with the power), throwing SerializationError.  log_n > 0: read only the prefix a circuit
+// of domain 2^log_n needs (2n - 1 / n / n / n points), so a large ceremony file is not read whole; it must not exceed the
+// file's power.  log_n = 0: every point.
+inline Powers read_ptau(std::istream& r, uint32_t log_n = 0) {
+    r.seekg(0, std::ios::end);
+    const uint64_t size = (uint64_t)r.tellg();
+    r.seekg(0);
+    char magic[4];
+    if (size < 12) throw SerializationError("ptau: bad magic (not a .ptau file)");
+    detail::read_exact(r, magic, 4);
+    if (memcmp(magic, "ptau", 4)) throw SerializationError("ptau: bad magic (not a .ptau file)");
+    const uint32_t version = detail::read_le<uint32_t>(r), nsec = detail::read_le<uint32_t>(r);
+    if (version != 1) throw SerializationError("ptau: unsupported version " + std::to_string(version) + " (expected 1)");
+    std::map<uint32_t, detail::Section> secs;
+    uint64_t at = 12;
+    for (uint32_t k = 0; k < nsec; k++) {
+        if (at + 12 > size) throw SerializationError("ptau: section header " + std::to_string(k) + " is truncated");
+        r.seekg((std::streamoff)at);
+        const uint32_t id = detail::read_le<uint32_t>(r);
+        const uint64_t len = detail::read_le<uint64_t>(r);
+        at += 12;
+        if (len > size - at) throw SerializationError("ptau: section " + std::to_string(id) + " is truncated");
+        secs.insert({id, {at, len}});
+        at += len;
+    }
+    for (uint32_t id = 1; id <= 6; id++)
+        if (!secs.count(id)) throw SerializationError("ptau: section " + std::to_string(id) + " is missing");
+    r.seekg((std::streamoff)secs[1].position);
+    const uint32_t n8 = detail::read_le<uint32_t>(r);
+    if (n8 != 32) throw SerializationError("ptau: field element size " + std::to_string(n8) + " is not BN254's (32)");
+    if (secs[1].size != 44) throw SerializationError("ptau: section 1 holds " + std::to_string(secs[1].size) + " bytes, not 44");
+    uint64_t q[4]; detail::read_exact(r, q, 32);
+    if (memcmp(q, detail::FQ_P, 32)) throw SerializationError("ptau: the curve's base field is not BN254's");
+    Powers p;
+    p.power = detail::read_le<uint32_t>(r);
+    p.ceremony_power = detail::read_le<uint32_t>(r);
+    if (p.power < 1 || p.power > 28) throw SerializationError("ptau: power " + std::to_string(p.power) + " is out of range (1..28)");
+    if (log_n > p.power) throw SerializationError("ptau: the circuit's domain 2^" + std::to_string(log_n) + " exceeds the ceremony's 2^" + std::to_string(p.power));
+    const uint64_t n = 1ull << p.power, m = log_n ? 1ull << log_n : n;
+    const uint64_t counts[5] = {2 * n - 1, n, n, n, 1}, reads[5] = {2 * m - 1, m, m, m, 1}, rows[5] = {64, 128, 64, 64, 128};
+    for (int k = 0; k < 5; k++) {
+        const detail::Section s = secs[2 + k];
+        if (s.size != counts[k] * rows[k])
+            throw SerializationError("ptau: section " + std::to_string(2 + k) + " holds " + std::to_string(s.size) + " bytes, but power " +
+                                     std::to_string(p.power) + " needs " + std::to_string(counts[k] * rows[k]));
+        r.seekg((std::streamoff)s.position);
+        void* dst;
+        switch (k) {
+            case 0: p.tau_g1.resize(reads[k]); dst = p.tau_g1.data(); break;
+            case 1: p.tau_g2.resize(reads[k]); dst = p.tau_g2.data(); break;
+            case 2: p.alpha_tau_g1.resize(reads[k]); dst = p.alpha_tau_g1.data(); break;
+            case 3: p.beta_tau_g1.resize(reads[k]); dst = p.beta_tau_g1.data(); break;
+            default: dst = &p.beta_g2; break;
+        }
+        detail::read_exact(r, dst, reads[k] * rows[k]);
+    }
+    return p;
 }
 
 // ---------------------------------------------------------------------------------------------- device side
@@ -590,6 +663,16 @@ inline std::vector<bool> batch_verdicts(const std::vector<std::vector<bool>>& li
     return out;
 }
 
+// the b2g_delta_key of a key's delta, L and H fields (the ABI reads `before` only; the pointers are not const there)
+inline b2g_delta_key delta_key(const ProvingKey& pk) {
+    b2g_delta_key d;
+    d.n_l = (uint32_t)pk.l_query.size(); d.n_h = (uint32_t)pk.h_query.size();
+    d.delta_g1 = const_cast<G1Affine*>(&pk.delta_g1); d.delta_g2 = const_cast<G2Affine*>(&pk.vk.delta_g2);
+    d.l_query = pk.l_query.empty() ? nullptr : const_cast<G1Affine*>(pk.l_query.data());
+    d.h_query = pk.h_query.empty() ? nullptr : const_cast<G1Affine*>(pk.h_query.data());
+    return d;
+}
+
 template <class QAP = CircomReduction>
 struct Groth16T {                                       // Groth16::<Bn254, QAP>
     // verification (host pairing, ark_circom_verifier.hpp): src/zkey.rs:868-870, 914-916; tests/groth16.rs:33-35
@@ -821,6 +904,82 @@ struct Groth16T {                                       // Groth16::<Bn254, QAP>
         check(rc);
         return pk;
     }
+    // `snarkjs groth16 setup circuit.r1cs pot.ptau` (b2g_setup_from_powers): the key of the matrices (with C) from a ceremony,
+    // gamma = delta = 1.  Throws std::invalid_argument when the powers hold fewer points than the circuit's domain reads.
+    static ProvingKey generate_parameters_from_powers_of_tau(const ConstraintMatrices& matrices, const Powers& powers,
+                                                             Gpu& gpu = Gpu::instance()) {
+        const size_t ni = matrices.num_instance_variables, nv = ni + matrices.num_witness_variables;
+        if (ni == 0) throw SynthesisError("generate_parameters_from_powers_of_tau: no instance variable");
+        if (matrices.num_constraints && matrices.c.empty())
+            throw SynthesisError("generate_parameters_from_powers_of_tau needs the C matrix (R1CS route); zkey matrices have none");
+        size_t n = 1;
+        while (n < matrices.num_constraints + ni) n <<= 1;
+        if (n <= (1ull << powers.power) &&
+            (powers.tau_g1.size() < 2 * n - 1 || powers.tau_g2.size() < n || powers.alpha_tau_g1.size() < n || powers.beta_tau_g1.size() < n))
+            throw std::invalid_argument("generate_parameters_from_powers_of_tau: the powers hold fewer points than the domain of " +
+                                        std::to_string(n) + " reads");
+        ProvingKey pk;
+        pk.vk.gamma_abc_g1.resize(ni); pk.a_query.resize(nv); pk.b_g1_query.resize(nv); pk.b_g2_query.resize(nv);
+        pk.l_query.resize(nv - ni); pk.h_query.resize(QAP::ID == B2G_REDUCTION_LIBSNARK ? n - 1 : n);
+        b2g_powers_desc pd;
+        memset(&pd, 0, sizeof pd);
+        pd.log_size = powers.power;
+        pd.tau_g1 = powers.tau_g1.data(); pd.tau_g2 = powers.tau_g2.data(); pd.alpha_tau_g1 = powers.alpha_tau_g1.data();
+        pd.beta_tau_g1 = powers.beta_tau_g1.data(); pd.beta_g2 = &powers.beta_g2;
+        b2g_setup_out out = {&pk.vk.alpha_g1, &pk.beta_g1, &pk.delta_g1, &pk.vk.beta_g2, &pk.vk.gamma_g2, &pk.vk.delta_g2,
+                             pk.vk.gamma_abc_g1.data(), pk.a_query.data(), pk.b_g1_query.data(), pk.b_g2_query.data(),
+                             pk.l_query.data(), pk.h_query.data()};
+        const Gpu::MatDesc md(matrices, nv, QAP::ID, true);
+        check(b2g_setup_from_powers(gpu.ctx(), &md.d, &pd, &out));
+        return pk;
+    }
+
+    // `snarkjs zkey contribute` (b2g_delta_update): pk with delta multiplied by x (nonzero, below r) and the L and H queries
+    // divided by it; the library's copies of x are wiped
+    static ProvingKey contribute(const ProvingKey& pk, const Fr& x, Gpu& gpu = Gpu::instance()) {
+        ProvingKey out;
+        out.vk = pk.vk; out.beta_g1 = pk.beta_g1; out.a_query = pk.a_query; out.b_g1_query = pk.b_g1_query;
+        out.b_g2_query = pk.b_g2_query;
+        out.l_query.resize(pk.l_query.size()); out.h_query.resize(pk.h_query.size());
+        b2g_delta_key before = delta_key(pk), after = delta_key(out);
+        BigInt256 xb = x.into_bigint();
+        const int rc = b2g_delta_update(gpu.ctx(), &before, xb.l, &after);
+        volatile uint64_t* wipe = xb.l;
+        for (int i = 0; i < 4; i++) wipe[i] = 0;
+        check(rc);
+        return out;
+    }
+    // the same with x = Fr::rand(rng), drawn again while zero (an Fr argument selects the call above)
+    template <class Rng, class = typename std::enable_if<!std::is_same<Rng, Fr>::value>::type>
+    static ProvingKey contribute(const ProvingKey& pk, Rng& rng, Gpu& gpu = Gpu::instance()) {
+        Fr x;
+        while (x.is_zero()) x = Fr::rand(rng);
+        const ProvingKey out = contribute(pk, x, gpu);
+        volatile uint64_t* wipe = x.l;
+        for (int i = 0; i < 4; i++) wipe[i] = 0;
+        return out;
+    }
+
+    // the delta checks of `snarkjs zkey verify` (b2g_delta_update_check, weights from std::random_device): whether `after`
+    // is `before` with one or more contributions.  The fields a contribution leaves alone are compared on the host.
+    static bool verify_contribution(const ProvingKey& before, const ProvingKey& after, Gpu& gpu = Gpu::instance()) {
+        auto same = [](const void* a, const void* b, size_t bytes) { return !memcmp(a, b, bytes); };
+        auto same_vec = [&](const auto& a, const auto& b) {
+            return a.size() == b.size() && (a.empty() || same(a.data(), b.data(), a.size() * sizeof(a[0])));
+        };
+        if (!same(&before.vk.alpha_g1, &after.vk.alpha_g1, 64) || !same(&before.beta_g1, &after.beta_g1, 64) ||
+            !same(&before.vk.beta_g2, &after.vk.beta_g2, 128) || !same(&before.vk.gamma_g2, &after.vk.gamma_g2, 128) ||
+            !same_vec(before.vk.gamma_abc_g1, after.vk.gamma_abc_g1) || !same_vec(before.a_query, after.a_query) ||
+            !same_vec(before.b_g1_query, after.b_g1_query) || !same_vec(before.b_g2_query, after.b_g2_query) ||
+            before.l_query.size() != after.l_query.size() || before.h_query.size() != after.h_query.size())
+            return false;
+        b2g_delta_key b = delta_key(before), a = delta_key(after);
+        const std::vector<uint32_t> w = batch_weights(before.l_query.size() + before.h_query.size());
+        uint8_t verdict = 0;
+        check(b2g_delta_update_check(gpu.ctx(), &b, &a, w.data(), &verdict));
+        return verdict != 0;
+    }
+
     // Groth16::generate_random_parameters_with_reduction(circuit, rng): alpha, beta, gamma, delta, tau drawn with Fr::rand in that
     // order, on the standard generators
     template <class Rng>

@@ -35,6 +35,12 @@
 //       tests/groth16.rs:75-105 in C++: draw the toxic waste with std::mt19937_64(seed), make the key with
 //       Groth16T<LibsnarkReduction>::generate_random_parameters_with_reduction (b2g_setup), print the five secrets, the key
 //       (serialize_proving_key, compressed, hex), the proof of the witness under the same rng and the host verifier's verdict
+//   B2G_SETUP_PTAU=<file.ptau> groth16_bench <circuit.r1cs> <witness.wtns> [seed]
+//       the same flow with a powers-of-tau ceremony in place of the toxic waste (CircomReduction, as snarkjs): read the prefix
+//       of the ceremony the circuit needs (read_ptau), make the key (generate_parameters_from_powers_of_tau), apply one
+//       contribution with x = Fr::rand(std::mt19937_64(seed)) (default seed 0x5E7), check it (verify_contribution), prove the
+//       witness under the same rng and verify on the host; print x, the contributed key (serialize_proving_key, compressed,
+//       hex), the check's verdict, the proof and the host verifier's verdict
 //       chain:<a> = the witness of the reference's squaring-chain bench family for input a
 //       (test-vectors/complex-circuit/input.json has a = 3), computed on the host instead of by WASM.
 #include <algorithm>
@@ -164,6 +170,38 @@ int main(int argc, char** argv) {
             for (uint8_t b : serialize_compressed(proof)) std::printf("%02x", b);
             std::printf("\n");
             std::printf("verified=%d\n", Groth16::verify_with_processed_vk(Groth16::process_vk(vk2), in2, p2) ? 1 : 0);
+            return 0;
+        }
+        if (const char* ptau = std::getenv("B2G_SETUP_PTAU")) {             // R1CS + ceremony -> key -> contribution -> check -> prove -> verify
+            if (argc < 3) { std::fprintf(stderr, "usage: B2G_SETUP_PTAU=<file.ptau> %s <circuit.r1cs> <witness.wtns> [seed]\n", argv[0]); return 2; }
+            typedef Groth16T<CircomReduction> G;
+            std::ifstream rf(argv[1], std::ios::binary);
+            if (!rf) throw SerializationError("cannot open r1cs");
+            const ConstraintMatrices matrices = R1CS::read(rf).to_matrices();
+            std::ifstream wf(argv[2], std::ios::binary);
+            if (!wf) throw SerializationError("cannot open wtns");
+            const std::vector<Fr> w = read_wtns(wf);
+            uint32_t log_n = 0;
+            while ((1ull << log_n) < matrices.num_constraints + matrices.num_instance_variables) log_n++;
+            std::ifstream pf(ptau, std::ios::binary);
+            if (!pf) throw SerializationError("cannot open ptau");
+            const Powers powers = read_ptau(pf, log_n ? log_n : 1);
+            const ProvingKey pk0 = G::generate_parameters_from_powers_of_tau(matrices, powers);
+            std::mt19937_64 rng(std::stoull(argc > 3 ? argv[3] : "0x5E7", nullptr, 0));
+            std::mt19937_64 replay = rng;                                    // the same draw, to print x
+            Fr x;
+            while (x.is_zero()) x = Fr::rand(replay);
+            const BigInt256 xb = x.into_bigint();
+            std::printf("x=0x%016llx%016llx%016llx%016llx\n", (unsigned long long)xb.l[3], (unsigned long long)xb.l[2],
+                        (unsigned long long)xb.l[1], (unsigned long long)xb.l[0]);
+            const ProvingKey pk = G::contribute(pk0, rng);
+            std::printf("key=");
+            for (uint8_t b : serialize_proving_key(pk)) std::printf("%02x", b);
+            std::printf("\ncontribution=%d\n", G::verify_contribution(pk0, pk) ? 1 : 0);
+            const Proof proof = G::prove(pk, matrices, w, rng);
+            std::printf("proof=%s\n", proof.hex().c_str());
+            const std::vector<Fr> inputs(w.begin() + 1, w.begin() + matrices.num_instance_variables);
+            std::printf("verified=%d\n", G::verify_with_processed_vk(G::process_vk(pk.vk), inputs, proof) ? 1 : 0);
             return 0;
         }
         if (const char* seed = std::getenv("B2G_SETUP")) {                  // R1CS -> setup on the GPU -> prove -> verify

@@ -31,6 +31,8 @@
  *                             Validate::Yes) of the G1 / G2 points of a ProvingKey<Bn254> or VerifyingKey<Bn254>
  *   b2g_setup              <- Groth16::generate_parameters_with_qap (ark-groth16 0.5), which
  *                             generate_random_parameters_with_reduction calls (tests/groth16.rs:25): a whole proving key
+ *   b2g_setup_from_powers  <- snarkjs groth16 setup (zkey new): a proving key from a powers-of-tau ceremony
+ *   b2g_delta_update / b2g_delta_update_check <- snarkjs zkey contribute / the delta checks of snarkjs zkey verify
  *   b2g_fixed_base_g1/g2  <- the batch fixed-base multiplications of that setup, for the standard generators only
  *
  * Conventions
@@ -465,12 +467,95 @@ typedef struct {
  * a generator at infinity or off its curve, or a g2 outside G2; B2G_E_DEVICE when the buffers do not fit in device memory. */
 B2G_API int b2g_setup(b2g_ctx* ctx, const b2g_mat_desc* circuit, const b2g_setup_secrets* secrets, b2g_setup_out* out);
 
+/* The points of a powers-of-tau ceremony of size 2^log_size (phase 1 of a snarkjs setup, sections 2-6 of a .ptau file), HOST
+ * arrays in the b2g_pk_desc layout (affine Montgomery, all-zero = infinity):
+ *   tau_g1 = tau^i g1 (i < 2^(p+1) - 1), tau_g2 = tau^i g2, alpha_tau_g1 = alpha tau^i g1, beta_tau_g1 = beta tau^i g1
+ *   (i < 2^p), beta_g2 = beta g2. */
+typedef struct {
+    uint32_t log_size;           /* p, at most 28 */
+    uint32_t reserved;
+    const void* tau_g1;
+    const void* tau_g2;
+    const void* alpha_tau_g1;
+    const void* beta_tau_g1;
+    const void* beta_g2;
+} b2g_powers_desc;
+
+/* b2g_setup_from_powers <- `snarkjs groth16 setup circuit.r1cs pot.ptau` (snarkjs zkey new): a proving key from a ceremony
+ * whose tau, alpha and beta nobody knows, with gamma = delta = 1 as snarkjs sets them.  The circuit and `out` are those of
+ * b2g_setup.  With n the least power of two >= m + num_inputs, the call needs n <= 2^log_size and reads only the first
+ * 2n - 1 / n / n / n points of tau_g1 / tau_g2 / alpha_tau_g1 / beta_tau_g1, so any ceremony at least as large serves.  With
+ * [L_r] = iNTT_n(tau_g1[0..n))_r (the inverse radix-2 transform over points, natural order, scaled by n^-1), and [L_r]_2,
+ * [alpha L_r], [beta L_r] likewise from tau_g2, alpha_tau_g1, beta_tau_g1:
+ *     a_query[j] = sum_r A[r][j] [L_r] (+ [L_(m+j)] for j < num_inputs), b_g1_query[j] / b_g2_query[j] the same over B with
+ *     [L_r] / [L_r]_2, gamma_abc_g1[j] (j < num_inputs) and l_query[j - num_inputs] (the others) =
+ *     sum_r (A[r][j] [beta L_r] + B[r][j] [alpha L_r] + C[r][j] [L_r]) (+ [beta L_(m+j)] for j < num_inputs),
+ *     alpha_g1 = alpha_tau_g1[0], beta_g1 = beta_tau_g1[0], delta_g1 = tau_g1[0], beta_g2 = beta_g2,
+ *     gamma_g2 = delta_g2 = tau_g2[0],
+ *     h_query (LibsnarkReduction) = tau_g1[i + n] - tau_g1[i], i < n - 1,
+ *     h_query (CircomReduction)   = the odd entries of the inverse transform over 2n points of (tau_g1[0..2n-1), infinity),
+ *                                   computed as 1/2 iNTT_n(y), y_i = omega_2n^-i (tau_g1[i] - tau_g1[i + n]).
+ * The key equals, byte for byte, b2g_setup(circuit, alpha, beta, gamma = 1, delta = 1, tau) on the generators g1 = tau_g1[0]
+ * and g2 = tau_g2[0].  The call checks only what it reads: every point read lies on its curve with coordinates below p, the
+ * G2 points are in G2, and tau_g1[0], tau_g2[0] are not at infinity.  Whether the arrays really are powers of one tau with
+ * the same alpha and beta is left to the ceremony's own verification (snarkjs powersoftau verify).
+ * Cost: four inverse transforms over G1 and one over G2 of n points, each (n/2) log2 n variable-base products; one product
+ * per nonzero (a coefficient k above r/2 multiplies the negated point by r - k, so +-1 and small constants are cheap).
+ * Synchronous.  Errors (every error leaves the context usable): the matrix checks and messages of b2g_setup (B2G_E_SHAPE);
+ * B2G_E_DOMAIN for n > 2^log_size or at b2g_setup's domain limits; B2G_E_INPUT for a point off its curve or with a coordinate
+ * >= p, a G2 point outside G2, or tau_g1[0] / tau_g2[0] at infinity, naming the array and index ("tau_g2[17]: not in G2");
+ * B2G_E_SHAPE for null pointers or a pending proof; B2G_E_DEVICE when the buffers do not fit in device memory. */
+B2G_API int b2g_setup_from_powers(b2g_ctx* ctx, const b2g_mat_desc* circuit, const b2g_powers_desc* powers, b2g_setup_out* out);
+
+/* The part of a proving key a delta contribution changes, HOST buffers in the b2g_pk_desc layout. */
+typedef struct {
+    uint32_t n_l, n_h;           /* points of l_query and h_query */
+    void* delta_g1;              /* 64 B */
+    void* delta_g2;              /* 128 B */
+    void* l_query;               /* n_l G1 (may be NULL when n_l == 0) */
+    void* h_query;               /* n_h G1 (may be NULL when n_h == 0) */
+} b2g_delta_key;
+
+/* b2g_delta_update <- `snarkjs zkey contribute` (phase 2): one contribution with the secret x (32 B canonical, in [1, r)):
+ *     after.delta_g1 = x before.delta_g1, after.delta_g2 = x before.delta_g2,
+ *     after.l_query[i] = x^-1 before.l_query[i], after.h_query[i] = x^-1 before.h_query[i];
+ * the other fields of the key are unchanged (the caller copies them).  A key from b2g_setup_from_powers given contributions
+ * x_1, ..., x_k equals b2g_setup(..., gamma = 1, delta = x_1 ... x_k, tau) byte for byte.  x and x^-1 are handled as
+ * b2g_setup handles its secrets: the library's host copy of x is wiped once it has reached the device, and every device
+ * buffer that held x or x^-1 is zeroed before it is freed.  snarkjs's transcript (the proof of knowledge of x, the hashes of
+ * zkey section 10) is not produced.
+ * Synchronous.  Errors (every error leaves the context usable): B2G_E_SHAPE for null pointers, counts that differ between
+ * before and after, or a pending proof; B2G_E_INPUT for x = 0 or x >= r, a point of `before` off its curve or with a
+ * coordinate >= p, or before.delta_g2 outside G2 (naming the field and index); B2G_E_DEVICE when the buffers do not fit. */
+B2G_API int b2g_delta_update(b2g_ctx* ctx, const b2g_delta_key* before, const void* x_canon, b2g_delta_key* after);
+
+/* b2g_delta_update_check <- `snarkjs zkey verify`'s check of the delta contributions: whether `after` is `before` with one or
+ * more contributions applied.  weights = (n_l + n_h) x 16 B nonzero 128-bit little-endian weights (rho_i for l_query, then
+ * sigma_i for h_query).  *verdict_out = 1 iff
+ *   the counts match; every point of `after` has coordinates below p and lies on its curve; after.delta_g1 and
+ *   after.delta_g2 are not at infinity and after.delta_g2 is in G2; before.delta_g2 is not at infinity;
+ *   e(delta_1', delta_2) = e(delta_1, delta_2');
+ *   e(sum rho_i L'_i + sum sigma_i H'_i, delta_2') = e(sum rho_i L_i + sum sigma_i H_i, delta_2).
+ * Soundness, as for b2g_verify_batch: an honest update (any chain of b2g_delta_update calls) always gives 1.  Any other
+ * `after` gives 0, except with probability at most 1 / (2^128 - 1) per equation over uniformly drawn nonzero weights, and only
+ * if the weights are drawn AFTER both keys are fixed, from a source the contributor cannot predict or influence.  The other
+ * fields of the key are not read: the host compares them (both mirrors do).
+ * Cost: two 128-bit G1 products per point, a tree of G1 sums, and four pairings.
+ * Synchronous.  Errors (every error leaves the context usable): B2G_E_SHAPE for null pointers or a pending proof; B2G_E_INPUT
+ * for a zero weight; B2G_E_DEVICE when the buffers do not fit. */
+B2G_API int b2g_delta_update_check(b2g_ctx* ctx, const b2g_delta_key* before, const b2g_delta_key* after, const void* weights,
+                                   uint8_t* verdict_out);
+
 /* Kernel-level entry points (parity tests, benchmarks). All pointers host. */
 B2G_API int b2g_msm_g1(b2g_ctx* ctx, const void* bases, const void* scalars, size_t n, int scalars_mont, void* out_xy_mont);
 B2G_API int b2g_msm_g2(b2g_ctx* ctx, const void* bases, const void* scalars, size_t n, int scalars_mont, void* out_xy_mont);
 B2G_API int b2g_ntt(b2g_ctx* ctx, void* data_mont, int log_n, int inverse);
 B2G_API int b2g_fixed_base_g1(b2g_ctx* ctx, const void* scalars_canon, size_t n, void* out_affine_mont);
 B2G_API int b2g_fixed_base_g2(b2g_ctx* ctx, const void* scalars_canon, size_t n, void* out_affine_mont);
+/* b2g_points_intt: the inverse radix-2 transform over n = 2^log_n affine points (g2 = 0: G1, 1: G2), in place, natural order,
+ * scaled by n^-1 as b2g_ntt scales it: out_k = n^-1 sum_i omega_n^(-ik) in_i (log_n in 1..27, else B2G_E_DOMAIN).  The points
+ * are not checked.  The kernel b2g_setup_from_powers runs. */
+B2G_API int b2g_points_intt(b2g_ctx* ctx, int g2, int log_n, void* points_mont);
 
 /* Element-wise device arithmetic, for unit parity tests of the field / group layers.
  * op: 0 fq_mul, 1 fq_add, 2 fq_sub, 3 fr_mul, 4 fr_add, 5 fr_sub, 6 fq_inv, 7 fr_inv (b ignored),
