@@ -58,6 +58,11 @@ class PowersDesc(C.Structure):
                [(k, C.c_void_p) for k in ('tau_g1', 'tau_g2', 'alpha_tau_g1', 'beta_tau_g1', 'beta_g2')]
 
 
+class PowersReport(C.Structure):
+    """b2g_powers_report: the verdict of b2g_powers_check (rule 0 ok, 1-5 a point rule, 6 the pairing product)"""
+    _fields_ = [('ok', C.c_uint8), ('rule', C.c_uint8), ('array', C.c_uint8), ('reserved', C.c_uint8 * 5), ('index', C.c_uint64)]
+
+
 class DeltaKey(C.Structure):
     """b2g_delta_key: the fields of a proving key a delta contribution changes (host buffers)"""
     _fields_ = [('n_l', C.c_uint32), ('n_h', C.c_uint32)] + [(k, C.c_void_p) for k in ('delta_g1', 'delta_g2', 'l_query', 'h_query')]
@@ -77,7 +82,8 @@ EXPORTS = ['b2g_last_error', 'b2g_version', 'b2g_device_count', 'b2g_ctx_create'
            'b2g_verify_batch_locate', 'b2g_verify_batch_locate_compressed', 'b2g_verify_batch_keys',
            'b2g_verify_batch_keys_compressed', 'b2g_verify_batch_keys_locate', 'b2g_verify_batch_keys_locate_compressed',
            'b2g_rerandomize_many', 'b2g_points_serialize', 'b2g_points_deserialize', 'b2g_setup',
-           'b2g_setup_from_powers', 'b2g_delta_update', 'b2g_delta_update_check', 'b2g_points_intt']
+           'b2g_setup_from_powers', 'b2g_delta_update', 'b2g_delta_update_check', 'b2g_points_intt',
+           'b2g_powers_msm', 'b2g_powers_check']
 
 _lib = None
 
@@ -124,6 +130,8 @@ def lib():
         L.b2g_delta_update.argtypes = [vp, C.POINTER(DeltaKey), vp, C.POINTER(DeltaKey)]
         L.b2g_delta_update_check.argtypes = [vp, C.POINTER(DeltaKey), C.POINTER(DeltaKey), vp, vp]
         L.b2g_points_intt.argtypes = [vp, i, i, vp]
+        L.b2g_powers_msm.argtypes = [vp, i, sz, vp, vp, vp]
+        L.b2g_powers_check.argtypes = [vp, C.POINTER(PowersDesc), C.c_uint32, vp, C.POINTER(PowersReport)]
         L.b2g_test_op.argtypes = [vp, i, vp, vp, sz, vp]
         L.b2g_last_timings.argtypes = [vp, vp]
         L.b2g_bench_device.argtypes = [vp, vp, vp, i, C.POINTER(C.c_float)]

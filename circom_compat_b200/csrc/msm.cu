@@ -638,6 +638,141 @@ void msm_run(const MsmPlan& plan, MsmScratch& s, const fe* scalars_dev, uint32_t
     msm_accumulate(plan, s, s, st);
 }
 
+// ------------------------------------------------------------------------------------------------ tableless streamed MSM
+constexpr uint32_t POWERS_CHUNK = 16;            // consecutive powers one thread of powers_scalars_kernel makes
+
+// pw[0] = rho^start, pw[1] = rho^POWERS_CHUNK (Montgomery), by square-and-multiply; one thread
+__global__ void powers_base_kernel(const fe* __restrict__ rho, uint64_t start, fe* __restrict__ pw) {
+    if (threadIdx.x != 0 || blockIdx.x != 0) return;
+    const fe r = *rho;
+    fe acc = Fr::one(), sq = r;
+    for (uint64_t e = start; e; e >>= 1) {
+        if (e & 1) acc = Fr::mul(acc, sq);
+        sq = Fr::sqr(sq);
+    }
+    pw[0] = acc;
+    fe c = r;
+    for (uint32_t k = 1; k < POWERS_CHUNK; k <<= 1) c = Fr::sqr(c);
+    pw[1] = c;
+}
+
+// canon[i] = rho^(start + i) in canonical form, i < n: thread t starts from rho^start (rho^CHUNK)^t and multiplies by rho
+__global__ void __launch_bounds__(256) powers_scalars_kernel(const fe* __restrict__ rho, const fe* __restrict__ pw, uint32_t n,
+                                                             fe* __restrict__ canon) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t i0 = t * POWERS_CHUNK;
+    if (i0 >= n) return;
+    fe x = pw[0], sq = pw[1];
+    for (uint32_t e = t; e; e >>= 1) {
+        if (e & 1) x = Fr::mul(x, sq);
+        sq = Fr::sqr(sq);
+    }
+    const fe r = *rho;
+    const uint32_t end = min(n, i0 + POWERS_CHUNK);
+    for (uint32_t i = i0; i < end; i++) {
+        fe_store(&canon[i], Fr::to_canonical(x));
+        x = Fr::mul(x, r);
+    }
+}
+
+// one thread per (window, scalar): the bucket key w * nb + |d| - 1 of every nonzero signed digit.  The scalars are powers of a
+// random rho, so the digits are spread over the buckets and one atomic per entry does not contend.
+__global__ void __launch_bounds__(256) powers_count_kernel(const fe* __restrict__ canon, uint32_t n, int c, int nwin, uint32_t nb,
+                                                           uint32_t* __restrict__ counts) {
+    const uint64_t tid = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t w = (uint32_t)(tid / n), i = (uint32_t)(tid % n);
+    if (w >= (uint32_t)nwin) return;
+    const int32_t d = msm_digit_at(canon[i].l, c, (int)w);
+    if (d) atomicAdd(&counts[w * nb + (uint32_t)(d < 0 ? -d : d) - 1u], 1u);
+}
+
+// the entries in bucket order: the base's index in the slice, bit 31 for a negative digit
+__global__ void __launch_bounds__(256) powers_scatter_kernel(const fe* __restrict__ canon, uint32_t n, int c, int nwin, uint32_t nb,
+                                                             const uint32_t* __restrict__ offsets, uint32_t* __restrict__ cursor,
+                                                             uint32_t* __restrict__ entries) {
+    const uint64_t tid = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t w = (uint32_t)(tid / n), i = (uint32_t)(tid % n);
+    if (w >= (uint32_t)nwin) return;
+    const int32_t d = msm_digit_at(canon[i].l, c, (int)w);
+    if (!d) return;
+    const uint32_t key = w * nb + (uint32_t)(d < 0 ? -d : d) - 1u;
+    entries[offsets[key] + atomicAdd(&cursor[key], 1u)] = i | (d < 0 ? 0x80000000u : 0u);
+}
+
+// acc += sum_w 2^(c w) W_w (Horner from the top window; one thread)
+template <class C, class F>
+__global__ void powers_horner_kernel(const void* __restrict__ windows, int nwin, int c, void* __restrict__ acc) {
+    if (threadIdx.x != 0 || blockIdx.x != 0) return;
+    typename C::Pt r = pt_load<F>(windows, nwin - 1);
+    for (int w = nwin - 2; w >= 0; w--) {
+        for (int k = 0; k < c; k++) r = C::dbl(r);
+        C::add(r, pt_load<F>(windows, w));
+    }
+    typename C::Pt a = pt_load<F>(acc, 0);
+    C::add(a, r);
+    pt_store<F>(acc, 0, a);
+}
+
+void powers_msm_alloc(PowersMsm& m, bool g2, uint32_t cap) {
+    m.g2 = g2;
+    m.cap = cap ? cap : 1;
+    m.c = powers_pick_c(m.cap);
+    m.nwin = msm_nwin(m.c);
+    m.nbuckets = 1u << (m.c - 1);
+    const size_t pt = g2 ? 256 : 128, nb = (size_t)m.nbuckets * m.nwin;
+    // the windows take the place of a batch's proofs: one "window" of nbuckets buckets per proof, nwin proofs
+    msm_scratch_alloc(m.s, m.cap, 1, m.nbuckets, g2, false, (uint32_t)m.nwin);
+    CUDA_CHECK(cudaMalloc(&m.s.counts, nb * 4));
+    CUDA_CHECK(cudaMalloc(&m.s.offsets, (nb + 1) * 4));
+    CUDA_CHECK(cudaMalloc(&m.s.cursor, nb * 4));
+    CUDA_CHECK(cudaMalloc(&m.s.entries, ((size_t)m.cap * m.nwin + 8) * 4));    // + 16 B: the bulk copy of the last slab
+    CUDA_CHECK(cudaMalloc(&m.s.scalars_canon, ((size_t)m.cap + POWERS_CHUNK) * sizeof(fe)));
+    CUDA_CHECK(cudaFree(m.s.result));
+    m.s.result = nullptr;
+    CUDA_CHECK(cudaMalloc(&m.s.result, (size_t)m.nwin * pt));
+    m.s.result_stride = pt;
+    CUDA_CHECK(cudaMalloc(&m.acc, pt));
+    CUDA_CHECK(cudaMalloc(&m.pw, 2 * sizeof(fe)));
+}
+
+void powers_msm_free(PowersMsm& m) {
+    msm_scratch_free(m.s);
+    if (m.acc) cudaFree(m.acc);
+    if (m.pw) cudaFree(m.pw);
+    m = PowersMsm();
+}
+
+void powers_msm_reset(PowersMsm& m, cudaStream_t st) { CUDA_CHECK(cudaMemsetAsync(m.acc, 0, m.g2 ? 256 : 128, st)); }
+
+template <class C, class F>
+static void powers_msm_slice_t(PowersMsm& m, const void* bases, uint32_t n, uint64_t start, const fe* rho, cudaStream_t st) {
+    if (n == 0) return;
+    if (n > m.cap) throw_error(B2G_E_SHAPE, "powers msm: slice larger than its buffers");
+    constexpr unsigned CTA = 256;
+    const uint32_t nb = m.nbuckets * (uint32_t)m.nwin;
+    powers_base_kernel<<<1, 1, 0, st>>>(rho, start, m.pw);
+    powers_scalars_kernel<<<(n + POWERS_CHUNK * CTA - 1) / (POWERS_CHUNK * CTA), CTA, 0, st>>>(rho, m.pw, n, m.s.scalars_canon);
+    CUDA_CHECK(cudaMemsetAsync(m.s.counts, 0, (size_t)nb * 4, st));
+    const unsigned blocks = (unsigned)(((uint64_t)n * m.nwin + CTA - 1) / CTA);
+    powers_count_kernel<<<blocks, CTA, 0, st>>>(m.s.scalars_canon, n, m.c, m.nwin, m.nbuckets, m.s.counts);
+    msm_scan_kernel<<<1, 1024, 0, st>>>(m.s.counts, nb, m.s.offsets, m.s.cursor);
+    powers_scatter_kernel<<<blocks, CTA, 0, st>>>(m.s.scalars_canon, n, m.c, m.nwin, m.nbuckets, m.s.offsets, m.s.cursor, m.s.entries);
+    g_launch_count += 5;
+    CUDA_CHECK(cudaGetLastError());
+    MsmPlan plan;
+    plan.n = n; plan.c = m.c; plan.nwin = 1; plan.nbuckets = m.nbuckets; plan.table = const_cast<void*>(bases); plan.g2 = m.g2;
+    m.s.sorted_n = n; m.s.sorted_count = (uint32_t)m.nwin;
+    msm_accumulate_t<C, F>(plan, m.s, m.s, st);
+    powers_horner_kernel<C, F><<<1, 1, 0, st>>>(m.s.result, m.nwin, m.c, m.acc);
+    g_launch_count += 1;
+    CUDA_CHECK(cudaGetLastError());
+}
+
+void powers_msm_slice(PowersMsm& m, const void* bases, uint32_t n, uint64_t start, const fe* rho, cudaStream_t st) {
+    if (m.g2) powers_msm_slice_t<G2, Fq2>(m, bases, n, start, rho, st);
+    else powers_msm_slice_t<G1, Fq>(m, bases, n, start, rho, st);
+}
+
 // A full entry slab is 48 KiB (128 runs x 96 entries) on top of the G1 accumulation kernel's static mbarrier word, which is
 // more than the default dynamic limit (48 KiB minus the static size): without the opt-in such launches fail with "invalid
 // argument".  The tail kernels use < 48 KiB of dynamic shared memory.

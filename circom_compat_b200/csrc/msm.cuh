@@ -64,4 +64,43 @@ inline int msm_pick_c(uint32_t n) {
 }
 inline int msm_nwin(int c) { return (255 + c - 1) / c; }
 
+// ------------------------------------------------------------------------------------------------ tableless streamed MSM
+// sum_i rho^i P_i over bases read once (b2g_powers_msm, b2g_powers_check), in slices of at most POWERS_SLICE points.  No
+// window table: a base costs one mixed addition per window, so every window keeps its own bucket set.  Per slice the scalars
+// rho^(start + i) are made on the device, then the batched pipeline above runs with the window in the place of the proof:
+// bucket key w * nbuckets + b, entry word = the base's index in the slice (| sign), accumulate and fold over the bases
+// themselves, the weighted reduction restarting per window (grid.y) and giving one sum per window.  A Horner combine
+// (c doublings per window) adds the slice's sum into a running device accumulator.
+constexpr uint32_t POWERS_SLICE = 1u << 22;
+
+// window size for n bases per slice: the least of nwin(c) * (n + 2^(c+1)) - one mixed addition per base and window, and the
+// running-sum reduction's two additions per bucket - over c in [4, 20].  2^22 bases: c = 17 (15 windows).
+inline int powers_pick_c(uint64_t n) {
+    int best = 4;
+    double cost = 1e300;
+    for (int c = 4; c <= 20; c++) {
+        const double k = (double)msm_nwin(c) * ((double)n + (double)(2ull << c));
+        if (k < cost) { cost = k; best = c; }
+    }
+    return best;
+}
+
+struct PowersMsm {
+    bool g2 = false;
+    int c = 0, nwin = 0;
+    uint32_t nbuckets = 0, cap = 0;     // buckets per window, bases per slice
+    MsmScratch s;                       // counts / offsets / entries over nwin * nbuckets buckets, result = nwin window sums
+    void* acc = nullptr;                // the running XYZZ sum
+    fe* pw = nullptr;                   // rho^start, rho^POWERS_CHUNK (Montgomery)
+};
+
+// buffers for slices of up to `cap` bases; the window size is picked for `cap`
+void powers_msm_alloc(PowersMsm& m, bool g2, uint32_t cap);
+void powers_msm_free(PowersMsm& m);
+// acc = infinity
+void powers_msm_reset(PowersMsm& m, cudaStream_t st);
+// acc += sum_{i < n} rho^(start + i) bases[i]: `bases` n affine Montgomery points on the device, `rho` one Montgomery Fr element
+// on the device.  Nothing synchronises with the host.
+void powers_msm_slice(PowersMsm& m, const void* bases, uint32_t n, uint64_t start, const fe* rho, cudaStream_t st);
+
 }  // namespace b2g

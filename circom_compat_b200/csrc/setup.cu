@@ -830,20 +830,6 @@ static void delta_update_run(b2g_ctx* ctx, const b2g_delta_key* a, const void* x
     CUDA_CHECK(cudaStreamSynchronize(st));
 }
 
-// runs the body of a C entry point; a buffer that did not fit leaves cudaErrorMemoryAllocation as the thread's last error:
-// it is cleared, so that the context's next call does not fail on it
-template <class Fn>
-static int setup_guarded(Fn&& fn) {
-    return guarded([&] {
-        try {
-            fn();
-        } catch (const B2gError& e) {
-            if (e.code == B2G_E_DEVICE) cudaGetLastError();
-            throw;
-        }
-    });
-}
-
 }  // namespace b2g
 
 extern "C" {
@@ -862,15 +848,15 @@ int b2g_setup(b2g_ctx* ctx, const b2g_mat_desc* circuit, const b2g_setup_secrets
 }
 
 int b2g_setup_from_powers(b2g_ctx* ctx, const b2g_mat_desc* circuit, const b2g_powers_desc* powers, b2g_setup_out* out) {
-    return b2g::setup_guarded([&] { b2g::setup_from_powers_run(ctx, circuit, powers, out); });
+    return b2g::guarded_clear([&] { b2g::setup_from_powers_run(ctx, circuit, powers, out); });
 }
 
 int b2g_points_intt(b2g_ctx* ctx, int g2, int log_n, void* points_mont) {
-    return b2g::setup_guarded([&] { b2g::points_intt_run(ctx, g2, log_n, points_mont); });
+    return b2g::guarded_clear([&] { b2g::points_intt_run(ctx, g2, log_n, points_mont); });
 }
 
 int b2g_delta_update(b2g_ctx* ctx, const b2g_delta_key* before, const void* x_canon, b2g_delta_key* after) {
-    return b2g::setup_guarded([&] { b2g::delta_update_run(ctx, before, x_canon, after); });
+    return b2g::guarded_clear([&] { b2g::delta_update_run(ctx, before, x_canon, after); });
 }
 
 }  // extern "C"

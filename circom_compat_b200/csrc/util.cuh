@@ -45,6 +45,20 @@ inline int guarded(Fn&& fn) {
     catch (...) { g_last_error = "unknown error"; return B2G_E_DEVICE; }
 }
 
+// guarded for entry points that allocate as they go: a buffer that did not fit leaves cudaErrorMemoryAllocation as the
+// thread's last error; it is cleared, so that the context's next call does not fail on it
+template <class Fn>
+inline int guarded_clear(Fn&& fn) {
+    return guarded([&] {
+        try {
+            fn();
+        } catch (const B2gError& e) {
+            if (e.code == B2G_E_DEVICE) cudaGetLastError();
+            throw;
+        }
+    });
+}
+
 // ------------------------------------------------------------------------------------------------ host helpers
 struct DevGuard {
     int prev = 0;

@@ -42,6 +42,7 @@
 #include <cstring>
 #include <memory>
 #include <string>
+#include <type_traits>
 #include <vector>
 #include "../../include/b2groth.h"
 #include "fixed.cuh"
@@ -1285,6 +1286,157 @@ uint64_t points_check(bool g2, const void* pts, size_t n, bool subgroup, cudaStr
     if (bad[0] < n && bad[0] <= bad[1]) { *why = 1; return bad[0]; }
     if (bad[1] < n) { *why = 2; return bad[1]; }
     return n;
+}
+
+// ---------------------------------------------------------------------------------------------- powers-of-tau point rules
+// the first rule the affine point p (raw words at w) breaks, in b2g_powers_check's order: 1 a coordinate >= p, 2 off its curve,
+// 3 at infinity, 4 outside G2 (only with `subgroup`), 5 not the generator (only with `gen`); 0 when it passes
+template <class C, class F>
+__device__ __forceinline__ uint32_t powers_rule(const uint8_t* w, bool gen, bool subgroup) {
+    constexpr int WORDS = 2 * Bytes<F>::ELEM / 32;
+    bool below = true;
+    for (int k = 0; k < WORDS; k++) below &= fe_below_p(fe_load(w + 32 * k));
+    if (!below) return 1;
+    const typename C::Aff p = aff_load<F>(w, 0);
+    if (!aff_on_curve<C, F>(p)) return 2;
+    if (C::aff_is_inf(p)) return 3;
+    if constexpr (std::is_same<F, Fq2>::value) { if (subgroup && !g2_in_subgroup(p)) return 4; }
+    if (gen) {
+        const typename C::Aff g = Gen<C>::get();
+        if (!F::eq(p.x, g.x) || !F::eq(p.y, g.y)) return 5;
+    }
+    return 0;
+}
+
+// bad = the lowest base + i whose point breaks a rule other than G2 membership; `gen`: point 0 of the array must be the generator
+template <class C, class F>
+__global__ void __launch_bounds__(128) powers_rules_kernel(const uint8_t* __restrict__ pts, uint32_t n, uint64_t base, int gen,
+                                                           unsigned long long* __restrict__ bad) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    if (powers_rule<C, F>(pts + (size_t)i * 2 * Bytes<F>::ELEM, gen && base + i == 0, false))
+        atomicMin(bad, (unsigned long long)(base + i));
+}
+
+// *rule = the rule the one point at pt breaks (0: none)
+template <class C, class F>
+__global__ void powers_rule_kernel(const uint8_t* __restrict__ pt, int gen, uint32_t* __restrict__ rule) {
+    if (threadIdx.x == 0 && blockIdx.x == 0) *rule = powers_rule<C, F>(pt, gen != 0, true);
+}
+
+void powers_rules(bool g2, const void* pts, uint32_t n, uint64_t base, bool gen, unsigned long long* bad, cudaStream_t st) {
+    if (n == 0) return;
+    const unsigned blocks = (n + 127) / 128;
+    if (g2) {
+        powers_rules_kernel<G2, Fq2><<<blocks, 128, 0, st>>>((const uint8_t*)pts, n, base, gen ? 1 : 0, bad);
+        points_g2_subgroup_kernel<<<blocks, 128, 0, st>>>((const uint8_t*)pts, n, base, bad);
+    } else {
+        powers_rules_kernel<G1, Fq><<<blocks, 128, 0, st>>>((const uint8_t*)pts, n, base, gen ? 1 : 0, bad);
+    }
+    g_launch_count += g2 ? 2 : 1;
+    CUDA_CHECK(cudaGetLastError());
+}
+
+uint32_t powers_point_rule(bool g2, const void* pt, bool gen, uint32_t* scratch, cudaStream_t st) {
+    if (g2) powers_rule_kernel<G2, Fq2><<<1, 1, 0, st>>>((const uint8_t*)pt, gen ? 1 : 0, scratch);
+    else powers_rule_kernel<G1, Fq><<<1, 1, 0, st>>>((const uint8_t*)pt, gen ? 1 : 0, scratch);
+    g_launch_count += 1;
+    CUDA_CHECK(cudaGetLastError());
+    uint32_t rule = 0;
+    CUDA_CHECK(cudaMemcpyAsync(&rule, scratch, 4, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    return rule;
+}
+
+__device__ __forceinline__ G1::Pt g1_at(const uint8_t* g1, int k) { return G1::from_affine(aff_load<Fq>(g1, k)); }
+
+// b2g_powers_check's pairing product, one block of 32 threads: *verdict = 1 iff the five-pair product of include/b2groth.h is 1.
+// sums = S_T, S_A, S_B (G1 XYZZ), S_U (G2 XYZZ); g1 = T_0, T_1, T_(2n-2), A_0, A_(n-1), B_0, B_(n-1); g2 = U_0, U_1, U_(n-1),
+// beta_2 (affine); ch = rho, sigma, pi, kappa, eps (canonical).  The products run on 11 threads, the Miller loops on 5.
+__global__ void __launch_bounds__(32) powers_verdict_kernel(const uint8_t* __restrict__ sums, const uint8_t* __restrict__ g1,
+                                                            const uint8_t* __restrict__ g2, const fe* __restrict__ ch, uint32_t log_n,
+                                                            uint32_t* __restrict__ verdict) {
+    __shared__ fe sc[3];                        // rho^(n-1), rho^(2n-2), kappa rho (canonical)
+    __shared__ G1::Pt p1[11];
+    __shared__ G2::Pt p2[2];
+    __shared__ G1::Aff a1[5];
+    __shared__ G2::Aff a2[2];
+    __shared__ fe12 f[5];
+    const uint32_t t = threadIdx.x;
+    if (t == 0) {
+        const fe rho = Fr::from_canonical(ch[0]);
+        fe pw = Fr::one(), sq = rho;
+        for (uint32_t e = (1u << log_n) - 1; e; e >>= 1) {
+            if (e & 1) pw = Fr::mul(pw, sq);
+            sq = Fr::sqr(sq);
+        }
+        sc[0] = Fr::to_canonical(pw);
+        sc[1] = Fr::to_canonical(Fr::sqr(pw));
+        sc[2] = Fr::to_canonical(Fr::mul(Fr::from_canonical(ch[3]), rho));
+    }
+    __syncthreads();
+    const G1::Pt st = pt_load<Fq>(sums, 0), sa = pt_load<Fq>(sums, 1), sb = pt_load<Fq>(sums, 2);
+    const G2::Pt su = pt_load<Fq2>(sums + 384, 0);
+    // the products: p1 = X_T, X_A, X_B, kappa T_0, -kappa rho T_1, -eps T_0, eps B_0, sigma (S_A - A_0), pi (S_B - B_0); p2 = Q4, Q3
+    if (t == 0) { G1::Pt r = st; G1::add(r, G1::neg(G1::mul_scalar(g1_at(g1, 2), sc[1].l))); p1[0] = r; }
+    else if (t == 1) { G1::Pt r = sa; G1::add(r, G1::neg(G1::mul_scalar(g1_at(g1, 4), sc[0].l))); p1[1] = r; }
+    else if (t == 2) { G1::Pt r = sb; G1::add(r, G1::neg(G1::mul_scalar(g1_at(g1, 6), sc[0].l))); p1[2] = r; }
+    else if (t == 3) p1[3] = G1::mul_scalar(g1_at(g1, 0), ch[3].l);
+    else if (t == 4) p1[4] = G1::neg(G1::mul_scalar(g1_at(g1, 1), sc[2].l));
+    else if (t == 5) p1[5] = G1::neg(G1::mul_scalar(g1_at(g1, 0), ch[4].l));
+    else if (t == 6) p1[6] = G1::mul_scalar(g1_at(g1, 5), ch[4].l);
+    else if (t == 7) { G1::Pt r = sa; G1::add(r, G1::neg(g1_at(g1, 3))); p1[7] = G1::mul_scalar(r, ch[1].l); }
+    else if (t == 8) { G1::Pt r = sb; G1::add(r, G1::neg(g1_at(g1, 5))); p1[8] = G1::mul_scalar(r, ch[2].l); }
+    else if (t == 9) {
+        G2::Pt r = su;
+        G2::add(r, G2::neg(G2::mul_scalar(G2::from_affine(aff_load<Fq2>(g2, 2)), sc[0].l)));
+        p2[0] = r;
+    } else if (t == 10) { G2::Pt r = su; G2::add(r, G2::neg(G2::from_affine(aff_load<Fq2>(g2, 0)))); p2[1] = r; }
+    __syncthreads();
+    if (t == 0) p1[9] = G1::mul_scalar(p1[1], ch[1].l);                   // sigma X_A
+    else if (t == 1) p1[10] = G1::mul_scalar(p1[2], ch[2].l);             // pi X_B
+    __syncthreads();
+    if (t == 0) {
+        G1::Pt hi = st;                                                    // P_hi
+        G1::add(hi, G1::neg(g1_at(g1, 0)));
+        G1::add(hi, p1[7]); G1::add(hi, p1[8]); G1::add(hi, p1[6]);
+        a1[0] = G1::to_affine(hi);
+    } else if (t == 1) {
+        G1::Pt lo = p1[0];                                                 // -P_lo
+        G1::add(lo, p1[9]); G1::add(lo, p1[10]);
+        a1[1] = G1::to_affine(G1::neg(G1::mul_scalar(lo, ch[0].l)));
+    } else if (t >= 2 && t < 5) {
+        a1[t] = G1::to_affine(p1[t + 1]);                                  // kappa T_0, -kappa rho T_1, -eps T_0
+    } else if (t == 5) {
+        a2[0] = G2::to_affine(p2[1]);                                      // S_U - U_0
+    } else if (t == 6) {
+        a2[1] = G2::to_affine(p2[0]);                                      // S_U - rho^(n-1) U_(n-1)
+    }
+    __syncthreads();
+    if (t < 5) {
+        G2::Aff q;
+        if (t == 0) q = aff_load<Fq2>(g2, 0);
+        else if (t == 1) q = aff_load<Fq2>(g2, 1);
+        else if (t == 2) q = a2[0];
+        else if (t == 3) q = a2[1];
+        else q = aff_load<Fq2>(g2, 3);
+        fe12 r;
+        miller_loop(r, !G1::aff_is_inf(a1[t]) && !G2::aff_is_inf(q), a1[t], q, 0, nullptr, nullptr);
+        f[t] = r;
+    }
+    __syncthreads();
+    if (t == 0) {
+        fe12 prod = f[0], e;
+        for (int k = 1; k < 5; k++) Fq12::mul(prod, prod, f[k]);
+        Fq12::final_exponentiation(e, prod);
+        *verdict = Fq12::eq(e, Fq12::one()) ? 1u : 0u;
+    }
+}
+
+void powers_verdict(const void* sums, const void* g1, const void* g2, const void* ch, uint32_t log_n, uint32_t* verdict, cudaStream_t st) {
+    powers_verdict_kernel<<<1, 32, 0, st>>>((const uint8_t*)sums, (const uint8_t*)g1, (const uint8_t*)g2, (const fe*)ch, log_n, verdict);
+    g_launch_count += 1;
+    CUDA_CHECK(cudaGetLastError());
 }
 
 // ---------------------------------------------------------------------------------------------- delta update check

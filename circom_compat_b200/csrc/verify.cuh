@@ -1,6 +1,7 @@
 // verify.cuh - what the context code (prover.cu) and the batched verifier (verify.cu) share.
 #pragma once
 #include <cstddef>
+#include <cstdint>
 #include <cuda_runtime.h>
 
 struct b2g_ctx;
@@ -27,5 +28,17 @@ int setup_generators_check(const void* g1, const void* g2, cudaStream_t st);
 // >= p or lies off its curve (*why = 1), or, with `subgroup`, is a G2 point outside G2 (*why = 2); n when every point passes.
 // Synchronises the stream.
 uint64_t points_check(bool g2, const void* pts, size_t n, bool subgroup, cudaStream_t st, int* why);
+
+// b2g_powers_check's point rules over the n affine Montgomery points of a device slice whose first point has index `base` in its
+// array: atomicMin of the index of every point with a coordinate >= p, off its curve, at infinity, outside G2 (G2 only) or, with
+// `gen`, other than the generator at index 0, into *bad (device).  Asynchronous.
+void powers_rules(bool g2, const void* pts, uint32_t n, uint64_t base, bool gen, unsigned long long* bad, cudaStream_t st);
+// the first of those rules the one device point at pt breaks: 1 a coordinate >= p, 2 off its curve, 3 at infinity, 4 outside
+// G2, 5 not the generator (only with gen); 0 when it passes.  scratch: 4 device bytes.  Synchronises the stream.
+uint32_t powers_point_rule(bool g2, const void* pt, bool gen, uint32_t* scratch, cudaStream_t st);
+// b2g_powers_check's pairing product (include/b2groth.h) into *verdict (device, 1 or 0).  sums = S_T, S_A, S_B (G1 XYZZ, 128 B
+// each), S_U (G2 XYZZ); g1 = T_0, T_1, T_(2n-2), A_0, A_(n-1), B_0, B_(n-1); g2 = U_0, U_1, U_(n-1), beta_2 (affine Montgomery);
+// ch = rho, sigma, pi, kappa, eps (32 B canonical each); all device.  Asynchronous.
+void powers_verdict(const void* sums, const void* g1, const void* g2, const void* ch, uint32_t log_n, uint32_t* verdict, cudaStream_t st);
 
 }  // namespace b2g

@@ -291,6 +291,18 @@ class Context:
         N.check(N.lib().b2g_points_intt(self._h, int(bool(g2)), log_n, _ptr(d)))
         return d
 
+    def powers_msm(self, points, rho, g2=False) -> np.ndarray:
+        """b2g_powers_msm: sum_i rho^i P_i over affine Montgomery points (rows of 8 / 16 words, read in place when contiguous)
+        and an int rho in [0, r), as the tableless streamed MSM of verify_powers_of_tau computes it; affine, 8 / 16 words"""
+        pts = _c(points).reshape(-1, 16 if g2 else 8)
+        rho = int(rho)
+        if not 0 <= rho < 1 << 256:
+            raise ValueError("rho must be a 256-bit unsigned integer")
+        rb = np.frombuffer(rho.to_bytes(32, 'little'), dtype=np.uint8).copy()
+        out = np.zeros(16 if g2 else 8, dtype=np.uint64)
+        N.check(N.lib().b2g_powers_msm(self._h, int(bool(g2)), pts.shape[0], _ptr(pts), _ptr(rb), _ptr(out)))
+        return out
+
     def fixed_base_g1(self, scalars_canon) -> np.ndarray:
         sc = _c(scalars_canon); n = sc.size // 4
         out = np.zeros((n, 8), dtype=np.uint64)
@@ -830,6 +842,45 @@ class Groth16:
         out = np.zeros(1, dtype=np.uint8)
         N.check(N.lib().b2g_delta_update_check(ctx._h, C.byref(d0), C.byref(d1), _ptr(wb), _ptr(out)))
         return bool(out[0])
+
+    @staticmethod
+    def verify_powers_of_tau(powers, log_n=None, ctx: Context = None, challenges=None):
+        """The algebraic checks of `snarkjs powersoftau verify` on the GPU (b2g_powers_check): whether the prefix a domain of
+        2^log_n points reads (the whole ceremony by default) holds powers of one tau with the same alpha and beta on the
+        standard generators.  `powers` is a ptau.read_ptau result or any object with the same fields; memory-mapped views are
+        read in place, once.  The five challenges (rho, sigma, pi, kappa, eps in [1, r)) are drawn with `secrets` unless
+        given.  Returns a ptau.PowersCheck: truthy when the ceremony passes, .reason naming the first failing point or the
+        failed pairing product.  A ceremony that is not one passes with probability at most 2n / (r - 1) when the challenges
+        are drawn after the file is fixed.  Raises ValueError for a bad log_n or arrays shorter than it reads."""
+        import secrets
+        from .ptau import ARRAYS, Powers, PowersCheck
+        power = int(powers.power)
+        log_n = power if log_n is None else int(log_n)
+        if log_n < 1:
+            raise ValueError(f"verify_powers_of_tau: log_n {log_n} is below 1")
+        pre = Powers(power, int(getattr(powers, 'ceremony_power', power)),
+                     *(np.asarray(getattr(powers, k)) for k in ARRAYS)).prefix(log_n)
+        if challenges is None:
+            challenges = [1 + secrets.randbelow(R_MOD - 1) for _ in range(5)]
+        challenges = [int(c) for c in challenges]
+        if len(challenges) != 5 or not all(0 <= c < 1 << 256 for c in challenges):
+            raise ValueError("verify_powers_of_tau: five challenges (rho, sigma, pi, kappa, eps), each below 2^256")
+        cb = np.frombuffer(b''.join(c.to_bytes(32, 'little') for c in challenges), dtype=np.uint8).copy()
+        pd = N.PowersDesc()
+        pd.log_size = power
+        keep = []
+        for name in ARRAYS:
+            a = _c(getattr(pre, name))
+            keep.append(a)
+            setattr(pd, name, a.ctypes.data)
+        rep = N.PowersReport()
+        ctx = ctx or default_context()
+        N.check(N.lib().b2g_powers_check(ctx._h, C.byref(pd), log_n, _ptr(cb), C.byref(rep)))
+        if rep.ok:
+            return PowersCheck(True)
+        if rep.rule == 6:
+            return PowersCheck(False, 6)
+        return PowersCheck(False, int(rep.rule), ARRAYS[rep.array], int(rep.index))
 
     # ---- verification (host pairing; circom_compat_b200/verifier.py).  Call sites in the reference: src/zkey.rs:868-870,
     # 914-916 (process_vk + verify_with_processed_vk), tests/groth16.rs:33-35 (SNARK::verify).

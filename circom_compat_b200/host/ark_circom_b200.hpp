@@ -27,6 +27,7 @@
 //                                                of ProvingKey<Bn254> / VerifyingKey<Bn254>, points decoded on the device
 //   ark_circom::read_ptau + Groth16::generate_parameters_from_powers_of_tau <- snarkjs groth16 setup (a key from a ceremony)
 //   ark_circom::Groth16::contribute / verify_contribution <- snarkjs zkey contribute / the delta checks of snarkjs zkey verify
+//   ark_circom::Groth16::verify_powers_of_tau <- the algebraic checks of snarkjs powersoftau verify
 //   ark_circom::read_wtns                              <- snarkjs .wtns (test-vectors/circuit2_js/witness.wtns; the reference
 //                                                         computes witnesses with WASM instead, out of scope here)
 // Parsing and key handling stay on the host; every field/curve operation of the proof runs in libb2groth.so.
@@ -545,6 +546,36 @@ struct VerifyCall {
     }
 };
 
+// The verdict of Groth16T::verify_powers_of_tau (b2g_powers_check): ok, or the reason of the failure in the messages of
+// b2g_setup_from_powers ("tau_g2[17]: not in G2"), or "the powers are not those of one tau, alpha and beta".
+struct PowersCheck {
+    bool ok = false;
+    int rule = 0;                 // b2g_powers_report's rule code
+    std::string array;            // rules 1-5: the array and the index of the first failing point
+    uint64_t index = 0;
+    explicit operator bool() const { return ok; }
+    std::string reason() const {
+        if (ok) return "";
+        if (rule == 6) return "the powers are not those of one tau, alpha and beta";
+        const bool g2 = array == "tau_g2" || array == "beta_g2";
+        static const char* const texts[6] = {"", "a coordinate >= p", "off the curve", "at infinity", "not in G2", "not the generator"};
+        return array + "[" + std::to_string(index) + "]: " + (rule == 2 && g2 ? "off the twist" : texts[rule]);
+    }
+};
+
+// the five challenges of the ceremony check (rho, sigma, pi, kappa, eps), uniform in [1, r), from std::random_device
+inline std::vector<BigInt256> powers_challenges() {
+    std::random_device rd;
+    std::vector<BigInt256> c(5);
+    for (BigInt256& b : c) {
+        do {
+            for (int t = 0; t < 4; t++) b.l[t] = ((uint64_t)rd() << 32) | rd();
+            b.l[3] &= 0x3FFFFFFFFFFFFFFFULL;
+        } while (detail::geq(b.l, detail::FR_P) || !(b.l[0] | b.l[1] | b.l[2] | b.l[3]));
+    }
+    return c;
+}
+
 // n nonzero 128-bit weights of the batch check (4 little-endian words each) from std::random_device
 inline std::vector<uint32_t> batch_weights(size_t n) {
     std::random_device rd;
@@ -932,6 +963,34 @@ struct Groth16T {                                       // Groth16::<Bn254, QAP>
         const Gpu::MatDesc md(matrices, nv, QAP::ID, true);
         check(b2g_setup_from_powers(gpu.ctx(), &md.d, &pd, &out));
         return pk;
+    }
+
+    // the algebraic checks of `snarkjs powersoftau verify` (b2g_powers_check): whether the prefix a domain of 2^log_n points
+    // reads (log_n = 0: the ceremony's power) holds powers of one tau with the same alpha and beta on the standard generators.
+    // The challenges come from std::random_device, drawn after the powers are fixed, unless five are given (canonical, in
+    // [1, r)).  Throws std::invalid_argument when log_n exceeds the power or the vectors hold fewer points than it reads.
+    static PowersCheck verify_powers_of_tau(const Powers& powers, uint32_t log_n = 0, Gpu& gpu = Gpu::instance(),
+                                            const std::vector<BigInt256>* challenges = nullptr) {
+        if (!log_n) log_n = powers.power;
+        if (log_n > powers.power) throw std::invalid_argument("verify_powers_of_tau: log_n exceeds the ceremony's power");
+        const size_t n = (size_t)1 << log_n;
+        if (powers.tau_g1.size() < 2 * n - 1 || powers.tau_g2.size() < n || powers.alpha_tau_g1.size() < n || powers.beta_tau_g1.size() < n)
+            throw std::invalid_argument("verify_powers_of_tau: the powers hold fewer points than a domain of " + std::to_string(n) + " reads");
+        const std::vector<BigInt256> drawn = challenges ? *challenges : powers_challenges();
+        if (drawn.size() != 5) throw std::invalid_argument("verify_powers_of_tau: five challenges (rho, sigma, pi, kappa, eps)");
+        b2g_powers_desc pd;
+        memset(&pd, 0, sizeof pd);
+        pd.log_size = powers.power;
+        pd.tau_g1 = powers.tau_g1.data(); pd.tau_g2 = powers.tau_g2.data(); pd.alpha_tau_g1 = powers.alpha_tau_g1.data();
+        pd.beta_tau_g1 = powers.beta_tau_g1.data(); pd.beta_g2 = &powers.beta_g2;
+        b2g_powers_report rep;
+        check(b2g_powers_check(gpu.ctx(), &pd, log_n, drawn.data(), &rep));
+        static const char* const arrays[5] = {"tau_g1", "tau_g2", "alpha_tau_g1", "beta_tau_g1", "beta_g2"};
+        PowersCheck r;
+        r.ok = rep.ok != 0;
+        r.rule = rep.rule;
+        if (!r.ok && rep.rule != 6) { r.array = arrays[rep.array]; r.index = rep.index; }
+        return r;
     }
 
     // `snarkjs zkey contribute` (b2g_delta_update): pk with delta multiplied by x (nonzero, below r) and the L and H queries

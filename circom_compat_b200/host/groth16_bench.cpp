@@ -41,6 +41,9 @@
 //       contribution with x = Fr::rand(std::mt19937_64(seed)) (default seed 0x5E7), check it (verify_contribution), prove the
 //       witness under the same rng and verify on the host; print x, the contributed key (serialize_proving_key, compressed,
 //       hex), the check's verdict, the proof and the host verifier's verdict
+//   B2G_PTAU_CHECK=<file.ptau> groth16_bench [log_n]
+//       check the ceremony (or the prefix a domain of 2^log_n points reads) with Groth16T::verify_powers_of_tau and print
+//       powers=1 or powers=0 with the reason, and the time of the check in ms (the file read not included)
 //       chain:<a> = the witness of the reference's squaring-chain bench family for input a
 //       (test-vectors/complex-circuit/input.json has a = 3), computed on the host instead of by WASM.
 #include <algorithm>
@@ -170,6 +173,20 @@ int main(int argc, char** argv) {
             for (uint8_t b : serialize_compressed(proof)) std::printf("%02x", b);
             std::printf("\n");
             std::printf("verified=%d\n", Groth16::verify_with_processed_vk(Groth16::process_vk(vk2), in2, p2) ? 1 : 0);
+            return 0;
+        }
+        if (const char* ptau = std::getenv("B2G_PTAU_CHECK")) {             // ceremony -> its check on the GPU
+            const uint32_t log_n = argc > 1 ? (uint32_t)std::stoul(argv[1]) : 0;
+            std::ifstream pf(ptau, std::ios::binary);
+            if (!pf) throw SerializationError("cannot open ptau");
+            const Powers powers = read_ptau(pf, log_n);
+            typedef Groth16T<CircomReduction> G;
+            const auto t0 = std::chrono::steady_clock::now();
+            const PowersCheck r = G::verify_powers_of_tau(powers, log_n);
+            const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+            std::printf("powers=%d\n", r.ok ? 1 : 0);
+            if (!r.ok) std::printf("reason=%s\n", r.reason().c_str());
+            std::printf("ms=%.3f\n", ms);
             return 0;
         }
         if (const char* ptau = std::getenv("B2G_SETUP_PTAU")) {             // R1CS + ceremony -> key -> contribution -> check -> prove -> verify

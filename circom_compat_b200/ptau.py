@@ -14,6 +14,9 @@ infinity.  The prepared Lagrange sections 12-15 are not read: b2g_setup_from_pow
 read_ptau returns zero-copy views of sections 2-6 over the file's memory map (or over the given bytes), as rows of 8 / 16
 uint64 words, the b2g_pk_desc layout.  Nothing is read beyond the headers until a caller touches the points, and the setup
 reads only the prefix its circuit needs, so a ceremony file much larger than memory serves small circuits.
+
+PowersCheck is the verdict of Groth16.verify_powers_of_tau (b2g_powers_check): truthy when the ceremony passes, with the
+reason of a failure in the messages b2g_setup_from_powers uses ("tau_g2[17]: not in G2").
 """
 from __future__ import annotations
 
@@ -55,6 +58,34 @@ class Powers:
             a = a[:count]
             out.append(np.array(a, dtype=np.uint64, order='C', copy=True) if copy else a)
         return Powers(self.power, self.ceremony_power, *out)
+
+
+ARRAYS = ('tau_g1', 'tau_g2', 'alpha_tau_g1', 'beta_tau_g1', 'beta_g2')
+NOT_POWERS = "the powers are not those of one tau, alpha and beta"
+# b2g_powers_report rule codes 1-5 (G1 text, G2 text)
+_RULES = {1: ('a coordinate >= p',) * 2, 2: ('off the curve', 'off the twist'), 3: ('at infinity',) * 2, 4: ('not in G2',) * 2,
+          5: ('not the generator',) * 2}
+
+
+@dataclass
+class PowersCheck:
+    """the verdict of a ceremony check: truthy when it passes.  rule (b2g_powers_report): 0 ok, 1 a coordinate >= p, 2 off its
+    curve, 3 at infinity, 4 outside G2, 5 not the generator (array / index name the point), 6 the ratio rules fail"""
+    ok: bool
+    rule: int = 0
+    array: str = None
+    index: int = None
+
+    def __bool__(self) -> bool:
+        return bool(self.ok)
+
+    @property
+    def reason(self):
+        if self.ok:
+            return None
+        if self.rule == 6:
+            return NOT_POWERS
+        return f"{self.array}[{self.index}]: {_RULES[self.rule][self.array in ('tau_g2', 'beta_g2')]}"
 
 
 def _buffer(src) -> np.ndarray:

@@ -33,6 +33,7 @@
  *                             generate_random_parameters_with_reduction calls (tests/groth16.rs:25): a whole proving key
  *   b2g_setup_from_powers  <- snarkjs groth16 setup (zkey new): a proving key from a powers-of-tau ceremony
  *   b2g_delta_update / b2g_delta_update_check <- snarkjs zkey contribute / the delta checks of snarkjs zkey verify
+ *   b2g_powers_check       <- the algebraic checks of snarkjs powersoftau verify
  *   b2g_fixed_base_g1/g2  <- the batch fixed-base multiplications of that setup, for the standard generators only
  *
  * Conventions
@@ -498,7 +499,7 @@ typedef struct {
  * The key equals, byte for byte, b2g_setup(circuit, alpha, beta, gamma = 1, delta = 1, tau) on the generators g1 = tau_g1[0]
  * and g2 = tau_g2[0].  The call checks only what it reads: every point read lies on its curve with coordinates below p, the
  * G2 points are in G2, and tau_g1[0], tau_g2[0] are not at infinity.  Whether the arrays really are powers of one tau with
- * the same alpha and beta is left to the ceremony's own verification (snarkjs powersoftau verify).
+ * the same alpha and beta is checked by b2g_powers_check, which callers run first.
  * Cost: four inverse transforms over G1 and one over G2 of n points, each (n/2) log2 n variable-base products; one product
  * per nonzero (a coefficient k above r/2 multiplies the negated point by r - k, so +-1 and small constants are cheap).
  * Synchronous.  Errors (every error leaves the context usable): the matrix checks and messages of b2g_setup (B2G_E_SHAPE);
@@ -506,6 +507,49 @@ typedef struct {
  * >= p, a G2 point outside G2, or tau_g1[0] / tau_g2[0] at infinity, naming the array and index ("tau_g2[17]: not in G2");
  * B2G_E_SHAPE for null pointers or a pending proof; B2G_E_DEVICE when the buffers do not fit in device memory. */
 B2G_API int b2g_setup_from_powers(b2g_ctx* ctx, const b2g_mat_desc* circuit, const b2g_powers_desc* powers, b2g_setup_out* out);
+
+/* The verdict of b2g_powers_check.  rule: 0 none (ok), 1 a coordinate >= p, 2 off its curve, 3 at infinity, 4 outside G2,
+ * 5 not the generator, 6 the powers are not those of one tau, alpha and beta.  array (rules 1-5): 0 tau_g1, 1 tau_g2,
+ * 2 alpha_tau_g1, 3 beta_tau_g1, 4 beta_g2; index: the point in that array. */
+typedef struct {
+    uint8_t ok;
+    uint8_t rule;
+    uint8_t array;
+    uint8_t reserved[5];
+    uint64_t index;
+} b2g_powers_report;
+
+/* b2g_powers_check <- the algebraic checks of `snarkjs powersoftau verify`: whether the prefix a domain of n = 2^log_n points
+ * reads (1 <= log_n <= log_size <= 28) is a ceremony, checked in one streamed pass over the host arrays.  With T = tau_g1
+ * (2n - 1 points), U = tau_g2 (n), A = alpha_tau_g1 (n), B = beta_tau_g1 (n) and beta_2 = beta_g2, out->ok = 1 iff
+ *   the point rules hold: every point read has coordinates below p, lies on its curve and is not at infinity; every G2 point
+ *   is in G2; T_0 = G1 = (1, 2) and U_0 = the standard G2 generator (ark-bn254, EIP-197);
+ *   and the ratio rules hold, all at once through one random linear combination:
+ *     e(T_(i+1), U_0) = e(T_i, U_1), i < 2n - 2;   e(A_(i+1), U_0) = e(A_i, U_1) and e(B_(i+1), U_0) = e(B_i, U_1), i < n - 1;
+ *     e(T_0, U_(i+1)) = e(T_1, U_i), i < n - 1;     e(B_0, U_0) = e(T_0, beta_2).
+ * challenges = 5 x 32 B canonical rho, sigma, pi, kappa, eps in [1, r).  With S_X = sum_(i < |X|) rho^i X_i (one tableless
+ * MSM per array), the shifted sums are sum_(i < M-1) rho^i X_(i+1) = rho^-1 (S_X - X_0) and sum_(i < M-1) rho^i X_i =
+ * S_X - rho^(M-1) X_(M-1), so that, multiplied through by rho, every equation above is one term of
+ *     P_hi = (S_T - T_0) + sigma (S_A - A_0) + pi (S_B - B_0) + eps B_0,
+ *     P_lo = rho [(S_T - rho^(2n-2) T_(2n-2)) + sigma (S_A - rho^(n-1) A_(n-1)) + pi (S_B - rho^(n-1) B_(n-1))],
+ *     e(P_hi, U_0) e(-P_lo, U_1) e(kappa T_0, S_U - U_0) e(-kappa rho T_1, S_U - rho^(n-1) U_(n-1)) e(-eps T_0, beta_2) == 1,
+ * each with its own monomial (rho^(i+1), sigma rho^(i+1), pi rho^(i+1), kappa rho^(i+1), eps).
+ * Soundness, as for b2g_verify_batch: an honest ceremony always gives ok = 1.  Once the point rules hold every point lies in a
+ * group of prime order r, so by Schwartz-Zippel a ceremony that breaks any ratio rule gives ok = 1 with probability at most
+ * 2n / (r - 1) (about 2^-224 at log_n = 28), and only if the challenges are drawn uniformly from [1, r) AFTER the ceremony is
+ * fixed, from a source its authors cannot predict or influence.
+ * A failure names the first point in section order (tau_g1, tau_g2, alpha_tau_g1, beta_tau_g1, beta_g2; lowest index first)
+ * that breaks a point rule, with the first rule it breaks in the order of the codes above; the pairing product (rule 6) is
+ * evaluated only when every point passes.  The transcript of snarkjs (the BLAKE2b hash chain and the contributions' proofs of
+ * knowledge) is not checked.
+ * The arrays are read once, in slices of 2^22 points through pinned staging buffers, the copy of one slice overlapping the work
+ * on the one before, so device memory does not grow with the ceremony.  Cost: one tableless MSM per array (about one mixed
+ * addition per point and window), the G2 subgroup test per G2 point, and five Miller loops with one final exponentiation.
+ * Synchronous.  Errors (every error leaves the context usable; a malformed point is a verdict, not an error): B2G_E_DOMAIN for
+ * log_n outside [1, log_size] or log_size > 28; B2G_E_INPUT for a challenge that is 0 or >= r; B2G_E_SHAPE for null pointers or
+ * a pending proof; B2G_E_DEVICE when the buffers do not fit. */
+B2G_API int b2g_powers_check(b2g_ctx* ctx, const b2g_powers_desc* powers, uint32_t log_n, const void* challenges,
+                             b2g_powers_report* out);
 
 /* The part of a proving key a delta contribution changes, HOST buffers in the b2g_pk_desc layout. */
 typedef struct {
@@ -556,6 +600,11 @@ B2G_API int b2g_fixed_base_g2(b2g_ctx* ctx, const void* scalars_canon, size_t n,
  * scaled by n^-1 as b2g_ntt scales it: out_k = n^-1 sum_i omega_n^(-ik) in_i (log_n in 1..27, else B2G_E_DOMAIN).  The points
  * are not checked.  The kernel b2g_setup_from_powers runs. */
 B2G_API int b2g_points_intt(b2g_ctx* ctx, int g2, int log_n, void* points_mont);
+/* b2g_powers_msm: sum_(i < n) rho^i P_i over n host affine points (g2 = 0: G1, 64 B each; 1: G2, 128 B), rho 32 B canonical
+ * (below r, else B2G_E_INPUT), out 64 / 128 B affine Montgomery (all-zero = infinity).  The tableless streamed MSM
+ * b2g_powers_check runs: the points are read once, in slices, and are not checked.  B2G_E_SHAPE for null pointers or a
+ * pending proof; n = 0 gives infinity. */
+B2G_API int b2g_powers_msm(b2g_ctx* ctx, int g2, size_t n, const void* bases, const void* rho_canon, void* out_affine);
 
 /* Element-wise device arithmetic, for unit parity tests of the field / group layers.
  * op: 0 fq_mul, 1 fq_add, 2 fq_sub, 3 fr_mul, 4 fr_add, 5 fr_sub, 6 fq_inv, 7 fr_inv (b ignored),
