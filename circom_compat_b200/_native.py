@@ -63,6 +63,19 @@ class PowersReport(C.Structure):
     _fields_ = [('ok', C.c_uint8), ('rule', C.c_uint8), ('array', C.c_uint8), ('reserved', C.c_uint8 * 5), ('index', C.c_uint64)]
 
 
+class KeyDesc(C.Structure):
+    """b2g_key_desc: a whole proving key with its counts (host arrays)"""
+    _fields_ = [(k, C.c_uint32) for k in ('n_vars', 'n_ic', 'n_l', 'n_h')] + \
+               [(k, C.c_void_p) for k in ('alpha_g1', 'beta_g1', 'delta_g1', 'beta_g2', 'gamma_g2', 'delta_g2', 'gamma_abc_g1',
+                                          'a_query', 'b_g1_query', 'b_g2_query', 'l_query', 'h_query')]
+
+
+class SetupReport(C.Structure):
+    """b2g_setup_report: the verdict of b2g_setup_check"""
+    _fields_ = [('ok', C.c_uint8), ('rule', C.c_uint8), ('side', C.c_uint8), ('field', C.c_uint8), ('reserved', C.c_uint8 * 4),
+                ('index', C.c_uint64)]
+
+
 class DeltaKey(C.Structure):
     """b2g_delta_key: the fields of a proving key a delta contribution changes (host buffers)"""
     _fields_ = [('n_l', C.c_uint32), ('n_h', C.c_uint32)] + [(k, C.c_void_p) for k in ('delta_g1', 'delta_g2', 'l_query', 'h_query')]
@@ -83,7 +96,7 @@ EXPORTS = ['b2g_last_error', 'b2g_version', 'b2g_device_count', 'b2g_ctx_create'
            'b2g_verify_batch_keys_compressed', 'b2g_verify_batch_keys_locate', 'b2g_verify_batch_keys_locate_compressed',
            'b2g_rerandomize_many', 'b2g_points_serialize', 'b2g_points_deserialize', 'b2g_setup',
            'b2g_setup_from_powers', 'b2g_delta_update', 'b2g_delta_update_check', 'b2g_points_intt',
-           'b2g_powers_msm', 'b2g_powers_check']
+           'b2g_powers_msm', 'b2g_powers_check', 'b2g_setup_check']
 
 _lib = None
 
@@ -132,6 +145,7 @@ def lib():
         L.b2g_points_intt.argtypes = [vp, i, i, vp]
         L.b2g_powers_msm.argtypes = [vp, i, sz, vp, vp, vp]
         L.b2g_powers_check.argtypes = [vp, C.POINTER(PowersDesc), C.c_uint32, vp, C.POINTER(PowersReport)]
+        L.b2g_setup_check.argtypes = [vp, C.POINTER(MatDesc), C.POINTER(PowersDesc), C.POINTER(KeyDesc), vp, C.POINTER(SetupReport)]
         L.b2g_test_op.argtypes = [vp, i, vp, vp, sz, vp]
         L.b2g_last_timings.argtypes = [vp, vp]
         L.b2g_bench_device.argtypes = [vp, vp, vp, i, C.POINTER(C.c_float)]

@@ -744,20 +744,32 @@ void powers_msm_free(PowersMsm& m) {
 
 void powers_msm_reset(PowersMsm& m, cudaStream_t st) { CUDA_CHECK(cudaMemsetAsync(m.acc, 0, m.g2 ? 256 : 128, st)); }
 
+void powers_scalars(const fe* rho, uint64_t start, uint32_t n, fe* pw, fe* canon, cudaStream_t st) {
+    if (n == 0) return;
+    constexpr unsigned CTA = 256;
+    powers_base_kernel<<<1, 1, 0, st>>>(rho, start, pw);
+    powers_scalars_kernel<<<(n + POWERS_CHUNK * CTA - 1) / (POWERS_CHUNK * CTA), CTA, 0, st>>>(rho, pw, n, canon);
+    g_launch_count += 2;
+    CUDA_CHECK(cudaGetLastError());
+}
+
 template <class C, class F>
-static void powers_msm_slice_t(PowersMsm& m, const void* bases, uint32_t n, uint64_t start, const fe* rho, cudaStream_t st) {
+static void powers_msm_slice_t(PowersMsm& m, const void* bases, uint32_t n, uint64_t start, const fe* rho, cudaStream_t st,
+                               const fe* scalars) {
     if (n == 0) return;
     if (n > m.cap) throw_error(B2G_E_SHAPE, "powers msm: slice larger than its buffers");
     constexpr unsigned CTA = 256;
     const uint32_t nb = m.nbuckets * (uint32_t)m.nwin;
-    powers_base_kernel<<<1, 1, 0, st>>>(rho, start, m.pw);
-    powers_scalars_kernel<<<(n + POWERS_CHUNK * CTA - 1) / (POWERS_CHUNK * CTA), CTA, 0, st>>>(rho, m.pw, n, m.s.scalars_canon);
+    if (!scalars) {
+        powers_scalars(rho, start, n, m.pw, m.s.scalars_canon, st);
+        scalars = m.s.scalars_canon;
+    }
     CUDA_CHECK(cudaMemsetAsync(m.s.counts, 0, (size_t)nb * 4, st));
     const unsigned blocks = (unsigned)(((uint64_t)n * m.nwin + CTA - 1) / CTA);
-    powers_count_kernel<<<blocks, CTA, 0, st>>>(m.s.scalars_canon, n, m.c, m.nwin, m.nbuckets, m.s.counts);
+    powers_count_kernel<<<blocks, CTA, 0, st>>>(scalars, n, m.c, m.nwin, m.nbuckets, m.s.counts);
     msm_scan_kernel<<<1, 1024, 0, st>>>(m.s.counts, nb, m.s.offsets, m.s.cursor);
-    powers_scatter_kernel<<<blocks, CTA, 0, st>>>(m.s.scalars_canon, n, m.c, m.nwin, m.nbuckets, m.s.offsets, m.s.cursor, m.s.entries);
-    g_launch_count += 5;
+    powers_scatter_kernel<<<blocks, CTA, 0, st>>>(scalars, n, m.c, m.nwin, m.nbuckets, m.s.offsets, m.s.cursor, m.s.entries);
+    g_launch_count += 3;
     CUDA_CHECK(cudaGetLastError());
     MsmPlan plan;
     plan.n = n; plan.c = m.c; plan.nwin = 1; plan.nbuckets = m.nbuckets; plan.table = const_cast<void*>(bases); plan.g2 = m.g2;
@@ -768,9 +780,9 @@ static void powers_msm_slice_t(PowersMsm& m, const void* bases, uint32_t n, uint
     CUDA_CHECK(cudaGetLastError());
 }
 
-void powers_msm_slice(PowersMsm& m, const void* bases, uint32_t n, uint64_t start, const fe* rho, cudaStream_t st) {
-    if (m.g2) powers_msm_slice_t<G2, Fq2>(m, bases, n, start, rho, st);
-    else powers_msm_slice_t<G1, Fq>(m, bases, n, start, rho, st);
+void powers_msm_slice(PowersMsm& m, const void* bases, uint32_t n, uint64_t start, const fe* rho, cudaStream_t st, const fe* scalars) {
+    if (m.g2) powers_msm_slice_t<G2, Fq2>(m, bases, n, start, rho, st, scalars);
+    else powers_msm_slice_t<G1, Fq>(m, bases, n, start, rho, st, scalars);
 }
 
 // A full entry slab is 48 KiB (128 runs x 96 entries) on top of the G1 accumulation kernel's static mbarrier word, which is

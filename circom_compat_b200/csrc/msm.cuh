@@ -67,7 +67,8 @@ inline int msm_nwin(int c) { return (255 + c - 1) / c; }
 // ------------------------------------------------------------------------------------------------ tableless streamed MSM
 // sum_i rho^i P_i over bases read once (b2g_powers_msm, b2g_powers_check), in slices of at most POWERS_SLICE points.  No
 // window table: a base costs one mixed addition per window, so every window keeps its own bucket set.  Per slice the scalars
-// rho^(start + i) are made on the device, then the batched pipeline above runs with the window in the place of the proof:
+// rho^(start + i) are made on the device (or given as a device vector: b2g_setup_check's transformed column weights), then
+// the batched pipeline above runs with the window in the place of the proof:
 // bucket key w * nbuckets + b, entry word = the base's index in the slice (| sign), accumulate and fold over the bases
 // themselves, the weighted reduction restarting per window (grid.y) and giving one sum per window.  A Horner combine
 // (c doublings per window) adds the slice's sum into a running device accumulator.
@@ -100,7 +101,11 @@ void powers_msm_free(PowersMsm& m);
 // acc = infinity
 void powers_msm_reset(PowersMsm& m, cudaStream_t st);
 // acc += sum_{i < n} rho^(start + i) bases[i]: `bases` n affine Montgomery points on the device, `rho` one Montgomery Fr element
-// on the device.  Nothing synchronises with the host.
-void powers_msm_slice(PowersMsm& m, const void* bases, uint32_t n, uint64_t start, const fe* rho, cudaStream_t st);
+// on the device.  With `scalars` (n canonical Fr elements on the device) the slice takes them instead of the powers of rho, and
+// rho and start are not read.  Nothing synchronises with the host.
+void powers_msm_slice(PowersMsm& m, const void* bases, uint32_t n, uint64_t start, const fe* rho, cudaStream_t st,
+                      const fe* scalars = nullptr);
+// canon[i] = rho^(start + i) in canonical form, i < n (rho Montgomery, device); pw: 2 device Fr elements of scratch
+void powers_scalars(const fe* rho, uint64_t start, uint32_t n, fe* pw, fe* canon, cudaStream_t st);
 
 }  // namespace b2g

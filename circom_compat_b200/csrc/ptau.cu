@@ -9,11 +9,25 @@
 //   sums          S_X = sum_i rho^i X_i per array by powers_msm_slice, the scalars made on the device per slice
 //   verdict       powers_verdict_kernel (verify.cu, with the rest of the pairing code): P_hi, P_lo and the G2 terms of
 //                 include/b2groth.h, five Miller loops, one product and one final exponentiation
+//
+// b2g_setup_check, a proving key against its circuit and ceremony, moves b2g_setup_from_powers's point transforms onto scalars:
+//   weights       w_j = rho^j and v_i = sigma^i by the powers kernels of the streamed MSM
+//   row products  c = A'w, Bw, Cw: one product per nonzero keyed by its row, then a reduce-by-key with the Fr addition, so a
+//                 row holding every column is summed by many threads; the public-input rows of A' add w_j at row m + j
+//   transforms    s = iNTT_n(c) on the scalar NTT; the E5 scalars h from v by the reduction's formula
+//   sums          the same streamed passes as above: the key's arrays with the powers of rho (sigma for h_query), the ceremony's
+//                 with the explicit scalars s and h; the point rules (setup_rules, verify.cu) in the same passes
+//   verdict       setup_check_verdict_kernel (verify.cu): E1-E3 compare sums, E4-E6 are three pairing products
+// Every scalar is canonical: the Montgomery product of a Montgomery coefficient and a canonical weight is the canonical product,
+// and the transform, being linear, maps canonical inputs to canonical outputs.
+#include <cub/cub.cuh>
 #include <algorithm>
 #include <cstring>
 #include <string>
 #include "../../include/b2groth.h"
 #include "msm.cuh"
+#include "ntt.cuh"
+#include "setup.cuh"
 #include "util.cuh"
 #include "verify.cuh"
 
@@ -89,10 +103,10 @@ struct MsmHold {
     ~MsmHold() { cudaStreamSynchronize(st); powers_msm_free(m); }
 };
 
-// one pass over `count` host points: with bad, the point rules (gen: point 0 must be the generator); with msm,
-// msm->acc = sum_i rho^i X_i
+// one pass over `count` host points: with bad, the point rules (b2g_powers_check's, gen: point 0 must be the generator; with
+// loose, b2g_setup_check's); with msm, msm->acc = sum_i k_i X_i, k_i = rho^(start + i) or, with scalars (device), scalars[i]
 static void powers_pass(Staging& sg, PowersMsm* msm, bool g2, const void* host, uint64_t count, bool gen, unsigned long long* bad,
-                        const fe* rho) {
+                        const fe* rho, bool loose = false, uint64_t start = 0, const fe* scalars = nullptr) {
     const size_t row = g2 ? 128 : 64;
     if (msm) powers_msm_reset(*msm, sg.st);
     uint64_t k = 0;
@@ -105,8 +119,9 @@ static void powers_pass(Staging& sg, PowersMsm* msm, bool g2, const void* host, 
         CUDA_CHECK(cudaMemcpyAsync(sg.dev[b], sg.host[b], (size_t)cnt * row, cudaMemcpyHostToDevice, sg.cp));
         CUDA_CHECK(cudaEventRecord(sg.copied[b], sg.cp));
         CUDA_CHECK(cudaStreamWaitEvent(sg.st, sg.copied[b], 0));
-        if (bad) powers_rules(g2, sg.dev[b], cnt, off, gen, bad, sg.st);
-        if (msm) powers_msm_slice(*msm, sg.dev[b], cnt, off, rho, sg.st);
+        if (bad && loose) setup_rules(g2, sg.dev[b], cnt, off, bad, sg.st);
+        else if (bad) powers_rules(g2, sg.dev[b], cnt, off, gen, bad, sg.st);
+        if (msm) powers_msm_slice(*msm, sg.dev[b], cnt, start + off, rho, sg.st, scalars ? scalars + off : nullptr);
         CUDA_CHECK(cudaEventRecord(sg.used[b], sg.st));
     }
 }
@@ -203,6 +218,247 @@ static void powers_check_run(b2g_ctx* ctx, const b2g_powers_desc* pw, uint32_t l
     out->rule = verdict ? 0 : 6;
 }
 
+// ---------------------------------------------------------------------------------------------- b2g_setup_check
+// mont[0] = rho, mont[1] = sigma, mont[2] = 1/2 (Montgomery) from canon = rho, sigma
+__global__ void check_consts_kernel(const fe* __restrict__ canon, fe* __restrict__ mont) {
+    if (threadIdx.x != 0 || blockIdx.x != 0) return;
+    fe two = fe_zero(); two.l[0] = 2;
+    mont[0] = Fr::from_canonical(canon[0]);
+    mont[1] = Fr::from_canonical(canon[1]);
+    mont[2] = Fr::inv(Fr::from_canonical(two));
+}
+
+// prod[k] = val[k] w[col[k]] (canonical) and row[k] = the row of nonzero k, by binary search in rowptr
+__global__ void __launch_bounds__(256) check_products_kernel(uint32_t nnz, uint32_t m, const uint32_t* __restrict__ rowptr,
+                                                             const uint32_t* __restrict__ col, const fe* __restrict__ val,
+                                                             const fe* __restrict__ w, fe* __restrict__ prod, uint32_t* __restrict__ row) {
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= nnz) return;
+    uint32_t lo = 0, hi = m - 1;                         // the last row r with rowptr[r] <= k (rowptr[m] = nnz > k)
+    while (lo < hi) {
+        const uint32_t mid = lo + (hi - lo + 1) / 2;
+        if (rowptr[mid] <= k) lo = mid; else hi = mid - 1;
+    }
+    fe_store(&prod[k], Fr::mul(fe_load_nc(&val[k]), fe_load_nc(&w[col[k]])));
+    row[k] = lo;
+}
+
+// c[rows[i]] = agg[i] for the *runs rows that occur
+__global__ void __launch_bounds__(256) check_scatter_kernel(uint32_t nnz, const uint32_t* __restrict__ runs, const uint32_t* __restrict__ rows,
+                                                            const fe* __restrict__ agg, fe* __restrict__ c) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= nnz || i >= *runs) return;
+    fe_store(&c[rows[i]], fe_load(&agg[i]));
+}
+
+// the public-input rows of A': c[m + j] = w[j], j < ni
+__global__ void __launch_bounds__(256) check_public_rows_kernel(uint32_t ni, uint32_t m, const fe* __restrict__ w, fe* __restrict__ c) {
+    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j < ni) fe_store(&c[m + j], fe_load(&w[j]));
+}
+
+// E5's scalars h (2n - 1, canonical).  CircomReduction: t = iNTT_n(v) at v, h_k = t_k omega_2n^-k / 2 and h_(k+n) = -h_k with
+// omega_2n^-k = -tw[n - k] for k > 0; LibsnarkReduction: v = sigma^i, h_k = -v_k (k < n - 1), h_(n-1) = 0, h_(k+n) = v_k
+__global__ void __launch_bounds__(256) check_h_kernel(uint32_t n, int libsnark, const fe* __restrict__ v, const fe* __restrict__ tw,
+                                                      const fe* __restrict__ half, fe* __restrict__ h) {
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n) return;
+    fe lo, hi;
+    if (libsnark) {
+        hi = fe_load(&v[k]);
+        lo = k + 1 < n ? Fr::neg(hi) : fe_zero();
+    } else {
+        lo = Fr::mul(fe_load(&v[k]), *half);
+        if (k) lo = Fr::neg(Fr::mul(lo, fe_load_nc(&tw[n - k])));
+        hi = Fr::neg(lo);
+    }
+    fe_store(&h[k], lo);
+    if (k + 1 < n) fe_store(&h[n + k], hi);
+}
+
+struct FrSum {
+    __device__ __forceinline__ fe operator()(const fe& a, const fe& b) const { return Fr::add(a, b); }
+};
+
+static const char* const KEY_NAMES[12] = {"alpha_g1", "beta_g1", "delta_g1", "beta_g2", "gamma_g2", "delta_g2", "gamma_abc_g1", "a_query",
+                                          "b_g1_query", "b_g2_query", "l_query", "h_query"};
+
+static bool all_zero_bytes(const void* p, size_t n) {
+    const uint8_t* b = (const uint8_t*)p;
+    return std::all_of(b, b + n, [](uint8_t x) { return x == 0; });
+}
+
+// the small device buffer of a key check: its layout
+enum : size_t {
+    SK_SUMS = 0,                     // the SC_ records (verify.cuh)
+    SK_G1 = SC_BYTES,                // delta_1, T_0 (affine)
+    SK_G2 = SK_G1 + 2 * 64,          // gamma_2, delta_2, U_0 (affine)
+    SK_CH = SK_G2 + 3 * 128,         // rho, sigma (canonical)
+    SK_MONT = SK_CH + 2 * 32,        // rho, sigma, 1/2 (Montgomery)
+    SK_PW = SK_MONT + 3 * 32,        // the powers kernels' two words
+    SK_BAD = SK_PW + 2 * 32,         // the lowest failing index of the 5 ceremony arrays, then of the 12 key fields
+    SK_POINT = SK_BAD + 160,         // the point a failure names (128 B)
+    SK_WORD = SK_POINT + 128,        // the verdict, or the failing point's rule
+    SK_RUNS = SK_WORD + 4,
+    SK_BYTES = SK_RUNS + 4
+};
+
+static void setup_check_run(b2g_ctx* ctx, const b2g_mat_desc* d, const b2g_powers_desc* pw, const b2g_key_desc* key, const void* challenges,
+                            b2g_setup_report* out) {
+    if (!ctx || !d || !pw || !key || !challenges || !out) throw_error(B2G_E_SHAPE, "null pointer");
+    memset(out, 0, sizeof(*out));
+    const CtxView cv = ctx_view(ctx);
+    if (cv.proof_pending) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
+    const int logn = mat_desc_check(d, true);
+    const bool libsnark = d->reduction == B2G_REDUCTION_LIBSNARK;
+    if (!libsnark && logn > 26) throw_error(B2G_E_DOMAIN, "PolynomialDegreeTooLarge: a CircomReduction setup transforms over 2n points, so n must fit 2^26");
+    if (pw->log_size > 28 || logn > (int)pw->log_size)
+        throw_error(B2G_E_DOMAIN, "PolynomialDegreeTooLarge: the circuit's domain of 2^" + std::to_string(logn) +
+                                      " points exceeds the ceremony's 2^" + std::to_string(pw->log_size) + " powers");
+    if (!pw->tau_g1 || !pw->tau_g2 || !pw->alpha_tau_g1 || !pw->beta_tau_g1 || !pw->beta_g2) throw_error(B2G_E_SHAPE, "null powers array");
+    static const char* const CH_NAMES[2] = {"rho", "sigma"};
+    for (int k = 0; k < 2; k++)
+        if (!scalar_ok((const uint8_t*)challenges + 32 * k)) throw_error(B2G_E_INPUT, std::string("challenge ") + CH_NAMES[k] + " is 0 or >= r");
+    const void* fields[12] = {key->alpha_g1, key->beta_g1, key->delta_g1, key->beta_g2, key->gamma_g2, key->delta_g2,
+                              key->gamma_abc_g1, key->a_query, key->b_g1_query, key->b_g2_query, key->l_query, key->h_query};
+    const uint64_t counts[12] = {1, 1, 1, 1, 1, 1, key->n_ic, key->n_vars, key->n_vars, key->n_vars, key->n_l, key->n_h};
+    for (int f = 0; f < 12; f++)
+        if (counts[f] && !fields[f]) throw_error(B2G_E_SHAPE, std::string("null key field ") + KEY_NAMES[f]);
+    const uint32_t m = d->num_constraints, ni = d->num_inputs, nv = d->n_vars;
+    const uint32_t maxnnz = std::max(d->a_rowptr[m], std::max(d->b_rowptr[m], d->c_rowptr[m]));
+    if (maxnnz > (uint32_t)INT32_MAX) throw_error(B2G_E_DEVICE, "b2g_setup_check: more than 2^31 - 1 nonzeros in one matrix");
+    const uint32_t n = 1u << logn, nh = libsnark ? n - 1 : n;
+    out->ok = 0;
+
+    // the counts, then the fields snarkjs copies from the ceremony
+    const std::pair<uint32_t, uint32_t> shapes[4] = {{7, nv}, {6, ni}, {10, nv - ni}, {11, nh}};
+    const uint32_t have[4] = {key->n_vars, key->n_ic, key->n_l, key->n_h};
+    for (int k = 0; k < 4; k++)
+        if (have[k] != shapes[k].second) { out->rule = 6; out->field = (uint8_t)shapes[k].first; out->index = shapes[k].second; return; }
+    const std::pair<const void*, size_t> same[4] = {{pw->alpha_tau_g1, 64}, {pw->beta_tau_g1, 64}, {pw->beta_g2, 128}, {pw->tau_g2, 128}};
+    const int same_field[4] = {0, 1, 3, 4};
+    for (int k = 0; k < 4; k++)
+        if (memcmp(fields[same_field[k]], same[k].first, same[k].second)) { out->rule = 7; out->field = (uint8_t)same_field[k]; return; }
+
+    DevGuard g(cv.device);
+    cudaStream_t st = cv.st;
+    DevBuf v(SK_BYTES);
+    uint8_t* V = v.p;
+    // the scalars: w (N), v then t (n), s^A, s^B, s^C (n each), h (2n; also the transforms' scratch before it holds h)
+    DevBuf sc(((size_t)nv + 6 * (size_t)n) * sizeof(fe));
+    fe *d_w = (fe*)sc.p, *d_v = d_w + nv, *d_s[3] = {d_v + n, d_v + 2 * (size_t)n, d_v + 3 * (size_t)n}, *d_h = d_v + 4 * (size_t)n;
+    fe* d_mont = (fe*)(V + SK_MONT);
+    unsigned long long* d_bad = (unsigned long long*)(V + SK_BAD);
+    CUDA_CHECK(cudaMemsetAsync(V, 0, SK_BYTES, st));
+    CUDA_CHECK(cudaMemsetAsync(d_bad, 0xff, 17 * 8, st));
+    CUDA_CHECK(cudaMemcpyAsync(V + SK_CH, challenges, 64, cudaMemcpyHostToDevice, st));
+    check_consts_kernel<<<1, 1, 0, st>>>((const fe*)(V + SK_CH), d_mont);
+    g_launch_count += 1;
+    CUDA_CHECK(cudaGetLastError());
+    powers_scalars(d_mont, 0, nv, (fe*)(V + SK_PW), d_w, st);
+    powers_scalars(d_mont + 1, 0, n, (fe*)(V + SK_PW), d_v, st);
+
+    // c = A'w, Bw, Cw by rows
+    CUDA_CHECK(cudaMemsetAsync(d_s[0], 0, 3 * (size_t)n * sizeof(fe), st));
+    if (maxnnz) {
+        DevBuf rowptr(((size_t)m + 1) * 4), col((size_t)maxnnz * 4), val((size_t)maxnnz * sizeof(fe)), rows((size_t)maxnnz * 4),
+            uniq((size_t)maxnnz * 4), prod((size_t)maxnnz * sizeof(fe)), agg((size_t)maxnnz * sizeof(fe));
+        uint32_t* d_runs = (uint32_t*)(V + SK_RUNS);
+        size_t temp_bytes = 0;
+        CUDA_CHECK(cub::DeviceReduce::ReduceByKey(nullptr, temp_bytes, (uint32_t*)rows.p, (uint32_t*)uniq.p, (fe*)prod.p, (fe*)agg.p,
+                                                  d_runs, FrSum(), (int)maxnnz, st));
+        DevBuf temp(temp_bytes);
+        const uint32_t* rowptrs[3] = {d->a_rowptr, d->b_rowptr, d->c_rowptr};
+        const uint32_t* cols[3] = {d->a_col, d->b_col, d->c_col};
+        const void* vals[3] = {d->a_val, d->b_val, d->c_val};
+        for (int x = 0; x < 3; x++) {
+            const uint32_t nnz = rowptrs[x][m];
+            if (!nnz) continue;
+            const unsigned blocks = (nnz + 255) / 256;
+            CUDA_CHECK(cudaMemcpyAsync(rowptr.p, rowptrs[x], ((size_t)m + 1) * 4, cudaMemcpyHostToDevice, st));
+            CUDA_CHECK(cudaMemcpyAsync(col.p, cols[x], (size_t)nnz * 4, cudaMemcpyHostToDevice, st));
+            CUDA_CHECK(cudaMemcpyAsync(val.p, vals[x], (size_t)nnz * sizeof(fe), cudaMemcpyHostToDevice, st));
+            check_products_kernel<<<blocks, 256, 0, st>>>(nnz, m, (const uint32_t*)rowptr.p, (const uint32_t*)col.p, (const fe*)val.p, d_w,
+                                                          (fe*)prod.p, (uint32_t*)rows.p);
+            size_t bytes = temp_bytes;
+            CUDA_CHECK(cub::DeviceReduce::ReduceByKey(temp.p, bytes, (uint32_t*)rows.p, (uint32_t*)uniq.p, (fe*)prod.p, (fe*)agg.p, d_runs,
+                                                      FrSum(), (int)nnz, st));
+            check_scatter_kernel<<<blocks, 256, 0, st>>>(nnz, d_runs, (const uint32_t*)uniq.p, (const fe*)agg.p, d_s[x]);
+            g_launch_count += 2;
+            CUDA_CHECK(cudaGetLastError());
+        }
+        CUDA_CHECK(cudaStreamSynchronize(st));                         // the buffers of this block are freed at its end
+    }
+    check_public_rows_kernel<<<(ni + 255) / 256, 256, 0, st>>>(ni, m, d_w, d_s[0]);
+    g_launch_count += 1;
+    CUDA_CHECK(cudaGetLastError());
+
+    // s = iNTT_n(c), in place; then h
+    NttDomain dom;
+    struct DomGuard { NttDomain& d; ~DomGuard() { ntt_domain_destroy(d); } } dg{dom};
+    ntt_domain_create(dom, logn, st);
+    for (int x = 0; x < 3; x++) ntt_plain(dom, d_s[x], d_h, true, st);
+    if (!libsnark) ntt_plain(dom, d_v, d_h, true, st);
+    check_h_kernel<<<(n + 255) / 256, 256, 0, st>>>(n, libsnark ? 1 : 0, d_v, dom.tw, d_mont + 2, d_h);
+    g_launch_count += 1;
+    CUDA_CHECK(cudaGetLastError());
+
+    // the streamed passes: ceremony arrays (rules on the prefix b2g_setup_from_powers reads), then the key's fields
+    const uint64_t g1_most = std::max<uint64_t>(2 * (uint64_t)n - 1, nv), g2_most = std::max<uint64_t>(n, nv);
+    MsmHold h1(false, g1_most, st), h2(true, g2_most, st);
+    Staging sg(std::max<size_t>(std::min<uint64_t>(g1_most, POWERS_SLICE) * 64, std::min<uint64_t>(g2_most, POWERS_SLICE) * 128), st);
+    const void* T = pw->tau_g1;
+    struct Pass { const void* host; uint64_t count; bool g2; int bad; const fe* rho; uint64_t start; const fe* scalars; size_t sum; };
+    const fe *rho = d_mont, *sigma = d_mont + 1;
+    const Pass passes[20] = {
+        {T, 2 * (uint64_t)n - 1, false, 0, nullptr, 0, d_h, SC_RH}, {pw->tau_g2, n, true, 1, nullptr, 0, d_s[1], SC_RB2},
+        {pw->alpha_tau_g1, n, false, 2, nullptr, 0, d_s[1], SC_RAL}, {pw->beta_tau_g1, n, false, 3, nullptr, 0, d_s[0], SC_RBE},
+        {pw->beta_g2, 1, true, 4, nullptr, 0, nullptr, 0},
+        {T, n, false, -1, nullptr, 0, d_s[0], SC_RA}, {T, n, false, -1, nullptr, 0, d_s[1], SC_RB1}, {T, n, false, -1, nullptr, 0, d_s[2], SC_RC},
+        {fields[0], 1, false, 5, nullptr, 0, nullptr, 0}, {fields[1], 1, false, 6, nullptr, 0, nullptr, 0},
+        {fields[2], 1, false, 7, nullptr, 0, nullptr, 0}, {fields[3], 1, true, 8, nullptr, 0, nullptr, 0},
+        {fields[4], 1, true, 9, nullptr, 0, nullptr, 0}, {fields[5], 1, true, 10, nullptr, 0, nullptr, 0},
+        {fields[6], ni, false, 11, rho, 0, nullptr, SC_KIC}, {fields[7], nv, false, 12, rho, 0, nullptr, SC_KA},
+        {fields[8], nv, false, 13, rho, 0, nullptr, SC_KB1}, {fields[9], nv, true, 14, rho, 0, nullptr, SC_KB2},
+        {fields[10], nv - ni, false, 15, rho, ni, nullptr, SC_KL}, {fields[11], nh, false, 16, sigma, 0, nullptr, SC_KH}};
+    for (const Pass& p : passes) {
+        const bool sum = p.rho || p.scalars;
+        PowersMsm* msm = sum ? (p.g2 ? &h2.m : &h1.m) : nullptr;
+        powers_pass(sg, msm, p.g2, p.host, p.count, false, p.bad >= 0 ? d_bad + p.bad : nullptr, p.rho, true, p.start, p.scalars);
+        if (msm) CUDA_CHECK(cudaMemcpyAsync(V + SK_SUMS + p.sum, msm->acc, p.g2 ? 256 : 128, cudaMemcpyDeviceToDevice, st));
+    }
+    uint64_t bad[17];
+    CUDA_CHECK(cudaMemcpyAsync(bad, d_bad, sizeof(bad), cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    // the points that must not be at infinity: tau_g1[0], tau_g2[0], delta_g1, delta_g2
+    if (all_zero_bytes(T, 64)) bad[0] = 0;
+    if (all_zero_bytes(pw->tau_g2, 128)) bad[1] = 0;
+    if (all_zero_bytes(key->delta_g1, 64)) bad[7] = 0;
+    if (all_zero_bytes(key->delta_g2, 128)) bad[10] = 0;
+    // the first failing point in pass order, which is report order: the ceremony's arrays, then the key's fields
+    for (const Pass& p : passes) {
+        if (p.bad < 0 || bad[p.bad] >= p.count) continue;
+        const size_t row = p.g2 ? 128 : 64;
+        CUDA_CHECK(cudaMemcpyAsync(V + SK_POINT, (const uint8_t*)p.host + bad[p.bad] * row, row, cudaMemcpyHostToDevice, st));
+        const uint32_t rule = powers_point_rule(p.g2, V + SK_POINT, false, (uint32_t*)(V + SK_WORD), st);
+        if (!rule) throw_error(B2G_E_DEVICE, "b2g_setup_check: the point rules disagree on point " + std::to_string(bad[p.bad]));
+        out->rule = (uint8_t)rule; out->side = p.bad < 5 ? 1 : 0; out->field = (uint8_t)(p.bad < 5 ? p.bad : p.bad - 5);
+        out->index = bad[p.bad];
+        return;
+    }
+
+    const std::pair<const void*, size_t> pts[5] = {{key->delta_g1, 64}, {T, 64}, {key->gamma_g2, 128}, {key->delta_g2, 128}, {pw->tau_g2, 128}};
+    for (int k = 0, off = 0; k < 5; off += (int)pts[k].second, k++)
+        CUDA_CHECK(cudaMemcpyAsync(V + SK_G1 + off, pts[k].first, pts[k].second, cudaMemcpyHostToDevice, st));
+    setup_check_verdict(V + SK_SUMS, V + SK_G1, V + SK_G2, (uint32_t*)(V + SK_WORD), st);
+    uint32_t verdict = 0;
+    CUDA_CHECK(cudaMemcpyAsync(&verdict, V + SK_WORD, 4, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    static const uint8_t EQ_FIELD[7] = {0, 7, 8, 9, 6, 11, 2};
+    if (verdict) { out->rule = 8; out->field = EQ_FIELD[verdict > 6 ? 0 : verdict]; return; }
+    out->ok = 1;
+}
+
 }  // namespace b2g
 
 extern "C" {
@@ -213,6 +469,11 @@ int b2g_powers_msm(b2g_ctx* ctx, int g2, size_t n, const void* bases, const void
 
 int b2g_powers_check(b2g_ctx* ctx, const b2g_powers_desc* powers, uint32_t log_n, const void* challenges, b2g_powers_report* out) {
     return b2g::guarded_clear([&] { b2g::powers_check_run(ctx, powers, log_n, challenges, out); });
+}
+
+int b2g_setup_check(b2g_ctx* ctx, const b2g_mat_desc* circuit, const b2g_powers_desc* powers, const b2g_key_desc* key,
+                    const void* challenges, b2g_setup_report* report) {
+    return b2g::guarded_clear([&] { b2g::setup_check_run(ctx, circuit, powers, key, challenges, report); });
 }
 
 }  // extern "C"

@@ -1252,15 +1252,16 @@ __global__ void setup_generators_kernel(const void* __restrict__ g1, const void*
     }
 }
 
-// bad = the lowest point with a coordinate >= p or off its curve (infinity = zeros passes)
+// bad = the lowest base + i whose point has a coordinate >= p or lies off its curve (infinity = zeros passes)
 template <class C, class F>
-__global__ void __launch_bounds__(128) points_curve_kernel(const uint8_t* __restrict__ pts, uint32_t n, unsigned long long* __restrict__ bad) {
+__global__ void __launch_bounds__(128) points_curve_kernel(const uint8_t* __restrict__ pts, uint32_t n, uint64_t base,
+                                                           unsigned long long* __restrict__ bad) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     constexpr int WORDS = 2 * Bytes<F>::ELEM / 32;
     bool ok = true;
     for (int k = 0; k < WORDS; k++) ok &= fe_below_p(fe_load(pts + ((size_t)i * WORDS + k) * 32));
-    if (!ok || !aff_on_curve<C, F>(aff_load<F>(pts, i))) atomicMin(bad, (unsigned long long)i);
+    if (!ok || !aff_on_curve<C, F>(aff_load<F>(pts, i))) atomicMin(bad, (unsigned long long)(base + i));
 }
 
 uint64_t points_check(bool g2, const void* pts, size_t n, bool subgroup, cudaStream_t st, int* why) {
@@ -1272,8 +1273,8 @@ uint64_t points_check(bool g2, const void* pts, size_t n, bool subgroup, cudaStr
     const unsigned blocks = (unsigned)((n + 127) / 128);
     cudaError_t e = cudaMemcpyAsync(d_bad, bad, sizeof(bad), cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) {
-        if (g2) points_curve_kernel<G2, Fq2><<<blocks, 128, 0, st>>>((const uint8_t*)pts, (uint32_t)n, d_bad);
-        else points_curve_kernel<G1, Fq><<<blocks, 128, 0, st>>>((const uint8_t*)pts, (uint32_t)n, d_bad);
+        if (g2) points_curve_kernel<G2, Fq2><<<blocks, 128, 0, st>>>((const uint8_t*)pts, (uint32_t)n, 0, d_bad);
+        else points_curve_kernel<G1, Fq><<<blocks, 128, 0, st>>>((const uint8_t*)pts, (uint32_t)n, 0, d_bad);
         if (g2 && subgroup) points_g2_subgroup_kernel<<<blocks, 128, 0, st>>>((const uint8_t*)pts, (uint32_t)n, 0, d_bad + 1);
         g_launch_count += g2 && subgroup ? 2 : 1;
         e = cudaGetLastError();
@@ -1435,6 +1436,73 @@ __global__ void __launch_bounds__(32) powers_verdict_kernel(const uint8_t* __res
 
 void powers_verdict(const void* sums, const void* g1, const void* g2, const void* ch, uint32_t log_n, uint32_t* verdict, cudaStream_t st) {
     powers_verdict_kernel<<<1, 32, 0, st>>>((const uint8_t*)sums, (const uint8_t*)g1, (const uint8_t*)g2, (const fe*)ch, log_n, verdict);
+    g_launch_count += 1;
+    CUDA_CHECK(cudaGetLastError());
+}
+
+// ---------------------------------------------------------------------------------------------- proving-key check
+void setup_rules(bool g2, const void* pts, uint32_t n, uint64_t base, unsigned long long* bad, cudaStream_t st) {
+    if (n == 0) return;
+    const unsigned blocks = (n + 127) / 128;
+    if (g2) {
+        points_curve_kernel<G2, Fq2><<<blocks, 128, 0, st>>>((const uint8_t*)pts, n, base, bad);
+        points_g2_subgroup_kernel<<<blocks, 128, 0, st>>>((const uint8_t*)pts, n, base, bad);
+    } else {
+        points_curve_kernel<G1, Fq><<<blocks, 128, 0, st>>>((const uint8_t*)pts, n, base, bad);
+    }
+    g_launch_count += g2 ? 2 : 1;
+    CUDA_CHECK(cudaGetLastError());
+}
+
+// b2g_setup_check's equations, one block of 32 threads: *verdict = the lowest failing equation (1-6), or 0.  E1-E3 compare the
+// XYZZ sums; the seven Miller loops of E4-E6 run on seven threads and the three final exponentiations on three.
+__global__ void __launch_bounds__(32) setup_check_verdict_kernel(const uint8_t* __restrict__ sums, const uint8_t* __restrict__ g1,
+                                                                 const uint8_t* __restrict__ g2, uint32_t* __restrict__ verdict) {
+    __shared__ G1::Aff a1[7];
+    __shared__ G2::Aff a2[7];
+    __shared__ fe12 f[7];
+    __shared__ uint32_t good[6];
+    const uint32_t t = threadIdx.x;
+    if (t == 0) good[0] = G1::pt_eq(pt_load<Fq>(sums + SC_KA, 0), pt_load<Fq>(sums + SC_RA, 0));
+    else if (t == 1) good[1] = G1::pt_eq(pt_load<Fq>(sums + SC_KB1, 0), pt_load<Fq>(sums + SC_RB1, 0));
+    else if (t == 2) good[2] = G2::pt_eq(pt_load<Fq2>(sums + SC_KB2, 0), pt_load<Fq2>(sums + SC_RB2, 0));
+    else if (t == 3) a1[0] = G1::to_affine(pt_load<Fq>(sums + SC_KIC, 0));
+    else if (t == 4) a1[1] = G1::to_affine(pt_load<Fq>(sums + SC_KL, 0));
+    else if (t == 5) {
+        G1::Pt r = pt_load<Fq>(sums + SC_RBE, 0);
+        G1::add(r, pt_load<Fq>(sums + SC_RAL, 0));
+        G1::add(r, pt_load<Fq>(sums + SC_RC, 0));
+        a1[2] = G1::to_affine(G1::neg(r));
+    } else if (t == 6) a1[3] = G1::to_affine(pt_load<Fq>(sums + SC_KH, 0));
+    else if (t == 7) a1[4] = G1::to_affine(G1::neg(pt_load<Fq>(sums + SC_RH, 0)));
+    else if (t == 8) a1[5] = aff_load<Fq>(g1, 0);                                  // delta_1
+    else if (t == 9) { G1::Aff p = aff_load<Fq>(g1, 1); if (!G1::aff_is_inf(p)) p.y = Fq::neg(p.y); a1[6] = p; }   // -T_0
+    // the G2 side of each pair: gamma_2, delta_2, U_0 | delta_2, U_0 | U_0, delta_2
+    if (t < 7) a2[t] = aff_load<Fq2>(g2, t == 0 ? 0 : t == 1 || t == 3 || t == 6 ? 1 : 2);
+    __syncthreads();
+    if (t < 7) {
+        fe12 r;
+        miller_loop(r, !G1::aff_is_inf(a1[t]) && !G2::aff_is_inf(a2[t]), a1[t], a2[t], 0, nullptr, nullptr);
+        f[t] = r;
+    }
+    __syncthreads();
+    if (t < 3) {                                   // E4: pairs 0-2, E5: pairs 3-4, E6: pairs 5-6
+        const int first = t == 0 ? 0 : t == 1 ? 3 : 5, last = t == 0 ? 3 : t == 1 ? 5 : 7;
+        fe12 prod = f[first], e;
+        for (int k = first + 1; k < last; k++) Fq12::mul(prod, prod, f[k]);
+        Fq12::final_exponentiation(e, prod);
+        good[3 + t] = Fq12::eq(e, Fq12::one()) ? 1u : 0u;
+    }
+    __syncthreads();
+    if (t == 0) {
+        uint32_t v = 0;
+        for (int k = 5; k >= 0; k--) if (!good[k]) v = k + 1;
+        *verdict = v;
+    }
+}
+
+void setup_check_verdict(const void* sums, const void* g1, const void* g2, uint32_t* verdict, cudaStream_t st) {
+    setup_check_verdict_kernel<<<1, 32, 0, st>>>((const uint8_t*)sums, (const uint8_t*)g1, (const uint8_t*)g2, verdict);
     g_launch_count += 1;
     CUDA_CHECK(cudaGetLastError());
 }

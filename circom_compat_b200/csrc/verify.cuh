@@ -41,4 +41,19 @@ uint32_t powers_point_rule(bool g2, const void* pt, bool gen, uint32_t* scratch,
 // ch = rho, sigma, pi, kappa, eps (32 B canonical each); all device.  Asynchronous.
 void powers_verdict(const void* sums, const void* g1, const void* g2, const void* ch, uint32_t log_n, uint32_t* verdict, cudaStream_t st);
 
+// b2g_setup_check's point rules over the n affine Montgomery points of a device slice whose first point has index `base` in its
+// array: atomicMin of the index of every point with a coordinate >= p, off its curve or, for G2, outside G2, into *bad (device).
+// Infinity passes.  Asynchronous.
+void setup_rules(bool g2, const void* pts, uint32_t n, uint64_t base, unsigned long long* bad, cudaStream_t st);
+// b2g_setup_check's sums, XYZZ records at these byte offsets of one device buffer of SC_BYTES (G1 128 B, G2 256 B): the key
+// side sum_j rho^j X_j of a_query, b_g1_query, b_g2_query, gamma_abc_g1, l_query (from rho^ni) and sum_i sigma^i h_query[i];
+// the ceremony side sum_k s_k Y_k of E1 (s^A T), E2 (s^B T), E3 (s^B U), E4 (s^A Be, s^B Al, s^C T) and E5 (h T)
+enum : size_t {
+    SC_KA = 0, SC_KB1 = 128, SC_KB2 = 256, SC_KIC = 512, SC_KL = 640, SC_KH = 768,
+    SC_RA = 896, SC_RB1 = 1024, SC_RB2 = 1152, SC_RBE = 1408, SC_RAL = 1536, SC_RC = 1664, SC_RH = 1792, SC_BYTES = 1920
+};
+// b2g_setup_check's equations E1-E6 (include/b2groth.h) into *verdict (device): the lowest failing equation 1-6, or 0.
+// sums: the SC_ records; g1 = delta_1, T_0; g2 = gamma_2, delta_2, U_0 (affine Montgomery); all device.  Asynchronous.
+void setup_check_verdict(const void* sums, const void* g1, const void* g2, uint32_t* verdict, cudaStream_t st);
+
 }  // namespace b2g

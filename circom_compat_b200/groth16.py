@@ -35,6 +35,8 @@
         <- snarkjs groth16 setup: a key from a powers-of-tau ceremony (ptau.read_ptau), gamma = delta = 1.
     Groth16.contribute(pk) / Groth16.verify_contribution(before, after)
         <- snarkjs zkey contribute / the delta checks of snarkjs zkey verify.
+    Groth16.verify_proving_key(circuit, powers, pk, matrices)
+        <- snarkjs zkey verify circuit.r1cs pot.ptau circuit.zkey: the key against its circuit and ceremony (b2g_setup_check).
 Arguments keep the reference's meaning; field elements are (n, 4) uint64 Montgomery limb arrays (fr_to_mont).
 """
 from __future__ import annotations
@@ -587,6 +589,39 @@ def _mont_points(points, g2: bool) -> np.ndarray:
     return np.frombuffer(b''.join(v.to_bytes(32, 'little') for v in vals), dtype='<u8').copy()
 
 
+def _circuit_desc(circuit, reduction):
+    """(b2g_mat_desc with C, the arrays it points into, n_vars, num_inputs, the domain size, the H query's size) of a
+    synth.Circuit or ConstraintMatrices with C, as the setup takes them"""
+    m, n_vars = (circuit.matrices(with_c=True), circuit.n_vars) if hasattr(circuit, 'matrices') else (circuit, circuit.n_vars)
+    d, keep = _mat_desc(m, n_vars, reduction.ID, with_c=True)
+    ni = m.num_instance_variables
+    if ni == 0 or ni > n_vars:
+        raise N.B2gError(N.B2G_E_SHAPE, "num_inputs out of range")
+    size = 1
+    while size < m.num_constraints + ni:
+        size <<= 1
+    return d, keep, n_vars, ni, size, size - 1 if reduction.ID == N.REDUCTION_LIBSNARK else size
+
+
+def _powers_desc(powers, size):
+    """(b2g_powers_desc, the arrays it points into) of the prefix of a ceremony a domain of `size` points reads, as views where
+    they can be; ValueError when an array is shorter.  A domain above the ceremony's power is left for the library to refuse
+    before it reads any point."""
+    from .ptau import ARRAYS, Powers
+    log_n = size.bit_length() - 1
+    pd = N.PowersDesc()
+    pd.log_size = int(powers.power)
+    arrays = {}
+    if log_n <= pd.log_size:
+        pre = Powers(int(powers.power), int(getattr(powers, 'ceremony_power', powers.power)),
+                     *(np.asarray(getattr(powers, k)) for k in ARRAYS)).prefix(log_n)
+        for name in ARRAYS:
+            a = _c(getattr(pre, name))
+            arrays[name] = a
+            setattr(pd, name, a.ctypes.data)
+    return pd, arrays
+
+
 def _delta_desc(arrs) -> 'N.DeltaKey':
     d = N.DeltaKey()
     d.n_l, d.n_h = arrs['l_query'].size // 8, arrs['h_query'].size // 8
@@ -756,29 +791,8 @@ class Groth16:
         generate_parameters_with_qap takes it) from a powers-of-tau ceremony (ptau.read_ptau, or any object with the same
         fields), with gamma = delta = 1.  Only the prefix of each array the circuit's domain needs is read."""
         ctx = ctx or default_context()
-        m, n_vars = (circuit.matrices(with_c=True), circuit.n_vars) if hasattr(circuit, 'matrices') else (circuit, circuit.n_vars)
-        d, keep = _mat_desc(m, n_vars, reduction.ID, with_c=True)
-        ni = m.num_instance_variables
-        if ni == 0 or ni > n_vars:
-            raise N.B2gError(N.B2G_E_SHAPE, "num_inputs out of range")
-        size = 1
-        while size < m.num_constraints + ni:
-            size <<= 1
-        nh = size - 1 if reduction.ID == N.REDUCTION_LIBSNARK else size
-        from .ptau import Powers
-        log_n = size.bit_length() - 1
-        pd = N.PowersDesc()
-        pd.log_size = int(powers.power)
-        arrays = {}
-        if log_n <= pd.log_size:                  # else the library refuses the domain before it reads any point
-            # checks that each array holds what the domain reads (ValueError otherwise), as views where they can be
-            pre = Powers(int(powers.power), int(getattr(powers, 'ceremony_power', powers.power)),
-                         *(np.asarray(getattr(powers, k)) for k in ('tau_g1', 'tau_g2', 'alpha_tau_g1', 'beta_tau_g1', 'beta_g2')))
-            pre = pre.prefix(log_n)
-            for name in ('tau_g1', 'tau_g2', 'alpha_tau_g1', 'beta_tau_g1', 'beta_g2'):
-                a = _c(getattr(pre, name))
-                arrays[name] = a
-                setattr(pd, name, a.ctypes.data)
+        d, keep, n_vars, ni, size, nh = _circuit_desc(circuit, reduction)
+        pd, arrays = _powers_desc(powers, size)
         shapes = {'alpha_g1': (1, 8), 'beta_g1': (1, 8), 'delta_g1': (1, 8), 'beta_g2': (1, 16), 'gamma_g2': (1, 16), 'delta_g2': (1, 16),
                   'gamma_abc_g1': (ni, 8), 'a_query': (n_vars, 8), 'b_g1_query': (n_vars, 8), 'b_g2_query': (n_vars, 16),
                   'l_query': (n_vars - ni, 8), 'h_query': (nh, 8)}
@@ -790,6 +804,47 @@ class Groth16:
         return ProvingKey(n_vars, ni - 1, nh, arrs['alpha_g1'], arrs['beta_g1'], arrs['beta_g2'], arrs['gamma_g2'], arrs['delta_g1'],
                           arrs['delta_g2'], arrs['gamma_abc_g1'], arrs['a_query'], arrs['b_g1_query'], arrs['b_g2_query'],
                           arrs['l_query'], arrs['h_query'])
+
+    @staticmethod
+    def verify_proving_key(circuit, powers, pk: ProvingKey, matrices: ConstraintMatrices = None, reduction=CircomReduction,
+                           ctx: Context = None, challenges=None):
+        """`snarkjs zkey verify circuit.r1cs pot.ptau circuit.zkey` on the GPU (b2g_setup_check), without snarkjs's transcript:
+        whether `pk` is the key generate_parameters_from_powers_of_tau makes from `circuit` and `powers`, followed by any chain
+        of `contribute` calls.  `circuit` and `powers` are what that call takes; `matrices`, the ConstraintMatrices read_zkey
+        returns with the key, must then hold the circuit's A and B (compared on the host, row by row in canonical form) and its
+        counts.  The key and the ceremony are read from host memory once, memory-mapped views in place.  The challenges rho
+        and sigma (in [1, r)) are drawn with `secrets` unless given.  Returns a keycheck.SetupCheck: truthy when the key
+        passes, .reason naming the first failing check.  A key that is not the circuit's passes with probability at most
+        max(n_vars, n) / (r - 1) when the challenges are drawn after the key and the ceremony are fixed."""
+        import secrets
+        from .keycheck import KEY_FIELDS, SetupCheck, matrices_reason, report_reason, shape_reason
+        d, keep, n_vars, ni, size, nh = _circuit_desc(circuit, reduction)
+        if matrices is not None:
+            why = matrices_reason(circuit.matrices() if hasattr(circuit, 'matrices') else circuit, matrices)
+            if why:
+                return SetupCheck(False, why)
+        arrs = {k: _c(getattr(pk, k)).reshape(-1, 16 if k in ('beta_g2', 'gamma_g2', 'delta_g2', 'b_g2_query') else 8)
+                for k in KEY_FIELDS}
+        want = {'alpha_g1': 1, 'beta_g1': 1, 'delta_g1': 1, 'beta_g2': 1, 'gamma_g2': 1, 'delta_g2': 1, 'gamma_abc_g1': ni,
+                'a_query': n_vars, 'b_g1_query': n_vars, 'b_g2_query': n_vars, 'l_query': n_vars - ni, 'h_query': nh}
+        for k in KEY_FIELDS:
+            if arrs[k].shape[0] != want[k]:
+                return SetupCheck(False, shape_reason(k, arrs[k].shape[0], want[k], reduction.__name__, size))
+        pd, arrays = _powers_desc(powers, size)
+        if challenges is None:
+            challenges = [1 + secrets.randbelow(R_MOD - 1) for _ in range(2)]
+        challenges = [int(c) for c in challenges]
+        if len(challenges) != 2 or not all(0 <= c < 1 << 256 for c in challenges):
+            raise ValueError("verify_proving_key: two challenges (rho, sigma), each below 2^256")
+        cb = np.frombuffer(b''.join(c.to_bytes(32, 'little') for c in challenges), dtype=np.uint8).copy()
+        kd = N.KeyDesc()
+        kd.n_vars, kd.n_ic, kd.n_l, kd.n_h = n_vars, ni, n_vars - ni, nh
+        for k, a in arrs.items():
+            setattr(kd, k, a.ctypes.data if a.size else None)
+        rep = N.SetupReport()
+        ctx = ctx or default_context()
+        N.check(N.lib().b2g_setup_check(ctx._h, C.byref(d), C.byref(pd), C.byref(kd), _ptr(cb), C.byref(rep)))
+        return SetupCheck(True) if rep.ok else SetupCheck(False, report_reason(rep))
 
     @staticmethod
     def contribute(pk: ProvingKey, rng=None, ctx: Context = None, x=None) -> ProvingKey:

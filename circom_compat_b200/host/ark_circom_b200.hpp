@@ -28,6 +28,7 @@
 //   ark_circom::read_ptau + Groth16::generate_parameters_from_powers_of_tau <- snarkjs groth16 setup (a key from a ceremony)
 //   ark_circom::Groth16::contribute / verify_contribution <- snarkjs zkey contribute / the delta checks of snarkjs zkey verify
 //   ark_circom::Groth16::verify_powers_of_tau <- the algebraic checks of snarkjs powersoftau verify
+//   ark_circom::Groth16::verify_proving_key <- snarkjs zkey verify: a key against its circuit and ceremony
 //   ark_circom::read_wtns                              <- snarkjs .wtns (test-vectors/circuit2_js/witness.wtns; the reference
 //                                                         computes witnesses with WASM instead, out of scope here)
 // Parsing and key handling stay on the host; every field/curve operation of the proof runs in libb2groth.so.
@@ -563,10 +564,40 @@ struct PowersCheck {
     }
 };
 
+// The verdict of Groth16T::verify_proving_key (b2g_setup_check): ok, or the reason of the failure in the words of
+// keycheck.py ("l_query[17]: off the curve", "alpha_g1 is not the ceremony's", "b_g2_query does not match the circuit and
+// ceremony", "matrix A differs from the circuit at row 17").
+struct SetupCheck {
+    bool ok = false;
+    std::string why;
+    explicit operator bool() const { return ok; }
+    const std::string& reason() const { return why; }
+};
+
+namespace detail {
+// the rows of a matrix sorted by column, duplicates summed mod r, zeros dropped (Montgomery values compare as canonical ones)
+inline std::vector<std::vector<std::pair<size_t, Fr>>> canonical_rows(const Matrix& m, size_t rows) {
+    std::vector<std::vector<std::pair<size_t, Fr>>> out(rows);
+    for (size_t r = 0; r < rows && r < m.size(); r++) {
+        std::map<size_t, Fr> acc;
+        for (const auto& e : m[r]) {
+            Fr& a = acc[e.second];
+            u128 c = 0;
+            uint64_t t[4];
+            for (int i = 0; i < 4; i++) { c += (u128)a.l[i] + e.first.l[i]; t[i] = (uint64_t)c; c >>= 64; }
+            if (c || geq(t, FR_P)) { u128 br = 0; for (int i = 0; i < 4; i++) { u128 d = (u128)t[i] - FR_P[i] - (uint64_t)br; t[i] = (uint64_t)d; br = (d >> 64) & 1; } }
+            memcpy(a.l, t, 32);
+        }
+        for (const auto& kv : acc) if (!kv.second.is_zero()) out[r].push_back(kv);
+    }
+    return out;
+}
+}  // namespace detail
+
 // the five challenges of the ceremony check (rho, sigma, pi, kappa, eps), uniform in [1, r), from std::random_device
-inline std::vector<BigInt256> powers_challenges() {
+inline std::vector<BigInt256> powers_challenges(size_t count = 5) {
     std::random_device rd;
-    std::vector<BigInt256> c(5);
+    std::vector<BigInt256> c(count);
     for (BigInt256& b : c) {
         do {
             for (int t = 0; t < 4; t++) b.l[t] = ((uint64_t)rd() << 32) | rd();
@@ -990,6 +1021,94 @@ struct Groth16T {                                       // Groth16::<Bn254, QAP>
         r.ok = rep.ok != 0;
         r.rule = rep.rule;
         if (!r.ok && rep.rule != 6) { r.array = arrays[rep.array]; r.index = rep.index; }
+        return r;
+    }
+
+    // `snarkjs zkey verify circuit.r1cs pot.ptau circuit.zkey` without its transcript (b2g_setup_check): whether pk is the key
+    // generate_parameters_from_powers_of_tau makes from the matrices (with C) and the ceremony, followed by any chain of
+    // contribute calls.  zkey_matrices, the matrices read_zkey returns with the key, must then hold the circuit's A and B
+    // (compared row by row in canonical form) and its counts.  The challenges rho and sigma come from std::random_device, drawn
+    // after the key is fixed, unless two are given (canonical, in [1, r)).  Throws std::invalid_argument when the powers hold
+    // fewer points than the circuit's domain reads.
+    static SetupCheck verify_proving_key(const ConstraintMatrices& matrices, const Powers& powers, const ProvingKey& pk,
+                                         const ConstraintMatrices* zkey_matrices = nullptr, Gpu& gpu = Gpu::instance(),
+                                         const std::vector<BigInt256>* challenges = nullptr) {
+        const size_t ni = matrices.num_instance_variables, nv = ni + matrices.num_witness_variables, m = matrices.num_constraints;
+        if (ni == 0) throw SynthesisError("verify_proving_key: no instance variable");
+        if (m && matrices.c.empty()) throw SynthesisError("verify_proving_key needs the C matrix (R1CS route); zkey matrices have none");
+        SetupCheck r;
+        if (zkey_matrices) {
+            const ConstraintMatrices& z = *zkey_matrices;
+            const size_t have[3] = {z.num_instance_variables, z.num_constraints, z.num_instance_variables + z.num_witness_variables};
+            const size_t want[3] = {ni, m, nv};
+            static const char* const what[3] = {"num_inputs", "num_constraints", "n_vars"};
+            for (int k = 0; k < 3; k++)
+                if (have[k] != want[k]) {
+                    r.why = std::string("the matrices' ") + what[k] + " " + std::to_string(have[k]) + " differs from the circuit's " + std::to_string(want[k]);
+                    return r;
+                }
+            const std::pair<const Matrix*, const Matrix*> mats[2] = {{&z.a, &matrices.a}, {&z.b, &matrices.b}};
+            for (int k = 0; k < 2; k++) {
+                const auto got = detail::canonical_rows(*mats[k].first, m), want_rows = detail::canonical_rows(*mats[k].second, m);
+                for (size_t row = 0; row < m; row++) {
+                    bool same = got[row].size() == want_rows[row].size();
+                    for (size_t e = 0; same && e < got[row].size(); e++)
+                        same = got[row][e].first == want_rows[row][e].first && got[row][e].second == want_rows[row][e].second;
+                    if (!same) { r.why = std::string("matrix ") + (k ? "B" : "A") + " differs from the circuit at row " + std::to_string(row); return r; }
+                }
+            }
+        }
+        size_t n = 1;
+        while (n < m + ni) n <<= 1;
+        const size_t nh = QAP::ID == B2G_REDUCTION_LIBSNARK ? n - 1 : n;
+        const std::pair<const char*, std::pair<size_t, size_t>> shapes[6] = {
+            {"gamma_abc_g1", {pk.vk.gamma_abc_g1.size(), ni}}, {"a_query", {pk.a_query.size(), nv}}, {"b_g1_query", {pk.b_g1_query.size(), nv}},
+            {"b_g2_query", {pk.b_g2_query.size(), nv}}, {"l_query", {pk.l_query.size(), nv - ni}}, {"h_query", {pk.h_query.size(), nh}}};
+        for (const auto& sh : shapes)
+            if (sh.second.first != sh.second.second) {
+                r.why = std::string(sh.first) + " holds " + std::to_string(sh.second.first) + " points; " +
+                        (std::string(sh.first) == "h_query" ? std::string("a ") + (QAP::ID == B2G_REDUCTION_LIBSNARK ? "LibsnarkReduction" : "CircomReduction") +
+                                                                  " domain of " + std::to_string(n) + " needs "
+                                                            : std::string("the circuit needs ")) + std::to_string(sh.second.second);
+                return r;
+            }
+        if (n <= (1ull << powers.power) &&
+            (powers.tau_g1.size() < 2 * n - 1 || powers.tau_g2.size() < n || powers.alpha_tau_g1.size() < n || powers.beta_tau_g1.size() < n))
+            throw std::invalid_argument("verify_proving_key: the powers hold fewer points than the domain of " + std::to_string(n) + " reads");
+        const std::vector<BigInt256> drawn = challenges ? *challenges : powers_challenges(2);
+        if (drawn.size() != 2) throw std::invalid_argument("verify_proving_key: two challenges (rho, sigma)");
+        b2g_powers_desc pd;
+        memset(&pd, 0, sizeof pd);
+        pd.log_size = powers.power;
+        pd.tau_g1 = powers.tau_g1.data(); pd.tau_g2 = powers.tau_g2.data(); pd.alpha_tau_g1 = powers.alpha_tau_g1.data();
+        pd.beta_tau_g1 = powers.beta_tau_g1.data(); pd.beta_g2 = &powers.beta_g2;
+        b2g_key_desc kd;
+        memset(&kd, 0, sizeof kd);
+        kd.n_vars = (uint32_t)nv; kd.n_ic = (uint32_t)ni; kd.n_l = (uint32_t)(nv - ni); kd.n_h = (uint32_t)nh;
+        kd.alpha_g1 = &pk.vk.alpha_g1; kd.beta_g1 = &pk.beta_g1; kd.delta_g1 = &pk.delta_g1;
+        kd.beta_g2 = &pk.vk.beta_g2; kd.gamma_g2 = &pk.vk.gamma_g2; kd.delta_g2 = &pk.vk.delta_g2;
+        kd.gamma_abc_g1 = pk.vk.gamma_abc_g1.data(); kd.a_query = pk.a_query.data(); kd.b_g1_query = pk.b_g1_query.data();
+        kd.b_g2_query = pk.b_g2_query.data(); kd.l_query = pk.l_query.empty() ? nullptr : pk.l_query.data(); kd.h_query = pk.h_query.data();
+        const Gpu::MatDesc md(matrices, nv, QAP::ID, true);
+        b2g_setup_report rep;
+        check(b2g_setup_check(gpu.ctx(), &md.d, &pd, &kd, drawn.data(), &rep));
+        r.ok = rep.ok != 0;
+        if (r.ok) return r;
+        static const char* const fields[12] = {"alpha_g1", "beta_g1", "delta_g1", "beta_g2", "gamma_g2", "delta_g2", "gamma_abc_g1",
+                                               "a_query", "b_g1_query", "b_g2_query", "l_query", "h_query"};
+        static const char* const arrays[5] = {"tau_g1", "tau_g2", "alpha_tau_g1", "beta_tau_g1", "beta_g2"};
+        const std::string name = rep.side ? arrays[rep.field % 5] : fields[rep.field % 12];
+        if (rep.rule == 8) {
+            if (rep.field == 6) r.why = "gamma_abc_g1 / l_query do not match the circuit and ceremony";
+            else if (rep.field == 2) r.why = "delta_g1 and delta_g2 disagree";
+            else r.why = name + " does not match the circuit and ceremony";
+        } else if (rep.rule == 7) {
+            r.why = name + " is not the ceremony's";
+        } else {
+            const bool g2 = name == "beta_g2" || name == "gamma_g2" || name == "delta_g2" || name == "b_g2_query" || name == "tau_g2";
+            static const char* const texts[5] = {"", "a coordinate >= p", "off the curve", "at infinity", "not in G2"};
+            r.why = name + "[" + std::to_string(rep.index) + "]: " + (rep.rule == 2 && g2 ? "off the twist" : rep.rule < 5 ? texts[rep.rule] : "?");
+        }
         return r;
     }
 

@@ -41,6 +41,9 @@
 //       contribution with x = Fr::rand(std::mt19937_64(seed)) (default seed 0x5E7), check it (verify_contribution), prove the
 //       witness under the same rng and verify on the host; print x, the contributed key (serialize_proving_key, compressed,
 //       hex), the check's verdict, the proof and the host verifier's verdict
+//   B2G_ZKEY_VERIFY=<file.ptau> groth16_bench <circuit.r1cs> <circuit.zkey>
+//       check the key against the circuit and the ceremony with Groth16T::verify_proving_key (CircomReduction, as snarkjs) and
+//       print key=1, or key=0 and the reason, and the time of the check in ms (the file reads not included)
 //   B2G_PTAU_CHECK=<file.ptau> groth16_bench [log_n]
 //       check the ceremony (or the prefix a domain of 2^log_n points reads) with Groth16T::verify_powers_of_tau and print
 //       powers=1 or powers=0 with the reason, and the time of the check in ms (the file read not included)
@@ -187,6 +190,28 @@ int main(int argc, char** argv) {
             std::printf("powers=%d\n", r.ok ? 1 : 0);
             if (!r.ok) std::printf("reason=%s\n", r.reason().c_str());
             std::printf("ms=%.3f\n", ms);
+            return 0;
+        }
+        if (const char* ptau = std::getenv("B2G_ZKEY_VERIFY")) {            // R1CS + ceremony + zkey -> the key's check on the GPU
+            if (argc < 3) { std::fprintf(stderr, "usage: B2G_ZKEY_VERIFY=<file.ptau> %s <circuit.r1cs> <circuit.zkey>\n", argv[0]); return 2; }
+            std::ifstream rf(argv[1], std::ios::binary);
+            if (!rf) throw SerializationError("cannot open r1cs");
+            const ConstraintMatrices matrices = R1CS::read(rf).to_matrices();
+            std::ifstream zf(argv[2], std::ios::binary);
+            if (!zf) throw SerializationError("cannot open zkey");
+            const auto key = read_zkey(zf);
+            uint32_t log_n = 1;
+            while ((1ull << log_n) < matrices.num_constraints + matrices.num_instance_variables) log_n++;
+            std::ifstream pf(ptau, std::ios::binary);
+            if (!pf) throw SerializationError("cannot open ptau");
+            const Powers powers = read_ptau(pf, log_n);
+            typedef Groth16T<CircomReduction> G;
+            const auto t0 = std::chrono::steady_clock::now();
+            const SetupCheck r = G::verify_proving_key(matrices, powers, key.first, &key.second);
+            const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+            std::printf("key=%d", r.ok ? 1 : 0);
+            if (!r.ok) std::printf(" %s", r.reason().c_str());
+            std::printf("\nms=%.3f\n", ms);
             return 0;
         }
         if (const char* ptau = std::getenv("B2G_SETUP_PTAU")) {             // R1CS + ceremony -> key -> contribution -> check -> prove -> verify

@@ -34,6 +34,7 @@
  *   b2g_setup_from_powers  <- snarkjs groth16 setup (zkey new): a proving key from a powers-of-tau ceremony
  *   b2g_delta_update / b2g_delta_update_check <- snarkjs zkey contribute / the delta checks of snarkjs zkey verify
  *   b2g_powers_check       <- the algebraic checks of snarkjs powersoftau verify
+ *   b2g_setup_check        <- snarkjs zkey verify: a proving key against its circuit and powers-of-tau ceremony
  *   b2g_fixed_base_g1/g2  <- the batch fixed-base multiplications of that setup, for the standard generators only
  *
  * Conventions
@@ -550,6 +551,69 @@ typedef struct {
  * a pending proof; B2G_E_DEVICE when the buffers do not fit. */
 B2G_API int b2g_powers_check(b2g_ctx* ctx, const b2g_powers_desc* powers, uint32_t log_n, const void* challenges,
                              b2g_powers_report* out);
+
+/* A whole proving key with its counts, HOST arrays in the b2g_pk_desc layout (affine Montgomery, all-zero = infinity).  An
+ * array may be NULL when its count is 0. */
+typedef struct {
+    uint32_t n_vars;             /* points of a_query, b_g1_query and b_g2_query */
+    uint32_t n_ic;               /* points of gamma_abc_g1 (num_inputs) */
+    uint32_t n_l;                /* points of l_query */
+    uint32_t n_h;                /* points of h_query */
+    const void *alpha_g1, *beta_g1, *delta_g1;           /* 64 B each */
+    const void *beta_g2, *gamma_g2, *delta_g2;           /* 128 B each */
+    const void *gamma_abc_g1, *a_query, *b_g1_query, *b_g2_query, *l_query, *h_query;
+} b2g_key_desc;
+
+/* The verdict of b2g_setup_check.  rule: 0 none (ok); 1 a coordinate >= p, 2 off its curve, 3 at infinity, 4 outside G2 (the
+ * point rules: side, field and index name the point); 6 the count of `field` is not the circuit's (index = the count the
+ * circuit needs); 7 `field` is not the ceremony's point; 8 an equation fails (field: 7 a_query E1, 8 b_g1_query E2,
+ * 9 b_g2_query E3, 6 gamma_abc_g1 / l_query E4, 11 h_query E5, 2 delta_g1 / delta_g2 E6).  side: 0 the key, 1 the ceremony.
+ * field (side 0): 0 alpha_g1, 1 beta_g1, 2 delta_g1, 3 beta_g2, 4 gamma_g2, 5 delta_g2, 6 gamma_abc_g1, 7 a_query,
+ * 8 b_g1_query, 9 b_g2_query, 10 l_query, 11 h_query; (side 1): b2g_powers_report's array codes. */
+typedef struct {
+    uint8_t ok;
+    uint8_t rule;
+    uint8_t side;
+    uint8_t field;
+    uint8_t reserved[4];
+    uint64_t index;
+} b2g_setup_report;
+
+/* b2g_setup_check <- `snarkjs zkey verify circuit.r1cs pot.ptau circuit.zkey` without its transcript: whether `key` is the key
+ * b2g_setup_from_powers makes from `circuit` and `powers`, followed by any chain of b2g_delta_update contributions.  The
+ * circuit and the powers are those of b2g_setup_from_powers.  With n the domain, m the constraints, ni = num_inputs, N = n_vars,
+ * A' = A with the public-input rows A'[m + j][j] = 1 (j < ni), T = tau_g1 (2n - 1 points), U = tau_g2, Al = alpha_tau_g1,
+ * Be = beta_tau_g1 (n each), and [L_r] = iNTT_n(T)_r, the transform matrix is symmetric, so for column weights w
+ *     sum_j w_j (sum_r M[r][j] [L_r]) = sum_k s_k T_k,   c = M w (by rows), s = iNTT_n(c) (a scalar transform).
+ * challenges = 2 x 32 B canonical rho, sigma in [1, r); w_j = rho^j (j < N), v_i = sigma^i; s^A, s^B, s^C transform A'w, Bw,
+ * Cw.  out->ok = 1 iff the counts are the circuit's (N, ni, N - ni, and n or n - 1 H points by the reduction); alpha_g1 = Al_0,
+ * beta_g1 = Be_0, beta_g2 = the ceremony's beta_g2 and gamma_g2 = U_0, byte for byte; the point rules hold (the prefix of the
+ * ceremony: b2g_setup_from_powers's rules; every key point: coordinates below p and on its curve, every G2 point in G2,
+ * delta_g1 and delta_g2 not at infinity; query points may be at infinity); and, in this order,
+ *     E1 sum_j w_j a_query[j] = sum_k s^A_k T_k          E2 sum_j w_j b_g1_query[j] = sum_k s^B_k T_k
+ *     E3 sum_j w_j b_g2_query[j] = sum_k s^B_k U_k
+ *     E4 e(sum_(j<ni) w_j IC_j, gamma_2) e(sum_(j>=ni) w_j L_(j-ni), delta_2) = e(sum_k (s^A_k Be_k + s^B_k Al_k + s^C_k T_k), U_0)
+ *     E5 e(sum_i v_i H_i, delta_2) = e(sum_k h_k T_k, U_0), with, for CircomReduction, t = 1/2 iNTT_n(v),
+ *        h_k = t_k omega_2n^-k (k < n), h_(k+n) = -t_k omega_2n^-k (k <= n - 2); for LibsnarkReduction h_k = -v_k (k < n - 1),
+ *        h_(n-1) = 0, h_k = v_(k-n) (n <= k <= 2n - 2)
+ *     E6 e(delta_1, U_0) = e(T_0, delta_2).
+ * Soundness, as for b2g_powers_check: an honest key always gives ok = 1.  Once the point rules hold every point lies in a group
+ * of prime order r, so by Schwartz-Zippel a key that breaks E1-E4 gives ok = 1 with probability at most (N - 1) / (r - 1), and
+ * one that breaks E5 at most (n - 1) / (r - 1), and only if the challenges are drawn uniformly from [1, r) AFTER the key and
+ * the ceremony are fixed, from a source their authors cannot predict or influence.  Whether the ceremony is one is
+ * b2g_powers_check's question; E6 holds for any delta_2 = x U_0 with delta_1 = x T_0.
+ * A failure reports the first failing check in the order above: counts, byte equalities, the ceremony's points (array order,
+ * lowest index first), the key's points (field order), then E1-E6.  The key arrays and the ceremony prefix are read once from
+ * host memory (memory-mapped files in place), in slices of 2^22 points through pinned staging buffers; device memory holds the
+ * matrices and about 32 B x (N + 6n) of scalars, never the points.  Cost: one tableless MSM per array read, four over T, the
+ * G2 subgroup test per G2 point, three scalar transforms of n points, and seven Miller loops with three final
+ * exponentiations.  The transcript of snarkjs (zkey section 10, the contributions' hashes and proofs of knowledge) is not
+ * checked.
+ * Synchronous.  Errors (every error leaves the context usable; a malformed point, a wrong count or a failed equation is a
+ * verdict, not an error): those of b2g_setup_from_powers for the circuit and the powers; B2G_E_INPUT for a challenge that is 0 or
+ * >= r; B2G_E_SHAPE for null pointers or fields or a pending proof; B2G_E_DEVICE when the buffers do not fit. */
+B2G_API int b2g_setup_check(b2g_ctx* ctx, const b2g_mat_desc* circuit, const b2g_powers_desc* powers, const b2g_key_desc* key,
+                            const void* challenges, b2g_setup_report* report);
 
 /* The part of a proving key a delta contribution changes, HOST buffers in the b2g_pk_desc layout. */
 typedef struct {
