@@ -58,8 +58,15 @@ class PowersDesc(C.Structure):
                [(k, C.c_void_p) for k in ('tau_g1', 'tau_g2', 'alpha_tau_g1', 'beta_tau_g1', 'beta_g2')]
 
 
+class LagrangeDesc(C.Structure):
+    """b2g_lagrange_desc / b2g_lagrange_out: the prepared Lagrange sections 12-15 of a ceremony prepared at power log_size"""
+    _fields_ = [('log_size', C.c_uint32), ('reserved', C.c_uint32)] + \
+               [(k, C.c_void_p) for k in ('tau_g1', 'tau_g2', 'alpha_tau_g1', 'beta_tau_g1')]
+
+
 class PowersReport(C.Structure):
-    """b2g_powers_report: the verdict of b2g_powers_check (rule 0 ok, 1-5 a point rule, 6 the pairing product)"""
+    """b2g_powers_report: the verdict of b2g_powers_check and b2g_lagrange_check (rule 0 ok, 1-5 a point rule, 6 the pairing
+    product, 7 a Lagrange section that is not the transform of its powers)"""
     _fields_ = [('ok', C.c_uint8), ('rule', C.c_uint8), ('array', C.c_uint8), ('reserved', C.c_uint8 * 5), ('index', C.c_uint64)]
 
 
@@ -96,7 +103,8 @@ EXPORTS = ['b2g_last_error', 'b2g_version', 'b2g_device_count', 'b2g_ctx_create'
            'b2g_verify_batch_keys_compressed', 'b2g_verify_batch_keys_locate', 'b2g_verify_batch_keys_locate_compressed',
            'b2g_rerandomize_many', 'b2g_points_serialize', 'b2g_points_deserialize', 'b2g_setup',
            'b2g_setup_from_powers', 'b2g_delta_update', 'b2g_delta_update_check', 'b2g_points_intt',
-           'b2g_powers_msm', 'b2g_powers_check', 'b2g_setup_check']
+           'b2g_powers_msm', 'b2g_powers_check', 'b2g_setup_check', 'b2g_powers_prepare', 'b2g_lagrange_check',
+           'b2g_setup_from_lagrange']
 
 _lib = None
 
@@ -146,6 +154,9 @@ def lib():
         L.b2g_powers_msm.argtypes = [vp, i, sz, vp, vp, vp]
         L.b2g_powers_check.argtypes = [vp, C.POINTER(PowersDesc), C.c_uint32, vp, C.POINTER(PowersReport)]
         L.b2g_setup_check.argtypes = [vp, C.POINTER(MatDesc), C.POINTER(PowersDesc), C.POINTER(KeyDesc), vp, C.POINTER(SetupReport)]
+        L.b2g_powers_prepare.argtypes = [vp, C.POINTER(PowersDesc), C.POINTER(LagrangeDesc)]
+        L.b2g_lagrange_check.argtypes = [vp, C.POINTER(PowersDesc), C.POINTER(LagrangeDesc), C.c_uint32, vp, C.POINTER(PowersReport)]
+        L.b2g_setup_from_lagrange.argtypes = [vp, C.POINTER(MatDesc), C.POINTER(PowersDesc), C.POINTER(LagrangeDesc), C.POINTER(SetupOut)]
         L.b2g_test_op.argtypes = [vp, i, vp, vp, sz, vp]
         L.b2g_last_timings.argtypes = [vp, vp]
         L.b2g_bench_device.argtypes = [vp, vp, vp, i, C.POINTER(C.c_float)]

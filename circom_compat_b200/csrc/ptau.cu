@@ -459,6 +459,121 @@ static void setup_check_run(b2g_ctx* ctx, const b2g_mat_desc* d, const b2g_power
     out->ok = 1;
 }
 
+// ---------------------------------------------------------------------------------------------- b2g_lagrange_check
+// s[j] += t[j], j < n (canonical)
+__global__ void __launch_bounds__(256) lagrange_accumulate_kernel(uint32_t n, const fe* __restrict__ t, fe* __restrict__ s) {
+    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j < n) fe_store(&s[j], Fr::add(fe_load(&s[j]), fe_load(&t[j])));
+}
+
+// the small device buffer of a Lagrange check: its layout
+enum : size_t {
+    LC_AFF = 0,                      // the eight sums in affine form: per section the Lagrange side, then the monomial side
+    LC_CH = LC_AFF + 2 * (3 * 64 + 128),
+    LC_RHO = LC_CH + 32,             // rho (Montgomery)
+    LC_PW = LC_RHO + 32,             // the powers kernels' two words
+    LC_BAD = LC_PW + 64,             // the lowest failing index of each Lagrange section
+    LC_POINT = LC_BAD + 4 * 8,
+    LC_WORD = LC_POINT + 128,
+    LC_BYTES = LC_WORD + 32
+};
+
+static void lagrange_check_run(b2g_ctx* ctx, const b2g_powers_desc* pw, const b2g_lagrange_desc* lg, uint32_t log_n, const void* rho,
+                               b2g_powers_report* out) {
+    if (!ctx || !pw || !lg || !rho || !out) throw_error(B2G_E_SHAPE, "null pointer");
+    memset(out, 0, sizeof(*out));
+    const CtxView cv = ctx_view(ctx);
+    if (cv.proof_pending) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
+    const uint32_t p = lg->log_size;
+    if (p > 26 || p > pw->log_size)
+        throw_error(B2G_E_DOMAIN, "b2g_lagrange_check: Lagrange sections of power " + std::to_string(p) + " exceed 26 or the ceremony's power " +
+                                      std::to_string(pw->log_size));
+    if (log_n < 1 || log_n > p)
+        throw_error(B2G_E_DOMAIN, "b2g_lagrange_check: log_n " + std::to_string(log_n) + " is outside 1.." + std::to_string(p));
+    if (!pw->tau_g1 || !pw->tau_g2 || !pw->alpha_tau_g1 || !pw->beta_tau_g1) throw_error(B2G_E_SHAPE, "null powers array");
+    if (!lg->tau_g1 || !lg->tau_g2 || !lg->alpha_tau_g1 || !lg->beta_tau_g1) throw_error(B2G_E_SHAPE, "null Lagrange array");
+    if (!scalar_ok((const uint8_t*)rho)) throw_error(B2G_E_INPUT, "challenge rho is 0 or >= r");
+    const uint64_t n = 1ull << log_n;
+    // section 12 reads blocks 0 .. log_n + 1 and 2n monomials, less the infinity that pads block p + 1
+    const uint64_t n12 = 4 * n - 1, n13 = 2 * n - 1, t12 = log_n == p ? 2 * n - 1 : 2 * n;
+    DevGuard g(cv.device);
+    cudaStream_t st = cv.st;
+    DevBuf v(LC_BYTES);
+    uint8_t* V = v.p;
+    fe* d_rho = (fe*)(V + LC_RHO);
+    unsigned long long* d_bad = (unsigned long long*)(V + LC_BAD);
+    CUDA_CHECK(cudaMemsetAsync(V, 0, LC_BYTES, st));
+    CUDA_CHECK(cudaMemsetAsync(d_bad, 0xff, 4 * 8, st));
+    CUDA_CHECK(cudaMemcpyAsync(V + LC_CH, rho, 32, cudaMemcpyHostToDevice, st));
+    powers_rho_kernel<<<1, 1, 0, st>>>((const fe*)(V + LC_CH), d_rho);
+    g_launch_count += 1;
+    CUDA_CHECK(cudaGetLastError());
+
+    // the weights w_g = rho^g (g < 4n - 1), then s = sum_k pad(iNTT_(2^k)(w of block k)): s13 over blocks 0 .. log_n, s12 the
+    // same plus block log_n + 1
+    DevBuf sc((n12 + 4 * 2 * n) * sizeof(fe));                     // w, then s12, s13, t and the transforms' scratch
+    fe *d_w = (fe*)sc.p, *d_s12 = d_w + n12, *d_s13 = d_s12 + 2 * n, *d_t = d_s13 + 2 * n, *d_tmp = d_t + 2 * n;
+    powers_scalars(d_rho, 0, (uint32_t)n12, (fe*)(V + LC_PW), d_w, st);
+    CUDA_CHECK(cudaMemsetAsync(d_s13, 0, 2 * n * sizeof(fe), st));
+    for (uint32_t k = 0; k <= log_n + 1; k++) {
+        const uint64_t m = 1ull << k;
+        CUDA_CHECK(cudaMemcpyAsync(d_t, d_w + (m - 1), m * sizeof(fe), cudaMemcpyDeviceToDevice, st));
+        if (k) {
+            NttDomain dom;
+            struct DomGuard { NttDomain& d; ~DomGuard() { ntt_domain_destroy(d); } } dg{dom};
+            ntt_domain_create(dom, (int)k, st);
+            ntt_plain(dom, d_t, d_tmp, true, st);
+            CUDA_CHECK(cudaStreamSynchronize(st));                     // dom is freed at the end of this block
+        }
+        if (k == log_n + 1) CUDA_CHECK(cudaMemcpyAsync(d_s12, d_s13, 2 * n * sizeof(fe), cudaMemcpyDeviceToDevice, st));
+        lagrange_accumulate_kernel<<<(unsigned)((m + 255) / 256), 256, 0, st>>>((uint32_t)m, d_t, k == log_n + 1 ? d_s12 : d_s13);
+        g_launch_count += 1;
+        CUDA_CHECK(cudaGetLastError());
+    }
+
+    // the streamed passes: each Lagrange section with the powers of rho and its point rules, then its monomials with s
+    MsmHold h1(false, n12, st), h2(true, n13, st);
+    Staging sg(std::max<size_t>(std::min<uint64_t>(n12, POWERS_SLICE) * 64, std::min<uint64_t>(n13, POWERS_SLICE) * 128), st);
+    struct Sec { const void* lag; uint64_t count; const void* mono; uint64_t terms; const fe* s; bool g2; };
+    const Sec secs[4] = {{lg->tau_g1, n12, pw->tau_g1, t12, d_s12, false}, {lg->tau_g2, n13, pw->tau_g2, n, d_s13, true},
+                         {lg->alpha_tau_g1, n13, pw->alpha_tau_g1, n, d_s13, false}, {lg->beta_tau_g1, n13, pw->beta_tau_g1, n, d_s13, false}};
+    size_t off = LC_AFF;
+    size_t at[4][2];
+    for (int x = 0; x < 4; x++) {
+        const Sec& c = secs[x];
+        PowersMsm& msm = c.g2 ? h2.m : h1.m;
+        const size_t row = c.g2 ? 128 : 64;
+        for (int side = 0; side < 2; side++) {
+            if (side == 0) powers_pass(sg, &msm, c.g2, c.lag, c.count, false, d_bad + x, d_rho, true);
+            else powers_pass(sg, &msm, c.g2, c.mono, c.terms, false, nullptr, nullptr, false, 0, c.s);
+            if (c.g2) powers_affine_kernel<G2, Fq2><<<1, 1, 0, st>>>(msm.acc, V + off);
+            else powers_affine_kernel<G1, Fq><<<1, 1, 0, st>>>(msm.acc, V + off);
+            g_launch_count += 1;
+            CUDA_CHECK(cudaGetLastError());
+            at[x][side] = off;
+            off += row;
+        }
+    }
+    uint8_t sums[LC_CH];
+    uint64_t bad[4];
+    CUDA_CHECK(cudaMemcpyAsync(sums, V, sizeof(sums), cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaMemcpyAsync(bad, d_bad, sizeof(bad), cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    for (int x = 0; x < 4; x++) {
+        const Sec& c = secs[x];
+        if (bad[x] >= c.count) continue;
+        const size_t row = c.g2 ? 128 : 64;
+        CUDA_CHECK(cudaMemcpyAsync(V + LC_POINT, (const uint8_t*)c.lag + bad[x] * row, row, cudaMemcpyHostToDevice, st));
+        const uint32_t rule = powers_point_rule(c.g2, V + LC_POINT, false, (uint32_t*)(V + LC_WORD), st);
+        if (!rule) throw_error(B2G_E_DEVICE, "b2g_lagrange_check: the point rules disagree on point " + std::to_string(bad[x]));
+        out->rule = (uint8_t)rule; out->array = (uint8_t)(5 + x); out->index = bad[x];
+        return;
+    }
+    for (int x = 0; x < 4; x++)
+        if (memcmp(sums + at[x][0], sums + at[x][1], secs[x].g2 ? 128 : 64)) { out->rule = 7; out->array = (uint8_t)(5 + x); return; }
+    out->ok = 1;
+}
+
 }  // namespace b2g
 
 extern "C" {
@@ -469,6 +584,11 @@ int b2g_powers_msm(b2g_ctx* ctx, int g2, size_t n, const void* bases, const void
 
 int b2g_powers_check(b2g_ctx* ctx, const b2g_powers_desc* powers, uint32_t log_n, const void* challenges, b2g_powers_report* out) {
     return b2g::guarded_clear([&] { b2g::powers_check_run(ctx, powers, log_n, challenges, out); });
+}
+
+int b2g_lagrange_check(b2g_ctx* ctx, const b2g_powers_desc* powers, const b2g_lagrange_desc* lagrange, uint32_t log_n,
+                       const void* rho_canon, b2g_powers_report* out) {
+    return b2g::guarded_clear([&] { b2g::lagrange_check_run(ctx, powers, lagrange, log_n, rho_canon, out); });
 }
 
 int b2g_setup_check(b2g_ctx* ctx, const b2g_mat_desc* circuit, const b2g_powers_desc* powers, const b2g_key_desc* key,

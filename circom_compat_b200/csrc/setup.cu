@@ -610,21 +610,51 @@ static void col_sums(const ColPlan& cp, uint32_t nv, uint32_t m, const void* bas
     CUDA_CHECK(cudaGetLastError());
 }
 
-// uploads n affine points (row bytes each) and refuses the array when one of them is off its curve, has a coordinate >= p
-// or (subgroup) lies outside G2; `name` names the array in the message
-static uint8_t* powers_upload(SetupMem& mem, const char* name, const void* host, size_t n, bool g2, bool subgroup, cudaStream_t st) {
+// copies n affine points (row bytes each) to the device buffer d and refuses the array when one of them is off its curve, has a
+// coordinate >= p or (subgroup) lies outside G2; `name` names the array in the message and `base` is the index of host[0] in it
+static void check_upload(const char* name, uint64_t base, const void* host, size_t n, bool g2, bool subgroup, uint8_t* d, cudaStream_t st) {
     const size_t row = g2 ? 128 : 64;
-    uint8_t* d = mem.alloc<uint8_t>(n * row);
     CUDA_CHECK(cudaMemcpyAsync(d, host, n * row, cudaMemcpyHostToDevice, st));
     int why = 0;
     const uint64_t bad = points_check(g2, d, n, subgroup, st, &why);
     if (bad < n)
-        throw_error(B2G_E_INPUT, std::string(name) + "[" + std::to_string(bad) + "]: " +
+        throw_error(B2G_E_INPUT, std::string(name) + "[" + std::to_string(base + bad) + "]: " +
                                      (why == 2 ? "not in G2" : g2 ? "off the twist or a coordinate >= p" : "off the curve or a coordinate >= p"));
+}
+
+// uploads n affine points into a new buffer of `mem`, refused as check_upload refuses them
+static uint8_t* powers_upload(SetupMem& mem, const char* name, const void* host, size_t n, bool g2, bool subgroup, cudaStream_t st,
+                              uint64_t base = 0) {
+    uint8_t* d = mem.alloc<uint8_t>(n * (g2 ? 128 : 64));
+    check_upload(name, base, host, n, g2, subgroup, d, st);
     return d;
 }
 
-static void setup_from_powers_run(b2g_ctx* ctx, const b2g_mat_desc* d, const b2g_powers_desc* pw, const b2g_setup_out* o) {
+// CircomReduction's H query from a Lagrange block: k[i] = -(2n)^-1 omega_2n^(2i+1) (canonical), i < n, from tw[j] = omega_2n^j
+// (j < n, Montgomery; omega_2n^(j+n) = -omega_2n^j) and inv2n = (2n)^-1 (canonical)
+__global__ void __launch_bounds__(256) hq_lagrange_scalars_kernel(uint32_t n, const fe* __restrict__ tw, const fe* __restrict__ inv2n,
+                                                                  fe* __restrict__ k) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t e = 2 * i + 1;
+    const fe w = e < n ? fe_load_nc(&tw[e]) : Fr::neg(fe_load_nc(&tw[e - n]));
+    fe_store(&k[i], Fr::neg(Fr::mul(w, *inv2n)));
+}
+
+// out[i] = blk[2i + 1] (+ corr[i] when corr is given), i < n
+__global__ void __launch_bounds__(128) hq_lagrange_kernel(const void* __restrict__ blk, uint32_t n, const void* __restrict__ corr,
+                                                          void* __restrict__ out) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    G1::Pt p = G1::from_affine(aff_load<Fq>(blk, 2 * (size_t)i + 1));
+    if (corr) G1::madd(p, aff_load<Fq>(corr, i));
+    aff_store<Fq>(out, i, G1::to_affine(p));
+}
+
+// b2g_setup_from_powers, or with lg b2g_setup_from_lagrange: the Lagrange points and the CircomReduction H query read from
+// the prepared sections instead of transformed
+static void setup_from_powers_run(b2g_ctx* ctx, const b2g_mat_desc* d, const b2g_powers_desc* pw, const b2g_setup_out* o,
+                                  const b2g_lagrange_desc* lg = nullptr) {
     if (!ctx || !d || !pw || !o) throw_error(B2G_E_SHAPE, "null pointer");
     const CtxView cv = ctx_view(ctx);
     if (cv.proof_pending) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
@@ -635,6 +665,15 @@ static void setup_from_powers_run(b2g_ctx* ctx, const b2g_mat_desc* d, const b2g
         throw_error(B2G_E_DOMAIN, "PolynomialDegreeTooLarge: the circuit's domain of 2^" + std::to_string(logn) +
                                       " points exceeds the ceremony's 2^" + std::to_string(pw->log_size) + " powers");
     if (!pw->tau_g1 || !pw->tau_g2 || !pw->alpha_tau_g1 || !pw->beta_tau_g1 || !pw->beta_g2) throw_error(B2G_E_SHAPE, "null powers array");
+    if (lg) {
+        if (!lg->tau_g1 || !lg->tau_g2 || !lg->alpha_tau_g1 || !lg->beta_tau_g1) throw_error(B2G_E_SHAPE, "null Lagrange array");
+        if (lg->log_size > 26 || lg->log_size > pw->log_size)
+            throw_error(B2G_E_DOMAIN, "b2g_setup_from_lagrange: Lagrange sections of power " + std::to_string(lg->log_size) +
+                                          " exceed 26 or the ceremony's power " + std::to_string(pw->log_size));
+        if (logn > (int)lg->log_size)
+            throw_error(B2G_E_DOMAIN, "PolynomialDegreeTooLarge: the circuit's domain of 2^" + std::to_string(logn) +
+                                          " points exceeds the Lagrange sections' 2^" + std::to_string(lg->log_size));
+    }
     const uint32_t m = d->num_constraints, ni = d->num_inputs, nv = d->n_vars;
     const size_t n = (size_t)1 << logn, nh = libsnark ? n - 1 : n;
     if (!o->alpha_g1 || !o->beta_g1 || !o->delta_g1 || !o->beta_g2 || !o->gamma_g2 || !o->delta_g2 || !o->gamma_abc_g1 || !o->a_query ||
@@ -665,25 +704,52 @@ static void setup_from_powers_run(b2g_ctx* ctx, const b2g_mat_desc* d, const b2g
     fe* d_sc = mem.alloc<fe>(2 * sizeof(fe));
     pts_scale_kernel<<<1, 1, 0, st>>>(dom.ct, d_sc);                       // ct[0] = n^-1
     g_launch_count += 1;
-    uint8_t* d_work = mem.alloc<uint8_t>(n * 256);
-    uint8_t* d_L1 = mem.alloc<uint8_t>(n * 64);
-    uint8_t* d_L2 = mem.alloc<uint8_t>(n * 128);
-    uint8_t* d_aL = mem.alloc<uint8_t>(n * 64);
-    uint8_t* d_bL = mem.alloc<uint8_t>(n * 64);
     const unsigned pblocks = (unsigned)((n + 127) / 128);
-    const std::pair<const uint8_t*, uint8_t*> g1_sets[3] = {{d_tau1, d_L1}, {d_atau, d_aL}, {d_btau, d_bL}};
-    for (const auto& s : g1_sets) {
-        pts_from_affine_kernel<G1, Fq><<<pblocks, 128, 0, st>>>(s.first, (uint32_t)n, d_work);
-        points_intt<G1, Fq>(dom, d_work, d_sc, s.second, st);
+    uint8_t *d_work = nullptr, *d_L1, *d_L2, *d_aL, *d_bL;
+    if (lg) {
+        // block log_n of each section, at its offset n - 1
+        d_L1 = powers_upload(mem, "lagrange_tau_g1", (const uint8_t*)lg->tau_g1 + (n - 1) * 64, n, false, false, st, n - 1);
+        d_L2 = powers_upload(mem, "lagrange_tau_g2", (const uint8_t*)lg->tau_g2 + (n - 1) * 128, n, true, true, st, n - 1);
+        d_aL = powers_upload(mem, "lagrange_alpha_tau_g1", (const uint8_t*)lg->alpha_tau_g1 + (n - 1) * 64, n, false, false, st, n - 1);
+        d_bL = powers_upload(mem, "lagrange_beta_tau_g1", (const uint8_t*)lg->beta_tau_g1 + (n - 1) * 64, n, false, false, st, n - 1);
+    } else {
+        d_work = mem.alloc<uint8_t>(n * 256);
+        d_L1 = mem.alloc<uint8_t>(n * 64);
+        d_L2 = mem.alloc<uint8_t>(n * 128);
+        d_aL = mem.alloc<uint8_t>(n * 64);
+        d_bL = mem.alloc<uint8_t>(n * 64);
+        const std::pair<const uint8_t*, uint8_t*> g1_sets[3] = {{d_tau1, d_L1}, {d_atau, d_aL}, {d_btau, d_bL}};
+        for (const auto& s : g1_sets) {
+            pts_from_affine_kernel<G1, Fq><<<pblocks, 128, 0, st>>>(s.first, (uint32_t)n, d_work);
+            points_intt<G1, Fq>(dom, d_work, d_sc, s.second, st);
+        }
+        pts_from_affine_kernel<G2, Fq2><<<pblocks, 128, 0, st>>>(d_tau2, (uint32_t)n, d_work);
+        points_intt<G2, Fq2>(dom, d_work, d_sc, d_L2, st);
+        g_launch_count += 4;
     }
-    pts_from_affine_kernel<G2, Fq2><<<pblocks, 128, 0, st>>>(d_tau2, (uint32_t)n, d_work);
-    points_intt<G2, Fq2>(dom, d_work, d_sc, d_L2, st);
-    g_launch_count += 4;
 
     // the H query
     uint8_t* d_h = mem.alloc<uint8_t>(n * 64);
     if (libsnark) {
         hq_libsnark_kernel<<<pblocks, 128, 0, st>>>(d_tau1, (uint32_t)n, d_h);
+        g_launch_count += 1;
+    } else if (lg) {
+        // the odd entries of block log_n + 1, less the term of T_(2n-1) when that block is not the padded top one
+        const uint8_t* d_blk = powers_upload(mem, "lagrange_tau_g1", (const uint8_t*)lg->tau_g1 + (2 * n - 1) * 64, 2 * n, false,
+                                             false, st, 2 * n - 1);
+        uint8_t* d_corr = nullptr;
+        const uint8_t* last = (const uint8_t*)pw->tau_g1 + (2 * n - 1) * 64;
+        if (logn < (int)lg->log_size && !(all_zero32(last) && all_zero32(last + 32))) {
+            const uint8_t* d_last = powers_upload(mem, "tau_g1", last, 1, false, false, st, 2 * n - 1);
+            void* d_tab = mem.alloc<void>(32 * 255 * 64);
+            fe* d_ks = mem.alloc<fe>(n * sizeof(fe));
+            d_corr = mem.alloc<uint8_t>(n * 64);
+            fixed_table_kernel<G1, Fq><<<(32 * 255 + 63) / 64, 64, 0, st>>>(d_tab, d_last);
+            hq_lagrange_scalars_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>((uint32_t)n, dom.tw, d_sc + 1, d_ks);
+            fixed_base_kernel<G1, Fq><<<pblocks, 128, 0, st>>>(d_tab, d_ks, (uint32_t)n, d_corr);
+            g_launch_count += 3;
+        }
+        hq_lagrange_kernel<<<pblocks, 128, 0, st>>>(d_blk, (uint32_t)n, d_corr, d_h);
         g_launch_count += 1;
     } else {
         hq_circom_kernel<<<pblocks, 128, 0, st>>>(d_tau1, (uint32_t)n, dom.tw, d_work);
@@ -761,6 +827,197 @@ static void points_intt_run(b2g_ctx* ctx, int g2, int logn, void* pts) {
     }
     CUDA_CHECK(cudaMemcpyAsync(pts, d_in, n * row, cudaMemcpyDeviceToHost, st));
     CUDA_CHECK(cudaStreamSynchronize(st));
+}
+
+// ---------------------------------------------------------------------------------------------- phase-2 preparation
+constexpr int SEG_LOG = 16;                     // blocks of fewer than 2^SEG_LOG points run in the segmented pass
+constexpr size_t PREP_PINNED = (size_t)64 << 20;  // bytes of the pinned buffer the output goes back through
+
+// the sections of one curve in the segmented pass (grid.y picks one): per section its input (affine), how many input points
+// there are (infinity beyond), its top block and its XYZZ work area and affine output, each block k at offset 2^k - 1
+struct SegSet {
+    const void* in[3];
+    uint64_t limit[3];
+    int top[3];
+    void* work[3];
+    void* out[3];
+};
+
+// work[2^k - 1 + i] = in[i] (infinity for i >= limit), k <= top, one point per thread
+template <class C, class F>
+__global__ void __launch_bounds__(128) seg_fill_kernel(SegSet s) {
+    const int y = blockIdx.y;
+    const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= (2ull << s.top[y]) - 1) return;
+    const uint64_t i = g + 1 - (1ull << (63 - __clzll(g + 1)));
+    pt_store<F>(s.work[y], g, i < s.limit[y] ? C::from_affine(aff_load<F>(s.in[y], i)) : C::infinity());
+}
+
+// round t of the segmented transform: stage k - 1 - t (pts_intt_stage_kernel's butterfly) of every block k in t + 1 .. top.
+// Block k has 2^(k-1) butterflies, so butterfly g of the round belongs to the block with 2^(k-1) <= g + 2^t < 2^k.  Its twiddle
+// omega_(2^(k+1))^x is tw[x 2^(L-k)] in the table of a domain of 2^L >= 2^k points.
+template <class C, class F>
+__global__ void __launch_bounds__(128) seg_stage_kernel(SegSet s, int t, int L, const fe* __restrict__ tw) {
+    const int y = blockIdx.y, top = s.top[y];
+    const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (top <= t || g >= (1ull << top) - (1ull << t)) return;
+    const uint64_t gg = g + (1ull << t);
+    const int k = 64 - __clzll(gg), sg = k - 1 - t;
+    const uint32_t b = (uint32_t)(gg - (1ull << (k - 1)));
+    const uint32_t h = 1u << sg, j = b & (h - 1), i0 = ((b >> sg) << (sg + 1)) | j, i1 = i0 + h;
+    const uint32_t e = j << t;
+    void* pts = s.work[y];
+    const uint64_t a0 = (1ull << k) - 1 + i0, a1 = (1ull << k) - 1 + i1;
+    const typename C::Pt u = pt_load<F>(pts, a0);
+    typename C::Pt v = pt_load<F>(pts, a1), sum = u;
+    C::add(sum, v);
+    C::add(v, C::neg(u));                                                  // v - u
+    if (e) {
+        const fe w = Fr::to_canonical(fe_load_nc(&tw[(size_t)((1u << k) - 2 * e) << (L - k)]));
+        v = C::mul_scalar(v, w.l);
+    } else {
+        v = C::neg(v);
+    }
+    pt_store<F>(pts, a0, sum);
+    pt_store<F>(pts, a1, v);
+}
+
+// out[2^k - 1 + i] = 2^-k work[2^k - 1 + bitrev_k(i)] in affine form, k <= top: every block's finish in one launch
+template <class C, class F>
+__global__ void __launch_bounds__(128) seg_finish_kernel(SegSet s, const fe* __restrict__ sc) {
+    const int y = blockIdx.y;
+    const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= (2ull << s.top[y]) - 1) return;
+    const int k = 63 - __clzll(g + 1);
+    const uint32_t i = (uint32_t)(g + 1 - (1ull << k)), src = k ? __brev(i) >> (32 - k) : 0u;
+    const fe scale = sc[k];
+    aff_store<F>(s.out[y], g, C::to_affine(C::mul_scalar(pt_load<F>(s.work[y], ((1ull << k) - 1) + src), scale.l)));
+}
+
+// sc[k] = 2^-k (canonical), k < 28
+__global__ void inv_pow2_kernel(fe* __restrict__ sc) {
+    if (threadIdx.x != 0 || blockIdx.x != 0) return;
+    fe two = fe_zero(); two.l[0] = 2;
+    const fe half = Fr::inv(Fr::from_canonical(two));
+    fe p = Fr::one();
+    for (int k = 0; k < 28; k++) { sc[k] = Fr::to_canonical(p); p = Fr::mul(p, half); }
+}
+
+struct PinnedBuf {
+    uint8_t* p = nullptr;
+    size_t bytes = 0;
+    explicit PinnedBuf(size_t b) : bytes(b) { CUDA_CHECK(cudaHostAlloc((void**)&p, b, cudaHostAllocDefault)); }
+    ~PinnedBuf() { if (p) cudaFreeHost(p); }
+};
+
+// host[0 .. bytes) = d[0 .. bytes) through the pinned buffer (host may be a memory-mapped file)
+static void to_host(PinnedBuf& pin, const uint8_t* d, size_t bytes, void* host, cudaStream_t st) {
+    for (size_t off = 0; off < bytes; off += pin.bytes) {
+        const size_t c = std::min(pin.bytes, bytes - off);
+        CUDA_CHECK(cudaMemcpyAsync(pin.p, d + off, c, cudaMemcpyDeviceToHost, st));
+        CUDA_CHECK(cudaStreamSynchronize(st));
+        memcpy((uint8_t*)host + off, pin.p, c);
+    }
+}
+
+static void powers_prepare_run(b2g_ctx* ctx, const b2g_powers_desc* pw, const b2g_lagrange_out* o) {
+    if (!ctx || !pw || !o) throw_error(B2G_E_SHAPE, "null pointer");
+    const CtxView cv = ctx_view(ctx);
+    if (cv.proof_pending) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
+    if (pw->log_size > 28) throw_error(B2G_E_DOMAIN, "b2g_powers_prepare: log_size " + std::to_string(pw->log_size) + " exceeds 28");
+    const int K = (int)o->log_size;
+    if (K < 1 || K > 26 || K > (int)pw->log_size)
+        throw_error(B2G_E_DOMAIN, "b2g_powers_prepare: power " + std::to_string(K) + " is outside 1.." +
+                                      std::to_string(std::min<uint32_t>(pw->log_size, 26)));
+    if (!pw->tau_g1 || !pw->tau_g2 || !pw->alpha_tau_g1 || !pw->beta_tau_g1) throw_error(B2G_E_SHAPE, "null powers array");
+    if (!o->tau_g1 || !o->tau_g2 || !o->alpha_tau_g1 || !o->beta_tau_g1) throw_error(B2G_E_SHAPE, "null output array");
+    if (all_zero32((const uint8_t*)pw->tau_g1) && all_zero32((const uint8_t*)pw->tau_g1 + 32)) throw_error(B2G_E_INPUT, "tau_g1[0]: at infinity");
+    {
+        bool inf = true;
+        for (int i = 0; i < 4; i++) inf = inf && all_zero32((const uint8_t*)pw->tau_g2 + 32 * i);
+        if (inf) throw_error(B2G_E_INPUT, "tau_g2[0]: at infinity");
+    }
+    DevGuard g(cv.device);
+    cudaStream_t st = cv.st;
+    SetupMem mem{st, {}};
+    const uint64_t nK = 1ull << K;
+    // sections in launch order: the three G1 ones (one segmented launch), then G2
+    struct Sec { const char* name; const uint8_t* in; uint8_t* out; uint64_t limit; int top; bool g2; };
+    const Sec secs[4] = {{"tau_g1", (const uint8_t*)pw->tau_g1, (uint8_t*)o->tau_g1, 2 * nK - 1, K + 1, false},
+                         {"alpha_tau_g1", (const uint8_t*)pw->alpha_tau_g1, (uint8_t*)o->alpha_tau_g1, nK, K, false},
+                         {"beta_tau_g1", (const uint8_t*)pw->beta_tau_g1, (uint8_t*)o->beta_tau_g1, nK, K, false},
+                         {"tau_g2", (const uint8_t*)pw->tau_g2, (uint8_t*)o->tau_g2, nK, K, true}};
+    fe* d_sc = mem.alloc<fe>(28 * sizeof(fe));
+    inv_pow2_kernel<<<1, 1, 0, st>>>(d_sc);
+    g_launch_count += 1;
+    PinnedBuf pin(std::min(PREP_PINNED, (size_t)(4 * nK - 1) * 64));
+
+    // blocks 0 .. min(top, SEG_LOG - 1) of every section: one segmented pass per curve
+    SegSet set[2] = {};
+    int seg_top = 0;
+    for (int x = 0; x < 4; x++) {
+        const Sec& c = secs[x];
+        const int top = std::min(c.top, SEG_LOG - 1);
+        const uint64_t cnt = std::min<uint64_t>(c.limit, 1ull << top), recs = (2ull << top) - 1;
+        SegSet& s = set[c.g2 ? 1 : 0];
+        const int y = c.g2 ? 0 : x;
+        s.in[y] = powers_upload(mem, c.name, c.in, cnt, c.g2, c.g2, st);
+        s.limit[y] = cnt;
+        s.top[y] = top;
+        s.work[y] = mem.alloc<uint8_t>(recs * (c.g2 ? 256 : 128));
+        s.out[y] = mem.alloc<uint8_t>(recs * (c.g2 ? 128 : 64));
+        seg_top = std::max(seg_top, top);
+    }
+    NttDomain seg_dom;
+    {
+        struct DomGuard { NttDomain& d; ~DomGuard() { ntt_domain_destroy(d); } } dg{seg_dom};
+        ntt_domain_create(seg_dom, seg_top, st);
+        const unsigned fill_blocks = (unsigned)(((2ull << seg_top) - 1 + 127) / 128);
+        seg_fill_kernel<G1, Fq><<<dim3(fill_blocks, 3), 128, 0, st>>>(set[0]);
+        seg_fill_kernel<G2, Fq2><<<dim3(fill_blocks, 1), 128, 0, st>>>(set[1]);
+        g_launch_count += 2;
+        const unsigned stage_blocks = (unsigned)(((1ull << seg_top) + 127) / 128);
+        for (int t = 0; t < seg_top; t++) {
+            seg_stage_kernel<G1, Fq><<<dim3(stage_blocks, 3), 128, 0, st>>>(set[0], t, seg_top, seg_dom.tw);
+            seg_stage_kernel<G2, Fq2><<<dim3(stage_blocks, 1), 128, 0, st>>>(set[1], t, seg_top, seg_dom.tw);
+        }
+        seg_finish_kernel<G1, Fq><<<dim3(fill_blocks, 3), 128, 0, st>>>(set[0], d_sc);
+        seg_finish_kernel<G2, Fq2><<<dim3(fill_blocks, 1), 128, 0, st>>>(set[1], d_sc);
+        g_launch_count += 2 * seg_top + 2;
+        CUDA_CHECK(cudaGetLastError());
+        for (int x = 0; x < 4; x++) {
+            const Sec& c = secs[x];
+            const SegSet& s = set[c.g2 ? 1 : 0];
+            const int y = c.g2 ? 0 : x;
+            to_host(pin, (const uint8_t*)s.out[y], ((2ull << s.top[y]) - 1) * (c.g2 ? 128 : 64), c.out, st);
+        }
+    }
+
+    // the larger blocks, one transform each, largest first, through one work area sized for the top block
+    if (K + 1 < SEG_LOG) return;
+    uint8_t* d_work = mem.alloc<uint8_t>((2 * nK) * 128);
+    uint8_t* d_aff = mem.alloc<uint8_t>((2 * nK) * 64);
+    for (const Sec& c : secs) {
+        const size_t row = c.g2 ? 128 : 64;
+        for (int k = c.top; k >= SEG_LOG; k--) {
+            const uint64_t n = 1ull << k, cnt = std::min<uint64_t>(c.limit, n);
+            check_upload(c.name, 0, c.in, cnt, c.g2, c.g2, d_aff, st);
+            if (cnt < n) CUDA_CHECK(cudaMemsetAsync(d_aff + cnt * row, 0, (n - cnt) * row, st));
+            NttDomain dom;
+            struct DomGuard { NttDomain& d; ~DomGuard() { ntt_domain_destroy(d); } } dg{dom};
+            ntt_domain_create(dom, k, st);
+            const unsigned blocks = (unsigned)((n + 127) / 128);
+            if (c.g2) {
+                pts_from_affine_kernel<G2, Fq2><<<blocks, 128, 0, st>>>(d_aff, (uint32_t)n, d_work);
+                points_intt<G2, Fq2>(dom, d_work, d_sc + k, d_aff, st);
+            } else {
+                pts_from_affine_kernel<G1, Fq><<<blocks, 128, 0, st>>>(d_aff, (uint32_t)n, d_work);
+                points_intt<G1, Fq>(dom, d_work, d_sc + k, d_aff, st);
+            }
+            g_launch_count += 1;
+            to_host(pin, d_aff, n * row, c.out + (n - 1) * row, st);
+        }
+    }
 }
 
 // ---------------------------------------------------------------------------------------------- delta contributions
@@ -853,6 +1110,18 @@ int b2g_setup_from_powers(b2g_ctx* ctx, const b2g_mat_desc* circuit, const b2g_p
 
 int b2g_points_intt(b2g_ctx* ctx, int g2, int log_n, void* points_mont) {
     return b2g::guarded_clear([&] { b2g::points_intt_run(ctx, g2, log_n, points_mont); });
+}
+
+int b2g_setup_from_lagrange(b2g_ctx* ctx, const b2g_mat_desc* circuit, const b2g_powers_desc* powers, const b2g_lagrange_desc* lagrange,
+                            b2g_setup_out* out) {
+    return b2g::guarded_clear([&] {
+        if (!lagrange) b2g::throw_error(B2G_E_SHAPE, "null pointer");
+        b2g::setup_from_powers_run(ctx, circuit, powers, out, lagrange);
+    });
+}
+
+int b2g_powers_prepare(b2g_ctx* ctx, const b2g_powers_desc* powers, const b2g_lagrange_out* out) {
+    return b2g::guarded_clear([&] { b2g::powers_prepare_run(ctx, powers, out); });
 }
 
 int b2g_delta_update(b2g_ctx* ctx, const b2g_delta_key* before, const void* x_canon, b2g_delta_key* after) {

@@ -622,6 +622,22 @@ def _powers_desc(powers, size):
     return pd, arrays
 
 
+def _lagrange_descs(powers, log_n):
+    """(b2g_powers_desc, b2g_lagrange_desc, the arrays they point into) of the prefix a domain of 2^log_n points reads from a
+    ceremony with prepared Lagrange sections (tau_g1 with 2n points below the prepared power: the top block reads them)"""
+    from .ptau import ARRAYS, LAGRANGE, Powers
+    pre = Powers(int(powers.power), int(getattr(powers, 'ceremony_power', powers.power)),
+                 *(np.asarray(getattr(powers, k)) for k in ARRAYS), lagrange=powers.lagrange).prefix(log_n)
+    pd, ld, keep = N.PowersDesc(), N.LagrangeDesc(), []
+    pd.log_size, ld.log_size = int(powers.power), int(pre.lagrange.power)
+    for desc, src, names in ((pd, pre, ARRAYS), (ld, pre.lagrange, LAGRANGE)):
+        for name in names:
+            a = _c(getattr(src, name))
+            keep.append(a)
+            setattr(desc, name, a.ctypes.data)
+    return pd, ld, keep
+
+
 def _delta_desc(arrs) -> 'N.DeltaKey':
     d = N.DeltaKey()
     d.n_l, d.n_h = arrs['l_query'].size // 8, arrs['h_query'].size // 8
@@ -789,10 +805,18 @@ class Groth16:
     def generate_parameters_from_powers_of_tau(circuit, powers, ctx: Context = None, reduction=CircomReduction) -> ProvingKey:
         """`snarkjs groth16 setup circuit.r1cs pot.ptau` on the GPU (b2g_setup_from_powers): the proving key of `circuit` (as
         generate_parameters_with_qap takes it) from a powers-of-tau ceremony (ptau.read_ptau, or any object with the same
-        fields), with gamma = delta = 1.  Only the prefix of each array the circuit's domain needs is read."""
+        fields), with gamma = delta = 1.  Only the prefix of each array the circuit's domain needs is read.  A ceremony that
+        carries prepared Lagrange sections (powers.lagrange, as read_ptau attaches them) takes b2g_setup_from_lagrange, which
+        reads the Lagrange points instead of transforming the powers and gives the same key when the sections are honest
+        (verify_powers_of_tau checks them); any other takes b2g_setup_from_powers."""
         ctx = ctx or default_context()
         d, keep, n_vars, ni, size, nh = _circuit_desc(circuit, reduction)
-        pd, arrays = _powers_desc(powers, size)
+        lag = getattr(powers, 'lagrange', None)
+        if lag is not None and size.bit_length() - 1 <= min(int(powers.power), int(lag.power)):
+            pd, ld, arrays = _lagrange_descs(powers, size.bit_length() - 1)
+        else:
+            ld = None
+            pd, arrays = _powers_desc(powers, size)
         shapes = {'alpha_g1': (1, 8), 'beta_g1': (1, 8), 'delta_g1': (1, 8), 'beta_g2': (1, 16), 'gamma_g2': (1, 16), 'delta_g2': (1, 16),
                   'gamma_abc_g1': (ni, 8), 'a_query': (n_vars, 8), 'b_g1_query': (n_vars, 8), 'b_g2_query': (n_vars, 16),
                   'l_query': (n_vars - ni, 8), 'h_query': (nh, 8)}
@@ -800,7 +824,10 @@ class Groth16:
         out = N.SetupOut()
         for k, a in arrs.items():
             setattr(out, k, a.ctypes.data if a.size else None)
-        N.check(N.lib().b2g_setup_from_powers(ctx._h, C.byref(d), C.byref(pd), C.byref(out)))
+        if ld is not None:
+            N.check(N.lib().b2g_setup_from_lagrange(ctx._h, C.byref(d), C.byref(pd), C.byref(ld), C.byref(out)))
+        else:
+            N.check(N.lib().b2g_setup_from_powers(ctx._h, C.byref(d), C.byref(pd), C.byref(out)))
         return ProvingKey(n_vars, ni - 1, nh, arrs['alpha_g1'], arrs['beta_g1'], arrs['beta_g2'], arrs['gamma_g2'], arrs['delta_g1'],
                           arrs['delta_g2'], arrs['gamma_abc_g1'], arrs['a_query'], arrs['b_g1_query'], arrs['b_g2_query'],
                           arrs['l_query'], arrs['h_query'])
@@ -899,6 +926,45 @@ class Groth16:
         return bool(out[0])
 
     @staticmethod
+    def prepare_powers_of_tau(powers, dst=None, power=None, ctx: Context = None):
+        """`snarkjs powersoftau prepare phase2` on the GPU (b2g_powers_prepare): the ceremony of power K (`power`, by default
+        min(powers.power, 26)) formed by the prefix of `powers`, with its Lagrange sections 12-15.  Returns a ptau.Powers with
+        .lagrange set; with `dst` (a path) the prepared .ptau is written there, the sections filled in place through a memory
+        map so that files larger than memory work, and the result is that file read back (memory-mapped).  The points read are
+        checked as generate_parameters_from_powers_of_tau checks them; whether they are a ceremony is verify_powers_of_tau's
+        question."""
+        from .ptau import ARRAYS, LAGRANGE, Lagrange, Powers, lagrange_counts, read_ptau, write_ptau
+        K = min(int(powers.power), 26) if power is None else int(power)
+        if not 1 <= K <= min(int(powers.power), 26):
+            raise ValueError(f"prepare_powers_of_tau: power {K} is outside 1..{min(int(powers.power), 26)}")
+        pre = Powers(K, int(getattr(powers, 'ceremony_power', powers.power)),
+                     *(np.asarray(getattr(powers, k)) for k in ARRAYS)).prefix(K)
+        if dst is not None:
+            write_ptau(dst, pre, lagrange_space=True)
+            mm = np.memmap(dst, dtype=np.uint8, mode='r+')
+            outs = [getattr(read_ptau(mm).lagrange, k) for k in LAGRANGE]
+        else:
+            mm = None
+            outs = [np.zeros((c, 16 if k == 'tau_g2' else 8), dtype=np.uint64) for k, c in zip(LAGRANGE, lagrange_counts(K))]
+        pd, keep = N.PowersDesc(), []
+        pd.log_size = int(powers.power)
+        for name in ARRAYS:
+            a = _c(getattr(pre, name))
+            keep.append(a)
+            setattr(pd, name, a.ctypes.data)
+        od = N.LagrangeDesc()
+        od.log_size = K
+        for name, a in zip(LAGRANGE, outs):
+            setattr(od, name, a.ctypes.data)
+        ctx = ctx or default_context()
+        N.check(N.lib().b2g_powers_prepare(ctx._h, C.byref(pd), C.byref(od)))
+        if mm is not None:
+            mm.flush()
+            del outs, mm
+            return read_ptau(dst)
+        return Powers(K, pre.ceremony_power, *(getattr(pre, k) for k in ARRAYS), lagrange=Lagrange(K, *outs))
+
+    @staticmethod
     def verify_powers_of_tau(powers, log_n=None, ctx: Context = None, challenges=None):
         """The algebraic checks of `snarkjs powersoftau verify` on the GPU (b2g_powers_check): whether the prefix a domain of
         2^log_n points reads (the whole ceremony by default) holds powers of one tau with the same alpha and beta on the
@@ -906,9 +972,14 @@ class Groth16:
         read in place, once.  The five challenges (rho, sigma, pi, kappa, eps in [1, r)) are drawn with `secrets` unless
         given.  Returns a ptau.PowersCheck: truthy when the ceremony passes, .reason naming the first failing point or the
         failed pairing product.  A ceremony that is not one passes with probability at most 2n / (r - 1) when the challenges
-        are drawn after the file is fixed.  Raises ValueError for a bad log_n or arrays shorter than it reads."""
+        are drawn after the file is fixed.  Raises ValueError for a bad log_n or arrays shorter than it reads.
+        When the ceremony carries prepared Lagrange sections (powers.lagrange) and passes, b2g_lagrange_check then decides
+        whether their blocks up to log_n (log_n + 1 for lagrange_tau_g1) are the transforms of the powers, with one more
+        challenge rho: the sixth entry of `challenges` when six are given, else drawn with `secrets`.  A wrong section passes
+        with probability at most (its point count) / (r - 1); a failure's reason is "lagrange_tau_g2[17]: not in G2" or
+        "lagrange_tau_g1 is not the transform of tau_g1"."""
         import secrets
-        from .ptau import ARRAYS, Powers, PowersCheck
+        from .ptau import ARRAYS, REPORT_ARRAYS, Powers, PowersCheck
         power = int(powers.power)
         log_n = power if log_n is None else int(log_n)
         if log_n < 1:
@@ -918,9 +989,10 @@ class Groth16:
         if challenges is None:
             challenges = [1 + secrets.randbelow(R_MOD - 1) for _ in range(5)]
         challenges = [int(c) for c in challenges]
-        if len(challenges) != 5 or not all(0 <= c < 1 << 256 for c in challenges):
-            raise ValueError("verify_powers_of_tau: five challenges (rho, sigma, pi, kappa, eps), each below 2^256")
-        cb = np.frombuffer(b''.join(c.to_bytes(32, 'little') for c in challenges), dtype=np.uint8).copy()
+        if len(challenges) not in (5, 6) or not all(0 <= c < 1 << 256 for c in challenges):
+            raise ValueError("verify_powers_of_tau: five challenges (rho, sigma, pi, kappa, eps), each below 2^256, and an "
+                             "optional sixth for the Lagrange sections")
+        cb = np.frombuffer(b''.join(c.to_bytes(32, 'little') for c in challenges[:5]), dtype=np.uint8).copy()
         pd = N.PowersDesc()
         pd.log_size = power
         keep = []
@@ -931,11 +1003,18 @@ class Groth16:
         rep = N.PowersReport()
         ctx = ctx or default_context()
         N.check(N.lib().b2g_powers_check(ctx._h, C.byref(pd), log_n, _ptr(cb), C.byref(rep)))
+        if rep.ok and getattr(powers, 'lagrange', None) is not None:
+            rho = challenges[5] if len(challenges) == 6 else 1 + secrets.randbelow(R_MOD - 1)
+            rb = np.frombuffer(int(rho).to_bytes(32, 'little'), dtype=np.uint8).copy()
+            lpd, ld, keep = _lagrange_descs(powers, log_n)
+            N.check(N.lib().b2g_lagrange_check(ctx._h, C.byref(lpd), C.byref(ld), log_n, _ptr(rb), C.byref(rep)))
         if rep.ok:
             return PowersCheck(True)
         if rep.rule == 6:
             return PowersCheck(False, 6)
-        return PowersCheck(False, int(rep.rule), ARRAYS[rep.array], int(rep.index))
+        if rep.rule == 7:
+            return PowersCheck(False, 7, REPORT_ARRAYS[rep.array])
+        return PowersCheck(False, int(rep.rule), REPORT_ARRAYS[rep.array], int(rep.index))
 
     # ---- verification (host pairing; circom_compat_b200/verifier.py).  Call sites in the reference: src/zkey.rs:868-870,
     # 914-916 (process_vk + verify_with_processed_vk), tests/groth16.rs:33-35 (SNARK::verify).

@@ -311,17 +311,28 @@ inline std::vector<Fr> read_wtns(std::istream& r) {
 // ---------------------------------------------------------------------------------------------- .ptau reader (host)
 // The points of a powers-of-tau ceremony of size 2^power (snarkjs .ptau sections 2-6; layout restated in ptau.py), affine
 // Montgomery as in a zkey.  The vectors may hold only a prefix of the ceremony: see read_ptau.
+// The prepared Lagrange sections 12-15 (snarkjs powersoftau prepare phase2; layout in ptau.py and include/b2groth.h): block k
+// of a section starts at point 2^k - 1 and holds iNTT_(2^k) of the first 2^k points of its monomial array.
+struct LagrangePoints {
+    uint32_t power = 0;                                         // the power they were prepared at (block power + 1 padded)
+    std::vector<G1Affine> tau_g1, alpha_tau_g1, beta_tau_g1;    // blocks 0 .. power + 1, 0 .. power, 0 .. power in the file
+    std::vector<G2Affine> tau_g2;                               // blocks 0 .. power
+};
+
 struct Powers {
     uint32_t power = 0, ceremony_power = 0;
     std::vector<G1Affine> tau_g1, alpha_tau_g1, beta_tau_g1;    // 2^(power+1) - 1, 2^power, 2^power points in the file
     std::vector<G2Affine> tau_g2;                               // 2^power
     G2Affine beta_g2;
+    bool prepared = false;                                      // lagrange holds sections 12-15 (or their prefix)
+    LagrangePoints lagrange;
 };
 
 // Parses a .ptau container with the checks of ptau.read_ptau (magic, version 1, BN254's field, sections 1-6 present, not
 // truncated, sizes that agree with the power), throwing SerializationError.  log_n > 0: read only the prefix a circuit
 // of domain 2^log_n needs (2n - 1 / n / n / n points), so a large ceremony file is not read whole; it must not exceed the
-// file's power.  log_n = 0: every point.
+// file's power.  log_n = 0: every point.  When sections 12-15 are all present with the sizes of the power, their blocks up to
+// log_n (+ 1 for tau_g1) are read too (prepared = true); below the power tau_g1 then keeps 2n points, as the top block reads.
 inline Powers read_ptau(std::istream& r, uint32_t log_n = 0) {
     r.seekg(0, std::ios::end);
     const uint64_t size = (uint64_t)r.tellg();
@@ -358,7 +369,14 @@ inline Powers read_ptau(std::istream& r, uint32_t log_n = 0) {
     if (p.power < 1 || p.power > 28) throw SerializationError("ptau: power " + std::to_string(p.power) + " is out of range (1..28)");
     if (log_n > p.power) throw SerializationError("ptau: the circuit's domain 2^" + std::to_string(log_n) + " exceeds the ceremony's 2^" + std::to_string(p.power));
     const uint64_t n = 1ull << p.power, m = log_n ? 1ull << log_n : n;
-    const uint64_t counts[5] = {2 * n - 1, n, n, n, 1}, reads[5] = {2 * m - 1, m, m, m, 1}, rows[5] = {64, 128, 64, 64, 128};
+    const uint64_t lag_counts[4] = {4 * n - 1, 2 * n - 1, 2 * n - 1, 2 * n - 1}, lag_rows[4] = {64, 128, 64, 64};
+    p.prepared = true;
+    for (int k = 0; k < 4; k++) {
+        auto it = secs.find(12 + k);
+        p.prepared = p.prepared && it != secs.end() && it->second.size == lag_counts[k] * lag_rows[k];
+    }
+    const uint64_t counts[5] = {2 * n - 1, n, n, n, 1}, rows[5] = {64, 128, 64, 64, 128};
+    const uint64_t reads[5] = {2 * m - 1 + (p.prepared && m < n ? 1 : 0), m, m, m, 1};
     for (int k = 0; k < 5; k++) {
         const detail::Section s = secs[2 + k];
         if (s.size != counts[k] * rows[k])
@@ -375,7 +393,52 @@ inline Powers read_ptau(std::istream& r, uint32_t log_n = 0) {
         }
         detail::read_exact(r, dst, reads[k] * rows[k]);
     }
+    if (p.prepared) {
+        p.lagrange.power = p.power;
+        const uint64_t lag_reads[4] = {4 * m - 1, 2 * m - 1, 2 * m - 1, 2 * m - 1};
+        p.lagrange.tau_g1.resize(lag_reads[0]); p.lagrange.tau_g2.resize(lag_reads[1]);
+        p.lagrange.alpha_tau_g1.resize(lag_reads[2]); p.lagrange.beta_tau_g1.resize(lag_reads[3]);
+        void* dsts[4] = {p.lagrange.tau_g1.data(), p.lagrange.tau_g2.data(), p.lagrange.alpha_tau_g1.data(), p.lagrange.beta_tau_g1.data()};
+        for (int k = 0; k < 4; k++) {
+            r.seekg((std::streamoff)secs[12 + k].position);
+            detail::read_exact(r, dsts[k], lag_reads[k] * lag_rows[k]);
+        }
+    }
     return p;
+}
+
+// Writes `p` as a .ptau container (sections 1-6, and 12-15 when prepared), as ptau.write_ptau does: the vectors must hold the
+// full counts of p.power (a prefix is refused with std::invalid_argument).  Section 7, the contribution transcript, is not
+// written.
+inline void write_ptau(std::ostream& w, const Powers& p) {
+    const uint64_t n = 1ull << p.power;
+    if (p.power < 1 || p.power > 28 || p.tau_g1.size() != 2 * n - 1 || p.tau_g2.size() != n || p.alpha_tau_g1.size() != n ||
+        p.beta_tau_g1.size() != n)
+        throw std::invalid_argument("write_ptau: the arrays do not hold the counts of power " + std::to_string(p.power));
+    if (p.prepared && (p.lagrange.power != p.power || p.lagrange.tau_g1.size() != 4 * n - 1 || p.lagrange.tau_g2.size() != 2 * n - 1 ||
+                       p.lagrange.alpha_tau_g1.size() != 2 * n - 1 || p.lagrange.beta_tau_g1.size() != 2 * n - 1))
+        throw std::invalid_argument("write_ptau: the Lagrange sections do not hold the counts of power " + std::to_string(p.power));
+    auto put32 = [&](uint32_t v) { w.write((const char*)&v, 4); };
+    auto put64 = [&](uint64_t v) { w.write((const char*)&v, 8); };
+    auto section = [&](uint32_t id, const void* data, uint64_t bytes) { put32(id); put64(bytes); w.write((const char*)data, (std::streamsize)bytes); };
+    w.write("ptau", 4);
+    put32(1);
+    put32(p.prepared ? 10 : 6);
+    put32(1); put64(44); put32(32);
+    w.write((const char*)detail::FQ_P, 32);
+    put32(p.power); put32(p.ceremony_power);
+    section(2, p.tau_g1.data(), p.tau_g1.size() * 64);
+    section(3, p.tau_g2.data(), p.tau_g2.size() * 128);
+    section(4, p.alpha_tau_g1.data(), p.alpha_tau_g1.size() * 64);
+    section(5, p.beta_tau_g1.data(), p.beta_tau_g1.size() * 64);
+    section(6, &p.beta_g2, 128);
+    if (p.prepared) {
+        section(12, p.lagrange.tau_g1.data(), p.lagrange.tau_g1.size() * 64);
+        section(13, p.lagrange.tau_g2.data(), p.lagrange.tau_g2.size() * 128);
+        section(14, p.lagrange.alpha_tau_g1.data(), p.lagrange.alpha_tau_g1.size() * 64);
+        section(15, p.lagrange.beta_tau_g1.data(), p.lagrange.beta_tau_g1.size() * 64);
+    }
+    if (!w) throw SerializationError("write_ptau: the write failed");
 }
 
 // ---------------------------------------------------------------------------------------------- device side
@@ -552,13 +615,14 @@ struct VerifyCall {
 struct PowersCheck {
     bool ok = false;
     int rule = 0;                 // b2g_powers_report's rule code
-    std::string array;            // rules 1-5: the array and the index of the first failing point
+    std::string array;            // rules 1-5: the array and the index of the first failing point; rule 7: the section
     uint64_t index = 0;
     explicit operator bool() const { return ok; }
     std::string reason() const {
         if (ok) return "";
         if (rule == 6) return "the powers are not those of one tau, alpha and beta";
-        const bool g2 = array == "tau_g2" || array == "beta_g2";
+        if (rule == 7) return array + " is not the transform of " + array.substr(9);
+        const bool g2 = array == "tau_g2" || array == "beta_g2" || array == "lagrange_tau_g2";
         static const char* const texts[6] = {"", "a coordinate >= p", "off the curve", "at infinity", "not in G2", "not the generator"};
         return array + "[" + std::to_string(index) + "]: " + (rule == 2 && g2 ? "off the twist" : texts[rule]);
     }
@@ -992,8 +1056,52 @@ struct Groth16T {                                       // Groth16::<Bn254, QAP>
                              pk.vk.gamma_abc_g1.data(), pk.a_query.data(), pk.b_g1_query.data(), pk.b_g2_query.data(),
                              pk.l_query.data(), pk.h_query.data()};
         const Gpu::MatDesc md(matrices, nv, QAP::ID, true);
-        check(b2g_setup_from_powers(gpu.ctx(), &md.d, &pd, &out));
+        if (powers.prepared && n <= (1ull << powers.lagrange.power)) {
+            // the Lagrange route (b2g_setup_from_lagrange): blocks log n and log n + 1 must be there, and 2n powers below
+            // the prepared power
+            const b2g_lagrange_desc ld = lagrange_desc(powers);
+            if (powers.lagrange.tau_g1.size() < 4 * n - 1 || powers.lagrange.tau_g2.size() < 2 * n - 1 ||
+                powers.lagrange.alpha_tau_g1.size() < 2 * n - 1 || powers.lagrange.beta_tau_g1.size() < 2 * n - 1 ||
+                (n < (1ull << powers.lagrange.power) && powers.tau_g1.size() < 2 * n))
+                throw std::invalid_argument("generate_parameters_from_powers_of_tau: the Lagrange sections hold fewer points than the "
+                                            "domain of " + std::to_string(n) + " reads");
+            check(b2g_setup_from_lagrange(gpu.ctx(), &md.d, &pd, &ld, &out));
+        } else {
+            check(b2g_setup_from_powers(gpu.ctx(), &md.d, &pd, &out));
+        }
         return pk;
+    }
+
+    // `snarkjs powersoftau prepare phase2` (b2g_powers_prepare): the ceremony of power `power` (0: min(powers.power, 26))
+    // formed by the prefix of `powers`, with its Lagrange sections.  Throws std::invalid_argument for a power out of range or
+    // vectors shorter than it reads.
+    static Powers prepare_powers_of_tau(const Powers& powers, uint32_t power = 0, Gpu& gpu = Gpu::instance()) {
+        const uint32_t K = power ? power : std::min<uint32_t>(powers.power, 26);
+        if (K < 1 || K > std::min<uint32_t>(powers.power, 26))
+            throw std::invalid_argument("prepare_powers_of_tau: power " + std::to_string(K) + " is out of range");
+        const size_t n = (size_t)1 << K;
+        if (powers.tau_g1.size() < 2 * n - 1 || powers.tau_g2.size() < n || powers.alpha_tau_g1.size() < n || powers.beta_tau_g1.size() < n)
+            throw std::invalid_argument("prepare_powers_of_tau: the powers hold fewer points than power " + std::to_string(K) + " reads");
+        Powers out;
+        out.power = K; out.ceremony_power = powers.ceremony_power;
+        out.tau_g1.assign(powers.tau_g1.begin(), powers.tau_g1.begin() + (2 * n - 1));
+        out.tau_g2.assign(powers.tau_g2.begin(), powers.tau_g2.begin() + n);
+        out.alpha_tau_g1.assign(powers.alpha_tau_g1.begin(), powers.alpha_tau_g1.begin() + n);
+        out.beta_tau_g1.assign(powers.beta_tau_g1.begin(), powers.beta_tau_g1.begin() + n);
+        out.beta_g2 = powers.beta_g2;
+        out.prepared = true;
+        out.lagrange.power = K;
+        out.lagrange.tau_g1.resize(4 * n - 1); out.lagrange.tau_g2.resize(2 * n - 1);
+        out.lagrange.alpha_tau_g1.resize(2 * n - 1); out.lagrange.beta_tau_g1.resize(2 * n - 1);
+        b2g_powers_desc pd;
+        memset(&pd, 0, sizeof pd);
+        pd.log_size = powers.power;
+        pd.tau_g1 = out.tau_g1.data(); pd.tau_g2 = out.tau_g2.data(); pd.alpha_tau_g1 = out.alpha_tau_g1.data();
+        pd.beta_tau_g1 = out.beta_tau_g1.data(); pd.beta_g2 = &out.beta_g2;
+        b2g_lagrange_out od = {K, 0, out.lagrange.tau_g1.data(), out.lagrange.tau_g2.data(), out.lagrange.alpha_tau_g1.data(),
+                               out.lagrange.beta_tau_g1.data()};
+        check(b2g_powers_prepare(gpu.ctx(), &pd, &od));
+        return out;
     }
 
     // the algebraic checks of `snarkjs powersoftau verify` (b2g_powers_check): whether the prefix a domain of 2^log_n points
@@ -1007,8 +1115,10 @@ struct Groth16T {                                       // Groth16::<Bn254, QAP>
         const size_t n = (size_t)1 << log_n;
         if (powers.tau_g1.size() < 2 * n - 1 || powers.tau_g2.size() < n || powers.alpha_tau_g1.size() < n || powers.beta_tau_g1.size() < n)
             throw std::invalid_argument("verify_powers_of_tau: the powers hold fewer points than a domain of " + std::to_string(n) + " reads");
-        const std::vector<BigInt256> drawn = challenges ? *challenges : powers_challenges();
-        if (drawn.size() != 5) throw std::invalid_argument("verify_powers_of_tau: five challenges (rho, sigma, pi, kappa, eps)");
+        std::vector<BigInt256> drawn = challenges ? *challenges : powers_challenges();
+        if (drawn.size() != 5 && drawn.size() != 6)
+            throw std::invalid_argument("verify_powers_of_tau: five challenges (rho, sigma, pi, kappa, eps) and an optional sixth");
+        if (powers.prepared && drawn.size() == 5) drawn.push_back(powers_challenges()[0]);  // the Lagrange check's rho
         b2g_powers_desc pd;
         memset(&pd, 0, sizeof pd);
         pd.log_size = powers.power;
@@ -1016,12 +1126,28 @@ struct Groth16T {                                       // Groth16::<Bn254, QAP>
         pd.beta_tau_g1 = powers.beta_tau_g1.data(); pd.beta_g2 = &powers.beta_g2;
         b2g_powers_report rep;
         check(b2g_powers_check(gpu.ctx(), &pd, log_n, drawn.data(), &rep));
-        static const char* const arrays[5] = {"tau_g1", "tau_g2", "alpha_tau_g1", "beta_tau_g1", "beta_g2"};
+        if (rep.ok && powers.prepared) {
+            // the Lagrange sections up to log_n (b2g_lagrange_check), with the sixth challenge
+            if (log_n > powers.lagrange.power || powers.lagrange.tau_g1.size() < 4 * n - 1 || powers.lagrange.tau_g2.size() < 2 * n - 1 ||
+                powers.lagrange.alpha_tau_g1.size() < 2 * n - 1 || powers.lagrange.beta_tau_g1.size() < 2 * n - 1 ||
+                (log_n < powers.lagrange.power && powers.tau_g1.size() < 2 * n))
+                throw std::invalid_argument("verify_powers_of_tau: the Lagrange sections hold fewer points than a domain of " +
+                                            std::to_string(n) + " reads");
+            const b2g_lagrange_desc ld = lagrange_desc(powers);
+            check(b2g_lagrange_check(gpu.ctx(), &pd, &ld, log_n, &drawn[5], &rep));
+        }
+        static const char* const arrays[9] = {"tau_g1", "tau_g2", "alpha_tau_g1", "beta_tau_g1", "beta_g2", "lagrange_tau_g1",
+                                              "lagrange_tau_g2", "lagrange_alpha_tau_g1", "lagrange_beta_tau_g1"};
         PowersCheck r;
         r.ok = rep.ok != 0;
         r.rule = rep.rule;
         if (!r.ok && rep.rule != 6) { r.array = arrays[rep.array]; r.index = rep.index; }
         return r;
+    }
+
+    static b2g_lagrange_desc lagrange_desc(const Powers& p) {
+        return b2g_lagrange_desc{p.lagrange.power, 0, p.lagrange.tau_g1.data(), p.lagrange.tau_g2.data(), p.lagrange.alpha_tau_g1.data(),
+                                 p.lagrange.beta_tau_g1.data()};
     }
 
     // `snarkjs zkey verify circuit.r1cs pot.ptau circuit.zkey` without its transcript (b2g_setup_check): whether pk is the key

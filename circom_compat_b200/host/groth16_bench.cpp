@@ -44,6 +44,9 @@
 //   B2G_ZKEY_VERIFY=<file.ptau> groth16_bench <circuit.r1cs> <circuit.zkey>
 //       check the key against the circuit and the ceremony with Groth16T::verify_proving_key (CircomReduction, as snarkjs) and
 //       print key=1, or key=0 and the reason, and the time of the check in ms (the file reads not included)
+//   B2G_PTAU_PREPARE=<in.ptau> groth16_bench <out.ptau> [power]
+//       prepare the ceremony (or the one of the given power formed by its prefix) for phase 2 with
+//       Groth16T::prepare_powers_of_tau and write it with its Lagrange sections 12-15; prints the power and the time in ms
 //   B2G_PTAU_CHECK=<file.ptau> groth16_bench [log_n]
 //       check the ceremony (or the prefix a domain of 2^log_n points reads) with Groth16T::verify_powers_of_tau and print
 //       powers=1 or powers=0 with the reason, and the time of the check in ms (the file read not included)
@@ -176,6 +179,22 @@ int main(int argc, char** argv) {
             for (uint8_t b : serialize_compressed(proof)) std::printf("%02x", b);
             std::printf("\n");
             std::printf("verified=%d\n", Groth16::verify_with_processed_vk(Groth16::process_vk(vk2), in2, p2) ? 1 : 0);
+            return 0;
+        }
+        if (const char* ptau = std::getenv("B2G_PTAU_PREPARE")) {           // ceremony -> its Lagrange sections -> a prepared file
+            if (argc < 2) { std::fprintf(stderr, "usage: B2G_PTAU_PREPARE=<in.ptau> %s <out.ptau> [power]\n", argv[0]); return 2; }
+            const uint32_t power = argc > 2 ? (uint32_t)std::stoul(argv[2]) : 0;
+            std::ifstream pf(ptau, std::ios::binary);
+            if (!pf) throw SerializationError("cannot open ptau");
+            const Powers powers = read_ptau(pf, power);
+            typedef Groth16T<CircomReduction> G;
+            const auto t0 = std::chrono::steady_clock::now();
+            const Powers prepared = G::prepare_powers_of_tau(powers, power);
+            const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+            std::ofstream of(argv[1], std::ios::binary);
+            if (!of) throw SerializationError("cannot open the output file");
+            write_ptau(of, prepared);
+            std::printf("power=%u\nms=%.3f\n", prepared.power, ms);
             return 0;
         }
         if (const char* ptau = std::getenv("B2G_PTAU_CHECK")) {             // ceremony -> its check on the GPU

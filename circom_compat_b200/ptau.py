@@ -8,12 +8,19 @@ The container, as the reader checks it (DESIGN.md restates it):
     section 4: alpha_tau_g1 = alpha tau^i G1,  i < 2^p
     section 5: beta_tau_g1  = beta tau^i G1,   i < 2^p
     section 6: beta_g2      = beta G2 (one point)
+    section 12: lagrange_tau_g1, blocks k = 0 .. p + 1 (2^(p+2) - 1 points)    section 13: lagrange_tau_g2, blocks k = 0 .. p
+    section 14: lagrange_alpha_tau_g1, blocks k = 0 .. p                         section 15: lagrange_beta_tau_g1, k = 0 .. p
 Points are Montgomery little-endian, G1 = x, y (64 B) and G2 = x.c0, x.c1, y.c0, y.c1 (128 B), as in a .zkey; all-zero is
-infinity.  The prepared Lagrange sections 12-15 are not read: b2g_setup_from_powers transforms the monomial powers itself.
+infinity.  Sections 12-15 are what `snarkjs powersoftau prepare phase2` adds: block k starts at point 2^k - 1 and holds
+iNTT_(2^k) of the first 2^k points of the matching monomial section (natural order, scaled by 2^-k), so entry i is L_i(tau)
+times the base point for the domain of 2^k points.  The top block of section 12 has only 2^(p+1) - 1 powers to work from and
+transforms (tau_g1[0 .. 2^(p+1) - 1), infinity).  The reader attaches them as Powers.lagrange only when all four are present
+with the sizes the power implies; otherwise lagrange is None and the Lagrange sections are ignored.
 
-read_ptau returns zero-copy views of sections 2-6 over the file's memory map (or over the given bytes), as rows of 8 / 16
+read_ptau returns zero-copy views of sections 2-6 (and 12-15) over the file's memory map (or over the given bytes), as rows of 8 / 16
 uint64 words, the b2g_pk_desc layout.  Nothing is read beyond the headers until a caller touches the points, and the setup
-reads only the prefix its circuit needs, so a ceremony file much larger than memory serves small circuits.
+reads only the prefix its circuit needs, so a ceremony file much larger than memory serves small circuits.  write_ptau
+streams a Powers back into a container, sections 12-15 included when it carries them.
 
 PowersCheck is the verdict of Groth16.verify_powers_of_tau (b2g_powers_check): truthy when the ceremony passes, with the
 reason of a failure in the messages b2g_setup_from_powers uses ("tau_g2[17]: not in G2").
@@ -21,6 +28,7 @@ reason of a failure in the messages b2g_setup_from_powers uses ("tau_g2[17]: not
 from __future__ import annotations
 
 import os
+import struct
 from dataclasses import dataclass
 
 import numpy as np
@@ -29,6 +37,25 @@ from .zkey import Q_MOD
 
 _G1, _G2 = 64, 128
 _MAX_POWER = 28
+LAGRANGE = ('tau_g1', 'tau_g2', 'alpha_tau_g1', 'beta_tau_g1')
+_LAGRANGE_IDS = (12, 13, 14, 15)
+
+
+def lagrange_counts(power: int) -> tuple:
+    """the points of sections 12-15 of a prepared ceremony of power p: blocks 0 .. p + 1 of G1, then blocks 0 .. p"""
+    return ((4 << power) - 1, (2 << power) - 1, (2 << power) - 1, (2 << power) - 1)
+
+
+@dataclass
+class Lagrange:
+    """sections 12-15 of a ceremony prepared at `power` (views; rows of 8 / 16 uint64 words, affine Montgomery): block k of a
+    section starts at row 2^k - 1 and holds iNTT_(2^k) of the first 2^k points of the monomial section of the same name.
+    Block power + 1 of tau_g1 transforms (tau_g1[0 .. 2^(power+1) - 1), infinity); a prefix keeps `power` and fewer blocks."""
+    power: int
+    tau_g1: np.ndarray
+    tau_g2: np.ndarray
+    alpha_tau_g1: np.ndarray
+    beta_tau_g1: np.ndarray
 
 
 @dataclass
@@ -41,26 +68,42 @@ class Powers:
     alpha_tau_g1: np.ndarray
     beta_tau_g1: np.ndarray
     beta_g2: np.ndarray
+    lagrange: Lagrange = None
 
     def prefix(self, log_n: int, copy: bool = False) -> 'Powers':
         """the points a circuit of domain 2^log_n reads (2n - 1 / n / n / n / 1), as views or, with copy, in host memory;
-        raises ValueError when the arrays hold fewer points or log_n exceeds the power"""
+        raises ValueError when the arrays hold fewer points or log_n exceeds the power.  The Lagrange sections, when present,
+        keep blocks up to log_n + 1 in tau_g1 and up to log_n in the others.  Below the prepared power their top tau_g1 block
+        transforms 2n powers, so the prefix then keeps 2n rows of tau_g1 (the last one is what that block reads)."""
         if not 0 <= log_n <= self.power:
             raise ValueError(f"ptau: a domain of 2^{log_n} points exceeds the ceremony's 2^{self.power}")
         n = 1 << log_n
-        out = []
-        for name, count, words in (('tau_g1', 2 * n - 1, 8), ('tau_g2', n, 16), ('alpha_tau_g1', n, 8), ('beta_tau_g1', n, 8),
-                                   ('beta_g2', 1, 16)):
-            a = np.asarray(getattr(self, name))
-            if a.ndim != 2 or a.shape[1] != words or a.shape[0] < count:
-                raise ValueError(f"ptau: {name} holds {a.shape[0] if a.ndim == 2 else a.size} rows of "
-                                 f"{a.shape[-1] if a.ndim else 0} words; a domain of {n} points reads {count} rows of {words}")
-            a = a[:count]
-            out.append(np.array(a, dtype=np.uint64, order='C', copy=True) if copy else a)
-        return Powers(self.power, self.ceremony_power, *out)
+        lag = self.lagrange
+        t1 = 2 * n if lag is not None and log_n < lag.power else 2 * n - 1
+        out = [_rows_of(getattr(self, name), name, count, words, n, copy)
+               for name, count, words in (('tau_g1', t1, 8), ('tau_g2', n, 16), ('alpha_tau_g1', n, 8), ('beta_tau_g1', n, 8),
+                                          ('beta_g2', 1, 16))]
+        if lag is not None:
+            if log_n > lag.power:
+                raise ValueError(f"ptau: a domain of 2^{log_n} points exceeds the Lagrange sections' 2^{lag.power}")
+            counts = lagrange_counts(log_n)
+            lag = Lagrange(lag.power, *(_rows_of(getattr(lag, name), 'lagrange_' + name, c, 16 if name == 'tau_g2' else 8, n, copy)
+                                        for name, c in zip(LAGRANGE, counts)))
+        return Powers(self.power, self.ceremony_power, *out, lagrange=lag)
+
+
+def _rows_of(a, name, count, words, n, copy):
+    a = np.asarray(a)
+    if a.ndim != 2 or a.shape[1] != words or a.shape[0] < count:
+        raise ValueError(f"ptau: {name} holds {a.shape[0] if a.ndim == 2 else a.size} rows of "
+                         f"{a.shape[-1] if a.ndim else 0} words; a domain of {n} points reads {count} rows of {words}")
+    a = a[:count]
+    return np.array(a, dtype=np.uint64, order='C', copy=True) if copy else a
 
 
 ARRAYS = ('tau_g1', 'tau_g2', 'alpha_tau_g1', 'beta_tau_g1', 'beta_g2')
+# b2g_powers_report array codes: ARRAYS, then the Lagrange sections 12-15
+REPORT_ARRAYS = ARRAYS + tuple('lagrange_' + k for k in LAGRANGE)
 NOT_POWERS = "the powers are not those of one tau, alpha and beta"
 # b2g_powers_report rule codes 1-5 (G1 text, G2 text)
 _RULES = {1: ('a coordinate >= p',) * 2, 2: ('off the curve', 'off the twist'), 3: ('at infinity',) * 2, 4: ('not in G2',) * 2,
@@ -70,7 +113,8 @@ _RULES = {1: ('a coordinate >= p',) * 2, 2: ('off the curve', 'off the twist'), 
 @dataclass
 class PowersCheck:
     """the verdict of a ceremony check: truthy when it passes.  rule (b2g_powers_report): 0 ok, 1 a coordinate >= p, 2 off its
-    curve, 3 at infinity, 4 outside G2, 5 not the generator (array / index name the point), 6 the ratio rules fail"""
+    curve, 3 at infinity, 4 outside G2, 5 not the generator (array / index name the point), 6 the ratio rules fail, 7 the
+    Lagrange section `array` is not the transform of its monomial section"""
     ok: bool
     rule: int = 0
     array: str = None
@@ -85,7 +129,9 @@ class PowersCheck:
             return None
         if self.rule == 6:
             return NOT_POWERS
-        return f"{self.array}[{self.index}]: {_RULES[self.rule][self.array in ('tau_g2', 'beta_g2')]}"
+        if self.rule == 7:
+            return f"{self.array} is not the transform of {self.array[len('lagrange_'):]}"
+        return f"{self.array}[{self.index}]: {_RULES[self.rule][self.array in ('tau_g2', 'beta_g2', 'lagrange_tau_g2')]}"
 
 
 def _buffer(src) -> np.ndarray:
@@ -152,4 +198,64 @@ def read_ptau(src) -> Powers:
         if length != count * rows[sid]:
             raise ValueError(f"ptau: section {sid} holds {length} bytes, but power {power} needs {count * rows[sid]}")
         views[sid] = buf[at:at + length].view('<u8').reshape(count, rows[sid] // 8)
-    return Powers(power, ceremony_power, views[2], views[3], views[4], views[5], views[6])
+    lagrange = None
+    lag_rows = dict(zip(_LAGRANGE_IDS, (_G1, _G2, _G1, _G1)))
+    lag_counts = dict(zip(_LAGRANGE_IDS, lagrange_counts(power)))
+    if all(sid in sections and sections[sid][1] == lag_counts[sid] * lag_rows[sid] for sid in _LAGRANGE_IDS):
+        lagrange = Lagrange(power, *(buf[sections[sid][0]:sections[sid][0] + sections[sid][1]].view('<u8')
+                                     .reshape(lag_counts[sid], lag_rows[sid] // 8) for sid in _LAGRANGE_IDS))
+    return Powers(power, ceremony_power, views[2], views[3], views[4], views[5], views[6], lagrange)
+
+
+_WRITE_CHUNK = 1 << 26                                  # bytes per write: a file far larger than memory streams through
+
+
+def write_ptau(dst, powers: Powers, lagrange_space: bool = False) -> None:
+    """Write `powers` as a snarkjs .ptau container at the path `dst` (or into a writable binary file object): sections 1-6,
+    then 12-15 when powers.lagrange is set.  The arrays must hold the full counts of powers.power (2^(p+1) - 1 / 2^p / 2^p /
+    2^p / 1 points, and lagrange_counts(p) with lagrange.power = p); a prefix of a larger ceremony is refused with a
+    ValueError.  The points are copied in pieces of 64 MiB, so memory-mapped arrays of any size stream to disk.  Section 7,
+    the contribution transcript, is not written: this library neither produces nor checks it, and a reader that needs it (a
+    `snarkjs powersoftau verify`) refuses the file.  With lagrange_space and no powers.lagrange, sections 12-15 are written as
+    zero-filled space (sparse where the file system allows) for a caller that fills them in place through a memory map, as
+    Groth16.prepare_powers_of_tau does."""
+    p = int(powers.power)
+    if not 1 <= p <= _MAX_POWER:
+        raise ValueError(f"ptau: power {p} is out of range (1..{_MAX_POWER})")
+    n = 1 << p
+    parts = [(sid, getattr(powers, name), count, words) for sid, name, count, words in
+             ((2, 'tau_g1', 2 * n - 1, 8), (3, 'tau_g2', n, 16), (4, 'alpha_tau_g1', n, 8), (5, 'beta_tau_g1', n, 8),
+              (6, 'beta_g2', 1, 16))]
+    lag = powers.lagrange
+    if lag is not None:
+        if int(lag.power) != p:
+            raise ValueError(f"ptau: the Lagrange sections are prepared at power {lag.power}, the ceremony has power {p}")
+        parts += [(sid, getattr(lag, name), count, 16 if name == 'tau_g2' else 8)
+                  for sid, name, count in zip(_LAGRANGE_IDS, LAGRANGE, lagrange_counts(p))]
+    reserve = []
+    if lag is None and lagrange_space:
+        reserve = [(sid, count * (128 if sid == 13 else 64)) for sid, count in zip(_LAGRANGE_IDS, lagrange_counts(p))]
+    arrays = []
+    for sid, a, count, words in parts:
+        a = np.asarray(a)
+        if a.dtype.itemsize != 8 or a.ndim != 2 or a.shape != (count, words):
+            raise ValueError(f"ptau: section {sid} needs {count} rows of {words} words at power {p}, not shape {a.shape}")
+        arrays.append((sid, a))
+    own = isinstance(dst, (str, os.PathLike))
+    f = open(dst, 'wb') if own else dst
+    try:
+        f.write(b'ptau' + struct.pack('<II', 1, 1 + len(arrays) + len(reserve)))
+        f.write(struct.pack('<IQI', 1, 4 + 32 + 8, 32) + Q_MOD.to_bytes(32, 'little') + struct.pack('<II', p, int(powers.ceremony_power)))
+        for sid, a in arrays:
+            f.write(struct.pack('<IQ', sid, a.nbytes))
+            step = max(1, _WRITE_CHUNK // (a.shape[1] * 8))
+            for at in range(0, a.shape[0], step):
+                f.write(np.ascontiguousarray(a[at:at + step], dtype='<u8').data)
+        for sid, nbytes in reserve:
+            f.write(struct.pack('<IQ', sid, nbytes))
+            f.seek(nbytes, os.SEEK_CUR)
+        if reserve:
+            f.truncate()
+    finally:
+        if own:
+            f.close()

@@ -34,6 +34,8 @@
  *   b2g_setup_from_powers  <- snarkjs groth16 setup (zkey new): a proving key from a powers-of-tau ceremony
  *   b2g_delta_update / b2g_delta_update_check <- snarkjs zkey contribute / the delta checks of snarkjs zkey verify
  *   b2g_powers_check       <- the algebraic checks of snarkjs powersoftau verify
+ *   b2g_powers_prepare / b2g_lagrange_check <- snarkjs powersoftau prepare phase2 / the check of its sections 12-15
+ *   b2g_setup_from_lagrange <- snarkjs groth16 setup from a prepared ceremony, with no point transforms
  *   b2g_setup_check        <- snarkjs zkey verify: a proving key against its circuit and powers-of-tau ceremony
  *   b2g_fixed_base_g1/g2  <- the batch fixed-base multiplications of that setup, for the standard generators only
  *
@@ -509,9 +511,75 @@ typedef struct {
  * B2G_E_SHAPE for null pointers or a pending proof; B2G_E_DEVICE when the buffers do not fit in device memory. */
 B2G_API int b2g_setup_from_powers(b2g_ctx* ctx, const b2g_mat_desc* circuit, const b2g_powers_desc* powers, b2g_setup_out* out);
 
-/* The verdict of b2g_powers_check.  rule: 0 none (ok), 1 a coordinate >= p, 2 off its curve, 3 at infinity, 4 outside G2,
- * 5 not the generator, 6 the powers are not those of one tau, alpha and beta.  array (rules 1-5): 0 tau_g1, 1 tau_g2,
- * 2 alpha_tau_g1, 3 beta_tau_g1, 4 beta_g2; index: the point in that array. */
+/* The prepared Lagrange sections 12-15 of a ceremony prepared at power p = log_size (what `snarkjs powersoftau prepare phase2`
+ * adds), HOST arrays in the b2g_pk_desc layout.  Block k of a section starts at point 2^k - 1 and holds iNTT_(2^k) of the first
+ * 2^k points of its monomial array (natural order, scaled by 2^-k), so entry i is L_i(tau) times the base point over the domain
+ * of 2^k points:
+ *   tau_g1        blocks k = 0 .. p + 1 (2^(p+2) - 1 points); block p + 1 transforms (tau_g1[0 .. 2^(p+1) - 1), infinity)
+ *   tau_g2, alpha_tau_g1, beta_tau_g1   blocks k = 0 .. p (2^(p+1) - 1 points each).
+ * A call for a domain of 2^log_n points reads only blocks up to log_n (+ 1 for tau_g1): any prefix of whole blocks serves. */
+typedef struct {
+    uint32_t log_size;           /* p, at most 26 */
+    uint32_t reserved;
+    const void* tau_g1;
+    const void* tau_g2;
+    const void* alpha_tau_g1;
+    const void* beta_tau_g1;
+} b2g_lagrange_desc;
+
+/* The output buffers of b2g_powers_prepare: sections 12-15 of a ceremony of power log_size, sized as b2g_lagrange_desc says. */
+typedef struct {
+    uint32_t log_size;
+    uint32_t reserved;
+    void* tau_g1;
+    void* tau_g2;
+    void* alpha_tau_g1;
+    void* beta_tau_g1;
+} b2g_lagrange_out;
+
+/* b2g_powers_prepare <- `snarkjs powersoftau prepare phase2`: sections 12-15 of the ceremony of power K = out->log_size formed by
+ * the prefix of `powers` (tau_g1[0 .. 2^(K+1) - 1), tau_g2 / alpha_tau_g1 / beta_tau_g1[0 .. 2^K)), 1 <= K <= min(log_size, 26),
+ * written into the caller's host buffers (memory-mapped output files serve).  Block K + 1 of tau_g1 is padded with infinity
+ * whatever the input's size, as a ceremony of power K has only 2^(K+1) - 1 powers; K is capped at 26 because that block is a
+ * 2^27-point transform, the limit of b2g_points_intt.
+ * Blocks of fewer than 2^16 points (all four sections) run as ONE segmented pass: one launch per round t, running stage
+ * k - 1 - t of every block k that has one (one launch for the three G1 sections, one for G2), the twiddles of every block taken
+ * from the largest small domain's table, then one segmented finish (bit-reverse, scale by 2^-k, affine) that writes each block
+ * at its section offset.  Below 2^16 points a block's stage is under two waves of the GPU, so per-block launches would only
+ * add latency; the launch count of these blocks is 2 x 15 + 4 whatever K is.  Larger blocks run the transform of
+ * b2g_points_intt, one block at a time.
+ * The call checks what it reads as b2g_setup_from_powers does: every point lies on its curve with coordinates below p, the G2
+ * points are in G2, tau_g1[0] and tau_g2[0] are not at infinity.  Whether the powers are a ceremony is b2g_powers_check's
+ * question.  Cost: per section, the transforms of all blocks, sum_k (2^k / 2) k variable-base products (about twice those of
+ * the top block).  Device memory: about 2^(K+1) x 256 B for the top G1 block (its XYZZ work area, its affine points and its
+ * domain's tables), about 40 MB for the segmented pass, and the output goes back through one 64 MiB pinned staging buffer.
+ * Synchronous.  Errors (every error leaves the context usable; on error the output buffers hold unspecified bytes):
+ * B2G_E_DOMAIN for K outside [1, min(log_size, 26)] or log_size > 28; B2G_E_INPUT for a point that breaks a rule, naming the
+ * array and index ("tau_g2[17]: not in G2"); B2G_E_SHAPE for null pointers or a pending proof; B2G_E_DEVICE when the buffers do
+ * not fit. */
+B2G_API int b2g_powers_prepare(b2g_ctx* ctx, const b2g_powers_desc* powers, const b2g_lagrange_out* out);
+
+/* b2g_setup_from_lagrange: b2g_setup_from_powers without its point transforms.  [L_r], [L_r]_2, [alpha L_r], [beta L_r] are
+ * read from block log_n of the four Lagrange sections instead of transformed; the column sums, the public-input rows and the
+ * LibsnarkReduction H query are those of b2g_setup_from_powers.  The CircomReduction H query is the odd entries of block
+ * log_n + 1 of lagrange tau_g1, which transforms all 2n powers T_0 .. T_(2n-1) except at log_n = lagrange->log_size, where that
+ * block is padded with infinity.  The key keeps b2g_setup_from_powers's (and the reference's) H, the transform of
+ * (T_0 .. T_(2n-2), infinity), so below the prepared power the call subtracts the term of T_(2n-1):
+ *     h_query[i] = B_(2i+1) - (2n)^-1 omega_2n^(2i+1) T_(2n-1)   (B: block log_n + 1),
+ * n products of one point from an 8-bit window table.  tau_g1 must then hold 2n points (it is read at 2n - 1).
+ * The key equals b2g_setup_from_powers's byte for byte when the Lagrange sections are the transforms of the powers, which
+ * b2g_lagrange_check decides.  The call reads and checks the same monomial points as b2g_setup_from_powers, and the Lagrange
+ * points it reads with the same rules (infinity allowed), naming them lagrange_tau_g1 .. lagrange_beta_tau_g1 with the index in
+ * their section.  Errors: those of b2g_setup_from_powers, and B2G_E_DOMAIN for n > 2^lagrange->log_size or
+ * lagrange->log_size > 26. */
+B2G_API int b2g_setup_from_lagrange(b2g_ctx* ctx, const b2g_mat_desc* circuit, const b2g_powers_desc* powers,
+                                    const b2g_lagrange_desc* lagrange, b2g_setup_out* out);
+
+/* The verdict of b2g_powers_check and b2g_lagrange_check.  rule: 0 none (ok), 1 a coordinate >= p, 2 off its curve, 3 at
+ * infinity, 4 outside G2, 5 not the generator, 6 the powers are not those of one tau, alpha and beta, 7 the Lagrange section
+ * `array` is not the transform of its monomial array.  array (rules 1-5, 7): 0 tau_g1, 1 tau_g2, 2 alpha_tau_g1, 3 beta_tau_g1,
+ * 4 beta_g2, 5 lagrange_tau_g1, 6 lagrange_tau_g2, 7 lagrange_alpha_tau_g1, 8 lagrange_beta_tau_g1; index: the point in that
+ * array (its index in the section for 5-8). */
 typedef struct {
     uint8_t ok;
     uint8_t rule;
@@ -551,6 +619,29 @@ typedef struct {
  * a pending proof; B2G_E_DEVICE when the buffers do not fit. */
 B2G_API int b2g_powers_check(b2g_ctx* ctx, const b2g_powers_desc* powers, uint32_t log_n, const void* challenges,
                              b2g_powers_report* out);
+
+/* b2g_lagrange_check: whether blocks 0 .. log_n of the Lagrange sections 13-15 and blocks 0 .. log_n + 1 of section 12
+ * (1 <= log_n <= lagrange->log_size <= 26) are the transforms of the monomial arrays of `powers`.  The transform matrix is
+ * symmetric, so for weights w over a section's blocks
+ *     sum_k sum_i w_(k,i) Lambda_(k,i) = sum_j s_j X_j,   s = sum_k pad(iNTT_(2^k)(w_k));
+ * with w at global section index g equal to rho^g (rho 32 B canonical in [1, r)), the Lagrange side is one streamed MSM in the
+ * powers-of-rho mode and the monomial side one in the explicit-scalar mode, s made once on the scalar NTT.  s is the same for
+ * sections 13-15 (over 2^log_n monomials); section 12 adds its top block (2^(log_n+1) monomials, read from tau_g1, which must
+ * then hold that many points), dropping the coefficient of the infinity that pads block p + 1 when log_n = p.  Each section
+ * gives one equality of points, three in G1 and one in G2; no pairing.  out->ok = 1 iff the point rules hold on every Lagrange
+ * point read (coordinates below p, on its curve, G2 points in G2; infinity allowed) and the four equalities hold.  The monomial
+ * arrays are not checked: b2g_powers_check, which callers run first, does that.
+ * Soundness: an honest file always gives ok = 1.  Once the point rules hold, a wrong section passes with probability at most
+ * (its point count) / (r - 1), and only if rho is drawn uniformly from [1, r) AFTER the file is fixed.  Blocks above log_n are
+ * not read.  A failure names the first failing point (section order, lowest index first), else the first failing section
+ * (rule 7).  The sections are read as b2g_powers_check reads its arrays, once, in slices through pinned staging buffers;
+ * device memory holds those buffers and 32 B x 12 x 2^log_n of scalars.  Cost: two tableless MSMs per section and log_n + 1
+ * scalar transforms.
+ * Synchronous.  Errors (every error leaves the context usable; a malformed point or a failed equality is a verdict): B2G_E_DOMAIN
+ * for log_n outside [1, lagrange->log_size], lagrange->log_size > 26 or above powers->log_size; B2G_E_INPUT for rho 0 or >= r;
+ * B2G_E_SHAPE for null pointers or a pending proof; B2G_E_DEVICE when the buffers do not fit. */
+B2G_API int b2g_lagrange_check(b2g_ctx* ctx, const b2g_powers_desc* powers, const b2g_lagrange_desc* lagrange, uint32_t log_n,
+                               const void* rho_canon, b2g_powers_report* out);
 
 /* A whole proving key with its counts, HOST arrays in the b2g_pk_desc layout (affine Montgomery, all-zero = infinity).  An
  * array may be NULL when its count is 0. */
