@@ -70,6 +70,16 @@ class PowersReport(C.Structure):
     _fields_ = [('ok', C.c_uint8), ('rule', C.c_uint8), ('array', C.c_uint8), ('reserved', C.c_uint8 * 5), ('index', C.c_uint64)]
 
 
+class PowersSecrets(C.Structure):
+    """b2g_powers_secrets: tau, alpha, beta of one phase-1 contribution (32 B canonical each, in [1, r))"""
+    _fields_ = [(k, C.c_void_p) for k in ('tau', 'alpha', 'beta')]
+
+
+class PowersOut(C.Structure):
+    """b2g_powers_out: the host arrays b2g_powers_contribute writes, with the counts of its input"""
+    _fields_ = [(k, C.c_void_p) for k in ('tau_g1', 'tau_g2', 'alpha_tau_g1', 'beta_tau_g1', 'beta_g2')]
+
+
 class KeyDesc(C.Structure):
     """b2g_key_desc: a whole proving key with its counts (host arrays)"""
     _fields_ = [(k, C.c_uint32) for k in ('n_vars', 'n_ic', 'n_l', 'n_h')] + \
@@ -104,7 +114,7 @@ EXPORTS = ['b2g_last_error', 'b2g_version', 'b2g_device_count', 'b2g_ctx_create'
            'b2g_rerandomize_many', 'b2g_points_serialize', 'b2g_points_deserialize', 'b2g_setup',
            'b2g_setup_from_powers', 'b2g_delta_update', 'b2g_delta_update_check', 'b2g_points_intt',
            'b2g_powers_msm', 'b2g_powers_check', 'b2g_setup_check', 'b2g_powers_prepare', 'b2g_lagrange_check',
-           'b2g_setup_from_lagrange']
+           'b2g_setup_from_lagrange', 'b2g_points_scale', 'b2g_powers_contribute']
 
 _lib = None
 
@@ -157,6 +167,8 @@ def lib():
         L.b2g_powers_prepare.argtypes = [vp, C.POINTER(PowersDesc), C.POINTER(LagrangeDesc)]
         L.b2g_lagrange_check.argtypes = [vp, C.POINTER(PowersDesc), C.POINTER(LagrangeDesc), C.c_uint32, vp, C.POINTER(PowersReport)]
         L.b2g_setup_from_lagrange.argtypes = [vp, C.POINTER(MatDesc), C.POINTER(PowersDesc), C.POINTER(LagrangeDesc), C.POINTER(SetupOut)]
+        L.b2g_points_scale.argtypes = [vp, i, sz, vp, vp, vp]
+        L.b2g_powers_contribute.argtypes = [vp, C.POINTER(PowersDesc), C.POINTER(PowersSecrets), C.POINTER(PowersOut)]
         L.b2g_test_op.argtypes = [vp, i, vp, vp, sz, vp]
         L.b2g_last_timings.argtypes = [vp, vp]
         L.b2g_bench_device.argtypes = [vp, vp, vp, i, C.POINTER(C.c_float)]

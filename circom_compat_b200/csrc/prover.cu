@@ -1480,6 +1480,7 @@ int b2g_fixed_base_g2(b2g_ctx* ctx, const void* scalars_canon, size_t n, void* o
 
 int b2g_test_op(b2g_ctx* ctx, int op, const void* a, const void* b, size_t n, void* out) {
     return guarded([&] {
+        if (ctx && op == SCALE_SPLIT_TEST_OP) { DevGuard g(ctx->device); scale_split_test_op(ctx->st[0], a, n, out); return; }
         if (ctx && op >= PAIRING_TEST_OP0) { DevGuard g(ctx->device); pairing_test_op(ctx->st[0], op, a, b, n, out); return; }
         TestOpShape s;
         if (!ctx || !a || !out || !test_op_shape(op, s)) throw_error(B2G_E_SHAPE, "bad arguments");

@@ -74,7 +74,8 @@ _TEST_OP_WORDS = {**{op: (4, 4, 4) for op in (0, 1, 2, 3, 4, 5, 14, 15, 16)}, 6:
                   46: (4, 0, 8), 47: (8, 0, 12), 48: (8, 0, 20),
                   # the verifier's stages: a verify_many Miller value, prepared lines, the window-table product (b: one
                   # G1 point for every row), the window table and verify_batch's prepared-pair Miller value
-                  49: (72, 0, 48), 50: (16, 0, 88 * 24), 51: (4, 8, 16), 52: (8, 0, 32 * 255 * 8), 53: (64, 0, 48)}
+                  49: (72, 0, 48), 50: (16, 0, 88 * 24), 51: (4, 8, 16), 52: (8, 0, 32 * 255 * 8), 53: (64, 0, 48),
+                  54: (4, 0, 16)}
 _TEST_OP_B_ONCE = {51}        # ops whose operand b is one row for all rows of a
 TEST_PAIR_RUN = 16            # entries per row of op 27; an entry is 16 words of affine point + 4 words whose bit 0 is the sign
 
@@ -303,6 +304,20 @@ class Context:
         rb = np.frombuffer(rho.to_bytes(32, 'little'), dtype=np.uint8).copy()
         out = np.zeros(16 if g2 else 8, dtype=np.uint64)
         N.check(N.lib().b2g_powers_msm(self._h, int(bool(g2)), pts.shape[0], _ptr(pts), _ptr(rb), _ptr(out)))
+        return out
+
+    def points_scale(self, points, scalars, g2=False) -> np.ndarray:
+        """b2g_points_scale: k_i P_i for affine Montgomery points (rows of 8 / 16 words) and one canonical scalar per point (ints
+        in [0, r), or rows of 4 uint64 words); affine rows of 8 / 16 words.  G2 points must be in G2: they are not checked."""
+        pts = _c(points).reshape(-1, 16 if g2 else 8)
+        if isinstance(scalars, np.ndarray):
+            sc = _c(scalars).reshape(-1, 4)
+        else:
+            sc = np.frombuffer(b''.join(int(k).to_bytes(32, 'little') for k in scalars), dtype='<u8').reshape(-1, 4)
+        if sc.shape[0] != pts.shape[0]:
+            raise ValueError(f"points_scale: {pts.shape[0]} points and {sc.shape[0]} scalars")
+        out = np.zeros_like(pts)
+        N.check(N.lib().b2g_points_scale(self._h, int(bool(g2)), pts.shape[0], _ptr(pts), _ptr(sc), _ptr(out)))
         return out
 
     def fixed_base_g1(self, scalars_canon) -> np.ndarray:
@@ -963,6 +978,61 @@ class Groth16:
             del outs, mm
             return read_ptau(dst)
         return Powers(K, pre.ceremony_power, *(getattr(pre, k) for k in ARRAYS), lagrange=Lagrange(K, *outs))
+
+    @staticmethod
+    def contribute_powers_of_tau(powers, dst=None, rng=None, ctx: Context = None, tau=None, alpha=None, beta=None):
+        """`snarkjs powersoftau contribute` on the GPU (b2g_powers_contribute): the ceremony of (tau t, alpha a, beta b) from
+        the whole ceremony `powers` of (tau, alpha, beta), with the secrets t, a, b in [1, r) drawn with `secrets` (or
+        rng.randrange when an rng is given) unless given.  The secrets are not returned and the byte buffers that carried them
+        are wiped; the contribution is sound only if nobody keeps them.  Returns a ptau.Powers with the input's power and
+        ceremony_power and no Lagrange sections (the input's no longer match).  With `dst` (a path) the container is written
+        first and its sections filled in place through a memory map, so a ceremony larger than host memory streams, and the
+        result is that file read back (memory-mapped).  Every point read is checked (on its curve, coordinates below p, not at
+        infinity, tau_g1[0] and tau_g2[0] the generators, G2 points in G2); whether the input is a ceremony is
+        verify_powers_of_tau's question, and verify_powers_of_tau on the output is the check of the result."""
+        import secrets as _secrets
+        from .ptau import ARRAYS, Powers, read_ptau, write_ptau
+        power = int(powers.power)
+        if not 1 <= power <= 28:
+            raise ValueError(f"contribute_powers_of_tau: power {power} is outside 1..28")
+        cp = int(getattr(powers, 'ceremony_power', power))
+        pre = Powers(power, cp, *(np.asarray(getattr(powers, k)) for k in ARRAYS)).prefix(power)
+        draw = (lambda: rng.randrange(1, R_MOD)) if rng is not None else (lambda: 1 + _secrets.randbelow(R_MOD - 1))
+        vals = [draw() if v is None else int(v) for v in (tau, alpha, beta)]
+        for name, v in zip(('tau', 'alpha', 'beta'), vals):
+            if not 1 <= v < R_MOD:
+                raise N.B2gError(N.B2G_E_INPUT, f"secret {name} is 0 or >= r")
+        sb = np.frombuffer(b''.join(v.to_bytes(32, 'little') for v in vals), dtype=np.uint8).copy()
+        del vals
+        try:
+            pd, keep = N.PowersDesc(), []
+            pd.log_size = power
+            for name in ARRAYS:
+                a = _c(getattr(pre, name))
+                keep.append(a)
+                setattr(pd, name, a.ctypes.data)
+            if dst is not None:
+                write_ptau(dst, pre, points_space=True)
+                mm = np.memmap(dst, dtype=np.uint8, mode='r+')
+                res = read_ptau(mm)
+                outs = [getattr(res, k) for k in ARRAYS]
+            else:
+                mm = None
+                outs = [np.zeros_like(a) for a in keep]
+            od = N.PowersOut()
+            for name, a in zip(ARRAYS, outs):
+                setattr(od, name, a.ctypes.data)
+            sd = N.PowersSecrets()
+            sd.tau, sd.alpha, sd.beta = sb.ctypes.data, sb.ctypes.data + 32, sb.ctypes.data + 64
+            ctx = ctx or default_context()
+            N.check(N.lib().b2g_powers_contribute(ctx._h, C.byref(pd), C.byref(sd), C.byref(od)))
+        finally:
+            sb[:] = 0
+        if mm is not None:
+            mm.flush()
+            del outs, res, mm
+            return read_ptau(dst)
+        return Powers(power, cp, *outs)
 
     @staticmethod
     def verify_powers_of_tau(powers, log_n=None, ctx: Context = None, challenges=None):

@@ -407,6 +407,26 @@ inline Powers read_ptau(std::istream& r, uint32_t log_n = 0) {
     return p;
 }
 
+// `snarkjs powersoftau new`: the ceremony of power p before any contribution (tau = alpha = beta = 1: every point the standard
+// generator); ceremony_power 0 means p.
+inline Powers new_powers_of_tau(uint32_t power, uint32_t ceremony_power = 0) {
+    if (power < 1 || power > 28) throw std::invalid_argument("new_powers_of_tau: power " + std::to_string(power) + " is outside 1..28");
+    static const uint64_t G1[8] = {0xd35d438dc58f0d9dULL, 0x0a78eb28f5c70b3dULL, 0x666ea36f7879462cULL, 0x0e0a77c19a07df2fULL,
+                                   0xa6ba871b8b1e1b3aULL, 0x14f1d651eb8e167bULL, 0xccdd46def0f28c58ULL, 0x1c14ef83340fbe5eULL};
+    static const uint64_t G2[16] = {0x8e83b5d102bc2026ULL, 0xdceb1935497b0172ULL, 0xfbb8264797811adfULL, 0x19573841af96503bULL,
+                                    0xafb4737da84c6140ULL, 0x6043dd5a5802d8c4ULL, 0x09e950fc52a02f86ULL, 0x14fef0833aea7b6bULL,
+                                    0x619dfa9d886be9f6ULL, 0xfe7fd297f59e9b78ULL, 0xff9e1a62231b7dfeULL, 0x28fd7eebae9e4206ULL,
+                                    0x64095b56c71856eeULL, 0xdc57f922327d3cbbULL, 0x55f935be33351076ULL, 0x0da4a0e693fd6482ULL};
+    G1Affine g1; G2Affine g2;
+    memcpy(&g1, G1, 64); memcpy(&g2, G2, 128);
+    const size_t n = (size_t)1 << power;
+    Powers p;
+    p.power = power; p.ceremony_power = ceremony_power ? ceremony_power : power;
+    p.tau_g1.assign(2 * n - 1, g1); p.tau_g2.assign(n, g2); p.alpha_tau_g1.assign(n, g1); p.beta_tau_g1.assign(n, g1);
+    p.beta_g2 = g2;
+    return p;
+}
+
 // Writes `p` as a .ptau container (sections 1-6, and 12-15 when prepared), as ptau.write_ptau does: the vectors must hold the
 // full counts of p.power (a prefix is refused with std::invalid_argument).  Section 7, the contribution transcript, is not
 // written.
@@ -1102,6 +1122,48 @@ struct Groth16T {                                       // Groth16::<Bn254, QAP>
                                out.lagrange.beta_tau_g1.data()};
         check(b2g_powers_prepare(gpu.ctx(), &pd, &od));
         return out;
+    }
+
+    // `snarkjs powersoftau contribute` (b2g_powers_contribute): the ceremony of (tau t, alpha a, beta b) from the whole
+    // ceremony `powers` of (tau, alpha, beta), the secrets canonical in [1, r); no Lagrange sections (the input's no longer
+    // match).  The library's copies of the secrets and the copies made here are wiped.  Throws std::invalid_argument for vectors
+    // without the counts of powers.power.
+    static Powers contribute_powers_of_tau(const Powers& powers, const BigInt256& t, const BigInt256& a, const BigInt256& b,
+                                           Gpu& gpu = Gpu::instance()) {
+        const size_t n = (size_t)1 << powers.power;
+        if (powers.tau_g1.size() != 2 * n - 1 || powers.tau_g2.size() != n || powers.alpha_tau_g1.size() != n || powers.beta_tau_g1.size() != n)
+            throw std::invalid_argument("contribute_powers_of_tau: the powers do not hold the counts of power " + std::to_string(powers.power));
+        Powers out;
+        out.power = powers.power; out.ceremony_power = powers.ceremony_power;
+        out.tau_g1.resize(2 * n - 1); out.tau_g2.resize(n); out.alpha_tau_g1.resize(n); out.beta_tau_g1.resize(n);
+        b2g_powers_desc pd;
+        memset(&pd, 0, sizeof pd);
+        pd.log_size = powers.power;
+        pd.tau_g1 = powers.tau_g1.data(); pd.tau_g2 = powers.tau_g2.data(); pd.alpha_tau_g1 = powers.alpha_tau_g1.data();
+        pd.beta_tau_g1 = powers.beta_tau_g1.data(); pd.beta_g2 = &powers.beta_g2;
+        b2g_powers_out od = {out.tau_g1.data(), out.tau_g2.data(), out.alpha_tau_g1.data(), out.beta_tau_g1.data(), &out.beta_g2};
+        BigInt256 sec[3] = {t, a, b};
+        const b2g_powers_secrets sd = {sec[0].l, sec[1].l, sec[2].l};
+        const int rc = b2g_powers_contribute(gpu.ctx(), &pd, &sd, &od);
+        volatile uint64_t* wipe = sec[0].l;
+        for (int i = 0; i < 12; i++) wipe[i] = 0;
+        check(rc);
+        return out;
+    }
+    // the same with t, a, b drawn from std::random_device by the Fr::rand limb rule, again while zero
+    static Powers contribute_powers_of_tau(const Powers& powers, Gpu& gpu = Gpu::instance()) {
+        std::random_device rd;
+        auto next = [&rd]() { return ((uint64_t)rd() << 32) | rd(); };
+        BigInt256 s[3];
+        for (BigInt256& x : s) {
+            Fr f;
+            while (f.is_zero()) f = Fr::rand(next);
+            x = f.into_bigint();
+            volatile uint64_t* wipe = f.l;
+            for (int i = 0; i < 4; i++) wipe[i] = 0;
+        }
+        struct Wipe { BigInt256* s; ~Wipe() { volatile uint64_t* w = s[0].l; for (int i = 0; i < 12; i++) w[i] = 0; } } guard{s};
+        return contribute_powers_of_tau(powers, s[0], s[1], s[2], gpu);
     }
 
     // the algebraic checks of `snarkjs powersoftau verify` (b2g_powers_check): whether the prefix a domain of 2^log_n points

@@ -47,6 +47,9 @@
 //   B2G_PTAU_PREPARE=<in.ptau> groth16_bench <out.ptau> [power]
 //       prepare the ceremony (or the one of the given power formed by its prefix) for phase 2 with
 //       Groth16T::prepare_powers_of_tau and write it with its Lagrange sections 12-15; prints the power and the time in ms
+//   B2G_PTAU_CONTRIBUTE=<in.ptau> groth16_bench <out.ptau> [tau alpha beta]
+//       one phase-1 contribution to the whole ceremony with Groth16T::contribute_powers_of_tau, the secrets drawn from
+//       std::random_device unless given (decimal, in [1, r)); writes the file and prints the power and the time in ms
 //   B2G_PTAU_CHECK=<file.ptau> groth16_bench [log_n]
 //       check the ceremony (or the prefix a domain of 2^log_n points reads) with Groth16T::verify_powers_of_tau and print
 //       powers=1 or powers=0 with the reason, and the time of the check in ms (the file read not included)
@@ -67,6 +70,23 @@ static uint64_t fnv(const void* p, size_t n, uint64_t h = 1469598103934665603ULL
     const uint8_t* b = (const uint8_t*)p;
     for (size_t i = 0; i < n; i++) { h ^= b[i]; h *= 1099511628211ULL; }
     return h;
+}
+
+// a decimal scalar below 2^256
+static BigInt256 parse_dec(const std::string& s) {
+    BigInt256 b = {{0, 0, 0, 0}};
+    if (s.empty()) throw std::invalid_argument("empty scalar");
+    for (char c : s) {
+        if (c < '0' || c > '9') throw std::invalid_argument("not a decimal scalar: " + s);
+        unsigned __int128 carry = (unsigned)(c - '0');
+        for (int i = 0; i < 4; i++) {
+            const unsigned __int128 t = (unsigned __int128)b.l[i] * 10 + carry;
+            b.l[i] = (uint64_t)t;
+            carry = t >> 64;
+        }
+        if (carry) throw std::invalid_argument("scalar too long: " + s);
+    }
+    return b;
 }
 
 static BigInt256 parse_hex(const std::string& s) {
@@ -195,6 +215,31 @@ int main(int argc, char** argv) {
             if (!of) throw SerializationError("cannot open the output file");
             write_ptau(of, prepared);
             std::printf("power=%u\nms=%.3f\n", prepared.power, ms);
+            return 0;
+        }
+        if (const char* ptau = std::getenv("B2G_PTAU_CONTRIBUTE")) {        // ceremony -> one contribution -> a new file
+            if (argc != 2 && argc != 5) {
+                std::fprintf(stderr, "usage: B2G_PTAU_CONTRIBUTE=<in.ptau> %s <out.ptau> [tau alpha beta]\n", argv[0]);
+                return 2;
+            }
+            std::ifstream pf(ptau, std::ios::binary);
+            if (!pf) throw SerializationError("cannot open ptau");
+            const Powers powers = read_ptau(pf);
+            typedef Groth16T<CircomReduction> G;
+            const auto t0 = std::chrono::steady_clock::now();
+            Powers out;
+            if (argc == 5) {
+                BigInt256 s[3];
+                for (int k = 0; k < 3; k++) s[k] = parse_dec(argv[2 + k]);
+                out = G::contribute_powers_of_tau(powers, s[0], s[1], s[2]);
+            } else {
+                out = G::contribute_powers_of_tau(powers);
+            }
+            const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+            std::ofstream of(argv[1], std::ios::binary);
+            if (!of) throw SerializationError("cannot open the output file");
+            write_ptau(of, out);
+            std::printf("power=%u\nms=%.3f\n", out.power, ms);
             return 0;
         }
         if (const char* ptau = std::getenv("B2G_PTAU_CHECK")) {             // ceremony -> its check on the GPU

@@ -207,10 +207,35 @@ def read_ptau(src) -> Powers:
     return Powers(power, ceremony_power, views[2], views[3], views[4], views[5], views[6], lagrange)
 
 
+def _generator_rows():
+    """the standard generators G1 = (1, 2) and G2 as one Montgomery row of 8 / 16 words each"""
+    from .zkey import Q_MOD
+    g2 = ((0x1800deef121f1e76426a00665e5c4479674322d4f75edadd46debd5cd992f6ed,
+           0x198e9393920d483a7260bfb731fb5d25f1aa493335a9e71297e485b7aef312c2),
+          (0x12c85ea5db8c6deb4aab71808dcb408fe3d1e7690c43d37b4ce6cc0166fa7daa,
+           0x090689d0585ff075ec9e99ad690c3395bc4b313370b38ef355acdadcd122975b))
+    enc = lambda vals: np.frombuffer(b''.join(((v << 256) % Q_MOD).to_bytes(32, 'little') for v in vals), dtype='<u8').copy()
+    return enc((1, 2)), enc((g2[0][0], g2[0][1], g2[1][0], g2[1][1]))
+
+
+def new_powers_of_tau(power: int, ceremony_power: int = None) -> Powers:
+    """`snarkjs powersoftau new`: the ceremony of power p before any contribution, tau = alpha = beta = 1, so every point is
+    the generator.  The arrays are read-only zero-copy broadcasts of one row (write_ptau streams them to a file;
+    Groth16.contribute_powers_of_tau reads them).  ceremony_power (default p) is kept in section 1."""
+    p = int(power)
+    if not 1 <= p <= _MAX_POWER:
+        raise ValueError(f"ptau: power {p} is out of range (1..{_MAX_POWER})")
+    cp = p if ceremony_power is None else int(ceremony_power)
+    g1, g2 = _generator_rows()
+    n = 1 << p
+    return Powers(p, cp, np.broadcast_to(g1, (2 * n - 1, 8)), np.broadcast_to(g2, (n, 16)), np.broadcast_to(g1, (n, 8)),
+                  np.broadcast_to(g1, (n, 8)), np.broadcast_to(g2, (1, 16)))
+
+
 _WRITE_CHUNK = 1 << 26                                  # bytes per write: a file far larger than memory streams through
 
 
-def write_ptau(dst, powers: Powers, lagrange_space: bool = False) -> None:
+def write_ptau(dst, powers: Powers, lagrange_space: bool = False, points_space: bool = False) -> None:
     """Write `powers` as a snarkjs .ptau container at the path `dst` (or into a writable binary file object): sections 1-6,
     then 12-15 when powers.lagrange is set.  The arrays must hold the full counts of powers.power (2^(p+1) - 1 / 2^p / 2^p /
     2^p / 1 points, and lagrange_counts(p) with lagrange.power = p); a prefix of a larger ceremony is refused with a
@@ -218,7 +243,8 @@ def write_ptau(dst, powers: Powers, lagrange_space: bool = False) -> None:
     the contribution transcript, is not written: this library neither produces nor checks it, and a reader that needs it (a
     `snarkjs powersoftau verify`) refuses the file.  With lagrange_space and no powers.lagrange, sections 12-15 are written as
     zero-filled space (sparse where the file system allows) for a caller that fills them in place through a memory map, as
-    Groth16.prepare_powers_of_tau does."""
+    Groth16.prepare_powers_of_tau does.  With points_space, sections 2-6 are written the same way, as space for the
+    counts of powers.power (their arrays are not read), for Groth16.contribute_powers_of_tau."""
     p = int(powers.power)
     if not 1 <= p <= _MAX_POWER:
         raise ValueError(f"ptau: power {p} is out of range (1..{_MAX_POWER})")
@@ -233,8 +259,11 @@ def write_ptau(dst, powers: Powers, lagrange_space: bool = False) -> None:
         parts += [(sid, getattr(lag, name), count, 16 if name == 'tau_g2' else 8)
                   for sid, name, count in zip(_LAGRANGE_IDS, LAGRANGE, lagrange_counts(p))]
     reserve = []
+    if points_space:
+        reserve = [(sid, count * words * 8) for sid, _, count, words in parts]
+        parts = []
     if lag is None and lagrange_space:
-        reserve = [(sid, count * (128 if sid == 13 else 64)) for sid, count in zip(_LAGRANGE_IDS, lagrange_counts(p))]
+        reserve += [(sid, count * (128 if sid == 13 else 64)) for sid, count in zip(_LAGRANGE_IDS, lagrange_counts(p))]
     arrays = []
     for sid, a, count, words in parts:
         a = np.asarray(a)

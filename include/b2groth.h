@@ -35,6 +35,7 @@
  *   b2g_delta_update / b2g_delta_update_check <- snarkjs zkey contribute / the delta checks of snarkjs zkey verify
  *   b2g_powers_check       <- the algebraic checks of snarkjs powersoftau verify
  *   b2g_powers_prepare / b2g_lagrange_check <- snarkjs powersoftau prepare phase2 / the check of its sections 12-15
+ *   b2g_powers_contribute <- snarkjs powersoftau contribute
  *   b2g_setup_from_lagrange <- snarkjs groth16 setup from a prepared ceremony, with no point transforms
  *   b2g_setup_check        <- snarkjs zkey verify: a proving key against its circuit and powers-of-tau ceremony
  *   b2g_fixed_base_g1/g2  <- the batch fixed-base multiplications of that setup, for the standard generators only
@@ -761,6 +762,54 @@ B2G_API int b2g_points_intt(b2g_ctx* ctx, int g2, int log_n, void* points_mont);
  * pending proof; n = 0 gives infinity. */
 B2G_API int b2g_powers_msm(b2g_ctx* ctx, int g2, size_t n, const void* bases, const void* rho_canon, void* out_affine);
 
+/* b2g_points_scale: out_i = k_i P_i over n host affine points (g2 = 0: G1, 64 B each; 1: G2, 128 B), each with its own
+ * canonical scalar k_i (scalars: n x 32 B little-endian, each below r, else B2G_E_INPUT naming the first that is not); out is
+ * n affine Montgomery points in the same layout (all-zero = infinity), byte-equal to b2g_fixed_base_g1 / g2 of s_i k_i for
+ * P_i = s_i G.  A point at infinity or k_i = 0 gives infinity.  G1 splits k = k1 + k2 lambda with |k1|, |k2| < 2^128 (GLV,
+ * phi(x, y) = (beta x, y)); G2 splits k = k1 + k2 6x^2 with k1, k2 < 2^127 (GLS, psi the twist Frobenius, which acts as [6x^2]
+ * only on G2: G2 points must be in G2, and, as for b2g_points_intt, the points are not checked).  Every lane runs the same 33
+ * signed 4-bit windows over both halves (4 doublings, two additions from a table of 1..8 P per point).  The points are
+ * streamed in slices of 2^22 through pinned staging buffers, so device memory does not grow with n.  Synchronous.  Errors:
+ * B2G_E_SHAPE for null pointers or a pending proof; B2G_E_DEVICE when the buffers do not fit. */
+B2G_API int b2g_points_scale(b2g_ctx* ctx, int g2, size_t n, const void* points, const void* scalars_canon, void* out);
+
+/* The secrets of one phase-1 contribution: tau, alpha, beta, 32 B canonical each, in [1, r). */
+typedef struct {
+    const void* tau;
+    const void* alpha;
+    const void* beta;
+} b2g_powers_secrets;
+
+/* The output of b2g_powers_contribute: caller-owned HOST arrays with the counts of the input ceremony (2^(p+1) - 1 / 2^p /
+ * 2^p / 2^p / 1 points), in the b2g_pk_desc layout; memory-mapped files serve.  None may overlap an input array. */
+typedef struct {
+    void* tau_g1;
+    void* tau_g2;
+    void* alpha_tau_g1;
+    void* beta_tau_g1;
+    void* beta_g2;
+} b2g_powers_out;
+
+/* b2g_powers_contribute <- `snarkjs powersoftau contribute` (phase 1): one contribution with the secrets (t, a, b) to the
+ * whole ceremony `in` of power p = in->log_size (sections 2-6 of a .ptau: T = tau_g1, U = tau_g2, A = alpha_tau_g1,
+ * B = beta_tau_g1, beta_2 = beta_g2):
+ *     T'_i = t^i T_i (i < 2^(p+1) - 1),  U'_i = t^i U_i,  A'_i = a t^i A_i,  B'_i = b t^i B_i (i < 2^p),  beta_2' = b beta_2.
+ * A ceremony of (tau, alpha, beta) becomes the ceremony of (tau t, alpha a, beta b).  The exponent of point i is its index in
+ * the whole array.  Each array is streamed once in slices of 2^22 points: the scalars c t^i (c = 1, a or b) are made on the
+ * device per slice, and each point is one b2g_points_scale product.  Cost: 2^(p+2) - 1 G1 and 2^p + 1 G2 variable-base
+ * products (about 1.3 billion points at p = 28), plus the point rules.  The call checks every point it reads, as
+ * b2g_powers_prepare does: coordinates below p, on its curve, not at infinity, tau_g1[0] and tau_g2[0] the standard generators,
+ * every G2 point in G2 (which the G2 split needs); the first failure is refused naming the array and index
+ * ("tau_g2[17]: not in G2").  The contribution is sound only if t, a and b are discarded: anyone who knows them can undo it.
+ * The library's host copy of the secrets is wiped once it has reached the device, every device buffer that held them or the
+ * per-point scalars (any two consecutive scalars give t) is zeroed before it is freed, on errors too, and nothing returns them.
+ * snarkjs's transcript (section 7: the hash chain and the proofs of knowledge of t, a and b) is not produced.
+ * Synchronous.  Errors (every error leaves the context usable; on error the output arrays hold unspecified bytes):
+ * B2G_E_DOMAIN for log_size outside 1..28; B2G_E_INPUT for a secret that is 0 or >= r, or a point that breaks a rule;
+ * B2G_E_SHAPE for null pointers, an output that overlaps the input, or a pending proof; B2G_E_DEVICE when the buffers do not
+ * fit. */
+B2G_API int b2g_powers_contribute(b2g_ctx* ctx, const b2g_powers_desc* in, const b2g_powers_secrets* secrets, const b2g_powers_out* out);
+
 /* Element-wise device arithmetic, for unit parity tests of the field / group layers.
  * op: 0 fq_mul, 1 fq_add, 2 fq_sub, 3 fr_mul, 4 fr_add, 5 fr_sub, 6 fq_inv, 7 fr_inv (b ignored),
  *     8 g1_add (a, b, out = n x 64 B affine), 9 g2_add (n x 128 B), 10 g1_dbl, 11 g2_dbl (b ignored),
@@ -803,6 +852,8 @@ B2G_API int b2g_powers_msm(b2g_ctx* ctx, int g2, size_t n, const void* bases, co
  *     52 the 8-bit window table of a G1 affine a (64 B): out = 32 x 255 affine points d * 256^w * a (w-major),
  *     53 the Miller value of verify_batch's two prepared pairs: a = 512 B, the prepared inputs and sum r C (G1 XYZZ, 128 B
  *        each), gamma, delta: out = 384 B.
+ * Op 54 is b2g_points_scale's scalar decomposition (b ignored): a = k (32 B canonical, below r): out = 128 B, the G1 split
+ *     k = k1 + k2 lambda (mod r), then the G2 split k = k1 + k2 6x^2, each half as 32 B little-endian two's complement.
  * Operand and result sizes per row therefore differ by op; b may be NULL where the op does not read it. */
 B2G_API int b2g_test_op(b2g_ctx* ctx, int op, const void* a, const void* b, size_t n, void* out);
 
