@@ -5,7 +5,7 @@ read_zkey, ProvingKey, ConstraintMatrices, CircomReduction, Groth16.  All arithm
 (hand-written sm_90a CUDA behind include/b2groth.h); there is no CPU fallback.
 """
 from .zkey import read_zkey, ProvingKey, ConstraintMatrices, fr_to_mont, fr_from_mont  # noqa: F401
-from .groth16 import Groth16, CircomReduction, LibsnarkReduction, Proof, Context, release, release_all  # noqa: F401
+from .groth16 import Groth16, CircomReduction, LibsnarkReduction, Proof, Context, ProvingKeyGroup, release, release_all  # noqa: F401
 from .r1cs import R1CSFile, R1CS, read_wtns  # noqa: F401
 from .builder import CircomConfig, CircomBuilder, CircomCircuit  # noqa: F401
 from .verifier import VerifyingKey, PreparedVerifyingKey, MalformedVerifyingKey  # noqa: F401

@@ -114,7 +114,8 @@ EXPORTS = ['b2g_last_error', 'b2g_version', 'b2g_device_count', 'b2g_ctx_create'
            'b2g_rerandomize_many', 'b2g_points_serialize', 'b2g_points_deserialize', 'b2g_setup',
            'b2g_setup_from_powers', 'b2g_delta_update', 'b2g_delta_update_check', 'b2g_points_intt',
            'b2g_powers_msm', 'b2g_powers_check', 'b2g_setup_check', 'b2g_powers_prepare', 'b2g_lagrange_check',
-           'b2g_setup_from_lagrange', 'b2g_points_scale', 'b2g_powers_contribute']
+           'b2g_setup_from_lagrange', 'b2g_points_scale', 'b2g_powers_contribute',
+           'b2g_pk_group_load', 'b2g_pk_group_free', 'b2g_prove_keys', 'b2g_pk_group_layout']
 
 _lib = None
 
@@ -141,6 +142,10 @@ def lib():
         L.b2g_witness_map.argtypes = [vp, vp, vp, vp, C.POINTER(C.c_uint32)]
         L.b2g_prove.argtypes = [vp, vp, vp, vp, vp, vp, vp]
         L.b2g_prove_many.argtypes = [vp, vp, vp, C.c_uint32, vp, vp, vp, vp]
+        L.b2g_pk_group_load.argtypes = [vp, C.c_uint32, C.POINTER(PkDesc), vp, C.POINTER(vp)]
+        L.b2g_pk_group_free.argtypes = [vp]
+        L.b2g_prove_keys.argtypes = [vp, vp, vp, vp, vp, vp, vp]
+        L.b2g_pk_group_layout.argtypes = [C.c_uint32, vp, vp, vp, vp, vp, vp, vp]
         L.b2g_prove_submit.argtypes = [vp, vp, vp, vp, vp, vp, vp]
         L.b2g_prove_wait.argtypes = [vp]
         L.b2g_host_register.argtypes = [vp, sz]

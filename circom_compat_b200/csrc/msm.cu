@@ -95,10 +95,8 @@ __device__ __forceinline__ int32_t msm_digit_at(const uint32_t* __restrict__ k, 
 // leader's with high probability, and on uniform data the rounds cost four ballots.  Lanes still pending add individually.
 constexpr int MSM_LEADER_ROUNDS = 2;
 
-__global__ void __launch_bounds__(256) msm_count_kernel(const fe* __restrict__ canon, uint32_t n, int c, int nwin, uint32_t nb, uint32_t* __restrict__ counts) {
-    canon += (size_t)blockIdx.y * n;
-    counts += (size_t)blockIdx.y * nb;
-    const uint64_t tid = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+// histogram of the digits of one (window, scalar) pair per thread: `tid` < n * nwin of one proof's canonical scalars
+__device__ __forceinline__ void msm_count_digits(const fe* __restrict__ canon, uint32_t n, int c, int nwin, uint32_t* __restrict__ counts, uint64_t tid) {
     const uint32_t w = (uint32_t)(tid / n), i = (uint32_t)(tid % n);
     int32_t d = 0;
     if (w < (uint32_t)nwin) d = msm_digit_at(canon[i].l, c, (int)w);
@@ -124,6 +122,12 @@ __global__ void __launch_bounds__(256) msm_count_kernel(const fe* __restrict__ c
         if (mine) pending = false;
     }
     if (pending) atomicAdd(&counts[b], 1u);
+}
+
+__global__ void __launch_bounds__(256) msm_count_kernel(const fe* __restrict__ canon, uint32_t n, int c, int nwin, uint32_t nb, uint32_t* __restrict__ counts) {
+    canon += (size_t)blockIdx.y * n;
+    counts += (size_t)blockIdx.y * nb;
+    msm_count_digits(canon, n, c, nwin, counts, (uint64_t)blockIdx.x * blockDim.x + threadIdx.x);
 }
 
 // ------------------------------------------------------------------------------------------------ (2) exclusive scan (one CTA)
@@ -161,18 +165,16 @@ __global__ void __launch_bounds__(1024) msm_scan_kernel(const uint32_t* __restri
 }
 
 // ------------------------------------------------------------------------------------------------ (3) scatter
-__global__ void __launch_bounds__(256) msm_scatter_kernel(const fe* __restrict__ canon, uint32_t n, uint32_t row_stride, int c, int nwin, uint32_t nb,
-                                   const uint32_t* __restrict__ offsets, uint32_t* __restrict__ cursor, uint32_t* __restrict__ entries) {
-    canon += (size_t)blockIdx.y * n;
-    offsets += (size_t)blockIdx.y * nb;                    // global positions in the batch's one sorted list
-    cursor += (size_t)blockIdx.y * nb;
-    const uint64_t tid = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+// the entries of one (window, scalar) pair per thread in bucket order: table row row0 + w * row_stride + i, bit 31 for a negative digit
+__device__ __forceinline__ void msm_scatter_digits(const fe* __restrict__ canon, uint32_t n, uint32_t row0, uint32_t row_stride, int c, int nwin,
+                                                   const uint32_t* __restrict__ offsets, uint32_t* __restrict__ cursor, uint32_t* __restrict__ entries,
+                                                   uint64_t tid) {
     const uint32_t w = (uint32_t)(tid / n), i = (uint32_t)(tid % n);
     int32_t d = 0;
     if (w < (uint32_t)nwin) d = msm_digit_at(canon[i].l, c, (int)w);
     const uint32_t b = d ? (uint32_t)(d < 0 ? -d : d) - 1u : 0xffffffffu;
     const uint32_t lane = threadIdx.x & 31;
-    const uint32_t entry = (w * row_stride + i) | (d < 0 ? 0x80000000u : 0u);
+    const uint32_t entry = (row0 + w * row_stride + i) | (d < 0 ? 0x80000000u : 0u);
     bool pending = d != 0;
     {   // hot bucket 0 first (see msm_count_kernel)
         const uint32_t hot = __ballot_sync(0xffffffffu, pending && b == 0u);
@@ -204,6 +206,14 @@ __global__ void __launch_bounds__(256) msm_scatter_kernel(const fe* __restrict__
         }
     }
     if (pending) entries[offsets[b] + atomicAdd(&cursor[b], 1u)] = entry;
+}
+
+__global__ void __launch_bounds__(256) msm_scatter_kernel(const fe* __restrict__ canon, uint32_t n, uint32_t row_stride, int c, int nwin, uint32_t nb,
+                                   const uint32_t* __restrict__ offsets, uint32_t* __restrict__ cursor, uint32_t* __restrict__ entries) {
+    canon += (size_t)blockIdx.y * n;
+    offsets += (size_t)blockIdx.y * nb;                    // global positions in the batch's one sorted list
+    cursor += (size_t)blockIdx.y * nb;
+    msm_scatter_digits(canon, n, 0u, row_stride, c, nwin, offsets, cursor, entries, (uint64_t)blockIdx.x * blockDim.x + threadIdx.x);
 }
 
 // ------------------------------------------------------------------------------------------------ (4) accumulate
@@ -514,6 +524,16 @@ void msm_build_table(MsmPlan& plan, const void* bases_dev, uint32_t n, bool g2, 
     else msm_build_table_t<G1, Fq>(plan, bases_dev, n, st);
 }
 
+// rows [0, nwin(c) * n) of `table` (a key's place in a group's arena, b2g_pk_group_load) at a window size given by the group
+void msm_build_table_into(void* table, const void* bases_dev, uint32_t n, int c, bool g2, cudaStream_t st) {
+    if (n == 0) return;
+    msm_validate_points(bases_dev, n, g2, st, "the query slice");
+    if (g2) msm_table_kernel<G2, Fq2><<<(n + 127) / 128, 128, 0, st>>>(bases_dev, n, c, msm_nwin(c), table);
+    else msm_table_kernel<G1, Fq><<<(n + 127) / 128, 128, 0, st>>>(bases_dev, n, c, msm_nwin(c), table);
+    g_launch_count += 1;
+    CUDA_CHECK(cudaGetLastError());
+}
+
 void msm_free_table(MsmPlan& plan) { if (plan.table) cudaFree(plan.table); plan.table = nullptr; }
 
 // count: proofs of a batch the buffers hold (sorted entries, buckets, fragments and partials scale with it)
@@ -574,6 +594,55 @@ void msm_sort(const MsmPlan& plan, MsmScratch& s, const fe* scalars_dev, uint32_
     msm_scan_kernel<<<1, 1024, 0, st>>>(s.counts, nb, s.offsets, s.cursor);
     // table rows are indexed w * plan.n + i (the table was built over plan.n bases, n may be shorter)
     msm_scatter_kernel<<<pair_grid, SORT_CTA, 0, st>>>(s.scalars_canon, n, plan.n, plan.c, plan.nwin, plan.nbuckets, s.offsets, s.cursor, s.entries);
+    g_launch_count += 4;
+    CUDA_CHECK(cudaGetLastError());
+}
+
+// ------------------------------------------------------------------------------------------------ keyed digit passes
+// A batch whose proofs belong to different keys (b2g_prove_keys): proof j = blockIdx.y reads its own row of `rows` - base
+// count n, first scalar, first canonical slot and the arena row of its key's table.  Its bucket key stays j * nb + b, so the
+// scan, accumulation, fold and weighted reduction run unchanged.  A CTA past the proof's own n (or n * nwin) pairs leaves
+// whole, so every warp that stays runs the ballots of the histogram and scatter with all its lanes.
+__global__ void __launch_bounds__(256) msm_canon_keyed_kernel(const fe* __restrict__ scalars, const KeyedRow* __restrict__ rows, int scalars_mont,
+                                                              fe* __restrict__ canon_out) {
+    const KeyedRow r = rows[blockIdx.y];
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= r.n) return;
+    fe k = fe_load_nc(&scalars[r.src + i]);
+    if (scalars_mont) k = Fr::to_canonical(k);
+    fe_store(&canon_out[r.canon + i], k);
+}
+
+__global__ void __launch_bounds__(256) msm_count_keyed_kernel(const fe* __restrict__ canon, const KeyedRow* __restrict__ rows, int c, int nwin, uint32_t nb,
+                                                              uint32_t* __restrict__ counts) {
+    const KeyedRow r = rows[blockIdx.y];
+    if ((uint64_t)blockIdx.x * blockDim.x >= (uint64_t)r.n * nwin) return;
+    msm_count_digits(canon + r.canon, r.n, c, nwin, counts + (size_t)blockIdx.y * nb, (uint64_t)blockIdx.x * blockDim.x + threadIdx.x);
+}
+
+__global__ void __launch_bounds__(256) msm_scatter_keyed_kernel(const fe* __restrict__ canon, const KeyedRow* __restrict__ rows, int c, int nwin, uint32_t nb,
+                                                                const uint32_t* __restrict__ offsets, uint32_t* __restrict__ cursor, uint32_t* __restrict__ entries) {
+    const KeyedRow r = rows[blockIdx.y];
+    if ((uint64_t)blockIdx.x * blockDim.x >= (uint64_t)r.n * nwin) return;
+    msm_scatter_digits(canon + r.canon, r.n, r.row, r.n, c, nwin, offsets + (size_t)blockIdx.y * nb, cursor + (size_t)blockIdx.y * nb, entries,
+                       (uint64_t)blockIdx.x * blockDim.x + threadIdx.x);
+}
+
+void msm_sort_keyed(const MsmPlan& plan, MsmScratch& s, const fe* scalars_dev, bool scalars_mont, const KeyedRow* rows_dev, uint32_t count,
+                    uint32_t max_n, uint64_t total_n, cudaStream_t st) {
+    // the accumulation sizes its runs by sorted_n * nwin * count: the mean base count per proof, rounded up, covers every entry
+    s.sorted_n = (uint32_t)((total_n + count - 1) / count); s.sorted_count = count;
+    if (total_n == 0 || plan.table == nullptr) { s.sorted_n = 0; return; }
+    if (s.sorted_n > s.cap_n || plan.nwin > s.cap_nwin || plan.nbuckets > s.cap_buckets || count > s.cap_count || !s.entries)
+        throw_error(B2G_E_SHAPE, "msm: keyed sort scratch too small");
+    const uint32_t nb = plan.nbuckets * count;
+    constexpr unsigned SORT_CTA = 256;
+    CUDA_CHECK(cudaMemsetAsync(s.counts, 0, (size_t)nb * 4, st));
+    const dim3 pair_grid((unsigned)(((uint64_t)max_n * plan.nwin + SORT_CTA - 1) / SORT_CTA), count);
+    msm_canon_keyed_kernel<<<dim3((max_n + SORT_CTA - 1) / SORT_CTA, count), SORT_CTA, 0, st>>>(scalars_dev, rows_dev, scalars_mont ? 1 : 0, s.scalars_canon);
+    msm_count_keyed_kernel<<<pair_grid, SORT_CTA, 0, st>>>(s.scalars_canon, rows_dev, plan.c, plan.nwin, plan.nbuckets, s.counts);
+    msm_scan_kernel<<<1, 1024, 0, st>>>(s.counts, nb, s.offsets, s.cursor);
+    msm_scatter_keyed_kernel<<<pair_grid, SORT_CTA, 0, st>>>(s.scalars_canon, rows_dev, plan.c, plan.nwin, plan.nbuckets, s.offsets, s.cursor, s.entries);
     g_launch_count += 4;
     CUDA_CHECK(cudaGetLastError());
 }

@@ -64,6 +64,16 @@ inline int msm_pick_c(uint32_t n) {
 }
 inline int msm_nwin(int c) { return (255 + c - 1) / c; }
 
+// Keyed batches (b2g_prove_keys): the proofs of one call belong to different keys whose tables of a query lie side by side
+// in one arena built at one window size.  Proof j's row: its base count, its first scalar (elements into the scalar vector),
+// its first slot of the canonical copy and the first arena row of its key (key k's row of base i in window w: row + w * n + i).
+struct KeyedRow { uint64_t src; uint64_t canon; uint32_t n; uint32_t row; };
+// sorts `count` proofs described by rows_dev (device) into one list of count * plan.nbuckets buckets; max_n / total_n: the
+// largest and the summed n of the rows.  plan: the group's c, nwin, nbuckets and arena.
+void msm_sort_keyed(const MsmPlan& plan, MsmScratch& s, const fe* scalars_dev, bool scalars_mont, const KeyedRow* rows_dev, uint32_t count,
+                    uint32_t max_n, uint64_t total_n, cudaStream_t st);
+void msm_build_table_into(void* table, const void* bases_dev, uint32_t n, int c, bool g2, cudaStream_t st);
+
 // ------------------------------------------------------------------------------------------------ tableless streamed MSM
 // sum_i rho^i P_i over bases read once (b2g_powers_msm, b2g_powers_check), in slices of at most POWERS_SLICE points.  No
 // window table: a base costs one mixed addition per window, so every window keeps its own bucket set.  Per slice the scalars

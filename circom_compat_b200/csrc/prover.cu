@@ -6,6 +6,8 @@
 //     streams 1..4: MSMs over l_query / a_query[1..] / b_g1_query[1..] / b_g2_query[1..] against the witness
 //     streams 2, 3: s*msm_A, r*msm_B1 right behind those MSMs; side stream: r*delta1, s*delta2, K_C (the (r, s)-only terms)
 //     stream 0: glue (A, B2 and C = K_C + s*msm_A + r*msm_B1 + msm_L + msm_H, three affine conversions) -> D2H 256 B
+#include <algorithm>
+#include <array>
 #include <atomic>
 #include <chrono>
 #include <cstring>
@@ -79,6 +81,12 @@ struct b2g_ctx {
     void* peer_mapped[64] = {};                // cudaIpcOpenMemHandle results (to close)
     int peers_imported = 0;
     VerifyBufs* vbufs = nullptr;               // b2g_verify_many scratch (verify.cu), grown on demand
+    // b2g_prove_keys: the per-proof rows of its three sorts and the key of every proof (rewritten by each call), and the pass
+    // captured as a graph of its own, for (group uid, buffer generation, counts of every key)
+    uint8_t* d_keyed = nullptr; size_t cap_keyed = 0;
+    cudaGraphExec_t gexec_keys = nullptr;
+    std::vector<uint64_t> gk_key;
+    uint64_t gk_launches = 0;
 };
 
 static std::atomic<uint64_t> g_next_uid{1};            // handles are told apart by uid, not by address (addresses get reused)
@@ -97,6 +105,25 @@ struct b2g_pk {
     // position (inside the shard's w[1..] range) of the j-th real base; the proof gathers those scalars and sorts them on their own
     uint32_t* d_bidx = nullptr;
     uint32_t b_compact = 0;
+};
+
+namespace b2g { struct KeyGlue; }
+
+// K proving keys loaded for proving under all of them in one pass (b2g_pk_group_load).  Every query's tables of all keys lie
+// in one arena built at one window size; key k's rows of query q start at row[q][k].  The per-key state a proof reads besides
+// those tables - glue constants, their window tables, the sparse-B compaction - sits in a b2g_pk of its own whose plan[q]
+// holds no table, only the key's base count of the query.
+struct b2g_pk_group {
+    uint64_t uid = g_next_uid++;
+    int device = 0;
+    std::vector<b2g_pk*> keys;
+    std::vector<b2g_mat*> mats;                // the caller's matrices, one per key (not owned)
+    MsmPlan plan[NQ];                          // per query: the group's c, nwin, nbuckets; table = the arena
+    std::vector<uint32_t> row[NQ];
+    KeyGlue* d_keys = nullptr;                 // per key: the four window tables of glue_pre
+    const uint8_t** d_consts = nullptr;        // per key: its d_consts (glue_post)
+    bool b_sparse = false;                     // some key's B query is compacted: B1 and B2 get a sort of their own
+    const uint32_t** d_bidx = nullptr;         // per key: d_bidx, null for a dense B query
 };
 
 struct b2g_mat {
@@ -126,13 +153,12 @@ CtxView ctx_view(b2g_ctx* ctx) { return {ctx->device, ctx->st[0], ctx->pending_o
 // C = K_C + s*msm_A + r*msm_B1 + msm_L + msm_H  (A = alpha + a0 + msm_A + r*delta1, B1 likewise).
 // One CTA per proof of a batch: CTA j reads (r, s) at rs[2j], rs[2j + 1] and writes pre + j * PRE_BYTES.
 constexpr size_t PRE_BYTES = 2 * 128 + 256;
-__global__ void __launch_bounds__(160) glue_pre_kernel(const void* __restrict__ tab_d1, const void* __restrict__ tab_d2, const void* __restrict__ tab_aa,
-                                                       const void* __restrict__ tab_bb, const Scalar256* __restrict__ rs, uint8_t* __restrict__ pre) {
+// one proof's precomputation by one CTA of 160 threads: (r, s) at rs[0], rs[1], result at pre
+__device__ __forceinline__ void glue_pre_one(const void* __restrict__ tab_d1, const void* __restrict__ tab_d2, const void* __restrict__ tab_aa,
+                                             const void* __restrict__ tab_bb, const Scalar256* __restrict__ rs, uint8_t* __restrict__ pre) {
     __shared__ G1::Pt sh1[4][32];
     __shared__ G2::Pt sh2[32];
     __shared__ G1::Pt res[4];
-    rs += 2 * blockIdx.x;
-    pre += (size_t)blockIdx.x * PRE_BYTES;
     const Scalar256 r = rs[0], s = rs[1];
     const int warp = threadIdx.x >> 5;
     const bool lead = (threadIdx.x & 31) == 0;
@@ -162,6 +188,11 @@ __global__ void __launch_bounds__(160) glue_pre_kernel(const void* __restrict__ 
         G1::add(kc, res[3]);
         pt_store<Fq>(pre, 1, kc);
     }
+}
+
+__global__ void __launch_bounds__(160) glue_pre_kernel(const void* __restrict__ tab_d1, const void* __restrict__ tab_d2, const void* __restrict__ tab_aa,
+                                                       const void* __restrict__ tab_bb, const Scalar256* __restrict__ rs, uint8_t* __restrict__ pre) {
+    glue_pre_one(tab_d1, tab_d2, tab_aa, tab_bb, rs + 2 * blockIdx.x, pre + (size_t)blockIdx.x * PRE_BYTES);
 }
 
 // out = k * p for one XYZZ point (the partial A / B1 MSM result of a rank) - in a whole proof issued on that MSM's own stream
@@ -219,6 +250,71 @@ __global__ void glue_post_kernel(const uint8_t* __restrict__ partials, int count
         G2::Aff b = G2::to_affine(acc);
         store_canon(proof, 2, b.x.c0); store_canon(proof, 3, b.x.c1); store_canon(proof, 4, b.y.c0); store_canon(proof, 5, b.y.c1);
     }
+}
+
+// ------------------------------------------------------------------------------------------------ keyed batches (b2g_prove_keys)
+// The window tables of one key of a group that glue_pre_keys_kernel reads (b2g_pk_group::d_keys)
+struct KeyGlue { const void *d1, *d2, *aa, *bb; };
+
+// CTA j = proof j of a keyed batch: glue_pre_kernel with proof j's key's tables (key_of[j])
+__global__ void __launch_bounds__(160) glue_pre_keys_kernel(const KeyGlue* __restrict__ keys, const uint32_t* __restrict__ key_of,
+                                                            const Scalar256* __restrict__ rs, uint8_t* __restrict__ pre) {
+    const KeyGlue k = keys[key_of[blockIdx.x]];
+    glue_pre_one(k.d1, k.d2, k.aa, k.bb, rs + 2 * blockIdx.x, pre + (size_t)blockIdx.x * PRE_BYTES);
+}
+
+// CTA j = proof j of a keyed batch: glue_post_kernel's assembly from proof j's one record, with its key's constants
+// (consts_of[key_of[j]]).  The body is glue_post_kernel's, restated rather than shared: sharing it changes the code
+// ptxas makes for glue_post_kernel (a smaller stack frame), and the one-key kernel is left exactly as it was.
+__global__ void glue_post_keys_kernel(const uint8_t* __restrict__ partials, const uint8_t* const* __restrict__ consts_of,
+                                      const uint32_t* __restrict__ key_of, const uint8_t* __restrict__ pre, uint8_t* __restrict__ proof) {
+    constexpr int count = 1;
+    const uint8_t* __restrict__ consts = consts_of[key_of[blockIdx.x]];
+    partials += (size_t)blockIdx.x * count * REC_BYTES;
+    pre += (size_t)blockIdx.x * PRE_BYTES;
+    proof += (size_t)blockIdx.x * 256;
+    const int warp = threadIdx.x >> 5;
+    if ((threadIdx.x & 31) != 0) return;
+    if (warp == 0) {
+        // A = r*delta1 + a_query[0] + msm_A + alpha1
+        G1::Pt acc = pt_load<Fq>(pre, 0);
+        G1::madd(acc, aff_load<Fq>(consts, 3));
+        for (int k = 0; k < count; k++) { G1::Pt q = pt_load<Fq>(partials + (size_t)k * REC_BYTES + 256, 0); G1::add(acc, q); }
+        G1::madd(acc, aff_load<Fq>(consts, 0));
+        G1::Aff a = G1::to_affine(acc);
+        store_canon(proof, 0, a.x); store_canon(proof, 1, a.y);
+    } else if (warp == 1) {
+        // C = K_C + sum_k (s*A_k + r*B1_k + L_k + H_k)
+        G1::Pt acc = pt_load<Fq>(pre, 1);
+        for (int k = 0; k < count; k++) {
+            const uint8_t* rec = partials + (size_t)k * REC_BYTES;
+            G1::Pt q = pt_load<Fq>(rec + B2G_PARTIAL_BYTES, 0); G1::add(acc, q);
+            q = pt_load<Fq>(rec + B2G_PARTIAL_BYTES + 128, 0); G1::add(acc, q);
+            q = pt_load<Fq>(rec + 128, 0); G1::add(acc, q);
+            q = pt_load<Fq>(rec, 0); G1::add(acc, q);
+        }
+        G1::Aff c = G1::to_affine(acc);
+        store_canon(proof, 6, c.x); store_canon(proof, 7, c.y);
+    } else {
+        // B2 = s*delta2 + b_g2_query[0] + msm_B2 + beta2
+        G2::Pt acc = pt_load<Fq2>(pre + 2 * 128, 0);
+        G2::madd(acc, aff_load<Fq2>(consts + 5 * 64, 2));
+        for (int k = 0; k < count; k++) { G2::Pt q = pt_load<Fq2>(partials + (size_t)k * REC_BYTES + 512, 0); G2::add(acc, q); }
+        G2::madd(acc, aff_load<Fq2>(consts + 5 * 64, 0));
+        G2::Aff b = G2::to_affine(acc);
+        store_canon(proof, 2, b.x.c0); store_canon(proof, 3, b.x.c1); store_canon(proof, 4, b.y.c0); store_canon(proof, 5, b.y.c1);
+    }
+}
+
+// blockIdx.y = proof j: the scalars of its B queries (rows brows[j]) from its witness (w[1..] at wrows[j].src), through its key's
+// compaction index when its B query is sparse (bidx[key] non-null), in the proof's own place of the gathered vector
+__global__ void __launch_bounds__(256) gather_scalars_keyed_kernel(const fe* __restrict__ w, const KeyedRow* __restrict__ wrows, const KeyedRow* __restrict__ brows,
+                                                                   const uint32_t* __restrict__ key_of, const uint32_t* const* __restrict__ bidx, fe* __restrict__ out) {
+    const KeyedRow b = brows[blockIdx.y];
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= b.n) return;
+    const uint32_t* idx = bidx[key_of[blockIdx.y]];
+    fe_store(&out[b.src + i], fe_load_nc(&w[wrows[blockIdx.y].src + (idx ? idx[i] : i)]));
 }
 
 // ------------------------------------------------------------------------------------------------ peer-memory exchange
@@ -548,17 +644,19 @@ static void ensure_scratch(b2g_ctx* ctx, const b2g_pk* pk, uint32_t count = 1) {
     ctx->scratch_ok = true;
 }
 
-// the witness map of `count` proofs side by side: one launch per kernel of the chain, the batch on a grid dimension
-static void run_witness_map(b2g_ctx* ctx, b2g_mat* mat, cudaStream_t st, uint32_t count = 1) {
+// the witness map of `count` proofs side by side: one launch per kernel of the chain, the batch on a grid dimension.  The
+// first witness at d_w + w_off, the first a / b / c / h vector at v_off (b2g_prove_keys: one key's proofs of a keyed batch).
+static void run_witness_map(b2g_ctx* ctx, b2g_mat* mat, cudaStream_t st, uint32_t count = 1, size_t w_off = 0, size_t v_off = 0) {
+    fe *w = ctx->d_w + w_off, *a = ctx->d_a + v_off, *b = ctx->d_b + v_off, *c = ctx->d_c + v_off, *h = ctx->d_h + v_off;
     if (mat->reduction == B2G_REDUCTION_LIBSNARK) {
         spmv_launch(mat->n, mat->m, mat->num_inputs, mat->a_rowptr, mat->a_col, mat->a_val, mat->b_rowptr, mat->b_col, mat->b_val,
-                    ctx->d_w, ctx->d_a, ctx->d_b, ctx->d_c, st, mat->c_rowptr, mat->c_col, mat->c_val, count, mat->n_vars);
-        ntt_witness_transform_libsnark(mat->dom, ctx->d_a, ctx->d_b, ctx->d_c, ctx->d_a, ctx->d_h, st, count);   // d_a doubles as scratch
+                    w, a, b, c, st, mat->c_rowptr, mat->c_col, mat->c_val, count, mat->n_vars);
+        ntt_witness_transform_libsnark(mat->dom, a, b, c, a, h, st, count);   // a doubles as scratch
         return;
     }
     spmv_launch(mat->n, mat->m, mat->num_inputs, mat->a_rowptr, mat->a_col, mat->a_val, mat->b_rowptr, mat->b_col, mat->b_val,
-                ctx->d_w, ctx->d_a, ctx->d_b, ctx->d_c, st, nullptr, nullptr, nullptr, count, mat->n_vars);
-    ntt_witness_transform(mat->dom, ctx->d_a, ctx->d_b, ctx->d_c, ctx->d_h, st, count);
+                w, a, b, c, st, nullptr, nullptr, nullptr, count, mat->n_vars);
+    ntt_witness_transform(mat->dom, a, b, c, h, st, count);
 }
 
 // a key's tables live on one device and describe one shard: checked before the first kernel that dereferences them
@@ -673,6 +771,61 @@ static void pk_release(b2g_pk* pk) {
     delete pk;
 }
 
+
+// Sparse B: the support of the B polynomials inside a shard's range [lo, lo + cnt) of w[1..] (a base counts if it is a real
+// point in either group).  True when fewer than 80 % of them are real: then idx = their positions and packed = their G1 / G2
+// bases side by side.
+static bool b_support(const b2g_pk_desc* d, uint32_t lo, uint32_t cnt, std::vector<uint32_t>& idx, std::vector<uint8_t> packed[2]) {
+    const uint8_t* b1 = (const uint8_t*)d->b_g1_query + (size_t)(1 + lo) * 64;
+    const uint8_t* b2 = (const uint8_t*)d->b_g2_query + (size_t)(1 + lo) * 128;
+    auto nonzero = [](const uint8_t* p, size_t n) { const uint64_t* w = (const uint64_t*)p; uint64_t o = 0; for (size_t i = 0; i < n / 8; i++) o |= w[i]; return o != 0; };
+    idx.clear();
+    for (uint32_t i = 0; i < cnt; i++) if (nonzero(b1 + (size_t)i * 64, 64) || nonzero(b2 + (size_t)i * 128, 128)) idx.push_back(i);
+    const char* off = getenv("B2G_NO_B_COMPACT");
+    if (!(off && *off == '1') && cnt >= 1024 && (uint64_t)idx.size() * 5 < (uint64_t)cnt * 4) {
+        packed[0].resize(idx.size() * 64 + 64); packed[1].resize(idx.size() * 128 + 128);
+        for (size_t j = 0; j < idx.size(); j++) { memcpy(&packed[0][j * 64], b1 + (size_t)idx[j] * 64, 64); memcpy(&packed[1][j * 128], b2 + (size_t)idx[j] * 128, 128); }
+        return true;
+    }
+    idx.clear();
+    return false;
+}
+
+// a key's glue constants and the 8-bit window tables of its fixed bases (delta_g1, delta_g2, alpha_g1 + a_query[0],
+// beta_g1 + b_g1_query[0]); synchronises `st`
+static void pk_load_glue(b2g_pk* pk, const b2g_pk_desc* d, cudaStream_t st) {
+    std::vector<uint8_t> consts(5 * 64 + 3 * 128);
+    memcpy(&consts[0], d->alpha_g1, 64); memcpy(&consts[64], d->beta_g1, 64); memcpy(&consts[128], d->delta_g1, 64);
+    memcpy(&consts[192], d->a_query, 64); memcpy(&consts[256], d->b_g1_query, 64);
+    memcpy(&consts[320], d->beta_g2, 128); memcpy(&consts[448], d->delta_g2, 128); memcpy(&consts[576], d->b_g2_query, 128);
+    pk->d_consts = dev_upload<uint8_t>(consts.data(), consts.size(), st);
+    // alpha, beta, delta and the three query[0] points never pass through a table build: G1Affine::new / G2Affine::new
+    // validate them in the reference (src/zkey.rs:340-360), so they are checked here as well
+    msm_validate_points(pk->d_consts, 5, false, st, "alpha_g1 / beta_g1 / delta_g1 / a_query[0] / b_g1_query[0]");
+    msm_validate_points(pk->d_consts + 5 * 64, 3, true, st, "beta_g2 / delta_g2 / b_g2_query[0]");
+    CUDA_CHECK(cudaMalloc(&pk->d_tab_delta1, 32 * 255 * 64));
+    CUDA_CHECK(cudaMalloc(&pk->d_tab_delta2, 32 * 255 * 128));
+    CUDA_CHECK(cudaMalloc(&pk->d_tab_aa, 32 * 255 * 64 + 64));
+    CUDA_CHECK(cudaMalloc(&pk->d_tab_bb, 32 * 255 * 64 + 64));
+    fixed_table_kernel<G1, Fq><<<(32 * 255 + 63) / 64, 64, 0, st>>>(pk->d_tab_delta1, pk->d_consts + 2 * 64);
+    fixed_table_kernel<G2, Fq2><<<(32 * 255 + 63) / 64, 64, 0, st>>>(pk->d_tab_delta2, pk->d_consts + 5 * 64 + 128);
+    // alpha1 + a_query[0] and beta1 + b_g1_query[0] (affine sums parked behind their tables), then their window tables
+    affine_sum_kernel<<<1, 1, 0, st>>>(pk->d_consts, 0, 3, (uint8_t*)pk->d_tab_aa + 32 * 255 * 64);
+    affine_sum_kernel<<<1, 1, 0, st>>>(pk->d_consts, 1, 4, (uint8_t*)pk->d_tab_bb + 32 * 255 * 64);
+    fixed_table_kernel<G1, Fq><<<(32 * 255 + 63) / 64, 64, 0, st>>>(pk->d_tab_aa, (uint8_t*)pk->d_tab_aa + 32 * 255 * 64);
+    fixed_table_kernel<G1, Fq><<<(32 * 255 + 63) / 64, 64, 0, st>>>(pk->d_tab_bb, (uint8_t*)pk->d_tab_bb + 32 * 255 * 64);
+    g_launch_count += 6;
+    CUDA_CHECK(cudaGetLastError());
+    CUDA_CHECK(cudaStreamSynchronize(st));
+}
+
+// header checks of a proving-key descriptor (b2g_pk_load, b2g_pk_group_load)
+static void pk_desc_check(const b2g_pk_desc* d) {
+    if (d->n_vars < d->n_public + 1 || d->domain_size == 0) throw_error(B2G_E_SHAPE, "bad proving-key header");
+    for (const void* p : {d->alpha_g1, d->beta_g1, d->delta_g1, d->beta_g2, d->delta_g2, d->a_query, d->b_g1_query, d->b_g2_query, d->h_query})
+        if (!p) throw_error(B2G_E_SHAPE, "null proving-key section");
+    if (d->n_vars - (d->n_public + 1) && !d->l_query) throw_error(B2G_E_SHAPE, "null proving-key section");
+}
 
 // (r, s) -> ctx->d_rs on stream 0.  Every entry point synchronises stream 0 before it returns (b2g_bench_device stages once),
 // so the pinned staging slot is free again by the time the next call overwrites it.  count proofs: r, s = count x 32 B each,
@@ -833,6 +986,8 @@ int b2g_ctx_destroy(b2g_ctx* ctx) {
         cudaEventDestroy(ctx->ev_w); cudaEventDestroy(ctx->ev_sort); cudaEventDestroy(ctx->ev_pre); cudaEventDestroy(ctx->ev_fork); cudaEventDestroy(ctx->ev_sortb); cudaStreamDestroy(ctx->st_glue);
         if (ctx->d_wb) cudaFree(ctx->d_wb);
         for (auto& g : ctx->gexec) if (g) cudaGraphExecDestroy(g);
+        if (ctx->gexec_keys) cudaGraphExecDestroy(ctx->gexec_keys);
+        if (ctx->d_keyed) cudaFree(ctx->d_keyed);
         if (ctx->h_rs) cudaFreeHost(ctx->h_rs);
         if (ctx->h_proof) cudaFreeHost(ctx->h_proof);
         if (ctx->d_rs) cudaFree(ctx->d_rs);
@@ -849,9 +1004,7 @@ int b2g_ctx_destroy(b2g_ctx* ctx) {
 int b2g_pk_load(b2g_ctx* ctx, const b2g_pk_desc* d, b2g_pk** out) {
     return guarded([&] {
         if (!ctx || !d || !out) throw_error(B2G_E_SHAPE, "null pointer");
-        if (d->n_vars < d->n_public + 1 || d->domain_size == 0) throw_error(B2G_E_SHAPE, "bad proving-key header");
-        for (const void* p : {d->alpha_g1, d->beta_g1, d->delta_g1, d->beta_g2, d->delta_g2, d->a_query, d->b_g1_query, d->b_g2_query, d->h_query})
-            if (!p) throw_error(B2G_E_SHAPE, "null proving-key section");
+        pk_desc_check(d);
         DevGuard g(ctx->device);
         cudaStream_t st = ctx->st[0];
         // everything allocated below is released if any later step throws (off-curve point, out of memory, ...)
@@ -865,7 +1018,6 @@ int b2g_pk_load(b2g_ctx* ctx, const b2g_pk_desc* d, b2g_pk** out) {
         // query sizes as paired with scalars by create_proof_with_assignment (SURVEY.md 3.4)
         // L, A, B1, B2 all pair bases with w[1..n_vars): L is re-indexed onto that range by prepending (l - 1) points at
         // infinity (l_query[j] belongs to w[l + j]), so the four queries share one digit sort per proof.
-        if (d->n_vars - li && !d->l_query) throw_error(B2G_E_SHAPE, "null proving-key section");
         std::vector<uint8_t> l_padded((size_t)(d->n_vars - 1) * 64, 0);
         if (d->n_vars - li) memcpy(l_padded.data() + (size_t)(li - 1) * 64, d->l_query, (size_t)(d->n_vars - li) * 64);
         const uint32_t total[NQ] = {d->domain_size, d->n_vars - 1, d->n_vars - 1, d->n_vars - 1, d->n_vars - 1};
@@ -882,19 +1034,9 @@ int b2g_pk_load(b2g_ctx* ctx, const b2g_pk_desc* d, b2g_pk** out) {
             pk->cnt[q] = (uint32_t)((uint64_t)total[q] * (r + 1) / R) - pk->lo[q];
             pk->scalar_off[q] = soff[q];
             if (total[q] && !src[q]) throw_error(B2G_E_SHAPE, "null proving-key section");
-            if (q == Q_B1) {
-                // support of the B polynomials inside this shard: a base counts if it is a real point in either group
-                const uint8_t* b1 = (const uint8_t*)d->b_g1_query + (size_t)(1 + pk->lo[q]) * 64;
-                const uint8_t* b2 = (const uint8_t*)d->b_g2_query + (size_t)(1 + pk->lo[q]) * 128;
-                auto nonzero = [](const uint8_t* p, size_t n) { const uint64_t* w = (const uint64_t*)p; uint64_t o = 0; for (size_t i = 0; i < n / 8; i++) o |= w[i]; return o != 0; };
-                for (uint32_t i = 0; i < pk->cnt[q]; i++) if (nonzero(b1 + (size_t)i * 64, 64) || nonzero(b2 + (size_t)i * 128, 128)) bidx.push_back(i);
-                const char* off = getenv("B2G_NO_B_COMPACT");
-                if (!(off && *off == '1') && pk->cnt[q] >= 1024 && (uint64_t)bidx.size() * 5 < (uint64_t)pk->cnt[q] * 4) {
-                    pk->b_compact = (uint32_t)bidx.size();
-                    bpacked[0].resize(bidx.size() * 64 + 64); bpacked[1].resize(bidx.size() * 128 + 128);
-                    for (size_t j = 0; j < bidx.size(); j++) { memcpy(&bpacked[0][j * 64], b1 + (size_t)bidx[j] * 64, 64); memcpy(&bpacked[1][j * 128], b2 + (size_t)bidx[j] * 128, 128); }
-                    pk->d_bidx = dev_upload<uint32_t>(bidx.data(), bidx.size() * 4, st);
-                } else bidx.clear();
+            if (q == Q_B1 && b_support(d, pk->lo[q], pk->cnt[q], bidx, bpacked)) {
+                pk->b_compact = (uint32_t)bidx.size();
+                pk->d_bidx = dev_upload<uint32_t>(bidx.data(), bidx.size() * 4, st);
             }
             if (pk->d_bidx && (q == Q_B1 || q == Q_B2)) {
                 if (pk->b_compact) guard.tmp = dev_upload<uint8_t>(bpacked[g2 ? 1 : 0].data(), (size_t)pk->b_compact * aff, st);
@@ -910,29 +1052,7 @@ int b2g_pk_load(b2g_ctx* ctx, const b2g_pk_desc* d, b2g_pk** out) {
             CUDA_CHECK(cudaStreamSynchronize(st));
             if (guard.tmp) { cudaFree(guard.tmp); guard.tmp = nullptr; }
         }
-        std::vector<uint8_t> consts(5 * 64 + 3 * 128);
-        memcpy(&consts[0], d->alpha_g1, 64); memcpy(&consts[64], d->beta_g1, 64); memcpy(&consts[128], d->delta_g1, 64);
-        memcpy(&consts[192], d->a_query, 64); memcpy(&consts[256], d->b_g1_query, 64);
-        memcpy(&consts[320], d->beta_g2, 128); memcpy(&consts[448], d->delta_g2, 128); memcpy(&consts[576], d->b_g2_query, 128);
-        pk->d_consts = dev_upload<uint8_t>(consts.data(), consts.size(), st);
-        // alpha, beta, delta and the three query[0] points never pass through a table build: G1Affine::new / G2Affine::new
-        // validate them in the reference (src/zkey.rs:340-360), so they are checked here as well
-        msm_validate_points(pk->d_consts, 5, false, st, "alpha_g1 / beta_g1 / delta_g1 / a_query[0] / b_g1_query[0]");
-        msm_validate_points(pk->d_consts + 5 * 64, 3, true, st, "beta_g2 / delta_g2 / b_g2_query[0]");
-        CUDA_CHECK(cudaMalloc(&pk->d_tab_delta1, 32 * 255 * 64));
-        CUDA_CHECK(cudaMalloc(&pk->d_tab_delta2, 32 * 255 * 128));
-        CUDA_CHECK(cudaMalloc(&pk->d_tab_aa, 32 * 255 * 64 + 64));
-        CUDA_CHECK(cudaMalloc(&pk->d_tab_bb, 32 * 255 * 64 + 64));
-        fixed_table_kernel<G1, Fq><<<(32 * 255 + 63) / 64, 64, 0, st>>>(pk->d_tab_delta1, pk->d_consts + 2 * 64);
-        fixed_table_kernel<G2, Fq2><<<(32 * 255 + 63) / 64, 64, 0, st>>>(pk->d_tab_delta2, pk->d_consts + 5 * 64 + 128);
-        // alpha1 + a_query[0] and beta1 + b_g1_query[0] (affine sums parked behind their tables), then their window tables
-        affine_sum_kernel<<<1, 1, 0, st>>>(pk->d_consts, 0, 3, (uint8_t*)pk->d_tab_aa + 32 * 255 * 64);
-        affine_sum_kernel<<<1, 1, 0, st>>>(pk->d_consts, 1, 4, (uint8_t*)pk->d_tab_bb + 32 * 255 * 64);
-        fixed_table_kernel<G1, Fq><<<(32 * 255 + 63) / 64, 64, 0, st>>>(pk->d_tab_aa, (uint8_t*)pk->d_tab_aa + 32 * 255 * 64);
-        fixed_table_kernel<G1, Fq><<<(32 * 255 + 63) / 64, 64, 0, st>>>(pk->d_tab_bb, (uint8_t*)pk->d_tab_bb + 32 * 255 * 64);
-        g_launch_count += 6;
-        CUDA_CHECK(cudaGetLastError());
-        CUDA_CHECK(cudaStreamSynchronize(st));
+        pk_load_glue(pk, d, st);
         guard.pk = nullptr;
         *out = pk;
     });
@@ -1498,6 +1618,404 @@ int b2g_test_op(b2g_ctx* ctx, int op, const void* a, const void* b, size_t n, vo
         cudaError_t e = cudaStreamSynchronize(st);
         cudaFree(da); if (db) cudaFree(db); cudaFree(dout);
         CUDA_CHECK(e);
+    });
+}
+
+}  // extern "C"
+
+// ================================================================================================== keyed batches
+namespace b2g {
+
+static const char* const QUERY_NAME[NQ] = {"H", "L", "A", "B1", "B2"};
+// the three sorts of a keyed pass: H over h, W over w[1..] (its entries serve L and A), B over the gathered B scalars (B1 and B2)
+enum { S_H = 0, S_W = 1, S_B = 2, NS = 3 };
+static const int SORT_QUERY[NS] = {Q_H, Q_A, Q_B1};
+
+// one key's base count per query: H the domain, L and A n_vars - 1, B1 and B2 n_vars - 1 or the count of its real B bases
+using KeyBases = std::array<uint32_t, NQ>;
+
+// the window size of each query (msm_pick_c on its largest base count in the group) and each key's first arena row
+struct GroupLayout {
+    int c[NQ] = {};
+    uint64_t rows[NQ] = {};
+    std::vector<uint32_t> row[NQ];
+};
+
+static GroupLayout group_layout(const std::vector<KeyBases>& bases) {
+    if (bases.empty()) throw_error(B2G_E_SHAPE, "b2g_pk_group_load: the group has no keys");
+    GroupLayout L;
+    for (int q = 0; q < NQ; q++) {
+        uint32_t most = 0;
+        for (const KeyBases& b : bases) most = std::max(most, b[q]);
+        L.c[q] = msm_pick_c(most ? most : 1);
+        const int nwin = msm_nwin(L.c[q]);
+        for (const KeyBases& b : bases) {
+            L.row[q].push_back((uint32_t)L.rows[q]);
+            L.rows[q] += (uint64_t)b[q] * nwin;
+            // an entry word is a table row with the sign in bit 31
+            if (L.rows[q] >= (1ull << 31))
+                throw_error(B2G_E_SHAPE, std::string("b2g_pk_group_load: the tables of query ") + QUERY_NAME[q] +
+                                         " reach 2^31 rows (the sign bit of an entry word); load fewer or smaller keys per group");
+        }
+    }
+    return L;
+}
+
+// the per-proof tables of one call: rows [S_H | S_W | S_B] x count, the key of every proof, and where each key's witnesses
+// (n_vars apart) and witness-map vectors (its domain apart) start in the call's buffers; proofs come key after key
+struct CallLayout {
+    uint32_t count = 0;
+    std::vector<KeyedRow> rows;
+    std::vector<uint32_t> key_of;
+    uint32_t max_n[NS] = {};
+    uint64_t total_n[NS] = {};
+    std::vector<uint64_t> w_off, v_off;
+    uint64_t total_w = 0, total_v = 0;
+};
+
+static CallLayout call_layout(const GroupLayout& G, const std::vector<KeyBases>& bases, const std::vector<uint32_t>& n_vars,
+                              const std::vector<uint32_t>& n_dom, const uint32_t* counts) {
+    const size_t K = bases.size();
+    uint64_t total = 0;
+    for (size_t k = 0; k < K; k++) total += counts[k];
+    if (total == 0 || total > MAX_BATCH) throw_error(B2G_E_SHAPE, "b2g_prove_keys: the total count must be in [1, " + std::to_string(MAX_BATCH) + "]");
+    CallLayout C;
+    C.count = (uint32_t)total;
+    C.rows.resize((size_t)NS * total);
+    for (size_t k = 0; k < K; k++) {
+        C.w_off.push_back(C.total_w); C.v_off.push_back(C.total_v);
+        for (uint32_t i = 0; i < counts[k]; i++) {
+            const uint32_t j = (uint32_t)C.key_of.size();
+            C.key_of.push_back((uint32_t)k);
+            const uint64_t src[NS] = {C.total_v, C.total_w + 1, C.total_n[S_B]};      // h[0], w[1], the gathered B scalars
+            for (int t = 0; t < NS; t++) {
+                const int q = SORT_QUERY[t];
+                C.rows[(size_t)t * total + j] = {src[t], C.total_n[t], bases[k][q], G.row[q][k]};
+                C.total_n[t] += bases[k][q];
+                C.max_n[t] = std::max(C.max_n[t], bases[k][q]);
+            }
+            C.total_w += n_vars[k]; C.total_v += n_dom[k];
+        }
+    }
+    // the sorted entries and bucket keys of the whole call are u32 positions into one list
+    for (int t = 0; t < NS; t++) {
+        const int q = SORT_QUERY[t];
+        if (C.total_n[t] * (uint64_t)msm_nwin(G.c[q]) >= (1ull << 32) || total << (G.c[q] - 1) >= (1ull << 32))
+            throw_error(B2G_E_SHAPE, std::string("b2g_prove_keys: proofs x bases x windows of query ") + QUERY_NAME[q] +
+                                     " reach 2^32 sorted entries; prove fewer per call");
+    }
+    return C;
+}
+
+static void group_release(b2g_pk_group* g) {
+    for (b2g_pk* pk : g->keys) pk_release(pk);
+    for (int q = 0; q < NQ; q++) msm_free_table(g->plan[q]);
+    if (g->d_keys) cudaFree(g->d_keys);
+    if (g->d_bidx) cudaFree(g->d_bidx);
+    if (g->d_consts) cudaFree(g->d_consts);
+    delete g;
+}
+
+static std::vector<KeyBases> group_bases(const b2g_pk_group* g) {
+    std::vector<KeyBases> b;
+    for (const b2g_pk* pk : g->keys) b.push_back({pk->plan[Q_H].n, pk->plan[Q_L].n, pk->plan[Q_A].n, pk->plan[Q_B1].n, pk->plan[Q_B2].n});
+    return b;
+}
+
+// the context's MSM scratch for a keyed call: every query holds count proofs of the mean base count of its sort (rounded up),
+// at the group's window size; H and L (the W sort) with sort buffers, and B1 (the B sort) when some key's B query is sparse.
+// Without one, B1 and B2 read the W sort as in a one-key proof with a dense B query.
+static void ensure_scratch_keys(b2g_ctx* ctx, const b2g_pk_group* g, const CallLayout& C) {
+    uint32_t navg[NQ];
+    const int sb = g->b_sparse ? S_B : S_W;
+    const int sort_of[NQ] = {S_H, S_W, S_W, sb, sb};
+    for (int q = 0; q < NQ; q++) navg[q] = std::max<uint32_t>(1, (uint32_t)((C.total_n[sort_of[q]] + C.count - 1) / C.count));
+    const size_t nwb = g->b_sparse ? C.total_n[S_B] : 0;
+    bool ok = ctx->scratch_ok && (!g->b_sparse || (ctx->scratch_bsort && nwb <= ctx->cap_wb));
+    for (int q = 0; q < NQ && ok; q++) {
+        const MsmPlan& p = g->plan[q]; const MsmScratch& sc = ctx->scratch[q];
+        if (navg[q] > sc.cap_n || p.nwin > sc.cap_nwin || p.nbuckets > sc.cap_buckets || C.count > sc.cap_count) ok = false;
+    }
+    if (ok) return;
+    CUDA_CHECK(cudaDeviceSynchronize());
+    for (int q = 0; q < NQ; q++) msm_scratch_free(ctx->scratch[q]);
+    ctx->scratch_ok = false; ctx->alloc_gen++;
+    for (int q = 0; q < NQ; q++) {
+        const MsmPlan& p = g->plan[q];
+        msm_scratch_alloc(ctx->scratch[q], navg[q], p.nwin, p.nbuckets, q == Q_B2, q == Q_H || q == Q_L || (q == Q_B1 && g->b_sparse), C.count);
+        cudaFree(ctx->scratch[q].result);
+        ctx->scratch[q].result = ctx->d_partial + PARTIAL_OFF[q];
+        ctx->scratch[q].result_owned = false;
+        ctx->scratch[q].result_stride = REC_BYTES;
+    }
+    ctx->scratch_bsort = g->b_sparse;
+    if (nwb > ctx->cap_wb) {
+        if (ctx->d_wb) cudaFree(ctx->d_wb);
+        ctx->d_wb = nullptr; ctx->cap_wb = 0;
+        CUDA_CHECK(cudaMalloc(&ctx->d_wb, (nwb + 1) * sizeof(fe)));
+        ctx->cap_wb = nwb;
+    }
+    ctx->scratch_ok = true;
+}
+
+// the rows and key_of of a call, in one device buffer the captured pass points into
+static void ensure_keyed_buffer(b2g_ctx* ctx, size_t bytes) {
+    if (bytes <= ctx->cap_keyed) return;
+    CUDA_CHECK(cudaDeviceSynchronize());
+    if (ctx->d_keyed) cudaFree(ctx->d_keyed);
+    ctx->d_keyed = nullptr; ctx->cap_keyed = 0; ctx->alloc_gen++;
+    CUDA_CHECK(cudaMalloc(&ctx->d_keyed, bytes));
+    ctx->cap_keyed = bytes;
+}
+
+// The keyed pass, launched as launch_msms + the glue launch a batch of one key: glue_pre on the side stream; the W sort on
+// the L stream and, when some key's B query is sparse, the B gather and sort on the B1 stream, both from the witnesses; the
+// A, B1, B2, L accumulations on their streams (A and B1 followed by s*A, r*B1); on stream 0 the witness map of every key
+// with proofs, then the H sort and accumulation; the assembly once everything is in.
+static void enqueue_keys(b2g_ctx* ctx, b2g_pk_group* g, const CallLayout& C, const uint32_t* counts) {
+    cudaStream_t s0 = ctx->st[0], ssort = ctx->st[Q_L], sb = ctx->st[Q_B1];
+    const uint32_t count = C.count;
+    const KeyedRow* rows = reinterpret_cast<const KeyedRow*>(ctx->d_keyed);
+    const uint32_t* key_of = reinterpret_cast<const uint32_t*>(rows + (size_t)NS * count);
+    const Scalar256* rs = reinterpret_cast<const Scalar256*>(ctx->d_rs);
+    CUDA_CHECK(cudaEventRecord(ctx->ev_fork, s0));
+    CUDA_CHECK(cudaStreamWaitEvent(ctx->st_glue, ctx->ev_fork, 0));
+    glue_pre_keys_kernel<<<count, 160, 0, ctx->st_glue>>>(g->d_keys, key_of, rs, ctx->d_pre);
+    CUDA_CHECK(cudaEventRecord(ctx->ev_pre, ctx->st_glue));
+    g_launch_count += 1;
+    CUDA_CHECK(cudaEventRecord(ctx->ev_w, s0));
+    CUDA_CHECK(cudaStreamWaitEvent(ssort, ctx->ev_w, 0));
+    msm_sort_keyed(g->plan[Q_A], ctx->scratch[Q_L], ctx->d_w, true, rows + (size_t)S_W * count, count, C.max_n[S_W], C.total_n[S_W], ssort);
+    CUDA_CHECK(cudaEventRecord(ctx->ev_sort, ssort));
+    if (g->b_sparse) {
+        CUDA_CHECK(cudaStreamWaitEvent(sb, ctx->ev_w, 0));
+        if (C.total_n[S_B]) {
+            gather_scalars_keyed_kernel<<<dim3((C.max_n[S_B] + 255) / 256, count), 256, 0, sb>>>(ctx->d_w, rows + (size_t)S_W * count, rows + (size_t)S_B * count,
+                                                                                                   key_of, g->d_bidx, ctx->d_wb);
+            g_launch_count += 1;
+        }
+        msm_sort_keyed(g->plan[Q_B1], ctx->scratch[Q_B1], ctx->d_wb, true, rows + (size_t)S_B * count, count, C.max_n[S_B], C.total_n[S_B], sb);
+        CUDA_CHECK(cudaEventRecord(ctx->ev_sortb, sb));
+    }
+    for (int q : WITNESS_ORDER) {
+        // with no sparse key, the B queries have the W sort's base counts, window size and arena rows: they read its entries
+        const bool on_b = g->b_sparse && (q == Q_B1 || q == Q_B2);
+        if (on_b) { if (q != Q_B1) CUDA_CHECK(cudaStreamWaitEvent(ctx->st[q], ctx->ev_sortb, 0)); }
+        else if (q != Q_L) CUDA_CHECK(cudaStreamWaitEvent(ctx->st[q], ctx->ev_sort, 0));
+        msm_accumulate(g->plan[q], on_b ? ctx->scratch[Q_B1] : ctx->scratch[Q_L], ctx->scratch[q], ctx->st[q]);
+        if (q == Q_A || q == Q_B1) {
+            scale_partial_kernel<<<count, 32, 0, ctx->st[q]>>>(ctx->d_partial + PARTIAL_OFF[q], q == Q_A ? rs + 1 : rs, ctx->d_partial + B2G_PARTIAL_BYTES + (q == Q_A ? 0 : 128), 2);
+            g_launch_count += 1;
+        }
+        CUDA_CHECK(cudaEventRecord(ctx->ev_done[q], ctx->st[q]));
+    }
+    for (size_t k = 0; k < g->keys.size(); k++)
+        if (counts[k]) run_witness_map(ctx, g->mats[k], s0, counts[k], C.w_off[k], C.v_off[k]);
+    msm_sort_keyed(g->plan[Q_H], ctx->scratch[Q_H], ctx->d_h, true, rows, count, C.max_n[S_H], C.total_n[S_H], s0);
+    msm_accumulate(g->plan[Q_H], ctx->scratch[Q_H], ctx->scratch[Q_H], s0);
+    for (int q = 1; q < NQ; q++) CUDA_CHECK(cudaStreamWaitEvent(s0, ctx->ev_done[q], 0));
+    CUDA_CHECK(cudaStreamWaitEvent(s0, ctx->ev_pre, 0));
+    glue_post_keys_kernel<<<count, 96, 0, s0>>>(ctx->d_partial, g->d_consts, key_of, ctx->d_pre, ctx->d_proof);
+    g_launch_count += 1;
+    CUDA_CHECK(cudaGetLastError());
+}
+
+// replays the keyed pass captured for (group, buffer generation, counts), capturing it first, as run_proof does for one key
+static void run_keys(b2g_ctx* ctx, b2g_pk_group* g, const CallLayout& C, const uint32_t* counts) {
+    cudaStream_t s0 = ctx->st[0];
+    if (!ctx->use_graph) { enqueue_keys(ctx, g, C, counts); return; }
+    std::vector<uint64_t> key = {g->uid, ctx->alloc_gen};
+    key.insert(key.end(), counts, counts + g->keys.size());
+    if (ctx->gexec_keys && ctx->gk_key != key) { cudaGraphExecDestroy(ctx->gexec_keys); ctx->gexec_keys = nullptr; }
+    if (!ctx->gexec_keys) {
+        const uint64_t before = g_launch_count.load();
+        cudaGraph_t graph = nullptr;
+        CUDA_CHECK(cudaStreamBeginCapture(s0, cudaStreamCaptureModeThreadLocal));
+        try { enqueue_keys(ctx, g, C, counts); }
+        catch (...) { cudaStreamEndCapture(s0, &graph); if (graph) cudaGraphDestroy(graph); cudaGetLastError(); g_launch_count = before; throw; }
+        cudaError_t e = cudaStreamEndCapture(s0, &graph);
+        if (e == cudaSuccess) e = cudaGraphInstantiate(&ctx->gexec_keys, graph, 0);
+        if (graph) cudaGraphDestroy(graph);
+        ctx->gk_launches = g_launch_count.load() - before;
+        g_launch_count = before;
+        if (e != cudaSuccess) {                       // not fatal: run this context without graphs from now on
+            cudaGetLastError();
+            ctx->gexec_keys = nullptr; ctx->use_graph = false;
+            enqueue_keys(ctx, g, C, counts);
+            return;
+        }
+        ctx->gk_key = key;
+    }
+    CUDA_CHECK(cudaGraphLaunch(ctx->gexec_keys, s0));
+    g_launch_count += ctx->gk_launches;
+}
+
+}  // namespace b2g
+
+extern "C" {
+
+int b2g_pk_group_load(b2g_ctx* ctx, uint32_t n_keys, const b2g_pk_desc* pks, b2g_mat* const* mats, b2g_pk_group** out) {
+    return guarded_clear([&] {
+        if (!ctx || !out || (n_keys && (!pks || !mats))) throw_error(B2G_E_SHAPE, "null pointer");
+        if (n_keys == 0) throw_error(B2G_E_SHAPE, "b2g_pk_group_load: the group has no keys");
+        if (ctx->shard_count != 1) throw_error(B2G_E_SHAPE, "b2g_pk_group_load: a key group needs an unsharded context");
+        // every key against its matrices, and the arena rows, before anything is allocated
+        std::vector<KeyBases> bases(n_keys);
+        std::vector<std::vector<uint32_t>> bidx(n_keys);
+        std::vector<std::array<std::vector<uint8_t>, 2>> bpacked(n_keys);
+        std::vector<char> sparse(n_keys, 0);
+        for (uint32_t k = 0; k < n_keys; k++) {
+            const b2g_pk_desc* d = &pks[k];
+            try {
+                pk_desc_check(d);
+                b2g_pk hdr;
+                hdr.device = ctx->device; hdr.n_vars = d->n_vars; hdr.n_public = d->n_public; hdr.domain = d->domain_size;
+                check_shapes(ctx, &hdr, mats[k]);
+            } catch (const B2gError& e) { throw_error(e.code, "b2g_pk_group_load: key " + std::to_string(k) + ": " + e.what()); }
+            const uint32_t nw = d->n_vars - 1;
+            sparse[k] = b_support(d, 0, nw, bidx[k], bpacked[k].data());
+            const uint32_t nb = sparse[k] ? (uint32_t)bidx[k].size() : nw;
+            bases[k] = {d->domain_size, nw, nw, nb, nb};
+        }
+        const GroupLayout L = group_layout(bases);
+        DevGuard dg(ctx->device);
+        cudaStream_t st = ctx->st[0];
+        struct GroupGuard {
+            b2g_pk_group* g = new b2g_pk_group(); void* tmp = nullptr;
+            ~GroupGuard() { if (tmp) cudaFree(tmp); if (g) { cudaDeviceSynchronize(); group_release(g); } }
+        } guard;
+        b2g_pk_group* g = guard.g;
+        g->device = ctx->device;
+        g->mats.assign(mats, mats + n_keys);
+        g->b_sparse = std::find(sparse.begin(), sparse.end(), 1) != sparse.end();
+        for (int q = 0; q < NQ; q++) {
+            MsmPlan& p = g->plan[q];
+            p.g2 = q == Q_B2; p.c = L.c[q]; p.nwin = msm_nwin(p.c); p.nbuckets = 1u << (p.c - 1); p.n = 0;
+            for (const KeyBases& b : bases) p.n = std::max(p.n, b[q]);
+            g->row[q] = L.row[q];
+            if (!L.rows[q]) continue;
+            const size_t bytes = L.rows[q] * (p.g2 ? 128 : 64);
+            if (cudaMalloc(&p.table, bytes) != cudaSuccess) {
+                cudaGetLastError(); p.table = nullptr;
+                throw_error(B2G_E_DEVICE, std::string("b2g_pk_group_load: the table arena of query ") + QUERY_NAME[q] + " (" +
+                                          std::to_string(bytes >> 20) + " MiB for " + std::to_string(n_keys) + " keys) does not fit in device memory");
+            }
+        }
+        std::vector<KeyGlue> glue(n_keys);
+        std::vector<const uint32_t*> bidx_dev(n_keys, nullptr);
+        std::vector<const uint8_t*> consts_dev(n_keys, nullptr);
+        for (uint32_t k = 0; k < n_keys; k++) {
+            const b2g_pk_desc* d = &pks[k];
+            b2g_pk* pk = new b2g_pk();
+            g->keys.push_back(pk);
+            pk->device = ctx->device; pk->n_vars = d->n_vars; pk->n_public = d->n_public; pk->domain = d->domain_size;
+            const uint32_t li = d->n_public + 1;
+            try {
+                // the bases of each query as b2g_pk_load pairs them with scalars, L re-indexed onto w[1..]
+                std::vector<uint8_t> l_padded((size_t)(d->n_vars - 1) * 64, 0);
+                if (d->n_vars - li) memcpy(l_padded.data() + (size_t)(li - 1) * 64, d->l_query, (size_t)(d->n_vars - li) * 64);
+                const void* src[NQ] = {d->h_query, l_padded.data(), (const uint8_t*)d->a_query + 64,
+                                       sparse[k] ? (const void*)bpacked[k][0].data() : (const uint8_t*)d->b_g1_query + 64,
+                                       sparse[k] ? (const void*)bpacked[k][1].data() : (const uint8_t*)d->b_g2_query + 128};
+                for (int q = 0; q < NQ; q++) {
+                    pk->plan[q].n = bases[k][q]; pk->plan[q].g2 = q == Q_B2;
+                    pk->cnt[q] = q == Q_H ? d->domain_size : d->n_vars - 1;
+                    pk->scalar_off[q] = q == Q_H ? 0 : 1;
+                    if (!bases[k][q]) continue;
+                    const size_t aff = q == Q_B2 ? 128 : 64;
+                    guard.tmp = dev_upload<uint8_t>(src[q], (size_t)bases[k][q] * aff, st);
+                    msm_build_table_into((uint8_t*)g->plan[q].table + (size_t)L.row[q][k] * aff, guard.tmp, bases[k][q], L.c[q], q == Q_B2, st);
+                    CUDA_CHECK(cudaStreamSynchronize(st));
+                    cudaFree(guard.tmp); guard.tmp = nullptr;
+                }
+                if (sparse[k]) {
+                    pk->b_compact = bases[k][Q_B1];
+                    pk->d_bidx = dev_upload<uint32_t>(bidx[k].data(), bidx[k].size() * 4, st);
+                }
+                pk_load_glue(pk, d, st);
+            } catch (const B2gError& e) { throw_error(e.code, "b2g_pk_group_load: key " + std::to_string(k) + ": " + e.what()); }
+            glue[k] = {pk->d_tab_delta1, pk->d_tab_delta2, pk->d_tab_aa, pk->d_tab_bb};
+            bidx_dev[k] = pk->d_bidx;
+            consts_dev[k] = pk->d_consts;
+        }
+        g->d_keys = dev_upload<KeyGlue>(glue.data(), glue.size() * sizeof(KeyGlue), st);
+        g->d_bidx = dev_upload<const uint32_t*>(bidx_dev.data(), bidx_dev.size() * sizeof(uint32_t*), st);
+        g->d_consts = dev_upload<const uint8_t*>(consts_dev.data(), consts_dev.size() * sizeof(uint8_t*), st);
+        CUDA_CHECK(cudaStreamSynchronize(st));
+        guard.g = nullptr;
+        *out = g;
+    });
+}
+
+int b2g_pk_group_free(b2g_pk_group* g) {
+    return guarded([&] {
+        if (!g) return;
+        DevGuard dg(g->device);
+        cudaDeviceSynchronize();
+        group_release(g);
+    });
+}
+
+int b2g_prove_keys(b2g_ctx* ctx, b2g_pk_group* g, const uint32_t* counts, const void* r_canon, const void* s_canon, const void* const* w_mont,
+                   uint8_t* proofs_out) {
+    return guarded_clear([&] {
+        if (!ctx || !g || !counts || !r_canon || !s_canon || !w_mont || !proofs_out) throw_error(B2G_E_SHAPE, "null pointer");
+        if (ctx->shard_count != 1) throw_error(B2G_E_SHAPE, "b2g_prove_keys needs an unsharded context");
+        if (ctx->pending_out) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
+        if (g->device != ctx->device) throw_error(B2G_E_SHAPE, "handle belongs to another device");
+        const std::vector<KeyBases> bases = group_bases(g);
+        GroupLayout L;
+        for (int q = 0; q < NQ; q++) { L.c[q] = g->plan[q].c; L.row[q] = g->row[q]; }
+        std::vector<uint32_t> n_vars, n_dom;
+        for (size_t k = 0; k < g->keys.size(); k++) { n_vars.push_back(g->mats[k]->n_vars); n_dom.push_back(g->mats[k]->n); }
+        const CallLayout C = call_layout(L, bases, n_vars, n_dom, counts);
+        for (uint32_t j = 0; j < C.count; j++) if (!w_mont[j]) throw_error(B2G_E_SHAPE, "null witness " + std::to_string(j));
+        DevGuard dg(ctx->device);
+        const size_t table_bytes = C.rows.size() * sizeof(KeyedRow) + C.key_of.size() * 4;
+        try {
+            ensure_witness_buffers(ctx, C.total_w, C.total_v);
+            ensure_batch_buffers(ctx, C.count);
+            ensure_scratch_keys(ctx, g, C);
+            ensure_keyed_buffer(ctx, table_bytes);
+        } catch (const B2gError& e) {
+            if (e.code != B2G_E_DEVICE) throw;
+            cudaGetLastError();
+            throw_error(B2G_E_DEVICE, "the device buffers of " + std::to_string(C.count) + " proof(s) under " + std::to_string(g->keys.size()) +
+                                      " key(s) do not fit in device memory; prove fewer per call (" + e.what() + ")");
+        }
+        cudaStream_t s0 = ctx->st[0];
+        for (uint32_t j = 0; j < C.count; j++) {
+            const size_t k = C.key_of[j];
+            CUDA_CHECK(cudaMemcpyAsync(ctx->d_w + C.rows[(size_t)S_W * C.count + j].src - 1, w_mont[j], (size_t)n_vars[k] * 32, cudaMemcpyHostToDevice, s0));
+        }
+        std::vector<uint8_t> table(table_bytes);
+        memcpy(table.data(), C.rows.data(), C.rows.size() * sizeof(KeyedRow));
+        memcpy(table.data() + C.rows.size() * sizeof(KeyedRow), C.key_of.data(), C.key_of.size() * 4);
+        CUDA_CHECK(cudaMemcpyAsync(ctx->d_keyed, table.data(), table_bytes, cudaMemcpyHostToDevice, s0));
+        stage_rs(ctx, r_canon, s_canon, C.count);
+        run_keys(ctx, g, C, counts);
+        ctx->pre_valid = false;
+        CUDA_CHECK(cudaMemcpyAsync(ctx->h_proof, ctx->d_proof, (size_t)C.count * 256, cudaMemcpyDeviceToHost, s0));
+        CUDA_CHECK(cudaStreamSynchronize(s0));
+        memcpy(proofs_out, ctx->h_proof, (size_t)C.count * 256);
+    });
+}
+
+int b2g_pk_group_layout(uint32_t n_keys, const uint32_t* bases, const uint32_t* n_vars, const uint32_t* n_dom, const uint32_t* counts,
+                        int32_t* c_out, uint32_t* row_out, uint64_t* rows_out) {
+    return guarded([&] {
+        if ((n_keys && !bases) || !c_out || !row_out || (counts && (!n_vars || !n_dom || !rows_out))) throw_error(B2G_E_SHAPE, "null pointer");
+        std::vector<KeyBases> b(n_keys);
+        for (uint32_t k = 0; k < n_keys; k++) for (int q = 0; q < NQ; q++) b[k][q] = bases[(size_t)k * NQ + q];
+        const GroupLayout L = group_layout(b);
+        for (int q = 0; q < NQ; q++) c_out[q] = L.c[q];
+        for (uint32_t k = 0; k < n_keys; k++) for (int q = 0; q < NQ; q++) row_out[(size_t)k * NQ + q] = L.row[q][k];
+        if (!counts) return;
+        const CallLayout C = call_layout(L, b, std::vector<uint32_t>(n_vars, n_vars + n_keys), std::vector<uint32_t>(n_dom, n_dom + n_keys), counts);
+        for (size_t i = 0; i < C.rows.size(); i++) {
+            const KeyedRow& r = C.rows[i];
+            rows_out[4 * i] = r.src; rows_out[4 * i + 1] = r.canon; rows_out[4 * i + 2] = r.n; rows_out[4 * i + 3] = r.row;
+        }
     });
 }
 

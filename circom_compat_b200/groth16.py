@@ -9,6 +9,8 @@
         <- Groth16::<Bn254, CircomReduction>::prove (src/zkey.rs:866): draws r then s, then the call above.
     Groth16.create_proofs(pk, rs, matrices, assignments)
         <- the first call above for many witnesses of one circuit, proved together in one device pass (b2g_prove_many).
+    Groth16.load_proving_keys([(pk, matrices), ...]) / Groth16.create_proofs_keys(group, [(rs, assignments), ...])
+        <- create_proofs for batches of witnesses under many keys, proved together in one device pass (b2g_prove_keys).
     Groth16.verify_many(vk, public_inputs, proofs)
         <- Groth16::verify_with_processed_vk (src/zkey.rs:869-870, 914-916) for many proofs of one key in one device pass
            (b2g_verify_many, with the key prepared on the device by b2g_vk_load <- process_vk).
@@ -132,6 +134,9 @@ def _refused_key(e):
 
 
 def release(obj):
+    if isinstance(obj, ProvingKeyGroup):
+        obj._free()
+        return
     for cache, free in _CACHES:
         for key in [k for k in cache if k[0] == id(obj)]:
             getattr(N.lib(), free)(cache.pop(key)[0])
@@ -141,6 +146,43 @@ def release_all():
     for cache, free in _CACHES:
         for key in list(cache):
             getattr(N.lib(), free)(cache.pop(key)[0])
+
+
+class ProvingKeyGroup:
+    """K proving keys loaded on one device for proving under all of them in one pass (Groth16.load_proving_keys,
+    b2g_pk_group_load).  It owns its device state and the matrix handles of its keys; release(group) frees them."""
+
+    def __init__(self, device: int, keys: list, h, mat_handles: list):
+        self.device, self.keys, self._h, self._mats = device, keys, h, mat_handles
+
+    @property
+    def n_keys(self) -> int:
+        return len(self.keys)
+
+    def _free(self):
+        if self._h:
+            N.lib().b2g_pk_group_free(self._h)
+            self._h = C.c_void_p()
+        for h in self._mats:
+            N.lib().b2g_matrices_free(h)
+        self._mats = []
+
+    def __del__(self):
+        try:
+            self._free()
+        except Exception:
+            pass
+
+
+def _pk_desc(pk: ProvingKey):
+    """(b2g_pk_desc, the arrays it points into) of a ProvingKey"""
+    d = N.PkDesc()
+    d.n_vars, d.n_public, d.domain_size = pk.n_vars, pk.n_public, pk.domain_size
+    keep = {}
+    for name in ('alpha_g1', 'beta_g1', 'delta_g1', 'beta_g2', 'delta_g2', 'a_query', 'b_g1_query', 'b_g2_query', 'l_query', 'h_query'):
+        keep[name] = _c(getattr(pk, name))
+        setattr(d, name, keep[name].ctypes.data if keep[name].size else None)
+    return d, keep
 
 
 class Context:
@@ -165,12 +207,7 @@ class Context:
     def pk_handle(self, pk: ProvingKey):
         key = (id(pk), self.device, self.shard_rank, self.shard_count)
         if key not in _PK_HANDLES:
-            d = N.PkDesc()
-            d.n_vars, d.n_public, d.domain_size = pk.n_vars, pk.n_public, pk.domain_size
-            keep = {}
-            for name in ('alpha_g1', 'beta_g1', 'delta_g1', 'beta_g2', 'delta_g2', 'a_query', 'b_g1_query', 'b_g2_query', 'l_query', 'h_query'):
-                keep[name] = _c(getattr(pk, name))
-                setattr(d, name, keep[name].ctypes.data if keep[name].size else None)
+            d, keep = _pk_desc(pk)
             h = C.c_void_p()
             N.check(N.lib().b2g_pk_load(self._h, C.byref(d), C.byref(h)))
             _PK_HANDLES[key] = (h, pk)
@@ -737,6 +774,74 @@ class Groth16:
         out = np.zeros((len(ws), 256), dtype=np.uint8)
         N.check(N.lib().b2g_prove_many(ctx._h, ph, mh, len(ws), _ptr(rr), _ptr(ss), ptrs, _ptr(out)))
         return [Proof(row.tobytes()) for row in out]
+
+    @staticmethod
+    def load_proving_keys(keys, ctx: Context = None, reduction=CircomReduction) -> ProvingKeyGroup:
+        """Loads keys = [(pk, matrices) or (pk, matrices, reduction), ...] on ctx's device for create_proofs_keys
+        (b2g_pk_group_load): every query's tables of all keys in one arena at one window size.  A key may appear more than
+        once; `reduction` applies to the pairs that name none.  Returns the group, freed by release(group).  A key the
+        library refuses raises B2gError naming its index; then nothing is loaded."""
+        ctx = ctx or default_context()
+        entries = [tuple(e) if len(e) == 3 else (e[0], e[1], reduction) for e in keys]
+        if not entries:
+            raise ValueError("load_proving_keys: the group has no keys")
+        descs, keep, mats, owned = [], [], [], {}
+        try:
+            for pk, m, red in entries:
+                d, k = _pk_desc(pk)
+                descs.append(d)
+                keep.append(k)
+                if (id(m), red.ID) not in owned:
+                    md, mk = _mat_desc(m, pk.n_vars, red.ID)
+                    h = C.c_void_p()
+                    N.check(N.lib().b2g_matrices_load(ctx._h, C.byref(md), C.byref(h)))
+                    owned[(id(m), red.ID)] = h
+                mats.append(owned[(id(m), red.ID)])
+            arr = (N.PkDesc * len(descs))(*descs)
+            hs = (C.c_void_p * len(mats))(*[h.value for h in mats])
+            g = C.c_void_p()
+            N.check(N.lib().b2g_pk_group_load(ctx._h, len(descs), arr, hs, C.byref(g)))
+        except BaseException:
+            for h in owned.values():
+                N.lib().b2g_matrices_free(h)
+            raise
+        return ProvingKeyGroup(ctx.device, [(pk, m, red) for pk, m, red in entries], g, list(owned.values()))
+
+    @staticmethod
+    def create_proofs_keys(group: ProvingKeyGroup, batches, ctx: Context = None) -> list:
+        """create_proofs for one batch per key of `group`, all in ONE device pass (b2g_prove_keys): batches = one
+        (rs, assignments) per key, in the group's order (an empty batch is allowed); returns one [Proof] per key, batch k's
+        proofs byte-identical to create_proofs(pk_k, rs_k, matrices_k, assignments_k)."""
+        ctx = ctx or default_context()
+        batches = [(list(rs), list(ws)) for rs, ws in batches]
+        if len(batches) != group.n_keys:
+            raise ValueError(f"create_proofs_keys: {len(batches)} batches for a group of {group.n_keys} keys")
+        if not group._h:
+            raise ValueError("create_proofs_keys: the group has been released")
+        ws, rr, ss, counts = [], [], [], []
+        for k, ((rs, assignments), (pk, _, _)) in enumerate(zip(batches, group.keys)):
+            if len(rs) != len(assignments):
+                raise ValueError(f"create_proofs_keys: key {k}: one (r, s) per assignment")
+            for w in assignments:
+                w = _c(w)
+                if w.size // 4 != pk.n_vars:
+                    raise ValueError(f"create_proofs_keys: key {k}: full_assignment length != n_vars")
+                ws.append(w)
+            rr += [_scalar_bytes(r) for r, _ in rs]
+            ss += [_scalar_bytes(s) for _, s in rs]
+            counts.append(len(assignments))
+        if not ws:
+            return [[] for _ in batches]
+        cnt = np.array(counts, dtype=np.uint32)
+        rr, ss = np.concatenate(rr), np.concatenate(ss)
+        ptrs = (C.c_void_p * len(ws))(*[w.ctypes.data for w in ws])
+        out = np.zeros((len(ws), 256), dtype=np.uint8)
+        N.check(N.lib().b2g_prove_keys(ctx._h, group._h, _ptr(cnt), _ptr(rr), _ptr(ss), ptrs, _ptr(out)))
+        proofs, at = [], 0
+        for c in counts:
+            proofs.append([Proof(row.tobytes()) for row in out[at:at + c]])
+            at += c
+        return proofs
 
     @staticmethod
     def submit(pk: ProvingKey, r, s, matrices: ConstraintMatrices, full_assignment, ctx: Context, reduction=CircomReduction) -> 'PendingProof':

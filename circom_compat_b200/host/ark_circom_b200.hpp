@@ -480,13 +480,19 @@ public:
     }
     b2g_ctx* ctx() { return ctx_; }
 
-    b2g_pk* pk(const ProvingKey& k) {
-        if (void* h = k.device.find(ctx_, 0)) return (b2g_pk*)h;
+    // the b2g_pk_desc of a key (pointing into it)
+    static b2g_pk_desc pk_desc(const ProvingKey& k) {
         b2g_pk_desc d; memset(&d, 0, sizeof d);
         d.n_vars = (uint32_t)k.a_query.size(); d.n_public = (uint32_t)k.vk.gamma_abc_g1.size() - 1; d.domain_size = (uint32_t)k.h_query.size();
         d.alpha_g1 = &k.vk.alpha_g1; d.beta_g1 = &k.beta_g1; d.delta_g1 = &k.delta_g1; d.beta_g2 = &k.vk.beta_g2; d.delta_g2 = &k.vk.delta_g2;
         d.a_query = k.a_query.data(); d.b_g1_query = k.b_g1_query.data(); d.b_g2_query = k.b_g2_query.data();
         d.l_query = k.l_query.data(); d.h_query = k.h_query.data();
+        return d;
+    }
+
+    b2g_pk* pk(const ProvingKey& k) {
+        if (void* h = k.device.find(ctx_, 0)) return (b2g_pk*)h;
+        const b2g_pk_desc d = pk_desc(k);
         b2g_pk* h = nullptr; check(b2g_pk_load(ctx_, &d, &h));
         k.device.put(ctx_, 0, h, [](void* p) { b2g_pk_free((b2g_pk*)p); });
         return h;
@@ -819,6 +825,21 @@ inline b2g_delta_key delta_key(const ProvingKey& pk) {
     return d;
 }
 
+// Proving keys loaded on one device for proving under all of them in one pass (Groth16T::load_proving_keys,
+// b2g_pk_group_load).  Owns the group's device state; the keys' matrices must outlive it.
+class ProvingKeyGroup {
+public:
+    ProvingKeyGroup(b2g_pk_group* h, std::vector<size_t> n_vars) : h_(h), n_vars_(std::move(n_vars)) {}
+    ~ProvingKeyGroup() { if (h_) b2g_pk_group_free(h_); }
+    ProvingKeyGroup(const ProvingKeyGroup&) = delete; ProvingKeyGroup& operator=(const ProvingKeyGroup&) = delete;
+    b2g_pk_group* handle() const { return h_; }
+    size_t n_keys() const { return n_vars_.size(); }
+    size_t n_vars(size_t k) const { return n_vars_[k]; }
+private:
+    b2g_pk_group* h_;
+    std::vector<size_t> n_vars_;
+};
+
 template <class QAP = CircomReduction>
 struct Groth16T {                                       // Groth16::<Bn254, QAP>
     // verification (host pairing, ark_circom_verifier.hpp): src/zkey.rs:868-870, 914-916; tests/groth16.rs:33-35
@@ -1018,6 +1039,54 @@ struct Groth16T {                                       // Groth16::<Bn254, QAP>
         std::vector<uint8_t> bytes(n * 256);
         check(b2g_prove_many(gpu.ctx(), gpu.pk(pk), gpu.mat(matrices, pk.a_query.size(), QAP::ID), (uint32_t)n, rb.data(), sb.data(), ws.data(), bytes.data()));
         for (size_t i = 0; i < n; i++) memcpy(out[i].bytes, bytes.data() + 256 * i, 256);
+        return out;
+    }
+
+    // create_proofs for many keys: keys[k] = (pk, matrices) loaded with QAP's reduction into one group (b2g_pk_group_load); a
+    // key may appear several times.
+    static std::unique_ptr<ProvingKeyGroup> load_proving_keys(const std::vector<std::pair<const ProvingKey*, const ConstraintMatrices*>>& keys,
+                                                              Gpu& gpu = Gpu::instance()) {
+        std::vector<b2g_pk_desc> descs;
+        std::vector<b2g_mat*> mats;
+        std::vector<size_t> n_vars;
+        for (const auto& k : keys) {
+            descs.push_back(Gpu::pk_desc(*k.first));
+            mats.push_back(gpu.mat(*k.second, k.first->a_query.size(), QAP::ID));
+            n_vars.push_back(k.first->a_query.size());
+        }
+        b2g_pk_group* h = nullptr;
+        check(b2g_pk_group_load(gpu.ctx(), (uint32_t)descs.size(), descs.data(), mats.data(), &h));
+        return std::unique_ptr<ProvingKeyGroup>(new ProvingKeyGroup(h, std::move(n_vars)));
+    }
+
+    // Batches of proofs under every key of a group in ONE device pass (b2g_prove_keys): batches[k] = (rs, assignments) of key k
+    // (may be empty); returns one vector of proofs per key, batch k byte-identical to create_proofs on key k.
+    using KeyBatch = std::pair<std::vector<std::pair<Fr, Fr>>, std::vector<const std::vector<Fr>*>>;
+    static std::vector<std::vector<Proof>> create_proofs_keys(const ProvingKeyGroup& group, const std::vector<KeyBatch>& batches,
+                                                              Gpu& gpu = Gpu::instance()) {
+        if (batches.size() != group.n_keys()) throw SynthesisError("create_proofs_keys: one batch per key of the group");
+        std::vector<uint32_t> counts;
+        std::vector<BigInt256> rb, sb;
+        std::vector<const void*> ws;
+        for (size_t k = 0; k < batches.size(); k++) {
+            const auto& b = batches[k];
+            if (b.first.size() != b.second.size()) throw SynthesisError("create_proofs_keys: one (r, s) per assignment");
+            for (size_t i = 0; i < b.first.size(); i++) {
+                if (b.second[i]->size() != group.n_vars(k)) throw SynthesisError("AssignmentMissing: full_assignment length != n_vars");
+                rb.push_back(b.first[i].first.into_bigint()); sb.push_back(b.first[i].second.into_bigint());
+                ws.push_back(b.second[i]->data());
+            }
+            counts.push_back((uint32_t)b.first.size());
+        }
+        std::vector<std::vector<Proof>> out(batches.size());
+        if (ws.empty()) return out;
+        std::vector<uint8_t> bytes(ws.size() * 256);
+        check(b2g_prove_keys(gpu.ctx(), group.handle(), counts.data(), rb.data(), sb.data(), ws.data(), bytes.data()));
+        size_t at = 0;
+        for (size_t k = 0; k < batches.size(); k++) {
+            out[k].resize(counts[k]);
+            for (auto& p : out[k]) { memcpy(p.bytes, bytes.data() + 256 * at, 256); at++; }
+        }
         return out;
     }
 

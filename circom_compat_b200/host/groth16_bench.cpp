@@ -7,6 +7,8 @@
 //                                                                   and the proof's ark-serialize compressed bytes
 //   groth16_bench <circuit.zkey> chain:<a>|<witness.wtns> [iters] [r_hex s_hex]
 //       B2G_MANY=K: also K proofs in one device pass (Groth16::create_proofs)
+//       B2G_PROVE_KEYS=K: also load K copies of the key as one group (Groth16::load_proving_keys) and prove one proof of
+//       chain:<a + k> under copy k, all in one device pass (Groth16::create_proofs_keys), timing the keyed call
 //       B2G_VERIFY_MANY=K: also prove K proofs, negate A in every other one, and compare Groth16::verify_many's verdicts with
 //       verify_with_processed_vk called per proof (timing both)
 //       B2G_VERIFY_BATCH=K: also prove K proofs and compare Groth16::verify_batch's verdict, on them and with the last
@@ -394,6 +396,25 @@ int main(int argc, char** argv) {
             for (int i = 0; i < k; i++) std::printf("many[%d]=%s\n", i, proofs[(size_t)i].hex().c_str());
             std::printf("batched (%d proofs in one device pass, one context): %.3f ms/proof over %d calls, first_identical=%d\n", k, pms, reps,
                         !memcmp(proofs[0].bytes, proof.bytes, 256) ? 1 : 0);
+        }
+        if (const char* pkeys = std::getenv("B2G_PROVE_KEYS")) {          // K copies of the key, one proof each, in one device pass
+            const int k = std::atoi(pkeys);
+            if (k < 1) throw SynthesisError("B2G_PROVE_KEYS must be >= 1");
+            std::vector<std::vector<Fr>> wv((size_t)k, full_assignment);
+            if (wsrc.rfind("chain:", 0) == 0)
+                for (int i = 1; i < k; i++) wv[(size_t)i] = chain_witness(params.a_query.size(), std::stoull(wsrc.substr(6)) + (unsigned long long)i);
+            std::vector<std::pair<const ProvingKey*, const ConstraintMatrices*>> keys((size_t)k, {&params, &matrices});
+            auto group = Groth16::load_proving_keys(keys);
+            std::vector<Groth16::KeyBatch> batches;
+            for (int i = 0; i < k; i++) batches.push_back({{{r, s}}, {&wv[(size_t)i]}});
+            auto proofs = Groth16::create_proofs_keys(*group, batches);      // also the warm-up of this shape
+            const int reps = iters > 0 ? iters : 1;
+            auto t1 = std::chrono::steady_clock::now();
+            for (int it = 0; it < reps; it++) proofs = Groth16::create_proofs_keys(*group, batches);
+            double pms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t1).count() / ((double)reps * k);
+            for (int i = 0; i < k; i++) std::printf("keys[%d]=%s\n", i, proofs[(size_t)i][0].hex().c_str());
+            std::printf("keyed (%d keys, one proof each, in one device pass): %.3f ms/proof over %d calls, first_identical=%d\n", k, pms, reps,
+                        !memcmp(proofs[0][0].bytes, proof.bytes, 256) ? 1 : 0);
         }
         if (const char* vm = std::getenv("B2G_VERIFY_MANY")) {           // batched verification against the host verifier
             const int k = std::atoi(vm);

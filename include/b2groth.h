@@ -13,6 +13,7 @@
  *   b2g_msm_g1 / b2g_msm_g2<- VariableBaseMSM::msm_bigint (ark-ec 0.5.0) as used by that function
  *   b2g_ntt                <- Radix2EvaluationDomain::{fft,ifft}_in_place (ark-poly 0.5.0) as used at qap.rs:60-81
  *   b2g_prove_many         <- the same function called for many witnesses of one circuit, in one device pass
+ *   b2g_prove_keys         <- the same function called for batches of witnesses under many keys, in one device pass
  *   b2g_prove_partial / b2g_prove_finish : the same proof split for base-range sharding over several GPUs
  *   b2g_vk_load            <- GrothBn::process_vk(&params.vk) (src/zkey.rs:868, 914): the prepared verifying key, on the device
  *   b2g_vk_load_many       <- the same for many keys in one device pass
@@ -76,6 +77,7 @@ extern "C" {
 typedef struct b2g_ctx b2g_ctx;
 typedef struct b2g_pk b2g_pk;
 typedef struct b2g_mat b2g_mat;
+typedef struct b2g_pk_group b2g_pk_group;
 typedef struct b2g_vk b2g_vk;
 
 /* Proving key as read_zkey() produces it (src/zkey.rs:121-130); every pointer is a HOST pointer. */
@@ -169,6 +171,42 @@ B2G_API int b2g_prove_wait(b2g_ctx* ctx);
  * 64, 1.1x at 2^16); from 2^18 up, where one proof fills the GPU, several contexts in flight are faster (README.md). */
 B2G_API int b2g_prove_many(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, uint32_t count, const void* r_canon, const void* s_canon,
                            const void* const* w_mont, uint8_t* proofs_out);
+/* b2g_prove_keys <- a caller's loop over Groth16::<Bn254, QAP>::create_proof_with_reduction_and_matrices for several keys
+ * (circuits), e.g. a prover service whose queue mixes deposit, transfer and withdraw circuits: batches of witnesses under
+ * n_keys proving keys in one device pass.
+ *
+ * b2g_pk_group_load loads n_keys keys (descs as b2g_pk_load takes them) with their matrix handles (mats[k] belongs to key k and
+ * must outlive the group; a key may appear several times).  For each query (H, L, A, B1, B2) the window tables of all keys
+ * are built into ONE arena at ONE window size c, msm_pick_c of the largest base count of that query in the group; key k's
+ * rows start at its own row offset.  Each key keeps its sparse-B compaction, glue constants and 8-bit window tables as
+ * b2g_pk_load builds them.  Device memory per key: its tables at the group's c (nwin(c) x bases x 64 B per G1 query,
+ * x 128 B for B2), 2.6 MB of glue tables, 704 B of constants and 4 B per real B base of a sparse key.  A small key in a
+ * group with a large one is built and sorted at the large key's c, so its proofs get 2^(c-1) buckets each (DESIGN.md
+ * section 4).
+ * Errors: B2G_E_SHAPE before anything is allocated for n_keys == 0, null pointers, a sharded context, a key whose
+ * header or matrices disagree (b2g_prove's shape checks; the message names the key), or a query whose arena reaches 2^31
+ * rows (the sign bit of an entry word); B2G_E_INPUT for an off-curve point (naming the key); B2G_E_DEVICE when the arena
+ * does not fit.  On any error everything built so far is freed.
+ *
+ * b2g_prove_keys proves counts[k] witnesses under key k for every k, synchronously.  r_canon / s_canon = total x 32 B and
+ * w_mont = total pointers (n_vars of the key each), key after key; proofs_out = total x 256 B in the same order.  The
+ * proofs of key k are byte-identical to b2g_prove_many(ctx, pk_k, mat_k, counts[k], ...) with the same (r, s) and
+ * witnesses.  Requires an unsharded context with no pending proof; 1 <= total <= 65535 (a count may be 0); and for each
+ * query, total proofs x bases x windows < 2^32 sorted entries over the whole call.  Errors as b2g_prove_many.  The pass is
+ * captured once as a CUDA graph per (group, counts) and replayed; the context keeps its buffers for the largest call. */
+B2G_API int b2g_pk_group_load(b2g_ctx* ctx, uint32_t n_keys, const b2g_pk_desc* pks, b2g_mat* const* mats, b2g_pk_group** out);
+B2G_API int b2g_pk_group_free(b2g_pk_group* group);
+B2G_API int b2g_prove_keys(b2g_ctx* ctx, b2g_pk_group* group, const uint32_t* counts, const void* r_canon, const void* s_canon,
+                           const void* const* w_mont, uint8_t* proofs_out);
+/* The host half of the two calls above, without a device: bases = n_keys x 5 base counts (H, L, A, B1, B2: the domain,
+ * n_vars - 1 for L and A, n_vars - 1 or the real B bases of a sparse key for B1 and B2); c_out = the group's 5 window sizes;
+ * row_out = n_keys x 5 first arena rows.  With counts (n_vars / n_dom = each key's witness length and matrices domain),
+ * rows_out = 3 x total rows of 4 u64 [first scalar, first canonical slot, base count, arena row] for the H sort (scalars in
+ * the call's h vectors), the W sort (w[1..], for L and A) and the B sort (the gathered B scalars, for B1 and B2).  Errors as
+ * the two calls for the same shapes. */
+B2G_API int b2g_pk_group_layout(uint32_t n_keys, const uint32_t* bases, const uint32_t* n_vars, const uint32_t* n_dom, const uint32_t* counts,
+                                int32_t* c_out, uint32_t* row_out, uint64_t* rows_out);
+
 /* Page-lock / release a host buffer (cudaHostRegister): a witness vector owned by the caller (a Rust Vec<Fr>, a std::vector)
  * uploads asynchronously and at full PCIe speed once registered.  Registering twice / unregistering an unknown pointer is not
  * an error. */
