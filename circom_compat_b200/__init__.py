@@ -12,4 +12,5 @@ from .verifier import VerifyingKey, PreparedVerifyingKey, MalformedVerifyingKey 
 from ._native import B2gError, PolynomialDegreeTooLarge  # noqa: F401
 from .ark_serialize import (serialize_proving_key, deserialize_proving_key, serialize_verifying_key,  # noqa: F401
                             deserialize_verifying_key, deserialize_verifying_keys)
+from .witness import WitnessCalculator, WitnessError, WasmModule  # noqa: F401
 from .ptau import read_ptau, write_ptau, new_powers_of_tau, Lagrange, Powers, PowersCheck  # noqa: F401

@@ -98,6 +98,18 @@ class DeltaKey(C.Structure):
     _fields_ = [('n_l', C.c_uint32), ('n_h', C.c_uint32)] + [(k, C.c_void_p) for k in ('delta_g1', 'delta_g2', 'l_query', 'h_query')]
 
 
+class WasmSummary(C.Structure):
+    """b2g_wasm_summary: what b2g_wasm_load read from a circom 2 module"""
+    _fields_ = [(k, C.c_uint32) for k in ('n32', 'witness_size', 'input_size', 'version', 'mem_pages')] + \
+               [('reserved', C.c_uint32 * 3)]
+
+
+class WasmLimits(C.Structure):
+    """b2g_wasm_limits: per-lane limits of the device interpreter and the device-memory budget of a call"""
+    _fields_ = [(k, C.c_uint32) for k in ('max_pages', 'max_depth', 'stack_slots', 'reserved')] + \
+               [('fuel', C.c_uint64), ('budget_bytes', C.c_uint64)]
+
+
 class KeyBatch(C.Structure):
     """b2g_key_batch: one batch of proofs under one verifying key (b2g_verify_batch_keys, b2g_verify_batch_keys_locate)"""
     _fields_ = [('vk', C.c_void_p), ('count', C.c_uint32), ('reserved', C.c_uint32)] + \
@@ -115,7 +127,9 @@ EXPORTS = ['b2g_last_error', 'b2g_version', 'b2g_device_count', 'b2g_ctx_create'
            'b2g_setup_from_powers', 'b2g_delta_update', 'b2g_delta_update_check', 'b2g_points_intt',
            'b2g_powers_msm', 'b2g_powers_check', 'b2g_setup_check', 'b2g_powers_prepare', 'b2g_lagrange_check',
            'b2g_setup_from_lagrange', 'b2g_points_scale', 'b2g_powers_contribute',
-           'b2g_pk_group_load', 'b2g_pk_group_free', 'b2g_prove_keys', 'b2g_pk_group_layout']
+           'b2g_pk_group_load', 'b2g_pk_group_free', 'b2g_prove_keys', 'b2g_pk_group_layout',
+           'b2g_wasm_load', 'b2g_wasm_load_module', 'b2g_wasm_free', 'b2g_wasm_info', 'b2g_wasm_get_limits',
+           'b2g_wasm_set_limits', 'b2g_witness_calculate', 'b2g_wasm_run']
 
 _lib = None
 
@@ -174,6 +188,14 @@ def lib():
         L.b2g_setup_from_lagrange.argtypes = [vp, C.POINTER(MatDesc), C.POINTER(PowersDesc), C.POINTER(LagrangeDesc), C.POINTER(SetupOut)]
         L.b2g_points_scale.argtypes = [vp, i, sz, vp, vp, vp]
         L.b2g_powers_contribute.argtypes = [vp, C.POINTER(PowersDesc), C.POINTER(PowersSecrets), C.POINTER(PowersOut)]
+        L.b2g_wasm_load.argtypes = [vp, vp, sz, C.POINTER(vp)]
+        L.b2g_wasm_load_module.argtypes = [vp, vp, sz, C.POINTER(vp)]
+        L.b2g_wasm_free.argtypes = [vp]
+        L.b2g_wasm_info.argtypes = [vp, C.POINTER(WasmSummary)]
+        L.b2g_wasm_get_limits.argtypes = [vp, C.POINTER(WasmLimits)]
+        L.b2g_wasm_set_limits.argtypes = [vp, C.POINTER(WasmLimits)]
+        L.b2g_witness_calculate.argtypes = [vp, vp, C.c_uint32, C.c_uint32, vp, vp, vp, i, vp, vp]
+        L.b2g_wasm_run.argtypes = [vp, vp, C.c_char_p, C.c_uint32, C.c_uint32, vp, vp, vp]
         L.b2g_test_op.argtypes = [vp, i, vp, vp, sz, vp]
         L.b2g_last_timings.argtypes = [vp, vp]
         L.b2g_bench_device.argtypes = [vp, vp, vp, i, C.POINTER(C.c_float)]

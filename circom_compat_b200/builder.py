@@ -3,10 +3,13 @@
   CircomConfig.new(wtns, r1cs) / CircomBuilder.{new, push_input, setup, build}   <- /root/reference/src/circom/builder.rs:30-117
   CircomCircuit{r1cs, witness}.get_public_inputs()                               <- /root/reference/src/circom/circuit.rs:12-26
 
-The reference computes witnesses by running the circuit's WASM under wasmer (src/witness/*), which stays on the host and
-is out of scope here (no WASM runtime in this image).  `wtns` is therefore any *witness source*: a callable
-`inputs: dict[str, list[int]] -> list[int]` (e.g. a wrapper around snarkjs / a WASM runtime), or the path of a `.wtns`
-file produced for those inputs.  Everything downstream (matrices, setup, prove) is the same as with the reference.
+`wtns` is the *witness source*:
+  - the path of the circuit's circom 2 `.wasm` (recognised by its `\0asm` magic), as CircomConfig::new(wasm, r1cs)
+    takes it: build() then computes the witness on the GPU with witness.WitnessCalculator, the device interpreter that
+    stands in for the reference's wasmer runtime (src/witness/*);
+  - a callable `inputs: dict[str, list[int]] -> list[int]` (e.g. a wrapper around snarkjs);
+  - or the path of a `.wtns` file produced for those inputs.
+Everything downstream (matrices, setup, prove) is the same as with the reference.
 """
 from __future__ import annotations
 
@@ -17,6 +20,14 @@ from .r1cs import R1CS, R1CSFile, read_wtns
 from .zkey import R_MOD
 
 WitnessSource = Union[str, Callable[[Dict[str, List[int]]], List[int]]]
+
+
+def _is_wasm(path) -> bool:
+    try:
+        with open(path, 'rb') as f:
+            return f.read(4) == b'\0asm'
+    except OSError:              # a .wtns path may name a file that is written later, before build()
+        return False
 
 
 @dataclass
@@ -42,12 +53,17 @@ class CircomConfig:
     r1cs: R1CS
     wtns: WitnessSource
     sanity_check: bool = False
+    wasm: Optional[object] = None          # the WitnessCalculator of a .wasm source
 
     @staticmethod
     def new(wtns: WitnessSource, r1cs_path: str) -> 'CircomConfig':
         with open(r1cs_path, 'rb') as f:
             r1cs = R1CS.from_file(R1CSFile.new(f.read()))
-        return CircomConfig(r1cs, wtns)
+        wasm = None
+        if not callable(wtns) and _is_wasm(wtns):
+            from .witness import WitnessCalculator
+            wasm = WitnessCalculator.new(wtns)
+        return CircomConfig(r1cs, wtns, wasm=wasm)
 
 
 @dataclass
@@ -70,7 +86,12 @@ class CircomBuilder:
     def build(self) -> CircomCircuit:
         circom = self.setup()
         src = self.cfg.wtns
-        witness = src(self.inputs) if callable(src) else read_wtns(open(src, 'rb').read())
+        if self.cfg.wasm is not None:
+            witness = self.cfg.wasm.calculate_witness(self.inputs, self.cfg.sanity_check)
+        elif callable(src):
+            witness = src(self.inputs)
+        else:
+            witness = read_wtns(open(src, 'rb').read())
         # negative outputs of a witness calculator map to r - |w| (src/witness/witness_calculator.rs:171-174)
         witness = [int(x) % R_MOD for x in witness]
         if len(witness) != circom.r1cs.num_variables:

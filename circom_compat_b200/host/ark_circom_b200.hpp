@@ -38,7 +38,9 @@
 #include <cstdint>
 #include <cstring>
 #include <exception>
+#include <fstream>
 #include <istream>
+#include <iterator>
 #include <map>
 #include <memory>
 #include <optional>
@@ -554,6 +556,97 @@ struct Reduction {
 };
 typedef Reduction<B2G_REDUCTION_CIRCOM> CircomReduction;       // src/circom/qap.rs:12-14 (snarkjs keys)
 typedef Reduction<B2G_REDUCTION_LIBSNARK> LibsnarkReduction;   // ark-groth16's default QAP (tests/groth16.rs:9,25-35; needs matrices.c)
+
+// ---------------------------------------------------------------------------------------------- circom 2 witnesses
+// WitnessCalculator (src/witness/witness_calculator.rs) with the circuit's .wasm run by the library's device interpreter
+// (b2g_wasm_load / b2g_witness_calculate): one lane per witness, many witnesses per call.  Input values are reduced
+// mod r; names are hashed with FNV-1a 64.  A lane that calls the circuit's exceptionHandler stops there.
+struct WitnessError : std::runtime_error {
+    uint32_t status;
+    WitnessError(uint32_t st, const std::string& m) : std::runtime_error(m), status(st) {}
+};
+
+class WitnessCalculator {
+public:
+    typedef std::vector<std::pair<std::string, std::vector<BigInt256>>> Inputs;   // (name, values), in order
+    uint32_t n32 = 0, n64 = 4, witness_size = 0, input_size = 0, version = 0;
+
+    explicit WitnessCalculator(const std::vector<uint8_t>& wasm, Gpu& gpu = Gpu::instance()) : gpu_(gpu) {
+        check(b2g_wasm_load(gpu.ctx(), wasm.data(), wasm.size(), &h_));
+        b2g_wasm_summary s; check(b2g_wasm_info(h_, &s));
+        n32 = s.n32; witness_size = s.witness_size; input_size = s.input_size; version = s.version;
+    }
+    static WitnessCalculator from_file(const std::string& path, Gpu& gpu = Gpu::instance()) {
+        std::ifstream f(path, std::ios::binary);
+        if (!f) throw SerializationError("cannot open " + path);
+        return WitnessCalculator(std::vector<uint8_t>((std::istreambuf_iterator<char>(f)), std::istreambuf_iterator<char>()), gpu);
+    }
+    ~WitnessCalculator() { if (h_) b2g_wasm_free(h_); }
+    WitnessCalculator(WitnessCalculator&& o) noexcept : n32(o.n32), n64(o.n64), witness_size(o.witness_size), input_size(o.input_size),
+        version(o.version), gpu_(o.gpu_), h_(o.h_) { o.h_ = nullptr; }
+    WitnessCalculator(const WitnessCalculator&) = delete;
+    WitnessCalculator& operator=(const WitnessCalculator&) = delete;
+    b2g_wasm* handle() const { return h_; }
+
+    static uint64_t fnv(const std::string& name) {
+        uint64_t h = 0xcbf29ce484222325ULL;
+        for (unsigned char c : name) { h ^= c; h *= 0x100000001b3ULL; }
+        return h;
+    }
+    static const char* status_name(uint32_t st) {
+        static const char* const ex[7] = {"Unknown error", "Signal not found", "Too many signals set", "Signal already set",
+                                          "Assert Failed", "Not enough memory", "Input signal array access exceeds the size"};
+        static const char* const tr[9] = {"ok", "unreachable executed", "memory access out of bounds", "integer divide by zero",
+                                          "integer overflow", "call stack exhausted", "instruction budget (fuel) exhausted",
+                                          "bad call_indirect", "getWitnessSize disagrees with the module's witness size"};
+        if (st >= B2G_WASM_EXCEPTION) return ex[st - B2G_WASM_EXCEPTION < 7 ? st - B2G_WASM_EXCEPTION : 0];
+        return st < 9 ? tr[st] : "unknown status";
+    }
+
+    // many witnesses with the same input names and lengths: out[i] (Montgomery Fr, witness_size each) and status[i]
+    void calculate_witnesses(const std::vector<Inputs>& batch, std::vector<std::vector<Fr>>& out, std::vector<uint32_t>& status,
+                             bool sanity_check = false) {
+        const size_t count = batch.size();
+        out.assign(count, std::vector<Fr>());
+        status.assign(count, 0);
+        if (!count) return;
+        std::vector<uint64_t> hashes; std::vector<uint32_t> counts;
+        for (const auto& in : batch[0]) { hashes.push_back(fnv(in.first)); counts.push_back((uint32_t)in.second.size()); }
+        std::vector<BigInt256> vals;
+        for (size_t i = 0; i < count; i++) {
+            if (batch[i].size() != hashes.size()) throw std::invalid_argument("calculate_witnesses: inputs differ in shape");
+            for (size_t k = 0; k < batch[i].size(); k++) {
+                if (fnv(batch[i][k].first) != hashes[k] || batch[i][k].second.size() != counts[k])
+                    throw std::invalid_argument("calculate_witnesses: inputs differ in shape");
+                for (BigInt256 v : batch[i][k].second) {
+                    while (detail::geq(v.l, detail::FR_P)) {            // v mod r (v < 2^256 < 6 r)
+                        unsigned __int128 br = 0;
+                        for (int j = 0; j < 4; j++) {
+                            const unsigned __int128 t = (unsigned __int128)v.l[j] - detail::FR_P[j] - br;
+                            v.l[j] = (uint64_t)t; br = (t >> 64) & 1;
+                        }
+                    }
+                    vals.push_back(v);
+                }
+            }
+        }
+        std::vector<Fr> flat((size_t)count * witness_size);
+        check(b2g_witness_calculate(gpu_.ctx(), h_, (uint32_t)count, (uint32_t)hashes.size(), hashes.data(), counts.data(),
+                                    vals.empty() ? nullptr : vals.data(), sanity_check ? 1 : 0, flat.data(), status.data()));
+        for (size_t i = 0; i < count; i++) out[i].assign(flat.begin() + i * witness_size, flat.begin() + (i + 1) * witness_size);
+    }
+    // calculate_witness_element: one witness as field elements; throws WitnessError naming the exception or trap
+    std::vector<Fr> calculate_witness_element(const Inputs& inputs, bool sanity_check = false) {
+        std::vector<std::vector<Fr>> out; std::vector<uint32_t> st;
+        calculate_witnesses({inputs}, out, st, sanity_check);
+        if (st[0]) throw WitnessError(st[0], status_name(st[0]));
+        return out[0];
+    }
+
+private:
+    Gpu& gpu_;
+    b2g_wasm* h_ = nullptr;
+};
 
 }  // namespace ark_circom
 #include "ark_circom_verifier.hpp"

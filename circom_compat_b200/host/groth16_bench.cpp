@@ -91,6 +91,19 @@ static BigInt256 parse_dec(const std::string& s) {
     return b;
 }
 
+// r - (v mod r), and 0 for a multiple of r: how snarkjs maps a negative input
+static BigInt256 negate_mod_r(BigInt256 v) {
+    auto sub = [](BigInt256& x, const uint64_t* y) {
+        unsigned __int128 br = 0;
+        for (int j = 0; j < 4; j++) { const unsigned __int128 t = (unsigned __int128)x.l[j] - y[j] - br; x.l[j] = (uint64_t)t; br = (t >> 64) & 1; }
+    };
+    while (ark_circom::detail::geq(v.l, ark_circom::detail::FR_P)) sub(v, ark_circom::detail::FR_P);
+    if (!(v.l[0] | v.l[1] | v.l[2] | v.l[3])) return v;
+    BigInt256 r; memcpy(r.l, ark_circom::detail::FR_P, 32);
+    sub(r, v.l);
+    return r;
+}
+
 static BigInt256 parse_hex(const std::string& s) {
     BigInt256 b = {{0, 0, 0, 0}};
     std::string t = s.rfind("0x", 0) == 0 ? s.substr(2) : s;
@@ -311,6 +324,56 @@ int main(int argc, char** argv) {
             const std::vector<Fr> inputs(w.begin() + 1, w.begin() + matrices.num_instance_variables);
             std::printf("verified=%d\n", G::verify_with_processed_vk(G::process_vk(pk.vk), inputs, proof) ? 1 : 0);
             return 0;
+        }
+        if (const char* wasm = std::getenv("B2G_WITNESS")) {                // .wasm + inputs -> witnesses on the GPU -> setup -> prove -> verify
+            if (argc < 3) { std::fprintf(stderr, "usage: B2G_WITNESS=<circuit.wasm> %s <circuit.r1cs> name=value ... [count]\n", argv[0]); return 2; }
+            typedef Groth16T<LibsnarkReduction> G;
+            std::ifstream rf(argv[1], std::ios::binary);
+            if (!rf) throw SerializationError("cannot open r1cs");
+            const R1CS r1cs = R1CS::read(rf);
+            const ConstraintMatrices matrices = r1cs.to_matrices();
+            WitnessCalculator::Inputs inputs;
+            size_t count = 1;
+            for (int i = 2; i < argc; i++) {                                 // name=value (decimal, a leading - maps to r - |v|), repeated for arrays
+                const std::string a = argv[i];
+                const size_t eq = a.find('=');
+                if (eq == std::string::npos) { count = std::stoul(a); continue; }
+                const std::string name = a.substr(0, eq), val = a.substr(eq + 1);
+                const bool neg = !val.empty() && val[0] == '-';
+                BigInt256 v = parse_dec(neg ? val.substr(1) : val);
+                if (neg) v = negate_mod_r(v);
+                auto it = std::find_if(inputs.begin(), inputs.end(), [&](const auto& e) { return e.first == name; });
+                if (it == inputs.end()) inputs.push_back({name, {v}}); else it->second.push_back(v);
+            }
+            WitnessCalculator calc = WitnessCalculator::from_file(wasm);
+            std::vector<std::vector<Fr>> ws; std::vector<uint32_t> status;
+            const auto t0 = std::chrono::steady_clock::now();
+            calc.calculate_witnesses(std::vector<WitnessCalculator::Inputs>(count, inputs), ws, status);
+            const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+            for (size_t i = 0; i < count; i++)
+                if (status[i]) { std::printf("witness %zu: %s\n", i, WitnessCalculator::status_name(status[i])); return 1; }
+            std::printf("witnesses %zu x %u wires in %.3f ms (%.1f witnesses/s, including the module's device state set-up)\n",
+                        count, calc.witness_size, ms, count / (ms * 1e-3));
+            if (const char* out = std::getenv("B2G_WITNESS_OUT")) {          // the Montgomery witnesses, witness-major
+                std::ofstream of(out, std::ios::binary);
+                for (const auto& w : ws) of.write((const char*)w.data(), w.size() * sizeof(Fr));
+            }
+            std::mt19937_64 rng(0x5EED);
+            const ProvingKey pk = G::generate_random_parameters_with_reduction(matrices, rng);
+            std::vector<std::pair<Fr, Fr>> rs;
+            std::vector<const std::vector<Fr>*> ptrs;
+            std::vector<std::vector<Fr>> pubs;
+            for (size_t i = 0; i < count; i++) {
+                const Fr r = Fr::rand(rng), s2 = Fr::rand(rng);
+                rs.push_back({r, s2});
+                ptrs.push_back(&ws[i]);
+                pubs.emplace_back(ws[i].begin() + 1, ws[i].begin() + matrices.num_instance_variables);
+            }
+            const std::vector<Proof> proofs = G::create_proofs(pk, matrices, rs, ptrs);
+            const std::vector<bool> ok = G::verify_many(G::process_vk(pk.vk), pubs, proofs);
+            const size_t good = (size_t)std::count(ok.begin(), ok.end(), true);
+            std::printf("verified %zu/%zu\n", good, count);
+            return good == count ? 0 : 1;
         }
         if (const char* seed = std::getenv("B2G_SETUP")) {                  // R1CS -> setup on the GPU -> prove -> verify
             if (argc < 3) { std::fprintf(stderr, "usage: B2G_SETUP=<seed> %s <circuit.r1cs> <witness.wtns>\n", argv[0]); return 2; }

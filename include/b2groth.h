@@ -40,6 +40,8 @@
  *   b2g_setup_from_lagrange <- snarkjs groth16 setup from a prepared ceremony, with no point transforms
  *   b2g_setup_check        <- snarkjs zkey verify: a proving key against its circuit and powers-of-tau ceremony
  *   b2g_fixed_base_g1/g2  <- the batch fixed-base multiplications of that setup, for the standard generators only
+ *   b2g_wasm_load / b2g_witness_calculate <- WitnessCalculator::new + calculate_witness (src/witness/witness_calculator.rs):
+ *                             a circom 2 circuit's .wasm run on the device, one lane per witness, many witnesses per call
  *
  * Conventions
  *   - every function returns 0 (B2G_OK) or a negative error code; b2g_last_error() gives a thread-local message.
@@ -914,6 +916,73 @@ B2G_API int b2g_bench_msm(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, int query, int
 /* number of kernel launches issued by this library (process-wide, all contexts) so far; a replayed proof graph counts the kernel
  * nodes it contains */
 B2G_API int b2g_launch_count(b2g_ctx* ctx, uint64_t* count);
+
+/* ---------------------------------------------------------------------------------------------- circom 2 witnesses
+ * A module is decoded, validated and translated on the host into the device interpreter's fixed-width code.  It must
+ * use only the integer subset of WebAssembly 1.0 (every i32/i64 numeric, comparison and conversion op, the sign
+ * extension ops, integer loads and stores, memory.size / memory.grow, select, drop, locals, globals, block, loop, if,
+ * br, br_if, br_table, return, call, call_indirect, unreachable, active data and element segments) and import nothing
+ * but the four circom 2 runtime functions (runtime.exceptionHandler, printErrorMessage, writeBufferMessage,
+ * showSharedRWMemory).  Anything else is refused with B2G_E_SHAPE and b2g_last_error() names the cause (the function
+ * index and opcode, the import, the missing export).
+ *
+ * b2g_wasm_load additionally requires the circom 2 protocol exports, and runs one lane on the device to read the
+ * field (getFieldNumLen32 must be 8 and getRawPrime BN254's r) and the sizes; a circom 1 module is refused.
+ * b2g_wasm_load_module loads any module of the subset for b2g_wasm_run (no protocol, no probe). */
+typedef struct b2g_wasm b2g_wasm;
+typedef struct {
+    uint32_t n32;            /* getFieldNumLen32 */
+    uint32_t witness_size;   /* getWitnessSize */
+    uint32_t input_size;     /* getInputSize */
+    uint32_t version;        /* getVersion: the circom major version */
+    uint32_t mem_pages;      /* initial linear memory, 64 KiB pages */
+    uint32_t reserved[3];
+} b2g_wasm_summary;
+/* Per-lane limits, read with b2g_wasm_get_limits and changed with b2g_wasm_set_limits.  memory.grow past max_pages
+ * returns -1; a call deeper than max_depth, or whose locals and operand stack do not fit in stack_slots 8-byte slots
+ * (the module's globals come first and need globals + 8 at least, else the limits are refused), ends the lane with
+ * B2G_WASM_STACK; a lane that runs more than `fuel` translated instructions ends with B2G_WASM_FUEL.  budget_bytes bounds
+ * the device memory a call uses for lane state: the lanes run in chunks of whole warps that fit it (0 = half the free
+ * device memory, at most 32 GiB); a call whose budget cannot hold one warp (32 lanes) is refused with B2G_E_SHAPE.
+ * Chunking does not change any result.  Defaults, sized from the module at load: its initial pages + 5 (within its
+ * declared maximum), 256, globals + 4096, 2^32, 0.  On an H100 one lane runs 1-5 M instructions/s, so the default fuel
+ * lets a lane caught in an endless loop hold the call for roughly 14 to 65 minutes: lower it for untrusted modules. */
+typedef struct {
+    uint32_t max_pages, max_depth, stack_slots, reserved;
+    uint64_t fuel, budget_bytes;
+} b2g_wasm_limits;
+/* lane statuses */
+#define B2G_WASM_OK 0
+#define B2G_WASM_UNREACHABLE 1     /* unreachable executed */
+#define B2G_WASM_MEMORY 2          /* a load or store outside the lane's memory */
+#define B2G_WASM_DIV_ZERO 3        /* integer division or remainder by zero */
+#define B2G_WASM_OVERFLOW 4        /* div_s of the minimum by -1 */
+#define B2G_WASM_STACK 5           /* call depth or stack slots exhausted */
+#define B2G_WASM_FUEL 6            /* instruction budget exhausted */
+#define B2G_WASM_INDIRECT 7        /* call_indirect of an empty or out-of-range element, or of the wrong type */
+#define B2G_WASM_PROTOCOL 8        /* getWitnessSize disagreed with the size the load read */
+#define B2G_WASM_EXCEPTION 0x100   /* + c: the circuit called runtime.exceptionHandler(c) (4 = assert failed, ...) */
+
+B2G_API int b2g_wasm_load(b2g_ctx* ctx, const void* bytes, size_t len, b2g_wasm** out);
+B2G_API int b2g_wasm_load_module(b2g_ctx* ctx, const void* bytes, size_t len, b2g_wasm** out);
+B2G_API int b2g_wasm_free(b2g_wasm* wasm);
+B2G_API int b2g_wasm_info(b2g_wasm* wasm, b2g_wasm_summary* out);
+B2G_API int b2g_wasm_get_limits(b2g_wasm* wasm, b2g_wasm_limits* out);
+B2G_API int b2g_wasm_set_limits(b2g_wasm* wasm, const b2g_wasm_limits* limits);
+/* count witnesses of one circuit, one device lane each, with no host step between the calls of the circom 2 protocol:
+ * init(sanity_check); for input k (FNV-1a 64 hash hashes[k], split into its high and low 32 bits) and each of its
+ * counts[k] values i: 8 x writeSharedRWMemory(j, limb j), setInputSignal(msb, lsb, i); getWitnessSize; for each wire
+ * i: getWitness(i) and 8 x readSharedRWMemory(j).  Every witness has the same inputs; values_canon holds count x
+ * sum(counts) 32-byte canonical values (below r), witness-major, inputs in order.  w_mont_out receives count x
+ * witness_size x 32 B in Montgomery form (b2g_prove_many's layout; all zeros for a lane that did not finish) and
+ * status_out one B2G_WASM_* status per witness. */
+B2G_API int b2g_witness_calculate(b2g_ctx* ctx, b2g_wasm* wasm, uint32_t count, uint32_t n_inputs, const uint64_t* hashes,
+                                  const uint32_t* counts, const void* values_canon, int sanity_check, void* w_mont_out,
+                                  uint32_t* status_out);
+/* count lanes each call the exported function `name` with nargs (at most 3) arguments, lane i taking
+ * args[i*nargs .. i*nargs+nargs) (i32 zero-extended, i64 as is); results[i] = its result (0 if it has none). */
+B2G_API int b2g_wasm_run(b2g_ctx* ctx, b2g_wasm* wasm, const char* name, uint32_t count, uint32_t nargs,
+                         const uint64_t* args, uint64_t* results, uint32_t* status_out);
 
 #ifdef __cplusplus
 }
