@@ -263,25 +263,6 @@ void scale_split_test_op(cudaStream_t st, const void* a, size_t n, void* out) {
 }
 
 // ---------------------------------------------------------------------------------------------- host side
-// a device buffer that may hold secrets: zeroed on the stream before it is freed, on success and on error alike
-struct SecretBuf {
-    uint8_t* p = nullptr;
-    size_t bytes;
-    cudaStream_t st;
-    SecretBuf(size_t b, cudaStream_t s) : bytes(b ? b : 1), st(s) { CUDA_CHECK(cudaMalloc(&p, bytes)); }
-    ~SecretBuf() {
-        if (!p) return;
-        cudaMemsetAsync(p, 0, bytes, st);
-        cudaStreamSynchronize(st);
-        cudaFree(p);
-    }
-};
-
-static void wipe(void* p, size_t n) {
-    volatile uint8_t* q = (volatile uint8_t*)p;
-    while (n--) *q++ = 0;
-}
-
 // where the scalars of a pass come from: host (n x 32 B canonical), or the device powers c t^(i) of t (Montgomery)
 struct ScaleScalars {
     const uint8_t* host = nullptr;
@@ -306,21 +287,16 @@ static void scale_pass(Staging& sg, bool g2, const void* in, void* out, uint64_t
     for (uint64_t off = 0; off < count; off += POWERS_SLICE, k++) {
         const uint32_t cnt = (uint32_t)std::min<uint64_t>(POWERS_SLICE, count - off);
         const int b = (int)(k & 1);
-        CUDA_CHECK(cudaEventSynchronize(sg.copied[b]));
-        memcpy(sg.host[b], (const uint8_t*)in + off * row, (size_t)cnt * row);
-        CUDA_CHECK(cudaStreamWaitEvent(sg.cp, sg.used[b], 0));
-        CUDA_CHECK(cudaMemcpyAsync(sg.dev[b], sg.host[b], (size_t)cnt * row, cudaMemcpyHostToDevice, sg.cp));
-        CUDA_CHECK(cudaEventRecord(sg.copied[b], sg.cp));
-        CUDA_CHECK(cudaStreamWaitEvent(st, sg.copied[b], 0));
-        if (bad) powers_rules(g2, sg.dev[b], cnt, off, gen, bad, st);
+        uint8_t* d = sg.upload(b, (const uint8_t*)in + off * row, (size_t)cnt * row);
+        if (bad) powers_rules(g2, d, cnt, off, gen, bad, st);
         if (sc.host) CUDA_CHECK(cudaMemcpyAsync(sc.d_k, sc.host + off * 32, (size_t)cnt * 32, cudaMemcpyHostToDevice, st));
         else powers_scalars(sc.t, off, cnt, sc.d_pw, sc.d_k, st);
         const unsigned blocks = (cnt + 127) / 128;
-        if (g2) points_scale_kernel<G2, Fq2><<<blocks, 128, 0, st>>>(sg.dev[b], cnt, sc.d_k, sc.c);
-        else points_scale_kernel<G1, Fq><<<blocks, 128, 0, st>>>(sg.dev[b], cnt, sc.d_k, sc.c);
+        if (g2) points_scale_kernel<G2, Fq2><<<blocks, 128, 0, st>>>(d, cnt, sc.d_k, sc.c);
+        else points_scale_kernel<G1, Fq><<<blocks, 128, 0, st>>>(d, cnt, sc.d_k, sc.c);
         g_launch_count += 1;
         CUDA_CHECK(cudaGetLastError());
-        CUDA_CHECK(cudaMemcpyAsync(sg.host[b], sg.dev[b], (size_t)cnt * row, cudaMemcpyDeviceToHost, st));
+        CUDA_CHECK(cudaMemcpyAsync(sg.host[b], d, (size_t)cnt * row, cudaMemcpyDeviceToHost, st));
         CUDA_CHECK(cudaEventRecord(sg.used[b], st));
         if (k) drain(b ^ 1);
         prev_off = off;
@@ -329,41 +305,23 @@ static void scale_pass(Staging& sg, bool g2, const void* in, void* out, uint64_t
     if (k) drain((int)((k - 1) & 1));
 }
 
-static const uint32_t R_WORDS[8] = {FrParams::P0, FrParams::P1, FrParams::P2, FrParams::P3, FrParams::P4, FrParams::P5, FrParams::P6, FrParams::P7};
-
 static void points_scale_run(b2g_ctx* ctx, int g2, size_t n, const void* pts, const void* scalars, void* out) {
     if (!ctx || (n && (!pts || !scalars || !out))) throw_error(B2G_E_SHAPE, "null pointer");
-    const CtxView cv = ctx_view(ctx);
-    if (cv.proof_pending) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
+    const CtxView cv = ctx_idle(ctx);
     const uint8_t* s = (const uint8_t*)scalars;
-    for (size_t i = 0; i < n; i++) {                    // k_i < r: the split's bounds need it
-        const uint8_t* x = s + 32 * i;
-        for (int w = 7; w >= 0; w--) {
-            uint32_t v; memcpy(&v, x + 4 * w, 4);
-            if (v != R_WORDS[w]) {
-                if (v > R_WORDS[w]) throw_error(B2G_E_INPUT, "scalars[" + std::to_string(i) + "] is not below r");
-                break;
-            }
-            if (w == 0) throw_error(B2G_E_INPUT, "scalars[" + std::to_string(i) + "] is not below r");
-        }
-    }
+    for (size_t i = 0; i < n; i++)                      // k_i < r: the split's bounds need it
+        if (!below(s + 32 * i, R_WORDS)) throw_error(B2G_E_INPUT, "scalars[" + std::to_string(i) + "] is not below r");
     if (n == 0) return;
     DevGuard g(cv.device);
     cudaStream_t st = cv.st;
     const size_t cap = std::min<size_t>(n, POWERS_SLICE);
-    SecretBuf k(cap * sizeof(fe), st);
-    Staging sg(cap * (g2 ? 128 : 64), st);
+    DevArena mem(st, true);
     ScaleScalars sc;
+    sc.d_k = mem.alloc<fe>(cap * sizeof(fe));
+    Staging sg(cap * (g2 ? 128 : 64), st);
     sc.host = s;
-    sc.d_k = (fe*)k.p;
     scale_pass(sg, g2 != 0, pts, out, n, sc, false, nullptr);
     CUDA_CHECK(cudaStreamSynchronize(st));
-}
-
-// mont[j] = canon[j] in Montgomery form, j < 3
-__global__ void contribute_consts_kernel(const fe* __restrict__ canon, fe* __restrict__ mont) {
-    if (threadIdx.x == 0 && blockIdx.x == 0)
-        for (int j = 0; j < 3; j++) mont[j] = Fr::from_canonical(canon[j]);
 }
 
 static bool overlaps(const void* a, size_t na, const void* b, size_t nb) {
@@ -373,11 +331,10 @@ static bool overlaps(const void* a, size_t na, const void* b, size_t nb) {
 
 static void powers_contribute_run(b2g_ctx* ctx, const b2g_powers_desc* pw, const b2g_powers_secrets* sec, const b2g_powers_out* o) {
     if (!ctx || !pw || !sec || !o) throw_error(B2G_E_SHAPE, "null pointer");
-    const CtxView cv = ctx_view(ctx);
-    if (cv.proof_pending) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
+    const CtxView cv = ctx_idle(ctx);
     const uint32_t p = pw->log_size;
     if (p < 1 || p > 28) throw_error(B2G_E_DOMAIN, "b2g_powers_contribute: log_size " + std::to_string(p) + " is outside 1..28");
-    if (!pw->tau_g1 || !pw->tau_g2 || !pw->alpha_tau_g1 || !pw->beta_tau_g1 || !pw->beta_g2) throw_error(B2G_E_SHAPE, "null powers array");
+    powers_arrays(pw, true);
     if (!o->tau_g1 || !o->tau_g2 || !o->alpha_tau_g1 || !o->beta_tau_g1 || !o->beta_g2) throw_error(B2G_E_SHAPE, "null output array");
     if (!sec->tau || !sec->alpha || !sec->beta) throw_error(B2G_E_SHAPE, "null secret");
     const uint64_t n = 1ull << p;
@@ -400,31 +357,21 @@ static void powers_contribute_run(b2g_ctx* ctx, const b2g_powers_desc* pw, const
     cudaStream_t st = cv.st;
     const uint64_t most = std::min<uint64_t>(2 * n - 1, POWERS_SLICE);
     // the secrets (canonical, then Montgomery), the powers kernels' words, and one slice of per-point scalars
-    SecretBuf keys(6 * sizeof(fe) + 2 * sizeof(fe), st);
-    SecretBuf scal((most + 16) * sizeof(fe), st);
-    fe* d_canon = (fe*)keys.p;
+    DevArena mem(st, true);
+    fe* d_canon = mem.alloc<fe>(6 * sizeof(fe) + 2 * sizeof(fe));
     fe* d_mont = d_canon + 3;
-    {
-        uint8_t h[3 * 32];
-        for (int j = 0; j < 3; j++) memcpy(h + 32 * j, secs[j], 32);
-        // on the call's stream; h is wiped once the copy is done
-        cudaError_t e = cudaMemcpyAsync(d_canon, h, sizeof(h), cudaMemcpyHostToDevice, st);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-        wipe(h, sizeof(h));
-        CUDA_CHECK(e);
-    }
-    contribute_consts_kernel<<<1, 1, 0, st>>>(d_canon, d_mont);
-    g_launch_count += 1;
-    CUDA_CHECK(cudaGetLastError());
+    fe* d_scal = mem.alloc<fe>((most + 16) * sizeof(fe));
+    upload_secrets(d_canon, secs, 3, st);
+    to_mont(d_canon, 3, d_mont, st);
     CUDA_CHECK(cudaMemsetAsync(d_canon, 0, 3 * sizeof(fe), st));   // only the Montgomery forms are read from here on
 
-    SecretBuf small(128 + 64 + 8 * 5, st);             // the failing point, its rule, the lowest failing index per array
-    unsigned long long* d_bad = (unsigned long long*)(small.p + 192);
+    uint8_t* small = mem.alloc(128 + 64 + 8 * 5);     // the failing point, its rule, the lowest failing index per array
+    unsigned long long* d_bad = (unsigned long long*)(small + 192);
     CUDA_CHECK(cudaMemsetAsync(d_bad, 0xff, 8 * 5, st));
     Staging sg(std::max<size_t>(most * 64, std::min<uint64_t>(n, POWERS_SLICE) * 128), st);
     ScaleScalars sc;
     sc.t = d_mont;
-    sc.d_k = (fe*)scal.p;
+    sc.d_k = d_scal;
     sc.d_pw = d_mont + 3;
     for (int a = 0; a < 5; a++) {
         const Array& x = arrays[a];
@@ -434,11 +381,8 @@ static void powers_contribute_run(b2g_ctx* ctx, const b2g_powers_desc* pw, const
         CUDA_CHECK(cudaMemcpyAsync(&bad, d_bad + a, 8, cudaMemcpyDeviceToHost, st));
         CUDA_CHECK(cudaStreamSynchronize(st));
         if (bad >= x.count) continue;
-        const size_t row = x.g2 ? 128 : 64;
-        CUDA_CHECK(cudaMemcpyAsync(small.p, (const uint8_t*)x.in + bad * row, row, cudaMemcpyHostToDevice, st));
-        const uint32_t rule = powers_point_rule(x.g2, small.p, x.gen && bad == 0, (uint32_t*)(small.p + 128), st);
+        const uint32_t rule = bad_point_rule("b2g_powers_contribute", x.in, bad, x.g2, x.gen, small, (uint32_t*)(small + 128), st);
         static const char* const RULES[6] = {"", "a coordinate >= p", "off the curve", "at infinity", "not in G2", "not the generator"};
-        if (!rule || rule > 5) throw_error(B2G_E_DEVICE, "b2g_powers_contribute: the point rules disagree on point " + std::to_string(bad));
         throw_error(B2G_E_INPUT, std::string(x.name) + "[" + std::to_string(bad) + "]: " + (rule == 2 && x.g2 ? "off the twist" : RULES[rule]));
     }
     CUDA_CHECK(cudaStreamSynchronize(st));

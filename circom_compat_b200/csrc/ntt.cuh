@@ -17,6 +17,15 @@ struct NttDomain {
 
 void ntt_domain_create(NttDomain& d, int logn, cudaStream_t st, bool libsnark = false);
 void ntt_domain_destroy(NttDomain& d);
+// an NttDomain of 2^logn points that is destroyed with its holder, also when its creation fails part way
+struct NttDomainHold : NttDomain {
+    NttDomainHold(int logn, cudaStream_t st) {
+        try { ntt_domain_create(*this, logn, st); } catch (...) { ntt_domain_destroy(*this); throw; }
+    }
+    NttDomainHold(const NttDomainHold&) = delete;
+    NttDomainHold& operator=(const NttDomainHold&) = delete;
+    ~NttDomainHold() { ntt_domain_destroy(*this); }
+};
 // count > 1: a batch of proofs whose vectors lie 2^logn elements apart (b2g_prove_many)
 void ntt_witness_transform(const NttDomain& d, fe* a, fe* b, fe* c, fe* out, cudaStream_t st, uint32_t count = 1);
 void ntt_transform_single(const NttDomain& d, fe* v, cudaStream_t st);

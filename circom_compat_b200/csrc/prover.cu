@@ -145,6 +145,12 @@ struct Scalar256 { uint32_t l[8]; };
 
 CtxView ctx_view(b2g_ctx* ctx) { return {ctx->device, ctx->st[0], ctx->pending_out != nullptr, &ctx->vbufs}; }
 
+CtxView ctx_idle(b2g_ctx* ctx) {
+    const CtxView cv = ctx_view(ctx);
+    if (cv.proof_pending) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
+    return cv;
+}
+
 // ------------------------------------------------------------------------------------------------ glue kernels
 // pre[0] = r*delta1, pre[1] = K_C = (r*s)*delta1 + s*(alpha1 + a_query[0]) + r*(beta1 + b_g1_query[0]) (G1 XYZZ, 128 B
 // each); then s*delta2 (G2 XYZZ, 256 B).  Every base here is fixed per key: its 8-bit window table is built at b2g_pk_load,
@@ -1194,7 +1200,7 @@ static void prove_submit(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, uint32_t count,
                          uint8_t* proofs_out) {
     if (!ctx || !r_canon || !s_canon || !w_mont || !proofs_out) throw_error(B2G_E_SHAPE, "null pointer");
     if (ctx->shard_count != 1) throw_error(B2G_E_SHAPE, "a whole proof (b2g_prove, b2g_prove_many) needs an unsharded context; use b2g_prove_partial/finish");
-    if (ctx->pending_out) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
+    ctx_idle(ctx);
     if (count == 0 || count > MAX_BATCH) throw_error(B2G_E_SHAPE, "b2g_prove_many: count must be in [1, " + std::to_string(MAX_BATCH) + "]");
     for (uint32_t j = 0; j < count; j++) if (!w_mont[j]) throw_error(B2G_E_SHAPE, "null witness " + std::to_string(j));
     const auto t0 = std::chrono::steady_clock::now();
@@ -1961,7 +1967,7 @@ int b2g_prove_keys(b2g_ctx* ctx, b2g_pk_group* g, const uint32_t* counts, const 
     return guarded_clear([&] {
         if (!ctx || !g || !counts || !r_canon || !s_canon || !w_mont || !proofs_out) throw_error(B2G_E_SHAPE, "null pointer");
         if (ctx->shard_count != 1) throw_error(B2G_E_SHAPE, "b2g_prove_keys needs an unsharded context");
-        if (ctx->pending_out) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
+        ctx_idle(ctx);
         if (g->device != ctx->device) throw_error(B2G_E_SHAPE, "handle belongs to another device");
         const std::vector<KeyBases> bases = group_bases(g);
         GroupLayout L;

@@ -20,7 +20,6 @@
 //   verdict       setup_check_verdict_kernel (verify.cu): E1-E3 compare sums, E4-E6 are three pairing products
 // Every scalar is canonical: the Montgomery product of a Montgomery coefficient and a canonical weight is the canonical product,
 // and the transform, being linear, maps canonical inputs to canonical outputs.
-#include <cub/cub.cuh>
 #include <algorithm>
 #include <cstring>
 #include <string>
@@ -47,8 +46,15 @@ enum : size_t {
     PV_BYTES = PV_WORD + 32
 };
 
-__global__ void powers_rho_kernel(const fe* __restrict__ canon, fe* __restrict__ mont) {
-    if (threadIdx.x == 0 && blockIdx.x == 0) *mont = Fr::from_canonical(*canon);
+__global__ void to_mont_kernel(const fe* __restrict__ canon, uint32_t n, fe* __restrict__ mont) {
+    if (threadIdx.x == 0 && blockIdx.x == 0)
+        for (uint32_t j = 0; j < n; j++) mont[j] = Fr::from_canonical(canon[j]);
+}
+
+void to_mont(const fe* canon, uint32_t n, fe* mont, cudaStream_t st) {
+    to_mont_kernel<<<1, 1, 0, st>>>(canon, n, mont);
+    g_launch_count += 1;
+    CUDA_CHECK(cudaGetLastError());
 }
 
 template <class C, class F>
@@ -73,70 +79,57 @@ static void powers_pass(Staging& sg, PowersMsm* msm, bool g2, const void* host, 
     for (uint64_t off = 0; off < count; off += POWERS_SLICE, k++) {
         const uint32_t cnt = (uint32_t)std::min<uint64_t>(POWERS_SLICE, count - off);
         const int b = (int)(k & 1);
-        CUDA_CHECK(cudaEventSynchronize(sg.copied[b]));               // the pinned buffer's last copy is done
-        memcpy(sg.host[b], (const uint8_t*)host + off * row, (size_t)cnt * row);
-        CUDA_CHECK(cudaStreamWaitEvent(sg.cp, sg.used[b], 0));         // the device buffer's last slice is done
-        CUDA_CHECK(cudaMemcpyAsync(sg.dev[b], sg.host[b], (size_t)cnt * row, cudaMemcpyHostToDevice, sg.cp));
-        CUDA_CHECK(cudaEventRecord(sg.copied[b], sg.cp));
-        CUDA_CHECK(cudaStreamWaitEvent(sg.st, sg.copied[b], 0));
-        if (bad && loose) setup_rules(g2, sg.dev[b], cnt, off, bad, sg.st);
-        else if (bad) powers_rules(g2, sg.dev[b], cnt, off, gen, bad, sg.st);
-        if (msm) powers_msm_slice(*msm, sg.dev[b], cnt, start + off, rho, sg.st, scalars ? scalars + off : nullptr);
+        const uint8_t* d = sg.upload(b, (const uint8_t*)host + off * row, (size_t)cnt * row);
+        if (bad && loose) setup_rules(g2, d, cnt, off, bad, sg.st);
+        else if (bad) powers_rules(g2, d, cnt, off, gen, bad, sg.st);
+        if (msm) powers_msm_slice(*msm, d, cnt, start + off, rho, sg.st, scalars ? scalars + off : nullptr);
         CUDA_CHECK(cudaEventRecord(sg.used[b], sg.st));
     }
 }
 
-struct DevBuf {
-    uint8_t* p = nullptr;
-    explicit DevBuf(size_t bytes) { CUDA_CHECK(cudaMalloc(&p, bytes)); }
-    ~DevBuf() { if (p) cudaFree(p); }
-};
-
 static void powers_msm_run(b2g_ctx* ctx, int g2, size_t n, const void* bases, const void* rho, void* out) {
     if (!ctx || !rho || !out || (n && !bases)) throw_error(B2G_E_SHAPE, "null pointer");
-    const CtxView cv = ctx_view(ctx);
-    if (cv.proof_pending) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
+    const CtxView cv = ctx_idle(ctx);
     const uint8_t* r = (const uint8_t*)rho;
-    if (!scalar_ok(r) && !std::all_of(r, r + 32, [](uint8_t b) { return b == 0; })) throw_error(B2G_E_INPUT, "rho is not below r");
+    if (!below(r, R_WORDS)) throw_error(B2G_E_INPUT, "rho is not below r");
     const size_t row = g2 ? 128 : 64;
     if (n == 0) { memset(out, 0, row); return; }
     DevGuard g(cv.device);
     cudaStream_t st = cv.st;
-    DevBuf v(PV_BYTES);
+    DevArena mem(st);
+    uint8_t* V = mem.alloc(PV_BYTES);
     MsmHold h(g2 != 0, n, st);
     Staging sg(std::min<size_t>(n, POWERS_SLICE) * row, st);
-    fe* d_rho = (fe*)(v.p + PV_RHO);
-    CUDA_CHECK(cudaMemcpyAsync(v.p + PV_CH, rho, 32, cudaMemcpyHostToDevice, st));
-    powers_rho_kernel<<<1, 1, 0, st>>>((const fe*)(v.p + PV_CH), d_rho);
-    g_launch_count += 1;
+    fe* d_rho = (fe*)(V + PV_RHO);
+    CUDA_CHECK(cudaMemcpyAsync(V + PV_CH, rho, 32, cudaMemcpyHostToDevice, st));
+    to_mont((const fe*)(V + PV_CH), 1, d_rho, st);
     powers_pass(sg, &h.m, g2 != 0, bases, n, false, nullptr, d_rho);
-    if (g2) powers_affine_kernel<G2, Fq2><<<1, 1, 0, st>>>(h.m.acc, v.p + PV_POINT);
-    else powers_affine_kernel<G1, Fq><<<1, 1, 0, st>>>(h.m.acc, v.p + PV_POINT);
+    if (g2) powers_affine_kernel<G2, Fq2><<<1, 1, 0, st>>>(h.m.acc, V + PV_POINT);
+    else powers_affine_kernel<G1, Fq><<<1, 1, 0, st>>>(h.m.acc, V + PV_POINT);
     g_launch_count += 1;
     CUDA_CHECK(cudaGetLastError());
-    CUDA_CHECK(cudaMemcpyAsync(out, v.p + PV_POINT, row, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaMemcpyAsync(out, V + PV_POINT, row, cudaMemcpyDeviceToHost, st));
     CUDA_CHECK(cudaStreamSynchronize(st));
 }
 
 static void powers_check_run(b2g_ctx* ctx, const b2g_powers_desc* pw, uint32_t log_n, const void* challenges, b2g_powers_report* out) {
     if (!ctx || !pw || !challenges || !out) throw_error(B2G_E_SHAPE, "null pointer");
     memset(out, 0, sizeof(*out));
-    const CtxView cv = ctx_view(ctx);
-    if (cv.proof_pending) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
+    const CtxView cv = ctx_idle(ctx);
     if (pw->log_size > 28) throw_error(B2G_E_DOMAIN, "b2g_powers_check: log_size " + std::to_string(pw->log_size) + " exceeds 28");
     if (log_n < 1 || log_n > pw->log_size)
         throw_error(B2G_E_DOMAIN, "b2g_powers_check: log_n " + std::to_string(log_n) + " is outside 1.." + std::to_string(pw->log_size));
-    if (!pw->tau_g1 || !pw->tau_g2 || !pw->alpha_tau_g1 || !pw->beta_tau_g1 || !pw->beta_g2) throw_error(B2G_E_SHAPE, "null powers array");
+    powers_arrays(pw, true);
     static const char* const CH_NAMES[5] = {"rho", "sigma", "pi", "kappa", "eps"};
     for (int k = 0; k < 5; k++)
         if (!scalar_ok((const uint8_t*)challenges + 32 * k)) throw_error(B2G_E_INPUT, std::string("challenge ") + CH_NAMES[k] + " is 0 or >= r");
     const uint64_t n = 1ull << log_n;
     DevGuard g(cv.device);
     cudaStream_t st = cv.st;
-    DevBuf v(PV_BYTES);
+    DevArena mem(st);
+    uint8_t* V = mem.alloc(PV_BYTES);
     MsmHold h1(false, 2 * n - 1, st), h2(true, n, st);
     Staging sg(std::max<size_t>(std::min<uint64_t>(2 * n - 1, POWERS_SLICE) * 64, std::min<uint64_t>(n, POWERS_SLICE) * 128), st);
-    uint8_t* V = v.p;
     const fe* d_rho = (const fe*)(V + PV_RHO);
     unsigned long long* d_bad = (unsigned long long*)(V + PV_BAD);
     const uint8_t *T = (const uint8_t*)pw->tau_g1, *U = (const uint8_t*)pw->tau_g2, *A = (const uint8_t*)pw->alpha_tau_g1,
@@ -147,9 +140,7 @@ static void powers_check_run(b2g_ctx* ctx, const b2g_powers_desc* pw, uint32_t l
     for (int k = 0; k < 7; k++) CUDA_CHECK(cudaMemcpyAsync(V + PV_G1 + 64 * k, g1_pts[k].first + 64 * g1_pts[k].second, 64, cudaMemcpyHostToDevice, st));
     const std::pair<const uint8_t*, uint64_t> g2_pts[4] = {{U, 0}, {U, 1}, {U, n - 1}, {(const uint8_t*)pw->beta_g2, 0}};
     for (int k = 0; k < 4; k++) CUDA_CHECK(cudaMemcpyAsync(V + PV_G2 + 128 * k, g2_pts[k].first + 128 * g2_pts[k].second, 128, cudaMemcpyHostToDevice, st));
-    powers_rho_kernel<<<1, 1, 0, st>>>((const fe*)(V + PV_CH), (fe*)(V + PV_RHO));
-    g_launch_count += 1;
-    CUDA_CHECK(cudaGetLastError());
+    to_mont((const fe*)(V + PV_CH), 1, (fe*)(V + PV_RHO), st);
 
     struct Array { const uint8_t* host; uint64_t count; bool g2, gen; PowersMsm* msm; size_t sum; };
     const Array arrays[5] = {{T, 2 * n - 1, false, true, &h1.m, 0}, {U, n, true, true, &h2.m, 384}, {A, n, false, false, &h1.m, 128},
@@ -163,10 +154,7 @@ static void powers_check_run(b2g_ctx* ctx, const b2g_powers_desc* pw, uint32_t l
         CUDA_CHECK(cudaStreamSynchronize(st));
         if (bad >= x.count) continue;
         // the first failing point of the first array with one: the first rule it breaks
-        const size_t row = x.g2 ? 128 : 64;
-        CUDA_CHECK(cudaMemcpyAsync(V + PV_POINT, x.host + bad * row, row, cudaMemcpyHostToDevice, st));
-        const uint32_t rule = powers_point_rule(x.g2, V + PV_POINT, x.gen && bad == 0, (uint32_t*)(V + PV_WORD), st);
-        if (!rule) throw_error(B2G_E_DEVICE, "b2g_powers_check: the point rules disagree on point " + std::to_string(bad));
+        const uint32_t rule = bad_point_rule("b2g_powers_check", x.host, bad, x.g2, x.gen, V + PV_POINT, (uint32_t*)(V + PV_WORD), st);
         out->ok = 0; out->rule = (uint8_t)rule; out->array = (uint8_t)a; out->index = bad;
         return;
     }
@@ -188,27 +176,15 @@ __global__ void check_consts_kernel(const fe* __restrict__ canon, fe* __restrict
     mont[2] = Fr::inv(Fr::from_canonical(two));
 }
 
-// prod[k] = val[k] w[col[k]] (canonical) and row[k] = the row of nonzero k, by binary search in rowptr
+// prod[k] = val[k] w[col[k]] (canonical) and row[k] = the row of nonzero k
 __global__ void __launch_bounds__(256) check_products_kernel(uint32_t nnz, uint32_t m, const uint32_t* __restrict__ rowptr,
                                                              const uint32_t* __restrict__ col, const fe* __restrict__ val,
                                                              const fe* __restrict__ w, fe* __restrict__ prod, uint32_t* __restrict__ row) {
     const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= nnz) return;
-    uint32_t lo = 0, hi = m - 1;                         // the last row r with rowptr[r] <= k (rowptr[m] = nnz > k)
-    while (lo < hi) {
-        const uint32_t mid = lo + (hi - lo + 1) / 2;
-        if (rowptr[mid] <= k) lo = mid; else hi = mid - 1;
-    }
+    const uint32_t r = mat_row(rowptr, m, k);
     fe_store(&prod[k], Fr::mul(fe_load_nc(&val[k]), fe_load_nc(&w[col[k]])));
-    row[k] = lo;
-}
-
-// c[rows[i]] = agg[i] for the *runs rows that occur
-__global__ void __launch_bounds__(256) check_scatter_kernel(uint32_t nnz, const uint32_t* __restrict__ runs, const uint32_t* __restrict__ rows,
-                                                            const fe* __restrict__ agg, fe* __restrict__ c) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= nnz || i >= *runs) return;
-    fe_store(&c[rows[i]], fe_load(&agg[i]));
+    row[k] = r;
 }
 
 // the public-input rows of A': c[m + j] = w[j], j < ni
@@ -236,17 +212,8 @@ __global__ void __launch_bounds__(256) check_h_kernel(uint32_t n, int libsnark, 
     if (k + 1 < n) fe_store(&h[n + k], hi);
 }
 
-struct FrSum {
-    __device__ __forceinline__ fe operator()(const fe& a, const fe& b) const { return Fr::add(a, b); }
-};
-
 static const char* const KEY_NAMES[12] = {"alpha_g1", "beta_g1", "delta_g1", "beta_g2", "gamma_g2", "delta_g2", "gamma_abc_g1", "a_query",
                                           "b_g1_query", "b_g2_query", "l_query", "h_query"};
-
-static bool all_zero_bytes(const void* p, size_t n) {
-    const uint8_t* b = (const uint8_t*)p;
-    return std::all_of(b, b + n, [](uint8_t x) { return x == 0; });
-}
 
 // the small device buffer of a key check: its layout
 enum : size_t {
@@ -267,15 +234,11 @@ static void setup_check_run(b2g_ctx* ctx, const b2g_mat_desc* d, const b2g_power
                             b2g_setup_report* out) {
     if (!ctx || !d || !pw || !key || !challenges || !out) throw_error(B2G_E_SHAPE, "null pointer");
     memset(out, 0, sizeof(*out));
-    const CtxView cv = ctx_view(ctx);
-    if (cv.proof_pending) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
-    const int logn = mat_desc_check(d, true);
+    const CtxView cv = ctx_idle(ctx);
+    const int logn = setup_domain(d);
     const bool libsnark = d->reduction == B2G_REDUCTION_LIBSNARK;
-    if (!libsnark && logn > 26) throw_error(B2G_E_DOMAIN, "PolynomialDegreeTooLarge: a CircomReduction setup transforms over 2n points, so n must fit 2^26");
-    if (pw->log_size > 28 || logn > (int)pw->log_size)
-        throw_error(B2G_E_DOMAIN, "PolynomialDegreeTooLarge: the circuit's domain of 2^" + std::to_string(logn) +
-                                      " points exceeds the ceremony's 2^" + std::to_string(pw->log_size) + " powers");
-    if (!pw->tau_g1 || !pw->tau_g2 || !pw->alpha_tau_g1 || !pw->beta_tau_g1 || !pw->beta_g2) throw_error(B2G_E_SHAPE, "null powers array");
+    powers_cover(pw, logn);
+    powers_arrays(pw, true);
     static const char* const CH_NAMES[2] = {"rho", "sigma"};
     for (int k = 0; k < 2; k++)
         if (!scalar_ok((const uint8_t*)challenges + 32 * k)) throw_error(B2G_E_INPUT, std::string("challenge ") + CH_NAMES[k] + " is 0 or >= r");
@@ -285,8 +248,7 @@ static void setup_check_run(b2g_ctx* ctx, const b2g_mat_desc* d, const b2g_power
     for (int f = 0; f < 12; f++)
         if (counts[f] && !fields[f]) throw_error(B2G_E_SHAPE, std::string("null key field ") + KEY_NAMES[f]);
     const uint32_t m = d->num_constraints, ni = d->num_inputs, nv = d->n_vars;
-    const uint32_t maxnnz = std::max(d->a_rowptr[m], std::max(d->b_rowptr[m], d->c_rowptr[m]));
-    if (maxnnz > (uint32_t)INT32_MAX) throw_error(B2G_E_DEVICE, "b2g_setup_check: more than 2^31 - 1 nonzeros in one matrix");
+    const uint32_t maxnnz = max_nnz(d, "b2g_setup_check");
     const uint32_t n = 1u << logn, nh = libsnark ? n - 1 : n;
     out->ok = 0;
 
@@ -302,11 +264,11 @@ static void setup_check_run(b2g_ctx* ctx, const b2g_mat_desc* d, const b2g_power
 
     DevGuard g(cv.device);
     cudaStream_t st = cv.st;
-    DevBuf v(SK_BYTES);
-    uint8_t* V = v.p;
+    DevArena mem(st);
+    uint8_t* V = mem.alloc(SK_BYTES);
     // the scalars: w (N), v then t (n), s^A, s^B, s^C (n each), h (2n; also the transforms' scratch before it holds h)
-    DevBuf sc(((size_t)nv + 6 * (size_t)n) * sizeof(fe));
-    fe *d_w = (fe*)sc.p, *d_v = d_w + nv, *d_s[3] = {d_v + n, d_v + 2 * (size_t)n, d_v + 3 * (size_t)n}, *d_h = d_v + 4 * (size_t)n;
+    fe* d_w = mem.alloc<fe>(((size_t)nv + 6 * (size_t)n) * sizeof(fe));
+    fe *d_v = d_w + nv, *d_s[3] = {d_v + n, d_v + 2 * (size_t)n, d_v + 3 * (size_t)n}, *d_h = d_v + 4 * (size_t)n;
     fe* d_mont = (fe*)(V + SK_MONT);
     unsigned long long* d_bad = (unsigned long long*)(V + SK_BAD);
     CUDA_CHECK(cudaMemsetAsync(V, 0, SK_BYTES, st));
@@ -321,42 +283,31 @@ static void setup_check_run(b2g_ctx* ctx, const b2g_mat_desc* d, const b2g_power
     // c = A'w, Bw, Cw by rows
     CUDA_CHECK(cudaMemsetAsync(d_s[0], 0, 3 * (size_t)n * sizeof(fe), st));
     if (maxnnz) {
-        DevBuf rowptr(((size_t)m + 1) * 4), col((size_t)maxnnz * 4), val((size_t)maxnnz * sizeof(fe)), rows((size_t)maxnnz * 4),
-            uniq((size_t)maxnnz * 4), prod((size_t)maxnnz * sizeof(fe)), agg((size_t)maxnnz * sizeof(fe));
+        DevArena mat(st);                                              // freed at the end of this block
+        uint32_t *rowptr = mat.alloc<uint32_t>(((size_t)m + 1) * 4), *col = mat.alloc<uint32_t>((size_t)maxnnz * 4);
+        fe* val = mat.alloc<fe>((size_t)maxnnz * sizeof(fe));
+        uint32_t *rows = mat.alloc<uint32_t>((size_t)maxnnz * 4), *uniq = mat.alloc<uint32_t>((size_t)maxnnz * 4);
+        fe *prod = mat.alloc<fe>((size_t)maxnnz * sizeof(fe)), *agg = mat.alloc<fe>((size_t)maxnnz * sizeof(fe));
         uint32_t* d_runs = (uint32_t*)(V + SK_RUNS);
         size_t temp_bytes = 0;
-        CUDA_CHECK(cub::DeviceReduce::ReduceByKey(nullptr, temp_bytes, (uint32_t*)rows.p, (uint32_t*)uniq.p, (fe*)prod.p, (fe*)agg.p,
-                                                  d_runs, FrSum(), (int)maxnnz, st));
-        DevBuf temp(temp_bytes);
-        const uint32_t* rowptrs[3] = {d->a_rowptr, d->b_rowptr, d->c_rowptr};
-        const uint32_t* cols[3] = {d->a_col, d->b_col, d->c_col};
-        const void* vals[3] = {d->a_val, d->b_val, d->c_val};
+        sum_by_key(nullptr, temp_bytes, rows, uniq, prod, agg, d_runs, maxnnz, nullptr, st);
+        void* temp = mat.alloc<void>(temp_bytes);
         for (int x = 0; x < 3; x++) {
-            const uint32_t nnz = rowptrs[x][m];
+            const uint32_t nnz = mat_nnz(d, x);
             if (!nnz) continue;
-            const unsigned blocks = (nnz + 255) / 256;
-            CUDA_CHECK(cudaMemcpyAsync(rowptr.p, rowptrs[x], ((size_t)m + 1) * 4, cudaMemcpyHostToDevice, st));
-            CUDA_CHECK(cudaMemcpyAsync(col.p, cols[x], (size_t)nnz * 4, cudaMemcpyHostToDevice, st));
-            CUDA_CHECK(cudaMemcpyAsync(val.p, vals[x], (size_t)nnz * sizeof(fe), cudaMemcpyHostToDevice, st));
-            check_products_kernel<<<blocks, 256, 0, st>>>(nnz, m, (const uint32_t*)rowptr.p, (const uint32_t*)col.p, (const fe*)val.p, d_w,
-                                                          (fe*)prod.p, (uint32_t*)rows.p);
+            mat_upload(d, x, rowptr, col, val, st);
+            check_products_kernel<<<(nnz + 255) / 256, 256, 0, st>>>(nnz, m, rowptr, col, val, d_w, prod, rows);
+            g_launch_count += 1;
             size_t bytes = temp_bytes;
-            CUDA_CHECK(cub::DeviceReduce::ReduceByKey(temp.p, bytes, (uint32_t*)rows.p, (uint32_t*)uniq.p, (fe*)prod.p, (fe*)agg.p, d_runs,
-                                                      FrSum(), (int)nnz, st));
-            check_scatter_kernel<<<blocks, 256, 0, st>>>(nnz, d_runs, (const uint32_t*)uniq.p, (const fe*)agg.p, d_s[x]);
-            g_launch_count += 2;
-            CUDA_CHECK(cudaGetLastError());
+            sum_by_key(temp, bytes, rows, uniq, prod, agg, d_runs, nnz, d_s[x], st);
         }
-        CUDA_CHECK(cudaStreamSynchronize(st));                         // the buffers of this block are freed at its end
     }
     check_public_rows_kernel<<<(ni + 255) / 256, 256, 0, st>>>(ni, m, d_w, d_s[0]);
     g_launch_count += 1;
     CUDA_CHECK(cudaGetLastError());
 
     // s = iNTT_n(c), in place; then h
-    NttDomain dom;
-    struct DomGuard { NttDomain& d; ~DomGuard() { ntt_domain_destroy(d); } } dg{dom};
-    ntt_domain_create(dom, logn, st);
+    NttDomainHold dom(logn, st);
     for (int x = 0; x < 3; x++) ntt_plain(dom, d_s[x], d_h, true, st);
     if (!libsnark) ntt_plain(dom, d_v, d_h, true, st);
     check_h_kernel<<<(n + 255) / 256, 256, 0, st>>>(n, libsnark ? 1 : 0, d_v, dom.tw, d_mont + 2, d_h);
@@ -391,17 +342,14 @@ static void setup_check_run(b2g_ctx* ctx, const b2g_mat_desc* d, const b2g_power
     CUDA_CHECK(cudaMemcpyAsync(bad, d_bad, sizeof(bad), cudaMemcpyDeviceToHost, st));
     CUDA_CHECK(cudaStreamSynchronize(st));
     // the points that must not be at infinity: tau_g1[0], tau_g2[0], delta_g1, delta_g2
-    if (all_zero_bytes(T, 64)) bad[0] = 0;
-    if (all_zero_bytes(pw->tau_g2, 128)) bad[1] = 0;
-    if (all_zero_bytes(key->delta_g1, 64)) bad[7] = 0;
-    if (all_zero_bytes(key->delta_g2, 128)) bad[10] = 0;
+    if (all_zero(T, 64)) bad[0] = 0;
+    if (all_zero(pw->tau_g2, 128)) bad[1] = 0;
+    if (all_zero(key->delta_g1, 64)) bad[7] = 0;
+    if (all_zero(key->delta_g2, 128)) bad[10] = 0;
     // the first failing point in pass order, which is report order: the ceremony's arrays, then the key's fields
     for (const Pass& p : passes) {
         if (p.bad < 0 || bad[p.bad] >= p.count) continue;
-        const size_t row = p.g2 ? 128 : 64;
-        CUDA_CHECK(cudaMemcpyAsync(V + SK_POINT, (const uint8_t*)p.host + bad[p.bad] * row, row, cudaMemcpyHostToDevice, st));
-        const uint32_t rule = powers_point_rule(p.g2, V + SK_POINT, false, (uint32_t*)(V + SK_WORD), st);
-        if (!rule) throw_error(B2G_E_DEVICE, "b2g_setup_check: the point rules disagree on point " + std::to_string(bad[p.bad]));
+        const uint32_t rule = bad_point_rule("b2g_setup_check", p.host, bad[p.bad], p.g2, false, V + SK_POINT, (uint32_t*)(V + SK_WORD), st);
         out->rule = (uint8_t)rule; out->side = p.bad < 5 ? 1 : 0; out->field = (uint8_t)(p.bad < 5 ? p.bad : p.bad - 5);
         out->index = bad[p.bad];
         return;
@@ -442,15 +390,14 @@ static void lagrange_check_run(b2g_ctx* ctx, const b2g_powers_desc* pw, const b2
                                b2g_powers_report* out) {
     if (!ctx || !pw || !lg || !rho || !out) throw_error(B2G_E_SHAPE, "null pointer");
     memset(out, 0, sizeof(*out));
-    const CtxView cv = ctx_view(ctx);
-    if (cv.proof_pending) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
+    const CtxView cv = ctx_idle(ctx);
     const uint32_t p = lg->log_size;
     if (p > 26 || p > pw->log_size)
         throw_error(B2G_E_DOMAIN, "b2g_lagrange_check: Lagrange sections of power " + std::to_string(p) + " exceed 26 or the ceremony's power " +
                                       std::to_string(pw->log_size));
     if (log_n < 1 || log_n > p)
         throw_error(B2G_E_DOMAIN, "b2g_lagrange_check: log_n " + std::to_string(log_n) + " is outside 1.." + std::to_string(p));
-    if (!pw->tau_g1 || !pw->tau_g2 || !pw->alpha_tau_g1 || !pw->beta_tau_g1) throw_error(B2G_E_SHAPE, "null powers array");
+    powers_arrays(pw, false);
     if (!lg->tau_g1 || !lg->tau_g2 || !lg->alpha_tau_g1 || !lg->beta_tau_g1) throw_error(B2G_E_SHAPE, "null Lagrange array");
     if (!scalar_ok((const uint8_t*)rho)) throw_error(B2G_E_INPUT, "challenge rho is 0 or >= r");
     const uint64_t n = 1ull << log_n;
@@ -458,30 +405,26 @@ static void lagrange_check_run(b2g_ctx* ctx, const b2g_powers_desc* pw, const b2
     const uint64_t n12 = 4 * n - 1, n13 = 2 * n - 1, t12 = log_n == p ? 2 * n - 1 : 2 * n;
     DevGuard g(cv.device);
     cudaStream_t st = cv.st;
-    DevBuf v(LC_BYTES);
-    uint8_t* V = v.p;
+    DevArena mem(st);
+    uint8_t* V = mem.alloc(LC_BYTES);
     fe* d_rho = (fe*)(V + LC_RHO);
     unsigned long long* d_bad = (unsigned long long*)(V + LC_BAD);
     CUDA_CHECK(cudaMemsetAsync(V, 0, LC_BYTES, st));
     CUDA_CHECK(cudaMemsetAsync(d_bad, 0xff, 4 * 8, st));
     CUDA_CHECK(cudaMemcpyAsync(V + LC_CH, rho, 32, cudaMemcpyHostToDevice, st));
-    powers_rho_kernel<<<1, 1, 0, st>>>((const fe*)(V + LC_CH), d_rho);
-    g_launch_count += 1;
-    CUDA_CHECK(cudaGetLastError());
+    to_mont((const fe*)(V + LC_CH), 1, d_rho, st);
 
     // the weights w_g = rho^g (g < 4n - 1), then s = sum_k pad(iNTT_(2^k)(w of block k)): s13 over blocks 0 .. log_n, s12 the
     // same plus block log_n + 1
-    DevBuf sc((n12 + 4 * 2 * n) * sizeof(fe));                     // w, then s12, s13, t and the transforms' scratch
-    fe *d_w = (fe*)sc.p, *d_s12 = d_w + n12, *d_s13 = d_s12 + 2 * n, *d_t = d_s13 + 2 * n, *d_tmp = d_t + 2 * n;
+    fe* d_w = mem.alloc<fe>((n12 + 4 * 2 * n) * sizeof(fe));       // w, then s12, s13, t and the transforms' scratch
+    fe *d_s12 = d_w + n12, *d_s13 = d_s12 + 2 * n, *d_t = d_s13 + 2 * n, *d_tmp = d_t + 2 * n;
     powers_scalars(d_rho, 0, (uint32_t)n12, (fe*)(V + LC_PW), d_w, st);
     CUDA_CHECK(cudaMemsetAsync(d_s13, 0, 2 * n * sizeof(fe), st));
     for (uint32_t k = 0; k <= log_n + 1; k++) {
         const uint64_t m = 1ull << k;
         CUDA_CHECK(cudaMemcpyAsync(d_t, d_w + (m - 1), m * sizeof(fe), cudaMemcpyDeviceToDevice, st));
         if (k) {
-            NttDomain dom;
-            struct DomGuard { NttDomain& d; ~DomGuard() { ntt_domain_destroy(d); } } dg{dom};
-            ntt_domain_create(dom, (int)k, st);
+            NttDomainHold dom((int)k, st);
             ntt_plain(dom, d_t, d_tmp, true, st);
             CUDA_CHECK(cudaStreamSynchronize(st));                     // dom is freed at the end of this block
         }
@@ -522,10 +465,7 @@ static void lagrange_check_run(b2g_ctx* ctx, const b2g_powers_desc* pw, const b2
     for (int x = 0; x < 4; x++) {
         const Sec& c = secs[x];
         if (bad[x] >= c.count) continue;
-        const size_t row = c.g2 ? 128 : 64;
-        CUDA_CHECK(cudaMemcpyAsync(V + LC_POINT, (const uint8_t*)c.lag + bad[x] * row, row, cudaMemcpyHostToDevice, st));
-        const uint32_t rule = powers_point_rule(c.g2, V + LC_POINT, false, (uint32_t*)(V + LC_WORD), st);
-        if (!rule) throw_error(B2G_E_DEVICE, "b2g_lagrange_check: the point rules disagree on point " + std::to_string(bad[x]));
+        const uint32_t rule = bad_point_rule("b2g_lagrange_check", c.lag, bad[x], c.g2, false, V + LC_POINT, (uint32_t*)(V + LC_WORD), st);
         out->rule = (uint8_t)rule; out->array = (uint8_t)(5 + x); out->index = bad[x];
         return;
     }

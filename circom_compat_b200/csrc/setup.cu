@@ -35,6 +35,7 @@
 #include "fixed.cuh"
 #include "ntt.cuh"
 #include "setup.cuh"
+#include "stage.cuh"
 #include "util.cuh"
 #include "verify.cuh"
 
@@ -72,28 +73,22 @@ __global__ void __launch_bounds__(256) setup_iota_kernel(uint32_t n, uint32_t* _
     if (i < n) out[i] = i;
 }
 
-// prod[k] = val[p] * L[row of p] for the k-th nonzero in column order, p = perm[k]; the row is found by binary search in rowptr,
-// so a long row costs no thread more than log2(m) steps
+// prod[k] = val[p] * L[row of p] for the k-th nonzero in column order, p = perm[k]
 __global__ void __launch_bounds__(256) setup_products_kernel(uint32_t nnz, uint32_t m, const uint32_t* __restrict__ rowptr,
                                                              const fe* __restrict__ val, const fe* __restrict__ L,
                                                              const uint32_t* __restrict__ perm, fe* __restrict__ prod) {
     const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= nnz) return;
-    const uint32_t p = perm[k];
-    uint32_t lo = 0, hi = m - 1;                         // the last row r with rowptr[r] <= p (rowptr[m] = nnz > p)
-    while (lo < hi) {
-        const uint32_t mid = lo + (hi - lo + 1) / 2;
-        if (rowptr[mid] <= p) lo = mid; else hi = mid - 1;
-    }
-    fe_store(&prod[k], Fr::mul(fe_load_nc(&val[p]), fe_load_nc(&L[lo])));
+    const uint32_t p = perm[k], row = mat_row(rowptr, m, p);
+    fe_store(&prod[k], Fr::mul(fe_load_nc(&val[p]), fe_load_nc(&L[row])));
 }
 
-// sums[col[i]] = agg[i] for the *runs columns that occur
-__global__ void __launch_bounds__(256) setup_scatter_kernel(uint32_t nnz, const uint32_t* __restrict__ runs, const uint32_t* __restrict__ col,
-                                                            const fe* __restrict__ agg, fe* __restrict__ sums) {
+// out[keys[i]] = agg[i] for the *runs keys that occur
+__global__ void __launch_bounds__(256) scatter_sums_kernel(uint32_t n, const uint32_t* __restrict__ runs, const uint32_t* __restrict__ keys,
+                                                           const fe* __restrict__ agg, fe* __restrict__ out) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= nnz || i >= *runs) return;
-    fe_store(&sums[col[i]], fe_load(&agg[i]));
+    if (i >= n || i >= *runs) return;
+    fe_store(&out[keys[i]], fe_load(&agg[i]));
 }
 
 // a_j += L_(m+j) for j < num_inputs; k_j = (beta a_j + alpha b_j + c_j) / (gamma or delta); a, b, k canonical in place
@@ -123,39 +118,27 @@ struct FrAddOp {
     __device__ __forceinline__ fe operator()(const fe& a, const fe& b) const { return Fr::add(a, b); }
 };
 
-// every device buffer of one setup; each is zeroed on the stream before it is freed, on success and on error alike
-struct SetupMem {
-    cudaStream_t st;
-    std::vector<std::pair<void*, size_t>> bufs;
-    template <class T> T* alloc(size_t bytes) {
-        void* p = nullptr;
-        CUDA_CHECK(cudaMalloc(&p, bytes ? bytes : 1));
-        bufs.push_back({p, bytes ? bytes : 1});
-        return (T*)p;
-    }
-    ~SetupMem() {
-        for (auto& b : bufs) cudaMemsetAsync(b.first, 0, b.second, st);
-        cudaStreamSynchronize(st);
-        for (auto& b : bufs) cudaFree(b.first);
-    }
-};
-
-static void secure_zero(void* p, size_t n) {
-    volatile uint8_t* q = (volatile uint8_t*)p;
-    while (n--) *q++ = 0;
+void sum_by_key(void* temp, size_t& temp_bytes, const uint32_t* keys, uint32_t* uniq, const fe* prod, fe* agg, uint32_t* runs,
+                uint32_t n, fe* out, cudaStream_t st) {
+    CUDA_CHECK(cub::DeviceReduce::ReduceByKey(temp, temp_bytes, keys, uniq, prod, agg, runs, FrAddOp(), (int)n, st));
+    if (!temp) return;
+    scatter_sums_kernel<<<(n + 255) / 256, 256, 0, st>>>(n, runs, uniq, agg, out);
+    g_launch_count += 1;
+    CUDA_CHECK(cudaGetLastError());
 }
 
-// little-endian 256-bit a < m (m as 8 words)
-static bool below(const uint8_t* a, const uint32_t* m) {
-    for (int i = 7; i >= 0; i--) {
-        uint32_t w; memcpy(&w, a + 4 * i, 4);
-        if (w != m[i]) return w < m[i];
+// the nonzeros of one matrix in column order: keys = the sorted columns (from col, which the sort consumes, under nv columns) and
+// perm = the nonzeros' indices in that order, through idx.  With temp null, only sets temp_bytes.
+static void sort_by_column(void* temp, size_t& temp_bytes, uint32_t* col, uint32_t* keys, uint32_t* idx, uint32_t* perm, uint32_t nnz,
+                           uint32_t nv, cudaStream_t st) {
+    int end_bit = 1;
+    while (end_bit < 32 && (1ull << end_bit) < nv) end_bit++;
+    if (temp) {
+        setup_iota_kernel<<<(nnz + 255) / 256, 256, 0, st>>>(nnz, idx);
+        g_launch_count += 1;
     }
-    return false;
+    CUDA_CHECK(cub::DeviceRadixSort::SortPairs(temp, temp_bytes, col, keys, idx, perm, (int)nnz, 0, end_bit, st));
 }
-static const uint32_t R_WORDS[8] = {FrParams::P0, FrParams::P1, FrParams::P2, FrParams::P3, FrParams::P4, FrParams::P5, FrParams::P6, FrParams::P7};
-static const uint32_t Q_WORDS[8] = {FqParams::P0, FqParams::P1, FqParams::P2, FqParams::P3, FqParams::P4, FqParams::P5, FqParams::P6, FqParams::P7};
-static bool all_zero32(const uint8_t* a) { for (int i = 0; i < 32; i++) if (a[i]) return false; return true; }
 
 constexpr size_t SETUP_SLICE = 1u << 20;                // points per fixed-base launch: bounds the output buffer to 128 MiB
 
@@ -174,34 +157,28 @@ static void setup_points(const void* table, const fe* scalars, size_t n, uint8_t
 
 static void setup_run(b2g_ctx* ctx, const b2g_mat_desc* d, const b2g_setup_secrets* sec, const b2g_setup_out* o) {
     if (!ctx || !d || !sec || !o) throw_error(B2G_E_SHAPE, "null pointer");
-    const CtxView cv = ctx_view(ctx);
-    if (cv.proof_pending) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
-    const int logn = mat_desc_check(d, true);
+    const CtxView cv = ctx_idle(ctx);
+    const int logn = setup_domain(d);
     const bool libsnark = d->reduction == B2G_REDUCTION_LIBSNARK;
-    if (!libsnark && logn > 26) throw_error(B2G_E_DOMAIN, "PolynomialDegreeTooLarge: a CircomReduction setup transforms over 2n points, so n must fit 2^26");
     const uint32_t m = d->num_constraints, ni = d->num_inputs, nv = d->n_vars;
     const size_t n = (size_t)1 << logn, nh = libsnark ? n - 1 : n;
     if (!sec->alpha || !sec->beta || !sec->gamma || !sec->delta || !sec->tau) throw_error(B2G_E_SHAPE, "null secret");
-    if (!o->alpha_g1 || !o->beta_g1 || !o->delta_g1 || !o->beta_g2 || !o->gamma_g2 || !o->delta_g2 || !o->gamma_abc_g1 || !o->a_query ||
-        !o->b_g1_query || !o->b_g2_query || (nv > ni && !o->l_query) || (nh && !o->h_query))
-        throw_error(B2G_E_SHAPE, "null output buffer");
+    setup_out_buffers(o, nv, ni, nh);
     const void* secs[5] = {sec->alpha, sec->beta, sec->gamma, sec->delta, sec->tau};
     static const char* names[5] = {"alpha", "beta", "gamma", "delta", "tau"};
     for (int i = 0; i < 5; i++)
         if (!below((const uint8_t*)secs[i], R_WORDS)) throw_error(B2G_E_INPUT, std::string("secret ") + names[i] + " is not below r");
-    if (all_zero32((const uint8_t*)sec->gamma)) throw_error(B2G_E_INPUT, "gamma is zero");
-    if (all_zero32((const uint8_t*)sec->delta)) throw_error(B2G_E_INPUT, "delta is zero");
+    if (all_zero(sec->gamma, 32)) throw_error(B2G_E_INPUT, "gamma is zero");
+    if (all_zero(sec->delta, 32)) throw_error(B2G_E_INPUT, "delta is zero");
     for (int i = 0; i < 2; i++)
-        if (sec->g1 && !below((const uint8_t*)sec->g1 + 32 * i, Q_WORDS)) throw_error(B2G_E_INPUT, "g1: coordinate not below p");
+        if (sec->g1 && !below((const uint8_t*)sec->g1 + 32 * i, P_WORDS)) throw_error(B2G_E_INPUT, "g1: coordinate not below p");
     for (int i = 0; i < 4; i++)
-        if (sec->g2 && !below((const uint8_t*)sec->g2 + 32 * i, Q_WORDS)) throw_error(B2G_E_INPUT, "g2: coordinate not below p");
-    const uint32_t annz = d->a_rowptr[m], bnnz = d->b_rowptr[m], cnnz = d->c_rowptr[m];
-    const uint32_t maxnnz = std::max(annz, std::max(bnnz, cnnz));
-    if (maxnnz > (uint32_t)INT32_MAX) throw_error(B2G_E_DEVICE, "b2g_setup: more than 2^31 - 1 nonzeros in one matrix");
+        if (sec->g2 && !below((const uint8_t*)sec->g2 + 32 * i, P_WORDS)) throw_error(B2G_E_INPUT, "g2: coordinate not below p");
+    const uint32_t maxnnz = max_nnz(d, "b2g_setup");
 
     DevGuard g(cv.device);
     cudaStream_t st = cv.st;
-    SetupMem mem{st, {}};
+    DevArena mem(st, true);
     // generators first: a bad one is refused before anything secret reaches the device
     uint8_t* d_gen = mem.alloc<uint8_t>(64 + 128);
     if (sec->g1) CUDA_CHECK(cudaMemcpyAsync(d_gen, sec->g1, 64, cudaMemcpyHostToDevice, st));
@@ -214,15 +191,7 @@ static void setup_run(b2g_ctx* ctx, const b2g_mat_desc* d, const b2g_setup_secre
     }
 
     fe* d_k = mem.alloc<fe>(K_COUNT * sizeof(fe));
-    {
-        uint8_t h_in[5 * 32];
-        for (int i = 0; i < 5; i++) memcpy(h_in + 32 * i, secs[i], 32);
-        // on the setup's stream, which is not ordered with the legacy default stream; h_in is wiped once the copy is done
-        cudaError_t e = cudaMemcpyAsync(d_k, h_in, sizeof(h_in), cudaMemcpyHostToDevice, st);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-        secure_zero(h_in, sizeof(h_in));
-        CUDA_CHECK(e);
-    }
+    upload_secrets(d_k, secs, 5, st);
     setup_consts_kernel<<<1, 1, 0, st>>>(d_k, logn, libsnark ? 1 : 0);
     g_launch_count += 1;
     CUDA_CHECK(cudaGetLastError());
@@ -231,9 +200,7 @@ static void setup_run(b2g_ctx* ctx, const b2g_mat_desc* d, const b2g_setup_secre
     const size_t ntmp = libsnark ? n : 2 * n;
     fe* d_L = mem.alloc<fe>(n * sizeof(fe));
     fe* d_tmp = mem.alloc<fe>(ntmp * sizeof(fe));
-    NttDomain dom;
-    struct DomGuard { NttDomain& d; ~DomGuard() { ntt_domain_destroy(d); } } dg{dom};
-    ntt_domain_create(dom, logn, st);
+    NttDomainHold dom(logn, st);
     ntt_powers(logn, d_k + K_PW, d_k + K_ONE, d_L, st);
     ntt_plain(dom, d_L, d_tmp, true, st);
 
@@ -244,8 +211,6 @@ static void setup_run(b2g_ctx* ctx, const b2g_mat_desc* d, const b2g_setup_secre
         CUDA_CHECK(cudaMemsetAsync(d_sum[x], 0, (size_t)nv * sizeof(fe), st));
     }
     if (maxnnz) {
-        int end_bit = 1;
-        while (end_bit < 32 && (1ull << end_bit) < nv) end_bit++;
         uint32_t* d_rowptr = mem.alloc<uint32_t>(((size_t)m + 1) * 4);
         uint32_t* d_col = mem.alloc<uint32_t>((size_t)maxnnz * 4);
         fe* d_val = mem.alloc<fe>((size_t)maxnnz * sizeof(fe));
@@ -256,31 +221,21 @@ static void setup_run(b2g_ctx* ctx, const b2g_mat_desc* d, const b2g_setup_secre
         fe* d_agg = mem.alloc<fe>((size_t)maxnnz * sizeof(fe));
         uint32_t* d_runs = mem.alloc<uint32_t>(4);
         size_t sort_bytes = 0, reduce_bytes = 0;
-        CUDA_CHECK(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, d_col, d_keys, d_idx, d_perm, (int)maxnnz, 0, end_bit, st));
-        CUDA_CHECK(cub::DeviceReduce::ReduceByKey(nullptr, reduce_bytes, d_keys, d_col, d_prod, d_agg, d_runs, FrAddOp(), (int)maxnnz, st));
+        sort_by_column(nullptr, sort_bytes, d_col, d_keys, d_idx, d_perm, maxnnz, nv, st);
+        sum_by_key(nullptr, reduce_bytes, d_keys, d_col, d_prod, d_agg, d_runs, maxnnz, nullptr, st);
         const size_t temp_bytes = std::max(sort_bytes, reduce_bytes);
         void* d_temp = mem.alloc<void>(temp_bytes);
-        const uint32_t* rowptrs[3] = {d->a_rowptr, d->b_rowptr, d->c_rowptr};
-        const uint32_t* cols[3] = {d->a_col, d->b_col, d->c_col};
-        const void* vals[3] = {d->a_val, d->b_val, d->c_val};
-        const uint32_t nnzs[3] = {annz, bnnz, cnnz};
         for (int x = 0; x < 3; x++) {
-            const uint32_t nnz = nnzs[x];
+            const uint32_t nnz = mat_nnz(d, x);
             if (!nnz) continue;
-            const unsigned blocks = (nnz + 255) / 256;
-            CUDA_CHECK(cudaMemcpyAsync(d_rowptr, rowptrs[x], ((size_t)m + 1) * 4, cudaMemcpyHostToDevice, st));
-            CUDA_CHECK(cudaMemcpyAsync(d_col, cols[x], (size_t)nnz * 4, cudaMemcpyHostToDevice, st));
-            CUDA_CHECK(cudaMemcpyAsync(d_val, vals[x], (size_t)nnz * sizeof(fe), cudaMemcpyHostToDevice, st));
-            setup_iota_kernel<<<blocks, 256, 0, st>>>(nnz, d_idx);
+            mat_upload(d, x, d_rowptr, d_col, d_val, st);
             size_t bytes = temp_bytes;
-            CUDA_CHECK(cub::DeviceRadixSort::SortPairs(d_temp, bytes, d_col, d_keys, d_idx, d_perm, (int)nnz, 0, end_bit, st));
-            setup_products_kernel<<<blocks, 256, 0, st>>>(nnz, m, d_rowptr, d_val, d_L, d_perm, d_prod);
+            sort_by_column(d_temp, bytes, d_col, d_keys, d_idx, d_perm, nnz, nv, st);
+            setup_products_kernel<<<(nnz + 255) / 256, 256, 0, st>>>(nnz, m, d_rowptr, d_val, d_L, d_perm, d_prod);
+            g_launch_count += 1;
             bytes = temp_bytes;
             // the unique columns overwrite d_col: the sort has consumed it
-            CUDA_CHECK(cub::DeviceReduce::ReduceByKey(d_temp, bytes, d_keys, d_col, d_prod, d_agg, d_runs, FrAddOp(), (int)nnz, st));
-            setup_scatter_kernel<<<blocks, 256, 0, st>>>(nnz, d_runs, d_col, d_agg, d_sum[x]);
-            g_launch_count += 3;
-            CUDA_CHECK(cudaGetLastError());
+            sum_by_key(d_temp, bytes, d_keys, d_col, d_prod, d_agg, d_runs, nnz, d_sum[x], st);
         }
     }
     setup_combine_kernel<<<(nv + 255) / 256, 256, 0, st>>>(nv, ni, m, d_k, d_L, d_sum[0], d_sum[1], d_sum[2]);
@@ -293,9 +248,7 @@ static void setup_run(b2g_ctx* ctx, const b2g_mat_desc* d, const b2g_setup_secre
         ntt_powers(logn, d_k + K_PW, d_k + K_HSCALE, d_tmp, st);
         setup_canonical_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>((uint32_t)n, 1, 0, d_tmp, d_h);
     } else {
-        NttDomain dom2;
-        struct Dom2Guard { NttDomain& d; ~Dom2Guard() { ntt_domain_destroy(d); } } dg2{dom2};
-        ntt_domain_create(dom2, logn + 1, st);
+        NttDomainHold dom2(logn + 1, st);
         fe* d_hv = mem.alloc<fe>(2 * n * sizeof(fe));
         ntt_powers(logn + 1, d_k + K_PW, d_k + K_HSCALE, d_hv, st);
         CUDA_CHECK(cudaMemsetAsync(d_hv + 2 * n - 1, 0, sizeof(fe), st));          // 2n - 1 powers, padded with one zero
@@ -475,14 +428,9 @@ __global__ void __launch_bounds__(128) colsum_products_kernel(uint32_t pieces, u
     const uint32_t start = colptr[j] + (q - ptr[j]) * PIECE_PRODUCTS, end = min(start + PIECE_PRODUCTS, colptr[j + 1]);
     typename C::Pt acc = C::infinity();
     for (uint32_t k = start; k < end; k++) {
-        const uint32_t p = perm[k];
-        uint32_t lo = 0, hi = m - 1;                     // the last row r with rowptr[r] <= p
-        while (lo < hi) {
-            const uint32_t mid = lo + (hi - lo + 1) / 2;
-            if (rowptr[mid] <= p) lo = mid; else hi = mid - 1;
-        }
+        const uint32_t p = perm[k], row = mat_row(rowptr, m, p);
         fe c = Fr::to_canonical(fe_load_nc(&val[p]));
-        typename C::Aff b = aff_load<F>(base, lo);
+        typename C::Aff b = aff_load<F>(base, row);
         const fe nc = Fr::neg(c);
         bool big = false;
         for (int w = 7; w >= 0; w--) if (c.l[w] != nc.l[w]) { big = c.l[w] > nc.l[w]; break; }
@@ -539,18 +487,12 @@ struct ColPlan {
     std::vector<uint32_t> pieces;
 };
 
-static ColPlan col_plan(SetupMem& mem, const b2g_mat_desc* d, int x, uint32_t nv, cudaStream_t st) {
+static ColPlan col_plan(DevArena& mem, const b2g_mat_desc* d, int x, uint32_t nv, cudaStream_t st) {
     const uint32_t m = d->num_constraints;
-    const uint32_t* rowptrs[3] = {d->a_rowptr, d->b_rowptr, d->c_rowptr};
-    const uint32_t* cols[3] = {d->a_col, d->b_col, d->c_col};
-    const void* vals[3] = {d->a_val, d->b_val, d->c_val};
     ColPlan cp;
-    cp.nnz = rowptrs[x][m];
+    cp.nnz = mat_nnz(d, x);
     if (!cp.nnz) return cp;
     const uint32_t nnz = cp.nnz;
-    const unsigned blocks = (nnz + 255) / 256;
-    int end_bit = 1;
-    while (end_bit < 32 && (1ull << end_bit) < nv) end_bit++;
     uint32_t* d_rowptr = mem.alloc<uint32_t>(((size_t)m + 1) * 4);
     uint32_t* d_col = mem.alloc<uint32_t>((size_t)nnz * 4);
     fe* d_val = mem.alloc<fe>((size_t)nnz * sizeof(fe));
@@ -559,15 +501,12 @@ static ColPlan col_plan(SetupMem& mem, const b2g_mat_desc* d, int x, uint32_t nv
     uint32_t* d_perm = mem.alloc<uint32_t>((size_t)nnz * 4);
     uint32_t* d_colptr = mem.alloc<uint32_t>(((size_t)nv + 1) * 4);
     size_t sort_bytes = 0;
-    CUDA_CHECK(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, d_col, d_keys, d_idx, d_perm, (int)nnz, 0, end_bit, st));
+    sort_by_column(nullptr, sort_bytes, d_col, d_keys, d_idx, d_perm, nnz, nv, st);
     void* d_temp = mem.alloc<void>(sort_bytes);
-    CUDA_CHECK(cudaMemcpyAsync(d_rowptr, rowptrs[x], ((size_t)m + 1) * 4, cudaMemcpyHostToDevice, st));
-    CUDA_CHECK(cudaMemcpyAsync(d_col, cols[x], (size_t)nnz * 4, cudaMemcpyHostToDevice, st));
-    CUDA_CHECK(cudaMemcpyAsync(d_val, vals[x], (size_t)nnz * sizeof(fe), cudaMemcpyHostToDevice, st));
-    setup_iota_kernel<<<blocks, 256, 0, st>>>(nnz, d_idx);
-    CUDA_CHECK(cub::DeviceRadixSort::SortPairs(d_temp, sort_bytes, d_col, d_keys, d_idx, d_perm, (int)nnz, 0, end_bit, st));
+    mat_upload(d, x, d_rowptr, d_col, d_val, st);
+    sort_by_column(d_temp, sort_bytes, d_col, d_keys, d_idx, d_perm, nnz, nv, st);
     colptr_kernel<<<(nv + 256) / 256, 256, 0, st>>>(nnz, nv, d_keys, d_colptr);
-    g_launch_count += 2;
+    g_launch_count += 1;
     CUDA_CHECK(cudaGetLastError());
     std::vector<uint32_t> cur(nv + 1);
     CUDA_CHECK(cudaMemcpyAsync(cur.data(), d_colptr, ((size_t)nv + 1) * 4, cudaMemcpyDeviceToHost, st));
@@ -623,7 +562,7 @@ static void check_upload(const char* name, uint64_t base, const void* host, size
 }
 
 // uploads n affine points into a new buffer of `mem`, refused as check_upload refuses them
-static uint8_t* powers_upload(SetupMem& mem, const char* name, const void* host, size_t n, bool g2, bool subgroup, cudaStream_t st,
+static uint8_t* powers_upload(DevArena& mem, const char* name, const void* host, size_t n, bool g2, bool subgroup, cudaStream_t st,
                               uint64_t base = 0) {
     uint8_t* d = mem.alloc<uint8_t>(n * (g2 ? 128 : 64));
     check_upload(name, base, host, n, g2, subgroup, d, st);
@@ -656,15 +595,11 @@ __global__ void __launch_bounds__(128) hq_lagrange_kernel(const void* __restrict
 static void setup_from_powers_run(b2g_ctx* ctx, const b2g_mat_desc* d, const b2g_powers_desc* pw, const b2g_setup_out* o,
                                   const b2g_lagrange_desc* lg = nullptr) {
     if (!ctx || !d || !pw || !o) throw_error(B2G_E_SHAPE, "null pointer");
-    const CtxView cv = ctx_view(ctx);
-    if (cv.proof_pending) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
-    const int logn = mat_desc_check(d, true);
+    const CtxView cv = ctx_idle(ctx);
+    const int logn = setup_domain(d);
     const bool libsnark = d->reduction == B2G_REDUCTION_LIBSNARK;
-    if (!libsnark && logn > 26) throw_error(B2G_E_DOMAIN, "PolynomialDegreeTooLarge: a CircomReduction setup transforms over 2n points, so n must fit 2^26");
-    if (pw->log_size > 28 || logn > (int)pw->log_size)
-        throw_error(B2G_E_DOMAIN, "PolynomialDegreeTooLarge: the circuit's domain of 2^" + std::to_string(logn) +
-                                      " points exceeds the ceremony's 2^" + std::to_string(pw->log_size) + " powers");
-    if (!pw->tau_g1 || !pw->tau_g2 || !pw->alpha_tau_g1 || !pw->beta_tau_g1 || !pw->beta_g2) throw_error(B2G_E_SHAPE, "null powers array");
+    powers_cover(pw, logn);
+    powers_arrays(pw, true);
     if (lg) {
         if (!lg->tau_g1 || !lg->tau_g2 || !lg->alpha_tau_g1 || !lg->beta_tau_g1) throw_error(B2G_E_SHAPE, "null Lagrange array");
         if (lg->log_size > 26 || lg->log_size > pw->log_size)
@@ -676,31 +611,21 @@ static void setup_from_powers_run(b2g_ctx* ctx, const b2g_mat_desc* d, const b2g
     }
     const uint32_t m = d->num_constraints, ni = d->num_inputs, nv = d->n_vars;
     const size_t n = (size_t)1 << logn, nh = libsnark ? n - 1 : n;
-    if (!o->alpha_g1 || !o->beta_g1 || !o->delta_g1 || !o->beta_g2 || !o->gamma_g2 || !o->delta_g2 || !o->gamma_abc_g1 || !o->a_query ||
-        !o->b_g1_query || !o->b_g2_query || (nv > ni && !o->l_query) || (nh && !o->h_query))
-        throw_error(B2G_E_SHAPE, "null output buffer");
-    const uint32_t maxnnz = std::max(d->a_rowptr[m], std::max(d->b_rowptr[m], d->c_rowptr[m]));
-    if (maxnnz > (uint32_t)INT32_MAX) throw_error(B2G_E_DEVICE, "b2g_setup_from_powers: more than 2^31 - 1 nonzeros in one matrix");
+    setup_out_buffers(o, nv, ni, nh);
+    max_nnz(d, "b2g_setup_from_powers");
 
     DevGuard g(cv.device);
     cudaStream_t st = cv.st;
-    SetupMem mem{st, {}};
+    DevArena mem(st, true);
     uint8_t* d_tau1 = powers_upload(mem, "tau_g1", pw->tau_g1, 2 * n - 1, false, false, st);
     uint8_t* d_tau2 = powers_upload(mem, "tau_g2", pw->tau_g2, n, true, true, st);
     uint8_t* d_atau = powers_upload(mem, "alpha_tau_g1", pw->alpha_tau_g1, n, false, false, st);
     uint8_t* d_btau = powers_upload(mem, "beta_tau_g1", pw->beta_tau_g1, n, false, false, st);
     powers_upload(mem, "beta_g2", pw->beta_g2, 1, true, true, st);
-    if (all_zero32((const uint8_t*)pw->tau_g1) && all_zero32((const uint8_t*)pw->tau_g1 + 32)) throw_error(B2G_E_INPUT, "tau_g1[0]: at infinity");
-    {
-        bool inf = true;
-        for (int i = 0; i < 4; i++) inf = inf && all_zero32((const uint8_t*)pw->tau_g2 + 32 * i);
-        if (inf) throw_error(B2G_E_INPUT, "tau_g2[0]: at infinity");
-    }
+    powers_first_finite(pw);
 
     // the Lagrange points: four transforms through one XYZZ work area
-    NttDomain dom;
-    struct DomGuard { NttDomain& d; ~DomGuard() { ntt_domain_destroy(d); } } dg{dom};
-    ntt_domain_create(dom, logn, st);
+    NttDomainHold dom(logn, st);
     fe* d_sc = mem.alloc<fe>(2 * sizeof(fe));
     pts_scale_kernel<<<1, 1, 0, st>>>(dom.ct, d_sc);                       // ct[0] = n^-1
     g_launch_count += 1;
@@ -739,7 +664,7 @@ static void setup_from_powers_run(b2g_ctx* ctx, const b2g_mat_desc* d, const b2g
                                              false, st, 2 * n - 1);
         uint8_t* d_corr = nullptr;
         const uint8_t* last = (const uint8_t*)pw->tau_g1 + (2 * n - 1) * 64;
-        if (logn < (int)lg->log_size && !(all_zero32(last) && all_zero32(last + 32))) {
+        if (logn < (int)lg->log_size && !all_zero(last, 64)) {
             const uint8_t* d_last = powers_upload(mem, "tau_g1", last, 1, false, false, st, 2 * n - 1);
             void* d_tab = mem.alloc<void>(32 * 255 * 64);
             fe* d_ks = mem.alloc<fe>(n * sizeof(fe));
@@ -801,19 +726,16 @@ static void setup_from_powers_run(b2g_ctx* ctx, const b2g_mat_desc* d, const b2g
 // b2g_points_intt: n = 2^logn affine points in place (host buffer)
 static void points_intt_run(b2g_ctx* ctx, int g2, int logn, void* pts) {
     if (!ctx || !pts) throw_error(B2G_E_SHAPE, "null pointer");
-    const CtxView cv = ctx_view(ctx);
-    if (cv.proof_pending) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
+    const CtxView cv = ctx_idle(ctx);
     if (logn < 1 || logn > 27) throw_error(B2G_E_DOMAIN, "b2g_points_intt: log_n must be in 1..27");
     const size_t n = (size_t)1 << logn, row = g2 ? 128 : 64;
     DevGuard g(cv.device);
     cudaStream_t st = cv.st;
-    SetupMem mem{st, {}};
+    DevArena mem(st, true);
     uint8_t* d_in = mem.alloc<uint8_t>(n * row);
     uint8_t* d_work = mem.alloc<uint8_t>(n * row * 2);
     fe* d_sc = mem.alloc<fe>(2 * sizeof(fe));
-    NttDomain dom;
-    struct DomGuard { NttDomain& d; ~DomGuard() { ntt_domain_destroy(d); } } dg{dom};
-    ntt_domain_create(dom, logn, st);
+    NttDomainHold dom(logn, st);
     pts_scale_kernel<<<1, 1, 0, st>>>(dom.ct, d_sc);
     g_launch_count += 2;
     CUDA_CHECK(cudaMemcpyAsync(d_in, pts, n * row, cudaMemcpyHostToDevice, st));
@@ -903,15 +825,8 @@ __global__ void inv_pow2_kernel(fe* __restrict__ sc) {
     for (int k = 0; k < 28; k++) { sc[k] = Fr::to_canonical(p); p = Fr::mul(p, half); }
 }
 
-struct PinnedBuf {
-    uint8_t* p = nullptr;
-    size_t bytes = 0;
-    explicit PinnedBuf(size_t b) : bytes(b) { CUDA_CHECK(cudaHostAlloc((void**)&p, b, cudaHostAllocDefault)); }
-    ~PinnedBuf() { if (p) cudaFreeHost(p); }
-};
-
 // host[0 .. bytes) = d[0 .. bytes) through the pinned buffer (host may be a memory-mapped file)
-static void to_host(PinnedBuf& pin, const uint8_t* d, size_t bytes, void* host, cudaStream_t st) {
+static void to_host(PinnedHost& pin, const uint8_t* d, size_t bytes, void* host, cudaStream_t st) {
     for (size_t off = 0; off < bytes; off += pin.bytes) {
         const size_t c = std::min(pin.bytes, bytes - off);
         CUDA_CHECK(cudaMemcpyAsync(pin.p, d + off, c, cudaMemcpyDeviceToHost, st));
@@ -922,24 +837,18 @@ static void to_host(PinnedBuf& pin, const uint8_t* d, size_t bytes, void* host, 
 
 static void powers_prepare_run(b2g_ctx* ctx, const b2g_powers_desc* pw, const b2g_lagrange_out* o) {
     if (!ctx || !pw || !o) throw_error(B2G_E_SHAPE, "null pointer");
-    const CtxView cv = ctx_view(ctx);
-    if (cv.proof_pending) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
+    const CtxView cv = ctx_idle(ctx);
     if (pw->log_size > 28) throw_error(B2G_E_DOMAIN, "b2g_powers_prepare: log_size " + std::to_string(pw->log_size) + " exceeds 28");
     const int K = (int)o->log_size;
     if (K < 1 || K > 26 || K > (int)pw->log_size)
         throw_error(B2G_E_DOMAIN, "b2g_powers_prepare: power " + std::to_string(K) + " is outside 1.." +
                                       std::to_string(std::min<uint32_t>(pw->log_size, 26)));
-    if (!pw->tau_g1 || !pw->tau_g2 || !pw->alpha_tau_g1 || !pw->beta_tau_g1) throw_error(B2G_E_SHAPE, "null powers array");
+    powers_arrays(pw, false);
     if (!o->tau_g1 || !o->tau_g2 || !o->alpha_tau_g1 || !o->beta_tau_g1) throw_error(B2G_E_SHAPE, "null output array");
-    if (all_zero32((const uint8_t*)pw->tau_g1) && all_zero32((const uint8_t*)pw->tau_g1 + 32)) throw_error(B2G_E_INPUT, "tau_g1[0]: at infinity");
-    {
-        bool inf = true;
-        for (int i = 0; i < 4; i++) inf = inf && all_zero32((const uint8_t*)pw->tau_g2 + 32 * i);
-        if (inf) throw_error(B2G_E_INPUT, "tau_g2[0]: at infinity");
-    }
+    powers_first_finite(pw);
     DevGuard g(cv.device);
     cudaStream_t st = cv.st;
-    SetupMem mem{st, {}};
+    DevArena mem(st, true);
     const uint64_t nK = 1ull << K;
     // sections in launch order: the three G1 ones (one segmented launch), then G2
     struct Sec { const char* name; const uint8_t* in; uint8_t* out; uint64_t limit; int top; bool g2; };
@@ -950,7 +859,7 @@ static void powers_prepare_run(b2g_ctx* ctx, const b2g_powers_desc* pw, const b2
     fe* d_sc = mem.alloc<fe>(28 * sizeof(fe));
     inv_pow2_kernel<<<1, 1, 0, st>>>(d_sc);
     g_launch_count += 1;
-    PinnedBuf pin(std::min(PREP_PINNED, (size_t)(4 * nK - 1) * 64));
+    PinnedHost pin(std::min(PREP_PINNED, (size_t)(4 * nK - 1) * 64));
 
     // blocks 0 .. min(top, SEG_LOG - 1) of every section: one segmented pass per curve
     SegSet set[2] = {};
@@ -968,10 +877,8 @@ static void powers_prepare_run(b2g_ctx* ctx, const b2g_powers_desc* pw, const b2
         s.out[y] = mem.alloc<uint8_t>(recs * (c.g2 ? 128 : 64));
         seg_top = std::max(seg_top, top);
     }
-    NttDomain seg_dom;
     {
-        struct DomGuard { NttDomain& d; ~DomGuard() { ntt_domain_destroy(d); } } dg{seg_dom};
-        ntt_domain_create(seg_dom, seg_top, st);
+        NttDomainHold seg_dom(seg_top, st);
         const unsigned fill_blocks = (unsigned)(((2ull << seg_top) - 1 + 127) / 128);
         seg_fill_kernel<G1, Fq><<<dim3(fill_blocks, 3), 128, 0, st>>>(set[0]);
         seg_fill_kernel<G2, Fq2><<<dim3(fill_blocks, 1), 128, 0, st>>>(set[1]);
@@ -1003,9 +910,7 @@ static void powers_prepare_run(b2g_ctx* ctx, const b2g_powers_desc* pw, const b2
             const uint64_t n = 1ull << k, cnt = std::min<uint64_t>(c.limit, n);
             check_upload(c.name, 0, c.in, cnt, c.g2, c.g2, d_aff, st);
             if (cnt < n) CUDA_CHECK(cudaMemsetAsync(d_aff + cnt * row, 0, (n - cnt) * row, st));
-            NttDomain dom;
-            struct DomGuard { NttDomain& d; ~DomGuard() { ntt_domain_destroy(d); } } dg{dom};
-            ntt_domain_create(dom, k, st);
+            NttDomainHold dom(k, st);
             const unsigned blocks = (unsigned)((n + 127) / 128);
             if (c.g2) {
                 pts_from_affine_kernel<G2, Fq2><<<blocks, 128, 0, st>>>(d_aff, (uint32_t)n, d_work);
@@ -1043,27 +948,18 @@ static void delta_update_run(b2g_ctx* ctx, const b2g_delta_key* a, const void* x
         (a->n_h && (!a->h_query || !b->h_query)))
         throw_error(B2G_E_SHAPE, "null key buffer");
     if (a->n_l != b->n_l || a->n_h != b->n_h) throw_error(B2G_E_SHAPE, "b2g_delta_update: the two keys' n_l / n_h differ");
-    const CtxView cv = ctx_view(ctx);
-    if (cv.proof_pending) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
+    const CtxView cv = ctx_idle(ctx);
     if (!below((const uint8_t*)x_canon, R_WORDS)) throw_error(B2G_E_INPUT, "x is not below r");
-    if (all_zero32((const uint8_t*)x_canon)) throw_error(B2G_E_INPUT, "x is zero");
+    if (all_zero(x_canon, 32)) throw_error(B2G_E_INPUT, "x is zero");
     DevGuard g(cv.device);
     cudaStream_t st = cv.st;
-    SetupMem mem{st, {}};
+    DevArena mem(st, true);
     uint8_t* d_d1 = powers_upload(mem, "delta_g1", a->delta_g1, 1, false, false, st);
     uint8_t* d_d2 = powers_upload(mem, "delta_g2", a->delta_g2, 1, true, true, st);
     uint8_t* d_l = powers_upload(mem, "l_query", a->l_query, a->n_l, false, false, st);
     uint8_t* d_h = powers_upload(mem, "h_query", a->h_query, a->n_h, false, false, st);
     fe* d_k = mem.alloc<fe>(2 * sizeof(fe));
-    {
-        uint8_t h_x[32];
-        memcpy(h_x, x_canon, 32);
-        // on the call's stream; h_x is wiped once the copy is done
-        cudaError_t e = cudaMemcpyAsync(d_k, h_x, 32, cudaMemcpyHostToDevice, st);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-        secure_zero(h_x, sizeof(h_x));
-        CUDA_CHECK(e);
-    }
+    upload_secrets(d_k, &x_canon, 1, st);
     delta_inverse_kernel<<<1, 1, 0, st>>>(d_k);
     const size_t most = std::max((size_t)std::max(a->n_l, a->n_h), (size_t)2);
     uint8_t* d_out = mem.alloc<uint8_t>(most * 64);
@@ -1092,16 +988,7 @@ static void delta_update_run(b2g_ctx* ctx, const b2g_delta_key* a, const void* x
 extern "C" {
 
 int b2g_setup(b2g_ctx* ctx, const b2g_mat_desc* circuit, const b2g_setup_secrets* secrets, b2g_setup_out* out) {
-    return b2g::guarded([&] {
-        try {
-            b2g::setup_run(ctx, circuit, secrets, out);
-        } catch (const b2g::B2gError& e) {
-            // a buffer that did not fit leaves cudaErrorMemoryAllocation as the thread's last error: clear it, so that the
-            // context's next call does not fail on it
-            if (e.code == B2G_E_DEVICE) cudaGetLastError();
-            throw;
-        }
-    });
+    return b2g::guarded_clear([&] { b2g::setup_run(ctx, circuit, secrets, out); });
 }
 
 int b2g_setup_from_powers(b2g_ctx* ctx, const b2g_mat_desc* circuit, const b2g_powers_desc* powers, b2g_setup_out* out) {

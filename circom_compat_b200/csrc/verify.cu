@@ -47,6 +47,7 @@
 #include "../../include/b2groth.h"
 #include "fixed.cuh"
 #include "pairing.cuh"
+#include "stage.cuh"
 #include "util.cuh"
 #include "verify.cuh"
 
@@ -849,8 +850,6 @@ __global__ void pairing_test_kernel(int op, const uint8_t* __restrict__ a, const
     Fq12::store(out + (size_t)i * F12_BYTES, r);
 }
 
-static bool all_zero(const void* p, size_t n);
-
 // ops 49-53 (see include/b2groth.h) run the kernels the verifier runs, not test copies of them: ptxas compiles each kernel
 // with its own copy of the __noinline__ calls it reaches (miller_loop_t, ell_fixed, the tower), so only a launch of the
 // shipped kernel tests the shipped machine code.  Per row of ops 49 and 53, a staging region holds the key's G2 points for
@@ -996,19 +995,6 @@ void pairing_test_op(cudaStream_t st, int op, const void* a, const void* b, size
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-static bool all_zero(const void* p, size_t n) {
-    const uint8_t* b = (const uint8_t*)p;
-    for (size_t i = 0; i < n; i++) if (b[i]) return false;
-    return true;
-}
-
-// a canonical 32-byte scalar below r
-static bool below_r(const uint32_t* k) {
-    const uint32_t r[8] = {FrParams::P0, FrParams::P1, FrParams::P2, FrParams::P3, FrParams::P4, FrParams::P5, FrParams::P6, FrParams::P7};
-    for (int i = 7; i >= 0; i--) if (k[i] != r[i]) return k[i] < r[i];
-    return false;
-}
-
 // grows one of the context's verification buffers to `bytes`; never shrinks it.  The buffer is marked empty before it is
 // reallocated, so a failed allocation leaves the context consistent.
 static void vbuf_grow(uint8_t*& p, size_t& cap, size_t bytes) {
@@ -1207,36 +1193,32 @@ static void vk_load_many(b2g_ctx* ctx, uint32_t n_keys, const b2g_vk_desc* descs
 // Returns the lowest bad index, or n.
 template <class Run>
 static uint64_t points_slices(const char* fn, b2g_ctx* ctx, size_t n, size_t in_row, size_t out_row, const void* in, void* out, Run&& run) {
-    const CtxView cv = ctx_view(ctx);
-    if (cv.proof_pending) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
+    const CtxView cv = ctx_idle(ctx);
     if (n == 0) return 0;
     DevGuard g(cv.device);
     cudaStream_t st = cv.st;
     const size_t slice = std::min(n, KEY_SLICE), bytes = slice * (in_row + out_row) + 8;
-    struct Buf { uint8_t* p = nullptr; ~Buf() { if (p) cudaFree(p); } } b;
-    if (cudaMalloc(&b.p, bytes) != cudaSuccess) {
+    DevArena mem(st);
+    uint8_t* d_in = nullptr;
+    try {
+        d_in = mem.alloc(bytes);
+    } catch (const B2gError&) {
         cudaGetLastError();
-        b.p = nullptr;
         throw_error(B2G_E_DEVICE, std::string(fn) + ": the device buffer of " + std::to_string(slice) + " points (" +
                                   std::to_string((bytes + (1 << 20) - 1) >> 20) + " MiB) does not fit in device memory");
     }
-    uint8_t *d_in = b.p, *d_out = b.p + slice * in_row;
+    uint8_t* d_out = d_in + slice * in_row;
     unsigned long long* d_bad = reinterpret_cast<unsigned long long*>(d_out + slice * out_row);
     uint64_t bad = n;
-    try {
-        CUDA_CHECK(cudaMemcpyAsync(d_bad, &bad, 8, cudaMemcpyHostToDevice, st));
-        for (size_t base = 0; base < n && bad == n; base += slice) {
-            const size_t m = std::min(slice, n - base);
-            CUDA_CHECK(cudaMemcpyAsync(d_in, (const uint8_t*)in + base * in_row, m * in_row, cudaMemcpyHostToDevice, st));
-            run(d_in, d_out, (uint32_t)m, (uint64_t)base, d_bad, st);
-            CUDA_CHECK(cudaGetLastError());
-            CUDA_CHECK(cudaMemcpyAsync((uint8_t*)out + base * out_row, d_out, m * out_row, cudaMemcpyDeviceToHost, st));
-            CUDA_CHECK(cudaMemcpyAsync(&bad, d_bad, 8, cudaMemcpyDeviceToHost, st));
-            CUDA_CHECK(cudaStreamSynchronize(st));
-        }
-    } catch (...) {
-        cudaStreamSynchronize(st);                         // nothing may still use the buffer when it is freed
-        throw;
+    CUDA_CHECK(cudaMemcpyAsync(d_bad, &bad, 8, cudaMemcpyHostToDevice, st));
+    for (size_t base = 0; base < n && bad == n; base += slice) {
+        const size_t m = std::min(slice, n - base);
+        CUDA_CHECK(cudaMemcpyAsync(d_in, (const uint8_t*)in + base * in_row, m * in_row, cudaMemcpyHostToDevice, st));
+        run(d_in, d_out, (uint32_t)m, (uint64_t)base, d_bad, st);
+        CUDA_CHECK(cudaGetLastError());
+        CUDA_CHECK(cudaMemcpyAsync((uint8_t*)out + base * out_row, d_out, m * out_row, cudaMemcpyDeviceToHost, st));
+        CUDA_CHECK(cudaMemcpyAsync(&bad, d_bad, 8, cudaMemcpyDeviceToHost, st));
+        CUDA_CHECK(cudaStreamSynchronize(st));
     }
     return bad;
 }
@@ -1559,8 +1541,7 @@ static void delta_check_run(b2g_ctx* ctx, const b2g_delta_key* a, const b2g_delt
     if (!a->delta_g1 || !a->delta_g2 || !b->delta_g1 || !b->delta_g2 || (a->n_l && !a->l_query) || (a->n_h && !a->h_query) ||
         (b->n_l && !b->l_query) || (b->n_h && !b->h_query))
         throw_error(B2G_E_SHAPE, "null key buffer");
-    const CtxView cv = ctx_view(ctx);
-    if (cv.proof_pending) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
+    const CtxView cv = ctx_idle(ctx);
     *verdict_out = 0;
     const uint64_t n64 = (uint64_t)a->n_l + a->n_h;
     if (n64 && !weights) throw_error(B2G_E_SHAPE, "null pointer");
@@ -1582,47 +1563,43 @@ static void delta_check_run(b2g_ctx* ctx, const b2g_delta_key* a, const b2g_delt
     const size_t o_x = o_rec + (size_t)n * 256, o_y = o_x + std::max(scratch, (size_t)1) * 128;
     const size_t o_tails = (o_y + std::max(scratch, (size_t)1) * 128 + 255) & ~(size_t)255, o_spans = o_tails + 2 * TAIL_BYTES;
     const size_t o_ok = o_spans + std::max(spans.size(), (size_t)1) * sizeof(Span), bytes = o_ok + 8;
-    struct Buf { uint8_t* p = nullptr; ~Buf() { if (p) cudaFree(p); } } buf;
-    if (cudaMalloc(&buf.p, bytes) != cudaSuccess) {
+    DevArena mem(st);
+    uint8_t* D = nullptr;
+    try {
+        D = mem.alloc(bytes);
+    } catch (const B2gError&) {
         cudaGetLastError();
-        buf.p = nullptr;
         throw_error(B2G_E_DEVICE, "b2g_delta_update_check: the device buffers (" + std::to_string((bytes + (1 << 20) - 1) >> 20) +
                                       " MiB) do not fit in device memory");
     }
-    uint8_t* D = buf.p;
-    try {
-        const uint32_t one = 1;
-        CUDA_CHECK(cudaMemsetAsync(D + o_tails, 0, 2 * TAIL_BYTES, st));
-        CUDA_CHECK(cudaMemcpyAsync(D + o_ok, &one, 4, cudaMemcpyHostToDevice, st));
-        CUDA_CHECK(cudaMemcpyAsync(D, a->delta_g1, 64, cudaMemcpyHostToDevice, st));
-        CUDA_CHECK(cudaMemcpyAsync(D + 64, a->delta_g2, 128, cudaMemcpyHostToDevice, st));
-        CUDA_CHECK(cudaMemcpyAsync(D + 192, b->delta_g1, 64, cudaMemcpyHostToDevice, st));
-        CUDA_CHECK(cudaMemcpyAsync(D + 256, b->delta_g2, 128, cudaMemcpyHostToDevice, st));
-        if (n) {
-            const size_t nl = a->n_l, nh = a->n_h;
-            if (nl) CUDA_CHECK(cudaMemcpyAsync(D + o_pts, b->l_query, nl * 64, cudaMemcpyHostToDevice, st));
-            if (nh) CUDA_CHECK(cudaMemcpyAsync(D + o_pts + nl * 64, b->h_query, nh * 64, cudaMemcpyHostToDevice, st));
-            if (nl) CUDA_CHECK(cudaMemcpyAsync(D + o_before, a->l_query, nl * 64, cudaMemcpyHostToDevice, st));
-            if (nh) CUDA_CHECK(cudaMemcpyAsync(D + o_before + nl * 64, a->h_query, nh * 64, cudaMemcpyHostToDevice, st));
-            CUDA_CHECK(cudaMemcpyAsync(D + o_w, weights, (size_t)n * 16, cudaMemcpyHostToDevice, st));
-            CUDA_CHECK(cudaMemcpyAsync(D + o_spans, spans.data(), spans.size() * sizeof(Span), cudaMemcpyHostToDevice, st));
-            delta_weigh_kernel<<<(n + 127) / 128, 128, 0, st>>>(D + o_pts, D + o_before, (const uint32_t*)(D + o_w), n, D + o_rec,
-                                                                (uint32_t*)(D + o_ok));
-            g_launch_count += 1;
-            reduce_run(levels, (const Span*)(D + o_spans), D + o_rec, 128, 128, nullptr, D + o_x, D + o_y,
-                       [&](uint32_t blocks, const uint8_t* src, size_t stride, const Span* sp, const uint8_t* mask, uint8_t* dst) {
-                           g1_sum_kernel<<<blocks, 128, 0, st>>>(src, stride, sp, mask, dst, D + o_tails);
-                       });
-        }
-        delta_verdict_kernel<<<1, 32, 0, st>>>(D, D + o_tails, (const uint32_t*)(D + o_ok), D + o_ok + 4);
+    const uint32_t one = 1;
+    CUDA_CHECK(cudaMemsetAsync(D + o_tails, 0, 2 * TAIL_BYTES, st));
+    CUDA_CHECK(cudaMemcpyAsync(D + o_ok, &one, 4, cudaMemcpyHostToDevice, st));
+    CUDA_CHECK(cudaMemcpyAsync(D, a->delta_g1, 64, cudaMemcpyHostToDevice, st));
+    CUDA_CHECK(cudaMemcpyAsync(D + 64, a->delta_g2, 128, cudaMemcpyHostToDevice, st));
+    CUDA_CHECK(cudaMemcpyAsync(D + 192, b->delta_g1, 64, cudaMemcpyHostToDevice, st));
+    CUDA_CHECK(cudaMemcpyAsync(D + 256, b->delta_g2, 128, cudaMemcpyHostToDevice, st));
+    if (n) {
+        const size_t nl = a->n_l, nh = a->n_h;
+        if (nl) CUDA_CHECK(cudaMemcpyAsync(D + o_pts, b->l_query, nl * 64, cudaMemcpyHostToDevice, st));
+        if (nh) CUDA_CHECK(cudaMemcpyAsync(D + o_pts + nl * 64, b->h_query, nh * 64, cudaMemcpyHostToDevice, st));
+        if (nl) CUDA_CHECK(cudaMemcpyAsync(D + o_before, a->l_query, nl * 64, cudaMemcpyHostToDevice, st));
+        if (nh) CUDA_CHECK(cudaMemcpyAsync(D + o_before + nl * 64, a->h_query, nh * 64, cudaMemcpyHostToDevice, st));
+        CUDA_CHECK(cudaMemcpyAsync(D + o_w, weights, (size_t)n * 16, cudaMemcpyHostToDevice, st));
+        CUDA_CHECK(cudaMemcpyAsync(D + o_spans, spans.data(), spans.size() * sizeof(Span), cudaMemcpyHostToDevice, st));
+        delta_weigh_kernel<<<(n + 127) / 128, 128, 0, st>>>(D + o_pts, D + o_before, (const uint32_t*)(D + o_w), n, D + o_rec,
+                                                            (uint32_t*)(D + o_ok));
         g_launch_count += 1;
-        CUDA_CHECK(cudaGetLastError());
-        CUDA_CHECK(cudaMemcpyAsync(verdict_out, D + o_ok + 4, 1, cudaMemcpyDeviceToHost, st));
-        CUDA_CHECK(cudaStreamSynchronize(st));
-    } catch (...) {
-        cudaStreamSynchronize(st);                         // nothing may still use the buffer when it is freed
-        throw;
+        reduce_run(levels, (const Span*)(D + o_spans), D + o_rec, 128, 128, nullptr, D + o_x, D + o_y,
+                   [&](uint32_t blocks, const uint8_t* src, size_t stride, const Span* sp, const uint8_t* mask, uint8_t* dst) {
+                       g1_sum_kernel<<<blocks, 128, 0, st>>>(src, stride, sp, mask, dst, D + o_tails);
+                   });
     }
+    delta_verdict_kernel<<<1, 32, 0, st>>>(D, D + o_tails, (const uint32_t*)(D + o_ok), D + o_ok + 4);
+    g_launch_count += 1;
+    CUDA_CHECK(cudaGetLastError());
+    CUDA_CHECK(cudaMemcpyAsync(verdict_out, D + o_ok + 4, 1, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaStreamSynchronize(st));
 }
 
 int setup_generators_check(const void* g1, const void* g2, cudaStream_t st) {
@@ -1677,8 +1654,7 @@ int b2g_vk_alpha_beta(b2g_vk* vk, void* out) {
 // context; returns the context
 static CtxView batch_args(const char* fn, b2g_ctx* ctx, uint32_t count) {
     if (count == 0) throw_error(B2G_E_SHAPE, std::string(fn) + ": count must be at least 1");
-    const CtxView cv = ctx_view(ctx);
-    if (cv.proof_pending) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
+    const CtxView cv = ctx_idle(ctx);
     return cv;
 }
 
@@ -1759,7 +1735,7 @@ int b2g_rerandomize_many(b2g_ctx* ctx, b2g_vk* vk, uint32_t count, const void* p
         for (uint32_t i = 0; i < count; i++)
             for (const auto& [name, r] : {std::pair{"r1", r1_canon}, std::pair{"r2", r2_canon}}) {
                 const uint32_t* k = (const uint32_t*)r + 8 * (size_t)i;
-                if (all_zero(k, 32) || !below_r(k))
+                if (all_zero(k, 32) || !below((const uint8_t*)k, R_WORDS))
                     throw_error(B2G_E_INPUT, std::string(fn) + ": factor " + name + " of proof " + std::to_string(i) +
                                              " is not in [1, r)");
             }
@@ -1991,7 +1967,7 @@ static void batch_check(const char* fn, int64_t key, const CtxView& cv, const b2
     const uint32_t n_public = b.vk->n_public;
     const uint32_t* pub = (const uint32_t*)b.public_inputs;
     for (size_t i = 0; i < (size_t)b.count * n_public; i++)
-        if (!below_r(pub + 8 * i)) fail(B2G_E_INPUT, "public input " + std::to_string(i % n_public) + " of proof " + std::to_string(i / n_public) +
+        if (!below((const uint8_t*)(pub + 8 * i), R_WORDS)) fail(B2G_E_INPUT, "public input " + std::to_string(i % n_public) + " of proof " + std::to_string(i / n_public) +
                                                      " is not below the scalar field modulus r");
     for (uint32_t i = 0; weighted && i < b.count; i++)
         if (all_zero((const uint8_t*)b.weights + 16 * (size_t)i, 16)) fail(B2G_E_INPUT, "weight " + std::to_string(i) + " is zero");

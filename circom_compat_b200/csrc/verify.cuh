@@ -14,6 +14,8 @@ void verify_bufs_free(VerifyBufs* v);
 // the parts of a context verify.cu uses (b2g_ctx is private to prover.cu)
 struct CtxView { int device; cudaStream_t st; bool proof_pending; VerifyBufs** vbufs; };
 CtxView ctx_view(b2g_ctx* ctx);
+// ctx_view of a context with no submitted proof pending; B2G_E_SHAPE otherwise
+CtxView ctx_idle(b2g_ctx* ctx);
 
 // b2g_test_op ops PAIRING_TEST_OP0 and up: the Fq12 tower and the pairing (verify.cu)
 constexpr int PAIRING_TEST_OP0 = 30;

@@ -19,6 +19,7 @@
 #include <vector>
 #include "../../include/b2groth.h"
 #include "fp.cuh"
+#include "stage.cuh"
 #include "util.cuh"
 #include "verify.cuh"
 
@@ -968,8 +969,7 @@ size_t lane_bytes(const b2g_wasm* w, size_t io_bytes) {
 template <class Stage, class Collect>
 void run_lanes(b2g_ctx* ctx, b2g_wasm* w, Prog base, uint32_t count, size_t io_in, size_t io_out, uint32_t* status_out,
                Stage&& stage, Collect&& collect) {
-    const CtxView cv = ctx_view(ctx);
-    if (cv.proof_pending) throw_error(B2G_E_SHAPE, "a submitted proof is still pending on this context: call b2g_prove_wait first");
+    const CtxView cv = ctx_idle(ctx);
     if (cv.device != w->device) throw_error(B2G_E_SHAPE, "the module was loaded on another device");
     DevGuard g(cv.device);
     cudaStream_t st = cv.st;
@@ -1062,8 +1062,7 @@ void probe(b2g_ctx* ctx, b2g_wasm* w) {
     if (status != 0) refuse("the module trapped while reporting its field and sizes (lane status " + std::to_string(status) + ")");
     w->info.version = res[0]; w->info.n32 = res[1]; w->info.witness_size = res[10]; w->info.input_size = res[11];
     if (w->info.n32 != 8) refuse("getFieldNumLen32 returned " + std::to_string(w->info.n32) + ": only 8 (a 254-bit field) is supported");
-    static const uint32_t R[8] = {FrParams::P0, FrParams::P1, FrParams::P2, FrParams::P3, FrParams::P4, FrParams::P5, FrParams::P6, FrParams::P7};
-    if (memcmp(res + 2, R, 32) != 0) refuse("the circuit's prime is not the BN254 scalar field modulus r");
+    if (memcmp(res + 2, R_WORDS, 32) != 0) refuse("the circuit's prime is not the BN254 scalar field modulus r");
     if (w->info.witness_size == 0) refuse("the module reports an empty witness");
 }
 
@@ -1157,12 +1156,11 @@ int b2g_witness_calculate(b2g_ctx* ctx, b2g_wasm* w, uint32_t count, uint32_t n_
         const uint32_t nv = (uint32_t)meta.size();
         if (count == 0) return;
         if (nv && !values_canon) throw_error(B2G_E_SHAPE, "null pointer");
-        static const uint32_t R[8] = {FrParams::P0, FrParams::P1, FrParams::P2, FrParams::P3, FrParams::P4, FrParams::P5, FrParams::P6, FrParams::P7};
         const uint32_t* vals = (const uint32_t*)values_canon;
         for (size_t e = 0; e < (size_t)count * nv; e++) {
             const uint32_t* x = vals + 8 * e;
             for (int j = 7; j >= 0; j--) {
-                if (x[j] != R[j]) { if (x[j] > R[j]) throw_error(B2G_E_INPUT, "values_canon[" + std::to_string(e) + "] is not below r"); break; }
+                if (x[j] != R_WORDS[j]) { if (x[j] > R_WORDS[j]) throw_error(B2G_E_INPUT, "values_canon[" + std::to_string(e) + "] is not below r"); break; }
                 if (j == 0) throw_error(B2G_E_INPUT, "values_canon[" + std::to_string(e) + "] is not below r");
             }
         }
