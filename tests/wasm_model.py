@@ -337,10 +337,14 @@ def _sext(v, bits, M):
 
 
 class Instance:
-    """one fresh instantiation: memory from the data segments, globals from their initialisers"""
+    """one fresh instantiation: memory from the data segments, globals from their initialisers.
 
-    def __init__(self, m: Module, max_pages=None, max_depth=1024, fuel=None):
+    trace: None (the default) or a dict that collects, per defined function k, the set of pcs (indices into
+    Module.body(k)) this instance executes; coverage tests pass one in, other callers pay nothing for it."""
+
+    def __init__(self, m: Module, max_pages=None, max_depth=1024, fuel=None, trace=None):
         self.m = m
+        self.trace = trace
         lo, hi = m.mem
         self.max_pages = max_pages if max_pages is not None else (hi if hi is not None else 65536)
         if hi is not None:
@@ -405,7 +409,10 @@ class Instance:
         nres = len(m.ftype(f)[1])
         st, labels = [], []        # labels: (pc to go to on a branch, arity on a branch, height, is loop)
         pc, n = 0, len(code)
+        tr = self.trace.setdefault(k, set()) if self.trace is not None else None
         while pc < n:
+            if tr is not None:
+                tr.add(pc)
             ins = code[pc]
             op = ins[0]
             pc += 1
