@@ -45,6 +45,14 @@ constexpr uint32_t MAX_BATCH = 65535;                 // proofs per b2g_prove_ma
 
 using namespace b2g;
 
+// a pass captured as a CUDA graph: the executable, the key it was captured for and the launches one replay stands for
+struct GraphSlot {
+    cudaGraphExec_t exec = nullptr;
+    std::vector<uint64_t> key;
+    uint64_t launches = 0;
+};
+enum { G_PROOF = 0, G_P2P = 1, G_KEYS = 2, NG = 3 };
+
 struct b2g_ctx {
     int device = 0, shard_rank = 0, shard_count = 1;
     cudaStream_t st[NQ] = {}, st_glue = nullptr;
@@ -69,10 +77,11 @@ struct b2g_ctx {
     // One proof's whole device pipeline (all streams, ~100 launches) captured once per (key, matrices) as a CUDA graph and
     // replayed with a single launch: the host cost of a proof drops from ~130 driver calls to a handful (B2G_GRAPH=0 disables)
     bool use_graph = true;
-    cudaGraphExec_t gexec[2] = {nullptr, nullptr};             // [0] whole proof (or batch), [1] sharded proof with the peer-memory exchange
-    uint64_t g_key[2][4] = {};                                  // (key uid, matrices uid, buffer generation, batch count) each graph was captured for
+    // [G_PROOF] whole proof (or batch) and [G_P2P] sharded proof with the peer-memory exchange, each captured for (key uid,
+    // matrices uid, buffer generation, batch count); [G_KEYS] the b2g_prove_keys pass, for (group uid, buffer generation,
+    // counts of every key), in a slot of its own so that it does not evict the one-key graph
+    GraphSlot graphs[NG];
     uint64_t alloc_gen = 1;                                    // bumped whenever a buffer the graphs point into is (re)allocated
-    uint64_t g_launches[2] = {0, 0};
     unsigned long long* d_epoch = nullptr;                     // exchange epoch (device-resident so that it survives graph replay)
     // peer-memory exchange (b2g_prove_sharded_p2p): own buffer + every rank's buffer as seen from this device
     uint8_t* d_xchg = nullptr;                 // exchange arena (layout at EVAL_OFF below); allocated when the context is wired to its peers
@@ -81,12 +90,8 @@ struct b2g_ctx {
     void* peer_mapped[64] = {};                // cudaIpcOpenMemHandle results (to close)
     int peers_imported = 0;
     VerifyBufs* vbufs = nullptr;               // b2g_verify_many scratch (verify.cu), grown on demand
-    // b2g_prove_keys: the per-proof rows of its three sorts and the key of every proof (rewritten by each call), and the pass
-    // captured as a graph of its own, for (group uid, buffer generation, counts of every key)
+    // b2g_prove_keys: the per-proof rows of its three sorts and the key of every proof (rewritten by each call)
     uint8_t* d_keyed = nullptr; size_t cap_keyed = 0;
-    cudaGraphExec_t gexec_keys = nullptr;
-    std::vector<uint64_t> gk_key;
-    uint64_t gk_launches = 0;
 };
 
 static std::atomic<uint64_t> g_next_uid{1};            // handles are told apart by uid, not by address (addresses get reused)
@@ -617,37 +622,42 @@ static void ensure_batch_buffers(b2g_ctx* ctx, uint32_t count) {
     if (ctx->scratch_ok) for (int q = 0; q < NQ; q++) ctx->scratch[q].result = ctx->d_partial + PARTIAL_OFF[q];
 }
 
-// per-stream MSM scratch of this context, sized for `pk` and `count` proofs.  Kept while later calls fit (a smaller batch
-// reuses it); re-created for exactly (pk, count) when they do not, so a larger key after a large batch does not inherit
-// that batch's size.
-static void ensure_scratch(b2g_ctx* ctx, const b2g_pk* pk, uint32_t count = 1) {
-    const size_t nwb = (size_t)pk->b_compact * count;
-    bool ok = ctx->scratch_ok && (!pk->d_bidx || (ctx->scratch_bsort && nwb <= ctx->cap_wb));
+// per-stream MSM scratch of this context for `count` proofs: query q at plan[q]'s window size and buckets with n[q] bases per
+// proof; H and L with sort buffers, and B1 too when bsort (B1 and B2 then read a B sort of their own, over nwb gathered B
+// scalars in d_wb; otherwise they read L's).  Kept while later calls fit (a smaller batch reuses it); re-created for exactly
+// this call when they do not, so a larger key after a large batch does not inherit that batch's size.
+static void ensure_scratch(b2g_ctx* ctx, const MsmPlan* plan, const uint32_t* n, uint32_t count, bool bsort, size_t nwb) {
+    bool ok = ctx->scratch_ok && (!bsort || (ctx->scratch_bsort && nwb <= ctx->cap_wb));
     for (int q = 0; q < NQ && ok; q++) {
-        const MsmPlan& p = pk->plan[q]; const MsmScratch& sc = ctx->scratch[q];
-        if ((p.n ? p.n : 1) > sc.cap_n || p.nwin > sc.cap_nwin || p.nbuckets > sc.cap_buckets || count > sc.cap_count) ok = false;
+        const MsmPlan& p = plan[q]; const MsmScratch& sc = ctx->scratch[q];
+        if (n[q] > sc.cap_n || p.nwin > sc.cap_nwin || p.nbuckets > sc.cap_buckets || count > sc.cap_count) ok = false;
     }
     if (ok) return;
     CUDA_CHECK(cudaDeviceSynchronize());
     for (int q = 0; q < NQ; q++) msm_scratch_free(ctx->scratch[q]);     // also the remains of an allocation that failed
     ctx->scratch_ok = false; ctx->alloc_gen++;
     for (int q = 0; q < NQ; q++) {
-        const MsmPlan& p = pk->plan[q];
-        msm_scratch_alloc(ctx->scratch[q], p.n ? p.n : 1, p.nwin, p.nbuckets, q == Q_B2, q == Q_H || q == Q_L || (q == Q_B1 && pk->d_bidx), count);
+        msm_scratch_alloc(ctx->scratch[q], n[q], plan[q].nwin, plan[q].nbuckets, q == Q_B2, q == Q_H || q == Q_L || (q == Q_B1 && bsort), count);
         cudaFree(ctx->scratch[q].result);
         ctx->scratch[q].result = ctx->d_partial + PARTIAL_OFF[q];
         ctx->scratch[q].result_owned = false;
         ctx->scratch[q].result_stride = REC_BYTES;
     }
-    ctx->scratch_bsort = pk->d_bidx != nullptr;
-    const size_t nwb_cap = (size_t)pk->b_compact * count;
-    if (nwb_cap > ctx->cap_wb) {
+    ctx->scratch_bsort = bsort;
+    if (nwb > ctx->cap_wb) {
         if (ctx->d_wb) cudaFree(ctx->d_wb);
         ctx->d_wb = nullptr; ctx->cap_wb = 0;
-        CUDA_CHECK(cudaMalloc(&ctx->d_wb, (nwb_cap + 1) * sizeof(fe)));
-        ctx->cap_wb = nwb_cap;
+        CUDA_CHECK(cudaMalloc(&ctx->d_wb, (nwb + 1) * sizeof(fe)));
+        ctx->cap_wb = nwb;
     }
     ctx->scratch_ok = true;
+}
+
+// the scratch of `count` proofs under one key
+static void ensure_scratch(b2g_ctx* ctx, const b2g_pk* pk, uint32_t count = 1) {
+    uint32_t n[NQ];
+    for (int q = 0; q < NQ; q++) n[q] = pk->plan[q].n ? pk->plan[q].n : 1;
+    ensure_scratch(ctx, pk->plan, n, count, pk->d_bidx != nullptr, (size_t)pk->b_compact * count);
 }
 
 // the witness map of `count` proofs side by side: one launch per kernel of the chain, the batch on a grid dimension.  The
@@ -724,6 +734,26 @@ static void run_witness_map_split(b2g_ctx* ctx, b2g_mat* mat, uint32_t lo, uint3
     CUDA_CHECK(cudaGetLastError());
 }
 
+// The four witness-query accumulations of `count` proofs in WITNESS_ORDER, each on its own stream behind the sort it reads:
+// the W sort (ev_sort, on the L stream) or, when bsort, for B1 and B2 the B sort (ev_sortb, on the B1 stream).  Each ends in
+// ev_done[q].  scale: s*msm_A and r*msm_B1 right behind those MSMs (d_rs must hold r, s); timed: phase events around each.
+static void accumulate_witness_queries(b2g_ctx* ctx, const MsmPlan* plan, bool bsort, uint32_t count, bool timed, bool scale) {
+    for (int q : WITNESS_ORDER) {
+        const bool on_b = bsort && (q == Q_B1 || q == Q_B2);
+        if (on_b) { if (q != Q_B1) CUDA_CHECK(cudaStreamWaitEvent(ctx->st[q], ctx->ev_sortb, 0)); }
+        else if (q != Q_L) CUDA_CHECK(cudaStreamWaitEvent(ctx->st[q], ctx->ev_sort, 0));
+        if (timed) CUDA_CHECK(cudaEventRecord(ctx->ev_t[2 * q], ctx->st[q]));
+        msm_accumulate(plan[q], on_b ? ctx->scratch[Q_B1] : ctx->scratch[Q_L], ctx->scratch[q], ctx->st[q]);
+        if (scale && (q == Q_A || q == Q_B1)) {
+            const Scalar256* rs = reinterpret_cast<const Scalar256*>(ctx->d_rs);
+            scale_partial_kernel<<<count, 32, 0, ctx->st[q]>>>(ctx->d_partial + PARTIAL_OFF[q], q == Q_A ? rs + 1 : rs, ctx->d_partial + B2G_PARTIAL_BYTES + (q == Q_A ? 0 : 128), 2);
+            g_launch_count += 1;
+        }
+        if (timed) CUDA_CHECK(cudaEventRecord(ctx->ev_t[2 * q + 1], ctx->st[q]));
+        CUDA_CHECK(cudaEventRecord(ctx->ev_done[q], ctx->st[q]));
+    }
+}
+
 // count > 1: a batch of proofs (witnesses pk->n_vars apart in d_w); every MSM sorts and accumulates the whole batch at once
 static void launch_msms(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, bool timed, bool scale, bool split_map = false, uint32_t count = 1) {
     cudaStream_t s0 = ctx->st[0], ssort = ctx->st[Q_L];
@@ -741,20 +771,7 @@ static void launch_msms(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, bool timed, bool
         msm_sort(pk->plan[Q_B1], ctx->scratch[Q_B1], ctx->d_wb, pk->b_compact, true, sb, count, pk->b_compact);
         CUDA_CHECK(cudaEventRecord(ctx->ev_sortb, sb));
     }
-    for (int q : WITNESS_ORDER) {
-        const bool on_b = bsparse && (q == Q_B1 || q == Q_B2);
-        if (on_b) { if (q != Q_B1) CUDA_CHECK(cudaStreamWaitEvent(ctx->st[q], ctx->ev_sortb, 0)); }
-        else if (q != Q_L) CUDA_CHECK(cudaStreamWaitEvent(ctx->st[q], ctx->ev_sort, 0));
-        if (timed) CUDA_CHECK(cudaEventRecord(ctx->ev_t[2 * q], ctx->st[q]));
-        msm_accumulate(pk->plan[q], on_b ? ctx->scratch[Q_B1] : ctx->scratch[Q_L], ctx->scratch[q], ctx->st[q]);
-        if (scale && (q == Q_A || q == Q_B1)) {
-            const Scalar256* rs = reinterpret_cast<const Scalar256*>(ctx->d_rs);
-            scale_partial_kernel<<<count, 32, 0, ctx->st[q]>>>(ctx->d_partial + PARTIAL_OFF[q], q == Q_A ? rs + 1 : rs, ctx->d_partial + B2G_PARTIAL_BYTES + (q == Q_A ? 0 : 128), 2);
-            g_launch_count += 1;
-        }
-        if (timed) CUDA_CHECK(cudaEventRecord(ctx->ev_t[2 * q + 1], ctx->st[q]));
-        CUDA_CHECK(cudaEventRecord(ctx->ev_done[q], ctx->st[q]));
-    }
+    accumulate_witness_queries(ctx, pk->plan, bsparse, count, timed, scale);
     if (timed) CUDA_CHECK(cudaEventRecord(ctx->ev_t[10], s0));
     if (split_map) run_witness_map_split(ctx, mat, pk->lo[Q_H], pk->cnt[Q_H], s0);
     else run_witness_map(ctx, mat, s0, count);
@@ -833,6 +850,25 @@ static void pk_desc_check(const b2g_pk_desc* d) {
     if (d->n_vars - (d->n_public + 1) && !d->l_query) throw_error(B2G_E_SHAPE, "null proving-key section");
 }
 
+// L, A, B1, B2 all pair bases with w[1..n_vars): L is re-indexed onto that range by prepending (l - 1) points at infinity
+// (l_query[j] belongs to w[l + j]), so the four queries share one digit sort per proof
+static std::vector<uint8_t> l_padded(const b2g_pk_desc* d) {
+    const uint32_t li = d->n_public + 1;
+    std::vector<uint8_t> l((size_t)(d->n_vars - 1) * 64, 0);
+    if (d->n_vars - li) memcpy(l.data() + (size_t)(li - 1) * 64, d->l_query, (size_t)(d->n_vars - li) * 64);
+    return l;
+}
+
+// one query's table from n host bases of `aff` bytes: uploaded to tmp (which a caller's guard frees if a step throws),
+// build(tmp), synchronise, free tmp
+template <class Build>
+static void table_from_host(void*& tmp, const void* src, uint32_t n, size_t aff, cudaStream_t st, Build build) {
+    if (n) tmp = dev_upload<uint8_t>(src, (size_t)n * aff, st);
+    build(tmp);
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    if (tmp) { cudaFree(tmp); tmp = nullptr; }
+}
+
 // (r, s) -> ctx->d_rs on stream 0.  Every entry point synchronises stream 0 before it returns (b2g_bench_device stages once),
 // so the pinned staging slot is free again by the time the next call overwrites it.  count proofs: r, s = count x 32 B each,
 // staged as r_j | s_j pairs.
@@ -845,25 +881,38 @@ static void stage_rs(b2g_ctx* ctx, const void* r, const void* s, uint32_t count 
     memcpy(ctx->pre_r, r, 32); memcpy(ctx->pre_s, s, 32);
 }
 
-// r*delta1, K_C and s*delta2 depend only on (r, s): forked from stream 0 (after d_rs is written and after the previous
-// proof's assembly has read d_pre) onto a side stream, so they overlap the MSMs
-static void launch_glue_pre(b2g_ctx* ctx, b2g_pk* pk, uint32_t count = 1) {
+// r*delta1, K_C and s*delta2 depend only on (r, s): launch(st_glue) enqueues the glue_pre kernel on a side stream forked from
+// stream 0 (after d_rs is written and after the previous proof's assembly has read d_pre), so it overlaps the MSMs; ev_pre
+// marks its end
+template <class Launch>
+static void fork_glue_pre(b2g_ctx* ctx, Launch launch) {
     CUDA_CHECK(cudaEventRecord(ctx->ev_fork, ctx->st[0]));
     CUDA_CHECK(cudaStreamWaitEvent(ctx->st_glue, ctx->ev_fork, 0));
-    glue_pre_kernel<<<count, 160, 0, ctx->st_glue>>>(pk->d_tab_delta1, pk->d_tab_delta2, pk->d_tab_aa, pk->d_tab_bb, reinterpret_cast<const Scalar256*>(ctx->d_rs), ctx->d_pre);
+    launch(ctx->st_glue);
     CUDA_CHECK(cudaEventRecord(ctx->ev_pre, ctx->st_glue));
-    ctx->pre_valid = true;
     g_launch_count += 1;
 }
 
-// partials_dev: `count` records of REC_BYTES per proof; nproofs > 1: proofs of a batch, each assembled from its own records
-static void launch_glue_post(b2g_ctx* ctx, b2g_pk* pk, const uint8_t* partials_dev, int count, cudaStream_t st, uint32_t nproofs = 1) {
+// launch() enqueues the glue_post kernel on `st` once glue_pre is in
+template <class Launch>
+static void join_glue_post(b2g_ctx* ctx, cudaStream_t st, Launch launch) {
     CUDA_CHECK(cudaStreamWaitEvent(st, ctx->ev_pre, 0));
-    glue_post_kernel<<<nproofs, 96, 0, st>>>(partials_dev, count, pk->d_consts, ctx->d_pre, ctx->d_proof);
+    launch();
     g_launch_count += 1;
     CUDA_CHECK(cudaGetLastError());
 }
 
+static void launch_glue_pre(b2g_ctx* ctx, b2g_pk* pk, uint32_t count = 1) {
+    fork_glue_pre(ctx, [&](cudaStream_t sg) {
+        glue_pre_kernel<<<count, 160, 0, sg>>>(pk->d_tab_delta1, pk->d_tab_delta2, pk->d_tab_aa, pk->d_tab_bb, reinterpret_cast<const Scalar256*>(ctx->d_rs), ctx->d_pre);
+    });
+    ctx->pre_valid = true;
+}
+
+// partials_dev: `count` records of REC_BYTES per proof; nproofs > 1: proofs of a batch, each assembled from its own records
+static void launch_glue_post(b2g_ctx* ctx, b2g_pk* pk, const uint8_t* partials_dev, int count, cudaStream_t st, uint32_t nproofs = 1) {
+    join_glue_post(ctx, st, [&] { glue_post_kernel<<<nproofs, 96, 0, st>>>(partials_dev, count, pk->d_consts, ctx->d_pre, ctx->d_proof); });
+}
 
 // Everything one proof does on the device between "witness and (r, s) are in HBM" and "proof bytes are in d_proof".
 // kind 0: whole proof, or `count` whole proofs of a batch; kind 1: base-sharded proof whose partials are exchanged through
@@ -885,37 +934,45 @@ static void enqueue_proof(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, int kind, bool
     }
 }
 
-// Replays the captured pipeline (capturing it first if this context has none for (pk, mat)); falls back to direct launches
-// when graphs are disabled or the capture fails.
-static void run_proof(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, int kind, uint32_t count = 1) {
+// Replays the pass captured in `slot` (capturing enqueue(false) first if the slot holds none for `key`); runs enqueue(true)
+// directly when graphs are disabled or the capture fails.  timers: the pass has phase timers, recorded around the replay.
+template <class Enqueue>
+static void run_graph(b2g_ctx* ctx, GraphSlot& slot, std::vector<uint64_t> key, bool timers, Enqueue enqueue) {
     cudaStream_t s0 = ctx->st[0];
-    if (!ctx->use_graph) { enqueue_proof(ctx, pk, mat, kind, true, count); return; }
-    const uint64_t key[4] = {pk->uid, mat->uid, ctx->alloc_gen, count};
-    if (ctx->gexec[kind] && memcmp(ctx->g_key[kind], key, sizeof key)) { cudaGraphExecDestroy(ctx->gexec[kind]); ctx->gexec[kind] = nullptr; }
-    if (!ctx->gexec[kind]) {
+    if (!ctx->use_graph) { enqueue(true); return; }
+    if (slot.exec && slot.key != key) { cudaGraphExecDestroy(slot.exec); slot.exec = nullptr; }
+    if (!slot.exec) {
         const uint64_t before = g_launch_count.load();
         cudaGraph_t graph = nullptr;
         CUDA_CHECK(cudaStreamBeginCapture(s0, cudaStreamCaptureModeThreadLocal));
-        try { enqueue_proof(ctx, pk, mat, kind, false, count); }
+        try { enqueue(false); }
         catch (...) { cudaStreamEndCapture(s0, &graph); if (graph) cudaGraphDestroy(graph); cudaGetLastError(); g_launch_count = before; throw; }
         cudaError_t e = cudaStreamEndCapture(s0, &graph);
-        if (e == cudaSuccess) e = cudaGraphInstantiate(&ctx->gexec[kind], graph, 0);
+        if (e == cudaSuccess) e = cudaGraphInstantiate(&slot.exec, graph, 0);
         if (graph) cudaGraphDestroy(graph);
-        ctx->g_launches[kind] = g_launch_count.load() - before;
+        slot.launches = g_launch_count.load() - before;
         g_launch_count = before;
         if (e != cudaSuccess) {                       // not fatal: run this context without graphs from now on
             cudaGetLastError();
-            ctx->gexec[kind] = nullptr; ctx->use_graph = false;
-            enqueue_proof(ctx, pk, mat, kind, true, count);
+            slot.exec = nullptr; ctx->use_graph = false;
+            enqueue(true);
             return;
         }
-        memcpy(ctx->g_key[kind], key, sizeof key);
+        slot.key = std::move(key);
     }
-    CUDA_CHECK(cudaEventRecord(ctx->ev_t[10], s0)); CUDA_CHECK(cudaEventRecord(ctx->ev_t[11], s0));    // phase timers are not part of the graph:
-    for (int i = 0; i < 10; i++) CUDA_CHECK(cudaEventRecord(ctx->ev_t[i], s0));                         // they read as zero
-    CUDA_CHECK(cudaGraphLaunch(ctx->gexec[kind], s0));
-    CUDA_CHECK(cudaEventRecord(ctx->ev_t[14], s0));
-    g_launch_count += ctx->g_launches[kind];
+    if (timers) {
+        CUDA_CHECK(cudaEventRecord(ctx->ev_t[10], s0)); CUDA_CHECK(cudaEventRecord(ctx->ev_t[11], s0));    // phase timers are not part of the graph:
+        for (int i = 0; i < 10; i++) CUDA_CHECK(cudaEventRecord(ctx->ev_t[i], s0));                         // they read as zero
+    }
+    CUDA_CHECK(cudaGraphLaunch(slot.exec, s0));
+    if (timers) CUDA_CHECK(cudaEventRecord(ctx->ev_t[14], s0));
+    g_launch_count += slot.launches;
+}
+
+// kind 0 (G_PROOF) or 1 (G_P2P), as enqueue_proof takes it
+static void run_proof(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, int kind, uint32_t count = 1) {
+    run_graph(ctx, ctx->graphs[kind], {pk->uid, mat->uid, ctx->alloc_gen, count}, true,
+              [&](bool timed) { enqueue_proof(ctx, pk, mat, kind, timed, count); });
 }
 
 static void collect_timings(b2g_ctx* ctx) {
@@ -926,6 +983,38 @@ static void collect_timings(b2g_ctx* ctx) {
     for (int q = 1; q < NQ; q++) ctx->last_ms[2 + q] = el(2 * q, 2 * q + 1);
     ctx->last_ms[7] = el(14, 15);           // glue + d2h
     ctx->last_ms[8] = el(12, 15);           // whole call
+}
+
+// The body of b2g_prove_many and b2g_prove_keys once their arguments are checked: grow() sizes the buffers (an out-of-memory
+// error is reworded to name the call's proofs, and for b2g_prove_keys its n_keys keys), the witnesses are
+// uploaded back to back (witness j: n_vars[key_of[j]] elements, key_of null for one key), (r, s) are staged, run() enqueues
+// the pass, and the count x 256 proof bytes are copied to the pinned slot h_proof.  Nothing here waits for the device.
+// timed: phase timers around the upload.
+template <class Grow, class Run>
+static void prove_pass(b2g_ctx* ctx, uint32_t count, size_t n_keys, bool timed, const void* r_canon, const void* s_canon, const void* const* w_mont,
+                       const uint32_t* n_vars, const uint32_t* key_of, Grow grow, Run run) {
+    try {
+        grow();
+    } catch (const B2gError& e) {
+        if (e.code != B2G_E_DEVICE) throw;
+        cudaGetLastError();
+        throw_error(B2G_E_DEVICE, "the device buffers of " + std::to_string(count) + " proof(s)" +
+                                  (n_keys ? " under " + std::to_string(n_keys) + " key(s)" : std::string()) + " do not fit in device memory" +
+                                  (count > 1 || n_keys ? "; prove fewer per call (" : " (") + e.what() + ")");
+    }
+    cudaStream_t s0 = ctx->st[0];
+    if (timed) CUDA_CHECK(cudaEventRecord(ctx->ev_t[12], s0));
+    size_t at = 0;
+    for (uint32_t j = 0; j < count; j++) {
+        const size_t n = n_vars[key_of ? key_of[j] : 0];
+        CUDA_CHECK(cudaMemcpyAsync(ctx->d_w + at, w_mont[j], n * 32, cudaMemcpyHostToDevice, s0));
+        at += n;
+    }
+    if (timed) CUDA_CHECK(cudaEventRecord(ctx->ev_t[13], s0));
+    stage_rs(ctx, r_canon, s_canon, count);
+    run();
+    ctx->pre_valid = false;
+    CUDA_CHECK(cudaMemcpyAsync(ctx->h_proof, ctx->d_proof, (size_t)count * 256, cudaMemcpyDeviceToHost, s0));
 }
 
 }  // namespace b2g
@@ -991,8 +1080,7 @@ int b2g_ctx_destroy(b2g_ctx* ctx) {
         for (int i = 0; i < NQ; i++) { if (ctx->scratch_ok) msm_scratch_free(ctx->scratch[i]); cudaStreamDestroy(ctx->st[i]); cudaEventDestroy(ctx->ev_done[i]); }
         cudaEventDestroy(ctx->ev_w); cudaEventDestroy(ctx->ev_sort); cudaEventDestroy(ctx->ev_pre); cudaEventDestroy(ctx->ev_fork); cudaEventDestroy(ctx->ev_sortb); cudaStreamDestroy(ctx->st_glue);
         if (ctx->d_wb) cudaFree(ctx->d_wb);
-        for (auto& g : ctx->gexec) if (g) cudaGraphExecDestroy(g);
-        if (ctx->gexec_keys) cudaGraphExecDestroy(ctx->gexec_keys);
+        for (GraphSlot& s : ctx->graphs) if (s.exec) cudaGraphExecDestroy(s.exec);
         if (ctx->d_keyed) cudaFree(ctx->d_keyed);
         if (ctx->h_rs) cudaFreeHost(ctx->h_rs);
         if (ctx->h_proof) cudaFreeHost(ctx->h_proof);
@@ -1020,16 +1108,12 @@ int b2g_pk_load(b2g_ctx* ctx, const b2g_pk_desc* d, b2g_pk** out) {
         } guard;
         b2g_pk* pk = guard.pk;
         pk->device = ctx->device; pk->shard_rank = ctx->shard_rank; pk->shard_count = ctx->shard_count; pk->n_vars = d->n_vars; pk->n_public = d->n_public; pk->domain = d->domain_size;
-        const uint32_t li = d->n_public + 1;
         // query sizes as paired with scalars by create_proof_with_assignment (SURVEY.md 3.4)
-        // L, A, B1, B2 all pair bases with w[1..n_vars): L is re-indexed onto that range by prepending (l - 1) points at
-        // infinity (l_query[j] belongs to w[l + j]), so the four queries share one digit sort per proof.
-        std::vector<uint8_t> l_padded((size_t)(d->n_vars - 1) * 64, 0);
-        if (d->n_vars - li) memcpy(l_padded.data() + (size_t)(li - 1) * 64, d->l_query, (size_t)(d->n_vars - li) * 64);
+        const std::vector<uint8_t> l = l_padded(d);
         const uint32_t total[NQ] = {d->domain_size, d->n_vars - 1, d->n_vars - 1, d->n_vars - 1, d->n_vars - 1};
         const uint32_t base_skip[NQ] = {0, 0, 1, 1, 1};             // query[0] is added separately for A/B1/B2
         const uint32_t soff[NQ] = {0, 1, 1, 1, 1};                  // first scalar: h[0] / w[1]
-        const void* src[NQ] = {d->h_query, l_padded.data(), d->a_query, d->b_g1_query, d->b_g2_query};
+        const void* src[NQ] = {d->h_query, l.data(), d->a_query, d->b_g1_query, d->b_g2_query};
         std::vector<uint32_t> bidx;                                   // real (non-infinity) B bases of this shard, see b2g_pk::d_bidx
         std::vector<uint8_t> bpacked[2];
         for (int q = 0; q < NQ; q++) {
@@ -1044,19 +1128,10 @@ int b2g_pk_load(b2g_ctx* ctx, const b2g_pk_desc* d, b2g_pk** out) {
                 pk->b_compact = (uint32_t)bidx.size();
                 pk->d_bidx = dev_upload<uint32_t>(bidx.data(), bidx.size() * 4, st);
             }
-            if (pk->d_bidx && (q == Q_B1 || q == Q_B2)) {
-                if (pk->b_compact) guard.tmp = dev_upload<uint8_t>(bpacked[g2 ? 1 : 0].data(), (size_t)pk->b_compact * aff, st);
-                msm_build_table(pk->plan[q], guard.tmp, pk->b_compact, g2, st);
-                g_launch_count += 1;
-                CUDA_CHECK(cudaStreamSynchronize(st));
-                if (guard.tmp) { cudaFree(guard.tmp); guard.tmp = nullptr; }
-                continue;
-            }
-            if (pk->cnt[q]) guard.tmp = dev_upload<uint8_t>((const uint8_t*)src[q] + (size_t)(base_skip[q] + pk->lo[q]) * aff, (size_t)pk->cnt[q] * aff, st);
-            msm_build_table(pk->plan[q], guard.tmp, pk->cnt[q], g2, st);
-            g_launch_count += 1;
-            CUDA_CHECK(cudaStreamSynchronize(st));
-            if (guard.tmp) { cudaFree(guard.tmp); guard.tmp = nullptr; }
+            const bool compact = pk->d_bidx && (q == Q_B1 || q == Q_B2);
+            const uint32_t n = compact ? pk->b_compact : pk->cnt[q];
+            const void* bases = compact ? (const void*)bpacked[g2 ? 1 : 0].data() : (const uint8_t*)src[q] + (size_t)(base_skip[q] + pk->lo[q]) * aff;
+            table_from_host(guard.tmp, bases, n, aff, st, [&](const void* b) { msm_build_table(pk->plan[q], b, n, g2, st); g_launch_count += 1; });
         }
         pk_load_glue(pk, d, st);
         guard.pk = nullptr;
@@ -1212,27 +1287,17 @@ static void prove_submit(b2g_ctx* ctx, b2g_pk* pk, b2g_mat* mat, uint32_t count,
         if ((uint64_t)count * p.n * p.nwin >= (1ull << 32) || (uint64_t)count * p.nbuckets >= (1ull << 32))
             throw_error(B2G_E_SHAPE, "b2g_prove_many: count x bases x windows of a query reaches 2^32 sorted entries; prove fewer per call");
     }
-    try {
-        ensure_witness_buffers(ctx, mat->n_vars, mat->n, count);
-        ensure_batch_buffers(ctx, count);
-        ensure_scratch(ctx, pk, count);
-    } catch (const B2gError& e) {
-        if (e.code != B2G_E_DEVICE) throw;
-        cudaGetLastError();
-        throw_error(B2G_E_DEVICE, "the device buffers of " + std::to_string(count) + " proof(s) do not fit in device memory" +
-                                  (count > 1 ? "; prove fewer per call (" : " (") + e.what() + ")");
-    }
-    cudaStream_t s0 = ctx->st[0];
-    CUDA_CHECK(cudaEventRecord(ctx->ev_t[12], s0));
-    for (uint32_t j = 0; j < count; j++)
-        CUDA_CHECK(cudaMemcpyAsync(ctx->d_w + (size_t)j * mat->n_vars, w_mont[j], (size_t)mat->n_vars * 32, cudaMemcpyHostToDevice, s0));
-    CUDA_CHECK(cudaEventRecord(ctx->ev_t[13], s0));
-    stage_rs(ctx, r_canon, s_canon, count);
-    ctx->last_ms[9] = (float)host_ms_since(t0);
-    run_proof(ctx, pk, mat, 0, count);
-    ctx->pre_valid = false;
-    CUDA_CHECK(cudaMemcpyAsync(ctx->h_proof, ctx->d_proof, (size_t)count * 256, cudaMemcpyDeviceToHost, s0));
-    CUDA_CHECK(cudaEventRecord(ctx->ev_t[15], s0));
+    prove_pass(ctx, count, 0, true, r_canon, s_canon, w_mont, &mat->n_vars, nullptr,
+               [&] {
+                   ensure_witness_buffers(ctx, mat->n_vars, mat->n, count);
+                   ensure_batch_buffers(ctx, count);
+                   ensure_scratch(ctx, pk, count);
+               },
+               [&] {
+                   ctx->last_ms[9] = (float)host_ms_since(t0);
+                   run_proof(ctx, pk, mat, 0, count);
+               });
+    CUDA_CHECK(cudaEventRecord(ctx->ev_t[15], ctx->st[0]));
     ctx->pending_out = proofs_out;
     ctx->pending_count = count;
     ctx->last_ms[10] = (float)host_ms_since(t0);
@@ -1728,42 +1793,6 @@ static std::vector<KeyBases> group_bases(const b2g_pk_group* g) {
     return b;
 }
 
-// the context's MSM scratch for a keyed call: every query holds count proofs of the mean base count of its sort (rounded up),
-// at the group's window size; H and L (the W sort) with sort buffers, and B1 (the B sort) when some key's B query is sparse.
-// Without one, B1 and B2 read the W sort as in a one-key proof with a dense B query.
-static void ensure_scratch_keys(b2g_ctx* ctx, const b2g_pk_group* g, const CallLayout& C) {
-    uint32_t navg[NQ];
-    const int sb = g->b_sparse ? S_B : S_W;
-    const int sort_of[NQ] = {S_H, S_W, S_W, sb, sb};
-    for (int q = 0; q < NQ; q++) navg[q] = std::max<uint32_t>(1, (uint32_t)((C.total_n[sort_of[q]] + C.count - 1) / C.count));
-    const size_t nwb = g->b_sparse ? C.total_n[S_B] : 0;
-    bool ok = ctx->scratch_ok && (!g->b_sparse || (ctx->scratch_bsort && nwb <= ctx->cap_wb));
-    for (int q = 0; q < NQ && ok; q++) {
-        const MsmPlan& p = g->plan[q]; const MsmScratch& sc = ctx->scratch[q];
-        if (navg[q] > sc.cap_n || p.nwin > sc.cap_nwin || p.nbuckets > sc.cap_buckets || C.count > sc.cap_count) ok = false;
-    }
-    if (ok) return;
-    CUDA_CHECK(cudaDeviceSynchronize());
-    for (int q = 0; q < NQ; q++) msm_scratch_free(ctx->scratch[q]);
-    ctx->scratch_ok = false; ctx->alloc_gen++;
-    for (int q = 0; q < NQ; q++) {
-        const MsmPlan& p = g->plan[q];
-        msm_scratch_alloc(ctx->scratch[q], navg[q], p.nwin, p.nbuckets, q == Q_B2, q == Q_H || q == Q_L || (q == Q_B1 && g->b_sparse), C.count);
-        cudaFree(ctx->scratch[q].result);
-        ctx->scratch[q].result = ctx->d_partial + PARTIAL_OFF[q];
-        ctx->scratch[q].result_owned = false;
-        ctx->scratch[q].result_stride = REC_BYTES;
-    }
-    ctx->scratch_bsort = g->b_sparse;
-    if (nwb > ctx->cap_wb) {
-        if (ctx->d_wb) cudaFree(ctx->d_wb);
-        ctx->d_wb = nullptr; ctx->cap_wb = 0;
-        CUDA_CHECK(cudaMalloc(&ctx->d_wb, (nwb + 1) * sizeof(fe)));
-        ctx->cap_wb = nwb;
-    }
-    ctx->scratch_ok = true;
-}
-
 // the rows and key_of of a call, in one device buffer the captured pass points into
 static void ensure_keyed_buffer(b2g_ctx* ctx, size_t bytes) {
     if (bytes <= ctx->cap_keyed) return;
@@ -1783,12 +1812,9 @@ static void enqueue_keys(b2g_ctx* ctx, b2g_pk_group* g, const CallLayout& C, con
     const uint32_t count = C.count;
     const KeyedRow* rows = reinterpret_cast<const KeyedRow*>(ctx->d_keyed);
     const uint32_t* key_of = reinterpret_cast<const uint32_t*>(rows + (size_t)NS * count);
-    const Scalar256* rs = reinterpret_cast<const Scalar256*>(ctx->d_rs);
-    CUDA_CHECK(cudaEventRecord(ctx->ev_fork, s0));
-    CUDA_CHECK(cudaStreamWaitEvent(ctx->st_glue, ctx->ev_fork, 0));
-    glue_pre_keys_kernel<<<count, 160, 0, ctx->st_glue>>>(g->d_keys, key_of, rs, ctx->d_pre);
-    CUDA_CHECK(cudaEventRecord(ctx->ev_pre, ctx->st_glue));
-    g_launch_count += 1;
+    fork_glue_pre(ctx, [&](cudaStream_t sg) {
+        glue_pre_keys_kernel<<<count, 160, 0, sg>>>(g->d_keys, key_of, reinterpret_cast<const Scalar256*>(ctx->d_rs), ctx->d_pre);
+    });
     CUDA_CHECK(cudaEventRecord(ctx->ev_w, s0));
     CUDA_CHECK(cudaStreamWaitEvent(ssort, ctx->ev_w, 0));
     msm_sort_keyed(g->plan[Q_A], ctx->scratch[Q_L], ctx->d_w, true, rows + (size_t)S_W * count, count, C.max_n[S_W], C.total_n[S_W], ssort);
@@ -1803,57 +1829,14 @@ static void enqueue_keys(b2g_ctx* ctx, b2g_pk_group* g, const CallLayout& C, con
         msm_sort_keyed(g->plan[Q_B1], ctx->scratch[Q_B1], ctx->d_wb, true, rows + (size_t)S_B * count, count, C.max_n[S_B], C.total_n[S_B], sb);
         CUDA_CHECK(cudaEventRecord(ctx->ev_sortb, sb));
     }
-    for (int q : WITNESS_ORDER) {
-        // with no sparse key, the B queries have the W sort's base counts, window size and arena rows: they read its entries
-        const bool on_b = g->b_sparse && (q == Q_B1 || q == Q_B2);
-        if (on_b) { if (q != Q_B1) CUDA_CHECK(cudaStreamWaitEvent(ctx->st[q], ctx->ev_sortb, 0)); }
-        else if (q != Q_L) CUDA_CHECK(cudaStreamWaitEvent(ctx->st[q], ctx->ev_sort, 0));
-        msm_accumulate(g->plan[q], on_b ? ctx->scratch[Q_B1] : ctx->scratch[Q_L], ctx->scratch[q], ctx->st[q]);
-        if (q == Q_A || q == Q_B1) {
-            scale_partial_kernel<<<count, 32, 0, ctx->st[q]>>>(ctx->d_partial + PARTIAL_OFF[q], q == Q_A ? rs + 1 : rs, ctx->d_partial + B2G_PARTIAL_BYTES + (q == Q_A ? 0 : 128), 2);
-            g_launch_count += 1;
-        }
-        CUDA_CHECK(cudaEventRecord(ctx->ev_done[q], ctx->st[q]));
-    }
+    // with no sparse key, the B queries have the W sort's base counts, window size and arena rows: they read its entries
+    accumulate_witness_queries(ctx, g->plan, g->b_sparse, count, false, true);
     for (size_t k = 0; k < g->keys.size(); k++)
         if (counts[k]) run_witness_map(ctx, g->mats[k], s0, counts[k], C.w_off[k], C.v_off[k]);
     msm_sort_keyed(g->plan[Q_H], ctx->scratch[Q_H], ctx->d_h, true, rows, count, C.max_n[S_H], C.total_n[S_H], s0);
     msm_accumulate(g->plan[Q_H], ctx->scratch[Q_H], ctx->scratch[Q_H], s0);
     for (int q = 1; q < NQ; q++) CUDA_CHECK(cudaStreamWaitEvent(s0, ctx->ev_done[q], 0));
-    CUDA_CHECK(cudaStreamWaitEvent(s0, ctx->ev_pre, 0));
-    glue_post_keys_kernel<<<count, 96, 0, s0>>>(ctx->d_partial, g->d_consts, key_of, ctx->d_pre, ctx->d_proof);
-    g_launch_count += 1;
-    CUDA_CHECK(cudaGetLastError());
-}
-
-// replays the keyed pass captured for (group, buffer generation, counts), capturing it first, as run_proof does for one key
-static void run_keys(b2g_ctx* ctx, b2g_pk_group* g, const CallLayout& C, const uint32_t* counts) {
-    cudaStream_t s0 = ctx->st[0];
-    if (!ctx->use_graph) { enqueue_keys(ctx, g, C, counts); return; }
-    std::vector<uint64_t> key = {g->uid, ctx->alloc_gen};
-    key.insert(key.end(), counts, counts + g->keys.size());
-    if (ctx->gexec_keys && ctx->gk_key != key) { cudaGraphExecDestroy(ctx->gexec_keys); ctx->gexec_keys = nullptr; }
-    if (!ctx->gexec_keys) {
-        const uint64_t before = g_launch_count.load();
-        cudaGraph_t graph = nullptr;
-        CUDA_CHECK(cudaStreamBeginCapture(s0, cudaStreamCaptureModeThreadLocal));
-        try { enqueue_keys(ctx, g, C, counts); }
-        catch (...) { cudaStreamEndCapture(s0, &graph); if (graph) cudaGraphDestroy(graph); cudaGetLastError(); g_launch_count = before; throw; }
-        cudaError_t e = cudaStreamEndCapture(s0, &graph);
-        if (e == cudaSuccess) e = cudaGraphInstantiate(&ctx->gexec_keys, graph, 0);
-        if (graph) cudaGraphDestroy(graph);
-        ctx->gk_launches = g_launch_count.load() - before;
-        g_launch_count = before;
-        if (e != cudaSuccess) {                       // not fatal: run this context without graphs from now on
-            cudaGetLastError();
-            ctx->gexec_keys = nullptr; ctx->use_graph = false;
-            enqueue_keys(ctx, g, C, counts);
-            return;
-        }
-        ctx->gk_key = key;
-    }
-    CUDA_CHECK(cudaGraphLaunch(ctx->gexec_keys, s0));
-    g_launch_count += ctx->gk_launches;
+    join_glue_post(ctx, s0, [&] { glue_post_keys_kernel<<<count, 96, 0, s0>>>(ctx->d_partial, g->d_consts, key_of, ctx->d_pre, ctx->d_proof); });
 }
 
 }  // namespace b2g
@@ -1915,12 +1898,10 @@ int b2g_pk_group_load(b2g_ctx* ctx, uint32_t n_keys, const b2g_pk_desc* pks, b2g
             b2g_pk* pk = new b2g_pk();
             g->keys.push_back(pk);
             pk->device = ctx->device; pk->n_vars = d->n_vars; pk->n_public = d->n_public; pk->domain = d->domain_size;
-            const uint32_t li = d->n_public + 1;
             try {
-                // the bases of each query as b2g_pk_load pairs them with scalars, L re-indexed onto w[1..]
-                std::vector<uint8_t> l_padded((size_t)(d->n_vars - 1) * 64, 0);
-                if (d->n_vars - li) memcpy(l_padded.data() + (size_t)(li - 1) * 64, d->l_query, (size_t)(d->n_vars - li) * 64);
-                const void* src[NQ] = {d->h_query, l_padded.data(), (const uint8_t*)d->a_query + 64,
+                // the bases of each query as b2g_pk_load pairs them with scalars
+                const std::vector<uint8_t> l = l_padded(d);
+                const void* src[NQ] = {d->h_query, l.data(), (const uint8_t*)d->a_query + 64,
                                        sparse[k] ? (const void*)bpacked[k][0].data() : (const uint8_t*)d->b_g1_query + 64,
                                        sparse[k] ? (const void*)bpacked[k][1].data() : (const uint8_t*)d->b_g2_query + 128};
                 for (int q = 0; q < NQ; q++) {
@@ -1929,10 +1910,9 @@ int b2g_pk_group_load(b2g_ctx* ctx, uint32_t n_keys, const b2g_pk_desc* pks, b2g
                     pk->scalar_off[q] = q == Q_H ? 0 : 1;
                     if (!bases[k][q]) continue;
                     const size_t aff = q == Q_B2 ? 128 : 64;
-                    guard.tmp = dev_upload<uint8_t>(src[q], (size_t)bases[k][q] * aff, st);
-                    msm_build_table_into((uint8_t*)g->plan[q].table + (size_t)L.row[q][k] * aff, guard.tmp, bases[k][q], L.c[q], q == Q_B2, st);
-                    CUDA_CHECK(cudaStreamSynchronize(st));
-                    cudaFree(guard.tmp); guard.tmp = nullptr;
+                    table_from_host(guard.tmp, src[q], bases[k][q], aff, st, [&](const void* b) {
+                        msm_build_table_into((uint8_t*)g->plan[q].table + (size_t)L.row[q][k] * aff, b, bases[k][q], L.c[q], q == Q_B2, st);
+                    });
                 }
                 if (sparse[k]) {
                     pk->b_compact = bases[k][Q_B1];
@@ -1978,31 +1958,28 @@ int b2g_prove_keys(b2g_ctx* ctx, b2g_pk_group* g, const uint32_t* counts, const 
         for (uint32_t j = 0; j < C.count; j++) if (!w_mont[j]) throw_error(B2G_E_SHAPE, "null witness " + std::to_string(j));
         DevGuard dg(ctx->device);
         const size_t table_bytes = C.rows.size() * sizeof(KeyedRow) + C.key_of.size() * 4;
-        try {
-            ensure_witness_buffers(ctx, C.total_w, C.total_v);
-            ensure_batch_buffers(ctx, C.count);
-            ensure_scratch_keys(ctx, g, C);
-            ensure_keyed_buffer(ctx, table_bytes);
-        } catch (const B2gError& e) {
-            if (e.code != B2G_E_DEVICE) throw;
-            cudaGetLastError();
-            throw_error(B2G_E_DEVICE, "the device buffers of " + std::to_string(C.count) + " proof(s) under " + std::to_string(g->keys.size()) +
-                                      " key(s) do not fit in device memory; prove fewer per call (" + e.what() + ")");
-        }
-        cudaStream_t s0 = ctx->st[0];
-        for (uint32_t j = 0; j < C.count; j++) {
-            const size_t k = C.key_of[j];
-            CUDA_CHECK(cudaMemcpyAsync(ctx->d_w + C.rows[(size_t)S_W * C.count + j].src - 1, w_mont[j], (size_t)n_vars[k] * 32, cudaMemcpyHostToDevice, s0));
-        }
-        std::vector<uint8_t> table(table_bytes);
-        memcpy(table.data(), C.rows.data(), C.rows.size() * sizeof(KeyedRow));
-        memcpy(table.data() + C.rows.size() * sizeof(KeyedRow), C.key_of.data(), C.key_of.size() * 4);
-        CUDA_CHECK(cudaMemcpyAsync(ctx->d_keyed, table.data(), table_bytes, cudaMemcpyHostToDevice, s0));
-        stage_rs(ctx, r_canon, s_canon, C.count);
-        run_keys(ctx, g, C, counts);
-        ctx->pre_valid = false;
-        CUDA_CHECK(cudaMemcpyAsync(ctx->h_proof, ctx->d_proof, (size_t)C.count * 256, cudaMemcpyDeviceToHost, s0));
-        CUDA_CHECK(cudaStreamSynchronize(s0));
+        prove_pass(ctx, C.count, g->keys.size(), false, r_canon, s_canon, w_mont, n_vars.data(), C.key_of.data(),
+                   [&] {
+                       // every query holds count proofs of the mean base count of its sort (rounded up), at the group's window size
+                       const int sb = g->b_sparse ? S_B : S_W;
+                       const int sort_of[NQ] = {S_H, S_W, S_W, sb, sb};
+                       uint32_t navg[NQ];
+                       for (int q = 0; q < NQ; q++) navg[q] = std::max<uint32_t>(1, (uint32_t)((C.total_n[sort_of[q]] + C.count - 1) / C.count));
+                       ensure_witness_buffers(ctx, C.total_w, C.total_v);
+                       ensure_batch_buffers(ctx, C.count);
+                       ensure_scratch(ctx, g->plan, navg, C.count, g->b_sparse, g->b_sparse ? C.total_n[S_B] : 0);
+                       ensure_keyed_buffer(ctx, table_bytes);
+                   },
+                   [&] {
+                       std::vector<uint8_t> table(table_bytes);
+                       memcpy(table.data(), C.rows.data(), C.rows.size() * sizeof(KeyedRow));
+                       memcpy(table.data() + C.rows.size() * sizeof(KeyedRow), C.key_of.data(), C.key_of.size() * 4);
+                       CUDA_CHECK(cudaMemcpyAsync(ctx->d_keyed, table.data(), table_bytes, cudaMemcpyHostToDevice, ctx->st[0]));
+                       std::vector<uint64_t> key = {g->uid, ctx->alloc_gen};
+                       key.insert(key.end(), counts, counts + g->keys.size());
+                       run_graph(ctx, ctx->graphs[G_KEYS], std::move(key), false, [&](bool) { enqueue_keys(ctx, g, C, counts); });
+                   });
+        CUDA_CHECK(cudaStreamSynchronize(ctx->st[0]));
         memcpy(proofs_out, ctx->h_proof, (size_t)C.count * 256);
     });
 }

@@ -602,6 +602,16 @@ def _scalar_bytes(v) -> np.ndarray:
     return a
 
 
+def _prove_inputs(n_vars: int, rs, assignments, what: str = ''):
+    """the witnesses of a prove call as contiguous arrays and its (r, s) as canonical limbs, r and s of every proof side by
+    side; a witness of another length than n_vars raises ValueError (prefixed with `what`)"""
+    ws = [_c(w) for w in assignments]
+    for w in ws:
+        if w.size // 4 != n_vars:
+            raise ValueError(what + "full_assignment length != n_vars")
+    return ws, [_scalar_bytes(r) for r, _ in rs], [_scalar_bytes(s) for _, s in rs]
+
+
 def fr_rand(rng) -> int:
     """Fr::rand of ark-ff 0.5 (SURVEY.md App. C.5), the rule Groth16::prove uses for r and s: four u64 limbs from the rng
     (limb 0 first), the top two bits of limb 3 cleared, rejected and redrawn if >= r, and the limbs taken AS the Montgomery
@@ -742,11 +752,8 @@ class Groth16:
         ctx = ctx or default_context()
         if num_inputs != matrices.num_instance_variables or num_constraints != matrices.num_constraints:
             raise ValueError("num_inputs / num_constraints disagree with the matrices")
-        w = _c(full_assignment)
-        if w.size // 4 != pk.n_vars:
-            raise ValueError("full_assignment length != n_vars")
+        (w,), (rr,), (ss,) = _prove_inputs(pk.n_vars, [(r, s)], [full_assignment])
         ph, mh = ctx.pk_handle(pk), ctx.mat_handle(matrices, pk.n_vars, reduction.ID)
-        rr, ss = _scalar_bytes(r), _scalar_bytes(s)
         out = np.zeros(256, dtype=np.uint8)
         N.check(N.lib().b2g_prove(ctx._h, ph, mh, _ptr(rr), _ptr(ss), _ptr(w), _ptr(out)))
         return Proof(out.tobytes())
@@ -763,13 +770,9 @@ class Groth16:
             raise ValueError("create_proofs: one (r, s) per assignment")
         if not assignments:
             return []
-        ws = [_c(w) for w in assignments]
-        for w in ws:
-            if w.size // 4 != pk.n_vars:
-                raise ValueError("full_assignment length != n_vars")
+        ws, rr, ss = _prove_inputs(pk.n_vars, rs, assignments)
         ph, mh = ctx.pk_handle(pk), ctx.mat_handle(matrices, pk.n_vars, reduction.ID)
-        rr = np.concatenate([_scalar_bytes(r) for r, _ in rs])
-        ss = np.concatenate([_scalar_bytes(s) for _, s in rs])
+        rr, ss = np.concatenate(rr), np.concatenate(ss)
         ptrs = (C.c_void_p * len(ws))(*[w.ctypes.data for w in ws])
         out = np.zeros((len(ws), 256), dtype=np.uint8)
         N.check(N.lib().b2g_prove_many(ctx._h, ph, mh, len(ws), _ptr(rr), _ptr(ss), ptrs, _ptr(out)))
@@ -822,13 +825,10 @@ class Groth16:
         for k, ((rs, assignments), (pk, _, _)) in enumerate(zip(batches, group.keys)):
             if len(rs) != len(assignments):
                 raise ValueError(f"create_proofs_keys: key {k}: one (r, s) per assignment")
-            for w in assignments:
-                w = _c(w)
-                if w.size // 4 != pk.n_vars:
-                    raise ValueError(f"create_proofs_keys: key {k}: full_assignment length != n_vars")
-                ws.append(w)
-            rr += [_scalar_bytes(r) for r, _ in rs]
-            ss += [_scalar_bytes(s) for _, s in rs]
+            kw, kr, ks = _prove_inputs(pk.n_vars, rs, assignments, f"create_proofs_keys: key {k}: ")
+            ws += kw
+            rr += kr
+            ss += ks
             counts.append(len(assignments))
         if not ws:
             return [[] for _ in batches]
@@ -847,11 +847,8 @@ class Groth16:
     def submit(pk: ProvingKey, r, s, matrices: ConstraintMatrices, full_assignment, ctx: Context, reduction=CircomReduction) -> 'PendingProof':
         """create_proof_with_reduction_and_matrices without the wait: enqueues the proof on `ctx` (one pending proof per
         context) and returns a handle whose .wait() yields the Proof.  One host thread + K contexts = K proofs in flight."""
-        w = _c(full_assignment)
-        if w.size // 4 != pk.n_vars:
-            raise ValueError("full_assignment length != n_vars")
+        (w,), (rr,), (ss,) = _prove_inputs(pk.n_vars, [(r, s)], [full_assignment])
         ph, mh = ctx.pk_handle(pk), ctx.mat_handle(matrices, pk.n_vars, reduction.ID)
-        rr, ss = _scalar_bytes(r), _scalar_bytes(s)
         out = np.zeros(256, dtype=np.uint8)
         N.check(N.lib().b2g_prove_submit(ctx._h, ph, mh, _ptr(rr), _ptr(ss), _ptr(w), _ptr(out)))
         return PendingProof(ctx, out, w)

@@ -1062,15 +1062,26 @@ struct Groth16T {                                       // Groth16::<Bn254, QAP>
         if (!p) throw SerializationError("rerandomize_proof: the proof is malformed (a coordinate >= p or a point off its curve)");
         return *p;
     }
+    // the inputs of a prove call, one proof at a time: (r, s) as canonical integers and the witness; a witness of another
+    // length than n_vars throws AssignmentMissing
+    struct ProveInputs {
+        std::vector<BigInt256> r, s;
+        std::vector<const void*> w;
+        void add(size_t n_vars, const std::pair<Fr, Fr>& rs, const std::vector<Fr>& assignment) {
+            if (assignment.size() != n_vars) throw SynthesisError("AssignmentMissing: full_assignment length != n_vars");
+            r.push_back(rs.first.into_bigint()); s.push_back(rs.second.into_bigint());
+            w.push_back(assignment.data());
+        }
+    };
     static Proof create_proof_with_reduction_and_matrices(const ProvingKey& pk, const Fr& r, const Fr& s, const ConstraintMatrices& matrices,
                                                           size_t num_inputs, size_t num_constraints, const std::vector<Fr>& full_assignment,
                                                           Gpu& gpu = Gpu::instance()) {
         if (num_inputs != matrices.num_instance_variables || num_constraints != matrices.num_constraints)
             throw SynthesisError("num_inputs / num_constraints disagree with the matrices");
-        if (full_assignment.size() != pk.a_query.size()) throw SynthesisError("AssignmentMissing: full_assignment length != n_vars");
-        BigInt256 rb = r.into_bigint(), sb = s.into_bigint();
+        ProveInputs in;
+        in.add(pk.a_query.size(), {r, s}, full_assignment);
         Proof p;
-        check(b2g_prove(gpu.ctx(), gpu.pk(pk), gpu.mat(matrices, full_assignment.size(), QAP::ID), rb.l, sb.l, full_assignment.data(), p.bytes));
+        check(b2g_prove(gpu.ctx(), gpu.pk(pk), gpu.mat(matrices, full_assignment.size(), QAP::ID), in.r[0].l, in.s[0].l, full_assignment.data(), p.bytes));
         return p;
     }
 
@@ -1086,15 +1097,14 @@ struct Groth16T {                                       // Groth16::<Bn254, QAP>
         std::vector<std::unique_ptr<Gpu>> gpus;
         for (int k = 0; k < inflight && (size_t)k < n; k++) gpus.emplace_back(new Gpu(device));
         std::vector<Proof> out(n);
-        std::vector<BigInt256> rb(n), sb(n);
+        ProveInputs in;
         for (size_t i = 0; i < n; i++) {
-            if (assignments[i]->size() != pk.a_query.size()) throw SynthesisError("AssignmentMissing: full_assignment length != n_vars");
-            rb[i] = rs[i].first.into_bigint(); sb[i] = rs[i].second.into_bigint();
+            in.add(pk.a_query.size(), rs[i], *assignments[i]);
             check(b2g_host_register(assignments[i]->data(), assignments[i]->size() * sizeof(Fr)));
         }
         auto submit = [&](size_t i) {
             Gpu& g = *gpus[i % gpus.size()];
-            check(b2g_prove_submit(g.ctx(), g.pk(pk), g.mat(matrices, assignments[i]->size(), QAP::ID), rb[i].l, sb[i].l, assignments[i]->data(), out[i].bytes));
+            check(b2g_prove_submit(g.ctx(), g.pk(pk), g.mat(matrices, assignments[i]->size(), QAP::ID), in.r[i].l, in.s[i].l, assignments[i]->data(), out[i].bytes));
         };
         size_t submitted = 0;
         try {
@@ -1121,16 +1131,11 @@ struct Groth16T {                                       // Groth16::<Bn254, QAP>
         if (rs.size() != assignments.size()) throw SynthesisError("create_proofs: one (r, s) per assignment");
         const size_t n = rs.size();
         if (n == 0) return {};
-        std::vector<BigInt256> rb(n), sb(n);
-        std::vector<const void*> ws(n);
-        for (size_t i = 0; i < n; i++) {
-            if (assignments[i]->size() != pk.a_query.size()) throw SynthesisError("AssignmentMissing: full_assignment length != n_vars");
-            rb[i] = rs[i].first.into_bigint(); sb[i] = rs[i].second.into_bigint();
-            ws[i] = assignments[i]->data();
-        }
+        ProveInputs in;
+        for (size_t i = 0; i < n; i++) in.add(pk.a_query.size(), rs[i], *assignments[i]);
         std::vector<Proof> out(n);
         std::vector<uint8_t> bytes(n * 256);
-        check(b2g_prove_many(gpu.ctx(), gpu.pk(pk), gpu.mat(matrices, pk.a_query.size(), QAP::ID), (uint32_t)n, rb.data(), sb.data(), ws.data(), bytes.data()));
+        check(b2g_prove_many(gpu.ctx(), gpu.pk(pk), gpu.mat(matrices, pk.a_query.size(), QAP::ID), (uint32_t)n, in.r.data(), in.s.data(), in.w.data(), bytes.data()));
         for (size_t i = 0; i < n; i++) memcpy(out[i].bytes, bytes.data() + 256 * i, 256);
         return out;
     }
@@ -1159,22 +1164,17 @@ struct Groth16T {                                       // Groth16::<Bn254, QAP>
                                                               Gpu& gpu = Gpu::instance()) {
         if (batches.size() != group.n_keys()) throw SynthesisError("create_proofs_keys: one batch per key of the group");
         std::vector<uint32_t> counts;
-        std::vector<BigInt256> rb, sb;
-        std::vector<const void*> ws;
+        ProveInputs in;
         for (size_t k = 0; k < batches.size(); k++) {
             const auto& b = batches[k];
             if (b.first.size() != b.second.size()) throw SynthesisError("create_proofs_keys: one (r, s) per assignment");
-            for (size_t i = 0; i < b.first.size(); i++) {
-                if (b.second[i]->size() != group.n_vars(k)) throw SynthesisError("AssignmentMissing: full_assignment length != n_vars");
-                rb.push_back(b.first[i].first.into_bigint()); sb.push_back(b.first[i].second.into_bigint());
-                ws.push_back(b.second[i]->data());
-            }
+            for (size_t i = 0; i < b.first.size(); i++) in.add(group.n_vars(k), b.first[i], *b.second[i]);
             counts.push_back((uint32_t)b.first.size());
         }
         std::vector<std::vector<Proof>> out(batches.size());
-        if (ws.empty()) return out;
-        std::vector<uint8_t> bytes(ws.size() * 256);
-        check(b2g_prove_keys(gpu.ctx(), group.handle(), counts.data(), rb.data(), sb.data(), ws.data(), bytes.data()));
+        if (in.w.empty()) return out;
+        std::vector<uint8_t> bytes(in.w.size() * 256);
+        check(b2g_prove_keys(gpu.ctx(), group.handle(), counts.data(), in.r.data(), in.s.data(), in.w.data(), bytes.data()));
         size_t at = 0;
         for (size_t k = 0; k < batches.size(); k++) {
             out[k].resize(counts[k]);

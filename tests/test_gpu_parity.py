@@ -492,19 +492,36 @@ def test_sharded_proof_equals_whole_proof(golden, complex_zkey_bytes):
         cx.close()
 
 
-def test_error_behaviour(ctx, test_zkey_bytes):
-    from circom_compat_b200 import read_zkey, Groth16, fr_to_mont, B2gError
+def test_error_behaviour(ctx, test_zkey_bytes, complex_zkey_bytes):
+    from circom_compat_b200 import read_zkey, Groth16, fr_to_mont, B2gError, _native as N
+    import ctypes as C
     pk, cm = read_zkey(test_zkey_bytes)
-    with pytest.raises(ValueError):
+    with pytest.raises(ValueError) as v:
         Groth16.create_proof_with_reduction_and_matrices(pk, 1, 1, cm, cm.num_instance_variables, cm.num_constraints, fr_to_mont([1, 2, 3]), ctx)
+    assert str(v.value) == "full_assignment length != n_vars"
     with pytest.raises(B2gError) as e:
         ctx.test_op(99, np.zeros((1, 4), dtype=np.uint64))            # unknown op: B2G_E_SHAPE, nothing launched
-    assert e.value.code == -2
+    assert e.value.code == -2 and e.value.msg == "bad arguments"
+    # b2g_prove: null pointers, and a key with another circuit's matrices
+    L = N.lib()
+    w = fr_to_mont([1, 33, 3, 11])
+    rr = np.zeros(4, dtype=np.uint64)
+    out = np.zeros(256, dtype=np.uint8)
+    pkc, cmc = read_zkey(complex_zkey_bytes)
+    ph, mh, mhc = ctx.pk_handle(pk), ctx.mat_handle(cm, pk.n_vars), ctx.mat_handle(cmc, pkc.n_vars)
+    assert L.b2g_prove(ctx._h, ph, mh, None, rr.ctypes.data, w.ctypes.data, out.ctypes.data) == N.B2G_E_SHAPE
+    assert L.b2g_last_error().decode() == "null pointer"
+    assert L.b2g_prove(ctx._h, ph, mh, rr.ctypes.data, rr.ctypes.data, None, out.ctypes.data) == N.B2G_E_SHAPE
+    assert L.b2g_last_error().decode() == "null witness 0"
+    assert L.b2g_prove(ctx._h, ph, mhc, rr.ctypes.data, rr.ctypes.data, w.ctypes.data, out.ctypes.data) == N.B2G_E_SHAPE
+    assert L.b2g_last_error().decode() == "proving key and matrices disagree on n_vars"
     # a sharded context refuses the whole-proof entry point, a whole context refuses foreign shards' keys
     from circom_compat_b200 import Context
     cx = Context(0, 0, 2)
-    with pytest.raises(B2gError):
-        Groth16.create_proof_with_reduction_and_matrices(pk, 1, 1, cm, cm.num_instance_variables, cm.num_constraints, fr_to_mont([1, 33, 3, 11]), cx)
+    with pytest.raises(B2gError) as e:
+        Groth16.create_proof_with_reduction_and_matrices(pk, 1, 1, cm, cm.num_instance_variables, cm.num_constraints, w, cx)
+    assert e.value.code == N.B2G_E_SHAPE
+    assert e.value.msg == "a whole proof (b2g_prove, b2g_prove_many) needs an unsharded context; use b2g_prove_partial/finish"
     cx.close()
     # domain limit: next_pow2(num_constraints + num_inputs) must leave room for the doubled domain (qap.rs:31,63-66)
     from circom_compat_b200 import PolynomialDegreeTooLarge, ConstraintMatrices

@@ -262,12 +262,20 @@ def test_refusals_leave_the_context_usable(ctx, keys):
     mats = (C.c_void_p * 2)(ctx.mat_handle(keys['c10'].cm, keys['c10'].pk.n_vars).value, ctx.mat_handle(keys['c12'].cm, keys['c12'].pk.n_vars).value)
     h = C.c_void_p()
     assert L.b2g_pk_group_load(ctx._h, 2, descs, mats, C.byref(h)) == N.B2G_E_SHAPE
-    msg = L.b2g_last_error().decode()
-    assert 'key 1: proving key and matrices disagree on n_vars' in msg and not h.value
+    def last():
+        return L.b2g_last_error().decode()
+
+    assert last() == "b2g_pk_group_load: key 1: proving key and matrices disagree on n_vars" and not h.value
     good()
-    # an empty group
+    # an empty group, null pointers, a sharded context
     assert L.b2g_pk_group_load(ctx._h, 0, None, None, C.byref(h)) == N.B2G_E_SHAPE
-    assert 'no keys' in L.b2g_last_error().decode()
+    assert last() == "b2g_pk_group_load: the group has no keys"
+    assert L.b2g_pk_group_load(ctx._h, 2, None, mats, C.byref(h)) == N.B2G_E_SHAPE
+    assert last() == "null pointer"
+    sharded = Context(0, 0, 2)
+    assert L.b2g_pk_group_load(sharded._h, 2, descs, mats, C.byref(h)) == N.B2G_E_SHAPE
+    assert last() == "b2g_pk_group_load: a key group needs an unsharded context"
+    sharded.close()
     with pytest.raises(ValueError):
         Groth16.load_proving_keys([], ctx)
     g = Groth16.load_proving_keys([(k.pk, k.cm, k.red) for k in ks], ctx)
@@ -281,28 +289,35 @@ def test_refusals_leave_the_context_usable(ctx, keys):
 
     try:
         one = (C.c_void_p * 1)(w.ctypes.data)
+        cnt = np.array([1, 0], dtype=np.uint32)
+        assert L.b2g_prove_keys(ctx._h, g._h, None, rr.ctypes.data, rr.ctypes.data, one, out.ctypes.data) == N.B2G_E_SHAPE
+        assert last() == "null pointer"
+        assert L.b2g_prove_keys(ctx._h, g._h, cnt.ctypes.data, rr.ctypes.data, None, one, out.ctypes.data) == N.B2G_E_SHAPE
+        assert last() == "null pointer"
         assert call(ctx, [0, 0], one) == N.B2G_E_SHAPE
-        assert 'total count must be in [1, 65535]' in L.b2g_last_error().decode()
+        assert last() == "b2g_prove_keys: the total count must be in [1, 65535]"
         many = (C.c_void_p * 65536)(*([w.ctypes.data] * 65536))
         assert call(ctx, [65535, 1], many) == N.B2G_E_SHAPE
-        assert 'total count must be in [1, 65535]' in L.b2g_last_error().decode()
+        assert last() == "b2g_prove_keys: the total count must be in [1, 65535]"
         assert call(ctx, [2, 0], (C.c_void_p * 2)(w.ctypes.data, None)) == N.B2G_E_SHAPE
-        assert 'null witness 1' in L.b2g_last_error().decode()
+        assert last() == "null witness 1"
         good()
         sharded = Context(0, 0, 2)
         assert call(sharded, [1, 0], one) == N.B2G_E_SHAPE
-        assert 'unsharded' in L.b2g_last_error().decode()
+        assert last() == "b2g_prove_keys needs an unsharded context"
         sharded.close()
         k = keys['bench']
         pending = Groth16.submit(k.pk, 1, 2, k.cm, k.ws[0], ctx)
         with pytest.raises(B2gError) as e:
             Groth16.create_proofs_keys(g, [([(1, 2)], [w]), ([], [])], ctx)
-        assert e.value.code == N.B2G_E_SHAPE and 'pending' in e.value.msg
+        assert e.value.code == N.B2G_E_SHAPE
+        assert e.value.msg == "a submitted proof is still pending on this context: call b2g_prove_wait first"
         assert pending.wait().data == _expect(ctx, k, [(1, 2)], [k.ws[0]])[0]
         with pytest.raises(ValueError):
             Groth16.create_proofs_keys(g, [([(1, 2)], [w])], ctx)       # one batch per key
-        with pytest.raises(ValueError):
+        with pytest.raises(ValueError) as v:
             Groth16.create_proofs_keys(g, [([(1, 2)], [w]), ([(1, 2)], [w])], ctx)   # a witness of the wrong length
+        assert str(v.value) == "create_proofs_keys: key 1: full_assignment length != n_vars"
         assert Groth16.create_proofs_keys(g, [([], []), ([], [])], ctx) == [[], []]
         good()
     finally:
@@ -412,12 +427,13 @@ def test_layout_refuses_2p32_entries():
             with pytest.raises(M.Refused):
                 M.call_layout(cs, rows, *args[:1], *args[1:])
             rc, msg = _layout(*args)
-            assert rc == N.B2G_E_SHAPE and '2^32 sorted entries' in msg
+            assert rc == N.B2G_E_SHAPE
+            assert msg == "b2g_prove_keys: proofs x bases x windows of query H reach 2^32 sorted entries; prove fewer per call"
     for counts in ([0, 0], [65535, 1]):
         rc, msg = _layout(bases, [10002, 4096], [1 << 14, 1 << 12], counts)
-        assert rc == N.B2G_E_SHAPE and 'total count must be in [1, 65535]' in msg
+        assert rc == N.B2G_E_SHAPE and msg == "b2g_prove_keys: the total count must be in [1, 65535]"
     rc, msg = _layout([])
-    assert rc == N.B2G_E_SHAPE and 'no keys' in msg
+    assert rc == N.B2G_E_SHAPE and msg == "b2g_pk_group_load: the group has no keys"
 
 
 def test_prove_keys_is_exported_and_declared():

@@ -260,16 +260,32 @@ def test_errors_leave_the_context_usable(ctx, golden, complex_key, chain_witness
         out = np.zeros(256 * max(count, 1), dtype=np.uint8)
         return L.b2g_prove_many(cx_h, ph, mh, count, rr.ctypes.data, rr.ctypes.data, ptrs, out.ctypes.data)
 
+    def last():
+        return L.b2g_last_error().decode()
+
     one = (C.c_void_p * 1)(w.ctypes.data)
-    assert call(ctx._h, 0, one) == N.B2G_E_SHAPE
+    rr = np.zeros(4, dtype=np.uint64)
+    out = np.zeros(256, dtype=np.uint8)
+    assert L.b2g_prove_many(ctx._h, ph, mh, 1, None, rr.ctypes.data, one, out.ctypes.data) == N.B2G_E_SHAPE
+    assert last() == "null pointer"
+    assert L.b2g_prove_many(ctx._h, ph, mh, 1, rr.ctypes.data, rr.ctypes.data, None, out.ctypes.data) == N.B2G_E_SHAPE
+    assert last() == "null pointer"
+    for count in (0, 65536):
+        assert call(ctx._h, count, one) == N.B2G_E_SHAPE
+        assert last() == "b2g_prove_many: count must be in [1, 65535]"
     assert call(ctx._h, 2, (C.c_void_p * 2)(w.ctypes.data, None)) == N.B2G_E_SHAPE
-    assert 'null witness 1' in L.b2g_last_error().decode()
+    assert last() == "null witness 1"
+    from circom_compat_b200 import Groth16
     sharded = Context(0, 0, 2)
     with pytest.raises(B2gError) as e:
-        from circom_compat_b200 import Groth16
         Groth16.create_proofs(pk, [(1, 2)], cm, [w], sharded)
     assert e.value.code == N.B2G_E_SHAPE
+    assert e.value.msg == "a whole proof (b2g_prove, b2g_prove_many) needs an unsharded context; use b2g_prove_partial/finish"
     sharded.close()
+    pending = Groth16.submit(pk, int(g['r']), int(g['s']), cm, w, ctx)
+    assert call(ctx._h, 1, one) == N.B2G_E_SHAPE
+    assert last() == "a submitted proof is still pending on this context: call b2g_prove_wait first"
+    assert pending.wait().data.hex() == g['proof_hex']
     # a count at which the witness queries (n_vars - 1 bases each) reach 2^32 sorted entries
     n = pk.n_vars - 1
     c = _pick_c(n)
@@ -278,7 +294,7 @@ def test_errors_leave_the_context_usable(ctx, golden, complex_key, chain_witness
     assert count <= 65535
     many = (C.c_void_p * count)(*([w.ctypes.data] * count))
     assert call(ctx._h, count, many) == N.B2G_E_SHAPE
-    assert '2^32' in L.b2g_last_error().decode()
+    assert last() == "b2g_prove_many: count x bases x windows of a query reaches 2^32 sorted entries; prove fewer per call"
     p = _many(pk, cm, [(int(g['r']), int(g['s']))] * 2, [w, w], ctx)
     assert p[0].hex() == g['proof_hex'] and p[1] == p[0]
 
