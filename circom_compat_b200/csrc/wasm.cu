@@ -1147,12 +1147,13 @@ int b2g_witness_calculate(b2g_ctx* ctx, b2g_wasm* w, uint32_t count, uint32_t n_
     return guarded_clear([&] {
         if (!ctx || !w || (n_inputs && (!hashes || !counts)) || (count && (!w_mont_out || !status_out))) throw_error(B2G_E_SHAPE, "null pointer");
         if (!w->circom) throw_error(B2G_E_SHAPE, "wasm: the module was not loaded as a circom 2 witness calculator (b2g_wasm_load)");
-        std::vector<uint3> meta;
+        uint64_t n_values = 0;
         for (uint32_t k = 0; k < n_inputs; k++)
-            for (uint32_t i = 0; i < counts[k]; i++) {
-                meta.push_back(make_uint3((uint32_t)(hashes[k] >> 32), (uint32_t)hashes[k], i));
-                if (meta.size() > (1u << 24)) throw_error(B2G_E_SHAPE, "too many input values");
-            }
+            if ((n_values += counts[k]) > (1u << 24)) throw_error(B2G_E_SHAPE, "too many input values");
+        std::vector<uint3> meta;
+        meta.reserve(n_values);
+        for (uint32_t k = 0; k < n_inputs; k++)
+            for (uint32_t i = 0; i < counts[k]; i++) meta.push_back(make_uint3((uint32_t)(hashes[k] >> 32), (uint32_t)hashes[k], i));
         const uint32_t nv = (uint32_t)meta.size();
         if (count == 0) return;
         if (nv && !values_canon) throw_error(B2G_E_SHAPE, "null pointer");

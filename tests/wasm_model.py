@@ -7,7 +7,8 @@ yardstick the device interpreter is tested against, one witness at a time.
 
 Lane statuses (the same numbers b2g_witness_calculate writes):
     0 ok, 1 unreachable, 2 memory access out of bounds, 3 integer division by zero, 4 integer overflow,
-    5 call stack exhausted, 6 fuel exhausted, 7 bad call_indirect, 0x100 + c the circuit called exceptionHandler(c)
+    5 call stack exhausted, 6 fuel exhausted, 7 bad call_indirect, 8 getWitnessSize after the inputs disagrees with
+    the size the module reported before init, 0x100 + c the circuit called exceptionHandler(c)
 """
 from __future__ import annotations
 
@@ -15,13 +16,13 @@ R_MOD = 218882428718392752222464057452572750885483644004160343436982041865758084
 PAGE = 65536
 M32, M64 = (1 << 32) - 1, (1 << 64) - 1
 
-OK, UNREACHABLE, MEMORY, DIV_ZERO, OVERFLOW, STACK, FUEL, INDIRECT = range(8)
+OK, UNREACHABLE, MEMORY, DIV_ZERO, OVERFLOW, STACK, FUEL, INDIRECT, PROTOCOL = range(9)
 EXCEPTION = 0x100
 
 RUNTIME_IMPORTS = {'exceptionHandler': (1, 0), 'printErrorMessage': (0, 0), 'writeBufferMessage': (0, 0),
                    'showSharedRWMemory': (0, 0)}
-PROTOCOL = ['getFieldNumLen32', 'getRawPrime', 'readSharedRWMemory', 'writeSharedRWMemory', 'init', 'setInputSignal',
-            'getWitnessSize', 'getWitness', 'getInputSize', 'getVersion']
+PROTOCOL_EXPORTS = ['getFieldNumLen32', 'getRawPrime', 'readSharedRWMemory', 'writeSharedRWMemory', 'init',
+                    'setInputSignal', 'getWitnessSize', 'getWitness', 'getInputSize', 'getVersion']
 
 
 class Refused(ValueError):
@@ -189,7 +190,7 @@ class Module:
                 raise Refused("the module defines no memory")
             self.mem = (0, 0)
         self.bodies = [None] * len(self.codes)
-        for nm in PROTOCOL if protocol else []:
+        for nm in PROTOCOL_EXPORTS if protocol else []:
             if nm not in self.exports or self.exports[nm][0] != 0:
                 raise Refused(f"the module does not export the circom 2 function {nm}")
 
@@ -578,6 +579,8 @@ class Calculator:
                         inst.call('writeSharedRWMemory', j, (v >> (32 * j)) & M32)
                     inst.call('setInputSignal', h >> 32, h & M32, i)
             n = inst.call('getWitnessSize')[0]
+            if n != self.witness_size:         # the witness would not have the rows the caller allocated
+                return PROTOCOL, None
             w = []
             for i in range(n):
                 inst.call('getWitness', i)
